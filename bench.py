@@ -28,33 +28,31 @@ N2 = 1024
 ALG_BYTES_PER_SAMPLE = 8          # 4 B spectrum read + 4 B f32 PCM write (SURVEY.md section 8d)
 
 
+DUMP_BYTES = 48 << 20             # --dump-outputs writes at most this many bytes in all (a seeded sample)
+
+
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3 3.35 TB/s), not measured"
 
 
-def ncu_traffic(streams, packets):
-    """DRAM bytes (read + write) per k_long launch from the committed `ncu --set full` capture of this
-    same workload (profiles/*_k_long_ncu_summary.txt, newest round); None for any other workload."""
-    if (streams, packets) != (4096, 16):
-        return None, None
-    import glob
-    import re
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_k_long_ncu_summary.txt")))
-    if not files:
-        return None, None
-    txt = open(files[-1]).read()
-    unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    tot = 0.0
-    for key in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-        m = re.search(re.escape(key) + r"\s+([0-9.]+)\s+(\w+)", txt)
-        if not m or m.group(2) not in unit:
-            return None, None
-        tot += float(m.group(1)) * unit[m.group(2)]
-    return tot, os.path.relpath(files[-1], ROOT)
+def dump_outputs(dirname, pcm, pwrs, seed=4321):
+    """Write what the timed path returned in its last step as DIR/<name>.npy (float32), so that two builds can be
+    compared output for output: `pcm` = the f32 planar PCM [k, channels, t] of a fixed, seeded sample of k streams
+    (in stream order; the first t samples of each), `state` = those streams' PreviousWindowRight after the step
+    [k, channels, 1024].  Each array gets half of DUMP_BYTES: all streams and samples when they fit, fewer otherwise."""
+    S, C, T = pcm.shape
+    half = DUMP_BYTES // 2
+    t = min(T, half // (4 * C))
+    k = max(1, min(S, half // (4 * C * max(t, N2))))
+    idx = np.sort(np.random.default_rng(seed).choice(S, k, replace=False))
+    os.makedirs(dirname, exist_ok=True)
+    import torch
+    np.save(os.path.join(dirname, "pcm.npy"), pcm[torch.from_numpy(idx).to(pcm.device), :, :t].cpu().numpy())
+    np.save(os.path.join(dirname, "state.npy"), np.stack([pwrs[i].data() for i in idx]))
 
 
 class ClockSampler:
@@ -171,6 +169,8 @@ def main():
     ap.add_argument("--mixed-streams", type=int, default=2048,
                     help="streams per GPU of the mixed short/long measurement (0: skip)")
     ap.add_argument("--sustained-sec", type=float, default=1.0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write rank 0's output of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -249,6 +249,8 @@ def main():
     barrier()
     ms_total = ev0.elapsed_time(ev1)
     launches = ctx.launch_count - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, pcm, pwrs)
     # The timed region lasts a few milliseconds (a burst, far below nvidia-smi's sampling period).  The same step is
     # then repeated back to back for >= --sustained-sec, timed the same way: that is the sustained value (power
     # capped clocks), and the window the clock / throttle samples are taken in.
@@ -446,7 +448,6 @@ def main():
             mixed["frac_of_hbm_peak"] = mixed["achieved_gbs"] / peak
         per_gpu = value / world
         achieved = per_gpu * ALG_BYTES_PER_SAMPLE / 1e9
-        traffic, traffic_src = ncu_traffic(S, P)
         line = {"metric": "Msamples/s IMDCT+window+OLA, 2048-pt long blocks", "value": value / 1e6,
                 "unit": "Msamples/s", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
                 "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -455,11 +456,10 @@ def main():
                                        "(BASELINE.json configs[1]); per GPU: streams x packets x 2 channels",
                            "streams_per_gpu": S, "packets_per_stream": P, "channels": C,
                            "bytes_in_per_step_per_gpu": S * P * C * N2 * 4,
-                           "l2_policy": "inputs+outputs per step (1 GiB at defaults) exceed the 126 MB L2",
+                           "l2_policy": "inputs+outputs per step (1 GiB at defaults) exceed the 50 MB L2",
                            "parallelism": f"streams sharded over {world} rank(s), no data-path collective"},
                 "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                             "frac": achieved / peak, "traffic": traffic, "traffic_unit": "bytes per launch (ncu dram read+write)",
-                             "traffic_source": traffic_src, "algorithmic_bytes_per_launch": S * P * C * N2 * ALG_BYTES_PER_SAMPLE,
+                             "frac": achieved / peak, "algorithmic_bytes_per_launch": S * P * C * N2 * ALG_BYTES_PER_SAMPLE,
                              "peak_source": peak_src,
                              "kernel": "k_long", "algorithmic_bytes_per_sample": ALG_BYTES_PER_SAMPLE},
                 "e2e": {"value": e2e_value / 1e6, "unit": "Msamples/s",

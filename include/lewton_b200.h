@@ -1,5 +1,5 @@
 /*
- * lewton_b200.h -- C ABI of the B200-native Vorbis packet-synthesis back-end.
+ * lewton_b200.h -- C ABI of the H100-native Vorbis packet-synthesis back-end.
  *
  * What it replaces (RustAudio/lewton @ bb2955b): the dense back half of
  *   audio::read_audio_packet_generic            src/audio.rs:988-1157
@@ -13,7 +13,7 @@
  * Style follows the crate's own C API (src/capi.rs:78-147): opaque pointers,
  * int status, out-parameters, explicit *_destroy.  Nothing unwinds across the
  * boundary.  There is NO CPU fallback: every entry point that computes fails
- * with LWB_ERR_NO_DEVICE / LWB_ERR_CUDA when no sm_100 device is usable.
+ * with LWB_ERR_NO_DEVICE / LWB_ERR_CUDA when no sm_90 device is usable.
  *
  * Threading: a ctx is bound to one CUDA device and is not thread-safe (the
  * reference is single-threaded and &mut-exclusive per stream); use one ctx per
@@ -49,7 +49,7 @@ enum {
     LWB_ERR_MISMATCH = 3,     /* where the reference panics: channel-count mismatch (:1086), mag==ang (:783) */
     LWB_ERR_INVALID = 4,      /* NULL / out-of-range argument */
     LWB_ERR_CUDA = 5,         /* a CUDA call failed; see lwb_last_error */
-    LWB_ERR_NO_DEVICE = 6     /* no usable sm_100 device: there is no CPU fallback */
+    LWB_ERR_NO_DEVICE = 6     /* no usable sm_90 device: there is no CPU fallback */
 };
 
 typedef struct lwb_ctx lwb_ctx;        /* one per GPU: stream, staging, launch state           */

@@ -5,11 +5,11 @@
  *
  * This is CPU code by nature (bit-serial Huffman / VQ decode); it is the part of lewton that stays
  * on the host in the drop-in design (INTEGRATION.md).  In a Rust build the crate's own front half
- * plays this role; this C++ restatement exists because Rust is not available in the build image,
+ * plays this role; this C++ restatement exists because the project is built without a Rust toolchain,
  * so that whole streams can be decoded end to end and the batch / residue entry points of the
  * CUDA back end can be driven by real bitstreams.
  *
- * Reference interfaces mirrored (file:line in /root/reference/src):
+ * Reference interfaces mirrored (file:line in the reference's src/):
  *   lwf_headers_parse            header.rs:221 read_header_ident, :309 read_header_comment,
  *                                :1082 read_header_setup
  *   lwf_packet_decode            audio.rs:919-986 (front half of read_audio_packet_generic),

@@ -1,4 +1,4 @@
-"""lewton_b200 -- B200-native Vorbis packet-synthesis back-end (the dense half of lewton's
+"""lewton_b200 -- H100-native Vorbis packet-synthesis back-end (the dense half of lewton's
 audio::read_audio_packet*), as a C-ABI shared library plus this thin Python mirror.
 
 Importing the package loads nothing; the first call into `lewton_b200.api` loads

@@ -1,7 +1,7 @@
 """ctypes binding of lewton_b200/liblewton_b200.so (declarations mirror include/lewton_b200.h).
 
 There is no CPU fallback: if the library cannot be loaded the import raises, and every compute
-entry point fails with LWB_ERR_NO_DEVICE when no sm_100 GPU is usable.
+entry point fails with LWB_ERR_NO_DEVICE when no sm_90 GPU is usable.
 """
 import ctypes as C
 import os

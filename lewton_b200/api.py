@@ -8,7 +8,7 @@ packet arrives as `DecodedPacket` = what that front half produces (mode, window 
 floor Y values, dense residue vectors).  Everything after audio.rs:988 runs on the GPU.
 
 This module is plumbing for tests, the bench and Python callers; the product is the shared
-library.  It never computes audio on the CPU: without the library / a B200 it raises.
+library.  It never computes audio on the CPU: without the library / an H100 it raises.
 """
 import ctypes as C
 import weakref
@@ -45,7 +45,7 @@ class Context:
         rc = cabi.lib().lwb_ctx_create(device, C.byref(self._h))
         if rc:
             self._h = None
-            raise AudioReadError(rc, "lwb_ctx_create failed (no sm_100 device? there is no CPU fallback)")
+            raise AudioReadError(rc, "lwb_ctx_create failed (no sm_90 device? there is no CPU fallback)")
         self.device = device
         self._children = weakref.WeakSet()      # setups / streams: destroyed before the ctx
 

@@ -1,8 +1,7 @@
-"""Build lewton_b200/liblewton_b200.so for sm_100a with nvcc (in-tree, so it travels to the GPU box).
+"""Build lewton_b200/liblewton_b200.so for sm_90a (H100) with nvcc, in the source tree.
 
-Also enforces the parity-critical property of the fused kernel at build time: its SASS must not
-contain a fused multiply-add (ptxas 12.9 contracts packed f32x2 mul+add even with explicit .rn;
-kernel_long.cuh is written so that no such pair exists -- this check keeps it that way).
+Also enforces the parity-critical property of the kernels at build time: their SASS must not
+contain a fused multiply-add, which would merge two of the reference's roundings into one.
 """
 import os
 import re
@@ -12,6 +11,7 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "liblewton_b200.so")
+K_LONG_REGS = 249          # k_long's registers per thread in the measured H100 build (DESIGN.md 4.1)
 SOURCES = ["lwb_api.cu", "host_objects.cuh", "path_generic.cuh", "path_long.cuh", "path_chain.cuh", "path_mixed.cuh", "path_mid.cuh",
            "tables_host.cpp", "frontend.cpp", "lwb_common.h", "kernels_generic.cuh", "kernel_long.cuh", "kernel_short.cuh", "kernel_mid.cuh", "kernel_chain.cuh", "kernel_prologue.cuh", "floor1_eval.cuh",
            "floor1_inverse_db.inc", "Makefile"]
@@ -37,9 +37,8 @@ def check_no_fma(so=SO):
 
 def hot_kernel_registers(log):
     """Registers per thread of k_long<float> / k_long<int16_t> from ptxas -v output.  The headline kernel is bound by
-    per-warp latency and touchy about its allocation: at 254-255 registers (two more live values, or a changed helper
-    template that only its sibling k_long_s uses) it lost 3-4 % (A/B on one box, DESIGN.md 4.4); 250 / 252 is the
-    allocation the measured numbers belong to."""
+    per-warp latency and sensitive to its allocation (a changed helper template that only its sibling k_long_s uses
+    can move it); K_LONG_REGS is the allocation the H100 numbers in DESIGN.md belong to."""
     regs = {}
     for m in re.finditer(r"Compiling entry function '(_ZN3lwb6k_longI([fs])EE[^']*)'.*?Used (\d+) registers", log, re.S):
         regs["k_long<float>" if m.group(2) == "f" else "k_long<int16_t>"] = int(m.group(3))
@@ -57,14 +56,14 @@ def build(force=False, verbose=False):
         if r.returncode:
             raise RuntimeError("nvcc build of liblewton_b200.so failed")
         regs = hot_kernel_registers(r.stdout + r.stderr)
-        if any(v > 252 for v in regs.values()):
-            print(f"lewton_b200 build: WARNING: {regs} -- k_long above 252 registers has measured 3-4 % slower; "
-                  "look at what changed in kernel_long.cuh's shared helpers")
+        if any(v > K_LONG_REGS for v in regs.values()):
+            print(f"lewton_b200 build: WARNING: {regs} -- k_long above {K_LONG_REGS} registers is not the allocation the "
+                  "measured numbers belong to; look at what changed in kernel_long.cuh's shared helpers")
         n = check_no_fma()
         if n:
             os.remove(SO)
             raise RuntimeError(f"{n} fused multiply-add instructions in the kernels' SASS: bit parity with "
-                               "the reference would be lost (see kernel_long.cuh vadd_p/vsub_p)")
+                               "the reference would be lost (see kernel_long.cuh vadd/vmul)")
     return SO
 
 

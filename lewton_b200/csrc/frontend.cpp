@@ -2077,8 +2077,8 @@ int batch_entropy(lwf_batcher *b, BatchArena &ar, lwf_stream_job *jobs, size_t j
             }
         if (!ar.vqrun.ensure((size_t)run_off[pkt_total] * sizeof(lwb_vq_run) + 16) || !ar.vqent.ensure((size_t)ent_off[pkt_total] * 2 + 16))
             return LWB_ERR_BUFFER;
-        // ~3 KB per stereo long packet: copied by the pool as well (one thread took as long over it as the whole pool
-        // over the entropy decode, profiles/r2j_stream_bench.jsonl)
+        // ~3 KB per stereo long packet: copied by the pool as well (one thread alone would take about as long over it as
+        // the whole pool over the entropy decode)
         std::atomic<size_t> next_copy(j0);
         auto copier = [&]() {
             for (;;) {

@@ -17,7 +17,7 @@
 //
 // This is the fallback for everything the fused long-block kernel (kernel_long.cuh) does not take;
 // it replaces the four-kernel path (kernels_generic.cuh) wherever channels <= 8 and the buffers fit
-// in shared memory, and is ~10-30x faster than it (profiles/r1_sweep_*).
+// in shared memory: a chain's buffers and state stay there instead of round-tripping HBM between kernels.
 #pragma once
 #include "kernels_generic.cuh"
 

@@ -19,9 +19,9 @@
 //     * phase A: one float4 of spectrum feeds both groups (c and 511-c come from the same quad),
 //     * phase C: the step-7 partner (c' <-> 511-c') of every value lives in the same lane,
 //     * output index m = 64*rev3(slot) + lane (or 63-lane): every store is a full 128 B line.
-//   Every operation is written on V = (group a, group b) pairs, which maps 1:1 onto Blackwell's
-//   packed add/sub/mul.rn.f32x2 (SASS FADD2/FMUL2; IEEE RN per lane, so parity-safe) and halves
-//   the FP issue slots of this issue-bound, non-FMA-able kernel.
+//   Every operation is written on V = (group a, group b) pairs: two independent scalar IEEE RN
+//   operations (SASS FADD/FMUL, never contracted into FFMA), which gives the scheduler two
+//   independent instruction streams per lane in this issue-bound, non-FMA-able kernel.
 //   Twiddles/window: a per-lane "pack" (built once per setup on the host from the uploaded
 //   tables) is staged in shared memory per CTA; phases A/B keep theirs in registers across the
 //   whole run, phase C reads its 48 pairs per block from the shared copy.
@@ -68,50 +68,13 @@ static_assert(sizeof(LongRun) == 48, "LongRun is copied by TMA in 16-byte units"
 struct V { float x, y; };    // (group a, group b)
 
 #if defined(__CUDA_ARCH__)
-#ifndef LWB_PACKED_F32X2
-#define LWB_PACKED_F32X2 1
-#endif
-#if LWB_PACKED_F32X2
-__device__ __forceinline__ unsigned long long v_bits(V a)
-{
-    unsigned long long r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a.x), "f"(a.y));
-    return r;
-}
-__device__ __forceinline__ V v_from(unsigned long long r)
-{
-    V a;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(a.x), "=f"(a.y) : "l"(r));
-    return a;
-}
-__device__ __forceinline__ V vadd(V a, V b)
-{
-    unsigned long long r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(v_bits(a)), "l"(v_bits(b)));
-    return v_from(r);
-}
-__device__ __forceinline__ V vsub(V a, V b)
-{
-    unsigned long long r;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(v_bits(a)), "l"(v_bits(b)));
-    return v_from(r);
-}
-__device__ __forceinline__ V vmul(V a, V b)
-{
-    unsigned long long r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(v_bits(a)), "l"(v_bits(b)));
-    return v_from(r);
-}
-#else
+// Hopper has no packed f32x2 arithmetic: a pair operation is two scalar FADD / FMUL.  The
+// __f*_rn intrinsics are never contracted into FFMA, so every rounding of the reference is kept.
 __device__ __forceinline__ V vadd(V a, V b) { return V{__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)}; }
 __device__ __forceinline__ V vsub(V a, V b) { return V{__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)}; }
 __device__ __forceinline__ V vmul(V a, V b) { return V{__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)}; }
-#endif
-// Add/sub whose operands are PRODUCTS.  ptxas (12.9) contracts mul.rn.f32x2 + add.rn.f32x2 into
-// FFMA2 even with explicit .rn and -fmad=false (it also rewrites fma(a,b,-0) and fma(a,1,c) back
-// to mul/add first), which would merge two of the reference's roundings into one.  Scalar
-// add.rn.f32 is never contracted, so the product-consuming adds stay scalar (FADD) while all
-// other adds and all multiplies are packed (FADD2 / FMUL2).
+// Add/sub whose operands are PRODUCTS (the operation order of the reference's butterflies, kept as
+// separate names so that the rounding structure stays visible at every call site).
 __device__ __forceinline__ V vadd_p(V a, V b) { return V{__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)}; }
 __device__ __forceinline__ V vsub_p(V a, V b) { return V{__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)}; }
 // -(a) - b for products: the scalar FADD takes both negations as free operand modifiers
@@ -545,12 +508,11 @@ __device__ __forceinline__ void lds_eo(uint32_t addr, float &e, float &o)
 
 // Twiddle residency: pack slots [kTwReg0, kTwReg1) live in registers for the whole kernel, the
 // rest is read from the CTA's shared copy of the pack when used (compile-time choice per slot).
-// Default (measured best on B200, profiles/variants_r1*.log): one block per warp, 8 warps per SM
-// (2 per scheduler, 242 registers, no spills), a 5-tile ring, phase A / B / step-7 twiddles resident
-// (slots 0..52) and the step-8 / window pairs fetched per block: 0.745 of the measured HBM peak.
-// 12 warps x 164 registers with slots 16..29 resident: 0.734; 16 warps x 128 registers, nothing
-// resident: 0.700; scalar instead of packed FP: -8 %; two blocks per warp (NB = 2) doubles the loop
-// body past the instruction cache: 2x slower.
+// Default (H100, DESIGN.md 4.1): one block per warp, 8 warps per SM (2 per scheduler, 249 registers,
+// no spills), a 5-tile ring, phase A / B / step-7 twiddles resident (slots 0..52) and the step-8 /
+// window pairs fetched per block.  12 warps x 167 registers with slots 16..29 resident, a 4-tile ring
+// and slots 0..44 resident measured the same on the long-block bench; 12 warps were 4 % slower on
+// mixed streams.
 #ifndef LWB_TW_REG0
 #define LWB_TW_REG0 0
 #endif
@@ -613,12 +575,12 @@ __device__ __forceinline__ int16_t d_sample_i16(float v)
     // (float-to-integer cvt saturates by definition) and turns NaN into 0; clamping after the
     // truncation equals clamping the float first (32767.x truncates to 32767, -32768.x to -32768).
     // (Pairing lanes to store two samples per 32-bit word was tried: the shuffles cost more than the
-    // half-line stores, 471 vs 518 Gsamples/s, profiles/variants_r1k.log.)
+    // half-line stores save.)
     short r;
     asm("cvt.rzi.s16.f32 %0, %1;" : "=h"(r) : "f"(__fmul_rn(v, 32768.0f)));
     return (int16_t)r;
 }
-__device__ __forceinline__ void st_pcm(float *p, float v) { __stcs(p, v); }    // .cs beats .cg / default (variants_r1k.log)
+__device__ __forceinline__ void st_pcm(float *p, float v) { __stcs(p, v); }    // streaming: the PCM is not read again
 __device__ __forceinline__ void st_pcm(int16_t *p, float v) { __stcs(reinterpret_cast<short *>(p), (short)d_sample_i16(v)); }
 
 // Step 8 + window + overlap-add + stores, all 8 slots of all NB blocks.  FIRST: packet 0 of the
@@ -682,8 +644,7 @@ __device__ __forceinline__ float lds_f32(uint32_t addr)
 // x[ls .. 1024): pl windowed samples, then the rest of the left half as is (audio.rs:1112-1120).
 // Rare (once per burst of short blocks), so plain scalar code; w = the short window slope.
 // EXPORT: k_long_s -- runs may export their left slope (flags bit 5), and the slope is read from its shared-memory copy
-// at w_s (through __ldg from global memory the four products of a lane each waited for an L2 round trip: 3.4 % of
-// k_long_s's stall samples on the 6-channel config)
+// at w_s (through __ldg from global memory the four products of a lane would each wait for an L2 round trip)
 // LS: ls as a compile-time constant (0: use the argument) -- with it every position test below folds per slot.
 template <int NB, typename OutT, typename RC = RunCur, bool EXPORT = false, int LS = 0>
 __device__ __forceinline__ void out_first_short(const TwMix &tw, int lane, const V O[NB][8], const V E[NB][8], V pe[NB][8],
@@ -933,7 +894,7 @@ k_long(const LongRun *__restrict__ runs, uint32_t n_groups, const float *__restr
                 // one just consumed, in stages slot_i+1 .. slot_i+ahead, so the next tile goes to
                 // slot_i+1+ahead (== slot_i once the ring is full).  One tile per packet: a ring left
                 // under-filled by groups shorter than itself is topped up at the next hand-over (a
-                // catch-up loop here costs 2-9% of the steady state, profiles/variants_r1k.log).
+                // catch-up loop here slowed the steady state down).
                 uint32_t ahead = lc - (p + 1) + nx_lc;
                 if (ahead < (uint32_t)kLongRing) {
                     uint32_t tgt = slot_i + 1 + ahead;
@@ -1056,8 +1017,8 @@ k_long(const LongRun *__restrict__ runs, uint32_t n_groups, const float *__restr
         nlc = __shfl_sync(0xffffffffu, nlc, 0);
         if (st_ != 2) break;
         // lane 0 has acquired the descriptor tile through its mbarrier wait; the warp barrier extends that
-        // to the other lanes (a shuffle alone is not a memory-ordering operation).  Letting every lane
-        // wait on the mbarrier itself costs 2 % (code layout), profiles/variants_r1k.log.
+        // to the other lanes (a shuffle alone is not a memory-ordering operation), which is cheaper than
+        // letting every lane wait on the mbarrier itself.
         __syncwarp();
 #pragma unroll
         for (int b = 0; b < NB; b++) cur[b] = run_cur(s_next[b]);

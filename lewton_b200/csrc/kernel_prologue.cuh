@@ -12,10 +12,10 @@
 //                       multiply (:1035-1037), float4 loads and stores.  The kernel is HBM-bound (4 B in + 4 B out per
 //                       coefficient); the per-bin floor arithmetic rides in its idle issue slots.
 //
-// History (profiles/r2*): the per-packet-CTA kernel took 5x its roofline time (serial unwrap on one lane per warp with
-// the CTA waiting, 8-way predicated register arrays).  A first split rendered the curve to a byte arena in a separate
-// kernel (16 bins per work item): its per-bin segment-crossing branches diverged (20 of 32 lanes active, 173 M
-// warp-instructions for 134 M bins, 0.27 ms) and the curve cost 2 B per coefficient of extra traffic.
+// History: the per-packet-CTA kernel was far from its roofline time (serial unwrap on one lane per warp with the CTA
+// waiting, 8-way predicated register arrays).  A first split rendered the curve to a byte arena in a separate kernel
+// (16 bins per work item): its per-bin segment-crossing branches diverged and the curve cost 2 B per coefficient of
+// extra traffic.
 #pragma once
 #include "kernels_generic.cuh"
 

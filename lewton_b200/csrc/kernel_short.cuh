@@ -10,9 +10,9 @@
 //     phase A: slot = bits 5,4,3  -> step 0, step 2, stages 0, 1              (imdct.rs:337-452)
 //     phase C: slot = bits 2,1,0  -> ld654, bit-reverse (renaming), step 7, step 8, window / OLA
 // with ONE shared-memory transpose in between (conflict-free for the eight blocks together).  Everything
-// else follows the long kernel: the reference's rounding DAG operation for operation, packed
-// add/sub/mul.rn.f32x2 on (group a, group b) pairs with scalar adds where an operand is a product
-// (no FMA contraction), twiddles from a per-lane pack, spectrum tiles by 1-D TMA into a per-warp ring.
+// else follows the long kernel: the reference's rounding DAG operation for operation, written on
+// (group a, group b) pairs of uncontracted IEEE RN operations, twiddles from a per-lane pack, spectrum
+// tiles by 1-D TMA into a per-warp ring.
 // Eight consecutive packets are 1024 consecutive PCM samples: block b's previous right half (the only
 // inter-packet state, audio.rs:847-861) is block b-1's p_even, fetched from the neighbouring lanes by
 // shuffle; block 0 takes it from the previous octet (registers) or the stream state (first octet).
@@ -262,7 +262,7 @@ __device__ __forceinline__ void copy_out4(int16_t *dst, uint32_t src)
 //     mbarrier) up to kShortRing stages ahead of where it CONSUMES them, across run boundaries.
 // PCM leaves through shared memory: the lanes' samples are staged (swizzled, conflict-free) and go out as one
 // 128-bit (f32) / 64-bit (i16) store per lane and packet, 512 / 256 contiguous bytes per instruction, instead of
-// 16-byte pieces of eight different lines per instruction (ncu: the L1 data pipe was the limiter at 81 %).
+// 16-byte pieces of eight different lines per instruction, which made the L1 data pipe the limiter.
 template <typename OutT>
 __global__ void __launch_bounds__(kShortWarps * 32, 1)
 k_short(const ShortRun *__restrict__ runs, uint32_t n_runs, const float *__restrict__ pack)

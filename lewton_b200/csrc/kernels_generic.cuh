@@ -326,7 +326,7 @@ __device__ __forceinline__ void d_imdct_to_v(const DevTables &tb, int n, const f
 // buffers U + q * bs and V + q * bs).  Arithmetic per block is identical to d_imdct_to_v; every stage
 // first loads the operands of all NP blocks, then computes, then stores, so that a thread has NP
 // independent dependency chains in flight instead of one -- the transform is latency-bound for small
-// n, where a stage is a single butterfly per lane (ncu: one instruction per ~54 cycles per warp).
+// n, where a stage is a single butterfly per lane and each instruction waits on the one before it.
 template <int NP, class Sync>
 __device__ __forceinline__ void d_imdct_to_v_np(const DevTables &tb, int n, const float *X, size_t xs, float *U, float *V, int bs,
                                                 int tid, int NT, Sync sync)

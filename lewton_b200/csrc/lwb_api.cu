@@ -59,7 +59,7 @@ extern "C" int lwb_ctx_create(int device, lwb_ctx **out)
     if (n <= 0 || device < 0 || device >= n) return LWB_ERR_NO_DEVICE;
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return LWB_ERR_NO_DEVICE;
-    if (prop.major != 10) return LWB_ERR_NO_DEVICE;       // kernels are built for sm_100a only
+    if (prop.major != 9 || prop.minor != 0) return LWB_ERR_NO_DEVICE;   // kernels are built for sm_90a only
     lwb_ctx *ctx = new (std::nothrow) lwb_ctx();
     if (!ctx) return LWB_ERR_BUFFER;
     ctx->device = device;
@@ -137,7 +137,7 @@ extern "C" void lwb_host_free(void *p) { if (p) cudaFreeHost(p); }
 // NUMA placement of the host side.  A rank that feeds GPU d through host buffers should run on, and
 // allocate its pinned memory from, the socket GPU d's PCIe root hangs off: with 4 GPUs per socket the
 // copies of all of them otherwise cross the inter-socket link of whichever node the pages landed on.
-// Plain syscalls (no libnuma in this image).  Returns the node, or -1 when it cannot be determined.
+// Plain syscalls (no libnuma dependency).  Returns the node, or -1 when it cannot be determined.
 extern "C" int lwb_bind_host_to_device(int device)
 {
     if (device < 0) {

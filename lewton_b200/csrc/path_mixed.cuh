@@ -316,7 +316,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         VqView vqv;
         if ((rc = stage_vq_arrays(ctx, io, r_lo, r_hi, sm, &vqv))) return rc;
         // descriptors of every round: [LongRun...][ChainDesc...][DevPacket (prologue of the long segments)...][mode bytes]
-        // A round with few fused-kernel runs leaves most of the 148 x 8 warps idle and lasts as long as its
+        // A round with few fused-kernel runs leaves most of the SMs x 8 warps idle and lasts as long as its
         // longest run: such rounds cut their runs (each cut costs one extra IMDCT, the primer packet whose
         // right half is all the next piece needs), as the all-long path does.
         const size_t target_runs = (size_t)ctx->sm_count * kLongWarps * 2;

@@ -7,8 +7,8 @@
  * The product (lewton_b200/) never links, imports or calls it.
  *
  * Why a restatement: the reference (RustAudio/lewton @ bb2955b, v0.10.2) is pure
- * Rust and this image has no rustc/cargo, so the reference cannot be compiled
- * here (oracle/_ref is therefore absent).  Each function below cites the
+ * Rust and this project is built without a Rust toolchain, so the reference is
+ * not compiled (oracle/_ref is therefore absent).  Each function below cites the
  * reference file:line whose arithmetic it follows, operation for operation, in
  * IEEE binary32 without contraction (-ffp-contract=off, no -ffast-math).
  *

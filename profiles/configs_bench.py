@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Throughput of the other shapes SURVEY.md section 8(d) asks to be reported beside the headline
-(device-resident, one B200, CUDA events on the library's stream, one JSON line per case):
+(device-resident, one H100, CUDA events on the library's stream, one JSON line per case):
 
   long_f32        S x P stereo long packets, spectrum entry, f32 planar           8 B / sample (the headline)
   long_i16        same, i16 planar output                                          6 B / sample
@@ -30,7 +30,7 @@ def main():
     from lewton_b200 import _cabi as cabi
     from helpers import make_setup, random_floor1_y
 
-    peak = 6650.0
+    peak = 3350.0          # H100 SXM data sheet (HBM3), when no measured peak is present
     pth = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pth):
         peak = float(json.load(open(pth))["hbm_gbs"])

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """How close is `e2e` (host buffers through lwb_decode_chains) to what the PCIe link gives?
-Measures on one B200: pinned H2D alone, D2H alone, both directions at once (256 MiB each, two
+Measures on one H100: pinned H2D alone, D2H alone, both directions at once (256 MiB each, two
 streams, CUDA events), then the e2e call with f32 and with i16 PCM.  One JSON line."""
 import json
 import os

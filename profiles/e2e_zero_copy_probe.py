@@ -1,5 +1,5 @@
-import sys, time, json
-sys.path.insert(0, '/root/repo')
+import os, sys, time, json
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import lewton_b200 as L
 from lewton_b200 import _cabi as cabi

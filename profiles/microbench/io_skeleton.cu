@@ -1,8 +1,8 @@
 // io_skeleton.cu -- how fast can the I/O pattern of k_long go with no arithmetic at all?
-// Same structure: 148 CTAs x W warps, each warp streams 4 KB tiles by 1-D TMA into a 3-deep ring,
+// Same structure: one CTA per SM x 12 warps, each warp streams 4 KB tiles by 1-D TMA into a 3-deep ring,
 // reads them with 8 LDS.128 per lane and writes 4 KB of output with 32 STG.32 per lane, each a full
 // 128-byte line (mode 0: k_long's scattered line order; mode 1: 8 coalesced STG.128 per lane).
-// Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o io_skeleton io_skeleton.cu
+// Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o io_skeleton io_skeleton.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdint>
@@ -91,14 +91,16 @@ int main(int argc, char **argv)
     const size_t smem = 12 * 3 * 4096 + 12 * 3 * 8 + 64;
     cudaFuncSetAttribute(k_io<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     cudaFuncSetAttribute(k_io<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
     for (int mode = 0; mode < 2; mode++) {
         float best = 1e9f;
         for (int it = 0; it < 12; it++) {
             cudaMemset(ticket, 0, 4);
             cudaEventRecord(e0);
-            if (mode == 0) k_io<0><<<148, 384, smem>>>(in, out, chains, packets, ticket);
-            else k_io<1><<<148, 384, smem>>>(in, out, chains, packets, ticket);
+            if (mode == 0) k_io<0><<<sms, 384, smem>>>(in, out, chains, packets, ticket);
+            else k_io<1><<<sms, 384, smem>>>(in, out, chains, packets, ticket);
             cudaEventRecord(e1); cudaEventSynchronize(e1);
             float ms; cudaEventElapsedTime(&ms, e0, e1);
             if (it >= 2 && ms < best) best = ms;

@@ -23,7 +23,7 @@ def main():
     from lewton_b200 import _cabi as cabi
     from helpers import mode_sequence
 
-    peak = 6650.0
+    peak = 3350.0          # H100 SXM data sheet (HBM3), when no measured peak is present
     pth = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pth):
         peak = float(json.load(open(pth))["hbm_gbs"])

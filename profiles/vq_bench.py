@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """End-to-end style line for the residue entries (SURVEY.md 8f rank 2): host (pinned) buffers in, PCM in host buffers out,
-through lwb_decode_chains / lwb_plan_execute, one B200.  The packets are real Vorbis audio packets made by
+through lwb_decode_chains / lwb_plan_execute, one H100.  The packets are real Vorbis audio packets made by
 tests/vorbis_packer.py (stereo, residue type 2, one coupling step, ~365 bytes per 2048-sample long packet = the size of a
 128 kbit/s stream), entropy-decoded ONCE on the host; what is timed is everything behind the entropy decode:
 

@@ -1,9 +1,8 @@
 #!/usr/bin/env python3
 """Extract the reference's own known-answer vectors into JSON fixtures.
 
-Run in the BUILD container only (it reads /root/reference, which does not exist
-on the GPU box); the JSON files it writes are committed and are what the tests
-read.  Nothing here is executed at test time.
+Usage: make_golden.py <path to the lewton source tree>.  The JSON files it writes
+are committed and are what the tests read.  Nothing here is executed at test time.
 
 Sources (all literal test data of the reference's own unit tests):
   * src/imdct_test.rs:11-981   IMDCT_{INPUT,OUTPUT}_TEST_ARR_{1,2,3}
@@ -17,7 +16,7 @@ import os
 import re
 import sys
 
-REF = sys.argv[1] if len(sys.argv) > 1 else "/root/reference"
+REF = sys.argv[1] if len(sys.argv) == 2 else None
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
@@ -37,6 +36,8 @@ def float_arrays(src):
 
 
 def main():
+    if REF is None:
+        sys.exit("usage: make_golden.py <path to the lewton source tree>")
     kat = float_arrays(read("src/imdct_test.rs"))
     assert set(kat) == {f"IMDCT_{d}_TEST_ARR_{i}" for d in ("INPUT", "OUTPUT") for i in (1, 2, 3)}, kat.keys()
     with open(os.path.join(HERE, "imdct_kat.json"), "w") as f:
