@@ -75,37 +75,38 @@ struct MixLaunch {
     const float *coeffs, *dense; const uint8_t *kinds; const uint32_t *ys; void *pcm;
 };
 
+// One launch of the residue entry's front stages (k_floor1_segments + k_prologue_fused, or k_prologue): floor x
+// decoupled residue -> ctx->spec for a list of packets with one channel count.  The packet list holds absolute element
+// offsets and packet rows; the arenas are biased instead (the spectrum by c_lo, floor / VQ arrays by their staging).
+struct FrontStages {
+    const DevPacket *pk = nullptr;     // device packet list
+    size_t n = 0;
+    unsigned C = 0;
+    bool fast = false;                 // the two-kernel form; else k_prologue with smem_old bytes of shared memory
+    size_t smem_old = 0;
+    int n2max = 0;                     // largest n/2 among the packets
+    uint64_t c_lo = 0;                 // element offset of ctx->spec[0]
+    uint64_t r_lo = 0, r_hi = 0;       // packet rows of the floor / VQ arrays
+    bool dense = false;                // whether the dense floor arena is passed
+};
+
 struct lwb_plan {
     lwb_ctx *ctx = nullptr;
     lwb_chain *chains = nullptr;
     size_t n_chains = 0;
     lwb_batch_io io;
-    // captured fused-path launch (valid while ctx->state_gen == gen)
+    // captured launch sequence (valid while ctx->state_gen == gen): the front stages if front.n, then either the
+    // rounds of mix_launch or, when there are none, one k_long over `runs`.  Every path that captures a residue-entry
+    // batch sets `front`; a spectrum-entry plan never does.
     bool captured = false;
     uint64_t gen = 0;
-    DevBuf runs;
+    FrontStages front;
+    DevBuf runs, pro, mix;             // descriptors the capture owns: k_long runs, the long path's front stages, the rest
     uint32_t n_groups = 0;
     const float *pack = nullptr;
     bool i16 = false;
-    // residue entry: the front-stage descriptors (one DevPacket per packet).  They depend only on the captured
-    // chain / mode arrays, never on stream state, so they stay valid for the plan's lifetime.
-    bool pro_captured = false, pro_fast = false;
-    DevBuf pro;
-    size_t n_pro = 0, pro_smem_old = 0;
-    unsigned pro_C = 0;
-    uint64_t pro_c_lo = 0, pro_c_hi = 0, pro_r_lo = 0, pro_r_hi = 0;
-    // captured mixed-path launch sequence (valid while ctx->state_gen == gen)
-    bool mixed_captured = false;
-    DevBuf mix;
     MixLaunch mix_launch;
     std::vector<MixRound> mix_rounds;
-    // ... residue entry: its front-stage descriptors sit in `mix` too
-    bool mix_pro = false, mix_pro_fast = false, mix_pro_dense = false;
-    const DevPacket *mix_pro_pk = nullptr;
-    size_t mix_pro_n = 0, mix_pro_smem_old = 0;
-    unsigned mix_pro_C = 0;
-    int mix_pro_n2max = 0;
-    uint64_t mix_pro_c_lo = 0, mix_pro_r_lo = 0, mix_pro_r_hi = 0;
 };
 
 struct lwb_stream {
@@ -158,6 +159,52 @@ static int ensure(lwb_ctx *ctx, DevBuf &b, size_t bytes)
     b.cap = want;
     ctx->state_gen++;              // captured plans may hold pointers into the arena that just moved
     return LWB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// host-memory pipeline and fused-kernel tickets
+// ---------------------------------------------------------------------------------------------
+constexpr uint32_t kTicketPool = 1024;
+
+// The per-context events of the host-memory pipeline and the fused kernels' ticket pool, made once by lwb_ctx_create.
+static int create_pipeline_objects(lwb_ctx *ctx)
+{
+    for (int k = 0; k < 65; k++) {
+        if (k < 64) CU(ctx, cudaEventCreateWithFlags(&ctx->ev_in[k], cudaEventDisableTiming));
+        CU(ctx, cudaEventCreateWithFlags(&ctx->ev_done[k], cudaEventDisableTiming));
+    }
+    for (int k = 0; k < 2; k++) {
+        CU(ctx, cudaEventCreateWithFlags(&ctx->ev_desc[k], cudaEventDisableTiming));
+        CU(ctx, cudaEventCreateWithFlags(&ctx->ev_kdone[k], cudaEventDisableTiming));
+    }
+    return ensure(ctx, ctx->ticket, kTicketPool * sizeof(unsigned int));
+}
+
+// The ticket of one k_long launch; the pool is zeroed on the compute stream once per wrap.
+static int next_ticket(lwb_ctx *ctx, unsigned int **ticket)
+{
+    if (ctx->ticket_next % kTicketPool == 0)
+        CU(ctx, cudaMemsetAsync(ctx->ticket.p, 0, kTicketPool * sizeof(unsigned int), ctx->stream));
+    *ticket = (unsigned int *)ctx->ticket.p + (ctx->ticket_next++ % kTicketPool);
+    return LWB_OK;
+}
+
+// The copy streams must not run ahead of work already queued on the compute stream that still reads or writes the
+// arenas (a previous call, a descriptor upload): order them behind it.
+static int order_copies_behind_compute(lwb_ctx *ctx)
+{
+    CU(ctx, cudaEventRecord(ctx->ev_done[64], ctx->stream));
+    CU(ctx, cudaStreamWaitEvent(ctx->copy_in, ctx->ev_done[64], 0));
+    CU(ctx, cudaStreamWaitEvent(ctx->copy_out, ctx->ev_done[64], 0));
+    return LWB_OK;
+}
+
+// Chunks of a host-memory batch, whose H2D / kernels / D2H overlap on three streams: one per 32 MiB of input, at most
+// 8 and at most one per chain.  LWB_E2E_CHUNKS=n sets the count, up to what ev_in / ev_done can index.
+static size_t host_chunks(size_t in_bytes, size_t n_chains)
+{
+    if (const char *e = getenv("LWB_E2E_CHUNKS")) return std::max<size_t>(1, std::min<size_t>((size_t)atol(e), std::min<size_t>(64, n_chains)));
+    return std::min<size_t>(std::max<size_t>(1, in_bytes >> 25), std::min<size_t>(8, n_chains));
 }
 
 static int ensure_pinned(lwb_ctx *ctx, size_t bytes)

@@ -71,6 +71,10 @@ extern "C" int lwb_ctx_create(int device, lwb_ctx **out)
         delete ctx;
         return LWB_ERR_CUDA;
     }
+    if (create_pipeline_objects(ctx)) {
+        lwb_ctx_destroy(ctx);
+        return LWB_ERR_CUDA;
+    }
     if (const char *e = getenv("LWB_SCRATCH_MB")) {
         long mb = atol(e);
         if (mb >= 1) ctx->x_cap_elems = (size_t)mb << 18;
@@ -516,6 +520,24 @@ extern "C" int lwb_decoded_sample_count(const lwb_setup *su, uint8_t mode, int p
 #include "path_mixed.cuh"
 #include "path_mid.cuh"
 
+// The batch paths in the order they are tried; what none of them takes goes to the four-kernel path (run_generic).
+using BatchPath = int (*)(lwb_ctx *, lwb_chain *, size_t, const lwb_batch_io *, uint64_t, bool *, lwb_plan *);
+static const BatchPath kBatchPaths[] = {
+    [](lwb_ctx *ctx, lwb_chain *chains, size_t n, const lwb_batch_io *io, uint64_t epoch, bool *handled, lwb_plan *plan) {
+        return try_long(ctx, chains, n, io, epoch, handled, plan);
+    },
+    try_long_residue, try_mid, try_mixed, try_chain};
+constexpr size_t kNumBatchPaths = sizeof(kBatchPaths) / sizeof(kBatchPaths[0]);
+
+// Index of the first batch path to try.  LWB_FORCE_GENERIC is a test switch that sends batches to the reference
+// paths: "1" to the four-kernel path only, any other value to the chain kernel and then the four-kernel path.
+static size_t first_batch_path()
+{
+    const char *fg = getenv("LWB_FORCE_GENERIC");
+    if (!fg) return 0;
+    return std::strcmp(fg, "1") == 0 ? kNumBatchPaths : kNumBatchPaths - 1;
+}
+
 static int decode_chains_impl(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, lwb_plan *prepared)
 {
     if (!ctx || (!chains && n_chains) || !io) return LWB_ERR_INVALID;
@@ -528,28 +550,14 @@ static int decode_chains_impl(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, 
         return fail(ctx, LWB_ERR_INVALID, "VQ entry needs vq_runs, vq_entries, their offsets and floor_kind");
     CU(ctx, cudaSetDevice(ctx->device));
     const uint64_t epoch = ++ctx->epoch;      // per context: concurrent calls on different contexts share nothing
-    {
+    if (prepared) {                           // the path that takes the batch captures it anew, if it can
+        prepared->captured = false;
+        prepared->mix_rounds.clear();
+    }
+    for (size_t k = first_batch_path(); k < kNumBatchPaths; k++) {
         bool handled = false;
-        const char *fg = getenv("LWB_FORCE_GENERIC");
-        const bool no_fused = fg && std::strcmp(fg, "2") == 0;
-        int rc0 = no_fused ? LWB_OK : try_long(ctx, chains, n_chains, io, epoch, &handled, nullptr, 0, prepared);
-        if (rc0 || handled) return rc0;
-        // residue-entry batches of uniform long blocks go front stages + fused kernel; everything else that fits
-        // goes to the segmented path or the chain kernel
-        if (!no_fused && !fg) {
-            rc0 = try_long_residue(ctx, chains, n_chains, io, epoch, &handled, prepared);
-            if (rc0 || handled) return rc0;
-        }
-        {
-            if (!no_fused) {
-                rc0 = try_mid(ctx, chains, n_chains, io, epoch, &handled, prepared);
-                if (rc0 || handled) return rc0;
-                rc0 = try_mixed(ctx, chains, n_chains, io, epoch, &handled, prepared);
-                if (rc0 || handled) return rc0;
-            }
-            rc0 = try_chain(ctx, chains, n_chains, io, epoch, &handled, prepared);
-            if (rc0 || handled) return rc0;
-        }
+        const int rc = kBatchPaths[k](ctx, chains, n_chains, io, epoch, &handled, prepared);
+        if (rc || handled) return rc;
     }
     const bool vq = io->entry == LWB_ENTRY_VQ;
     const bool residue = io->entry != LWB_ENTRY_SPECTRUM;
@@ -617,18 +625,8 @@ static int decode_chains_impl(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, 
         }
         if ((rc = stage_vq_arrays(ctx, io, r_lo, r_hi, ctx->stream, &ar.vq))) return rc;
         if (residue) {
-            // absolute packet rows address the (biased) device views: kinds_row0 stays 0
+            // absolute packet rows address the (biased) device views
             if ((rc = stage_floor_arrays(ctx, io, r_lo, r_hi, (unsigned)uniform_c, ctx->stream, &ar.kinds, &ar.ys))) return rc;
-            ar.kinds_row0 = 0;
-        }
-        if (residue && plan_is_long(plan, io)) {
-            // residue entry, uniform long blocks: k_prologue forms the spectrum on the device, the fused
-            // kernel does the rest (one extra spectrum round trip compared with the spectrum entry)
-            if ((rc = run_prologue_all(ctx, plan, ar, (size_t)(c_hi - c_lo)))) return rc;
-            bool handled = false;
-            rc = try_long(ctx, chains, n_chains, io, epoch, &handled, (const float *)ctx->spec.p, ar.coeff_base);
-            if (rc) return rc;
-            if (handled) return LWB_OK;            // try_long has committed results and stream states
         }
         rc = run_generic(ctx, plan, io, ar);
         if (rc) return rc;
@@ -681,63 +679,20 @@ extern "C" void lwb_plan_destroy(lwb_plan *p)
     delete p;
 }
 
-// Replays the captured front stages of a residue-entry plan (device-memory batches only: host-memory batches are
-// never captured as a whole).  Host floor arrays change from step to step and are uploaded again; device floor
-// arrays are read in place.
-static int replay_front_stages(lwb_plan *p)
-{
-    lwb_ctx *ctx = p->ctx;
-    const lwb_batch_io *io = &p->io;
-    const uint8_t *d_kinds;
-    const uint32_t *d_ys;
-    int rc = stage_floor_arrays(ctx, io, p->pro_r_lo, p->pro_r_hi, p->pro_C, ctx->stream, &d_kinds, &d_ys);
-    if (rc) return rc;
-    VqView vqv;
-    if ((rc = stage_vq_arrays(ctx, io, p->pro_r_lo, p->pro_r_hi, ctx->stream, &vqv))) return rc;
-    return launch_prologue(ctx, (const DevPacket *)p->pro.p, p->n_pro, p->pro_C, p->pro_fast, p->pro_smem_old, kLongN2,
-                           io->entry == LWB_ENTRY_VQ ? nullptr : io->coeffs, io->dense_floor, d_kinds, d_ys, (float *)ctx->spec.p - p->pro_c_lo, vqv);
-}
-
 extern "C" int lwb_plan_execute(lwb_plan *p)
 {
     if (!p) return LWB_ERR_INVALID;
     lwb_ctx *ctx = p->ctx;
-    if (p->captured && p->gen == ctx->state_gen && !getenv("LWB_FORCE_GENERIC")) {
-        // steady state: nothing about the batch or the stream states has changed shape since the
-        // descriptors were built -- the per-chain results in the caller's array are still right,
-        // the stream states stay (has, 1024): just launch.
-        CU(ctx, cudaSetDevice(ctx->device));
-        if (p->pro_captured) {             // residue entry: the front stages write ctx->spec, which the captured runs read
-            int prc = replay_front_stages(p);
-            if (prc) return prc;
-        }
-        constexpr uint32_t kTicketPool = 1024;
-        if (ctx->ticket_next % kTicketPool == 0)
-            CU(ctx, cudaMemsetAsync(ctx->ticket.p, 0, kTicketPool * sizeof(unsigned int), ctx->stream));
-        unsigned int *ticket = (unsigned int *)ctx->ticket.p + (ctx->ticket_next++ % kTicketPool);
-        if (long_launch(ctx->stream, (const LongRun *)p->runs.p, p->n_groups, p->pack, ticket, ctx->sm_count, p->i16))
-            return fail(ctx, LWB_ERR_CUDA, "long kernel launch", cudaGetLastError());
-        ctx->launches++;
-        return LWB_OK;
-    }
-    if (p->mixed_captured && p->gen == ctx->state_gen && !getenv("LWB_FORCE_GENERIC")) {
-        CU(ctx, cudaSetDevice(ctx->device));
-        if (p->mix_pro) {                  // residue entry: front stages over every packet, then the rounds on ctx->spec
-            const lwb_batch_io *io = &p->io;
-            const uint8_t *d_kinds;
-            const uint32_t *d_ys;
-            int prc = stage_floor_arrays(ctx, io, p->mix_pro_r_lo, p->mix_pro_r_hi, p->mix_pro_C, ctx->stream, &d_kinds, &d_ys);
-            if (prc) return prc;
-            VqView vqv;
-            if ((prc = stage_vq_arrays(ctx, io, p->mix_pro_r_lo, p->mix_pro_r_hi, ctx->stream, &vqv))) return prc;
-            prc = launch_prologue(ctx, p->mix_pro_pk, p->mix_pro_n, p->mix_pro_C, p->mix_pro_fast, p->mix_pro_smem_old, p->mix_pro_n2max,
-                                  io->entry == LWB_ENTRY_VQ ? nullptr : io->coeffs, p->mix_pro_dense ? io->dense_floor : nullptr, d_kinds, d_ys,
-                                  (float *)ctx->spec.p - p->mix_pro_c_lo, vqv);
-            if (prc) return prc;
-        }
-        return mixed_launch_rounds(ctx, p->mix_launch, p->mix_rounds);
-    }
-    return decode_chains_impl(ctx, p->chains, p->n_chains, &p->io, p);
+    if (!p->captured || p->gen != ctx->state_gen || first_batch_path() != 0)
+        return decode_chains_impl(ctx, p->chains, p->n_chains, &p->io, p);
+    // steady state: nothing about the batch or the stream states has changed shape since the descriptors were
+    // built -- the per-chain results in the caller's array and the stream states are still right: just launch.
+    // (Host floor arrays change from step to step and are uploaded again; device floor arrays are read in place.)
+    CU(ctx, cudaSetDevice(ctx->device));
+    int rc;
+    if (p->front.n && (rc = front_stages_run(ctx, &p->io, p->front))) return rc;    // they write ctx->spec, which the launch reads
+    if (p->mix_rounds.empty()) return launch_long(ctx, (const LongRun *)p->runs.p, p->n_groups, p->pack, p->i16);
+    return mixed_launch_rounds(ctx, p->mix_launch, p->mix_rounds);
 }
 
 // ---------------------------------------------------------------------------------------------

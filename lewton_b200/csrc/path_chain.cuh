@@ -14,7 +14,7 @@ static size_t chain_smem(unsigned maxc, int n1max, int np)
 }
 static int chain_np(unsigned maxc, int n1max, int wpc, bool residue)
 {
-    if (residue || wpc != 1 || getenv("LWB_CHAIN_NP1")) return 1;
+    if (residue || wpc != 1) return 1;
     int np = 4;
     while (np > 1 && chain_smem(maxc, n1max, np) > 64 * 1024) np >>= 1;
     return np;
@@ -58,7 +58,6 @@ __global__ void k_row_copy(const RowCopy *__restrict__ rc)
 
 static int mixed_launch_rounds(lwb_ctx *ctx, const MixLaunch &ml, const std::vector<MixRound> &rounds)
 {
-    constexpr uint32_t kTicketPool = 1024;
     cudaStream_t sm = ctx->stream;
     int rc = LWB_OK;
     for (const MixRound &rd : rounds) {
@@ -73,9 +72,8 @@ static int mixed_launch_rounds(lwb_ctx *ctx, const MixLaunch &ml, const std::vec
             ctx->launches++;
         }
         if (rd.nr) {
-            if (ctx->ticket_next % kTicketPool == 0)
-                CU(ctx, cudaMemsetAsync(ctx->ticket.p, 0, kTicketPool * sizeof(unsigned int), sm));
-            unsigned int *ticket = (unsigned int *)ctx->ticket.p + (ctx->ticket_next++ % kTicketPool);
+            unsigned int *ticket;
+            if ((rc = next_ticket(ctx, &ticket))) return rc;
             if (kLongNB != 1) return fail(ctx, LWB_ERR_INVALID, "mixed path needs one run per warp");
             // one pass over many short runs: the static deal with its deeper lookahead (k_long_s); rounds: tickets
             if (rd.flat ? long_launch_static(sm, (const LongRun *)ml.db + rd.r0, (uint32_t)rd.nr, ml.pack, ctx->sm_count, ml.i16, ml.w_short, ml.ls)
@@ -113,9 +111,6 @@ static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
 {
     *handled = false;
     const uint64_t gen_at_entry = ctx->state_gen;
-    if (plan) plan->mixed_captured = false;
-    if (const char *e = getenv("LWB_FORCE_GENERIC"))
-        if (std::strcmp(e, "1") == 0) return LWB_OK;          // "1": the four-kernel path; "2": no fused kernel only
     if (io->entry == LWB_ENTRY_VQ) return LWB_OK;            // (its residue stage runs inside the kernel, on dense vectors)
     const bool residue = io->entry == LWB_ENTRY_RESIDUE;
     const bool planar = is_planar(io->out_format);
@@ -259,7 +254,7 @@ static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         std::vector<MixRound> rounds(1, MixRound{0, 0, 0, 0, 0, n_launch});
         if ((rc = mixed_launch_rounds(ctx, ml, rounds))) return rc;
         if (capture) {
-            plan->mixed_captured = true;
+            plan->captured = true;
             plan->gen = gen_at_entry;
             plan->mix_launch = ml;
             plan->mix_rounds = std::move(rounds);

@@ -91,7 +91,7 @@ static int launch(lwb_ctx *ctx, K kernel, dim3 grid, dim3 block, size_t smem, Ar
 // channels and 16-byte aligned rows (prologue_is_fast); anything else takes the per-packet-CTA kernel.
 static bool prologue_is_fast(const DevPacket *h_pk, size_t n_pk, unsigned C, const float *res, const float *dense, const float *spec)
 {
-    bool fast = C <= 8 && n_pk * (size_t)C < 0xffffffffu && !getenv("LWB_OLD_PROLOGUE");
+    bool fast = C <= 8 && n_pk * (size_t)C < 0xffffffffu;
     for (size_t i = 0; fast && i < n_pk; i++) {
         const uint64_t e = h_pk[i].coeff_off;
         fast = (((res ? reinterpret_cast<uintptr_t>(res + e) : 0) | reinterpret_cast<uintptr_t>(spec + e) |
@@ -227,12 +227,78 @@ static int stage_vq_arrays(lwb_ctx *ctx, const lwb_batch_io *io, uint64_t r_lo, 
     return LWB_OK;
 }
 
+// ---------------------------------------------------------------------------------------------
+// front stages of the fused paths (FrontStages)
+// ---------------------------------------------------------------------------------------------
+// Writes the front-stage descriptors of packets [p0, p0 + n) of chain c, packet p0 starting at element offset `coeff`:
+// one DevPacket per packet, whatever its blocksize.  Returns the element offset behind the last one.
+static uint64_t write_front_packets(const lwb_chain *c, uint32_t p0, uint32_t n, uint64_t coeff, DevPacket *out)
+{
+    const lwb_setup *su = c->stream->setup;
+    for (uint32_t q = 0; q < n; q++) {
+        const uint8_t mode = c->mode_numbers[p0 + q];
+        const bool lng = su->host.mode_blockflag[mode] != 0;
+        const uint32_t nq = 1u << (lng ? su->bs1 : su->bs0);
+        DevPacket &d = out[q];
+        std::memset(&d, 0, sizeof(d));
+        d.setup = su->d_setup;
+        d.coeff_off = coeff;
+        d.pkt_index = c->packet_index + p0 + q;
+        d.n = (uint16_t)nq;
+        d.blockflag = lng;
+        d.mapping = su->host.mode_mapping[mode];
+        d.channels = su->channels;
+        coeff += (uint64_t)su->channels * (nq >> 1);
+    }
+    return coeff;
+}
+
+// The arenas the front stages read and write, biased by fs.c_lo: the caller's residues and dense floors (device
+// memory) or their staged copies in ctx->coeffs / ctx->dense (host memory), and ctx->spec.
+struct FrontArenas { const float *res, *dense; float *spec; };
+static FrontArenas front_arenas(lwb_ctx *ctx, const lwb_batch_io *io, const FrontStages &fs)
+{
+    const bool host = io->memory == LWB_MEM_HOST;
+    FrontArenas a;
+    a.res = io->entry == LWB_ENTRY_VQ ? nullptr : host ? (const float *)ctx->coeffs.p - fs.c_lo : io->coeffs;
+    a.dense = !fs.dense ? nullptr : host ? (const float *)ctx->dense.p - fs.c_lo : io->dense_floor;
+    a.spec = (float *)ctx->spec.p - fs.c_lo;
+    return a;
+}
+
+// Whether the two-kernel form takes fs's packets (host copy h_pk of its list).
+static bool front_stages_fast(lwb_ctx *ctx, const lwb_batch_io *io, const FrontStages &fs, const DevPacket *h_pk)
+{
+    const FrontArenas a = front_arenas(ctx, io, fs);
+    return prologue_is_fast(h_pk, fs.n, fs.C, a.res, a.dense, a.spec);
+}
+
+// Packets [k0, k0 + n) of fs on floor / VQ views the caller has staged.
+static int front_stages_launch(lwb_ctx *ctx, const lwb_batch_io *io, const FrontStages &fs, size_t k0, size_t n,
+                               const uint8_t *kinds, const uint32_t *ys, const VqView &vq)
+{
+    const FrontArenas a = front_arenas(ctx, io, fs);
+    return launch_prologue(ctx, fs.pk + k0, n, fs.C, fs.fast, fs.smem_old, fs.n2max, a.res, a.dense, kinds, ys, a.spec, vq);
+}
+
+// Stages the floor and VQ arrays of fs's packet rows on the compute stream (host arrays are uploaded, device arrays
+// read in place) and launches the front stages over every packet of fs.
+static int front_stages_run(lwb_ctx *ctx, const lwb_batch_io *io, const FrontStages &fs)
+{
+    const uint8_t *kinds;
+    const uint32_t *ys;
+    VqView vq;
+    int rc;
+    if ((rc = stage_floor_arrays(ctx, io, fs.r_lo, fs.r_hi, fs.C, ctx->stream, &kinds, &ys))) return rc;
+    if ((rc = stage_vq_arrays(ctx, io, fs.r_lo, fs.r_hi, ctx->stream, &vq))) return rc;
+    return front_stages_launch(ctx, io, fs, 0, fs.n, kinds, ys, vq);
+}
+
 struct DevArenas {
     const float *coeffs;      // device
     const float *dense;       // device or null
     const uint8_t *kinds;     // device or null
     const uint32_t *ys;       // device or null
-    uint64_t kinds_row0;      // first packet row uploaded
     void *pcm;                // device
     uint64_t coeff_base;      // element offset that device coeffs[0] corresponds to
     uint64_t pcm_base;        // element offset that device pcm[0] corresponds to
@@ -297,7 +363,7 @@ static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_bat
                 d.x_off = xo;
                 d.out_stride = pc.c->out_stride;
                 d.out_off = pc.c->out_offset - ar.pcm_base + (planar ? pp.sample_pos : pp.sample_pos * C);
-                d.pkt_index = pc.c->packet_index + start[ci] + k - ar.kinds_row0;
+                d.pkt_index = pc.c->packet_index + start[ci] + k;
                 d.prev_packet = k ? (int32_t)(di - 1) : -1;
                 d.prev_rs = k ? hp[di - 1].rs : 0;
                 d.state_stride = (uint32_t)state_stride(su);

@@ -97,6 +97,18 @@ static bool batch_is_uniform_long(lwb_ctx *ctx, const lwb_chain *chains, size_t 
     return true;
 }
 
+// One k_long launch over n_groups groups of runs.
+static int launch_long(lwb_ctx *ctx, const LongRun *runs, uint32_t n_groups, const float *pack, bool i16)
+{
+    unsigned int *ticket;
+    int rc = next_ticket(ctx, &ticket);
+    if (rc) return rc;
+    if (long_launch(ctx->stream, runs, n_groups, pack, ticket, ctx->sm_count, i16))
+        return fail(ctx, LWB_ERR_CUDA, "long kernel launch", cudaGetLastError());
+    ctx->launches++;
+    return LWB_OK;
+}
+
 // `spectrum_dev`: when non-null the spectrum has already been formed on the device (residue entry:
 // k_prologue wrote it to ctx->spec, element offset `spectrum_base` = its [0]); the input side of the
 // batch is then neither validated as a spectrum entry nor copied.
@@ -109,40 +121,23 @@ struct LongSlice {
 };
 
 static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, uint64_t epoch,
-                    bool *handled, const float *spectrum_dev = nullptr, uint64_t spectrum_base = 0,
-                    lwb_plan *plan = nullptr, bool capture_with_spectrum_dev = false, LongSlice slice = LongSlice())
+                    bool *handled, lwb_plan *plan = nullptr, const float *spectrum_dev = nullptr, uint64_t spectrum_base = 0,
+                    LongSlice slice = LongSlice())
 {
     *handled = false;
     const uint64_t gen_at_entry = ctx->state_gen;
-    if (plan) plan->captured = false;
     if (!spectrum_dev && io->entry != LWB_ENTRY_SPECTRUM) return LWB_OK;
-    if (io->out_format != LWB_OUT_F32_PLANAR && io->out_format != LWB_OUT_I16_PLANAR) return LWB_OK;
-    if (getenv("LWB_FORCE_GENERIC")) return LWB_OK;
+    if (!batch_is_uniform_long(ctx, chains, n_chains, io)) return LWB_OK;      // (the generic path reports bad chains)
     const bool i16 = io->out_format == LWB_OUT_I16_PLANAR;
     const size_t esz = i16 ? 2 : 4;
+    const float *pack = chains[0].stream->setup->host.tab[1].pack;          // one twiddle pack per launch
     std::vector<LongItem> items;
     items.reserve(n_chains);
-    const float *pack = nullptr;
     size_t chan_chains = 0;
     for (size_t i = 0; i < n_chains; i++) {
         lwb_chain *c = &chains[i];
-        if (!c->stream || c->stream->ctx != ctx || (c->n_packets && !c->mode_numbers)) return LWB_OK;   // generic path reports it
-        const lwb_stream *s = c->stream;
-        const lwb_setup *su = s->setup;
-        if (su->bs1 != kLongBs || !su->host.tab[1].pack) return LWB_OK;
-        if (pack && pack != su->host.tab[1].pack) return LWB_OK;          // one twiddle pack per launch
-        pack = su->host.tab[1].pack;
-        if ((c->out_offset & 3) || (c->out_stride & 3) || (c->coeff_offset & 3)) return LWB_OK;
-        if (s->has && s->plen != (uint32_t)kLongN2) return LWB_OK;
-        const uint32_t P = c->n_packets;
-        for (uint32_t k = 0; k < P; k++) {
-            const uint8_t m = c->mode_numbers[k];
-            if (m >= su->n_modes || !su->host.mode_blockflag[m]) return LWB_OK;
-            if (c->prev_window_flags && !c->prev_window_flags[k]) return LWB_OK;
-            if (c->next_window_flags && !c->next_window_flags[k]) return LWB_OK;
-        }
-        items.push_back(LongItem{c, P, s->has});
-        if (P) chan_chains += su->channels;
+        items.push_back(LongItem{c, c->n_packets, c->stream->has});
+        if (c->n_packets) chan_chains += c->stream->setup->channels;
     }
     *handled = true;
     // from here on this path owns the batch
@@ -170,25 +165,11 @@ static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_
     if (const char *e = getenv("LWB_LONG_TARGET_RUNS")) target_runs = (size_t)atol(e);
     const size_t min_run = 8;                              // packets per run below which a cut costs > 12%
     int rc;
-    constexpr uint32_t kTicketPool = 1024;
-    if (!ctx->ticket.p) {
-        if ((rc = ensure(ctx, ctx->ticket, kTicketPool * sizeof(unsigned int)))) return rc;
-        for (int k = 0; k < 2; k++) {
-            CU(ctx, cudaEventCreateWithFlags(&ctx->ev_desc[k], cudaEventDisableTiming));
-            CU(ctx, cudaEventCreateWithFlags(&ctx->ev_kdone[k], cudaEventDisableTiming));
-        }
-    }
 
     const bool host = io->memory == LWB_MEM_HOST;          // the pcm arena is in host memory
     const bool in_host = host && !spectrum_dev;            // ... and so is the coefficient arena
-    // host memory: chunks of chains, H2D / kernel / D2H of consecutive chunks overlap on three streams
-    size_t n_chunks = 1;
-    if (host) {
-        const size_t bytes = (size_t)(c_hi - c_lo) * 4;
-        n_chunks = std::min<size_t>(std::max<size_t>(1, bytes >> 25), std::min<size_t>(8, items.size()));   // profiles/e2e_chunks_r1.log
-        if (const char *e = getenv("LWB_E2E_CHUNKS")) n_chunks = std::max<size_t>(1, std::min<size_t>((size_t)atol(e), std::min<size_t>(64, items.size())));
-        if (slice.active) n_chunks = 1;                    // the caller's slices are the chunks
-    }
+    // host memory: chunks of chains (the caller's slices are the chunks)
+    const size_t n_chunks = host && !slice.active ? host_chunks((size_t)(c_hi - c_lo) * 4, items.size()) : 1;
     const float *d_coeffs = spectrum_dev ? spectrum_dev : io->coeffs;
     char *d_pcm = (char *)io->pcm;
     uint64_t cbase = spectrum_dev ? spectrum_base : 0, obase = 0;
@@ -202,17 +183,7 @@ static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_
         else if (o_hi > o_lo && (rc = ensure(ctx, ctx->pcm, (size_t)(o_hi - o_lo) * esz))) return rc;
         d_pcm = (char *)ctx->pcm.p;
         obase = o_lo;
-        if (!ctx->ev_in[0])
-            for (int k = 0; k < 65; k++) {
-                if (k < 64) CU(ctx, cudaEventCreateWithFlags(&ctx->ev_in[k], cudaEventDisableTiming));
-                CU(ctx, cudaEventCreateWithFlags(&ctx->ev_done[k], cudaEventDisableTiming));
-            }
-        // the copy streams must not run ahead of work already queued on the compute stream that
-        // still reads/writes the arenas (previous call): order them behind it
-        if (!slice.active) {
-            CU(ctx, cudaEventRecord(ctx->ev_done[64], ctx->stream));
-            CU(ctx, cudaStreamWaitEvent(ctx->copy_in, ctx->ev_done[64], 0));
-        }
+        if (!slice.active && (rc = order_copies_behind_compute(ctx))) return rc;
     }
     // count runs
     std::vector<size_t> cuts(items.size(), 1);
@@ -234,7 +205,7 @@ static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_
     ctx->runs_par ^= 1;
     // a plan (device-memory batches) owns its descriptor buffer so that later executions can reuse it
     // (runs that read ctx->spec stay valid because growing any ctx arena bumps state_gen, see ensure())
-    const bool capture = plan && !host && (!spectrum_dev || capture_with_spectrum_dev) && n_chunks == 1;
+    const bool capture = plan && !host && n_chunks == 1;
     DevBuf &rb = capture ? plan->runs : ctx->runs_buf[par];
     if ((rc = ensure(ctx, rb, cap_runs * sizeof(LongRun)))) return rc;
     LongRun *const d_runs_base = (LongRun *)rb.p;
@@ -318,12 +289,7 @@ static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_
             CU(ctx, cudaEventRecord(ctx->ev_in[k], ctx->copy_in));
             CU(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_in[k], 0));
         }
-        if (ctx->ticket_next % kTicketPool == 0)
-            CU(ctx, cudaMemsetAsync(ctx->ticket.p, 0, kTicketPool * sizeof(unsigned int), ctx->stream));
-        unsigned int *ticket = (unsigned int *)ctx->ticket.p + (ctx->ticket_next++ % kTicketPool);
-        if (long_launch(ctx->stream, d_runs_base + cp.r0, (uint32_t)(cp.nr / kLongNB), pack, ticket, ctx->sm_count, i16))
-            return fail(ctx, LWB_ERR_CUDA, "long kernel launch", cudaGetLastError());
-        ctx->launches++;
+        if ((rc = launch_long(ctx, d_runs_base + cp.r0, (uint32_t)(cp.nr / kLongNB), pack, i16))) return rc;
         if (host && cp.ko_hi > cp.ko_lo) {
             const size_t evk = slice.active ? (size_t)slice.ev_slot : k;
             CU(ctx, cudaEventRecord(ctx->ev_done[evk], ctx->stream));
@@ -349,58 +315,6 @@ static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_
     return LWB_OK;
 }
 
-// Residue-entry batches whose every packet is a long block with long neighbours (what the fused
-// kernel takes) -- decided from the generic plan.
-static bool plan_is_long(const std::vector<PlanChain> &plan, const lwb_batch_io *io)
-{
-    if (io->out_format != LWB_OUT_F32_PLANAR && io->out_format != LWB_OUT_I16_PLANAR) return false;
-    if (getenv("LWB_FORCE_GENERIC")) return false;
-    for (auto &pc : plan) {
-        const lwb_setup *su = pc.c->stream->setup;
-        if (su->bs1 != kLongBs || !su->host.tab[1].pack) return false;
-        if (pc.c->status != LWB_OK) return false;
-        for (auto &pp : pc.pk) {
-            if (!pp.g.blockflag || pp.g.ls != 0 || pp.g.rs != (pp.g.n >> 1) || pp.g.re != pp.g.n) return false;
-            if (pp.plen != 0 && pp.plen != (pp.g.n >> 1)) return false;
-        }
-    }
-    return true;
-}
-
-// k_prologue over every packet of the plan: ctx->spec[coeff_off] <- floor x decoupled residue.
-static int run_prologue_all(lwb_ctx *ctx, std::vector<PlanChain> &plan, const DevArenas &ar, size_t spec_elems)
-{
-    size_t n_desc = 0;
-    for (auto &pc : plan) n_desc += pc.pk.size();
-    if (!n_desc) return LWB_OK;
-    int rc;
-    if ((rc = ensure_pinned(ctx, n_desc * sizeof(DevPacket)))) return rc;
-    if ((rc = ensure(ctx, ctx->desc, n_desc * sizeof(DevPacket)))) return rc;
-    if ((rc = ensure(ctx, ctx->spec, spec_elems * sizeof(float)))) return rc;
-    CU(ctx, cudaStreamSynchronize(ctx->stream));          // pinned descriptor staging is reused
-    DevPacket *hp = (DevPacket *)ctx->h_desc;
-    size_t di = 0;
-    for (auto &pc : plan) {
-        const lwb_setup *su = pc.c->stream->setup;
-        for (size_t k = 0; k < pc.pk.size(); k++) {
-            const PlanPacket &pp = pc.pk[k];
-            DevPacket &d = hp[di++];
-            std::memset(&d, 0, sizeof(d));
-            d.setup = su->d_setup;
-            d.coeff_off = pp.coeff_off - ar.coeff_base;
-            d.pkt_index = pc.c->packet_index + k - ar.kinds_row0;
-            d.n = (uint16_t)pp.g.n;
-            d.blockflag = pp.g.blockflag;
-            d.mapping = pp.g.mapping;
-            d.channels = su->channels;
-        }
-    }
-    CU(ctx, cudaMemcpyAsync(ctx->desc.p, hp, n_desc * sizeof(DevPacket), cudaMemcpyHostToDevice, ctx->stream));
-    return launch_prologue(ctx, (const DevPacket *)ctx->desc.p, hp, n_desc, plan[0].c->stream->setup->channels, prologue_smem_of(plan),
-                           ar.coeffs, ar.dense, ar.kinds, ar.ys, (float *)ctx->spec.p, ar.vq);
-}
-
-
 // Residue-entry batches whose every packet is a long block with long neighbours: the front stages
 // (k_floor1_segments + k_prologue_fused, or k_prologue) form the spectrum on the device, the fused kernel does the
 // rest.  Planned straight from the chain list like try_long (no per-packet PlanChain vectors); a prepared batch
@@ -410,7 +324,7 @@ static int try_long_residue(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, co
                             lwb_plan *plan)
 {
     *handled = false;
-    if (io->entry == LWB_ENTRY_SPECTRUM || getenv("LWB_FORCE_GENERIC")) return LWB_OK;
+    if (io->entry == LWB_ENTRY_SPECTRUM) return LWB_OK;
     if (!batch_is_uniform_long(ctx, chains, n_chains, io)) return LWB_OK;
     const bool vq = io->entry == LWB_ENTRY_VQ;
     if (!io->floor_kind) return fail(ctx, LWB_ERR_INVALID, "residue entry needs floor_kind");
@@ -446,26 +360,25 @@ static int try_long_residue(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, co
     cudaStream_t sm = ctx->stream;
     const size_t elems = (size_t)(c_hi - c_lo);
     const bool host = io->memory == LWB_MEM_HOST;
-    const float *d_res = vq ? nullptr : io->coeffs, *d_dense = need_dense ? io->dense_floor : nullptr;
     if (host) {
-        if (!vq) {
-            if ((rc = ensure(ctx, ctx->coeffs, elems * 4))) return rc;
-            d_res = (const float *)ctx->coeffs.p - c_lo;
-        }
-        if (need_dense) {
-            if ((rc = ensure(ctx, ctx->dense, elems * 4))) return rc;
-            d_dense = (const float *)ctx->dense.p - c_lo;
-        }
+        if (!vq && (rc = ensure(ctx, ctx->coeffs, elems * 4))) return rc;
+        if (need_dense && (rc = ensure(ctx, ctx->dense, elems * 4))) return rc;
     }
     if ((rc = ensure(ctx, ctx->spec, elems * 4))) return rc;
-    float *d_spec = (float *)ctx->spec.p - c_lo;
-    // front-stage descriptors: absolute element offsets and packet rows (the arena pointers are biased instead)
-    const DevPacket *d_pk;
-    bool fast;
-    const size_t smem_old = prologue_smem((int)C, kLongBs);
-    if (plan && plan->pro_captured && plan->n_pro == n_pk) {
-        d_pk = (const DevPacket *)plan->pro.p;
-        fast = plan->pro_fast;
+    FrontStages fs;
+    fs.n = n_pk;
+    fs.C = C;
+    fs.smem_old = prologue_smem((int)C, kLongBs);
+    fs.n2max = kLongN2;
+    fs.c_lo = c_lo;
+    fs.r_lo = r_lo;
+    fs.r_hi = r_hi;
+    fs.dense = need_dense;
+    if (plan && plan->pro.p && plan->front.pk == plan->pro.p && plan->front.n == n_pk) {
+        // a prepared batch re-planned (host memory: every execution): the packet list of the previous execution
+        // depends only on the plan's chain and mode arrays
+        fs.pk = plan->front.pk;
+        fs.fast = plan->front.fast;
     } else {
         Staging *st;
         if ((rc = acquire_staging(ctx, n_pk * sizeof(DevPacket), &st))) return rc;
@@ -474,43 +387,20 @@ static int try_long_residue(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, co
         DevPacket *hp = (DevPacket *)st->h;
         size_t di = 0;
         for (size_t i = 0; i < n_chains; i++) {
-            const lwb_chain *c = &chains[i];
-            const lwb_setup *su = c->stream->setup;
-            for (uint32_t k = 0; k < c->n_packets; k++) {
-                DevPacket &d = hp[di++];
-                std::memset(&d, 0, sizeof(d));
-                d.setup = su->d_setup;
-                d.coeff_off = c->coeff_offset + (uint64_t)k * C * kLongN2;
-                d.pkt_index = c->packet_index + k;
-                d.n = kLongN;
-                d.blockflag = 1;
-                d.mapping = su->host.mode_mapping[c->mode_numbers[k]];
-                d.channels = (uint8_t)C;
-            }
+            write_front_packets(&chains[i], 0, chains[i].n_packets, chains[i].coeff_offset, hp + di);
+            di += chains[i].n_packets;
         }
-        fast = prologue_is_fast(hp, n_pk, C, d_res, d_dense, d_spec);
+        fs.pk = (const DevPacket *)db.p;
+        fs.fast = front_stages_fast(ctx, io, fs, hp);
         CU(ctx, cudaMemcpyAsync(db.p, hp, n_pk * sizeof(DevPacket), cudaMemcpyHostToDevice, sm));
         CU(ctx, cudaEventRecord(st->ev, sm));
         st->pending = true;
-        d_pk = (const DevPacket *)db.p;
-        if (plan) {
-            plan->pro_captured = true;
-            plan->pro_fast = fast;
-            plan->n_pro = n_pk;
-            plan->pro_smem_old = smem_old;
-            plan->pro_C = C;
-            plan->pro_c_lo = c_lo; plan->pro_c_hi = c_hi; plan->pro_r_lo = r_lo; plan->pro_r_hi = r_hi;
-        }
     }
+    if (plan) plan->front = fs;
     if (!host) {
-        const uint8_t *d_kinds;
-        const uint32_t *d_ys;
-        if ((rc = stage_floor_arrays(ctx, io, r_lo, r_hi, C, sm, &d_kinds, &d_ys))) return rc;
-        VqView vqv;
-        if ((rc = stage_vq_arrays(ctx, io, r_lo, r_hi, sm, &vqv))) return rc;
-        if ((rc = launch_prologue(ctx, d_pk, n_pk, C, fast, smem_old, kLongN2, d_res, d_dense, d_kinds, d_ys, d_spec, vqv))) return rc;
+        if ((rc = front_stages_run(ctx, io, fs))) return rc;
         bool h2 = false;
-        rc = try_long(ctx, chains, n_chains, io, epoch, &h2, (const float *)ctx->spec.p, c_lo, plan, true);
+        rc = try_long(ctx, chains, n_chains, io, epoch, &h2, plan, (const float *)ctx->spec.p, c_lo);
         if (rc) return rc;
         if (!h2) return fail(ctx, LWB_ERR_INVALID, "internal: uniform long residue batch refused by the fused path");
         return LWB_OK;
@@ -518,8 +408,7 @@ static int try_long_residue(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, co
     // Host memory: slices of chains flow through three streams -- copy_in brings a slice's inputs (dense residues, or
     // VQ runs / entries, and its floor rows), the compute stream runs its front stages and the fused kernel, copy_out
     // takes its PCM home -- so that H2D, kernels and D2H of consecutive slices overlap (the link is duplex).
-    size_t n_sl = std::min<size_t>(std::max<size_t>(1, (n_pk * (size_t)C * kLongN2 * 4) >> 25), std::min<size_t>(8, n_chains));
-    if (const char *e = getenv("LWB_E2E_CHUNKS")) n_sl = std::max<size_t>(1, std::min<size_t>((size_t)atol(e), std::min<size_t>(32, n_chains)));
+    const size_t n_sl = host_chunks(n_pk * (size_t)C * kLongN2 * 4, n_chains);
     // whole-batch staging (absolute rows / offsets address it); each slice copies its own part
     const size_t esz = io->out_format == LWB_OUT_I16_PLANAR ? 2 : 4;
     uint64_t o_lo = ~0ull, o_hi = 0;
@@ -558,15 +447,7 @@ static int try_long_residue(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, co
     } else if ((rc = stage_vq_arrays(ctx, io, r_lo, r_hi, sm, &vqv))) {
         return rc;
     }
-    if (!ctx->ev_in[0])
-        for (int k = 0; k < 65; k++) {
-            if (k < 64) CU(ctx, cudaEventCreateWithFlags(&ctx->ev_in[k], cudaEventDisableTiming));
-            CU(ctx, cudaEventCreateWithFlags(&ctx->ev_done[k], cudaEventDisableTiming));
-        }
-    // the copy streams must not run ahead of work already queued on the compute stream (previous call, descriptor upload)
-    CU(ctx, cudaEventRecord(ctx->ev_done[64], sm));
-    CU(ctx, cudaStreamWaitEvent(ctx->copy_in, ctx->ev_done[64], 0));
-    CU(ctx, cudaStreamWaitEvent(ctx->copy_out, ctx->ev_done[64], 0));
+    if ((rc = order_copies_behind_compute(ctx))) return rc;
     size_t pk0 = 0;
     for (size_t sl = 0; sl < n_sl; sl++) {
         const size_t i0 = n_chains * sl / n_sl, i1 = n_chains * (sl + 1) / n_sl;
@@ -604,7 +485,7 @@ static int try_long_residue(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, co
         }
         CU(ctx, cudaEventRecord(ctx->ev_in[sl], ci));
         CU(ctx, cudaStreamWaitEvent(sm, ctx->ev_in[sl], 0));
-        if ((rc = launch_prologue(ctx, d_pk + pk0, npk_sl, C, fast, smem_old, kLongN2, d_res, d_dense, d_kinds, d_ys, d_spec, vqv))) return rc;
+        if ((rc = front_stages_launch(ctx, io, fs, pk0, npk_sl, d_kinds, d_ys, vqv))) return rc;
         pk0 += npk_sl;
         bool h2 = false;
         LongSlice ls;
@@ -612,7 +493,7 @@ static int try_long_residue(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, co
         ls.o_lo = o_lo;
         ls.o_hi = o_hi;
         ls.ev_slot = (int)sl;
-        rc = try_long(ctx, chains + i0, i1 - i0, io, epoch, &h2, (const float *)ctx->spec.p, c_lo, nullptr, false, ls);
+        rc = try_long(ctx, chains + i0, i1 - i0, io, epoch, &h2, nullptr, (const float *)ctx->spec.p, c_lo, ls);
         if (rc) return rc;
         if (!h2) return fail(ctx, LWB_ERR_INVALID, "internal: uniform long residue batch refused by the fused path");
     }

@@ -6,19 +6,13 @@
 #pragma once
 
 struct MidGroup { LongRun r[4]; uint32_t n_packets; };
-static size_t n_pk_all(const lwb_chain *chains, size_t n_chains)
-{
-    size_t n = 0;
-    for (size_t i = 0; i < n_chains; i++) n += chains[i].n_packets;
-    return n;
-}
 
 static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, uint64_t epoch, bool *handled,
                    lwb_plan *plan = nullptr)
 {
     *handled = false;
     const uint64_t gen_at_entry = ctx->state_gen;
-    if (getenv("LWB_FORCE_GENERIC") || getenv("LWB_NO_MID")) return LWB_OK;
+    if (getenv("LWB_NO_MID")) return LWB_OK;
     if (io->out_format != LWB_OUT_F32_PLANAR && io->out_format != LWB_OUT_I16_PLANAR) return LWB_OK;
     const bool vq = io->entry == LWB_ENTRY_VQ, residue = io->entry != LWB_ENTRY_SPECTRUM;
     if (residue && !io->floor_kind) return LWB_OK;            // (the chain kernel words the error)
@@ -60,7 +54,6 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
     if (!pack || !n_runs) return LWB_OK;
     const size_t kMidN2 = 1024u >> kb, NBg = (size_t)1 << kb;
     *handled = true;
-    if (plan) plan->mixed_captured = false;
 
     const bool host = io->memory == LWB_MEM_HOST;
     cudaStream_t sm = ctx->stream;
@@ -90,7 +83,7 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
         o_hi = std::max(o_hi, c->out_offset + (uint64_t)(C - 1) * c->out_stride + c->n_samples);
     }
     if (need_dense && !io->dense_floor) return fail(ctx, LWB_ERR_INVALID, "dense_floor missing");
-    const float *d_coeffs = vq ? nullptr : io->coeffs, *d_dense = need_dense ? io->dense_floor : nullptr;
+    const float *d_coeffs = vq ? nullptr : io->coeffs;
     char *d_pcm = (char *)io->pcm;
     if (host) {
         if (o_hi > o_lo && (rc = ensure(ctx, ctx->pcm, (size_t)(o_hi - o_lo) * esz))) return rc;
@@ -102,57 +95,45 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
         if (need_dense) {
             if ((rc = ensure(ctx, ctx->dense, (size_t)(c_hi - c_lo) * 4))) return rc;
             CU(ctx, cudaMemcpyAsync(ctx->dense.p, io->dense_floor + c_lo, (size_t)(c_hi - c_lo) * 4, cudaMemcpyHostToDevice, sm));
-            d_dense = (const float *)ctx->dense.p - c_lo;
         }
         d_pcm = (char *)ctx->pcm.p - o_lo * esz;
     }
     // A prepared batch in device memory owns its descriptors (run groups, then the front stages' packet list) and replays
-    // them while no stream changes shape (lwb_plan_execute: mix_pro, then the round).
+    // them while no stream changes shape (lwb_plan_execute).
     const bool capture = plan && !host;
     DevBuf &dbuf = capture ? plan->mix : ctx->cdesc;
     const size_t NBcap = (size_t)1 << kb;
     const size_t off_pro = (n_runs * NBcap * sizeof(LongRun) + 15) & ~(size_t)15;      // (an upper bound: every run its own group)
-    if ((rc = ensure(ctx, dbuf, off_pro + (residue ? n_pk_all(chains, n_chains) * sizeof(DevPacket) : 0) + 16))) return rc;
-    bool pro_fast = false;
+    if ((rc = ensure(ctx, dbuf, off_pro + n_pk * sizeof(DevPacket) + 16))) return rc;
+    FrontStages fs;
     if (residue) {
         // front stages over every packet of the batch: residue (or VQ records) + floors -> spectrum arena, same element
         // offsets as the coefficient arena
         if ((rc = ensure(ctx, ctx->spec, (size_t)(c_hi - c_lo) * 4))) return rc;
-        float *d_spec = (float *)ctx->spec.p - c_lo;
+        DevPacket *d_pro = (DevPacket *)((char *)dbuf.p + off_pro);
+        fs.pk = d_pro;
+        fs.n = n_pk;
+        fs.C = (unsigned)uniform_c;
+        fs.smem_old = prologue_smem(uniform_c, 11 - kb);
+        fs.n2max = (int)kMidN2;
+        fs.c_lo = c_lo;
+        fs.r_lo = r_lo;
+        fs.r_hi = r_hi;
+        fs.dense = need_dense;
         Staging *stp;
         if ((rc = acquire_staging(ctx, n_pk * sizeof(DevPacket), &stp))) return rc;
         DevPacket *hp = (DevPacket *)stp->h;
         size_t di = 0;
         for (size_t i = 0; i < n_chains; i++) {
-            const lwb_chain *c = &chains[i];
-            const lwb_setup *su = c->stream->setup;
-            for (uint32_t k = 0; k < c->n_packets; k++) {
-                DevPacket &d = hp[di++];
-                std::memset(&d, 0, sizeof(d));
-                d.setup = su->d_setup;
-                d.coeff_off = c->coeff_offset + (uint64_t)k * su->channels * kMidN2;
-                d.pkt_index = c->packet_index + k;
-                d.n = (uint16_t)(2 * kMidN2);
-                d.blockflag = 1;
-                d.mapping = su->host.mode_mapping[c->mode_numbers[k]];
-                d.channels = (uint8_t)su->channels;
-            }
+            write_front_packets(&chains[i], 0, chains[i].n_packets, chains[i].coeff_offset, hp + di);
+            di += chains[i].n_packets;
         }
-        const bool fast = prologue_is_fast(hp, n_pk, (unsigned)uniform_c, d_coeffs, d_dense, d_spec);
-        DevPacket *d_pro = (DevPacket *)((char *)dbuf.p + off_pro);
+        fs.fast = front_stages_fast(ctx, io, fs, hp);
         CU(ctx, cudaMemcpyAsync(d_pro, hp, n_pk * sizeof(DevPacket), cudaMemcpyHostToDevice, sm));
         CU(ctx, cudaEventRecord(stp->ev, sm));
         stp->pending = true;
-        const uint8_t *d_kinds = nullptr;
-        const uint32_t *d_ys = nullptr;
-        if ((rc = stage_floor_arrays(ctx, io, r_lo, r_hi, (unsigned)uniform_c, sm, &d_kinds, &d_ys))) return rc;
-        VqView vqv;
-        if ((rc = stage_vq_arrays(ctx, io, r_lo, r_hi, sm, &vqv))) return rc;
-        pro_fast = fast;
-        if ((rc = launch_prologue(ctx, d_pro, n_pk, (unsigned)uniform_c, fast, prologue_smem(uniform_c, 11 - kb),
-                                  (int)kMidN2, d_coeffs, d_dense, d_kinds, d_ys, d_spec, vqv)))
-            return rc;
-        d_coeffs = d_spec;                                  // k_mid reads the spectrum
+        if ((rc = front_stages_run(ctx, io, fs))) return rc;
+        d_coeffs = (const float *)ctx->spec.p - c_lo;       // k_mid reads the spectrum
     }
     // runs, then groups of two runs of equal length (an odd one gets a dummy partner), longest first, dealt balanced
     std::vector<LongRun> runs;
@@ -219,21 +200,11 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
     std::vector<MixRound> rounds(1, rd);
     if ((rc = mixed_launch_rounds(ctx, ml, rounds))) return rc;
     if (capture) {
-        plan->mixed_captured = true;
+        plan->captured = true;
         plan->gen = gen_at_entry;
+        plan->front = fs;                   // (no packets: spectrum entry)
         plan->mix_launch = ml;
         plan->mix_rounds = std::move(rounds);
-        plan->mix_pro = residue;
-        if (residue) {                      // replayed by lwb_plan_execute in front of the round
-            plan->mix_pro_pk = (const DevPacket *)((char *)dbuf.p + off_pro);
-            plan->mix_pro_n = n_pk;
-            plan->mix_pro_fast = pro_fast;
-            plan->mix_pro_C = (unsigned)uniform_c;
-            plan->mix_pro_smem_old = prologue_smem(uniform_c, 11 - kb);
-            plan->mix_pro_c_lo = c_lo; plan->mix_pro_r_lo = r_lo; plan->mix_pro_r_hi = r_hi;
-            plan->mix_pro_dense = need_dense;
-            plan->mix_pro_n2max = (int)kMidN2;
-        }
     }
     if (host) {
         if (o_hi > o_lo)

@@ -42,8 +42,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
 {
     *handled = false;
     const uint64_t gen_at_entry = ctx->state_gen;
-    if (plan) plan->mixed_captured = false;
-    if (getenv("LWB_FORCE_GENERIC") || getenv("LWB_NO_MIXED")) return LWB_OK;
+    if (getenv("LWB_NO_MIXED")) return LWB_OK;
     if (io->out_format != LWB_OUT_F32_PLANAR && io->out_format != LWB_OUT_I16_PLANAR) return LWB_OK;
     const bool vq = io->entry == LWB_ENTRY_VQ;
     const bool residue = io->entry != LWB_ENTRY_SPECTRUM;
@@ -280,7 +279,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
     if (max_rounds) {
         const bool host = io->memory == LWB_MEM_HOST;
         cudaStream_t sm = ctx->stream;
-        const float *d_coeffs = io->coeffs, *d_dense = io->dense_floor;
+        const float *d_coeffs = io->coeffs;
         char *d_pcm = (char *)io->pcm;
         if (vq) d_coeffs = nullptr;
         if (host) {
@@ -289,27 +288,12 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                 if ((rc = ensure(ctx, ctx->coeffs, (size_t)(c_hi - c_lo) * 4))) return rc;
                 d_coeffs = (const float *)ctx->coeffs.p - c_lo;       // the copies themselves go chunk by chunk, below
             }
-            if (need_dense) {
-                if ((rc = ensure(ctx, ctx->dense, (size_t)(c_hi - c_lo) * 4))) return rc;
-                d_dense = (const float *)ctx->dense.p - c_lo;
-            }
+            if (need_dense && (rc = ensure(ctx, ctx->dense, (size_t)(c_hi - c_lo) * 4))) return rc;
             d_pcm = (char *)ctx->pcm.p - o_lo * esz;
-            if (!ctx->ev_in[0])
-                for (int k = 0; k < 65; k++) {
-                    if (k < 64) CU(ctx, cudaEventCreateWithFlags(&ctx->ev_in[k], cudaEventDisableTiming));
-                    CU(ctx, cudaEventCreateWithFlags(&ctx->ev_done[k], cudaEventDisableTiming));
-                }
-            // the copy streams must not run ahead of work already queued on the compute stream
-            CU(ctx, cudaEventRecord(ctx->ev_done[64], sm));
-            CU(ctx, cudaStreamWaitEvent(ctx->copy_in, ctx->ev_done[64], 0));
-            CU(ctx, cudaStreamWaitEvent(ctx->copy_out, ctx->ev_done[64], 0));
+            if ((rc = order_copies_behind_compute(ctx))) return rc;
         }
-        // host memory: chunks of chains, so that H2D / kernels / D2H of consecutive chunks overlap on three streams
-        size_t n_chunks = 1;
-        if (host) {
-            n_chunks = std::min<size_t>(std::max<size_t>(1, ((size_t)(c_hi - c_lo) * 4) >> 25), std::min<size_t>(8, n_chains));
-            if (const char *e = getenv("LWB_E2E_CHUNKS")) n_chunks = std::max<size_t>(1, std::min<size_t>((size_t)atol(e), std::min<size_t>(64, n_chains)));
-        }
+        // host memory: chunks of chains
+        const size_t n_chunks = host ? host_chunks((size_t)(c_hi - c_lo) * 4, n_chains) : 1;
         const uint8_t *d_kinds = nullptr;
         const uint32_t *d_ys = nullptr;
         if (residue && (rc = stage_floor_arrays(ctx, io, r_lo, r_hi, (unsigned)uniform_c, sm, &d_kinds, &d_ys))) return rc;
@@ -357,13 +341,12 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
             }
             ck.round_cut.assign(max_rounds, 1);
             ck.round_cut_s.assign(max_rounds, 1);
-            if (!getenv("LWB_MIXED_NO_CUTS"))
-                for (size_t r = 0; r < max_rounds; r++) {
-                    if (round_long[r] && round_long[r] < target_runs)
-                        ck.round_cut[r] = (uint32_t)std::min<size_t>(16, (target_runs + round_long[r] - 1) / round_long[r]);
-                    if (round_short[r] && round_short[r] < target_sruns)
-                        ck.round_cut_s[r] = (uint32_t)std::min<size_t>(64, (target_sruns + round_short[r] - 1) / round_short[r]);
-                }
+            for (size_t r = 0; r < max_rounds; r++) {
+                if (round_long[r] && round_long[r] < target_runs)
+                    ck.round_cut[r] = (uint32_t)std::min<size_t>(16, (target_runs + round_long[r] - 1) / round_long[r]);
+                if (round_short[r] && round_short[r] < target_sruns)
+                    ck.round_cut_s[r] = (uint32_t)std::min<size_t>(64, (target_sruns + round_short[r] - 1) / round_short[r]);
+            }
             for (size_t i = ck.i0; i < ck.i1; i++)
                 for (uint32_t q = 0; q < walks[i].n_seg; q++) {
                     const Seg &sg = segs[walks[i].seg0 + q];
@@ -416,24 +399,10 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         size_t wr = 0, ws = 0, wc = 0, wp = 0;
         std::vector<LongRun> tmp_lr;
         std::vector<ShortRun> tmp_sr;
-        // front-stage descriptors of one segment (residue entry): one per packet, whatever its blocksize
-        auto emit_pro = [&](const lwb_chain *c, const lwb_setup *su, const Seg &sg) {
-            uint64_t co = sg.coeff;
-            for (uint32_t q = 0; q < sg.n; q++) {
-                const uint8_t mode = c->mode_numbers[sg.p0 + q];
-                const bool lng = su->host.mode_blockflag[mode] != 0;
-                const uint32_t nq = 1u << (lng ? su->bs1 : su->bs0);
-                DevPacket &dp = h_pro[wp++];
-                std::memset(&dp, 0, sizeof(dp));
-                dp.setup = su->d_setup;
-                dp.coeff_off = co;
-                dp.pkt_index = c->packet_index + sg.p0 + q;
-                dp.n = (uint16_t)nq;
-                dp.blockflag = lng;
-                dp.mapping = su->host.mode_mapping[mode];
-                dp.channels = (uint8_t)su->channels;
-                co += (uint64_t)su->channels * (nq >> 1);
-            }
+        // front-stage descriptors of one segment (residue entry)
+        auto emit_pro = [&](const lwb_chain *c, const Seg &sg) {
+            write_front_packets(c, sg.p0, sg.n, sg.coeff, h_pro + wp);
+            wp += sg.n;
         };
         for (Chunk &ck : chunks) {
             ck.rounds.assign(max_rounds, MixRound{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0});
@@ -497,7 +466,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                                 }
                             }
                         }
-                        if (residue) emit_pro(c, su, sg);
+                        if (residue) emit_pro(c, sg);
                       }
                     }
                 // short-block runs: one per channel (and per cut) of every short segment of this round
@@ -551,7 +520,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                             }
                         }
                     }
-                    if (residue) emit_pro(c, su, sg);
+                    if (residue) emit_pro(c, sg);
                   }
                 }
                 for (size_t i = ck.i0; i < ck.i1; i++) {
@@ -563,7 +532,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                     const lwb_chain *c = &chains[i];
                     const lwb_stream *s = c->stream;
                     const lwb_setup *su = s->setup;
-                    if (residue) emit_pro(c, su, sg);
+                    if (residue) emit_pro(c, sg);
                     ChainDesc &d = h_cd[wc++];
                     std::memset(&d, 0, sizeof(d));
                     d.setup = su->d_setup;
@@ -619,22 +588,22 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         CU(ctx, cudaMemcpyAsync(db, hb, total, cudaMemcpyHostToDevice, sm));
         CU(ctx, cudaEventRecord(st->ev, sm));
         st->pending = true;
-        constexpr uint32_t kTicketPool = 1024;
-        if (!ctx->ticket.p) {
-            if ((rc = ensure(ctx, ctx->ticket, kTicketPool * sizeof(unsigned int)))) return rc;
-            for (int k = 0; k < 2; k++) {
-                CU(ctx, cudaEventCreateWithFlags(&ctx->ev_desc[k], cudaEventDisableTiming));
-                CU(ctx, cudaEventCreateWithFlags(&ctx->ev_kdone[k], cudaEventDisableTiming));
-            }
-        }
         MixLaunch ml;
         ml.db = db; ml.off_sr = off_sr; ml.off_cd = off_cd; ml.off_by = off_by; ml.off_rc = off_rc; ml.off_sg = off_sg; ml.pack = pack; ml.spack = spack; ml.w_short = w_short; ml.mpack = nullptr; ml.mid_kb = 0; ml.ls = ls_long;
         ml.i16 = i16; ml.residue = false; ml.out_format = io->out_format; ml.warps = maxc * wpc; ml.smem = smem;
         ml.n1max = n1max; ml.wpc = wpc; ml.np = np; ml.coeffs = residue ? d_spec : d_coeffs; ml.dense = nullptr; ml.kinds = nullptr; ml.ys = nullptr;
         ml.pcm = d_pcm;
-        bool pro_fast = false;
-        if (residue && n_pro)
-            pro_fast = prologue_is_fast(h_pro, n_pro, maxc, d_coeffs, need_dense ? d_dense : nullptr, d_spec);
+        FrontStages fs;                         // (residue entry: every packet of the batch, chunk by chunk)
+        fs.pk = (const DevPacket *)(db + off_pro);
+        fs.n = n_pro;
+        fs.C = maxc;
+        fs.smem_old = prologue_smem(maxc, kLongBs);
+        fs.n2max = n1max_all >> 1;
+        fs.c_lo = c_lo;
+        fs.r_lo = r_lo;
+        fs.r_hi = r_hi;
+        fs.dense = need_dense;
+        if (fs.n) fs.fast = front_stages_fast(ctx, io, fs, h_pro);
         for (size_t k = 0; k < n_chunks; k++) {
             Chunk &ck = chunks[k];
             if (ck.kc_hi <= ck.kc_lo) continue;
@@ -648,10 +617,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                 CU(ctx, cudaEventRecord(ctx->ev_in[k], ctx->copy_in));
                 CU(ctx, cudaStreamWaitEvent(sm, ctx->ev_in[k], 0));
             }
-            if (residue && ck.np_)
-                if ((rc = launch_prologue(ctx, (const DevPacket *)(db + off_pro) + ck.p0, ck.np_, maxc, pro_fast, prologue_smem(maxc, kLongBs), n1max_all >> 1,
-                                          d_coeffs, need_dense ? d_dense : nullptr, d_kinds, d_ys, const_cast<float *>(d_spec), vqv)))
-                    return rc;
+            if (ck.np_ && (rc = front_stages_launch(ctx, io, fs, ck.p0, ck.np_, d_kinds, d_ys, vqv))) return rc;
             if ((rc = mixed_launch_rounds(ctx, ml, ck.rounds))) return rc;
             if (host && ck.ko_hi > ck.ko_lo) {
                 CU(ctx, cudaEventRecord(ctx->ev_done[k], sm));
@@ -661,21 +627,11 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
             }
         }
         if (capture) {
-            plan->mixed_captured = true;
+            plan->captured = true;
             plan->gen = gen_at_entry;
+            plan->front = fs;
             plan->mix_launch = ml;
             plan->mix_rounds = std::move(chunks[0].rounds);
-            plan->mix_pro = residue && n_pro;
-            if (plan->mix_pro) {            // replayed by lwb_plan_execute in front of the rounds
-                plan->mix_pro_pk = (const DevPacket *)(db + off_pro);
-                plan->mix_pro_n = n_pro;
-                plan->mix_pro_fast = pro_fast;
-                plan->mix_pro_C = maxc;
-                plan->mix_pro_smem_old = prologue_smem(maxc, kLongBs);
-                plan->mix_pro_c_lo = c_lo; plan->mix_pro_r_lo = r_lo; plan->mix_pro_r_hi = r_hi;
-                plan->mix_pro_dense = need_dense;
-                plan->mix_pro_n2max = n1max_all >> 1;
-            }
         }
         if (host) {
             CU(ctx, cudaStreamSynchronize(ctx->copy_out));
