@@ -240,7 +240,14 @@ typedef struct lwb_vq_run {
 enum { LWB_MEM_HOST = 0, LWB_MEM_DEVICE = 1 };
 
 /* One stream's run of consecutive packets.  Input arenas are chain-major: the chain's packets
- * follow each other, each packet as [channels][n/2 of that packet]. */
+ * follow each other, each packet as [channels][n/2 of that packet].
+ * Output: a chain writes exactly n_samples elements per channel plane at out_offset + c * out_stride
+ * (planar), or n_samples * channels elements at out_offset (interleaved), and nothing else in `pcm`,
+ * in either memory space: the gaps between planes and between chains keep what the caller put there.
+ * Any element offsets and any pointer alignment are accepted.  The fused kernels take device-memory
+ * batches whose coeffs / dense_floor / pcm are 16-byte aligned and whose coeff_offset, out_offset and
+ * out_stride are multiples of 4 (host-memory batches: the offsets only); anything else runs on the
+ * chain kernel, which gives the same results more slowly. */
 typedef struct lwb_chain {
     lwb_stream *stream;
     uint32_t n_packets;

@@ -43,6 +43,8 @@ struct lwb_ctx {
     uint64_t state_gen = 1;        // bumped whenever any stream's (has, len) changes: plans key on it
     std::string err;
     uint64_t launches = 0;
+    std::vector<PcmSpan> pcm_spans;        // scratch of copy_pcm_to_host
+    std::vector<PcmCopy> pcm_copies;
     std::deque<CachedTables> tables;       // (deque: setups hold copies of dt, growth never moves an entry)
     // grow-only device arenas
     DevBuf coeffs, dense, pcm, spec, segtab, vqoff, vqrec, magic, x, desc, kinds, ys, chains, ticket, cdesc, cbytes;
@@ -205,6 +207,42 @@ static size_t host_chunks(size_t in_bytes, size_t n_chains)
 {
     if (const char *e = getenv("LWB_E2E_CHUNKS")) return std::max<size_t>(1, std::min<size_t>((size_t)atol(e), std::min<size_t>(64, n_chains)));
     return std::min<size_t>(std::max<size_t>(1, in_bytes >> 25), std::min<size_t>(8, n_chains));
+}
+
+static size_t elem_size(int fmt) { return (fmt == LWB_OUT_F32_PLANAR || fmt == LWB_OUT_F32_INTERLEAVED) ? 4 : 2; }
+static bool is_planar(int fmt) { return fmt == LWB_OUT_F32_PLANAR || fmt == LWB_OUT_I16_PLANAR; }
+
+// D2H of the PCM that chains [i0, i1) produced, from the staging buffer `stage`, which holds arena element `obase` at
+// its start.  Only the write set is copied (pcm_copy_plan.h): the gaps between planes and between chains are the
+// caller's memory, and the kernels never wrote them in the staging buffer.
+static int copy_pcm_to_host(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chain *chains, size_t i0, size_t i1,
+                            const void *stage, uint64_t obase, cudaStream_t st)
+{
+    const size_t esz = elem_size(io->out_format);
+    const bool planar = is_planar(io->out_format);
+    ctx->pcm_spans.clear();
+    for (size_t i = i0; i < i1; i++) {
+        const lwb_chain *c = &chains[i];
+        pcm_chain_spans(planar, c->stream->setup->channels, c->out_offset, c->out_stride, c->n_samples, ctx->pcm_spans);
+    }
+    plan_pcm_copies(ctx->pcm_spans, (uint64_t)INT32_MAX / esz, ctx->pcm_copies);
+    for (const PcmCopy &cp : ctx->pcm_copies) {
+        char *dst = (char *)io->pcm + cp.off * esz;
+        const char *src = (const char *)stage + (cp.off - obase) * esz;
+        if (cp.height == 1) CU(ctx, cudaMemcpyAsync(dst, src, cp.width * esz, cudaMemcpyDeviceToHost, st));
+        else CU(ctx, cudaMemcpy2DAsync(dst, cp.pitch * esz, src, cp.pitch * esz, cp.width * esz, cp.height, cudaMemcpyDeviceToHost, st));
+    }
+    return LWB_OK;
+}
+
+// The fused kernels load coefficients with TMA bulk copies and store PCM with vector stores, which need 16-byte aligned
+// addresses.  Element offsets that are multiples of 4 keep that when the arenas are 16-byte aligned: the library's
+// staging of host-memory batches always is, a caller's device arena may not be (the chain kernel takes those).
+static bool device_arenas_aligned(const lwb_batch_io *io)
+{
+    if (io->memory != LWB_MEM_DEVICE) return true;
+    return ((reinterpret_cast<uintptr_t>(io->coeffs) | reinterpret_cast<uintptr_t>(io->pcm) |
+             reinterpret_cast<uintptr_t>(io->dense_floor)) & 15) == 0;
 }
 
 static int ensure_pinned(lwb_ctx *ctx, size_t bytes)

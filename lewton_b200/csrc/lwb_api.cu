@@ -26,6 +26,7 @@
 #include "kernel_chain.cuh"
 #include "kernel_prologue.cuh"
 #include "lwb_common.h"
+#include "pcm_copy_plan.h"
 
 namespace lwb {
 int generate_tables(int bs, float *a, float *b, float *c, float *window, uint32_t *bitrev);
@@ -601,7 +602,7 @@ static int decode_chains_impl(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, 
         DevArenas ar = DevArenas();
         const size_t esz = elem_size(io->out_format);
         if (io->memory == LWB_MEM_HOST) {
-            // stage: H2D of the used coefficient range, D2H of the used pcm range
+            // stage: H2D of the used coefficient range, D2H of the samples the chains produced
             if (o_hi > o_lo && (rc = ensure(ctx, ctx->pcm, (o_hi - o_lo) * esz))) return rc;
             if (!vq) {
                 if ((rc = ensure(ctx, ctx->coeffs, (c_hi - c_lo) * sizeof(float)))) return rc;
@@ -631,9 +632,7 @@ static int decode_chains_impl(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, 
         rc = run_generic(ctx, plan, io, ar);
         if (rc) return rc;
         if (io->memory == LWB_MEM_HOST) {
-            if (o_hi > o_lo)
-                CU(ctx, cudaMemcpyAsync((char *)io->pcm + o_lo * esz, ctx->pcm.p, (o_hi - o_lo) * esz,
-                                        cudaMemcpyDeviceToHost, ctx->stream));
+            if (o_hi > o_lo && (rc = copy_pcm_to_host(ctx, io, chains, 0, n_chains, ctx->pcm.p, o_lo, ctx->stream))) return rc;
             CU(ctx, cudaStreamSynchronize(ctx->stream));
         }
     }

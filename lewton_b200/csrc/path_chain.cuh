@@ -260,8 +260,7 @@ static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
             plan->mix_rounds = std::move(rounds);
         }
         if (host) {
-            if (o_hi > o_lo)
-                CU(ctx, cudaMemcpyAsync((char *)io->pcm + o_lo * esz, ctx->pcm.p, (size_t)(o_hi - o_lo) * esz, cudaMemcpyDeviceToHost, sm));
+            if (o_hi > o_lo && (rc = copy_pcm_to_host(ctx, io, chains, 0, n_chains, ctx->pcm.p, o_lo, sm))) return rc;
             CU(ctx, cudaStreamSynchronize(sm));
         }
     }

@@ -20,9 +20,6 @@ struct PlanChain {
     bool clear_after;       // OLA guard fired on packet pk.size(): state becomes empty
 };
 
-static size_t elem_size(int fmt) { return (fmt == LWB_OUT_F32_PLANAR || fmt == LWB_OUT_F32_INTERLEAVED) ? 4 : 2; }
-static bool is_planar(int fmt) { return fmt == LWB_OUT_F32_PLANAR || fmt == LWB_OUT_I16_PLANAR; }
-
 static int plan_chain(lwb_chain *c, PlanChain *pc)
 {
     const lwb_stream *s = c->stream;

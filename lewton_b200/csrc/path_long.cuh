@@ -85,7 +85,7 @@ static bool batch_is_uniform_long(lwb_ctx *ctx, const lwb_chain *chains, size_t 
         if (su->bs1 != kLongBs || !su->host.tab[1].pack) return false;
         if (pack && pack != su->host.tab[1].pack) return false;
         pack = su->host.tab[1].pack;
-        if ((c->out_offset & 3) || (c->out_stride & 3) || (c->coeff_offset & 3)) return false;
+        if ((c->out_offset & 3) || (c->out_stride & 3) || (c->coeff_offset & 3) || !device_arenas_aligned(io)) return false;
         if (s->has && s->plen != (uint32_t)kLongN2) return false;
         for (uint32_t k = 0; k < c->n_packets; k++) {
             const uint8_t m = c->mode_numbers[k];
@@ -211,7 +211,7 @@ static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_
     LongRun *const d_runs_base = (LongRun *)rb.p;
     LongRun *h_runs = (LongRun *)st->h, *w = h_runs;
     std::vector<LongRun> tmp;
-    struct ChunkPlan { size_t r0, nr; uint64_t kc_lo, kc_hi, ko_lo, ko_hi; };
+    struct ChunkPlan { size_t r0, nr, i0, i1; uint64_t kc_lo, kc_hi, ko_lo, ko_hi; };       // runs, chains (= items), ranges
     std::vector<ChunkPlan> cplan;
     std::vector<uint32_t> order;
     for (size_t k = 0; k < n_chunks; k++) {
@@ -266,7 +266,7 @@ static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_
                 i = j;
             }
         }
-        cplan.push_back(ChunkPlan{(size_t)(w0 - h_runs), (size_t)(w - w0), kc_lo, kc_hi, ko_lo, ko_hi});
+        cplan.push_back(ChunkPlan{(size_t)(w0 - h_runs), (size_t)(w - w0), i0, i1, kc_lo, kc_hi, ko_lo, ko_hi});
     }
     // one descriptor upload for the whole call, on the copy stream, behind the kernel that last read
     // this half of the double buffer
@@ -294,8 +294,7 @@ static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_
             const size_t evk = slice.active ? (size_t)slice.ev_slot : k;
             CU(ctx, cudaEventRecord(ctx->ev_done[evk], ctx->stream));
             CU(ctx, cudaStreamWaitEvent(ctx->copy_out, ctx->ev_done[evk], 0));
-            CU(ctx, cudaMemcpyAsync((char *)io->pcm + cp.ko_lo * esz, (char *)ctx->pcm.p + (cp.ko_lo - obase) * esz,
-                                    (size_t)(cp.ko_hi - cp.ko_lo) * esz, cudaMemcpyDeviceToHost, ctx->copy_out));
+            if ((rc = copy_pcm_to_host(ctx, io, chains, cp.i0, cp.i1, ctx->pcm.p, obase, ctx->copy_out))) return rc;
         }
     }
     CU(ctx, cudaEventRecord(ctx->ev_kdone[par], ctx->stream));

@@ -17,6 +17,7 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
     const bool vq = io->entry == LWB_ENTRY_VQ, residue = io->entry != LWB_ENTRY_SPECTRUM;
     if (residue && !io->floor_kind) return LWB_OK;            // (the chain kernel words the error)
     if (vq) return LWB_OK;                                    // (VQ records of such streams: the general path, as before)
+    if (!device_arenas_aligned(io)) return LWB_OK;
     int uniform_c = -1;
     const bool i16 = io->out_format == LWB_OUT_I16_PLANAR;
     const size_t esz = i16 ? 2 : 4;
@@ -207,8 +208,7 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
         plan->mix_rounds = std::move(rounds);
     }
     if (host) {
-        if (o_hi > o_lo)
-            CU(ctx, cudaMemcpyAsync((char *)io->pcm + o_lo * esz, ctx->pcm.p, (size_t)(o_hi - o_lo) * esz, cudaMemcpyDeviceToHost, sm));
+        if (o_hi > o_lo && (rc = copy_pcm_to_host(ctx, io, chains, 0, n_chains, ctx->pcm.p, o_lo, sm))) return rc;
         CU(ctx, cudaStreamSynchronize(sm));
     }
     for (size_t i = 0; i < n_chains; i++)

@@ -44,6 +44,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
     const uint64_t gen_at_entry = ctx->state_gen;
     if (getenv("LWB_NO_MIXED")) return LWB_OK;
     if (io->out_format != LWB_OUT_F32_PLANAR && io->out_format != LWB_OUT_I16_PLANAR) return LWB_OK;
+    if (!device_arenas_aligned(io)) return LWB_OK;
     const bool vq = io->entry == LWB_ENTRY_VQ;
     const bool residue = io->entry != LWB_ENTRY_SPECTRUM;
     const bool i16 = io->out_format == LWB_OUT_I16_PLANAR;
@@ -622,8 +623,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
             if (host && ck.ko_hi > ck.ko_lo) {
                 CU(ctx, cudaEventRecord(ctx->ev_done[k], sm));
                 CU(ctx, cudaStreamWaitEvent(ctx->copy_out, ctx->ev_done[k], 0));
-                CU(ctx, cudaMemcpyAsync((char *)io->pcm + ck.ko_lo * esz, (char *)ctx->pcm.p + (ck.ko_lo - o_lo) * esz,
-                                        (size_t)(ck.ko_hi - ck.ko_lo) * esz, cudaMemcpyDeviceToHost, ctx->copy_out));
+                if ((rc = copy_pcm_to_host(ctx, io, chains, ck.i0, ck.i1, ctx->pcm.p, o_lo, ctx->copy_out))) return rc;
             }
         }
         if (capture) {

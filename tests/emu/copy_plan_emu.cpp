@@ -1,0 +1,26 @@
+// copy_plan_emu.cpp -- TEST INFRASTRUCTURE: the PCM copy-back planner of the host-memory batch paths
+// (lewton_b200/csrc/pcm_copy_plan.h), run on the host so that its copies can be checked against the write set.
+#include <cstddef>
+#include <cstdint>
+
+#include "../../lewton_b200/csrc/pcm_copy_plan.h"
+
+// copies: [cap][4] = (off, width, pitch, height) in elements.  Returns the number of copies, or -1 if cap is too small.
+extern "C" long lwb_emu_copy_plan(int planar, size_t n_chains, const uint32_t *channels, const uint64_t *out_offset,
+                                  const uint64_t *out_stride, const uint32_t *n_samples, uint64_t max_pitch, uint64_t *copies,
+                                  size_t cap)
+{
+    std::vector<lwb::PcmSpan> spans;
+    std::vector<lwb::PcmCopy> plan;
+    for (size_t i = 0; i < n_chains; i++)
+        lwb::pcm_chain_spans(planar != 0, channels[i], out_offset[i], out_stride[i], n_samples[i], spans);
+    lwb::plan_pcm_copies(spans, max_pitch, plan);
+    if (plan.size() > cap) return -1;
+    for (size_t k = 0; k < plan.size(); k++) {
+        copies[4 * k] = plan[k].off;
+        copies[4 * k + 1] = plan[k].width;
+        copies[4 * k + 2] = plan[k].pitch;
+        copies[4 * k + 3] = plan[k].height;
+    }
+    return (long)plan.size();
+}

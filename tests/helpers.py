@@ -2,6 +2,7 @@
 import numpy as np
 
 import lewton_b200 as L
+from lewton_b200 import _cabi as cabi
 
 
 def bits_equal(a, b):
@@ -22,6 +23,54 @@ def mismatch_report(a, b):
     b = np.ascontiguousarray(b, np.float32).ravel()
     bad = np.nonzero(~((a.view(np.uint32) == b.view(np.uint32)) | ((a == 0) & (b == 0)) | (np.isnan(a) & np.isnan(b))))[0]
     return f"{bad.size} of {a.size} differ; first at {bad[:5]}: got {a[bad[:5]]} want {b[bad[:5]]}"
+
+
+F32_GUARD = 0x7fa5a5a5        # a NaN with a fixed payload: no kernel produces it, compared bit for bit
+I16_GUARD = 0x5a5a
+
+
+def write_set(chains, channels_of, fmt):
+    """The element intervals each chain produced, as the ABI states them (include/lewton_b200.h, lwb_chain):
+    planar: [out_offset + c * out_stride, + n_samples) per channel c; interleaved: [out_offset, + n_samples * C).
+    chains: ChainSpec objects after the call; channels_of(i) -> channel count of chain i.
+    Returns [(chain index, [(start, length), ...])]."""
+    planar = fmt in (cabi.OUT_F32_PLANAR, cabi.OUT_I16_PLANAR)
+    out = []
+    for i, c in enumerate(chains):
+        C, n = channels_of(i), int(c.n_samples)
+        if planar:
+            spans = [(int(c.out_offset) + k * int(c.out_stride), n) for k in range(C)]
+        else:
+            spans = [(int(c.out_offset), n * C)]
+        out.append((i, [s for s in spans if s[1]]))
+    return out
+
+
+def _bits(buf):
+    return buf.view(np.uint32 if buf.dtype == np.float32 else np.uint16)
+
+
+def fill_guard(buf):
+    """Fills an f32 / i16 output arena with the sentinel before a call; returns it."""
+    _bits(buf)[...] = F32_GUARD if buf.dtype == np.float32 else I16_GUARD
+    return buf
+
+
+def assert_contained(buf, ws, what=""):
+    """Every element of `buf` outside the write set `ws` (see write_set) still holds the sentinel."""
+    flat = _bits(buf.reshape(-1))
+    outside = np.ones(flat.size, bool)
+    for _, spans in ws:
+        for s, n in spans:
+            assert s + n <= flat.size, f"{what}: a chain's write set ends past the arena ({s} + {n} > {flat.size})"
+            outside[s:s + n] = False
+    guard = F32_GUARD if buf.dtype == np.float32 else I16_GUARD
+    bad = np.nonzero(outside & (flat != guard))[0]
+    if bad.size:
+        i = int(bad[0])
+        near = [k for k, spans in ws if spans and min(s for s, _ in spans) <= i < max(s + n for s, n in spans)]
+        raise AssertionError(f"{what}: {bad.size} elements outside the write set were written; first at {i} "
+                             f"(value bits {int(flat[i]):#x}), inside the extent of chains {near[:4]}")
 
 
 def random_floor1(rng, n2):
