@@ -70,6 +70,15 @@ const char *lwb_last_error(const lwb_ctx *ctx);
 void *lwb_ctx_cuda_stream(lwb_ctx *ctx);
 /* kernels launched by this ctx since creation (bench.py's gpu_launches) */
 uint64_t lwb_ctx_launch_count(const lwb_ctx *ctx);
+/* The kernels a batch can launch, one id per __global__ function (k_mid's n = 1024 and n = 512 instances share
+ * one).  Which of them ran tells which batch path took a batch: every path gives the same bytes. */
+enum { LWB_KERNEL_LONG = 0, LWB_KERNEL_LONG_S = 1, LWB_KERNEL_MID = 2, LWB_KERNEL_SHORT = 3, LWB_KERNEL_SHORT_G = 4,
+       LWB_KERNEL_ROW_COPY = 5, LWB_KERNEL_CHAIN = 6, LWB_KERNEL_FLOOR1_SEGMENTS = 7, LWB_KERNEL_PROLOGUE_FUSED = 8,
+       LWB_KERNEL_PROLOGUE = 9, LWB_KERNEL_IMDCT = 10, LWB_KERNEL_OVERLAP = 11, LWB_KERNEL_SAVE_STATE = 12,
+       LWB_KERNEL_COUNT = 13 };
+/* debug: launches of kernel `kernel_id` (LWB_KERNEL_*) by this ctx since creation (0 for an unknown id); the
+ * counts of all ids sum to lwb_ctx_launch_count */
+uint64_t lwb_ctx_kernel_launches(const lwb_ctx *ctx, int kernel_id);
 /* pinned host memory for the host-buffer entry points (optional; plain malloc'd memory works, slower) */
 void *lwb_host_alloc(size_t bytes);
 void lwb_host_free(void *p);

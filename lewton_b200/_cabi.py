@@ -17,6 +17,9 @@ FLOOR_UNUSED, FLOOR_ONE, FLOOR_DENSE = 0, 1, 2
 OUT_F32_PLANAR, OUT_I16_PLANAR, OUT_F32_INTERLEAVED, OUT_I16_INTERLEAVED = 0, 1, 2, 3
 ENTRY_SPECTRUM, ENTRY_RESIDUE, ENTRY_VQ = 0, 1, 2
 MEM_HOST, MEM_DEVICE = 0, 1
+# LWB_KERNEL_* ids in order: KERNELS[id] is the kernel's name
+KERNELS = ("k_long", "k_long_s", "k_mid", "k_short", "k_short_g", "k_row_copy", "k_chain", "k_floor1_segments",
+           "k_prologue_fused", "k_prologue", "k_imdct", "k_overlap", "k_save_state")
 
 vp, u8p, fp, u32p = C.c_void_p, C.POINTER(C.c_uint8), C.POINTER(C.c_float), C.POINTER(C.c_uint32)
 
@@ -93,6 +96,7 @@ SYMBOLS = {
     "lwb_last_error": (C.c_char_p, [vp]),
     "lwb_ctx_cuda_stream": (vp, [vp]),
     "lwb_ctx_launch_count": (C.c_uint64, [vp]),
+    "lwb_ctx_kernel_launches": (C.c_uint64, [vp, C.c_int]),
     "lwb_host_alloc": (vp, [C.c_size_t]),
     "lwb_bind_host_to_device": (C.c_int, [C.c_int]),
     "lwb_host_free": (None, [vp]),

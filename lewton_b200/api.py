@@ -64,6 +64,10 @@ class Context:
     def launch_count(self):
         return cabi.lib().lwb_ctx_launch_count(self._h)
 
+    def kernel_launches(self):
+        """{kernel name: launches since creation} (lwb_ctx_kernel_launches); the counts sum to launch_count."""
+        return {name: cabi.lib().lwb_ctx_kernel_launches(self._h, k) for k, name in enumerate(cabi.KERNELS)}
+
     def device_alloc(self, nbytes):
         p = C.c_void_p()
         self.check(cabi.lib().lwb_device_alloc(self._h, nbytes, C.byref(p)))

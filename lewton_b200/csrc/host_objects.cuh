@@ -43,6 +43,7 @@ struct lwb_ctx {
     uint64_t state_gen = 1;        // bumped whenever any stream's (has, len) changes: plans key on it
     std::string err;
     uint64_t launches = 0;
+    uint64_t kernel_launches[LWB_KERNEL_COUNT] = {};   // per LWB_KERNEL_* id; they sum to `launches`
     std::vector<PcmSpan> pcm_spans;        // scratch of copy_pcm_to_host
     std::vector<PcmCopy> pcm_copies;
     std::deque<CachedTables> tables;       // (deque: setups hold copies of dt, growth never moves an entry)
@@ -139,6 +140,14 @@ static int fail(lwb_ctx *ctx, int code, const char *what, cudaError_t e = cudaSu
         }
     }
     return code;
+}
+
+// One kernel launch enqueued: the total and the count of its kernel.  Only launch() and launched() (path_generic.cuh)
+// call this; tests/test_cabi_cpu.py checks that every launch site goes through one of them.
+static inline void count_launch(lwb_ctx *ctx, int kernel_id)
+{
+    ctx->launches++;
+    ctx->kernel_launches[kernel_id]++;
 }
 
 #define CU(ctx, call)                                                        \

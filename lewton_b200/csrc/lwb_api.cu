@@ -127,6 +127,10 @@ extern "C" int lwb_ctx_synchronize(lwb_ctx *ctx)
 extern "C" const char *lwb_last_error(const lwb_ctx *ctx) { return ctx ? ctx->err.c_str() : "no context"; }
 extern "C" void *lwb_ctx_cuda_stream(lwb_ctx *ctx) { return ctx ? (void *)ctx->stream : nullptr; }
 extern "C" uint64_t lwb_ctx_launch_count(const lwb_ctx *ctx) { return ctx ? ctx->launches : 0; }
+extern "C" uint64_t lwb_ctx_kernel_launches(const lwb_ctx *ctx, int kernel_id)
+{
+    return ctx && kernel_id >= 0 && kernel_id < LWB_KERNEL_COUNT ? ctx->kernel_launches[kernel_id] : 0;
+}
 
 extern "C" void *lwb_host_alloc(size_t bytes)
 {
@@ -805,7 +809,7 @@ extern "C" int lwb_debug_packet_taps(lwb_stream *s, const lwb_packet *pkt, float
         CU(ctx, cudaMalloc(&tmp_kinds, C));
         CU(ctx, cudaMemcpyAsync(tmp_dense, ones.data(), C * n2 * 4, cudaMemcpyHostToDevice, st));
         CU(ctx, cudaMemcpyAsync(tmp_kinds, kd.data(), C, cudaMemcpyHostToDevice, st));
-        rc = launch(ctx, k_prologue, dim3(1), dim3(kPrologueThreads), prologue_smem(su->channels, su->bs1), dp, (const float *)ctx->coeffs.p,
+        rc = launch(ctx, LWB_KERNEL_PROLOGUE, k_prologue, dim3(1), dim3(kPrologueThreads), prologue_smem(su->channels, su->bs1), dp, (const float *)ctx->coeffs.p,
                     (const float *)tmp_dense, (const uint8_t *)tmp_kinds, (const uint32_t *)ctx->ys.p,
                     (float *)ctx->spec.p);
         if (!rc) {
@@ -817,13 +821,13 @@ extern "C" int lwb_debug_packet_taps(lwb_stream *s, const lwb_packet *pkt, float
         cudaFree(tmp_kinds);
         if (rc) return rc;
     }
-    if ((rc = launch(ctx, k_prologue, dim3(1), dim3(kPrologueThreads), prologue_smem(su->channels, su->bs1), dp, (const float *)ctx->coeffs.p,
+    if ((rc = launch(ctx, LWB_KERNEL_PROLOGUE, k_prologue, dim3(1), dim3(kPrologueThreads), prologue_smem(su->channels, su->bs1), dp, (const float *)ctx->coeffs.p,
                      (const float *)ctx->dense.p, (const uint8_t *)ctx->kinds.p, (const uint32_t *)ctx->ys.p,
                      (float *)ctx->spec.p)))
         return rc;
     if (pre_mdct) CU(ctx, cudaMemcpyAsync(pre_mdct, ctx->spec.p, C * n2 * 4, cudaMemcpyDeviceToHost, st));
     if (post_mdct) {
-        if ((rc = launch(ctx, k_imdct, dim3(1, (unsigned)C), dim3(kImdctThreads), g.n * sizeof(float), dp,
+        if ((rc = launch(ctx, LWB_KERNEL_IMDCT, k_imdct, dim3(1, (unsigned)C), dim3(kImdctThreads), g.n * sizeof(float), dp,
                          (const float *)ctx->spec.p, (float *)ctx->x.p)))
             return rc;
         CU(ctx, cudaMemcpyAsync(post_mdct, ctx->x.p, C * g.n * 4, cudaMemcpyDeviceToHost, st));

@@ -29,11 +29,11 @@ static int launch_chain(lwb_ctx *ctx, int fmt, unsigned n_chains, unsigned warps
     case F:                                                                                                  \
         if (wpc == 1) {                                                                                      \
             cudaFuncSetAttribute(k_chain<F, ENTRY, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            return launch(ctx, k_chain<F, ENTRY, false>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, \
+            return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, false>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, \
                           kinds, ys, pcm, n1max, wpc, np);                                                    \
         }                                                                                                    \
         cudaFuncSetAttribute(k_chain<F, ENTRY, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-        return launch(ctx, k_chain<F, ENTRY, true>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, kinds, \
+        return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, true>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, kinds, \
                       ys, pcm, n1max, wpc, 1);
     switch (fmt) {
         LWB_CHAIN_CASE(LWB_OUT_F32_PLANAR)
@@ -61,36 +61,36 @@ static int mixed_launch_rounds(lwb_ctx *ctx, const MixLaunch &ml, const std::vec
     cudaStream_t sm = ctx->stream;
     int rc = LWB_OK;
     for (const MixRound &rd : rounds) {
-        if (rd.nm) {             // uniform 1024-point batches (path_mid.cuh)
-            if (mid_launch(sm, (const LongRun *)ml.db, (uint32_t)rd.nm, ml.mpack, ctx->sm_count, ml.i16, ml.mid_kb))
-                return fail(ctx, LWB_ERR_CUDA, "mid kernel launch", cudaGetLastError());
-            ctx->launches++;
-        }
-        if (rd.nx) {
-            k_row_copy<<<(unsigned)rd.nx, 64, 0, sm>>>((const RowCopy *)(ml.db + ml.off_rc) + rd.x0);
-            if (cudaGetLastError() != cudaSuccess) return fail(ctx, LWB_ERR_CUDA, "row copy launch", cudaGetLastError());
-            ctx->launches++;
-        }
+        if (rd.nm &&             // uniform 1024-point batches (path_mid.cuh)
+            (rc = launched(ctx, LWB_KERNEL_MID, mid_launch(sm, (const LongRun *)ml.db, (uint32_t)rd.nm, ml.mpack, ctx->sm_count, ml.i16, ml.mid_kb),
+                           "mid kernel launch")))
+            return rc;
+        if (rd.nx && (rc = launch(ctx, LWB_KERNEL_ROW_COPY, k_row_copy, dim3((unsigned)rd.nx), dim3(64), 0, (const RowCopy *)(ml.db + ml.off_rc) + rd.x0)))
+            return rc;
         if (rd.nr) {
             unsigned int *ticket;
             if ((rc = next_ticket(ctx, &ticket))) return rc;
             if (kLongNB != 1) return fail(ctx, LWB_ERR_INVALID, "mixed path needs one run per warp");
             // one pass over many short runs: the static deal with its deeper lookahead (k_long_s); rounds: tickets
-            if (rd.flat ? long_launch_static(sm, (const LongRun *)ml.db + rd.r0, (uint32_t)rd.nr, ml.pack, ctx->sm_count, ml.i16, ml.w_short, ml.ls)
-                        : long_launch(sm, (const LongRun *)ml.db + rd.r0, (uint32_t)rd.nr, ml.pack, ticket, ctx->sm_count, ml.i16, ml.w_short, ml.ls))
-                return fail(ctx, LWB_ERR_CUDA, "long kernel launch", cudaGetLastError());
-            ctx->launches++;
+            if (rd.flat)
+                rc = launched(ctx, LWB_KERNEL_LONG_S,
+                              long_launch_static(sm, (const LongRun *)ml.db + rd.r0, (uint32_t)rd.nr, ml.pack, ctx->sm_count, ml.i16, ml.w_short, ml.ls),
+                              "long kernel launch");
+            else
+                rc = launched(ctx, LWB_KERNEL_LONG,
+                              long_launch(sm, (const LongRun *)ml.db + rd.r0, (uint32_t)rd.nr, ml.pack, ticket, ctx->sm_count, ml.i16, ml.w_short, ml.ls),
+                              "long kernel launch");
+            if (rc) return rc;
         }
-        if (rd.ns) {
-            if (short_launch(sm, (const ShortRun *)(ml.db + ml.off_sr) + rd.s0, (uint32_t)rd.ns, ml.spack, ctx->sm_count, ml.i16))
-                return fail(ctx, LWB_ERR_CUDA, "short kernel launch", cudaGetLastError());
-            ctx->launches++;
-        }
-        if (rd.ng) {             // bursts: eight short runs of equal length per warp (k_short_g)
-            if (short_launch_groups(sm, (const ShortRun *)(ml.db + ml.off_sg) + rd.g0 * kShortOct, (uint32_t)rd.ng, ml.spack, ctx->sm_count, ml.i16))
-                return fail(ctx, LWB_ERR_CUDA, "short burst kernel launch", cudaGetLastError());
-            ctx->launches++;
-        }
+        if (rd.ns &&
+            (rc = launched(ctx, LWB_KERNEL_SHORT, short_launch(sm, (const ShortRun *)(ml.db + ml.off_sr) + rd.s0, (uint32_t)rd.ns, ml.spack, ctx->sm_count, ml.i16),
+                           "short kernel launch")))
+            return rc;
+        if (rd.ng &&             // bursts: eight short runs of equal length per warp (k_short_g)
+            (rc = launched(ctx, LWB_KERNEL_SHORT_G,
+                           short_launch_groups(sm, (const ShortRun *)(ml.db + ml.off_sg) + rd.g0 * kShortOct, (uint32_t)rd.ng, ml.spack, ctx->sm_count, ml.i16),
+                           "short burst kernel launch")))
+            return rc;
         if (rd.nc) {
             const ChainDesc *dcd = (const ChainDesc *)(ml.db + ml.off_cd) + rd.c0;
             const uint8_t *dby = (const uint8_t *)(ml.db + ml.off_by);

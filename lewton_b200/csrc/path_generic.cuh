@@ -73,13 +73,23 @@ static size_t prologue_smem_of(const std::vector<PlanChain> &plan)
     return m;
 }
 
+// Every launch of the library goes through launch() or launched(), which count it under its kernel's LWB_KERNEL_* id.
 template <typename K, typename... Args>
-static int launch(lwb_ctx *ctx, K kernel, dim3 grid, dim3 block, size_t smem, Args... args)
+static int launch(lwb_ctx *ctx, int kernel_id, K kernel, dim3 grid, dim3 block, size_t smem, Args... args)
 {
     kernel<<<grid, block, smem, ctx->stream>>>(args...);
-    ctx->launches++;
+    count_launch(ctx, kernel_id);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, LWB_ERR_CUDA, "kernel launch", e);
+    return LWB_OK;
+}
+
+// A launch made by a launch wrapper of the kernel headers (long_launch, mid_launch, short_launch, ...), which returns
+// non-zero when it failed; `what` words the failure.
+static int launched(lwb_ctx *ctx, int kernel_id, int wrapper_rc, const char *what)
+{
+    if (wrapper_rc) return fail(ctx, LWB_ERR_CUDA, what, cudaGetLastError());
+    count_launch(ctx, kernel_id);
     return LWB_OK;
 }
 
@@ -109,7 +119,7 @@ static int launch_prologue(lwb_ctx *ctx, const DevPacket *d_pk, size_t n_pk, uns
     if (vq.runs && (!fast || (size_t)C * n2max > kVqMaxElems))
         return fail(ctx, LWB_ERR_INVALID, "VQ entry needs <= 8 channels, aligned arenas and channels * n/2 <= 12288");
     if (!fast)
-        return launch(ctx, k_prologue, dim3((unsigned)n_pk), dim3(kPrologueThreads), smem_old, d_pk, res, dense, kinds, ys, spec);
+        return launch(ctx, LWB_KERNEL_PROLOGUE, k_prologue, dim3((unsigned)n_pk), dim3(kPrologueThreads), smem_old, d_pk, res, dense, kinds, ys, spec);
     // per (packet, channel) row (ctx scratch): the packed flagged segments of its floor curve, the bin -> segment
     // index (bitmap + prefix counts) and the segment count
     const size_t rows = n_pk * C, tab_bytes = rows * kSegStride * sizeof(uint4), ix_bytes = rows * seg_index_stride(words);
@@ -127,15 +137,15 @@ static int launch_prologue(lwb_ctx *ctx, const DevPacket *d_pk, size_t n_pk, uns
     uint4 *tab = (uint4 *)ctx->segtab.p;
     unsigned char *ix = (unsigned char *)ctx->segtab.p + tab_bytes;
     uint8_t *cnt = ix + ix_bytes;
-    rc = launch(ctx, k_floor1_segments, dim3((unsigned)((rows + kSegRows - 1) / kSegRows)), dim3(kSegThreads), floor1_segments_smem(words), d_pk,
+    rc = launch(ctx, LWB_KERNEL_FLOOR1_SEGMENTS, k_floor1_segments, dim3((unsigned)((rows + kSegRows - 1) / kSegRows)), dim3(kSegThreads), floor1_segments_smem(words), d_pk,
                 (uint32_t)rows, (int)C, kinds, ys, tab, cnt, ix, words, (const uint32_t *)ctx->magic.p);
     if (rc) return rc;
     const size_t grid = std::min<size_t>(n_pk, (size_t)ctx->sm_count * (C > 2 ? 4 : 8));
     const VqDev vd{vq.runs, vq.run_off, vq.entries, vq.ent_off};
     if (vq.runs)
-        return launch(ctx, k_prologue_fused<true>, dim3((unsigned)grid), dim3(kPfThreads), prologue_fused_smem((int)C, words, (size_t)C * n2max), d_pk,
+        return launch(ctx, LWB_KERNEL_PROLOGUE_FUSED, k_prologue_fused<true>, dim3((unsigned)grid), dim3(kPfThreads), prologue_fused_smem((int)C, words, (size_t)C * n2max), d_pk,
                       (uint32_t)n_pk, res, dense, kinds, (const uint4 *)tab, (const uint8_t *)cnt, (const unsigned char *)ix, words, spec, vd);
-    return launch(ctx, k_prologue_fused<false>, dim3((unsigned)grid), dim3(kPfThreads), prologue_fused_smem((int)C, words), d_pk, (uint32_t)n_pk, res, dense,
+    return launch(ctx, LWB_KERNEL_PROLOGUE_FUSED, k_prologue_fused<false>, dim3((unsigned)grid), dim3(kPfThreads), prologue_fused_smem((int)C, words), d_pk, (uint32_t)n_pk, res, dense,
                   kinds, (const uint4 *)tab, (const uint8_t *)cnt, (const unsigned char *)ix, words, spec, vd);
 }
 static int launch_prologue(lwb_ctx *ctx, const DevPacket *d_pk, const DevPacket *h_pk, size_t n_pk, unsigned C, size_t smem_old,
@@ -393,18 +403,18 @@ static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_bat
                 return rc;
             spec = (const float *)ctx->spec.p;
         }
-        if ((rc = launch(ctx, k_imdct, dim3((unsigned)n_desc, maxc), dim3(kImdctThreads), maxn * sizeof(float), dp,
+        if ((rc = launch(ctx, LWB_KERNEL_IMDCT, k_imdct, dim3((unsigned)n_desc, maxc), dim3(kImdctThreads), maxn * sizeof(float), dp,
                          spec, (float *)ctx->x.p)))
             return rc;
         dim3 g2((unsigned)n_desc, maxc), b2(kOverlapThreads);
         switch (io->out_format) {
-        case LWB_OUT_F32_PLANAR: rc = launch(ctx, k_overlap<LWB_OUT_F32_PLANAR>, g2, b2, 0, dp, (const float *)ctx->x.p, ar.pcm); break;
-        case LWB_OUT_I16_PLANAR: rc = launch(ctx, k_overlap<LWB_OUT_I16_PLANAR>, g2, b2, 0, dp, (const float *)ctx->x.p, ar.pcm); break;
-        case LWB_OUT_F32_INTERLEAVED: rc = launch(ctx, k_overlap<LWB_OUT_F32_INTERLEAVED>, g2, b2, 0, dp, (const float *)ctx->x.p, ar.pcm); break;
-        default: rc = launch(ctx, k_overlap<LWB_OUT_I16_INTERLEAVED>, g2, b2, 0, dp, (const float *)ctx->x.p, ar.pcm); break;
+        case LWB_OUT_F32_PLANAR: rc = launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<LWB_OUT_F32_PLANAR>, g2, b2, 0, dp, (const float *)ctx->x.p, ar.pcm); break;
+        case LWB_OUT_I16_PLANAR: rc = launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<LWB_OUT_I16_PLANAR>, g2, b2, 0, dp, (const float *)ctx->x.p, ar.pcm); break;
+        case LWB_OUT_F32_INTERLEAVED: rc = launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<LWB_OUT_F32_INTERLEAVED>, g2, b2, 0, dp, (const float *)ctx->x.p, ar.pcm); break;
+        default: rc = launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<LWB_OUT_I16_INTERLEAVED>, g2, b2, 0, dp, (const float *)ctx->x.p, ar.pcm); break;
         }
         if (rc) return rc;
-        if ((rc = launch(ctx, k_save_state, g2, b2, 0, dp, (const float *)ctx->x.p))) return rc;
+        if ((rc = launch(ctx, LWB_KERNEL_SAVE_STATE, k_save_state, g2, b2, 0, dp, (const float *)ctx->x.p))) return rc;
     }
     return LWB_OK;
 }

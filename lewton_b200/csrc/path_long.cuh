@@ -103,10 +103,7 @@ static int launch_long(lwb_ctx *ctx, const LongRun *runs, uint32_t n_groups, con
     unsigned int *ticket;
     int rc = next_ticket(ctx, &ticket);
     if (rc) return rc;
-    if (long_launch(ctx->stream, runs, n_groups, pack, ticket, ctx->sm_count, i16))
-        return fail(ctx, LWB_ERR_CUDA, "long kernel launch", cudaGetLastError());
-    ctx->launches++;
-    return LWB_OK;
+    return launched(ctx, LWB_KERNEL_LONG, long_launch(ctx->stream, runs, n_groups, pack, ticket, ctx->sm_count, i16), "long kernel launch");
 }
 
 // `spectrum_dev`: when non-null the spectrum has already been formed on the device (residue entry:

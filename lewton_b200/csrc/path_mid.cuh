@@ -48,7 +48,9 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
             if (g.n != n_blk || g.ls != 0 || g.rs != n2_blk || g.re != n_blk) return LWB_OK;
         }
         if (c->n_packets) {
-            if (c->out_stride < (uint64_t)c->n_packets * n2_blk) return LWB_OK;     // (the chain kernel words the error)
+            // the planes hold the samples the chain produces: none for the first packet of an empty stream
+            const uint64_t produced = (uint64_t)(c->n_packets - (c->stream->has ? 0u : 1u)) * n2_blk;
+            if (c->out_stride < produced) return LWB_OK;     // (the chain kernel words the error)
             n_runs += su->channels;
         }
     }

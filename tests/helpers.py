@@ -1,8 +1,53 @@
-"""Shared test helpers: random setups / packets, and the oracle-driven reference decode."""
+"""Shared test helpers: random setups / packets, the oracle-driven reference decode, and which kernels ran."""
+import contextlib
+
 import numpy as np
+import pytest
 
 import lewton_b200 as L
 from lewton_b200 import _cabi as cabi
+
+# kernel names (Context.kernel_launches) by the path they belong to
+ALL_KERNELS = frozenset(cabi.KERNELS)
+GENERIC = frozenset({"k_prologue", "k_imdct", "k_overlap", "k_save_state"})      # the four-kernel path
+FRONT = frozenset({"k_floor1_segments", "k_prologue_fused"})                     # two-kernel front stages
+FUSED = frozenset({"k_long", "k_long_s", "k_mid", "k_short", "k_short_g"})       # the fused synthesis kernels
+
+
+@contextlib.contextmanager
+def expect_kernels(ctx, ran=(), not_ran=()):
+    """Checks which kernels the block launched on ctx.  ran: names that must have run (a dict: exact launch counts);
+    not_ran: names that must not.  Yields a dict that holds {name: launches} of the block once it has finished."""
+    unknown = (set(ran) | set(not_ran)) - ALL_KERNELS
+    assert not unknown, f"no such kernels: {sorted(unknown)}"
+    k0 = ctx.kernel_launches()
+    delta = {}
+    yield delta
+    k1 = ctx.kernel_launches()
+    delta.update({k: k1[k] - k0[k] for k in k1})
+    launched = {k: v for k, v in delta.items() if v}
+    if isinstance(ran, dict):
+        wrong = {k: delta[k] for k, v in ran.items() if delta[k] != v}
+        assert not wrong, f"expected launches {ran}, got {launched}"
+    else:
+        missing = sorted(k for k in ran if not delta[k])
+        assert not missing, f"expected {missing} to run; launched {launched}"
+    extra = sorted(k for k in not_ran if delta[k])
+    assert not extra, f"expected {extra} not to run; launched {launched}"
+
+
+@pytest.fixture(autouse=True)
+def launches_are_attributed(request):
+    """GPU tests (modules import this fixture): across every test, the per-kernel launch counts of the module's ctx
+    grow by exactly as much as its total launch count, so a launch site that does not attribute itself fails."""
+    if request.node.get_closest_marker("gpu") is None or "ctx" not in request.fixturenames:
+        yield
+        return
+    ctx = request.getfixturevalue("ctx")
+    t0, k0 = ctx.launch_count, sum(ctx.kernel_launches().values())
+    yield
+    t1, k1 = ctx.launch_count, sum(ctx.kernel_launches().values())
+    assert k1 - k0 == t1 - t0, f"{t1 - t0} launches, {k1 - k0} of them attributed to a kernel"
 
 
 def bits_equal(a, b):

@@ -12,8 +12,10 @@ import pytest
 
 import lewton_b200 as L
 from lewton_b200 import _cabi as cabi
-from helpers import (RefStream, assert_contained, bits_equal, fill_guard, make_setup, mismatch_report, random_floor1_y,
-                     write_set)
+from helpers import (ALL_KERNELS, FRONT, FUSED, GENERIC, RefStream, assert_contained, bits_equal, expect_kernels, fill_guard,
+                     launches_are_attributed, make_setup, mismatch_report, random_floor1_y, write_set)
+
+launches_are_attributed  # (autouse)
 
 pytestmark = pytest.mark.gpu
 
@@ -263,19 +265,23 @@ class Batch:
 # ------------------------------------------------------------------------------------------------
 # every path, every layout
 # ------------------------------------------------------------------------------------------------
-SHAPES = {   # name: channels, blocksize_0, blocksize_1, share of short blocks, residue entry, environment
-    "long": (2, 8, 11, 0.0, False, None),                               # k_long
-    "mid1024": (2, 10, 10, 0.0, False, None),                           # k_mid, n = 1024
-    "mid512": (1, 9, 9, 0.0, False, None),                              # k_mid, n = 512
-    "short": (2, 8, 8, 0.0, False, None),                               # k_short
-    "mixed": (2, 8, 11, 0.5, False, None),                              # one pass of k_long + k_short
-    "mixed_rounds": (2, 8, 11, 0.5, False, {"LWB_MIXED_ROUNDS": "1"}),  # rounds of k_long / k_short / k_chain
-    "chain": (6, 8, 11, 0.3, False, {"LWB_NO_MIXED": "1"}),             # the chain kernel
-    "generic": (2, 8, 11, 0.3, False, {"LWB_FORCE_GENERIC": "1"}),      # the four-kernel path
-    "residue_long": (2, 8, 11, 0.0, True, None),                        # front stages + k_long
-    "residue_mid": (2, 10, 10, 0.0, True, None),                        # front stages + k_mid
-    "residue_mixed": (2, 8, 11, 0.3, True, None),                       # front stages + segmented kernels
+SHAPES = {   # name: channels, blocksize_0, blocksize_1, share of short blocks, residue entry, environment, the kernels the
+             # shape exists to reach (planar output, 16-byte aligned offsets)
+    "long": (2, 8, 11, 0.0, False, None, {"k_long"}),
+    "mid1024": (2, 10, 10, 0.0, False, None, {"k_mid"}),                               # n = 1024
+    "mid512": (1, 9, 9, 0.0, False, None, {"k_mid"}),                                  # n = 512
+    "short": (2, 8, 8, 0.0, False, None, {"k_short"}),
+    "mixed": (2, 8, 11, 0.5, False, None, {"k_long_s", "k_short_g"}),                  # the one pass, bursts of short blocks
+    "mixed_rounds": (2, 8, 11, 0.5, False, {"LWB_MIXED_ROUNDS": "1"}, {"k_long", "k_short"}),   # rounds
+    "chain": (6, 8, 11, 0.3, False, {"LWB_NO_MIXED": "1"}, {"k_chain"}),
+    "generic": (2, 8, 11, 0.3, False, {"LWB_FORCE_GENERIC": "1"}, {"k_imdct", "k_overlap", "k_save_state"}),   # four-kernel path
+    "residue_long": (2, 8, 11, 0.0, True, None, FRONT | {"k_long"}),
+    "residue_mid": (2, 10, 10, 0.0, True, None, FRONT | {"k_mid"}),
+    "residue_mixed": (2, 8, 11, 0.3, True, None, FRONT | {"k_long_s"}),                # front stages + the one pass
 }
+# kernels a shape's environment switches off, whatever the layout
+SWITCHED_OFF = {"mixed_rounds": {"k_long_s", "k_short_g", "k_row_copy"}, "chain": ALL_KERNELS - {"k_chain"},
+                "generic": ALL_KERNELS - GENERIC}
 
 
 def merged(*envs):
@@ -291,9 +297,10 @@ def merged(*envs):
 def test_every_path_writes_exactly_its_samples_in_every_layout(ctx, oracle, shape, memory, fmt):
     """Seven chains (one without packets) over three consecutive batches -- fresh streams first, so their first packet
     emits nothing -- in each layout; host-memory batches run their third batch in three pipelined chunks."""
-    C, bs0, bs1, p_short, residue, env = SHAPES[shape]
+    C, bs0, bs1, p_short, residue, env, reach = SHAPES[shape]
     rng = np.random.default_rng(100 * list(SHAPES).index(shape) + 10 * memory + fmt)
     kind = Kind(ctx, C, bs0, bs1)
+    reached = set()
     for layout in LAYOUTS:
         streams = [Stream(oracle, kind) for _ in range(7)]
         lengths = [[int(rng.integers(0, 7)) if s != 1 else 0 for s in range(7)] for _ in range(3)]
@@ -303,9 +310,14 @@ def test_every_path_writes_exactly_its_samples_in_every_layout(ctx, oracle, shap
             items = [(st, Packets(rng, st, lengths[b][s], residue)) for s, st in enumerate(streams)]
             batch = Batch(items, fmt, layout, rng, residue)
             chunks = {"LWB_E2E_CHUNKS": "3"} if memory == cabi.MEM_HOST and b == 2 else None
-            rc, pcm = batch.run(ctx, memory, env=merged(env, chunks))
+            with expect_kernels(ctx, not_ran=SWITCHED_OFF.get(shape, ())) as launched:
+                rc, pcm = batch.run(ctx, memory, env=merged(env, chunks))
             assert rc == 0, (layout, b, rc)
             batch.check(oracle, pcm, (shape, layout, b))
+            if layout != "odd":
+                reached |= {k for k, v in launched.items() if v}
+    if fmt in PLANAR or not reach & FUSED:             # (the fused kernels write planar output only)
+        assert reach <= reached, (sorted(reach - reached), sorted(reached))
 
 
 @pytest.mark.parametrize("memory", [cabi.MEM_HOST, cabi.MEM_DEVICE])
@@ -314,7 +326,7 @@ def test_every_path_writes_exactly_its_samples_in_every_layout(ctx, oracle, shap
 def test_prepared_batch_replays_into_a_padded_layout(ctx, oracle, shape, fmt, memory):
     """One prepared batch (lwb_plan_execute) run four times with new spectra in the same arenas: every step bit-exact and
     contained, in a padded layout and in one with offsets that are not multiples of 4."""
-    C, bs0, bs1, p_short, _, _ = SHAPES[shape]
+    C, bs0, bs1, p_short, _, _, _ = SHAPES[shape]
     for layout in ("padded", "odd"):
         rng = np.random.default_rng(77 + len(shape) + memory)
         kind = Kind(ctx, C, bs0, bs1)
@@ -343,6 +355,7 @@ def test_prepared_batch_replays_into_a_padded_layout(ctx, oracle, shape, fmt, me
         else:
             a_in, a_out = ctx.device_alloc(coeffs.nbytes), ctx.device_alloc(pcm.nbytes)
         plan = L.Batch(ctx, first.specs, cabi.ENTRY_SPECTRUM, memory, a_in, a_out, fmt)
+        kernels = []
         for step in range(4):
             if step:
                 first.items = [(st, Packets(rng, st, P, False, bf)) for st, bf in zip(streams, seqs)]
@@ -352,12 +365,16 @@ def test_prepared_batch_replays_into_a_padded_layout(ctx, oracle, shape, fmt, me
             if memory == cabi.MEM_DEVICE:
                 ctx.h2d(a_in, coeffs)
                 ctx.h2d(a_out, pcm)
-            plan.run()
+            with expect_kernels(ctx) as launched:
+                plan.run()
+            kernels.append(launched)
             ctx.synchronize()
             if memory == cabi.MEM_DEVICE:
                 ctx.d2h(pcm, a_out)
             plan.collect()
             first.check(oracle, pcm, (shape, layout, "step", step))
+        # step 0 runs on fresh streams and changes their state; step 1 plans and captures, steps 2 and 3 replay
+        assert kernels[1] == kernels[2] == kernels[3], (layout, kernels)      # a replay launches what the capture did
         plan.close()
         if memory == cabi.MEM_DEVICE:
             ctx.device_free(a_in)
@@ -374,7 +391,7 @@ def test_consecutive_calls_append_to_one_planar_buffer(ctx, oracle, shape, memor
     """Three calls decode one stereo stream into one [2][total] buffer, each at out_offset = the samples so far and
     out_stride = total: the buffer must end up as the oracle's concatenation.  A call that copied back the span between
     its first and last plane would overwrite channel 1's earlier samples."""
-    C, bs0, bs1, p_short, _, _ = SHAPES[shape]
+    C, bs0, bs1, p_short, _, _, _ = SHAPES[shape]
     rng = np.random.default_rng(5150 + memory + 2 * fmt)
     st = Stream(oracle, Kind(ctx, C, bs0, bs1))
     lengths = [5, 4, 6]
@@ -525,8 +542,9 @@ def test_heterogeneous_residue_batches(ctx, oracle, memory, fmt, seed):
 @pytest.mark.parametrize("shape", ["long", "mid1024", "short", "mixed", "residue_long", "residue_mixed"])
 def test_misaligned_device_arenas_match_aligned(ctx, oracle, shape, fmt):
     """coeffs / pcm (and the dense floor of the residue entry) 4, 8 or 12 bytes past a 16-byte boundary: the fused
-    kernels' bulk copies and vector stores cannot take them, so the batch runs elsewhere -- with the same bytes."""
-    C, bs0, bs1, p_short, residue, env = SHAPES[shape]
+    kernels' bulk copies and vector stores cannot take them, so the batch runs on the chain kernel -- with the same bytes.
+    The aligned batches reach the shape's fused kernels."""
+    C, bs0, bs1, p_short, residue, env, reach = SHAPES[shape]
     kind = Kind(ctx, C, bs0, bs1)
     arenas = {}
     for shift in (0, 4, 8, 12):
@@ -535,13 +553,18 @@ def test_misaligned_device_arenas_match_aligned(ctx, oracle, shape, fmt):
         lengths = rng.integers(1, 8, (2, 5))
         for s, st in enumerate(streams):
             st.plan(rng, int(lengths[:, s].sum()), p_short)
+        reached = set()
         for b in range(2):
             items = [(st, Packets(rng, st, int(lengths[b, s]), residue)) for s, st in enumerate(streams)]
             batch = Batch(items, fmt, "padded", rng, residue)
-            rc, pcm = batch.run(ctx, cabi.MEM_DEVICE, shift=shift, env=env)
+            with expect_kernels(ctx, ran={"k_chain"} if shift else (), not_ran=ALL_KERNELS - {"k_chain"} if shift else ()) as launched:
+                rc, pcm = batch.run(ctx, cabi.MEM_DEVICE, shift=shift, env=env)
+            reached |= {k for k, v in launched.items() if v}
             assert rc == 0, (shift, b, rc)
             batch.check(oracle, pcm, (shape, shift, b))
             arenas[(shift, b)] = pcm
+        if not shift:
+            assert reach & FUSED <= reached, (sorted(reach), sorted(reached))
         for st in streams:
             st.pwr.close()
     for shift in (4, 8, 12):

@@ -31,6 +31,86 @@ def test_header_symbols_exported(lib):
     assert lib.lwb_abi_version() == 3
 
 
+CSRC = os.path.join(ROOT, "lewton_b200", "csrc")
+# launch wrappers of the kernel headers -> the LWB_KERNEL_* id of the kernel each one launches
+WRAPPERS = {"long_launch": "LWB_KERNEL_LONG", "long_launch_static": "LWB_KERNEL_LONG_S", "mid_launch": "LWB_KERNEL_MID",
+            "short_launch": "LWB_KERNEL_SHORT", "short_launch_groups": "LWB_KERNEL_SHORT_G"}
+
+
+def _kernel_id(kernel):
+    return "LWB_KERNEL_" + kernel[2:].upper()
+
+
+def _csrc_texts():
+    out = {}
+    for f in sorted(os.listdir(CSRC)):
+        if f.endswith((".cu", ".cuh", ".h", ".cpp")):
+            txt = open(os.path.join(CSRC, f)).read()
+            # comments blanked (lengths kept, so that offsets still point at the same lines)
+            out[f] = re.sub(r"//[^\n]*|/\*.*?\*/", lambda m: re.sub(r"[^\n]", " ", m.group(0)), txt, flags=re.S)
+    return out
+
+
+def _enclosing_function(txt, pos):
+    """Name of the function whose definition starts (at column 0) last before offset `pos`."""
+    name = None
+    for m in re.finditer(r"^(?!#|\s|\{|\}|template\b|struct\b|namespace\b)[^\n;]*?\b(\w+)\s*\(", txt[:pos], re.M):
+        if m.group(1) not in ("__launch_bounds__",):
+            name = m.group(1)
+    return name
+
+
+def test_header_kernel_ids_match_the_kernels():
+    """One LWB_KERNEL_* id per __global__ function of the library, in the order _cabi.KERNELS names them."""
+    from lewton_b200 import _cabi
+    hdr = open(os.path.join(ROOT, "include", "lewton_b200.h")).read()
+    ids = dict((k, int(v)) for k, v in re.findall(r"\b(LWB_KERNEL_\w+)\s*=\s*(\d+)", hdr))
+    assert ids.pop("LWB_KERNEL_COUNT") == len(ids) == len(_cabi.KERNELS)
+    assert [ids[_kernel_id(k)] for k in _cabi.KERNELS] == list(range(len(_cabi.KERNELS)))
+    kernels = set()
+    for txt in _csrc_texts().values():
+        kernels |= set(re.findall(r"__global__\s+void\s+(?:__launch_bounds__\([^)]*\)\s*)?(k_\w+)\s*\(", txt))
+    assert kernels == set(_cabi.KERNELS)
+
+
+def test_every_kernel_launch_is_attributed_to_its_kernel():
+    """Every `<<<` of the library sits in launch() (path_generic.cuh) or in a launch wrapper of a kernel header; every
+    launch() call names the id of the kernel it launches, every wrapper call goes through launched() with the id of the
+    wrapper's kernel, and only those two count launches.  So a launch site that does not attribute itself fails here,
+    and Context.kernel_launches() tells exactly which kernels a batch ran."""
+    texts = _csrc_texts()
+    sites = 0
+    for f, txt in texts.items():
+        assert not re.search(r"\bcu(da)?(Launch\w*|GraphLaunch)\s*\(", txt), f"{f}: launches outside <<<>>>"
+        for m in re.finditer(r"<<<", txt):
+            fn = _enclosing_function(txt, m.start())
+            line = txt[txt.rfind("\n", 0, m.start()) + 1:m.start()]
+            if fn == "launch":
+                assert f == "path_generic.cuh" and line.strip() == "kernel", (f, line)
+            else:
+                assert fn in WRAPPERS, f"{f}: a launch in {fn}() that no kernel id accounts for: {line.strip()}"
+                k = re.search(r"\b(k_\w+)\s*(<[^<>]*>)?\s*$", line)
+                assert k and _kernel_id(k.group(1)) == WRAPPERS[fn], (f, fn, line)
+            sites += 1
+        for m in re.finditer(r"\blaunch\s*\(", txt):
+            if re.match(r"static int launch\(", txt[txt.rfind("\n", 0, m.start()) + 1:]):
+                continue                                                        # the definition
+            a = re.match(r"launch\s*\(\s*ctx\s*,\s*(LWB_KERNEL_\w+)\s*,\s*(k_\w+)", txt[m.start():])
+            assert a, f"{f}: launch() without a kernel id: {txt[m.start():m.start() + 80]!r}"
+            assert a.group(1) == _kernel_id(a.group(2)), (f, a.group(0))
+        for w, kid in WRAPPERS.items():
+            for m in re.finditer(r"\b%s\s*\(" % w, txt):
+                if re.match(r"[^\n]*\binline int %s\(" % w, txt[txt.rfind("\n", 0, m.start()) + 1:]):
+                    continue                                                    # the definition
+                before = re.search(r"launched\s*\(\s*ctx\s*,\s*(LWB_KERNEL_\w+)\s*,\s*$", txt[:m.start()])
+                assert before and before.group(1) == kid, f"{f}: {w}() not counted as {kid}"
+        for m in re.finditer(r"\bcount_launch\s*\(|(\+\+|--)\s*\w+\s*->\s*(kernel_)?launches\b|"
+                             r"->\s*(launches|kernel_launches\s*\[[^\]]*\])\s*(\+\+|--|[-+]?=(?!=))", txt):
+            fn = _enclosing_function(txt, m.end())
+            assert fn in ("launch", "launched", "count_launch"), f"{f}: launches counted in {fn}()"
+    assert sites >= 10
+
+
 def test_struct_layouts_match_header(lib, tmp_path):
     """sizeof of every ABI struct as the C compiler sees it == the ctypes mirror."""
     from lewton_b200 import _cabi

@@ -8,10 +8,13 @@ import pytest
 
 import lewton_b200 as L
 import vorbis_packer as vp
-from helpers import RefStream, bits_equal, mismatch_report
+from helpers import (ALL_KERNELS, FRONT, RefStream, bits_equal, expect_kernels, launches_are_attributed,
+                     mismatch_report)
 from lewton_b200 import _cabi as cabi
 from lewton_b200 import frontend as fe
 from test_frontend_cpu import floor0_expected
+
+launches_are_attributed  # (autouse)
 
 pytestmark = pytest.mark.gpu
 
@@ -593,6 +596,76 @@ def test_vq_entry_accumulates_the_residue_on_the_device(ctx, oracle, channels, r
     assert np.array_equal(pcm.view(np.uint8), outs[cabi.ENTRY_RESIDUE][0].view(np.uint8)), "VQ entry and dense residue entry differ"
     for a, b in zip(states, outs[cabi.ENTRY_RESIDUE][2]):
         assert (a is None) == (b is None) and (a is None or bits_equal(a, b))
+
+
+@pytest.mark.filterwarnings("ignore:overflow encountered:RuntimeWarning")      # (the packer's own f32 sums)
+def test_vq_entry_sums_that_overflow_to_inf(ctx, oracle):
+    """VQ books whose values are finite but within a factor of two of FLT_MAX (minimum +-2^127, delta 2^120): two passes
+    over a bin overflow the f32 sum to +-inf (and +inf + -inf to NaN) in d_vq_accumulate, as the reference's `+=` does
+    (audio.rs:595, :611).  Uniform long stereo packets, so k_floor1_segments + k_prologue_fused<VQ> form the spectrum
+    and k_long transforms it; bit-identical to the oracle and to the dense residue entry of the same packets."""
+    rng = np.random.default_rng(531)
+    S, P, channels = 4, 6, 2
+    spec = vp.StreamSpec(rng, channels=channels, residue_types=[1], cascade_p=1.0)
+    for i in spec.vq_ids:
+        spec.books[i].set_values(2.0 ** 127 * (1 if i % 2 else -1), 2.0 ** 120, False)
+    assert all(np.all(np.isfinite(spec.books[i].vq)) for i in spec.vq_ids)
+    hdr = fe.Headers(spec.ident_packet(), spec.comment_packet(), spec.setup_packet())
+    assert hdr.vq_capable()
+    su = hdr.make_setup(ctx)
+    streams, wants, overflowed = [], [], False
+    for s in range(S):
+        pkts, infos = [], []
+        for mode, prev, nxt in consistent_modes(spec, rng, P, p_short=0.0):
+            pk, info = spec.audio_packet(mode, prev, nxt, p_unused=0.1)
+            pkts.append(pk)
+            infos.append(info)
+            overflowed |= bool(np.any(np.isinf(spec.expected(info)[1])))
+        streams.append(pkts)
+        wants.append(np.concatenate(oracle_pcm(oracle, spec, infos)[0], axis=1))
+    assert overflowed, "test should overflow a residue sum to inf"
+    assert all(not np.all(np.isfinite(w)) for w in wants[:2]), "test should carry inf / NaN to the output"
+    stride = P * (1 << spec.bs1) // 2
+    outs = {}
+    for entry in (cabi.ENTRY_VQ, cabi.ENTRY_RESIDUE):
+        pwrs = [L.PreviousWindowRight(su) for _ in range(S)]
+        coeffs, kinds, ys, runs, ents, roffs, eoffs, chains = [], [], [], [], [], [0], [0], []
+        for s, pkts in enumerate(streams):
+            modes, prevs, nexts = [], [], []
+            for pk in pkts:
+                dense = hdr.decode_packet(pk)
+                dp, rr, ee = hdr.decode_packet_vq(pk)
+                k, y, _ = dense.pack()
+                kinds.append(k)
+                ys.append(y)
+                coeffs.append(dense.residue.ravel())
+                runs.append(rr)
+                ents.append(ee)
+                roffs.append(roffs[-1] + len(rr))
+                eoffs.append(eoffs[-1] + len(ee))
+                modes.append(dp.mode_number); prevs.append(dp.prev_window_flag); nexts.append(dp.next_window_flag)
+            chains.append(L.ChainSpec(pwrs[s], np.array(modes, np.uint8), np.array(prevs, np.uint8), np.array(nexts, np.uint8),
+                                      coeff_offset=s * channels * stride, packet_index=s * P,
+                                      out_offset=s * channels * stride, out_stride=stride))
+        kw = dict(floor_kind=np.concatenate(kinds), floor1_y=np.concatenate(ys))
+        if entry == cabi.ENTRY_VQ:
+            kw["vq"] = (np.concatenate(runs), np.array(roffs, np.uint64), np.concatenate(ents), np.array(eoffs, np.uint64))
+        pcm = np.zeros(S * channels * stride, np.float32)
+        with expect_kernels(ctx, ran={"k_floor1_segments": 1, "k_prologue_fused": 1, "k_long": 1},
+                            not_ran=ALL_KERNELS - FRONT - {"k_long"}):
+            L.decode_chains(ctx, chains, entry, cabi.MEM_HOST, None if entry == cabi.ENTRY_VQ else np.concatenate(coeffs), pcm,
+                            cabi.OUT_F32_PLANAR, **kw)
+        outs[entry] = (pcm, [p.data() for p in pwrs])
+        for s in range(S):
+            n = wants[s].shape[1]
+            assert chains[s].status == 0 and chains[s].n_samples == n, (entry, s)
+            got = pcm[s * channels * stride:(s + 1) * channels * stride].reshape(channels, stride)[:, :n]
+            assert bits_equal(got, wants[s]), (entry, s, mismatch_report(got, wants[s]))
+        for p in pwrs:
+            p.close()
+    assert np.array_equal(outs[cabi.ENTRY_VQ][0].view(np.uint8), outs[cabi.ENTRY_RESIDUE][0].view(np.uint8))
+    for a, b in zip(outs[cabi.ENTRY_VQ][1], outs[cabi.ENTRY_RESIDUE][1]):
+        assert bits_equal(a, b)
 
 
 def test_stream_batcher_vq_entry(ctx, oracle):

@@ -8,8 +8,11 @@ import pytest
 
 import lewton_b200 as L
 from lewton_b200 import _cabi as cabi
-from helpers import (RefStream, assert_contained, bits_equal, fill_guard, make_setup, mismatch_report, mode_sequence,
-                     random_floor1, random_floor1_y, write_set)
+from helpers import (ALL_KERNELS, FRONT, GENERIC, RefStream, assert_contained, bits_equal, expect_kernels, fill_guard,
+                     launches_are_attributed, make_setup, mismatch_report, mode_sequence, random_floor1, random_floor1_y,
+                     write_set)
+
+launches_are_attributed  # (autouse)
 
 pytestmark = pytest.mark.gpu
 
@@ -255,6 +258,13 @@ def run_batch(ctx, su, pwrs, spec, n_packets, memory, env=None):
     return chains, pcm
 
 
+def long_batch_kernels(env):
+    """expect_kernels arguments for a uniform long spectrum batch run under `env` (see run_batch)."""
+    fg = (env or {}).get("LWB_FORCE_GENERIC")
+    ran = {"k_imdct", "k_overlap", "k_save_state"} if fg == "1" else {"k_chain"} if fg else {"k_long"}
+    return dict(ran=ran, not_ran=ALL_KERNELS - ran)
+
+
 def oracle_batch(oracle, spec, states=None):
     S, P, C, n2 = spec.shape
     outs, finals = [], []
@@ -284,13 +294,15 @@ def test_batch_long_blocks_vs_oracle(ctx, oracle, memory, env):
     pwrs = [L.PreviousWindowRight(su) for _ in range(S)]
     spec1 = (rng.standard_normal((S, P, C, 1024)) * 0.05).astype(np.float32)
     spec2 = (rng.standard_normal((S, P, C, 1024)) * 0.05).astype(np.float32)
-    chains, pcm1 = run_batch(ctx, su, pwrs, spec1, P, memory, env)
+    with expect_kernels(ctx, **long_batch_kernels(env)):
+        chains, pcm1 = run_batch(ctx, su, pwrs, spec1, P, memory, env)
     want1, st1 = oracle_batch(oracle, spec1)
     for s in range(S):
         assert chains[s].status == 0 and chains[s].packets_done == P and chains[s].n_samples == (P - 1) * 1024
         assert bits_equal(pcm1[s][:, : (P - 1) * 1024], want1[s]), (s, mismatch_report(pcm1[s][:, : (P - 1) * 1024], want1[s]))
         assert bits_equal(pwrs[s].data(), st1[s])
-    chains, pcm2 = run_batch(ctx, su, pwrs, spec2, P, memory, env)
+    with expect_kernels(ctx, **long_batch_kernels(env)):
+        chains, pcm2 = run_batch(ctx, su, pwrs, spec2, P, memory, env)
     want2, st2 = oracle_batch(oracle, spec2, st1)
     for s in range(S):
         assert chains[s].n_samples == P * 1024
@@ -321,15 +333,18 @@ def test_fused_and_generic_agree_at_scale(ctx, oracle):
     spec = (rng.standard_normal((S, P, C, 1024)) * 0.02).astype(np.float32)
     pa = [L.PreviousWindowRight(su) for _ in range(S)]
     pb = [L.PreviousWindowRight(su) for _ in range(S)]
-    _, fused = run_batch(ctx, su, pa, spec, P, cabi.MEM_DEVICE)
-    _, generic = run_batch(ctx, su, pb, spec, P, cabi.MEM_DEVICE, {"LWB_FORCE_GENERIC": "1"})
+    with expect_kernels(ctx, **long_batch_kernels(None)):
+        _, fused = run_batch(ctx, su, pa, spec, P, cabi.MEM_DEVICE)
+    with expect_kernels(ctx, **long_batch_kernels({"LWB_FORCE_GENERIC": "1"})):
+        _, generic = run_batch(ctx, su, pb, spec, P, cabi.MEM_DEVICE, {"LWB_FORCE_GENERIC": "1"})
     assert np.array_equal(fused.view(np.uint32), generic.view(np.uint32))
     want, _ = oracle_batch(oracle, spec[:3])
     for s in range(3):
         assert bits_equal(fused[s][:, : (P - 1) * 1024], want[s])
     # linearity of the whole path in exact arithmetic: scaling the input by 2 scales the output by 2
     pc = [L.PreviousWindowRight(su) for _ in range(S)]
-    _, doubled = run_batch(ctx, su, pc, spec * np.float32(2), P, cabi.MEM_DEVICE)
+    with expect_kernels(ctx, **long_batch_kernels(None)):
+        _, doubled = run_batch(ctx, su, pc, spec * np.float32(2), P, cabi.MEM_DEVICE)
     assert np.array_equal(doubled.view(np.uint32), (fused * np.float32(2)).view(np.uint32))
 
 
@@ -423,7 +438,8 @@ def test_special_values_on_gpu(ctx, oracle):
     assert np.any(np.isnan(want[1]))
     for env in (None, {"LWB_FORCE_GENERIC": "1"}, {"LWB_FORCE_GENERIC": "2"}):
         pwrs = [L.PreviousWindowRight(su) for _ in range(2)]
-        _, pcm = run_batch(ctx, su, pwrs, spec, 4, cabi.MEM_HOST, env)
+        with expect_kernels(ctx, **long_batch_kernels(env)):
+            _, pcm = run_batch(ctx, su, pwrs, spec, 4, cabi.MEM_HOST, env)
         for s in range(2):
             assert bits_equal(pcm[s][:, :3072], want[s]), (env, s, mismatch_report(pcm[s][:, :3072], want[s]))
             assert bits_equal(pwrs[s].data(), fin[s])
@@ -445,12 +461,14 @@ def test_fused_i16_planar_output(ctx, oracle, memory):
                           out_stride=stride) for s in range(S)]
     pcm = np.zeros((S, C, stride), np.int16)
     if memory == cabi.MEM_HOST:
-        L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, memory, spec, pcm, cabi.OUT_I16_PLANAR)
+        with expect_kernels(ctx, **long_batch_kernels(None)):
+            L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, memory, spec, pcm, cabi.OUT_I16_PLANAR)
     else:
         d_in, d_out = ctx.device_alloc(spec.nbytes), ctx.device_alloc(pcm.nbytes)
         ctx.h2d(d_in, spec)
         ctx.h2d(d_out, pcm)
-        L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, memory, d_in, d_out, cabi.OUT_I16_PLANAR)
+        with expect_kernels(ctx, **long_batch_kernels(None)):
+            L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, memory, d_in, d_out, cabi.OUT_I16_PLANAR)
         ctx.synchronize()
         ctx.d2h(pcm, d_out)
         ctx.device_free(d_in)
@@ -476,52 +494,52 @@ def test_residue_entry_long_batch_uses_prologue_plus_fused(ctx, oracle, memory, 
     su = make_setup(ctx, channels, bs0, bs1, modes=modes, mappings=mappings, floors=floors)
     pwrs = [L.PreviousWindowRight(su) for _ in range(S)]
     refs = [RefStream(oracle, channels, bs0, bs1, modes, mappings, floors) for _ in range(S)]
-    launches0 = ctx.launch_count
-    for batch in range(2):
-        res = (rng.standard_normal((S, P, channels, 1024)) * rng.integers(0, 2, (S, P, channels, 1024))).astype(np.float32)
-        kinds = np.zeros((S, P, channels), np.uint8)
-        ys = np.zeros((S, P, channels, cabi.MAX_POSTS), np.uint32)
-        want = []
-        for s in range(S):
-            parts = []
-            for p in range(P):
-                fl = []
-                for c in range(channels):
-                    mult, xs = floors[mappings[0]["floor_of_channel"][c]]
-                    fl.append(None if rng.random() < 0.1 else random_floor1_y(rng, mult, len(xs)))
-                k, y, _ = L.DecodedPacket(1, res[s, p], fl).pack()
-                kinds[s, p], ys[s, p] = k, y
-                rc, pcm = refs[s].packet(1, 1, 1, res[s, p], fl)
-                assert rc == 0
-                parts.append(pcm)
-            want.append(np.concatenate(parts, axis=1))
-        stride = P * 1024
-        chains = [L.ChainSpec(pwrs[s], np.ones(P, np.uint8), coeff_offset=s * P * channels * 1024, packet_index=s * P,
-                              out_offset=s * channels * stride, out_stride=stride) for s in range(S)]
-        dt = np.float32 if fmt == "f32" else np.int16
-        of = cabi.OUT_F32_PLANAR if fmt == "f32" else cabi.OUT_I16_PLANAR
-        pcm = np.zeros((S, channels, stride), dt)
-        if memory == cabi.MEM_HOST:
-            L.decode_chains(ctx, chains, cabi.ENTRY_RESIDUE, memory, res, pcm, of, floor_kind=kinds, floor1_y=ys)
-        else:
-            d_in, d_out = ctx.device_alloc(res.nbytes), ctx.device_alloc(pcm.nbytes)
-            ctx.h2d(d_in, res)
-            ctx.h2d(d_out, pcm)
-            L.decode_chains(ctx, chains, cabi.ENTRY_RESIDUE, memory, d_in, d_out, of, floor_kind=kinds, floor1_y=ys)
-            ctx.synchronize()
-            ctx.d2h(pcm, d_out)
-            ctx.device_free(d_in)
-            ctx.device_free(d_out)
-        for s in range(S):
-            n = want[s].shape[1]
-            assert chains[s].status == 0 and chains[s].n_samples == n
-            if fmt == "f32":
-                assert bits_equal(pcm[s][:, :n], want[s]), (batch, s, mismatch_report(pcm[s][:, :n], want[s]))
+    with expect_kernels(ctx, ran={"k_floor1_segments": 2, "k_prologue_fused": 2, "k_long": 2},
+                        not_ran=ALL_KERNELS - FRONT - {"k_long"}):
+        for batch in range(2):
+            res = (rng.standard_normal((S, P, channels, 1024)) * rng.integers(0, 2, (S, P, channels, 1024))).astype(np.float32)
+            kinds = np.zeros((S, P, channels), np.uint8)
+            ys = np.zeros((S, P, channels, cabi.MAX_POSTS), np.uint32)
+            want = []
+            for s in range(S):
+                parts = []
+                for p in range(P):
+                    fl = []
+                    for c in range(channels):
+                        mult, xs = floors[mappings[0]["floor_of_channel"][c]]
+                        fl.append(None if rng.random() < 0.1 else random_floor1_y(rng, mult, len(xs)))
+                    k, y, _ = L.DecodedPacket(1, res[s, p], fl).pack()
+                    kinds[s, p], ys[s, p] = k, y
+                    rc, pcm = refs[s].packet(1, 1, 1, res[s, p], fl)
+                    assert rc == 0
+                    parts.append(pcm)
+                want.append(np.concatenate(parts, axis=1))
+            stride = P * 1024
+            chains = [L.ChainSpec(pwrs[s], np.ones(P, np.uint8), coeff_offset=s * P * channels * 1024, packet_index=s * P,
+                                  out_offset=s * channels * stride, out_stride=stride) for s in range(S)]
+            dt = np.float32 if fmt == "f32" else np.int16
+            of = cabi.OUT_F32_PLANAR if fmt == "f32" else cabi.OUT_I16_PLANAR
+            pcm = np.zeros((S, channels, stride), dt)
+            if memory == cabi.MEM_HOST:
+                L.decode_chains(ctx, chains, cabi.ENTRY_RESIDUE, memory, res, pcm, of, floor_kind=kinds, floor1_y=ys)
             else:
-                assert np.array_equal(pcm[s][:, :n], oracle.quantise_i16(want[s])), (batch, s)
-            assert bits_equal(pwrs[s].data(), refs[s].pwr.data())
-    # 2 batches x (k_floor1_segments + k_prologue_fused + fused kernel) = 6 launches: the generic IMDCT/overlap kernels did not run
-    assert ctx.launch_count - launches0 == 6
+                d_in, d_out = ctx.device_alloc(res.nbytes), ctx.device_alloc(pcm.nbytes)
+                ctx.h2d(d_in, res)
+                ctx.h2d(d_out, pcm)
+                L.decode_chains(ctx, chains, cabi.ENTRY_RESIDUE, memory, d_in, d_out, of, floor_kind=kinds, floor1_y=ys)
+                ctx.synchronize()
+                ctx.d2h(pcm, d_out)
+                ctx.device_free(d_in)
+                ctx.device_free(d_out)
+            for s in range(S):
+                n = want[s].shape[1]
+                assert chains[s].status == 0 and chains[s].n_samples == n
+                if fmt == "f32":
+                    assert bits_equal(pcm[s][:, :n], want[s]), (batch, s, mismatch_report(pcm[s][:, :n], want[s]))
+                else:
+                    assert np.array_equal(pcm[s][:, :n], oracle.quantise_i16(want[s])), (batch, s)
+                assert bits_equal(pwrs[s].data(), refs[s].pwr.data())
+        # 2 batches x (k_floor1_segments + k_prologue_fused + fused kernel): the generic IMDCT/overlap kernels did not run
 
 
 def test_prepared_batch_reuses_descriptors_and_replans_on_state_change(ctx, oracle):
@@ -689,6 +707,27 @@ def test_chain_kernel_vs_four_kernel_path_mixed_sequences(ctx, oracle, channels,
 _COUPLING_51 = [(0, 1), (2, 3), (0, 4)]
 
 
+def _mixed_variant_kernels(name, bs0, residue, memory):
+    """expect_kernels arguments of one variant of test_mixed_streams_are_segmented_between_fused_and_chain_kernels: the
+    kernels that variant exists to run, and the ones its switch disables."""
+    if name == "chain":                                  # LWB_NO_MIXED: the chain kernel alone, its own front half
+        return dict(ran={"k_chain"}, not_ran=ALL_KERNELS - {"k_chain"})
+    not_ran = set(GENERIC) | {"k_mid"}
+    ran = set(FRONT) if residue else set()
+    if bs0 == 8 and name in ("mixed", "mixed_nobalance", "mixed_nobursts", "mixed_chunked"):
+        ran |= {"k_long_s"}                              # the one-pass schedule
+        if memory == cabi.MEM_DEVICE:
+            not_ran |= {"k_long", "k_chain"}             # (no rounds behind it)
+    else:                                                # rounds: k_long, and k_short (bs0 == 8) or k_chain for the rest
+        ran |= {"k_long", "k_short" if bs0 == 8 and name != "mixed_noshort" else "k_chain"}
+        not_ran |= {"k_long_s", "k_short_g", "k_row_copy"}
+    if name == "mixed_nobursts":
+        not_ran |= {"k_short_g"}
+    if name == "mixed_noshort" or bs0 != 8:
+        not_ran |= {"k_short", "k_short_g"}
+    return dict(ran=ran, not_ran=not_ran)
+
+
 @pytest.mark.parametrize("entry,memory,fmt,seed,bs0,channels", [
     ("spectrum", cabi.MEM_HOST, cabi.OUT_F32_PLANAR, 80, 8, 2),
     ("spectrum", cabi.MEM_DEVICE, cabi.OUT_I16_PLANAR, 81, 8, 2),
@@ -785,30 +824,33 @@ def test_mixed_streams_are_segmented_between_fused_and_chain_kernels(ctx, oracle
             if env:
                 os.environ.update(env)
             launches0 = ctx.launch_count
-            try:
-                kw = dict(floor_kind=kinds, floor1_y=ys, dense_floor=dense) if residue else {}
-                if memory == cabi.MEM_DEVICE:
-                    d_in = ctx.device_alloc(coeffs.nbytes)
-                    d_out = ctx.device_alloc(max(pcm.nbytes, 4))
-                    ctx.h2d(d_in, coeffs)
-                    if residue:
-                        d_dense = ctx.device_alloc(dense.nbytes)
-                        ctx.h2d(d_dense, dense)
-                        kw["dense_floor"] = d_dense
-                    L.decode_chains(ctx, chains, cabi.ENTRY_RESIDUE if residue else cabi.ENTRY_SPECTRUM, memory, d_in, d_out, fmt, **kw)
-                    ctx.d2h(pcm, d_out)
-                    ctx.device_free(d_in)
-                    ctx.device_free(d_out)
-                    if residue:
-                        ctx.device_free(d_dense)
-                else:
-                    L.decode_chains(ctx, chains, cabi.ENTRY_RESIDUE if residue else cabi.ENTRY_SPECTRUM, memory, coeffs, pcm, fmt, **kw)
-            finally:
-                if env:
-                    for k in env:
-                        del os.environ[k]
-            n_launch = ctx.launch_count - launches0
+            with expect_kernels(ctx, **_mixed_variant_kernels(name, bs0, residue, memory)) as launched:
+                try:
+                    kw = dict(floor_kind=kinds, floor1_y=ys, dense_floor=dense) if residue else {}
+                    if memory == cabi.MEM_DEVICE:
+                        d_in = ctx.device_alloc(coeffs.nbytes)
+                        d_out = ctx.device_alloc(max(pcm.nbytes, 4))
+                        ctx.h2d(d_in, coeffs)
+                        if residue:
+                            d_dense = ctx.device_alloc(dense.nbytes)
+                            ctx.h2d(d_dense, dense)
+                            kw["dense_floor"] = d_dense
+                        L.decode_chains(ctx, chains, cabi.ENTRY_RESIDUE if residue else cabi.ENTRY_SPECTRUM, memory, d_in, d_out, fmt, **kw)
+                        ctx.d2h(pcm, d_out)
+                        ctx.device_free(d_in)
+                        ctx.device_free(d_out)
+                        if residue:
+                            ctx.device_free(d_dense)
+                    else:
+                        L.decode_chains(ctx, chains, cabi.ENTRY_RESIDUE if residue else cabi.ENTRY_SPECTRUM, memory, coeffs, pcm, fmt, **kw)
+                finally:
+                    if env:
+                        for k in env:
+                            del os.environ[k]
+                n_launch = ctx.launch_count - launches0
             one_pass = name in ("mixed", "mixed_nobalance", "mixed_nobursts") and bs0 == 8
+            if one_pass:        # the pass's short segments: k_short (eight packets and more) and / or k_short_g (bursts)
+                assert launched["k_short"] + launched["k_short_g"] >= 1, launched
             if one_pass and memory == cabi.MEM_DEVICE:
                 # (two front stages +) k_long + k_short, no rounds; streams with history: their state rows are copied first
                 # k_short takes the short runs of eight packets and more, k_short_g the bursts: one of them or both
@@ -885,17 +927,17 @@ def test_mid_block_kernel_uniform_batches(ctx, oracle, bs, channels, fmt, memory
                     out_off += stride * channels
                 coeffs = np.concatenate(coeffs)
                 pcm = np.zeros(out_off, dt)
-                launches0 = ctx.launch_count
-                if memory == cabi.MEM_DEVICE:
-                    d_in, d_out = ctx.device_alloc(coeffs.nbytes), ctx.device_alloc(pcm.nbytes)
-                    ctx.h2d(d_in, coeffs)
-                    L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, memory, d_in, d_out, fmt)
-                    ctx.d2h(pcm, d_out)
-                    ctx.device_free(d_in)
-                    ctx.device_free(d_out)
-                else:
-                    L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, memory, coeffs, pcm, fmt)
-                assert ctx.launch_count - launches0 == 1
+                k = "k_mid" if name == "mid" else "k_chain"
+                with expect_kernels(ctx, ran={k: 1}, not_ran=ALL_KERNELS - {k}):
+                    if memory == cabi.MEM_DEVICE:
+                        d_in, d_out = ctx.device_alloc(coeffs.nbytes), ctx.device_alloc(pcm.nbytes)
+                        ctx.h2d(d_in, coeffs)
+                        L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, memory, d_in, d_out, fmt)
+                        ctx.d2h(pcm, d_out)
+                        ctx.device_free(d_in)
+                        ctx.device_free(d_out)
+                    else:
+                        L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, memory, coeffs, pcm, fmt)
                 pos = 0
                 got_all = []
                 for s in range(S):
@@ -960,27 +1002,31 @@ def test_segmented_paths_agree_with_chain_kernel_on_arbitrary_flags(ctx, fmt, se
         pwrs = [L.PreviousWindowRight(su) for _ in range(S)]
         log = []
         launches0 = ctx.launch_count
-        if env:
-            os.environ.update(env)
-        try:
-            for seqs, coeffs in batches:
-                chains, coeff_off = [], 0
-                stride = P * 1536          # (a long block in front of a short one emits up to 1472 samples)
-                for s in range(S):
-                    mode_ids, prev, nxt = seqs[s]
-                    chains.append(L.ChainSpec(pwrs[s], mode_ids, prev, nxt, coeff_offset=coeff_off, out_offset=s * C * stride,
-                                              out_stride=stride))
-                    coeff_off += int(sum(C * (1024 if m == 1 else 128) for m in mode_ids))
-                pcm = np.zeros(S * C * stride, dt)
-                L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, cabi.MEM_HOST, coeffs, pcm, fmt)
-                rows = pcm.reshape(S, C, stride)
-                log.append(([(c.status, c.n_samples, c.packets_done) for c in chains],
-                            [rows[s, :, :chains[s].n_samples].copy() for s in range(S)],
-                            [None if p.is_empty() else p.data().copy() for p in pwrs]))
-        finally:
+        # LWB_MIXED_ROUNDS turns the one pass (k_long_s) off, LWB_NO_MIXED the fused kernels
+        off = {"segmented": set(), "rounds": {"k_long_s", "k_short_g", "k_row_copy"}, "chain": ALL_KERNELS - {"k_chain"}}[name]
+        with expect_kernels(ctx, ran={"segmented": {"k_long_s"} if not p_bad else set(), "rounds": {"k_long"},
+                                      "chain": {"k_chain"}}[name], not_ran=off | GENERIC):
             if env:
-                for k in env:
-                    del os.environ[k]
+                os.environ.update(env)
+            try:
+                for seqs, coeffs in batches:
+                    chains, coeff_off = [], 0
+                    stride = P * 1536          # (a long block in front of a short one emits up to 1472 samples)
+                    for s in range(S):
+                        mode_ids, prev, nxt = seqs[s]
+                        chains.append(L.ChainSpec(pwrs[s], mode_ids, prev, nxt, coeff_offset=coeff_off, out_offset=s * C * stride,
+                                                  out_stride=stride))
+                        coeff_off += int(sum(C * (1024 if m == 1 else 128) for m in mode_ids))
+                    pcm = np.zeros(S * C * stride, dt)
+                    L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, cabi.MEM_HOST, coeffs, pcm, fmt)
+                    rows = pcm.reshape(S, C, stride)
+                    log.append(([(c.status, c.n_samples, c.packets_done) for c in chains],
+                                [rows[s, :, :chains[s].n_samples].copy() for s in range(S)],
+                                [None if p.is_empty() else p.data().copy() for p in pwrs]))
+            finally:
+                if env:
+                    for k in env:
+                        del os.environ[k]
         results[name] = log
         results[name + "_launches"] = ctx.launch_count - launches0
     # clean chains take the one pass (when they are the larger part of the batch), the others their rounds behind it
@@ -1046,7 +1092,11 @@ def test_one_pass_schedule_many_runs_per_warp(ctx, oracle, fmt, bursts, p_short)
             coeffs = np.concatenate(coeffs)
             pcm = np.zeros(out_off, dt)
             launches0 = ctx.launch_count
-            L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, cabi.MEM_HOST, coeffs, pcm, fmt)
+            # the one pass: k_long_s, then k_short_g over the bursts (LWB_NO_BURSTS: k_short takes them), k_row_copy once
+            # there is state to move
+            ran = {"k_long_s", "k_short_g" if bursts else "k_short"} | ({"k_row_copy"} if batch else set())
+            with expect_kernels(ctx, ran=ran, not_ran=GENERIC | {"k_long", "k_chain", "k_mid"} | (set() if bursts else {"k_short_g"})):
+                L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, cabi.MEM_HOST, coeffs, pcm, fmt)
             assert ctx.launch_count - launches0 <= 4 * 8, ctx.launch_count - launches0      # (copy +) k_long_s + k_short (+ k_short_g) per host chunk
             pos = 0
             for s in range(S):
@@ -1091,7 +1141,8 @@ def test_fused_kernel_many_short_runs_per_warp(ctx, oracle, P):
     chains = [L.ChainSpec(pwrs[s], modes, coeff_offset=s * P * 1024, out_offset=s * stride, out_stride=stride) for s in range(S)]
     pcm = np.full(S * stride, np.nan, np.float32)
     launches0 = ctx.launch_count
-    L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, cabi.MEM_HOST, spec, pcm, cabi.OUT_F32_PLANAR)
+    with expect_kernels(ctx, **long_batch_kernels(None)):
+        L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, cabi.MEM_HOST, spec, pcm, cabi.OUT_F32_PLANAR)
     assert ctx.launch_count - launches0 <= 8            # fused kernel (one launch per host chunk)
     got = pcm.reshape(S, stride)[:, :n]
     for s in range(S):
@@ -1115,7 +1166,8 @@ def test_fused_kernel_many_short_runs_per_warp(ctx, oracle, P):
     n2 = want2[0].shape[1]
     pcm2 = np.full(S * P * 1024, np.nan, np.float32)
     chains2 = [L.ChainSpec(pwrs[s], modes, coeff_offset=s * P * 1024, out_offset=s * P * 1024, out_stride=P * 1024) for s in range(S)]
-    L.decode_chains(ctx, chains2, cabi.ENTRY_SPECTRUM, cabi.MEM_HOST, spec, pcm2, cabi.OUT_F32_PLANAR)
+    with expect_kernels(ctx, **long_batch_kernels(None)):
+        L.decode_chains(ctx, chains2, cabi.ENTRY_SPECTRUM, cabi.MEM_HOST, spec, pcm2, cabi.OUT_F32_PLANAR)
     got2 = pcm2.reshape(S, P * 1024)[:, :n2]
     assert n2 == P * 1024
     for d in range(D):
@@ -1179,17 +1231,20 @@ def test_mid_block_kernel_residue_entry(ctx, oracle, bs, channels, fmt, memory, 
                                       out_offset=s * channels * stride, out_stride=stride) for s in range(S)]
                 pcm = fill_guard(np.empty(S * channels * stride, dt))
                 launches0 = ctx.launch_count
-                if memory == cabi.MEM_DEVICE:
-                    d_in, d_out, d_dense = ctx.device_alloc(coeffs.nbytes), ctx.device_alloc(pcm.nbytes), ctx.device_alloc(dense.nbytes)
-                    ctx.h2d(d_in, coeffs)
-                    ctx.h2d(d_dense, dense)
-                    ctx.h2d(d_out, pcm)
-                    L.decode_chains(ctx, chains, cabi.ENTRY_RESIDUE, memory, d_in, d_out, fmt, floor_kind=kinds, floor1_y=ys, dense_floor=d_dense)
-                    ctx.d2h(pcm, d_out)
-                    for h in (d_in, d_out, d_dense):
-                        ctx.device_free(h)
-                else:
-                    L.decode_chains(ctx, chains, cabi.ENTRY_RESIDUE, memory, coeffs, pcm, fmt, floor_kind=kinds, floor1_y=ys, dense_floor=dense)
+                # mid: the front stages, then k_mid; LWB_NO_MID: the chain kernel with its own front half
+                want_k = {"k_floor1_segments": 1, "k_prologue_fused": 1, "k_mid": 1} if name == "mid" else {"k_chain": 1}
+                with expect_kernels(ctx, ran=want_k, not_ran=ALL_KERNELS - set(want_k)):
+                    if memory == cabi.MEM_DEVICE:
+                        d_in, d_out, d_dense = ctx.device_alloc(coeffs.nbytes), ctx.device_alloc(pcm.nbytes), ctx.device_alloc(dense.nbytes)
+                        ctx.h2d(d_in, coeffs)
+                        ctx.h2d(d_dense, dense)
+                        ctx.h2d(d_out, pcm)
+                        L.decode_chains(ctx, chains, cabi.ENTRY_RESIDUE, memory, d_in, d_out, fmt, floor_kind=kinds, floor1_y=ys, dense_floor=d_dense)
+                        ctx.d2h(pcm, d_out)
+                        for h in (d_in, d_out, d_dense):
+                            ctx.device_free(h)
+                    else:
+                        L.decode_chains(ctx, chains, cabi.ENTRY_RESIDUE, memory, coeffs, pcm, fmt, floor_kind=kinds, floor1_y=ys, dense_floor=dense)
                 assert ctx.launch_count - launches0 == (3 if name == "mid" else 1)
                 for s in range(S):
                     n = want[s].shape[1]
@@ -1223,7 +1278,9 @@ def test_mid_block_kernel_residue_entry(ctx, oracle, bs, channels, fmt, memory, 
         batch = L.Batch(ctx, chains, cabi.ENTRY_RESIDUE, cabi.MEM_DEVICE, d_in, d_out, fmt, floor_kind=kinds, floor1_y=ys, dense_floor=d_dense)
         for it in range(4):
             pcm = np.zeros(S * channels * stride, dt)
-            batch.run()
+            with expect_kernels(ctx, ran={"k_floor1_segments": 1, "k_prologue_fused": 1, "k_mid": 1},
+                                not_ran=ALL_KERNELS - FRONT - {"k_mid"}):
+                batch.run()
             ctx.synchronize()
             ctx.d2h(pcm, d_out)
             batch.collect()
@@ -1269,9 +1326,8 @@ def test_prepared_mid_batch_replays(ctx, oracle, bs):
     for it in range(4):
         pcm = np.full(S * channels * stride, np.nan, np.float32)
         ctx.h2d(d_out, pcm)
-        l0 = ctx.launch_count
-        batch.run()
-        assert ctx.launch_count - l0 == 1
+        with expect_kernels(ctx, ran={"k_mid": 1}, not_ran=ALL_KERNELS - {"k_mid"}):
+            batch.run()
         ctx.synchronize()
         ctx.d2h(pcm, d_out)
         batch.collect()
@@ -1325,12 +1381,14 @@ def test_prepared_mixed_batch_replays_captured_rounds(ctx, oracle):
     d_out = ctx.device_alloc(S * channels * stride * 4)
     ctx.h2d(d_in, spec)
     batch = L.Batch(ctx, chains, cabi.ENTRY_SPECTRUM, cabi.MEM_DEVICE, d_in, d_out, cabi.OUT_F32_PLANAR)
-    counts = []
+    counts, kernels = [], []
     for it in range(4):
         pcm = np.full(S * channels * stride, np.nan, np.float32)
         ctx.h2d(d_out, pcm)
         l0 = ctx.launch_count
-        batch.run()
+        with expect_kernels(ctx, ran={"k_long_s"}, not_ran=GENERIC | {"k_mid", "k_long"}) as launched:
+            batch.run()
+        kernels.append(launched)
         counts.append(ctx.launch_count - l0)
         ctx.synchronize()
         ctx.d2h(pcm, d_out)
@@ -1348,6 +1406,7 @@ def test_prepared_mixed_batch_replays_captured_rounds(ctx, oracle):
             assert bits_equal(got, want), (it, s, mismatch_report(got, want))
             assert bits_equal(pwrs[s].data(), refs[s].pwr.data()), (it, s)
     assert counts[1] == counts[2] == counts[3] and counts[1] >= 3, counts
+    assert kernels[1] == kernels[2] == kernels[3], kernels       # a replay launches what the capturing execution did
     batch.close()
     ctx.device_free(d_in)
     ctx.device_free(d_out)
@@ -1411,7 +1470,7 @@ def test_prepared_residue_batches_replay_front_stages(ctx, oracle, shape, channe
                         floor_memory=cabi.MEM_DEVICE)
     else:
         batch = L.Batch(ctx, chains, cabi.ENTRY_RESIDUE, cabi.MEM_DEVICE, d_in, d_out, fmt, floor_kind=kinds, floor1_y=ys)
-    counts = []
+    counts, kernels = [], []
     for it in range(4):
         coeffs, want = [], []
         for s in range(S):
@@ -1439,7 +1498,13 @@ def test_prepared_residue_batches_replay_front_stages(ctx, oracle, shape, channe
         pcm = np.zeros(S * channels * stride, np.float32 if f32 else np.int16)
         ctx.h2d(d_out, pcm)
         l0 = ctx.launch_count
-        batch.run()
+        if shape == "long":
+            ran, not_ran = {"k_floor1_segments": 1, "k_prologue_fused": 1, "k_long": 1}, ALL_KERNELS - FRONT - {"k_long"}
+        else:
+            ran, not_ran = FRONT | {"k_long_s"}, GENERIC | {"k_mid"}
+        with expect_kernels(ctx, ran=ran, not_ran=not_ran) as launched:
+            batch.run()
+        kernels.append(launched)
         counts.append(ctx.launch_count - l0)
         ctx.synchronize()
         ctx.d2h(pcm, d_out)
@@ -1454,6 +1519,7 @@ def test_prepared_residue_batches_replay_front_stages(ctx, oracle, shape, channe
                 assert np.array_equal(got, oracle.quantise_i16(want[s])), (it, s)
             assert bits_equal(pwrs[s].data(), refs[s].pwr.data()), (it, s)
     assert counts[2] == counts[3], counts
+    assert kernels[1] == kernels[2] == kernels[3], kernels       # step 1 captures, steps 2 and 3 replay: the same kernels
     if shape == "long":
         assert counts[3] == 3, counts              # k_floor1_segments + k_prologue_fused + k_long, nothing else
     batch.close()
@@ -1509,22 +1575,24 @@ def test_short_block_kernel_uniform_batches(ctx, oracle, channels, P, S, fmt, me
             if env:
                 os.environ.update(env)
             l0 = ctx.launch_count
-            try:
-                if memory == cabi.MEM_DEVICE:
-                    d_in, d_out = ctx.device_alloc(spec.nbytes), ctx.device_alloc(pcm.nbytes)
-                    ctx.h2d(d_in, spec)
-                    ctx.h2d(d_out, pcm)
-                    L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, memory, d_in, d_out, fmt)
-                    ctx.synchronize()
-                    ctx.d2h(pcm, d_out)
-                    ctx.device_free(d_in)
-                    ctx.device_free(d_out)
-                else:
-                    L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, memory, spec, pcm, fmt)
-            finally:
-                if env:
-                    for k in env:
-                        del os.environ[k]
+            k = "k_short" if name == "short" else "k_chain"
+            with expect_kernels(ctx, ran={k: 1}, not_ran=ALL_KERNELS - {k}):
+                try:
+                    if memory == cabi.MEM_DEVICE:
+                        d_in, d_out = ctx.device_alloc(spec.nbytes), ctx.device_alloc(pcm.nbytes)
+                        ctx.h2d(d_in, spec)
+                        ctx.h2d(d_out, pcm)
+                        L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, memory, d_in, d_out, fmt)
+                        ctx.synchronize()
+                        ctx.d2h(pcm, d_out)
+                        ctx.device_free(d_in)
+                        ctx.device_free(d_out)
+                    else:
+                        L.decode_chains(ctx, chains, cabi.ENTRY_SPECTRUM, memory, spec, pcm, fmt)
+                finally:
+                    if env:
+                        for k in env:
+                            del os.environ[k]
             assert ctx.launch_count - l0 == 1, (name, ctx.launch_count - l0)       # one k_short (or one k_chain) launch
             outs[(name, batch)] = pcm
             for s in range(S):

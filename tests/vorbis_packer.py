@@ -135,23 +135,29 @@ class Codebook:
             else:
                 self.lookup_values = entries * dims
             self.multiplicands = rng.integers(0, 1 << self.value_bits, self.lookup_values).tolist()
-            vq = np.zeros((entries, dims), np.float32)
-            mn, dl = np.float32(self.minimum), np.float32(self.delta)
-            for e in range(entries):
-                last = np.float32(0)
-                div = 1
-                for k in range(dims):
-                    if lookup_type == 1:
-                        mo = (e // div) % self.lookup_values
-                        div *= self.lookup_values
-                    else:
-                        mo = e * dims + k
-                    v = np.float32(np.float32(np.float32(self.multiplicands[mo]) * dl) + mn) + last
-                    v = np.float32(v)
-                    if self.sequence_p:
-                        last = v
-                    vq[e, k] = v
-            self.vq = vq
+            self.set_values(self.minimum, self.delta, self.sequence_p)
+
+    def set_values(self, minimum, delta, sequence_p):
+        """Value mapping of a VQ book (minimum, delta: exactly representable as Vorbis float32) and its vq table."""
+        self.minimum, self.delta, self.sequence_p = minimum, delta, sequence_p
+        entries, dims = self.entries, self.dims
+        vq = np.zeros((entries, dims), np.float32)
+        mn, dl = np.float32(self.minimum), np.float32(self.delta)
+        for e in range(entries):
+            last = np.float32(0)
+            div = 1
+            for k in range(dims):
+                if self.lookup_type == 1:
+                    mo = (e // div) % self.lookup_values
+                    div *= self.lookup_values
+                else:
+                    mo = e * dims + k
+                v = np.float32(np.float32(np.float32(self.multiplicands[mo]) * dl) + mn) + last
+                v = np.float32(v)
+                if self.sequence_p:
+                    last = v
+                vq[e, k] = v
+        self.vq = vq
 
     def write_header(self, w):
         w.write(0x564342, 24)
