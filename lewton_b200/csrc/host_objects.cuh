@@ -72,10 +72,17 @@ struct MixRound { size_t r0, nr, s0, ns, c0, nc, x0, nx, g0, ng, flat, nm; };   
                                                                             // round; flat: the one-pass round (static deal, k_long_s);
                                                                             // nm: groups of k_mid (path_mid.cuh, from the buffer's start)
 struct RowCopy { const float *src; float *dst; uint32_t n4, pad; };  // n4 float4s, copied in front of the round's kernels
+struct ChainShape { unsigned warps; size_t smem; int n1max, wpc, np; };     // k_chain's block and shared memory
+// The arguments of mixed_launch_rounds (and of a captured k_long: pack and i16).  Built by aggregate initialisation;
+// the members a path leaves out are zero.
 struct MixLaunch {
-    char *db; size_t off_sr, off_cd, off_by, off_rc, off_sg;
-    const float *pack, *spack, *w_short, *mpack; int ls, mid_kb; bool i16, residue; int out_format; unsigned warps; size_t smem; int n1max, wpc, np;
-    const float *coeffs, *dense; const uint8_t *kinds; const uint32_t *ys; void *pcm;
+    char *db;                                   // descriptor buffer
+    void *pcm; int out_format; bool i16;
+    const float *pack; int ls; const float *w_short;                   // k_long / k_long_s
+    const float *spack;                                                 // k_short / k_short_g
+    const float *mpack; int mid_kb;                                     // k_mid
+    size_t off_sr, off_cd, off_by, off_rc, off_sg;                      // ShortRun, ChainDesc, mode bytes, RowCopy, bursts in db
+    bool residue; ChainShape chain; const float *coeffs, *dense; const uint8_t *kinds; const uint32_t *ys;   // k_chain
 };
 
 // One launch of the residue entry's front stages (k_floor1_segments + k_prologue_fused, or k_prologue): floor x
@@ -105,12 +112,22 @@ struct lwb_plan {
     uint64_t gen = 0;
     FrontStages front;
     DevBuf runs, pro, mix;             // descriptors the capture owns: k_long runs, the long path's front stages, the rest
-    uint32_t n_groups = 0;
-    const float *pack = nullptr;
-    bool i16 = false;
+    uint32_t n_groups = 0;             // k_long groups of `runs`
     MixLaunch mix_launch;
     std::vector<MixRound> mix_rounds;
 };
+
+// Records the launches a path made for a prepared batch; lwb_plan_execute replays them while ctx->state_gen == gen.
+static void capture(lwb_plan *plan, uint64_t gen, const FrontStages &front, const MixLaunch &ml, std::vector<MixRound> rounds,
+                    uint32_t n_groups = 0)
+{
+    plan->captured = true;
+    plan->gen = gen;
+    plan->front = front;
+    plan->mix_launch = ml;
+    plan->mix_rounds = std::move(rounds);
+    plan->n_groups = n_groups;
+}
 
 struct lwb_stream {
     lwb_ctx *ctx = nullptr;

@@ -526,12 +526,8 @@ extern "C" int lwb_decoded_sample_count(const lwb_setup *su, uint8_t mode, int p
 #include "path_mid.cuh"
 
 // The batch paths in the order they are tried; what none of them takes goes to the four-kernel path (run_generic).
-using BatchPath = int (*)(lwb_ctx *, lwb_chain *, size_t, const lwb_batch_io *, uint64_t, bool *, lwb_plan *);
-static const BatchPath kBatchPaths[] = {
-    [](lwb_ctx *ctx, lwb_chain *chains, size_t n, const lwb_batch_io *io, uint64_t epoch, bool *handled, lwb_plan *plan) {
-        return try_long(ctx, chains, n, io, epoch, handled, plan);
-    },
-    try_long_residue, try_mid, try_mixed, try_chain};
+using BatchPath = int (*)(lwb_ctx *, lwb_chain *, size_t, const lwb_batch_io *, bool *, lwb_plan *);
+static const BatchPath kBatchPaths[] = {try_long, try_long_residue, try_mid, try_mixed, try_chain};
 constexpr size_t kNumBatchPaths = sizeof(kBatchPaths) / sizeof(kBatchPaths[0]);
 
 // Index of the first batch path to try.  LWB_FORCE_GENERIC is a test switch that sends batches to the reference
@@ -554,97 +550,53 @@ static int decode_chains_impl(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, 
     if (io->entry == LWB_ENTRY_VQ && (!io->vq_runs || !io->vq_run_offsets || !io->vq_entries || !io->vq_entry_offsets || !io->floor_kind))
         return fail(ctx, LWB_ERR_INVALID, "VQ entry needs vq_runs, vq_entries, their offsets and floor_kind");
     CU(ctx, cudaSetDevice(ctx->device));
+    // what every path relies on: valid chains, each stream in one chain, and the residue entries' floor kinds and
+    // single channel count
     const uint64_t epoch = ++ctx->epoch;      // per context: concurrent calls on different contexts share nothing
-    if (prepared) {                           // the path that takes the batch captures it anew, if it can
-        prepared->captured = false;
-        prepared->mix_rounds.clear();
-    }
-    for (size_t k = first_batch_path(); k < kNumBatchPaths; k++) {
-        bool handled = false;
-        const int rc = kBatchPaths[k](ctx, chains, n_chains, io, epoch, &handled, prepared);
-        if (rc || handled) return rc;
-    }
-    const bool vq = io->entry == LWB_ENTRY_VQ;
-    const bool residue = io->entry != LWB_ENTRY_SPECTRUM;
-    const bool planar = is_planar(io->out_format);
-    std::vector<PlanChain> plan(n_chains);
-    uint64_t c_lo = ~0ull, c_hi = 0, o_lo = ~0ull, o_hi = 0, r_lo = ~0ull, r_hi = 0;
-    int uniform_c = -1;
-    bool need_dense = false;
+    const unsigned C = chains[0].stream ? chains[0].stream->setup->channels : 0;
     for (size_t i = 0; i < n_chains; i++) {
         lwb_chain *c = &chains[i];
         if (!c->stream || c->stream->ctx != ctx || (c->n_packets && !c->mode_numbers))
             return fail(ctx, LWB_ERR_INVALID, "chain: bad stream or mode list");
         if (c->stream->busy_epoch == epoch) return fail(ctx, LWB_ERR_INVALID, "a stream appears in two chains of one batch");
         c->stream->busy_epoch = epoch;
-        const int C = c->stream->setup->channels;
-        if (residue) {
-            if (uniform_c < 0) uniform_c = C;
-            if (uniform_c != C) return fail(ctx, LWB_ERR_INVALID, "residue batches need one channel count");
+        if (io->entry != LWB_ENTRY_SPECTRUM) {
+            if (c->stream->setup->channels != C) return fail(ctx, LWB_ERR_INVALID, "residue batches need one channel count");
             if (!io->floor_kind) return fail(ctx, LWB_ERR_INVALID, "residue entry needs floor_kind");
         }
-        plan_chain(c, &plan[i]);
+    }
+    if (prepared) {                           // the path that takes the batch captures it anew, if it can
+        prepared->captured = false;
+        prepared->mix_rounds.clear();
+    }
+    for (size_t k = first_batch_path(); k < kNumBatchPaths; k++) {
+        bool handled = false;
+        const int rc = kBatchPaths[k](ctx, chains, n_chains, io, &handled, prepared);
+        if (rc || handled) return rc;
+    }
+    std::vector<PlanChain> plan(n_chains);
+    std::vector<ChainWalk> walks(n_chains);
+    BatchExtent ext;
+    int rc;
+    for (size_t i = 0; i < n_chains; i++) {
+        lwb_chain *c = &chains[i];
         PlanChain &pc = plan[i];
-        if (pc.pk.empty()) continue;
-        const PlanPacket &last = pc.pk.back();
-        c_lo = std::min(c_lo, c->coeff_offset);
-        c_hi = std::max(c_hi, last.coeff_off + (uint64_t)C * (last.g.n >> 1));
-        const uint64_t ext = planar ? (uint64_t)(C - 1) * c->out_stride + c->n_samples : (uint64_t)c->n_samples * C;
-        if (planar && c->out_stride < c->n_samples) return fail(ctx, LWB_ERR_BUFFER, "chain: out_stride smaller than the samples produced");
-        o_lo = std::min(o_lo, c->out_offset);
-        o_hi = std::max(o_hi, c->out_offset + ext);
-        if (residue) {
-            r_lo = std::min(r_lo, c->packet_index);
-            r_hi = std::max<uint64_t>(r_hi, c->packet_index + pc.pk.size());
-            int krc = scan_floor_kinds(ctx, io, c->packet_index * C, (c->packet_index + pc.pk.size()) * C, &need_dense);
-            if (krc) return krc;
-        }
+        pc.c = c;
+        pc.pk.reserve(c->n_packets);
+        walks[i] = walk_chain(c, [&](uint32_t, const Geom &g, bool has, uint32_t plen, uint64_t coeff, uint64_t pos) {
+            pc.pk.push_back(PlanPacket{g, has ? plen : 0, coeff, pos});
+        });
+        set_chain_result(c, walks[i]);
+        if ((rc = ext.add(ctx, io, c, walks[i].done, walks[i].coeff_end, walks[i].n_samples))) return rc;
     }
-    if (need_dense && !io->dense_floor) return fail(ctx, LWB_ERR_INVALID, "dense_floor missing");
-    int rc = LWB_OK;
-    if (c_hi > c_lo) {
-        DevArenas ar = DevArenas();
-        const size_t esz = elem_size(io->out_format);
-        if (io->memory == LWB_MEM_HOST) {
-            // stage: H2D of the used coefficient range, D2H of the samples the chains produced
-            if (o_hi > o_lo && (rc = ensure(ctx, ctx->pcm, (o_hi - o_lo) * esz))) return rc;
-            if (!vq) {
-                if ((rc = ensure(ctx, ctx->coeffs, (c_hi - c_lo) * sizeof(float)))) return rc;
-                CU(ctx, cudaMemcpyAsync(ctx->coeffs.p, io->coeffs + c_lo, (c_hi - c_lo) * sizeof(float),
-                                        cudaMemcpyHostToDevice, ctx->stream));
-                ar.coeffs = (const float *)ctx->coeffs.p;
-            }
-            ar.coeff_base = c_lo;
-            if (need_dense) {
-                if ((rc = ensure(ctx, ctx->dense, (c_hi - c_lo) * sizeof(float)))) return rc;
-                CU(ctx, cudaMemcpyAsync(ctx->dense.p, io->dense_floor + c_lo, (c_hi - c_lo) * sizeof(float),
-                                        cudaMemcpyHostToDevice, ctx->stream));
-                ar.dense = (const float *)ctx->dense.p;
-            }
-            ar.pcm = ctx->pcm.p;
-            ar.pcm_base = o_lo;
-        } else {
-            ar.coeffs = vq ? nullptr : io->coeffs;
-            ar.dense = io->dense_floor;
-            ar.pcm = io->pcm;
-        }
-        if ((rc = stage_vq_arrays(ctx, io, r_lo, r_hi, ctx->stream, &ar.vq))) return rc;
-        if (residue) {
-            // absolute packet rows address the (biased) device views
-            if ((rc = stage_floor_arrays(ctx, io, r_lo, r_hi, (unsigned)uniform_c, ctx->stream, &ar.kinds, &ar.ys))) return rc;
-        }
-        rc = run_generic(ctx, plan, io, ar);
-        if (rc) return rc;
-        if (io->memory == LWB_MEM_HOST) {
-            if (o_hi > o_lo && (rc = copy_pcm_to_host(ctx, io, chains, 0, n_chains, ctx->pcm.p, o_lo, ctx->stream))) return rc;
-            CU(ctx, cudaStreamSynchronize(ctx->stream));
-        }
+    if ((rc = ext.finish(ctx, io))) return rc;
+    if (!ext.empty()) {
+        BatchArenas ar;
+        if ((rc = ar.open(ctx, io, ext, C, false)) || (rc = ar.upload(0, ext)) || (rc = run_generic(ctx, plan, io, ar)) ||
+            (rc = ar.download(0, chains, 0, n_chains, ext)) || (rc = ar.finish()))
+            return rc;
     }
-    // commit the host-side view of every stream's state
-    for (auto &pc : plan) {
-        lwb_stream *s = pc.c->stream;
-        if (!pc.pk.empty() || pc.clear_after) set_stream_state(s, pc.end_has, pc.end_plen);
-    }
+    commit_stream_states(chains, walks);
     return LWB_OK;
 }
 
@@ -694,7 +646,7 @@ extern "C" int lwb_plan_execute(lwb_plan *p)
     CU(ctx, cudaSetDevice(ctx->device));
     int rc;
     if (p->front.n && (rc = front_stages_run(ctx, &p->io, p->front))) return rc;    // they write ctx->spec, which the launch reads
-    if (p->mix_rounds.empty()) return launch_long(ctx, (const LongRun *)p->runs.p, p->n_groups, p->pack, p->i16);
+    if (p->mix_rounds.empty()) return launch_long(ctx, (const LongRun *)p->runs.p, p->n_groups, p->mix_launch.pack, p->mix_launch.i16);
     return mixed_launch_rounds(ctx, p->mix_launch, p->mix_rounds);
 }
 

@@ -1,5 +1,5 @@
 // path_generic.cuh -- part of the C-ABI translation unit (included by lwb_api.cu, not compiled on its own):
-// per-packet planning of a batch and the four-kernel path (kernels_generic.cuh).
+// the chain walk, extent and host-memory pipeline every batch path shares, and the four-kernel path (kernels_generic.cuh).
 #pragma once
 
 // ---------------------------------------------------------------------------------------------
@@ -15,53 +15,81 @@ struct PlanPacket {
 struct PlanChain {
     lwb_chain *c;
     std::vector<PlanPacket> pk;
-    bool end_has;           // stream state after the planned packets
-    uint32_t end_plen;
-    bool clear_after;       // OLA guard fired on packet pk.size(): state becomes empty
 };
 
-static int plan_chain(lwb_chain *c, PlanChain *pc)
+// What one chain decodes: the packets up to the first with a bad mode or an overlap the reference refuses, the samples
+// they produce and the stream state they leave (audio.rs:1056-1073, 1083-1154).
+struct ChainWalk {
+    uint32_t done = 0;            // packets decoded
+    int status = LWB_OK;
+    uint64_t n_samples = 0;       // per channel
+    bool end_has = false;         // stream state after them
+    uint32_t end_plen = 0;
+    bool clear_after = false;     // the OLA guard fired on packet `done`: the state becomes empty
+    uint64_t coeff_end = 0;       // element offset behind the last decoded packet
+};
+
+// Walks chain c from its stream's state, with no side effects.  on_packet(k, g, has, plen, coeff, pos) sees every packet
+// that decodes: its geometry, the state entering it, its coefficient offset and the samples the chain produced before it.
+template <typename F>
+static ChainWalk walk_chain(const lwb_chain *c, F &&on_packet)
 {
-    const lwb_stream *s = c->stream;
-    const lwb_setup *su = s->setup;
-    bool has = s->has;
-    uint32_t plen = s->plen;
+    const lwb_setup *su = c->stream->setup;
+    ChainWalk w;
+    bool has = c->stream->has;
+    uint32_t plen = c->stream->plen;
     uint64_t coeff = c->coeff_offset, pos = 0;
-    pc->c = c;
-    pc->clear_after = false;
-    c->status = LWB_OK;
-    pc->pk.reserve(c->n_packets);
-    for (uint32_t i = 0; i < c->n_packets; i++) {
-        PlanPacket pp;
-        int rc = geometry(su, c->mode_numbers[i], c->prev_window_flags ? c->prev_window_flags[i] : 1,
-                          c->next_window_flags ? c->next_window_flags[i] : 1, &pp.g);
-        if (rc) { c->status = rc; break; }
+    for (uint32_t k = 0; k < c->n_packets; k++) {
+        Geom g;
+        const int rc = geometry(su, c->mode_numbers[k], c->prev_window_flags ? c->prev_window_flags[k] : 1,
+                                c->next_window_flags ? c->next_window_flags[k] : 1, &g);
+        if (rc) { w.status = rc; break; }
         if (has) {
-            const uint32_t slope_len = 1u << ((pp.g.slope_sel ? su->bs1 : su->bs0) - 1);
+            const uint32_t slope_len = 1u << ((g.slope_sel ? su->bs1 : su->bs0) - 1);
             if (slope_len < plen) {             // audio.rs:1107-1111; :1083 has already taken the state
-                c->status = LWB_ERR_BAD_FORMAT;
-                pc->clear_after = true;
+                w.status = LWB_ERR_BAD_FORMAT;
+                w.clear_after = true;
                 break;
             }
-            if (pp.g.ls + plen > pp.g.n) {      // chan[range] would be out of bounds: a panic in the reference
-                c->status = LWB_ERR_MISMATCH;
+            if (g.ls + plen > g.n) {            // chan[range] would be out of bounds: a panic in the reference
+                w.status = LWB_ERR_MISMATCH;
                 break;
             }
         }
-        pp.plen = has ? plen : 0;
-        pp.coeff_off = coeff;
-        pp.sample_pos = pos;
-        coeff += (uint64_t)su->channels * (pp.g.n >> 1);
-        if (has) pos += pp.g.rs - pp.g.ls;
+        on_packet(k, g, has, plen, coeff, pos);
+        coeff += (uint64_t)su->channels * (g.n >> 1);
+        if (has) pos += g.rs - g.ls;
         has = true;
-        plen = pp.g.re - pp.g.rs;
-        pc->pk.push_back(pp);
+        plen = g.re - g.rs;
+        w.done++;
     }
-    pc->end_has = pc->clear_after ? false : has;
-    pc->end_plen = pc->clear_after ? 0 : plen;
-    c->packets_done = (uint32_t)pc->pk.size();
-    c->n_samples = (uint32_t)pos;
-    return LWB_OK;
+    w.n_samples = pos;
+    w.end_has = !w.clear_after && has;
+    w.end_plen = w.clear_after ? 0 : plen;
+    w.coeff_end = coeff;
+    return w;
+}
+
+static void set_chain_result(lwb_chain *c, const ChainWalk &w)
+{
+    c->status = w.status;
+    c->packets_done = w.done;
+    c->n_samples = (uint32_t)w.n_samples;
+}
+
+// The stream states the walks of a batch leave, committed once the batch's work is queued.
+static void commit_stream_states(lwb_chain *chains, const std::vector<ChainWalk> &walks)
+{
+    for (size_t i = 0; i < walks.size(); i++)
+        if (walks[i].done || walks[i].clear_after) set_stream_state(chains[i].stream, walks[i].end_has, walks[i].end_plen);
+}
+
+// The three mode bytes (mode, previous and next window flag) of packet k of chain c, as the chain kernel reads them.
+static void write_mode_bytes(const lwb_chain *c, uint32_t k, uint8_t *out)
+{
+    out[0] = c->mode_numbers[k];
+    out[1] = c->prev_window_flags ? c->prev_window_flags[k] : 1;
+    out[2] = c->next_window_flags ? c->next_window_flags[k] : 1;
 }
 
 // dynamic shared memory k_prologue needs for the chains of a batch (curve bytes of the largest block)
@@ -174,65 +202,178 @@ static int scan_floor_kinds(lwb_ctx *ctx, const lwb_batch_io *io, uint64_t row_l
     return LWB_OK;
 }
 
-// Device view of the floor arrays for packet rows [r_lo, r_hi) of a batch with C channels, biased so that ABSOLUTE
-// row indices address them: host arrays are uploaded to ctx->kinds / ctx->ys on `sm`, device arrays are used in place.
-static int stage_floor_arrays(lwb_ctx *ctx, const lwb_batch_io *io, uint64_t r_lo, uint64_t r_hi, unsigned C, cudaStream_t sm,
-                              const uint8_t **d_kinds, const uint32_t **d_ys)
+// The floor and VQ arrays (LWB_ENTRY_VQ) of packet rows [r_lo, r_hi) of a batch with C channels as the device sees
+// them, biased so that ABSOLUTE rows and offsets address them.  Host arrays get room in ctx->kinds / ys / vqoff / vqrec,
+// which upload_floor_rows fills; device arrays are used in place.
+struct FloorViews {
+    const uint8_t *kinds = nullptr;
+    const uint32_t *ys = nullptr;
+    VqView vq;
+};
+
+static int floor_views(lwb_ctx *ctx, const lwb_batch_io *io, uint64_t r_lo, uint64_t r_hi, unsigned C, FloorViews *v)
 {
-    *d_kinds = nullptr;
-    *d_ys = nullptr;
+    *v = FloorViews();
+    if (io->entry == LWB_ENTRY_SPECTRUM) return LWB_OK;
+    const bool vq = io->entry == LWB_ENTRY_VQ;
     if (io->floor_memory == LWB_MEM_DEVICE) {
-        *d_kinds = io->floor_kind;
-        *d_ys = io->floor1_y;
+        v->kinds = io->floor_kind;
+        v->ys = io->floor1_y;
+        if (vq) v->vq = VqView{io->vq_runs, io->vq_run_offsets, io->vq_entries, io->vq_entry_offsets};
         return LWB_OK;
     }
     if (r_hi <= r_lo) return LWB_OK;
     int rc;
     const size_t rows = (size_t)(r_hi - r_lo) * C;
     if ((rc = ensure(ctx, ctx->kinds, rows))) return rc;
-    CU(ctx, cudaMemcpyAsync(ctx->kinds.p, io->floor_kind + r_lo * C, rows, cudaMemcpyHostToDevice, sm));
-    *d_kinds = (const uint8_t *)ctx->kinds.p - r_lo * C;
+    v->kinds = (const uint8_t *)ctx->kinds.p - r_lo * C;
     if (io->floor1_y) {
         if ((rc = ensure(ctx, ctx->ys, rows * LWB_MAX_POSTS * sizeof(uint32_t)))) return rc;
-        CU(ctx, cudaMemcpyAsync(ctx->ys.p, io->floor1_y + r_lo * C * LWB_MAX_POSTS, rows * LWB_MAX_POSTS * sizeof(uint32_t),
-                                cudaMemcpyHostToDevice, sm));
-        *d_ys = (const uint32_t *)ctx->ys.p - r_lo * C * LWB_MAX_POSTS;
+        v->ys = (const uint32_t *)ctx->ys.p - r_lo * C * LWB_MAX_POSTS;
     }
-    return LWB_OK;
-}
-
-// LWB_ENTRY_VQ: device view of the VQ runs / entries of packet rows [r_lo, r_hi), biased so that absolute rows and
-// absolute offsets address it (host arrays are uploaded to ctx scratch on `sm`: four copies, all small).
-static int stage_vq_arrays(lwb_ctx *ctx, const lwb_batch_io *io, uint64_t r_lo, uint64_t r_hi, cudaStream_t sm, VqView *out)
-{
-    *out = VqView();
-    if (io->entry != LWB_ENTRY_VQ) return LWB_OK;
-    if (io->floor_memory == LWB_MEM_DEVICE) {
-        out->runs = io->vq_runs;
-        out->run_off = io->vq_run_offsets;
-        out->entries = io->vq_entries;
-        out->ent_off = io->vq_entry_offsets;
-        return LWB_OK;
-    }
-    if (r_hi <= r_lo) return LWB_OK;
-    int rc;
+    if (!vq) return LWB_OK;
     const uint64_t o_lo = io->vq_run_offsets[r_lo], o_hi = io->vq_run_offsets[r_hi];
     const uint64_t e_lo = io->vq_entry_offsets[r_lo], e_hi = io->vq_entry_offsets[r_hi];
     if (o_hi < o_lo || e_hi < e_lo) return fail(ctx, LWB_ERR_INVALID, "vq offsets must be non-decreasing");
-    const size_t nrow = (size_t)(r_hi - r_lo) + 1, nrun = (size_t)(o_hi - o_lo), nent = (size_t)(e_hi - e_lo);
-    const size_t b_off = nrow * sizeof(uint64_t), b_run = std::max<size_t>(nrun, 1) * sizeof(lwb_vq_run);
-    if ((rc = ensure(ctx, ctx->vqoff, 2 * b_off)) || (rc = ensure(ctx, ctx->vqrec, b_run + std::max<size_t>(nent, 1) * sizeof(uint16_t) + 16))) return rc;
-    char *d_off = (char *)ctx->vqoff.p, *d_rec = (char *)ctx->vqrec.p;
-    CU(ctx, cudaMemcpyAsync(d_off, io->vq_run_offsets + r_lo, b_off, cudaMemcpyHostToDevice, sm));
-    CU(ctx, cudaMemcpyAsync(d_off + b_off, io->vq_entry_offsets + r_lo, b_off, cudaMemcpyHostToDevice, sm));
-    if (nrun) CU(ctx, cudaMemcpyAsync(d_rec, io->vq_runs + o_lo, nrun * sizeof(lwb_vq_run), cudaMemcpyHostToDevice, sm));
-    if (nent) CU(ctx, cudaMemcpyAsync(d_rec + b_run, io->vq_entries + e_lo, nent * sizeof(uint16_t), cudaMemcpyHostToDevice, sm));
-    out->run_off = (const uint64_t *)d_off - r_lo;
-    out->ent_off = (const uint64_t *)(d_off + b_off) - r_lo;
-    out->runs = (const lwb_vq_run *)d_rec - o_lo;
-    out->entries = (const uint16_t *)(d_rec + b_run) - e_lo;
+    const size_t b_off = ((size_t)(r_hi - r_lo) + 1) * sizeof(uint64_t), b_run = std::max<size_t>((size_t)(o_hi - o_lo), 1) * sizeof(lwb_vq_run);
+    if ((rc = ensure(ctx, ctx->vqoff, 2 * b_off)) ||
+        (rc = ensure(ctx, ctx->vqrec, b_run + std::max<size_t>((size_t)(e_hi - e_lo), 1) * sizeof(uint16_t) + 16)))
+        return rc;
+    v->vq.run_off = (const uint64_t *)ctx->vqoff.p - r_lo;
+    v->vq.ent_off = (const uint64_t *)((char *)ctx->vqoff.p + b_off) - r_lo;
+    v->vq.runs = (const lwb_vq_run *)ctx->vqrec.p - o_lo;
+    v->vq.entries = (const uint16_t *)((char *)ctx->vqrec.p + b_run) - e_lo;
     return LWB_OK;
 }
+
+// H2D of the host floor and VQ arrays of rows [a, b) into views v, on `sm`.
+static int upload_floor_rows(lwb_ctx *ctx, const lwb_batch_io *io, uint64_t a, uint64_t b, unsigned C, const FloorViews &v, cudaStream_t sm)
+{
+    if (io->entry == LWB_ENTRY_SPECTRUM || io->floor_memory == LWB_MEM_DEVICE || b <= a) return LWB_OK;
+    const size_t rows = (size_t)(b - a) * C;
+    CU(ctx, cudaMemcpyAsync(const_cast<uint8_t *>(v.kinds) + a * C, io->floor_kind + a * C, rows, cudaMemcpyHostToDevice, sm));
+    if (io->floor1_y)
+        CU(ctx, cudaMemcpyAsync(const_cast<uint32_t *>(v.ys) + a * C * LWB_MAX_POSTS, io->floor1_y + a * C * LWB_MAX_POSTS,
+                                rows * LWB_MAX_POSTS * sizeof(uint32_t), cudaMemcpyHostToDevice, sm));
+    if (io->entry != LWB_ENTRY_VQ) return LWB_OK;
+    const uint64_t o_a = io->vq_run_offsets[a], o_b = io->vq_run_offsets[b], e_a = io->vq_entry_offsets[a], e_b = io->vq_entry_offsets[b];
+    const size_t b_off = ((size_t)(b - a) + 1) * sizeof(uint64_t);
+    CU(ctx, cudaMemcpyAsync(const_cast<uint64_t *>(v.vq.run_off) + a, io->vq_run_offsets + a, b_off, cudaMemcpyHostToDevice, sm));
+    CU(ctx, cudaMemcpyAsync(const_cast<uint64_t *>(v.vq.ent_off) + a, io->vq_entry_offsets + a, b_off, cudaMemcpyHostToDevice, sm));
+    if (o_b > o_a) CU(ctx, cudaMemcpyAsync(const_cast<lwb_vq_run *>(v.vq.runs) + o_a, io->vq_runs + o_a, (size_t)(o_b - o_a) * sizeof(lwb_vq_run), cudaMemcpyHostToDevice, sm));
+    if (e_b > e_a) CU(ctx, cudaMemcpyAsync(const_cast<uint16_t *>(v.vq.entries) + e_a, io->vq_entries + e_a, (size_t)(e_b - e_a) * sizeof(uint16_t), cudaMemcpyHostToDevice, sm));
+    return LWB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// extent and host-memory pipeline of a batch
+// ---------------------------------------------------------------------------------------------
+// The ranges a batch, or a chunk of it, reads and writes: coefficient elements [c_lo, c_hi), PCM elements [o_lo, o_hi)
+// and, for the residue entries, packet rows [r_lo, r_hi).
+struct BatchExtent {
+    uint64_t c_lo = ~0ull, c_hi = 0, o_lo = ~0ull, o_hi = 0, r_lo = ~0ull, r_hi = 0;
+    bool need_dense = false;      // a decoded row has a dense floor
+    bool scan = true;             // check the floor kinds of the rows added (a chunk's rows were checked with its batch)
+
+    // Chain c decodes `done` packets, whose coefficients end at coeff_end, into n_samples samples per channel.
+    int add(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chain *c, uint32_t done, uint64_t coeff_end, uint64_t n_samples)
+    {
+        if (!done) return LWB_OK;
+        const unsigned C = c->stream->setup->channels;
+        const bool planar = is_planar(io->out_format);
+        if (planar && c->out_stride < n_samples) return fail(ctx, LWB_ERR_BUFFER, "chain: out_stride smaller than the samples produced");
+        c_lo = std::min(c_lo, c->coeff_offset);
+        c_hi = std::max(c_hi, coeff_end);
+        o_lo = std::min(o_lo, c->out_offset);
+        o_hi = std::max(o_hi, c->out_offset + (planar ? (uint64_t)(C - 1) * c->out_stride + n_samples : n_samples * C));
+        if (io->entry == LWB_ENTRY_SPECTRUM) return LWB_OK;
+        r_lo = std::min(r_lo, c->packet_index);
+        r_hi = std::max<uint64_t>(r_hi, c->packet_index + done);
+        return scan ? scan_floor_kinds(ctx, io, c->packet_index * C, (c->packet_index + done) * C, &need_dense) : LWB_OK;
+    }
+    int finish(lwb_ctx *ctx, const lwb_batch_io *io) const
+    {
+        return need_dense && !io->dense_floor ? fail(ctx, LWB_ERR_INVALID, "dense_floor missing") : LWB_OK;
+    }
+    bool empty() const { return c_hi <= c_lo; }
+};
+
+// The arenas of a batch as its kernels address them: coefficients, dense floors and PCM by absolute element offset,
+// floor and VQ arrays by absolute packet row (FloorViews).  A host-memory batch is staged in the context's arenas,
+// chunk by chunk: upload(k) brings chunk k's inputs, download(k) takes its PCM home behind its kernels.  With the copy
+// streams (copy_in / copy_out, ordered by ev_in[k] / ev_done[k]) the copies of one chunk overlap the kernels of
+// another; otherwise everything runs on the compute stream.  A device-memory batch uses the caller's arenas in place.
+struct BatchArenas {
+    const float *coeffs = nullptr, *dense = nullptr;
+    char *pcm = nullptr;
+    FloorViews fl;
+    lwb_ctx *ctx = nullptr;
+    const lwb_batch_io *io = nullptr;
+    bool host = false;
+    unsigned C = 0;
+    uint64_t c_lo = 0, o_lo = 0;
+    cudaStream_t up = nullptr, down = nullptr;
+
+    int open(lwb_ctx *ctx_, const lwb_batch_io *io_, const BatchExtent &ext, unsigned C_, bool copy_streams)
+    {
+        ctx = ctx_;
+        io = io_;
+        C = C_;
+        c_lo = ext.c_lo;
+        o_lo = ext.o_lo;
+        host = io->memory == LWB_MEM_HOST;
+        const bool vq = io->entry == LWB_ENTRY_VQ;
+        up = host && copy_streams ? ctx->copy_in : ctx->stream;
+        down = host && copy_streams ? ctx->copy_out : ctx->stream;
+        int rc;
+        if (host) {
+            const size_t esz = elem_size(io->out_format), bytes = (size_t)(ext.c_hi - ext.c_lo) * sizeof(float);
+            if (ext.o_hi > ext.o_lo && (rc = ensure(ctx, ctx->pcm, (size_t)(ext.o_hi - ext.o_lo) * esz))) return rc;
+            if (!vq && (rc = ensure(ctx, ctx->coeffs, bytes))) return rc;
+            if (ext.need_dense && (rc = ensure(ctx, ctx->dense, bytes))) return rc;
+            coeffs = vq ? nullptr : (const float *)ctx->coeffs.p - c_lo;
+            dense = ext.need_dense ? (const float *)ctx->dense.p - c_lo : nullptr;
+            pcm = (char *)ctx->pcm.p - o_lo * esz;
+        } else {
+            coeffs = vq ? nullptr : io->coeffs;
+            dense = io->dense_floor;
+            pcm = (char *)io->pcm;
+        }
+        if ((rc = floor_views(ctx, io, ext.r_lo, ext.r_hi, C, &fl))) return rc;
+        return up != ctx->stream ? order_copies_behind_compute(ctx) : LWB_OK;
+    }
+    int upload(size_t k, const BatchExtent &ck)
+    {
+        int rc;
+        if (host) {
+            const size_t bytes = (size_t)(ck.c_hi - ck.c_lo) * sizeof(float);
+            if (coeffs) CU(ctx, cudaMemcpyAsync(const_cast<float *>(coeffs) + ck.c_lo, io->coeffs + ck.c_lo, bytes, cudaMemcpyHostToDevice, up));
+            if (dense) CU(ctx, cudaMemcpyAsync(const_cast<float *>(dense) + ck.c_lo, io->dense_floor + ck.c_lo, bytes, cudaMemcpyHostToDevice, up));
+        }
+        if ((rc = upload_floor_rows(ctx, io, ck.r_lo, ck.r_hi, C, fl, up))) return rc;
+        if (up == ctx->stream) return LWB_OK;
+        CU(ctx, cudaEventRecord(ctx->ev_in[k], up));
+        CU(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_in[k], 0));
+        return LWB_OK;
+    }
+    // chains [i0, i1) of the batch make up chunk k
+    int download(size_t k, const lwb_chain *chains, size_t i0, size_t i1, const BatchExtent &ck)
+    {
+        if (!host || ck.o_hi <= ck.o_lo) return LWB_OK;
+        if (down != ctx->stream) {
+            CU(ctx, cudaEventRecord(ctx->ev_done[k], ctx->stream));
+            CU(ctx, cudaStreamWaitEvent(down, ctx->ev_done[k], 0));
+        }
+        return copy_pcm_to_host(ctx, io, chains, i0, i1, ctx->pcm.p, o_lo, down);
+    }
+    int finish()
+    {
+        if (!host) return LWB_OK;
+        if (down != ctx->stream) CU(ctx, cudaStreamSynchronize(down));
+        CU(ctx, cudaStreamSynchronize(ctx->stream));
+        return LWB_OK;
+    }
+};
 
 // ---------------------------------------------------------------------------------------------
 // front stages of the fused paths (FrontStages)
@@ -281,43 +422,33 @@ static bool front_stages_fast(lwb_ctx *ctx, const lwb_batch_io *io, const FrontS
 }
 
 // Packets [k0, k0 + n) of fs on floor / VQ views the caller has staged.
-static int front_stages_launch(lwb_ctx *ctx, const lwb_batch_io *io, const FrontStages &fs, size_t k0, size_t n,
-                               const uint8_t *kinds, const uint32_t *ys, const VqView &vq)
+static int front_stages_launch(lwb_ctx *ctx, const lwb_batch_io *io, const FrontStages &fs, size_t k0, size_t n, const FloorViews &fl)
 {
     const FrontArenas a = front_arenas(ctx, io, fs);
-    return launch_prologue(ctx, fs.pk + k0, n, fs.C, fs.fast, fs.smem_old, fs.n2max, a.res, a.dense, kinds, ys, a.spec, vq);
+    return launch_prologue(ctx, fs.pk + k0, n, fs.C, fs.fast, fs.smem_old, fs.n2max, a.res, a.dense, fl.kinds, fl.ys, a.spec, fl.vq);
 }
 
 // Stages the floor and VQ arrays of fs's packet rows on the compute stream (host arrays are uploaded, device arrays
 // read in place) and launches the front stages over every packet of fs.
 static int front_stages_run(lwb_ctx *ctx, const lwb_batch_io *io, const FrontStages &fs)
 {
-    const uint8_t *kinds;
-    const uint32_t *ys;
-    VqView vq;
+    FloorViews fl;
     int rc;
-    if ((rc = stage_floor_arrays(ctx, io, fs.r_lo, fs.r_hi, fs.C, ctx->stream, &kinds, &ys))) return rc;
-    if ((rc = stage_vq_arrays(ctx, io, fs.r_lo, fs.r_hi, ctx->stream, &vq))) return rc;
-    return front_stages_launch(ctx, io, fs, 0, fs.n, kinds, ys, vq);
+    if ((rc = floor_views(ctx, io, fs.r_lo, fs.r_hi, fs.C, &fl))) return rc;
+    if ((rc = upload_floor_rows(ctx, io, fs.r_lo, fs.r_hi, fs.C, fl, ctx->stream))) return rc;
+    return front_stages_launch(ctx, io, fs, 0, fs.n, fl);
 }
 
-struct DevArenas {
-    const float *coeffs;      // device
-    const float *dense;       // device or null
-    const uint8_t *kinds;     // device or null
-    const uint32_t *ys;       // device or null
-    void *pcm;                // device
-    uint64_t coeff_base;      // element offset that device coeffs[0] corresponds to
-    uint64_t pcm_base;        // element offset that device pcm[0] corresponds to
-    VqView vq;                // LWB_ENTRY_VQ
-};
-
-// Generic path: rounds of packets bounded by the IMDCT scratch.
-static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_batch_io *io, const DevArenas &ar)
+// Generic path: rounds of packets bounded by the IMDCT scratch.  Its descriptors address a host-memory batch's
+// staging from its start (element c_lo / o_lo), a device-memory batch's arenas from element 0.
+static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_batch_io *io, const BatchArenas &ar)
 {
     size_t maxp = 0;
     for (auto &pc : plan) maxp = std::max(maxp, pc.pk.size());
     if (maxp == 0) return LWB_OK;
+    const uint64_t coeff_base = ar.host ? ar.c_lo : 0, pcm_base = ar.host ? ar.o_lo : 0;
+    const float *coeffs = ar.coeffs ? ar.coeffs + coeff_base : nullptr, *dense = ar.dense ? ar.dense + coeff_base : nullptr;
+    void *pcm = ar.pcm + pcm_base * elem_size(io->out_format);
     // x elements of one "packet column" (packet i of every chain), to size the rounds
     std::vector<uint32_t> start(plan.size(), 0);
     const bool planar = is_planar(io->out_format);
@@ -366,10 +497,10 @@ static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_bat
                 std::memset(&d, 0, sizeof(d));
                 d.setup = su->d_setup;
                 d.state = s->d_state;
-                d.coeff_off = pp.coeff_off - ar.coeff_base;
+                d.coeff_off = pp.coeff_off - coeff_base;
                 d.x_off = xo;
                 d.out_stride = pc.c->out_stride;
-                d.out_off = pc.c->out_offset - ar.pcm_base + (planar ? pp.sample_pos : pp.sample_pos * C);
+                d.out_off = pc.c->out_offset - pcm_base + (planar ? pp.sample_pos : pp.sample_pos * C);
                 d.pkt_index = pc.c->packet_index + start[ci] + k;
                 d.prev_packet = k ? (int32_t)(di - 1) : -1;
                 d.prev_rs = k ? hp[di - 1].rs : 0;
@@ -395,11 +526,11 @@ static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_bat
         }
         CU(ctx, cudaMemcpyAsync(ctx->desc.p, hp, n_desc * sizeof(DevPacket), cudaMemcpyHostToDevice, ctx->stream));
         const DevPacket *dp = (const DevPacket *)ctx->desc.p;
-        const float *spec = ar.coeffs;
+        const float *spec = coeffs;
         if (io->entry != LWB_ENTRY_SPECTRUM) {
             if ((rc = ensure(ctx, ctx->spec, spec_hi * sizeof(float)))) return rc;
-            if ((rc = launch_prologue(ctx, dp, hp, n_desc, maxc, prologue_smem_of(plan), ar.coeffs, ar.dense, ar.kinds, ar.ys,
-                                      (float *)ctx->spec.p, ar.vq)))
+            if ((rc = launch_prologue(ctx, dp, hp, n_desc, maxc, prologue_smem_of(plan), coeffs, dense, ar.fl.kinds, ar.fl.ys,
+                                      (float *)ctx->spec.p, ar.fl.vq)))
                 return rc;
             spec = (const float *)ctx->spec.p;
         }
@@ -408,10 +539,10 @@ static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_bat
             return rc;
         dim3 g2((unsigned)n_desc, maxc), b2(kOverlapThreads);
         switch (io->out_format) {
-        case LWB_OUT_F32_PLANAR: rc = launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<LWB_OUT_F32_PLANAR>, g2, b2, 0, dp, (const float *)ctx->x.p, ar.pcm); break;
-        case LWB_OUT_I16_PLANAR: rc = launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<LWB_OUT_I16_PLANAR>, g2, b2, 0, dp, (const float *)ctx->x.p, ar.pcm); break;
-        case LWB_OUT_F32_INTERLEAVED: rc = launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<LWB_OUT_F32_INTERLEAVED>, g2, b2, 0, dp, (const float *)ctx->x.p, ar.pcm); break;
-        default: rc = launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<LWB_OUT_I16_INTERLEAVED>, g2, b2, 0, dp, (const float *)ctx->x.p, ar.pcm); break;
+        case LWB_OUT_F32_PLANAR: rc = launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<LWB_OUT_F32_PLANAR>, g2, b2, 0, dp, (const float *)ctx->x.p, pcm); break;
+        case LWB_OUT_I16_PLANAR: rc = launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<LWB_OUT_I16_PLANAR>, g2, b2, 0, dp, (const float *)ctx->x.p, pcm); break;
+        case LWB_OUT_F32_INTERLEAVED: rc = launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<LWB_OUT_F32_INTERLEAVED>, g2, b2, 0, dp, (const float *)ctx->x.p, pcm); break;
+        default: rc = launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<LWB_OUT_I16_INTERLEAVED>, g2, b2, 0, dp, (const float *)ctx->x.p, pcm); break;
         }
         if (rc) return rc;
         if ((rc = launch(ctx, LWB_KERNEL_SAVE_STATE, k_save_state, g2, b2, 0, dp, (const float *)ctx->x.p))) return rc;

@@ -7,18 +7,15 @@
 
 struct MidGroup { LongRun r[4]; uint32_t n_packets; };
 
-static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, uint64_t epoch, bool *handled,
-                   lwb_plan *plan = nullptr)
+static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, bool *handled, lwb_plan *plan)
 {
     *handled = false;
     const uint64_t gen_at_entry = ctx->state_gen;
     if (getenv("LWB_NO_MID")) return LWB_OK;
     if (io->out_format != LWB_OUT_F32_PLANAR && io->out_format != LWB_OUT_I16_PLANAR) return LWB_OK;
     const bool vq = io->entry == LWB_ENTRY_VQ, residue = io->entry != LWB_ENTRY_SPECTRUM;
-    if (residue && !io->floor_kind) return LWB_OK;            // (the chain kernel words the error)
     if (vq) return LWB_OK;                                    // (VQ records of such streams: the general path, as before)
     if (!device_arenas_aligned(io)) return LWB_OK;
-    int uniform_c = -1;
     const bool i16 = io->out_format == LWB_OUT_I16_PLANAR;
     const size_t esz = i16 ? 2 : 4;
     const float *pack = nullptr;
@@ -27,13 +24,8 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
     size_t n_runs = 0;
     for (size_t i = 0; i < n_chains; i++) {
         const lwb_chain *c = &chains[i];
-        if (!c->stream || c->stream->ctx != ctx || (c->n_packets && !c->mode_numbers)) return LWB_OK;
         const lwb_setup *su = c->stream->setup;
         if (su->channels > 8 || (su->bs1 != 10 && su->bs1 != 9) || !su->host.tab[1].pack) return LWB_OK;
-        if (residue) {                                        // the front stages want one channel count per batch
-            if (uniform_c < 0) uniform_c = (int)su->channels;
-            if (uniform_c != (int)su->channels) return LWB_OK;
-        }
         if (pack && pack != su->host.tab[1].pack) return LWB_OK;
         pack = su->host.tab[1].pack;
         kb = 11 - su->bs1;
@@ -56,55 +48,31 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
     }
     if (!pack || !n_runs) return LWB_OK;
     const size_t kMidN2 = 1024u >> kb, NBg = (size_t)1 << kb;
+    const unsigned C = chains[0].stream->setup->channels;     // (residue entry: the batch's one channel count)
     *handled = true;
 
     const bool host = io->memory == LWB_MEM_HOST;
     cudaStream_t sm = ctx->stream;
     int rc;
-    uint64_t c_lo = ~0ull, c_hi = 0, o_lo = ~0ull, o_hi = 0, r_lo = ~0ull, r_hi = 0;
-    bool need_dense = false;
+    BatchExtent ext;
     size_t n_pk = 0;
     for (size_t i = 0; i < n_chains; i++) {
         lwb_chain *c = &chains[i];
-        lwb_stream *s = c->stream;
-        if (s->busy_epoch == epoch) return fail(ctx, LWB_ERR_INVALID, "a stream appears in two chains of one batch");
-        s->busy_epoch = epoch;
-        const unsigned C = s->setup->channels;
-        if (residue && c->n_packets) {
-            r_lo = std::min(r_lo, c->packet_index);
-            r_hi = std::max<uint64_t>(r_hi, c->packet_index + c->n_packets);
-            if ((rc = scan_floor_kinds(ctx, io, c->packet_index * C, (c->packet_index + c->n_packets) * C, &need_dense))) return rc;
-            n_pk += c->n_packets;
-        }
         c->status = LWB_OK;
         c->packets_done = c->n_packets;
-        c->n_samples = c->n_packets ? (uint32_t)((c->n_packets - (s->has ? 0u : 1u)) * (uint32_t)kMidN2) : 0u;
-        if (!c->n_packets) continue;
-        c_lo = std::min(c_lo, c->coeff_offset);
-        c_hi = std::max(c_hi, c->coeff_offset + (uint64_t)c->n_packets * C * kMidN2);
-        o_lo = std::min(o_lo, c->out_offset);
-        o_hi = std::max(o_hi, c->out_offset + (uint64_t)(C - 1) * c->out_stride + c->n_samples);
+        c->n_samples = c->n_packets ? (uint32_t)((c->n_packets - (c->stream->has ? 0u : 1u)) * (uint32_t)kMidN2) : 0u;
+        if (residue) n_pk += c->n_packets;
+        const uint64_t coeff_end = c->coeff_offset + (uint64_t)c->n_packets * c->stream->setup->channels * kMidN2;
+        if ((rc = ext.add(ctx, io, c, c->n_packets, coeff_end, c->n_samples))) return rc;
     }
-    if (need_dense && !io->dense_floor) return fail(ctx, LWB_ERR_INVALID, "dense_floor missing");
-    const float *d_coeffs = vq ? nullptr : io->coeffs;
-    char *d_pcm = (char *)io->pcm;
-    if (host) {
-        if (o_hi > o_lo && (rc = ensure(ctx, ctx->pcm, (size_t)(o_hi - o_lo) * esz))) return rc;
-        if (!vq) {
-            if ((rc = ensure(ctx, ctx->coeffs, (size_t)(c_hi - c_lo) * 4))) return rc;
-            CU(ctx, cudaMemcpyAsync(ctx->coeffs.p, io->coeffs + c_lo, (size_t)(c_hi - c_lo) * 4, cudaMemcpyHostToDevice, sm));
-            d_coeffs = (const float *)ctx->coeffs.p - c_lo;
-        }
-        if (need_dense) {
-            if ((rc = ensure(ctx, ctx->dense, (size_t)(c_hi - c_lo) * 4))) return rc;
-            CU(ctx, cudaMemcpyAsync(ctx->dense.p, io->dense_floor + c_lo, (size_t)(c_hi - c_lo) * 4, cudaMemcpyHostToDevice, sm));
-        }
-        d_pcm = (char *)ctx->pcm.p - o_lo * esz;
-    }
+    if ((rc = ext.finish(ctx, io))) return rc;
+    BatchArenas ar;
+    if ((rc = ar.open(ctx, io, ext, C, false)) || (rc = ar.upload(0, ext))) return rc;
+    const float *d_coeffs = ar.coeffs;
     // A prepared batch in device memory owns its descriptors (run groups, then the front stages' packet list) and replays
     // them while no stream changes shape (lwb_plan_execute).
-    const bool capture = plan && !host;
-    DevBuf &dbuf = capture ? plan->mix : ctx->cdesc;
+    const bool cap = plan && !host;
+    DevBuf &dbuf = cap ? plan->mix : ctx->cdesc;
     const size_t NBcap = (size_t)1 << kb;
     const size_t off_pro = (n_runs * NBcap * sizeof(LongRun) + 15) & ~(size_t)15;      // (an upper bound: every run its own group)
     if ((rc = ensure(ctx, dbuf, off_pro + n_pk * sizeof(DevPacket) + 16))) return rc;
@@ -112,17 +80,17 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
     if (residue) {
         // front stages over every packet of the batch: residue (or VQ records) + floors -> spectrum arena, same element
         // offsets as the coefficient arena
-        if ((rc = ensure(ctx, ctx->spec, (size_t)(c_hi - c_lo) * 4))) return rc;
+        if ((rc = ensure(ctx, ctx->spec, (size_t)(ext.c_hi - ext.c_lo) * 4))) return rc;
         DevPacket *d_pro = (DevPacket *)((char *)dbuf.p + off_pro);
         fs.pk = d_pro;
         fs.n = n_pk;
-        fs.C = (unsigned)uniform_c;
-        fs.smem_old = prologue_smem(uniform_c, 11 - kb);
+        fs.C = C;
+        fs.smem_old = prologue_smem((int)C, 11 - kb);
         fs.n2max = (int)kMidN2;
-        fs.c_lo = c_lo;
-        fs.r_lo = r_lo;
-        fs.r_hi = r_hi;
-        fs.dense = need_dense;
+        fs.c_lo = ext.c_lo;
+        fs.r_lo = ext.r_lo;
+        fs.r_hi = ext.r_hi;
+        fs.dense = ext.need_dense;
         Staging *stp;
         if ((rc = acquire_staging(ctx, n_pk * sizeof(DevPacket), &stp))) return rc;
         DevPacket *hp = (DevPacket *)stp->h;
@@ -135,8 +103,8 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
         CU(ctx, cudaMemcpyAsync(d_pro, hp, n_pk * sizeof(DevPacket), cudaMemcpyHostToDevice, sm));
         CU(ctx, cudaEventRecord(stp->ev, sm));
         stp->pending = true;
-        if ((rc = front_stages_run(ctx, io, fs))) return rc;
-        d_coeffs = (const float *)ctx->spec.p - c_lo;       // k_mid reads the spectrum
+        if ((rc = front_stages_launch(ctx, io, fs, 0, fs.n, ar.fl))) return rc;
+        d_coeffs = (const float *)ctx->spec.p - ext.c_lo;       // k_mid reads the spectrum
     }
     // runs, then groups of two runs of equal length (an odd one gets a dummy partner), longest first, dealt balanced
     std::vector<LongRun> runs;
@@ -151,7 +119,7 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
             LongRun lr;
             std::memset(&lr, 0, sizeof(lr));
             lr.in = d_coeffs + c->coeff_offset + (size_t)ch * kMidN2;
-            lr.out = d_pcm + (c->out_offset + (size_t)ch * c->out_stride) * esz;
+            lr.out = ar.pcm + (c->out_offset + (size_t)ch * c->out_stride) * esz;
             lr.state = s->d_state + (size_t)ch * state_stride(su);
             lr.in_stride = (uint32_t)(C * kMidN2);
             lr.n_packets = c->n_packets;
@@ -189,30 +157,14 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
     CU(ctx, cudaMemcpyAsync(dbuf.p, h, bytes, cudaMemcpyHostToDevice, sm));
     CU(ctx, cudaEventRecord(st->ev, sm));
     st->pending = true;
-    MixLaunch ml;
-    std::memset(&ml, 0, sizeof(ml));
-    ml.db = (char *)dbuf.p;
-    ml.mpack = pack;
-    ml.mid_kb = kb;
-    ml.i16 = i16;
-    ml.out_format = io->out_format;
-    ml.pcm = d_pcm;
+    const MixLaunch ml{(char *)dbuf.p, ar.pcm, io->out_format, i16, nullptr, 0, nullptr, nullptr, pack, kb};
     MixRound rd;
     std::memset(&rd, 0, sizeof(rd));
     rd.nm = groups.size();
     std::vector<MixRound> rounds(1, rd);
     if ((rc = mixed_launch_rounds(ctx, ml, rounds))) return rc;
-    if (capture) {
-        plan->captured = true;
-        plan->gen = gen_at_entry;
-        plan->front = fs;                   // (no packets: spectrum entry)
-        plan->mix_launch = ml;
-        plan->mix_rounds = std::move(rounds);
-    }
-    if (host) {
-        if (o_hi > o_lo && (rc = copy_pcm_to_host(ctx, io, chains, 0, n_chains, ctx->pcm.p, o_lo, sm))) return rc;
-        CU(ctx, cudaStreamSynchronize(sm));
-    }
+    if (cap) capture(plan, gen_at_entry, fs, ml, std::move(rounds));
+    if ((rc = ar.download(0, chains, 0, n_chains, ext)) || (rc = ar.finish())) return rc;
     for (size_t i = 0; i < n_chains; i++)
         if (chains[i].n_packets) set_stream_state(chains[i].stream, true, (uint32_t)kMidN2);
     return LWB_OK;

@@ -37,15 +37,13 @@ static void balance_static_deal(Run *runs, size_t n, size_t W, std::vector<Run> 
 // a group of k_short_g: eight runs of one length (the deal above moves it as a unit)
 struct ShortGroup { ShortRun r[kShortOct]; uint32_t n_packets; };
 
-static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, uint64_t epoch, bool *handled,
-                     lwb_plan *plan = nullptr)
+static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, bool *handled, lwb_plan *plan)
 {
     *handled = false;
     const uint64_t gen_at_entry = ctx->state_gen;
     if (getenv("LWB_NO_MIXED")) return LWB_OK;
     if (io->out_format != LWB_OUT_F32_PLANAR && io->out_format != LWB_OUT_I16_PLANAR) return LWB_OK;
     if (!device_arenas_aligned(io)) return LWB_OK;
-    const bool vq = io->entry == LWB_ENTRY_VQ;
     const bool residue = io->entry != LWB_ENTRY_SPECTRUM;
     const bool i16 = io->out_format == LWB_OUT_I16_PLANAR;
     const size_t esz = i16 ? 2 : 4;
@@ -55,7 +53,6 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
     const float *pack = nullptr, *spack = nullptr, *w_short = nullptr;
     for (size_t i = 0; i < n_chains; i++) {
         const lwb_chain *c = &chains[i];
-        if (!c->stream || c->stream->ctx != ctx || (c->n_packets && !c->mode_numbers)) return LWB_OK;
         const lwb_setup *su = c->stream->setup;
         if (su->channels > 8) return LWB_OK;
         // one twiddle pack per launch of each fused kernel (setups with identical tables share theirs, see
@@ -93,55 +90,33 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
     if (fast_like * 2 < total_packets) return LWB_OK;
     const int bs0e = bs0 >= 0 ? bs0 : kShortBs;
     const int ls_long = (kLongN - (1 << bs0e)) >> 2, pl_short = 1 << (bs0e - 1);
-    if (residue && !io->floor_kind) return fail(ctx, LWB_ERR_INVALID, "residue entry needs floor_kind");
     *handled = true;
 
     enum { SEG_CHAIN = 0, SEG_LONG = 1, SEG_SHORT = 2 };
     struct Seg { int kind; bool first_short, last_short; uint32_t p0, n; bool has; uint32_t plen; uint64_t coeff, pos; };
     bool chain_sees_long = false;       // the chain kernel's shared memory is sized for what it actually gets
-    struct Walk { uint32_t seg0, n_seg; bool end_has; uint32_t end_plen; bool touched; uint32_t boff; uint64_t coeff_end; size_t slot0; };
+    struct Walk { uint32_t seg0, n_seg; uint32_t boff; size_t slot0; };
     std::vector<Walk> walks(n_chains);
+    std::vector<ChainWalk> results(n_chains);
     std::vector<Seg> segs;
     segs.reserve(n_chains * 2);
     struct Pk { bool has; uint32_t plen; uint64_t coeff, pos; };
     std::vector<Pk> pk;
     std::vector<uint8_t> bytes(total_packets * 3 + 16);
     size_t boff = 0, max_rounds = 0;
-    uint64_t c_lo = ~0ull, c_hi = 0, o_lo = ~0ull, o_hi = 0, r_lo = ~0ull, r_hi = 0;
-    int uniform_c = -1;
-    bool need_dense = false;
+    BatchExtent ext;
+    int rc = LWB_OK;
     std::vector<uint8_t> is_l;           // bit0 k_long packet, bit1 follows a short block, bit2 precedes one; bit3 k_short packet
     for (size_t i = 0; i < n_chains; i++) {
         lwb_chain *c = &chains[i];
-        lwb_stream *s = c->stream;
-        const lwb_setup *su = s->setup;
-        if (s->busy_epoch == epoch) return fail(ctx, LWB_ERR_INVALID, "a stream appears in two chains of one batch");
-        s->busy_epoch = epoch;
-        const unsigned C = su->channels;
-        if (residue) {
-            if (uniform_c < 0) uniform_c = (int)C;
-            if (uniform_c != (int)C) return fail(ctx, LWB_ERR_INVALID, "residue batches need one channel count");
-        }
+        const lwb_setup *su = c->stream->setup;
         Walk &w = walks[i];
         w.boff = (uint32_t)boff;
-        bool has = s->has, clear_after = false;
-        uint32_t plen = s->plen, done = 0;
-        uint64_t coeff = c->coeff_offset, pos = 0;
-        c->status = LWB_OK;
         // pass 1: geometry + which packets the fused kernel may take (state entering them is empty or 1024)
         if (pk.size() < c->n_packets) { pk.resize(c->n_packets); is_l.resize(c->n_packets); }
         w.seg0 = (uint32_t)segs.size();
         w.n_seg = 0;
-        for (uint32_t k = 0; k < c->n_packets; k++) {
-            Geom g;
-            int grc = geometry(su, c->mode_numbers[k], c->prev_window_flags ? c->prev_window_flags[k] : 1,
-                               c->next_window_flags ? c->next_window_flags[k] : 1, &g);
-            if (grc) { c->status = grc; break; }
-            if (has) {
-                const uint32_t slope_len = 1u << ((g.slope_sel ? su->bs1 : su->bs0) - 1);
-                if (slope_len < plen) { c->status = LWB_ERR_BAD_FORMAT; clear_after = true; break; }
-                if (g.ls + plen > g.n) { c->status = LWB_ERR_MISMATCH; break; }
-            }
+        const ChainWalk &cw = results[i] = walk_chain(c, [&](uint32_t k, const Geom &g, bool has, uint32_t plen, uint64_t coeff, uint64_t pos) {
             pk[k] = Pk{has, plen, coeff, pos};
             is_l[k] = 0;
             if (g.blockflag && g.n == (uint32_t)kLongN && su->host.tab[1].pack == pack && pack) {
@@ -151,24 +126,13 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                        g.rs == (uint32_t)kShortN2 && g.re == (uint32_t)kShortN && (!has || plen == (uint32_t)kShortN2)) {
                 is_l[k] = 8;            // a full-window 256-point block on top of an empty or 128-sample state
             }
-            bytes[boff + 3 * k] = c->mode_numbers[k];
-            bytes[boff + 3 * k + 1] = c->prev_window_flags ? c->prev_window_flags[k] : 1;
-            bytes[boff + 3 * k + 2] = c->next_window_flags ? c->next_window_flags[k] : 1;
-            if (has) pos += g.rs - g.ls;
-            coeff += (uint64_t)C * (g.n >> 1);
-            has = true;
-            plen = g.re - g.rs;
-            done++;
-        }
-        c->packets_done = done;
-        c->n_samples = (uint32_t)pos;
-        w.end_has = clear_after ? false : has;
-        w.end_plen = clear_after ? 0u : plen;
-        w.touched = done > 0 || clear_after;
-        w.coeff_end = coeff;
+            write_mode_bytes(c, k, &bytes[boff + 3 * k]);
+        });
+        const uint32_t done = cw.done;
+        set_chain_result(c, cw);
         boff += (size_t)done * 3;
+        if ((rc = ext.add(ctx, io, c, done, cw.coeff_end, cw.n_samples))) return rc;
         if (!done) continue;
-        if (c->out_stride < pos) return fail(ctx, LWB_ERR_BUFFER, "chain: out_stride smaller than the samples produced");
         // pass 2: segments.  A fused-kernel run starts at a long block that follows a short one and ends at
         // one that precedes a short one; everything else is handed to the chain kernel.
         uint32_t k = 0;
@@ -191,19 +155,8 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         }
         w.n_seg = (uint32_t)segs.size() - w.seg0;
         max_rounds = std::max<size_t>(max_rounds, w.n_seg);
-        c_lo = std::min(c_lo, c->coeff_offset);
-        c_hi = std::max(c_hi, coeff);
-        o_lo = std::min(o_lo, c->out_offset);
-        o_hi = std::max(o_hi, c->out_offset + (uint64_t)(C - 1) * c->out_stride + pos);
-        if (residue) {
-            r_lo = std::min(r_lo, c->packet_index);
-            r_hi = std::max<uint64_t>(r_hi, c->packet_index + done);
-            int krc = scan_floor_kinds(ctx, io, c->packet_index * C, (c->packet_index + done) * C, &need_dense);
-            if (krc) return krc;
-        }
     }
-    if (need_dense && !io->dense_floor) return fail(ctx, LWB_ERR_INVALID, "dense_floor missing");
-    int rc = LWB_OK;
+    if ((rc = ext.finish(ctx, io))) return rc;
     // One pass instead of rounds: where every chain alternates strictly between long and short segments, the only
     // thing a segment needs from its predecessor is the pl = 128 samples the two blocks overlap in, and the sum
     // x[ls + i] w[i] + prev[i] w[pl-1-i] (audio.rs:1112-1118) does not care which of its two products exists first.
@@ -273,33 +226,15 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
     auto round_of = [&](size_t i, uint32_t q) { return chain_flat[i] ? (size_t)0 : round_base + q; };
     const int n1max_all = n1max;         // largest blocksize of the batch (front stages); n1max below sizes the chain kernel
     if (!chain_sees_long) n1max = n0max;
-    int wpc = std::max(1, std::min(8, n1max / 1024));
-    while (wpc > 1 && (unsigned)wpc * maxc > 32) wpc >>= 1;
-    const int np = chain_np(maxc, n1max, wpc, false);      // residue entry: the front stages run first, the kernels see a spectrum
-    const size_t smem = chain_smem(maxc, n1max, np);
     if (max_rounds) {
         const bool host = io->memory == LWB_MEM_HOST;
         cudaStream_t sm = ctx->stream;
-        const float *d_coeffs = io->coeffs;
-        char *d_pcm = (char *)io->pcm;
-        if (vq) d_coeffs = nullptr;
-        if (host) {
-            if (o_hi > o_lo && (rc = ensure(ctx, ctx->pcm, (size_t)(o_hi - o_lo) * esz))) return rc;
-            if (!vq) {
-                if ((rc = ensure(ctx, ctx->coeffs, (size_t)(c_hi - c_lo) * 4))) return rc;
-                d_coeffs = (const float *)ctx->coeffs.p - c_lo;       // the copies themselves go chunk by chunk, below
-            }
-            if (need_dense && (rc = ensure(ctx, ctx->dense, (size_t)(c_hi - c_lo) * 4))) return rc;
-            d_pcm = (char *)ctx->pcm.p - o_lo * esz;
-            if ((rc = order_copies_behind_compute(ctx))) return rc;
-        }
+        BatchArenas ar;
+        if ((rc = ar.open(ctx, io, ext, maxc, true))) return rc;
+        const float *d_coeffs = ar.coeffs;
+        char *d_pcm = ar.pcm;
         // host memory: chunks of chains
-        const size_t n_chunks = host ? host_chunks((size_t)(c_hi - c_lo) * 4, n_chains) : 1;
-        const uint8_t *d_kinds = nullptr;
-        const uint32_t *d_ys = nullptr;
-        if (residue && (rc = stage_floor_arrays(ctx, io, r_lo, r_hi, (unsigned)uniform_c, sm, &d_kinds, &d_ys))) return rc;
-        VqView vqv;
-        if ((rc = stage_vq_arrays(ctx, io, r_lo, r_hi, sm, &vqv))) return rc;
+        const size_t n_chunks = host ? host_chunks((size_t)(ext.c_hi - ext.c_lo) * 4, n_chains) : 1;
         // descriptors of every round: [LongRun...][ChainDesc...][DevPacket (prologue of the long segments)...][mode bytes]
         // A round with few fused-kernel runs leaves most of the SMs x 8 warps idle and lasts as long as its
         // longest run: such rounds cut their runs (each cut costs one extra IMDCT, the primer packet whose
@@ -309,7 +244,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         constexpr uint32_t kMinCutRun = 6, kMinCutShort = 16;       // packets per piece (a cut costs one more transform)
         struct Chunk {
             size_t i0, i1, p0, np_;                      // chains, prologue packets
-            uint64_t kc_lo, kc_hi, ko_lo, ko_hi;         // coefficient / pcm element ranges
+            BatchExtent ext;
             std::vector<uint32_t> round_cut, round_cut_s;
             std::vector<MixRound> rounds;
         };
@@ -325,8 +260,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
             Chunk &ck = chunks[k];
             ck.i0 = n_chains * k / n_chunks;
             ck.i1 = n_chains * (k + 1) / n_chunks;
-            ck.kc_lo = ck.ko_lo = ~0ull;
-            ck.kc_hi = ck.ko_hi = 0;
+            ck.ext.scan = false;
             std::vector<size_t> round_long(max_rounds, 0), round_short(max_rounds, 0);
             for (size_t i = ck.i0; i < ck.i1; i++) {
                 const unsigned C = chains[i].stream->setup->channels;
@@ -334,11 +268,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                     if (segs[walks[i].seg0 + q].kind == SEG_LONG) round_long[round_of(i, q)] += C;
                     if (segs[walks[i].seg0 + q].kind == SEG_SHORT) round_short[round_of(i, q)] += C;
                 }
-                if (!walks[i].n_seg) continue;
-                ck.kc_lo = std::min(ck.kc_lo, chains[i].coeff_offset);
-                ck.kc_hi = std::max(ck.kc_hi, walks[i].coeff_end);
-                ck.ko_lo = std::min(ck.ko_lo, chains[i].out_offset);
-                ck.ko_hi = std::max(ck.ko_hi, chains[i].out_offset + (uint64_t)(C - 1) * chains[i].out_stride + chains[i].n_samples);
+                if ((rc = ck.ext.add(ctx, io, &chains[i], results[i].done, results[i].coeff_end, results[i].n_samples))) return rc;
             }
             ck.round_cut.assign(max_rounds, 1);
             ck.round_cut_s.assign(max_rounds, 1);
@@ -361,8 +291,8 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                 }
         }
         // a prepared batch (device memory, spectrum entry) owns its descriptors so that later executions replay them
-        const bool capture = plan && !host;
-        DevBuf &dbuf = capture ? plan->mix : ctx->cdesc;
+        const bool cap = plan && !host;
+        DevBuf &dbuf = cap ? plan->mix : ctx->cdesc;
         const size_t off_sr = n_runs * sizeof(LongRun), off_cd = off_sr + n_sruns * sizeof(ShortRun), off_pro = off_cd + n_cd * sizeof(ChainDesc);
         const size_t off_rc = off_pro + n_pro * sizeof(DevPacket);
         // burst groups: every length class of every chunk is padded to a multiple of eight runs
@@ -394,8 +324,8 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         std::memcpy(hb + off_by, bytes.data(), boff);
         const float *d_spec = nullptr;
         if (residue) {
-            if ((rc = ensure(ctx, ctx->spec, (size_t)(c_hi - c_lo) * 4))) return rc;
-            d_spec = (const float *)ctx->spec.p - c_lo;          // same element offsets as the coefficient arena
+            if ((rc = ensure(ctx, ctx->spec, (size_t)(ext.c_hi - ext.c_lo) * 4))) return rc;
+            d_spec = (const float *)ctx->spec.p - ext.c_lo;      // same element offsets as the coefficient arena
         }
         size_t wr = 0, ws = 0, wc = 0, wp = 0;
         std::vector<LongRun> tmp_lr;
@@ -589,57 +519,31 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         CU(ctx, cudaMemcpyAsync(db, hb, total, cudaMemcpyHostToDevice, sm));
         CU(ctx, cudaEventRecord(st->ev, sm));
         st->pending = true;
-        MixLaunch ml;
-        ml.db = db; ml.off_sr = off_sr; ml.off_cd = off_cd; ml.off_by = off_by; ml.off_rc = off_rc; ml.off_sg = off_sg; ml.pack = pack; ml.spack = spack; ml.w_short = w_short; ml.mpack = nullptr; ml.mid_kb = 0; ml.ls = ls_long;
-        ml.i16 = i16; ml.residue = false; ml.out_format = io->out_format; ml.warps = maxc * wpc; ml.smem = smem;
-        ml.n1max = n1max; ml.wpc = wpc; ml.np = np; ml.coeffs = residue ? d_spec : d_coeffs; ml.dense = nullptr; ml.kinds = nullptr; ml.ys = nullptr;
-        ml.pcm = d_pcm;
+        // (residue entry: the front stages run first, the chain kernel sees a spectrum)
+        const MixLaunch ml{db, d_pcm, io->out_format, i16, pack, ls_long, w_short, spack, nullptr, 0, off_sr, off_cd, off_by, off_rc, off_sg,
+                           false, chain_shape(maxc, n1max, false), residue ? d_spec : d_coeffs};
         FrontStages fs;                         // (residue entry: every packet of the batch, chunk by chunk)
         fs.pk = (const DevPacket *)(db + off_pro);
         fs.n = n_pro;
         fs.C = maxc;
         fs.smem_old = prologue_smem(maxc, kLongBs);
         fs.n2max = n1max_all >> 1;
-        fs.c_lo = c_lo;
-        fs.r_lo = r_lo;
-        fs.r_hi = r_hi;
-        fs.dense = need_dense;
+        fs.c_lo = ext.c_lo;
+        fs.r_lo = ext.r_lo;
+        fs.r_hi = ext.r_hi;
+        fs.dense = ext.need_dense;
         if (fs.n) fs.fast = front_stages_fast(ctx, io, fs, h_pro);
         for (size_t k = 0; k < n_chunks; k++) {
             Chunk &ck = chunks[k];
-            if (ck.kc_hi <= ck.kc_lo) continue;
-            if (host) {
-                if (!vq)
-                    CU(ctx, cudaMemcpyAsync((float *)ctx->coeffs.p + (ck.kc_lo - c_lo), io->coeffs + ck.kc_lo, (size_t)(ck.kc_hi - ck.kc_lo) * 4,
-                                            cudaMemcpyHostToDevice, ctx->copy_in));
-                if (need_dense)
-                    CU(ctx, cudaMemcpyAsync((float *)ctx->dense.p + (ck.kc_lo - c_lo), io->dense_floor + ck.kc_lo,
-                                            (size_t)(ck.kc_hi - ck.kc_lo) * 4, cudaMemcpyHostToDevice, ctx->copy_in));
-                CU(ctx, cudaEventRecord(ctx->ev_in[k], ctx->copy_in));
-                CU(ctx, cudaStreamWaitEvent(sm, ctx->ev_in[k], 0));
-            }
-            if (ck.np_ && (rc = front_stages_launch(ctx, io, fs, ck.p0, ck.np_, d_kinds, d_ys, vqv))) return rc;
-            if ((rc = mixed_launch_rounds(ctx, ml, ck.rounds))) return rc;
-            if (host && ck.ko_hi > ck.ko_lo) {
-                CU(ctx, cudaEventRecord(ctx->ev_done[k], sm));
-                CU(ctx, cudaStreamWaitEvent(ctx->copy_out, ctx->ev_done[k], 0));
-                if ((rc = copy_pcm_to_host(ctx, io, chains, ck.i0, ck.i1, ctx->pcm.p, o_lo, ctx->copy_out))) return rc;
-            }
+            if (ck.ext.empty()) continue;
+            if ((rc = ar.upload(k, ck.ext)) || (ck.np_ && (rc = front_stages_launch(ctx, io, fs, ck.p0, ck.np_, ar.fl))) ||
+                (rc = mixed_launch_rounds(ctx, ml, ck.rounds)) || (rc = ar.download(k, chains, ck.i0, ck.i1, ck.ext)))
+                return rc;
         }
-        if (capture) {
-            plan->captured = true;
-            plan->gen = gen_at_entry;
-            plan->front = fs;
-            plan->mix_launch = ml;
-            plan->mix_rounds = std::move(chunks[0].rounds);
-        }
-        if (host) {
-            CU(ctx, cudaStreamSynchronize(ctx->copy_out));
-            CU(ctx, cudaStreamSynchronize(sm));
-        }
+        if (cap) capture(plan, gen_at_entry, fs, ml, std::move(chunks[0].rounds));
+        if ((rc = ar.finish())) return rc;
     }
-    for (size_t i = 0; i < n_chains; i++)
-        if (walks[i].touched) set_stream_state(chains[i].stream, walks[i].end_has, walks[i].end_plen);
+    commit_stream_states(chains, results);
     return LWB_OK;
 }
 
