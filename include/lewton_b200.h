@@ -299,7 +299,11 @@ typedef struct lwb_batch_io {
 /* All chains must use setups with the same channel count per chain's own stream; chains may
  * mix setups.  Returns LWB_OK when the batch ran (per-chain status holds format errors), or a
  * CUDA / argument error.  With LWB_MEM_HOST the call returns after the PCM has landed in `pcm`;
- * with LWB_MEM_DEVICE it returns after the launches are enqueued on lwb_ctx_cuda_stream(). */
+ * with LWB_MEM_DEVICE it returns after the launches are enqueued on lwb_ctx_cuda_stream().  Such a batch's host-memory
+ * floor / VQ arrays (floor_memory == LWB_MEM_HOST) are uploaded by copies queued on that stream, which read them when
+ * the stream reaches them, as cudaMemcpyAsync reads pinned memory: keep them unchanged until the batch's work has run
+ * (lwb_ctx_synchronize, or an event recorded on the stream after the call).  The chain array and the mode and flag
+ * arrays are read before the call returns. */
 int lwb_decode_chains(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io);
 
 /* Prepared batches.  A decode server submits the same batch shape step after step (same streams,

@@ -415,32 +415,8 @@ class Batch:
         """vq: LWB_ENTRY_VQ arrays (runs, run_offsets, entries, entry_offsets): numpy arrays or device pointers."""
         self.ctx, self.chains = ctx, list(chains)
         self._keep = (coeffs, pcm, floor_kind, floor1_y, dense_floor, vq)
-        self._arr = arr = (cabi.Chain * len(self.chains))()
-        for i, c in enumerate(self.chains):
-            arr[i].stream = c.pwr._h
-            arr[i].n_packets = len(c.modes)
-            arr[i].mode_numbers = _ptr(c.modes, cabi.u8p)
-            if c.prev is not None:
-                arr[i].prev_window_flags = _ptr(c.prev, cabi.u8p)
-            if c.next is not None:
-                arr[i].next_window_flags = _ptr(c.next, cabi.u8p)
-            arr[i].coeff_offset, arr[i].packet_index = c.coeff_offset, c.packet_index
-            arr[i].out_offset, arr[i].out_stride = c.out_offset, c.out_stride
-
-        def addr(x):
-            if x is None:
-                return None
-            if isinstance(x, np.ndarray):
-                return x.ctypes.data
-            return int(x)
-
-        self._io = io = cabi.BatchIo()
-        io.entry, io.memory, io.out_format = entry, memory, out_format
-        io.coeffs, io.pcm, io.dense_floor = addr(coeffs), addr(pcm), addr(dense_floor)
-        io.floor_kind, io.floor1_y = addr(floor_kind), addr(floor1_y)
-        io.floor_memory = floor_memory
-        if vq is not None:
-            io.vq_runs, io.vq_run_offsets, io.vq_entries, io.vq_entry_offsets = (addr(x) for x in vq)
+        self._arr, self._io = _marshal(self.chains, entry, memory, coeffs, pcm, out_format, floor_kind, floor1_y,
+                                       dense_floor, floor_memory, vq)
         self._n = len(self.chains)
         self._plan = C.c_void_p()
         ctx.check(cabi.lib().lwb_plan_create(ctx._h, self._arr, self._n, C.byref(self._io), C.byref(self._plan)))
@@ -466,19 +442,52 @@ class Batch:
             pass
 
     def collect(self):
-        for i, c in enumerate(self.chains):
-            c.n_samples, c.packets_done, c.status = self._arr[i].n_samples, self._arr[i].packets_done, self._arr[i].status
-        return self.chains
+        return _collect(self.chains, self._arr)
+
+
+def _marshal(chains, entry, memory, coeffs, pcm, out_format, floor_kind, floor1_y, dense_floor, floor_memory, vq):
+    """The lwb_chain array and lwb_batch_io of a batch (they point into the ChainSpecs' arrays and the arenas)."""
+    arr = (cabi.Chain * len(chains))()
+    for i, c in enumerate(chains):
+        arr[i].stream = c.pwr._h
+        arr[i].n_packets = len(c.modes)
+        arr[i].mode_numbers = _ptr(c.modes, cabi.u8p)
+        if c.prev is not None:
+            arr[i].prev_window_flags = _ptr(c.prev, cabi.u8p)
+        if c.next is not None:
+            arr[i].next_window_flags = _ptr(c.next, cabi.u8p)
+        arr[i].coeff_offset, arr[i].packet_index = c.coeff_offset, c.packet_index
+        arr[i].out_offset, arr[i].out_stride = c.out_offset, c.out_stride
+
+    def addr(x):
+        if x is None:
+            return None
+        if isinstance(x, np.ndarray):
+            return x.ctypes.data
+        return int(x)
+
+    io = cabi.BatchIo()
+    io.entry, io.memory, io.out_format = entry, memory, out_format
+    io.coeffs, io.pcm, io.dense_floor = addr(coeffs), addr(pcm), addr(dense_floor)
+    io.floor_kind, io.floor1_y = addr(floor_kind), addr(floor1_y)
+    io.floor_memory = floor_memory
+    if vq is not None:
+        io.vq_runs, io.vq_run_offsets, io.vq_entries, io.vq_entry_offsets = (addr(x) for x in vq)
+    return arr, io
+
+
+def _collect(chains, arr):
+    for i, c in enumerate(chains):
+        c.n_samples, c.packets_done, c.status = arr[i].n_samples, arr[i].packets_done, arr[i].status
+    return chains
 
 
 def decode_chains(ctx, chains, entry, memory, coeffs, pcm, out_format, floor_kind=None, floor1_y=None,
                   dense_floor=None, floor_memory=cabi.MEM_HOST, vq=None):
     """lwb_decode_chains.  coeffs/pcm/dense_floor: numpy arrays (MEM_HOST) or integer device
     pointers (MEM_DEVICE); floor_kind/floor1_y: numpy arrays (floor_memory MEM_HOST) or integer
-    device pointers (MEM_DEVICE)."""
-    b = Batch(ctx, chains, entry, memory, coeffs, pcm, out_format, floor_kind, floor1_y, dense_floor, floor_memory, vq)
-    try:
-        b.run()
-        return b.collect()
-    finally:
-        b.close()
+    device pointers (MEM_DEVICE).  A MEM_DEVICE batch returns once its work is queued on ctx.cuda_stream."""
+    chains = list(chains)
+    arr, io = _marshal(chains, entry, memory, coeffs, pcm, out_format, floor_kind, floor1_y, dense_floor, floor_memory, vq)
+    ctx.check(cabi.lib().lwb_decode_chains(ctx._h, arr, len(chains), C.byref(io)))
+    return _collect(chains, arr)

@@ -127,6 +127,7 @@ struct LongRuns {
     LongRun *h = nullptr, *d = nullptr;
     size_t n = 0;
     int par = 0;                       // which half of the double-buffered descriptors (ctx->runs_buf) they take
+    bool own = false;                  // in a prepared batch's own buffer rather than ctx->runs_buf[par]
 };
 
 // Builds the runs of chains [0, n_chains) for n_chunks launches; each launch should see >= target_runs runs.  `own`:
@@ -166,6 +167,7 @@ static int long_build_runs(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chain
     lr->par = ctx->runs_par;
     ctx->runs_par ^= 1;
     DevBuf &rb = own ? *own : ctx->runs_buf[lr->par];
+    lr->own = own != nullptr;
     if ((rc = ensure(ctx, rb, cap_runs * sizeof(LongRun)))) return rc;
     lr->d = (LongRun *)rb.p;
     LongRun *h_runs = (LongRun *)lr->st->h, *w = h_runs;
@@ -222,8 +224,12 @@ static int long_build_runs(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chain
 }
 
 // One descriptor upload for all the runs, on `ds`, behind the kernel that last read this half of the double buffer.
+// A prepared batch's own buffer has no halves: every launch queued so far may be one of its replays, which read that
+// buffer and record no ev_kdone, so a re-plan's upload waits for all of them.
 static int long_upload_runs(lwb_ctx *ctx, const LongRuns &lr, cudaStream_t ds)
 {
+    int rc;
+    if (lr.own && ds != ctx->stream && (rc = order_copies_behind_compute(ctx))) return rc;
     CU(ctx, cudaStreamWaitEvent(ds, ctx->ev_kdone[lr.par], 0));
     CU(ctx, cudaMemcpyAsync(lr.d, lr.h, lr.n * sizeof(LongRun), cudaMemcpyHostToDevice, ds));
     CU(ctx, cudaEventRecord(ctx->ev_desc[lr.par], ds));
