@@ -120,6 +120,9 @@ SYMBOLS = {
     "lwb_decode_spectrum": (C.c_int, [vp, C.c_uint8, C.c_int, C.c_int, vp, C.c_int, vp, C.c_size_t,
                                       C.POINTER(C.c_size_t)]),
     "lwb_decode_chains": (C.c_int, [vp, C.POINTER(Chain), C.c_size_t, C.POINTER(BatchIo)]),
+    "lwb_submit_chains": (C.c_int, [vp, C.POINTER(Chain), C.c_size_t, C.POINTER(BatchIo), C.POINTER(C.c_uint64)]),
+    "lwb_ticket_query": (C.c_int, [vp, C.c_uint64, C.POINTER(C.c_int)]),
+    "lwb_ticket_wait": (C.c_int, [vp, C.c_uint64]),
     "lwb_plan_create": (C.c_int, [vp, C.POINTER(Chain), C.c_size_t, C.POINTER(BatchIo), C.POINTER(vp)]),
     "lwb_plan_execute": (C.c_int, [vp]),
     "lwb_plan_destroy": (None, [vp]),

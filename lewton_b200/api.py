@@ -83,6 +83,20 @@ class Context:
     def d2h(self, arr, src):
         self.check(cabi.lib().lwb_memcpy_d2h(self._h, _ptr(arr), src, arr.nbytes))
 
+    def host_alloc(self, shape, dtype):
+        """A page-locked numpy array (lwb_host_alloc), as host-memory submit_chains needs; freed with its last view."""
+        return np.asarray(_PinnedBlock(shape, dtype))
+
+    def submit_chains(self, chains, entry, memory, coeffs, pcm, out_format, floor_kind=None, floor1_y=None,
+                      dense_floor=None, floor_memory=cabi.MEM_HOST, vq=None):
+        """lwb_submit_chains: decode_chains' arguments; queues the batch and returns its Ticket at once.  Host arrays of a
+        MEM_HOST batch must be page-locked (host_alloc), and stay unchanged, and `pcm` unread, until the ticket is done."""
+        chains = list(chains)
+        arr, io = _marshal(chains, entry, memory, coeffs, pcm, out_format, floor_kind, floor1_y, dense_floor, floor_memory, vq)
+        t = C.c_uint64()
+        self.check(cabi.lib().lwb_submit_chains(self._h, arr, len(chains), C.byref(io), C.byref(t)))
+        return Ticket(self, t.value, chains, arr, (coeffs, pcm, floor_kind, floor1_y, dense_floor, vq, io))
+
     def close(self):
         if self._h:
             # readers (frontend.OggStreamReader) own streams and setups of their own: they go first
@@ -442,6 +456,51 @@ class Batch:
             pass
 
     def collect(self):
+        return _collect(self.chains, self._arr)
+
+
+class _PinnedBlock:
+    """Owner of one lwb_host_alloc block, exposed to numpy as an array; freed when the last array over it goes."""
+
+    def __init__(self, shape, dtype):
+        dtype = np.dtype(dtype)
+        shape = (int(shape),) if np.isscalar(shape) else tuple(int(s) for s in shape)
+        nbytes = int(np.prod(shape, dtype=np.int64)) * dtype.itemsize
+        self._p = cabi.lib().lwb_host_alloc(nbytes)
+        if not self._p:
+            raise AudioReadError(cabi.ERR_CUDA, f"lwb_host_alloc({nbytes}) failed")
+        self.__array_interface__ = {"data": (self._p, False), "shape": shape, "typestr": dtype.str, "descr": dtype.descr,
+                                    "version": 3}
+
+    def __del__(self):
+        if getattr(self, "_p", None):
+            cabi.lib().lwb_host_free(self._p)
+            self._p = None
+
+
+class Ticket:
+    """A batch queued by Context.submit_chains.  It keeps every array of the batch alive until it is done; wait() copies
+    the chain results into the ChainSpecs (the library wrote them before submit_chains returned)."""
+
+    def __init__(self, ctx, ticket, chains, arr, keep):
+        self.ctx, self.id, self.chains = ctx, ticket, chains
+        self._arr, self._keep = arr, keep
+
+    def done(self):
+        """lwb_ticket_query: whether every copy and kernel of the batch has finished.  Never blocks."""
+        if self._keep is not None:
+            d = C.c_int()
+            self.ctx.check(cabi.lib().lwb_ticket_query(self.ctx._h, self.id, C.byref(d)))
+            if not d.value:
+                return False
+            self._keep = None
+        return True
+
+    def wait(self):
+        """lwb_ticket_wait; returns the chains with their results."""
+        if self._keep is not None:
+            self.ctx.check(cabi.lib().lwb_ticket_wait(self.ctx._h, self.id))
+            self._keep = None
         return _collect(self.chains, self._arr)
 
 

@@ -19,6 +19,16 @@ struct Staging {
     bool pending = false;
 };
 
+// Device copies of one batch's host arrays (coefficients, dense floors, floor and VQ arrays) and its PCM before the
+// D2H.  Host-memory batches take the context's kHostSets sets in turn, so that the uploads of one batch overlap the
+// kernels and copies of the one before it: a set is reused only behind `done`, which is recorded after the last kernel
+// and the last D2H of the batch that used it last.
+struct ArenaSet {
+    DevBuf coeffs, dense, pcm, kinds, ys, vqoff, vqrec;
+    cudaEvent_t done = nullptr;
+};
+constexpr int kHostSets = 2;
+
 // CachedBlocksizeDerived (header_cached.rs:27-31) on the device, shared by all setups of a context with the same tables
 struct CachedTables {
     DevTables dt;                  // device pointers; dt.pack = the fused kernels' twiddle pack (bs 11: k_long, bs 8: k_short)
@@ -48,9 +58,18 @@ struct lwb_ctx {
     std::vector<PcmCopy> pcm_copies;
     std::deque<CachedTables> tables;       // (deque: setups hold copies of dt, growth never moves an entry)
     // grow-only device arenas
-    DevBuf coeffs, dense, pcm, spec, segtab, vqoff, vqrec, magic, x, desc, kinds, ys, chains, ticket, cdesc, cbytes;
+    DevBuf spec, segtab, magic, x, desc, chains, ticket, cdesc, cbytes;
+    ArenaSet host_sets[kHostSets]; // host-memory batches, in turn
+    int host_next = 0;
+    ArenaSet ordered;              // in compute-stream order: device-memory batches' host floor arrays, the debug taps
     Staging stage[3];              // ring: a batch's descriptors are written while the previous copies may still run
     int stage_next = 0;
+    // completion tickets (lwb_submit_chains, and every host-memory batch): ticket t's event is ticket_events[t -
+    // tickets_done - 1]; they are retired in order
+    uint64_t tickets_issued = 0, tickets_done = 0;
+    std::deque<cudaEvent_t> ticket_events;
+    std::vector<cudaEvent_t> spare_events;
+    bool pinned_only = false;      // set while a host-memory lwb_submit_chains queues its batch
     // pinned staging for descriptors (four-kernel path)
     void *h_desc = nullptr;
     size_t h_desc_cap = 0;
@@ -173,11 +192,14 @@ static inline void count_launch(lwb_ctx *ctx, int kernel_id)
         if (e__ != cudaSuccess) return fail((ctx), LWB_ERR_CUDA, #call, e__); \
     } while (0)
 
-static int ensure(lwb_ctx *ctx, DevBuf &b, size_t bytes)
+// Grows b to at least `bytes`.  The old buffer is freed once the last work that may use it has finished: the work
+// before `in_use` when the arena belongs to a host set, else everything queued on the compute stream.
+static int ensure(lwb_ctx *ctx, DevBuf &b, size_t bytes, cudaEvent_t in_use = nullptr)
 {
     if (bytes <= b.cap) return LWB_OK;
     if (b.p) {
-        CU(ctx, cudaStreamSynchronize(ctx->stream));
+        if (in_use) CU(ctx, cudaEventSynchronize(in_use));
+        else CU(ctx, cudaStreamSynchronize(ctx->stream));
         CU(ctx, cudaFree(b.p));
         b.p = nullptr;
         b.cap = 0;
@@ -205,7 +227,65 @@ static int create_pipeline_objects(lwb_ctx *ctx)
         CU(ctx, cudaEventCreateWithFlags(&ctx->ev_desc[k], cudaEventDisableTiming));
         CU(ctx, cudaEventCreateWithFlags(&ctx->ev_kdone[k], cudaEventDisableTiming));
     }
+    for (ArenaSet &s : ctx->host_sets) CU(ctx, cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
     return ensure(ctx, ctx->ticket, kTicketPool * sizeof(unsigned int));
+}
+
+// Retires tickets in order up to `upto`: the completed ones, or (block) all of them, waiting for each.
+static int retire_tickets(lwb_ctx *ctx, uint64_t upto, bool block);
+
+// Orders copy_out behind everything queued so far on copy_in and the compute stream, then records `set`'s `done`
+// there (if given): what a set's next user waits for.
+static int order_copy_out_behind_all(lwb_ctx *ctx, ArenaSet *set)
+{
+    CU(ctx, cudaEventRecord(ctx->ev_done[64], ctx->copy_in));
+    CU(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_done[64], 0));
+    CU(ctx, cudaEventRecord(ctx->ev_done[64], ctx->stream));
+    CU(ctx, cudaStreamWaitEvent(ctx->copy_out, ctx->ev_done[64], 0));
+    if (set) CU(ctx, cudaEventRecord(set->done, ctx->copy_out));
+    return LWB_OK;
+}
+
+// Queues the completion ticket of the batch just queued: an event on copy_out behind the batch's last kernel and its
+// last D2H.  `set`: the host set the batch used, whose `done` is recorded at the same point.  The ticket counts as
+// issued only once its event is recorded.  Tickets that have completed are retired first (without waiting), so that
+// a caller who never queries them does not accumulate events.
+static int issue_ticket(lwb_ctx *ctx, ArenaSet *set)
+{
+    int rc;
+    if ((rc = retire_tickets(ctx, ctx->tickets_issued, false)) || (rc = order_copy_out_behind_all(ctx, set))) return rc;
+    cudaEvent_t ev;
+    if (ctx->spare_events.empty()) {
+        CU(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    } else {
+        ev = ctx->spare_events.back();
+        ctx->spare_events.pop_back();
+    }
+    const cudaError_t e = cudaEventRecord(ev, ctx->copy_out);
+    if (e != cudaSuccess) {
+        ctx->spare_events.push_back(ev);
+        return fail(ctx, LWB_ERR_CUDA, "cudaEventRecord(ticket)", e);
+    }
+    ctx->ticket_events.push_back(ev);
+    ctx->tickets_issued++;
+    return LWB_OK;
+}
+
+static int retire_tickets(lwb_ctx *ctx, uint64_t upto, bool block)
+{
+    while (ctx->tickets_done < upto) {
+        cudaEvent_t ev = ctx->ticket_events.front();
+        const cudaError_t e = block ? cudaEventSynchronize(ev) : cudaEventQuery(ev);
+        if (e == cudaErrorNotReady) {
+            cudaGetLastError();
+            return LWB_OK;
+        }
+        if (e != cudaSuccess) return fail(ctx, LWB_ERR_CUDA, "ticket", e);
+        ctx->ticket_events.pop_front();
+        ctx->spare_events.push_back(ev);
+        ctx->tickets_done++;
+    }
+    return LWB_OK;
 }
 
 // The ticket of one k_long launch; the pool is zeroed on the compute stream once per wrap.

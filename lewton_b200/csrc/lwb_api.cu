@@ -88,15 +88,34 @@ extern "C" int lwb_ctx_create(int device, lwb_ctx **out)
     return LWB_OK;
 }
 
+// The compute stream and both copy streams: a host-memory batch's last D2H may still run after its kernels.
+static cudaError_t sync_all_streams(lwb_ctx *ctx)
+{
+    cudaError_t e = cudaStreamSynchronize(ctx->stream);
+    for (cudaStream_t s : {ctx->copy_in, ctx->copy_out}) {
+        const cudaError_t e2 = s ? cudaStreamSynchronize(s) : cudaSuccess;
+        if (e == cudaSuccess) e = e2;
+    }
+    return e;
+}
+
 extern "C" void lwb_ctx_destroy(lwb_ctx *ctx)
 {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
-    cudaStreamSynchronize(ctx->stream);
-    for (DevBuf *b : {&ctx->coeffs, &ctx->dense, &ctx->pcm, &ctx->spec, &ctx->segtab, &ctx->vqoff, &ctx->vqrec, &ctx->magic, &ctx->x, &ctx->desc,
-                      &ctx->kinds, &ctx->ys, &ctx->chains, &ctx->ticket, &ctx->runs_buf[0], &ctx->runs_buf[1],
-                      &ctx->cdesc, &ctx->cbytes})
+    sync_all_streams(ctx);
+    for (DevBuf *b : {&ctx->spec, &ctx->segtab, &ctx->magic, &ctx->x, &ctx->desc, &ctx->chains, &ctx->ticket, &ctx->runs_buf[0],
+                      &ctx->runs_buf[1], &ctx->cdesc, &ctx->cbytes})
         if (b->p) cudaFree(b->p);
+    auto free_set = [](ArenaSet &s) {
+        for (DevBuf *b : {&s.coeffs, &s.dense, &s.pcm, &s.kinds, &s.ys, &s.vqoff, &s.vqrec})
+            if (b->p) cudaFree(b->p);
+        if (s.done) cudaEventDestroy(s.done);
+    };
+    for (ArenaSet &s : ctx->host_sets) free_set(s);
+    free_set(ctx->ordered);
+    for (cudaEvent_t e : ctx->ticket_events) cudaEventDestroy(e);
+    for (cudaEvent_t e : ctx->spare_events) cudaEventDestroy(e);
     for (CachedTables &ct : ctx->tables)
         for (void *p : ct.allocs) cudaFree(p);
     if (ctx->h_desc) cudaFreeHost(ctx->h_desc);
@@ -120,8 +139,8 @@ extern "C" int lwb_ctx_synchronize(lwb_ctx *ctx)
 {
     if (!ctx) return LWB_ERR_INVALID;
     CU(ctx, cudaSetDevice(ctx->device));
-    CU(ctx, cudaStreamSynchronize(ctx->stream));
-    return LWB_OK;
+    CU(ctx, sync_all_streams(ctx));
+    return retire_tickets(ctx, ctx->tickets_issued, true);
 }
 
 extern "C" const char *lwb_last_error(const lwb_ctx *ctx) { return ctx ? ctx->err.c_str() : "no context"; }
@@ -451,7 +470,7 @@ extern "C" void lwb_stream_destroy(lwb_stream *s)
 {
     if (!s) return;
     cudaSetDevice(s->ctx->device);
-    cudaStreamSynchronize(s->ctx->stream);
+    sync_all_streams(s->ctx);
     cudaFree(s->d_state);
     delete s;
 }
@@ -539,7 +558,8 @@ static size_t first_batch_path()
     return std::strcmp(fg, "1") == 0 ? kNumBatchPaths : kNumBatchPaths - 1;
 }
 
-static int decode_chains_impl(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, lwb_plan *prepared)
+// Checks, plans and queues one batch; a host-memory batch that queues work issues its ticket (BatchArenas::finish).
+static int queue_batch(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, lwb_plan *prepared)
 {
     if (!ctx || (!chains && n_chains) || !io) return LWB_ERR_INVALID;
     if (io->entry != LWB_ENTRY_SPECTRUM && io->entry != LWB_ENTRY_RESIDUE && io->entry != LWB_ENTRY_VQ) return fail(ctx, LWB_ERR_INVALID, "bad entry");
@@ -600,9 +620,66 @@ static int decode_chains_impl(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, 
     return LWB_OK;
 }
 
+// One batch.  ticket == nullptr: the synchronous entry points, which return once a host-memory batch's PCM has landed
+// (they wait for the ticket it issued).  Else lwb_submit_chains: *ticket identifies the batch's work, whatever its
+// memory space, and nothing is waited for.
+static int decode_chains_impl(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, lwb_plan *prepared,
+                              uint64_t *ticket = nullptr)
+{
+    if (!ctx) return LWB_ERR_INVALID;
+    const uint64_t issued = ctx->tickets_issued;
+    int rc = queue_batch(ctx, chains, n_chains, io, prepared);
+    if (rc) return rc;
+    if (!ticket) return ctx->tickets_issued != issued ? retire_tickets(ctx, ctx->tickets_issued, true) : LWB_OK;
+    if (ctx->tickets_issued == issued) {        // a device-memory or empty batch (which may not have set the device)
+        CU(ctx, cudaSetDevice(ctx->device));
+        if ((rc = issue_ticket(ctx, nullptr))) return rc;
+    }
+    *ticket = ctx->tickets_issued;
+    return LWB_OK;
+}
+
 extern "C" int lwb_decode_chains(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io)
 {
     return decode_chains_impl(ctx, chains, n_chains, io, nullptr);
+}
+
+// ---------------------------------------------------------------------------------------------
+// asynchronous batches
+// ---------------------------------------------------------------------------------------------
+extern "C" int lwb_submit_chains(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, uint64_t *ticket)
+{
+    if (!ctx || !ticket || (!chains && n_chains) || !io) return LWB_ERR_INVALID;
+    // a submit that fails leaves every chain result as it was (stream states are committed only by a batch that queued)
+    struct Result { uint32_t n_samples, packets_done; int32_t status; };
+    std::vector<Result> saved(n_chains);
+    for (size_t i = 0; i < n_chains; i++) saved[i] = Result{chains[i].n_samples, chains[i].packets_done, chains[i].status};
+    ctx->pinned_only = io->memory == LWB_MEM_HOST;
+    const int rc = decode_chains_impl(ctx, chains, n_chains, io, nullptr, ticket);
+    ctx->pinned_only = false;
+    if (rc)
+        for (size_t i = 0; i < n_chains; i++) {
+            chains[i].n_samples = saved[i].n_samples;
+            chains[i].packets_done = saved[i].packets_done;
+            chains[i].status = saved[i].status;
+        }
+    return rc;
+}
+
+extern "C" int lwb_ticket_query(lwb_ctx *ctx, uint64_t ticket, int *done)
+{
+    if (!ctx || !done || ticket == 0 || ticket > ctx->tickets_issued) return LWB_ERR_INVALID;
+    CU(ctx, cudaSetDevice(ctx->device));
+    const int rc = retire_tickets(ctx, ticket, false);
+    *done = ticket <= ctx->tickets_done;
+    return rc;
+}
+
+extern "C" int lwb_ticket_wait(lwb_ctx *ctx, uint64_t ticket)
+{
+    if (!ctx || ticket == 0 || ticket > ctx->tickets_issued) return LWB_ERR_INVALID;
+    CU(ctx, cudaSetDevice(ctx->device));
+    return retire_tickets(ctx, ticket, true);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -727,9 +804,9 @@ extern "C" int lwb_debug_packet_taps(lwb_stream *s, const lwb_packet *pkt, float
         need_y |= pkt->floor_kind[c] == LWB_FLOOR_ONE;
     }
     if ((need_dense && !pkt->dense_floor) || (need_y && !pkt->floor1_y)) return LWB_ERR_INVALID;
-    if ((rc = ensure(ctx, ctx->coeffs, C * n2 * 4)) || (rc = ensure(ctx, ctx->spec, C * n2 * 4)) ||
-        (rc = ensure(ctx, ctx->x, C * g.n * 4)) || (rc = ensure(ctx, ctx->kinds, C)) ||
-        (rc = ensure(ctx, ctx->ys, C * LWB_MAX_POSTS * 4)) || (rc = ensure(ctx, ctx->dense, C * n2 * 4)) ||
+    if ((rc = ensure(ctx, ctx->ordered.coeffs, C * n2 * 4)) || (rc = ensure(ctx, ctx->spec, C * n2 * 4)) ||
+        (rc = ensure(ctx, ctx->x, C * g.n * 4)) || (rc = ensure(ctx, ctx->ordered.kinds, C)) ||
+        (rc = ensure(ctx, ctx->ordered.ys, C * LWB_MAX_POSTS * 4)) || (rc = ensure(ctx, ctx->ordered.dense, C * n2 * 4)) ||
         (rc = ensure(ctx, ctx->desc, sizeof(DevPacket))) || (rc = ensure_pinned(ctx, sizeof(DevPacket))))
         return rc;
     CU(ctx, cudaStreamSynchronize(ctx->stream));
@@ -745,10 +822,10 @@ extern "C" int lwb_debug_packet_taps(lwb_stream *s, const lwb_packet *pkt, float
     d->channels = (uint8_t)C;
     cudaStream_t st = ctx->stream;
     CU(ctx, cudaMemcpyAsync(ctx->desc.p, d, sizeof(*d), cudaMemcpyHostToDevice, st));
-    CU(ctx, cudaMemcpyAsync(ctx->coeffs.p, pkt->residue, C * n2 * 4, cudaMemcpyHostToDevice, st));
-    CU(ctx, cudaMemcpyAsync(ctx->kinds.p, pkt->floor_kind, C, cudaMemcpyHostToDevice, st));
-    if (need_y) CU(ctx, cudaMemcpyAsync(ctx->ys.p, pkt->floor1_y, C * LWB_MAX_POSTS * 4, cudaMemcpyHostToDevice, st));
-    if (need_dense) CU(ctx, cudaMemcpyAsync(ctx->dense.p, pkt->dense_floor, C * n2 * 4, cudaMemcpyHostToDevice, st));
+    CU(ctx, cudaMemcpyAsync(ctx->ordered.coeffs.p, pkt->residue, C * n2 * 4, cudaMemcpyHostToDevice, st));
+    CU(ctx, cudaMemcpyAsync(ctx->ordered.kinds.p, pkt->floor_kind, C, cudaMemcpyHostToDevice, st));
+    if (need_y) CU(ctx, cudaMemcpyAsync(ctx->ordered.ys.p, pkt->floor1_y, C * LWB_MAX_POSTS * 4, cudaMemcpyHostToDevice, st));
+    if (need_dense) CU(ctx, cudaMemcpyAsync(ctx->ordered.dense.p, pkt->dense_floor, C * n2 * 4, cudaMemcpyHostToDevice, st));
     const DevPacket *dp = (const DevPacket *)ctx->desc.p;
     if (post_inverse) {
         // audio.rs:1004 tap: coupling only -- run the prologue with every floor "dense = 1.0"?  No:
@@ -761,8 +838,8 @@ extern "C" int lwb_debug_packet_taps(lwb_stream *s, const lwb_packet *pkt, float
         CU(ctx, cudaMalloc(&tmp_kinds, C));
         CU(ctx, cudaMemcpyAsync(tmp_dense, ones.data(), C * n2 * 4, cudaMemcpyHostToDevice, st));
         CU(ctx, cudaMemcpyAsync(tmp_kinds, kd.data(), C, cudaMemcpyHostToDevice, st));
-        rc = launch(ctx, LWB_KERNEL_PROLOGUE, k_prologue, dim3(1), dim3(kPrologueThreads), prologue_smem(su->channels, su->bs1), dp, (const float *)ctx->coeffs.p,
-                    (const float *)tmp_dense, (const uint8_t *)tmp_kinds, (const uint32_t *)ctx->ys.p,
+        rc = launch(ctx, LWB_KERNEL_PROLOGUE, k_prologue, dim3(1), dim3(kPrologueThreads), prologue_smem(su->channels, su->bs1), dp, (const float *)ctx->ordered.coeffs.p,
+                    (const float *)tmp_dense, (const uint8_t *)tmp_kinds, (const uint32_t *)ctx->ordered.ys.p,
                     (float *)ctx->spec.p);
         if (!rc) {
             cudaError_t e = cudaMemcpyAsync(post_inverse, ctx->spec.p, C * n2 * 4, cudaMemcpyDeviceToHost, st);
@@ -773,8 +850,8 @@ extern "C" int lwb_debug_packet_taps(lwb_stream *s, const lwb_packet *pkt, float
         cudaFree(tmp_kinds);
         if (rc) return rc;
     }
-    if ((rc = launch(ctx, LWB_KERNEL_PROLOGUE, k_prologue, dim3(1), dim3(kPrologueThreads), prologue_smem(su->channels, su->bs1), dp, (const float *)ctx->coeffs.p,
-                     (const float *)ctx->dense.p, (const uint8_t *)ctx->kinds.p, (const uint32_t *)ctx->ys.p,
+    if ((rc = launch(ctx, LWB_KERNEL_PROLOGUE, k_prologue, dim3(1), dim3(kPrologueThreads), prologue_smem(su->channels, su->bs1), dp, (const float *)ctx->ordered.coeffs.p,
+                     (const float *)ctx->ordered.dense.p, (const uint8_t *)ctx->ordered.kinds.p, (const uint32_t *)ctx->ordered.ys.p,
                      (float *)ctx->spec.p)))
         return rc;
     if (pre_mdct) CU(ctx, cudaMemcpyAsync(pre_mdct, ctx->spec.p, C * n2 * 4, cudaMemcpyDeviceToHost, st));

@@ -203,15 +203,16 @@ static int scan_floor_kinds(lwb_ctx *ctx, const lwb_batch_io *io, uint64_t row_l
 }
 
 // The floor and VQ arrays (LWB_ENTRY_VQ) of packet rows [r_lo, r_hi) of a batch with C channels as the device sees
-// them, biased so that ABSOLUTE rows and offsets address them.  Host arrays get room in ctx->kinds / ys / vqoff / vqrec,
-// which upload_floor_rows fills; device arrays are used in place.
+// them, biased so that ABSOLUTE rows and offsets address them.  Host arrays get room in the kinds / ys / vqoff / vqrec
+// arenas of `set` (grown behind `in_use`, see ensure()), which upload_floor_rows fills; device arrays are used in place.
 struct FloorViews {
     const uint8_t *kinds = nullptr;
     const uint32_t *ys = nullptr;
     VqView vq;
 };
 
-static int floor_views(lwb_ctx *ctx, const lwb_batch_io *io, uint64_t r_lo, uint64_t r_hi, unsigned C, FloorViews *v)
+static int floor_views(lwb_ctx *ctx, const lwb_batch_io *io, ArenaSet &set, cudaEvent_t in_use, uint64_t r_lo, uint64_t r_hi,
+                       unsigned C, FloorViews *v)
 {
     *v = FloorViews();
     if (io->entry == LWB_ENTRY_SPECTRUM) return LWB_OK;
@@ -225,24 +226,24 @@ static int floor_views(lwb_ctx *ctx, const lwb_batch_io *io, uint64_t r_lo, uint
     if (r_hi <= r_lo) return LWB_OK;
     int rc;
     const size_t rows = (size_t)(r_hi - r_lo) * C;
-    if ((rc = ensure(ctx, ctx->kinds, rows))) return rc;
-    v->kinds = (const uint8_t *)ctx->kinds.p - r_lo * C;
+    if ((rc = ensure(ctx, set.kinds, rows, in_use))) return rc;
+    v->kinds = (const uint8_t *)set.kinds.p - r_lo * C;
     if (io->floor1_y) {
-        if ((rc = ensure(ctx, ctx->ys, rows * LWB_MAX_POSTS * sizeof(uint32_t)))) return rc;
-        v->ys = (const uint32_t *)ctx->ys.p - r_lo * C * LWB_MAX_POSTS;
+        if ((rc = ensure(ctx, set.ys, rows * LWB_MAX_POSTS * sizeof(uint32_t), in_use))) return rc;
+        v->ys = (const uint32_t *)set.ys.p - r_lo * C * LWB_MAX_POSTS;
     }
     if (!vq) return LWB_OK;
     const uint64_t o_lo = io->vq_run_offsets[r_lo], o_hi = io->vq_run_offsets[r_hi];
     const uint64_t e_lo = io->vq_entry_offsets[r_lo], e_hi = io->vq_entry_offsets[r_hi];
     if (o_hi < o_lo || e_hi < e_lo) return fail(ctx, LWB_ERR_INVALID, "vq offsets must be non-decreasing");
     const size_t b_off = ((size_t)(r_hi - r_lo) + 1) * sizeof(uint64_t), b_run = std::max<size_t>((size_t)(o_hi - o_lo), 1) * sizeof(lwb_vq_run);
-    if ((rc = ensure(ctx, ctx->vqoff, 2 * b_off)) ||
-        (rc = ensure(ctx, ctx->vqrec, b_run + std::max<size_t>((size_t)(e_hi - e_lo), 1) * sizeof(uint16_t) + 16)))
+    if ((rc = ensure(ctx, set.vqoff, 2 * b_off, in_use)) ||
+        (rc = ensure(ctx, set.vqrec, b_run + std::max<size_t>((size_t)(e_hi - e_lo), 1) * sizeof(uint16_t) + 16, in_use)))
         return rc;
-    v->vq.run_off = (const uint64_t *)ctx->vqoff.p - r_lo;
-    v->vq.ent_off = (const uint64_t *)((char *)ctx->vqoff.p + b_off) - r_lo;
-    v->vq.runs = (const lwb_vq_run *)ctx->vqrec.p - o_lo;
-    v->vq.entries = (const uint16_t *)((char *)ctx->vqrec.p + b_run) - e_lo;
+    v->vq.run_off = (const uint64_t *)set.vqoff.p - r_lo;
+    v->vq.ent_off = (const uint64_t *)((char *)set.vqoff.p + b_off) - r_lo;
+    v->vq.runs = (const lwb_vq_run *)set.vqrec.p - o_lo;
+    v->vq.entries = (const uint16_t *)((char *)set.vqrec.p + b_run) - e_lo;
     return LWB_OK;
 }
 
@@ -298,9 +299,50 @@ struct BatchExtent {
     bool empty() const { return c_hi <= c_lo; }
 };
 
+// Whether host bytes [lo, hi) * esz of `base` begin and end in page-locked memory (the runtime tells; pageable memory
+// is "unregistered").
+static bool page_locked(const void *base, uint64_t lo, uint64_t hi, size_t esz)
+{
+    if (hi <= lo) return true;
+    for (const char *p : {(const char *)base + lo * esz, (const char *)base + hi * esz - 1}) {
+        cudaPointerAttributes a;
+        if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+            cudaGetLastError();
+            return false;
+        }
+        if (a.type != cudaMemoryTypeHost) return false;
+    }
+    return true;
+}
+
+// A host-memory submit copies straight from and to the caller's arrays, after the call has returned: every range of
+// them the batch touches must be page-locked.
+static int check_page_locked(lwb_ctx *ctx, const lwb_batch_io *io, const BatchExtent &ext, unsigned C)
+{
+    const char *bad = nullptr;
+    if (io->entry != LWB_ENTRY_VQ && !page_locked(io->coeffs, ext.c_lo, ext.c_hi, sizeof(float))) bad = "coeffs";
+    else if (ext.need_dense && !page_locked(io->dense_floor, ext.c_lo, ext.c_hi, sizeof(float))) bad = "dense_floor";
+    else if (!page_locked(io->pcm, ext.o_lo, ext.o_hi, elem_size(io->out_format))) bad = "pcm";
+    else if (io->entry != LWB_ENTRY_SPECTRUM && io->floor_memory == LWB_MEM_HOST && ext.r_hi > ext.r_lo) {
+        const uint64_t a = ext.r_lo * C, b = ext.r_hi * C;
+        if (!page_locked(io->floor_kind, a, b, 1)) bad = "floor_kind";
+        else if (io->floor1_y && !page_locked(io->floor1_y, a * LWB_MAX_POSTS, b * LWB_MAX_POSTS, sizeof(uint32_t))) bad = "floor1_y";
+        else if (io->entry == LWB_ENTRY_VQ) {
+            if (!page_locked(io->vq_run_offsets, ext.r_lo, ext.r_hi + 1, sizeof(uint64_t))) bad = "vq_run_offsets";
+            else if (!page_locked(io->vq_entry_offsets, ext.r_lo, ext.r_hi + 1, sizeof(uint64_t))) bad = "vq_entry_offsets";
+            else if (!page_locked(io->vq_runs, io->vq_run_offsets[ext.r_lo], io->vq_run_offsets[ext.r_hi], sizeof(lwb_vq_run))) bad = "vq_runs";
+            else if (!page_locked(io->vq_entries, io->vq_entry_offsets[ext.r_lo], io->vq_entry_offsets[ext.r_hi], sizeof(uint16_t))) bad = "vq_entries";
+        }
+    }
+    if (!bad) return LWB_OK;
+    return fail(ctx, LWB_ERR_INVALID, (std::string("host-memory submit: ") + bad +
+                                       " is not page-locked (lwb_host_alloc, cudaHostAlloc or cudaHostRegister)").c_str());
+}
+
 // The arenas of a batch as its kernels address them: coefficients, dense floors and PCM by absolute element offset,
-// floor and VQ arrays by absolute packet row (FloorViews).  A host-memory batch is staged in the context's arenas,
-// chunk by chunk: upload(k) brings chunk k's inputs, download(k) takes its PCM home behind its kernels.  With the copy
+// floor and VQ arrays by absolute packet row (FloorViews).  A host-memory batch is staged in the next of the context's
+// host sets, chunk by chunk: upload(k) brings chunk k's inputs, download(k) takes its PCM home behind its kernels.  Its
+// uploads wait on the GPU for the batch that used the set before (ArenaSet::done) and nothing else.  With the copy
 // streams (copy_in / copy_out, ordered by ev_in[k] / ev_done[k]) the copies of one chunk overlap the kernels of
 // another; otherwise everything runs on the compute stream.  A device-memory batch uses the caller's arenas in place.
 struct BatchArenas {
@@ -309,6 +351,7 @@ struct BatchArenas {
     FloorViews fl;
     lwb_ctx *ctx = nullptr;
     const lwb_batch_io *io = nullptr;
+    ArenaSet *set = nullptr;
     bool host = false;
     unsigned C = 0;
     uint64_t c_lo = 0, o_lo = 0;
@@ -326,21 +369,28 @@ struct BatchArenas {
         up = host && copy_streams ? ctx->copy_in : ctx->stream;
         down = host && copy_streams ? ctx->copy_out : ctx->stream;
         int rc;
+        cudaEvent_t in_use = nullptr;
         if (host) {
+            if (ctx->pinned_only && (rc = check_page_locked(ctx, io, ext, C))) return rc;
+            set = &ctx->host_sets[ctx->host_next];
+            ctx->host_next = (ctx->host_next + 1) % kHostSets;
+            in_use = set->done;
             const size_t esz = elem_size(io->out_format), bytes = (size_t)(ext.c_hi - ext.c_lo) * sizeof(float);
-            if (ext.o_hi > ext.o_lo && (rc = ensure(ctx, ctx->pcm, (size_t)(ext.o_hi - ext.o_lo) * esz))) return rc;
-            if (!vq && (rc = ensure(ctx, ctx->coeffs, bytes))) return rc;
-            if (ext.need_dense && (rc = ensure(ctx, ctx->dense, bytes))) return rc;
-            coeffs = vq ? nullptr : (const float *)ctx->coeffs.p - c_lo;
-            dense = ext.need_dense ? (const float *)ctx->dense.p - c_lo : nullptr;
-            pcm = (char *)ctx->pcm.p - o_lo * esz;
+            if (ext.o_hi > ext.o_lo && (rc = ensure(ctx, set->pcm, (size_t)(ext.o_hi - ext.o_lo) * esz, in_use))) return rc;
+            if (!vq && (rc = ensure(ctx, set->coeffs, bytes, in_use))) return rc;
+            if (ext.need_dense && (rc = ensure(ctx, set->dense, bytes, in_use))) return rc;
+            coeffs = vq ? nullptr : (const float *)set->coeffs.p - c_lo;
+            dense = ext.need_dense ? (const float *)set->dense.p - c_lo : nullptr;
+            pcm = (char *)set->pcm.p - o_lo * esz;
         } else {
+            set = &ctx->ordered;
             coeffs = vq ? nullptr : io->coeffs;
             dense = io->dense_floor;
             pcm = (char *)io->pcm;
         }
-        if ((rc = floor_views(ctx, io, ext.r_lo, ext.r_hi, C, &fl))) return rc;
-        return up != ctx->stream ? order_copies_behind_compute(ctx) : LWB_OK;
+        if ((rc = floor_views(ctx, io, *set, in_use, ext.r_lo, ext.r_hi, C, &fl))) return rc;
+        if (host) CU(ctx, cudaStreamWaitEvent(up, set->done, 0));
+        return LWB_OK;
     }
     int upload(size_t k, const BatchExtent &ck)
     {
@@ -364,15 +414,28 @@ struct BatchArenas {
             CU(ctx, cudaEventRecord(ctx->ev_done[k], ctx->stream));
             CU(ctx, cudaStreamWaitEvent(down, ctx->ev_done[k], 0));
         }
-        return copy_pcm_to_host(ctx, io, chains, i0, i1, ctx->pcm.p, o_lo, down);
+        return copy_pcm_to_host(ctx, io, chains, i0, i1, set->pcm.p, o_lo, down);
     }
+    // The batch is queued: a host-memory batch records its ticket, which also releases its set to the next user.
     int finish()
     {
-        if (!host) return LWB_OK;
-        if (down != ctx->stream) CU(ctx, cudaStreamSynchronize(down));
-        CU(ctx, cudaStreamSynchronize(ctx->stream));
-        return LWB_OK;
+        finished = true;
+        return host ? issue_ticket(ctx, set) : LWB_OK;
     }
+    // A host-memory batch that failed after open() still releases its set behind whatever it had queued, so that the
+    // set's next user waits for copies and kernels that may still read it.  (Failures here are dropped: the batch
+    // already reports the first one.)
+    ~BatchArenas()
+    {
+        if (!host || !set || finished) return;
+        cudaEventRecord(ctx->ev_done[64], ctx->copy_in);
+        cudaStreamWaitEvent(ctx->stream, ctx->ev_done[64], 0);
+        cudaEventRecord(ctx->ev_done[64], ctx->stream);
+        cudaStreamWaitEvent(ctx->copy_out, ctx->ev_done[64], 0);
+        cudaEventRecord(set->done, ctx->copy_out);
+        cudaGetLastError();
+    }
+    bool finished = false;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -401,42 +464,41 @@ static uint64_t write_front_packets(const lwb_chain *c, uint32_t p0, uint32_t n,
     return coeff;
 }
 
-// The arenas the front stages read and write, biased by fs.c_lo: the caller's residues and dense floors (device
-// memory) or their staged copies in ctx->coeffs / ctx->dense (host memory), and ctx->spec.
+// The arenas the front stages read and write, biased by fs.c_lo (== the c_lo of the batch's arenas ar): residues and
+// dense floors as ar holds them (the caller's in device memory, their staged copies in host memory), and ctx->spec.
 struct FrontArenas { const float *res, *dense; float *spec; };
-static FrontArenas front_arenas(lwb_ctx *ctx, const lwb_batch_io *io, const FrontStages &fs)
+static FrontArenas front_arenas(lwb_ctx *ctx, const BatchArenas &ar, const FrontStages &fs)
 {
-    const bool host = io->memory == LWB_MEM_HOST;
-    FrontArenas a;
-    a.res = io->entry == LWB_ENTRY_VQ ? nullptr : host ? (const float *)ctx->coeffs.p - fs.c_lo : io->coeffs;
-    a.dense = !fs.dense ? nullptr : host ? (const float *)ctx->dense.p - fs.c_lo : io->dense_floor;
-    a.spec = (float *)ctx->spec.p - fs.c_lo;
-    return a;
+    return FrontArenas{ar.coeffs, fs.dense ? ar.dense : nullptr, (float *)ctx->spec.p - fs.c_lo};
 }
 
 // Whether the two-kernel form takes fs's packets (host copy h_pk of its list).
-static bool front_stages_fast(lwb_ctx *ctx, const lwb_batch_io *io, const FrontStages &fs, const DevPacket *h_pk)
+static bool front_stages_fast(lwb_ctx *ctx, const BatchArenas &ar, const FrontStages &fs, const DevPacket *h_pk)
 {
-    const FrontArenas a = front_arenas(ctx, io, fs);
+    const FrontArenas a = front_arenas(ctx, ar, fs);
     return prologue_is_fast(h_pk, fs.n, fs.C, a.res, a.dense, a.spec);
 }
 
-// Packets [k0, k0 + n) of fs on floor / VQ views the caller has staged.
-static int front_stages_launch(lwb_ctx *ctx, const lwb_batch_io *io, const FrontStages &fs, size_t k0, size_t n, const FloorViews &fl)
+// Packets [k0, k0 + n) of fs on the floor / VQ views of ar, which the caller has staged.
+static int front_stages_launch(lwb_ctx *ctx, const BatchArenas &ar, const FrontStages &fs, size_t k0, size_t n)
 {
-    const FrontArenas a = front_arenas(ctx, io, fs);
-    return launch_prologue(ctx, fs.pk + k0, n, fs.C, fs.fast, fs.smem_old, fs.n2max, a.res, a.dense, fl.kinds, fl.ys, a.spec, fl.vq);
+    const FrontArenas a = front_arenas(ctx, ar, fs);
+    return launch_prologue(ctx, fs.pk + k0, n, fs.C, fs.fast, fs.smem_old, fs.n2max, a.res, a.dense, ar.fl.kinds, ar.fl.ys, a.spec, ar.fl.vq);
 }
 
-// Stages the floor and VQ arrays of fs's packet rows on the compute stream (host arrays are uploaded, device arrays
-// read in place) and launches the front stages over every packet of fs.
+// A device-memory batch's front stages alone: stages the floor and VQ arrays of fs's packet rows on the compute stream
+// (host arrays are uploaded, device arrays read in place) and launches the front stages over every packet of fs.
 static int front_stages_run(lwb_ctx *ctx, const lwb_batch_io *io, const FrontStages &fs)
 {
-    FloorViews fl;
+    BatchExtent ext;
+    ext.c_lo = fs.c_lo;
+    ext.r_lo = fs.r_lo;
+    ext.r_hi = fs.r_hi;
+    ext.need_dense = fs.dense;
+    BatchArenas ar;
     int rc;
-    if ((rc = floor_views(ctx, io, fs.r_lo, fs.r_hi, fs.C, &fl))) return rc;
-    if ((rc = upload_floor_rows(ctx, io, fs.r_lo, fs.r_hi, fs.C, fl, ctx->stream))) return rc;
-    return front_stages_launch(ctx, io, fs, 0, fs.n, fl);
+    if ((rc = ar.open(ctx, io, ext, fs.C, false)) || (rc = ar.upload(0, ext))) return rc;
+    return front_stages_launch(ctx, ar, fs, 0, fs.n);
 }
 
 // Generic path: rounds of packets bounded by the IMDCT scratch.  Its descriptors address a host-memory batch's

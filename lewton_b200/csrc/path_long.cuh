@@ -266,9 +266,11 @@ static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_
     const bool cap = plan && !host;
     BatchArenas ar;
     LongRuns lr;
+    // (host memory: the runs go up on copy_in, ahead of the chunks' inputs; behind copy_out's PCM copies the kernels
+    // would wait for the D2H of the batch before)
     if ((rc = ar.open(ctx, io, ext, 0, true)) ||
         (rc = long_build_runs(ctx, chains, n_chains, n_chunks, ar.coeffs, ar.pcm, i16 ? 2 : 4, cap ? &plan->runs : nullptr, &lr)) ||
-        (rc = long_upload_runs(ctx, lr, ctx->copy_out)))
+        (rc = long_upload_runs(ctx, lr, host ? ctx->copy_in : ctx->copy_out)))
         return rc;
     for (size_t k = 0; k < lr.chunks.size(); k++) {
         const LongRuns::Chunk &ck = lr.chunks[k];
@@ -309,6 +311,8 @@ static int try_long_residue(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, co
     for (size_t i = 0; i < n_chains; i++) n_pk += chains[i].n_packets;
     cudaStream_t sm = ctx->stream;
     if ((rc = ensure(ctx, ctx->spec, (size_t)(ext.c_hi - ext.c_lo) * 4))) return rc;
+    BatchArenas ar;
+    if ((rc = ar.open(ctx, io, ext, C, true))) return rc;
     FrontStages fs;
     fs.n = n_pk;
     fs.C = C;
@@ -335,14 +339,12 @@ static int try_long_residue(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, co
             di += chains[i].n_packets;
         }
         fs.pk = (const DevPacket *)db.p;
-        fs.fast = front_stages_fast(ctx, io, fs, hp);
+        fs.fast = front_stages_fast(ctx, ar, fs, hp);
         CU(ctx, cudaMemcpyAsync(db.p, hp, n_pk * sizeof(DevPacket), cudaMemcpyHostToDevice, sm));
         CU(ctx, cudaEventRecord(st->ev, sm));
         st->pending = true;
     }
     if (plan) plan->front = fs;
-    BatchArenas ar;
-    if ((rc = ar.open(ctx, io, ext, C, true))) return rc;
     const uint64_t gen = ctx->state_gen;
     const bool cap = plan && !host;
     // Host memory: slices of chains flow through three streams -- copy_in brings a slice's inputs (dense residues, or
@@ -362,7 +364,7 @@ static int try_long_residue(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, co
         size_t npk = 0;
         for (size_t i = i0; i < i1; i++) npk += chains[i].n_packets;
         LongRuns lr;
-        if ((rc = ar.upload(sl, se)) || (rc = front_stages_launch(ctx, io, fs, pk0, npk, ar.fl)) ||
+        if ((rc = ar.upload(sl, se)) || (rc = front_stages_launch(ctx, ar, fs, pk0, npk)) ||
             (rc = long_build_runs(ctx, chains + i0, i1 - i0, 1, spec, ar.pcm, i16 ? 2 : 4, cap ? &plan->runs : nullptr, &lr)) ||
             (rc = long_upload_runs(ctx, lr, host ? ctx->copy_in : ctx->copy_out)) ||
             (rc = launch_long(ctx, lr.d, (uint32_t)(lr.n / kLongNB), pack, i16)) || (rc = ar.download(sl, chains, i0, i1, se)))

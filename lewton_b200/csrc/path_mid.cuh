@@ -99,11 +99,11 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
             write_front_packets(&chains[i], 0, chains[i].n_packets, chains[i].coeff_offset, hp + di);
             di += chains[i].n_packets;
         }
-        fs.fast = front_stages_fast(ctx, io, fs, hp);
+        fs.fast = front_stages_fast(ctx, ar, fs, hp);
         CU(ctx, cudaMemcpyAsync(d_pro, hp, n_pk * sizeof(DevPacket), cudaMemcpyHostToDevice, sm));
         CU(ctx, cudaEventRecord(stp->ev, sm));
         stp->pending = true;
-        if ((rc = front_stages_launch(ctx, io, fs, 0, fs.n, ar.fl))) return rc;
+        if ((rc = front_stages_launch(ctx, ar, fs, 0, fs.n))) return rc;
         d_coeffs = (const float *)ctx->spec.p - ext.c_lo;       // k_mid reads the spectrum
     }
     // runs, then groups of two runs of equal length (an odd one gets a dummy partner), longest first, dealt balanced

@@ -532,11 +532,11 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         fs.r_lo = ext.r_lo;
         fs.r_hi = ext.r_hi;
         fs.dense = ext.need_dense;
-        if (fs.n) fs.fast = front_stages_fast(ctx, io, fs, h_pro);
+        if (fs.n) fs.fast = front_stages_fast(ctx, ar, fs, h_pro);
         for (size_t k = 0; k < n_chunks; k++) {
             Chunk &ck = chunks[k];
             if (ck.ext.empty()) continue;
-            if ((rc = ar.upload(k, ck.ext)) || (ck.np_ && (rc = front_stages_launch(ctx, io, fs, ck.p0, ck.np_, ar.fl))) ||
+            if ((rc = ar.upload(k, ck.ext)) || (ck.np_ && (rc = front_stages_launch(ctx, ar, fs, ck.p0, ck.np_))) ||
                 (rc = mixed_launch_rounds(ctx, ml, ck.rounds)) || (rc = ar.download(k, chains, ck.i0, ck.i1, ck.ext)))
                 return rc;
         }
