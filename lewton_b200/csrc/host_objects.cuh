@@ -64,6 +64,7 @@ struct lwb_ctx {
     ArenaSet ordered;              // in compute-stream order: device-memory batches' host floor arrays, the debug taps
     Staging stage[3];              // ring: a batch's descriptors are written while the previous copies may still run
     int stage_next = 0;
+    std::vector<void *> stage_old; // staging outgrown, freed with the context (cudaFreeHost waits for the whole device)
     // completion tickets (lwb_submit_chains, and every host-memory batch): ticket t's event is ticket_events[t -
     // tickets_done - 1]; they are retired in order
     uint64_t tickets_issued = 0, tickets_done = 0;
@@ -208,6 +209,38 @@ static int ensure(lwb_ctx *ctx, DevBuf &b, size_t bytes, cudaEvent_t in_use = nu
     CU(ctx, cudaMalloc(&b.p, want));
     b.cap = want;
     ctx->state_gen++;              // captured plans may hold pointers into the arena that just moved
+    return LWB_OK;
+}
+
+// The next slot of the staging ring, at least `bytes` large, once the copy that last read it has finished.  A slot that
+// grows keeps its old buffer until the context is destroyed: freeing it would wait for the whole device, other
+// contexts' queued work included.  (Each growth at least doubles the slot, so the old buffers hold less than it does.)
+static int acquire_staging(lwb_ctx *ctx, size_t bytes, Staging **out)
+{
+    Staging &st = ctx->stage[ctx->stage_next];
+    ctx->stage_next = (ctx->stage_next + 1) % 3;
+    if (!st.ev) CU(ctx, cudaEventCreateWithFlags(&st.ev, cudaEventDisableTiming));
+    if (st.pending) {
+        CU(ctx, cudaEventSynchronize(st.ev));      // waits for the descriptor copy only, not for kernels
+        st.pending = false;
+    }
+    if (st.cap < bytes) {
+        if (st.h) ctx->stage_old.push_back(st.h);
+        st.h = nullptr;
+        st.cap = 0;
+        CU(ctx, cudaHostAlloc(&st.h, bytes * 2 + 4096, cudaHostAllocDefault));
+        st.cap = bytes * 2 + 4096;
+    }
+    *out = &st;
+    return LWB_OK;
+}
+
+// H2D of `bytes` from `src`, inside staging slot `st`, to `dst` on stream `s`; the slot is taken again behind this copy.
+static int upload_staging(lwb_ctx *ctx, Staging *st, const void *src, void *dst, size_t bytes, cudaStream_t s)
+{
+    CU(ctx, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s));
+    CU(ctx, cudaEventRecord(st->ev, s));
+    st->pending = true;
     return LWB_OK;
 }
 

@@ -119,6 +119,7 @@ extern "C" void lwb_ctx_destroy(lwb_ctx *ctx)
     for (CachedTables &ct : ctx->tables)
         for (void *p : ct.allocs) cudaFree(p);
     if (ctx->h_desc) cudaFreeHost(ctx->h_desc);
+    for (void *h : ctx->stage_old) cudaFreeHost(h);
     for (Staging &st : ctx->stage) {
         if (st.h) cudaFreeHost(st.h);
         if (st.ev) cudaEventDestroy(st.ev);
@@ -546,7 +547,7 @@ extern "C" int lwb_decoded_sample_count(const lwb_setup *su, uint8_t mode, int p
 
 // The batch paths in the order they are tried; what none of them takes goes to the four-kernel path (run_generic).
 using BatchPath = int (*)(lwb_ctx *, lwb_chain *, size_t, const lwb_batch_io *, bool *, lwb_plan *);
-static const BatchPath kBatchPaths[] = {try_long, try_long_residue, try_mid, try_mixed, try_chain};
+static const BatchPath kBatchPaths[] = {try_long, try_mid, try_mixed, try_chain};
 constexpr size_t kNumBatchPaths = sizeof(kBatchPaths) / sizeof(kBatchPaths[0]);
 
 // Index of the first batch path to try.  LWB_FORCE_GENERIC is a test switch that sends batches to the reference

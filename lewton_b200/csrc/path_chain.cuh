@@ -180,10 +180,9 @@ static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         DevBuf &dbuf = cap ? plan->mix : ctx->cdesc;
         const size_t used_desc = n_launch * sizeof(ChainDesc);
         if ((rc = ensure(ctx, dbuf, used_desc + boff + 16))) return rc;
-        CU(ctx, cudaMemcpyAsync(dbuf.p, hd, used_desc, cudaMemcpyHostToDevice, sm));
-        CU(ctx, cudaMemcpyAsync((char *)dbuf.p + used_desc, hb, boff + 16, cudaMemcpyHostToDevice, sm));
-        CU(ctx, cudaEventRecord(st->ev, sm));
-        st->pending = true;
+        if ((rc = upload_staging(ctx, st, hd, dbuf.p, used_desc, sm)) ||
+            (rc = upload_staging(ctx, st, hb, (char *)dbuf.p + used_desc, boff + 16, sm)))
+            return rc;
         const MixLaunch ml{(char *)dbuf.p, ar.pcm, io->out_format, false, nullptr, 0, nullptr, nullptr, nullptr, 0, 0, 0, used_desc, 0, 0,
                            residue, chain_shape(maxc, n1max, residue), ar.coeffs, ar.dense, ar.fl.kinds, ar.fl.ys};
         std::vector<MixRound> rounds(1, MixRound{0, 0, 0, 0, 0, n_launch});

@@ -479,6 +479,41 @@ static bool front_stages_fast(lwb_ctx *ctx, const BatchArenas &ar, const FrontSt
     return prologue_is_fast(h_pk, fs.n, fs.C, a.res, a.dense, a.spec);
 }
 
+// The front stages of n packets with C channels, none larger than n1max, over the arenas of `ext`; the packet list
+// (pk, fast) is the caller's.
+static FrontStages front_stages_of(const BatchExtent &ext, unsigned C, int n1max, size_t n)
+{
+    FrontStages fs;
+    fs.n = n;
+    fs.C = C;
+    fs.smem_old = prologue_smem((int)C, __builtin_ctz((unsigned)n1max));
+    fs.n2max = n1max >> 1;
+    fs.c_lo = ext.c_lo;
+    fs.r_lo = ext.r_lo;
+    fs.r_hi = ext.r_hi;
+    fs.dense = ext.need_dense;
+    return fs;
+}
+
+// Writes the packet list of every packet of chains [0, n_chains) into ring staging and uploads it, on the compute
+// stream, to `off` bytes into `db`: fs->pk and fs->fast.
+static int stage_front_packets(lwb_ctx *ctx, const BatchArenas &ar, const lwb_chain *chains, size_t n_chains, DevBuf &db, size_t off,
+                               FrontStages *fs)
+{
+    const size_t bytes = fs->n * sizeof(DevPacket);
+    Staging *st;
+    int rc;
+    if ((rc = acquire_staging(ctx, bytes, &st)) || (rc = ensure(ctx, db, off + bytes))) return rc;
+    DevPacket *hp = (DevPacket *)st->h, *w = hp;
+    for (size_t i = 0; i < n_chains; i++) {
+        write_front_packets(&chains[i], 0, chains[i].n_packets, chains[i].coeff_offset, w);
+        w += chains[i].n_packets;
+    }
+    fs->pk = (const DevPacket *)((char *)db.p + off);
+    fs->fast = front_stages_fast(ctx, ar, *fs, hp);
+    return upload_staging(ctx, st, hp, (char *)db.p + off, bytes, ctx->stream);
+}
+
 // Packets [k0, k0 + n) of fs on the floor / VQ views of ar, which the caller has staged.
 static int front_stages_launch(lwb_ctx *ctx, const BatchArenas &ar, const FrontStages &fs, size_t k0, size_t n)
 {

@@ -3,7 +3,7 @@
 #pragma once
 
 // ---------------------------------------------------------------------------------------------
-// Fused path (kernel_long.cuh).  Eligible batches: spectrum entry, planar f32 out, every packet a
+// Fused path (kernel_long.cuh).  Eligible batches: any entry, planar f32 / i16 out, every packet a
 // long block of blocksize 2^11 with long neighbours, every stream either empty or holding a
 // 1024-sample right half.  Planned directly from the chain list in O(chains + mode bytes) -- at
 // 0.8 G blocks/s per GPU a per-packet host plan would be the bottleneck.
@@ -14,60 +14,48 @@ struct LongItem {
     bool has_prev;
 };
 
-static int acquire_staging(lwb_ctx *ctx, size_t bytes, Staging **out)
+// Cuts `whole`, the run of one channel (a LongRun or a ShortRun: in, out, state, in_stride, n_packets, has_prev), into
+// `cuts` pieces w[0, cuts), for when there are too few runs to fill the machine.  Every piece after the first
+// re-transforms the packet before its first one as a primer (its right half is all the piece needs), which keeps the
+// pieces independent at the cost of one extra transform per cut.  Packet 0 of the run emits first_emit samples, every
+// later one n2, of esz bytes each.  Only the last piece stores the state.
+template <typename Run>
+static void cut_run(const Run &whole, size_t cuts, size_t first_emit, size_t n2, size_t esz, Run *w)
 {
-    Staging &st = ctx->stage[ctx->stage_next];
-    ctx->stage_next = (ctx->stage_next + 1) % 3;
-    if (!st.ev) CU(ctx, cudaEventCreateWithFlags(&st.ev, cudaEventDisableTiming));
-    if (st.pending) {
-        CU(ctx, cudaEventSynchronize(st.ev));      // waits for the descriptor copy only, not for kernels
-        st.pending = false;
+    const size_t P = whole.n_packets;
+    for (size_t k = 0; k < cuts; k++) {
+        const size_t p0 = P * k / cuts, p1 = P * (k + 1) / cuts;   // this piece emits packets [p0, p1)
+        Run &r = w[k];
+        std::memset(&r, 0, sizeof(r));
+        r.in_stride = whole.in_stride;
+        r.state = whole.state;
+        r.write_state = (k + 1 == cuts);
+        if (k == 0) {
+            r.in = whole.in;
+            r.out = whole.out;
+            r.n_packets = (uint32_t)(p1 - p0);
+            r.has_prev = whole.has_prev;
+        } else {
+            const size_t primer = p0 - 1;
+            r.in = whole.in + primer * whole.in_stride;
+            r.out = (char *)whole.out + (first_emit + primer * n2) * esz;          // behind the samples before packet p0
+            r.n_packets = (uint32_t)(p1 - p0 + 1);
+            r.has_prev = 0;
+        }
     }
-    if (st.cap < bytes) {
-        if (st.h) cudaFreeHost(st.h);
-        st.h = nullptr;
-        st.cap = 0;
-        CU(ctx, cudaHostAlloc(&st.h, bytes * 2 + 4096, cudaHostAllocDefault));
-        st.cap = bytes * 2 + 4096;
-    }
-    *out = &st;
-    return LWB_OK;
 }
 
-// Appends the runs of one chain.  A chain (one channel of one stream) is cut into several runs
-// when there are too few chains to fill the machine; every run after the first re-transforms the
-// packet before its first one as a primer (its right half is all the run needs), which keeps
-// runs independent at the cost of one extra IMDCT per cut.  coeffs / pcm: arenas addressed by absolute element offset.
+// Appends the runs of one chain, each channel cut into `cuts` pieces.  coeffs / pcm: arenas addressed by absolute
+// element offset.
 static void long_runs_of(const LongItem &it, size_t cuts, const float *coeffs, char *pcm, size_t esz, LongRun *&w)
 {
     const lwb_stream *s = it.c->stream;
     const lwb_setup *su = s->setup;
     const unsigned C = su->channels;
-    const size_t P = it.P;
-    for (unsigned ch = 0; ch < C; ch++) {
-        const float *in0 = coeffs + it.c->coeff_offset + (size_t)ch * kLongN2;
-        char *out0 = pcm + (it.c->out_offset + (size_t)ch * it.c->out_stride) * esz;
-        for (size_t k = 0; k < cuts; k++) {
-            const size_t p0 = P * k / cuts, p1 = P * (k + 1) / cuts;   // this run emits packets [p0, p1)
-            LongRun &r = *w++;
-            std::memset(&r, 0, sizeof(r));
-            r.in_stride = (uint32_t)(C * kLongN2);
-            r.state = s->d_state + (size_t)ch * state_stride(su);
-            r.write_state = (k + 1 == cuts);
-            if (k == 0) {
-                r.in = in0;
-                r.n_packets = (uint32_t)(p1 - p0);
-                r.has_prev = it.has_prev;
-                r.out = out0;
-            } else {
-                r.in = in0 + (p0 - 1) * (size_t)r.in_stride;           // primer = packet p0 - 1
-                r.n_packets = (uint32_t)(p1 - p0 + 1);
-                r.has_prev = 0;
-                // samples emitted before packet p0: packets 0..p0-1, minus the first if no state
-                r.out = out0 + (size_t)(p0 - (it.has_prev ? 0 : 1)) * kLongN2 * esz;
-            }
-        }
-    }
+    for (unsigned ch = 0; ch < C; ch++, w += cuts)
+        cut_run(LongRun{coeffs + it.c->coeff_offset + (size_t)ch * kLongN2, pcm + (it.c->out_offset + (size_t)ch * it.c->out_stride) * esz,
+                        s->d_state + (size_t)ch * state_stride(su), (uint32_t)(C * kLongN2), it.P, it.has_prev},
+                cuts, it.has_prev ? kLongN2 : 0, kLongN2, esz, w);
 }
 
 // Every packet a long block of the fast blocksize with long neighbours, every stream empty or
@@ -95,33 +83,36 @@ static bool batch_is_uniform_long(const lwb_chain *chains, size_t n_chains, cons
     return true;
 }
 
-// The result of every chain of a uniform long batch, in closed form: all its packets decode, and each emits 1024
-// samples but the first of an empty stream.
-static void set_long_results(lwb_chain *chains, size_t n_chains)
+// A uniform batch (k_long, k_mid: every packet a full-window block of one size n = 2 * n2) in closed form.  Sets the
+// results of chains [i0, i1) -- all their packets decode, each emits n2 samples but the first of an empty stream --
+// and adds them to `ext`.
+static int uniform_extent(lwb_ctx *ctx, const lwb_batch_io *io, lwb_chain *chains, size_t i0, size_t i1, uint32_t n2, BatchExtent *ext)
 {
-    for (size_t i = 0; i < n_chains; i++) {
+    for (size_t i = i0; i < i1; i++) {
         lwb_chain *c = &chains[i];
         c->status = LWB_OK;
         c->packets_done = c->n_packets;
-        c->n_samples = c->n_packets ? (uint32_t)((c->n_packets - (c->stream->has ? 0 : 1)) * kLongN2) : 0;
+        c->n_samples = c->n_packets ? (c->n_packets - (c->stream->has ? 0u : 1u)) * n2 : 0u;
     }
-}
-
-// Adds chains [i0, i1) of a uniform long batch, their results set, to `ext`.
-static int long_extent(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chain *chains, size_t i0, size_t i1, BatchExtent *ext)
-{
     int rc = LWB_OK;
     for (size_t i = i0; i < i1 && !rc; i++) {
         const lwb_chain *c = &chains[i];
-        rc = ext->add(ctx, io, c, c->n_packets, c->coeff_offset + (uint64_t)c->n_packets * c->stream->setup->channels * kLongN2, c->n_samples);
+        rc = ext->add(ctx, io, c, c->n_packets, c->coeff_offset + (uint64_t)c->n_packets * c->stream->setup->channels * n2, c->n_samples);
     }
     return rc;
 }
 
-// The k_long runs of a batch, or of one slice of a residue batch, in pinned staging: chunk k launches runs
-// [r0, r0 + nr) of chains [i0, i1); chunks without runs are left out.
+// ... and once it is queued, the state it leaves: every stream that decoded a packet holds its last n2-sample right half.
+static void commit_uniform_states(lwb_chain *chains, size_t n_chains, uint32_t n2)
+{
+    for (size_t i = 0; i < n_chains; i++)
+        if (chains[i].n_packets) set_stream_state(chains[i].stream, true, n2);
+}
+
+// The k_long runs of a batch in pinned staging: chunk k (chains [n_chains * k / n_chunks, n_chains * (k + 1) / n_chunks))
+// launches runs [r0, r0 + nr).
 struct LongRuns {
-    struct Chunk { size_t r0, nr, i0, i1; };
+    struct Chunk { size_t r0, nr; };
     std::vector<Chunk> chunks;
     Staging *st = nullptr;
     LongRun *h = nullptr, *d = nullptr;
@@ -189,7 +180,6 @@ static int long_build_runs(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chain
         }
         for (size_t i = i0; i < i1; i++)
             if (items[i].P) long_runs_of(items[i], cuts[i], coeffs, pcm, esz, gen);
-        if (!chunk_runs) continue;
         if (kLongNB == 1) {
             w = gen;
         } else {
@@ -217,7 +207,7 @@ static int long_build_runs(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chain
                 i = j;
             }
         }
-        lr->chunks.push_back(LongRuns::Chunk{(size_t)(w0 - h_runs), (size_t)(w - w0), i0, i1});
+        lr->chunks.push_back(LongRuns::Chunk{(size_t)(w0 - h_runs), (size_t)(w - w0)});
     }
     lr->n = (size_t)(w - h_runs);
     return LWB_OK;
@@ -231,10 +221,8 @@ static int long_upload_runs(lwb_ctx *ctx, const LongRuns &lr, cudaStream_t ds)
     int rc;
     if (lr.own && ds != ctx->stream && (rc = order_copies_behind_compute(ctx))) return rc;
     CU(ctx, cudaStreamWaitEvent(ds, ctx->ev_kdone[lr.par], 0));
-    CU(ctx, cudaMemcpyAsync(lr.d, lr.h, lr.n * sizeof(LongRun), cudaMemcpyHostToDevice, ds));
+    if ((rc = upload_staging(ctx, lr.st, lr.h, lr.d, lr.n * sizeof(LongRun), ds))) return rc;
     CU(ctx, cudaEventRecord(ctx->ev_desc[lr.par], ds));
-    CU(ctx, cudaEventRecord(lr.st->ev, ds));
-    lr.st->pending = true;
     CU(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_desc[lr.par], 0));
     return LWB_OK;
 }
@@ -248,133 +236,75 @@ static int launch_long(lwb_ctx *ctx, const LongRun *runs, uint32_t n_groups, con
     return launched(ctx, LWB_KERNEL_LONG, long_launch(ctx->stream, runs, n_groups, pack, ticket, ctx->sm_count, i16), "long kernel launch");
 }
 
+// The fused long-block path for all three entries.  A residue-entry batch (LWB_ENTRY_RESIDUE or LWB_ENTRY_VQ) runs
+// the front stages (k_floor1_segments + k_prologue_fused, or k_prologue) over each chunk's packets first: they form its
+// spectrum in ctx->spec, which k_long then reads instead of the coefficient arena.  Planned straight from the chain
+// list (no per-packet PlanChain vectors).  A prepared batch keeps the front stages' packet list and, in device memory,
+// the runs, so that a replay has no host work (lwb_plan_execute).  Host memory: chunks of chains flow through three
+// streams -- copy_in brings a chunk's inputs (coefficients, or residues / VQ records and floor rows), the compute
+// stream runs its kernels, copy_out takes its PCM home -- so that H2D, kernels and D2H of consecutive chunks overlap
+// (the link is duplex).  The runs of all chunks are built while the first chunk's inputs copy and go up once, on
+// copy_in behind those inputs: behind copy_out's PCM copies the kernels would wait for the D2H of the batch before.
 static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, bool *handled, lwb_plan *plan)
 {
     *handled = false;
-    const uint64_t gen_at_entry = ctx->state_gen;
-    if (io->entry != LWB_ENTRY_SPECTRUM || !batch_is_uniform_long(chains, n_chains, io)) return LWB_OK;
+    if (!batch_is_uniform_long(chains, n_chains, io)) return LWB_OK;
     *handled = true;
-    set_long_results(chains, n_chains);
     BatchExtent ext;
     int rc;
-    if ((rc = long_extent(ctx, io, chains, 0, n_chains, &ext))) return rc;
+    if ((rc = uniform_extent(ctx, io, chains, 0, n_chains, kLongN2, &ext)) || (rc = ext.finish(ctx, io))) return rc;
     if (ext.empty()) return LWB_OK;
-    const bool i16 = io->out_format == LWB_OUT_I16_PLANAR, host = io->memory == LWB_MEM_HOST;
+    const unsigned C = chains[0].stream->setup->channels;                  // (residue entries: the batch's one count)
+    const bool residue = io->entry != LWB_ENTRY_SPECTRUM, i16 = io->out_format == LWB_OUT_I16_PLANAR, host = io->memory == LWB_MEM_HOST;
     const float *pack = chains[0].stream->setup->host.tab[1].pack;          // one twiddle pack per launch
-    // host memory: chunks of chains
     const size_t n_chunks = host ? host_chunks((size_t)(ext.c_hi - ext.c_lo) * 4, n_chains) : 1;
     const bool cap = plan && !host;
     BatchArenas ar;
+    if ((rc = ar.open(ctx, io, ext, C, true))) return rc;
+    const float *in = ar.coeffs;
+    FrontStages fs;
+    if (residue) {
+        size_t n_pk = 0;
+        for (size_t i = 0; i < n_chains; i++) n_pk += chains[i].n_packets;
+        if ((rc = ensure(ctx, ctx->spec, (size_t)(ext.c_hi - ext.c_lo) * 4))) return rc;
+        fs = front_stages_of(ext, C, kLongN, n_pk);
+        if (plan && plan->pro.p && plan->front.pk == plan->pro.p && plan->front.n == n_pk) {
+            // a prepared batch re-planned (host memory: every execution): the packet list of the previous execution
+            // depends only on the plan's chain and mode arrays
+            fs.pk = plan->front.pk;
+            fs.fast = plan->front.fast;
+        } else if ((rc = stage_front_packets(ctx, ar, chains, n_chains, plan ? plan->pro : ctx->desc, 0, &fs))) {
+            return rc;
+        }
+        if (plan) plan->front = fs;
+        in = (const float *)ctx->spec.p - ext.c_lo;                         // same element offsets as the coefficients
+    }
     LongRuns lr;
-    // (host memory: the runs go up on copy_in, ahead of the chunks' inputs; behind copy_out's PCM copies the kernels
-    // would wait for the D2H of the batch before)
-    if ((rc = ar.open(ctx, io, ext, 0, true)) ||
-        (rc = long_build_runs(ctx, chains, n_chains, n_chunks, ar.coeffs, ar.pcm, i16 ? 2 : 4, cap ? &plan->runs : nullptr, &lr)) ||
-        (rc = long_upload_runs(ctx, lr, host ? ctx->copy_in : ctx->copy_out)))
-        return rc;
-    for (size_t k = 0; k < lr.chunks.size(); k++) {
-        const LongRuns::Chunk &ck = lr.chunks[k];
+    uint64_t gen = 0;
+    size_t pk0 = 0;
+    for (size_t k = 0; k < n_chunks; k++) {
+        const size_t i0 = n_chains * k / n_chunks, i1 = n_chains * (k + 1) / n_chunks;
         BatchExtent ke;
         ke.scan = false;
-        if ((rc = long_extent(ctx, io, chains, ck.i0, ck.i1, &ke)) || (rc = ar.upload(k, ke)) ||
-            (rc = launch_long(ctx, lr.d + ck.r0, (uint32_t)(ck.nr / kLongNB), pack, i16)) ||
-            (rc = ar.download(k, chains, ck.i0, ck.i1, ke)))
-            return rc;
-    }
-    CU(ctx, cudaEventRecord(ctx->ev_kdone[lr.par], ctx->stream));
-    if (cap) capture(plan, gen_at_entry, FrontStages(), MixLaunch{nullptr, nullptr, 0, i16, pack}, {}, (uint32_t)(lr.chunks[0].nr / kLongNB));
-    if ((rc = ar.finish())) return rc;
-    for (size_t i = 0; i < n_chains; i++)
-        if (chains[i].n_packets) set_stream_state(chains[i].stream, true, kLongN2);
-    return LWB_OK;
-}
-
-// Residue-entry batches whose every packet is a long block with long neighbours: the front stages
-// (k_floor1_segments + k_prologue_fused, or k_prologue) form the spectrum on the device, the fused kernel does the
-// rest.  Planned straight from the chain list like try_long (no per-packet PlanChain vectors); a prepared batch
-// keeps the front-stage descriptors and, for device-memory batches, the fused kernel's runs, so that a replay
-// is three launches with no host work (lwb_plan_execute).
-static int try_long_residue(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, bool *handled, lwb_plan *plan)
-{
-    *handled = false;
-    if (io->entry == LWB_ENTRY_SPECTRUM || !batch_is_uniform_long(chains, n_chains, io)) return LWB_OK;
-    *handled = true;
-    set_long_results(chains, n_chains);
-    BatchExtent ext;
-    int rc;
-    if ((rc = long_extent(ctx, io, chains, 0, n_chains, &ext)) || (rc = ext.finish(ctx, io))) return rc;
-    if (ext.empty()) return LWB_OK;
-    const unsigned C = chains[0].stream->setup->channels;
-    const bool i16 = io->out_format == LWB_OUT_I16_PLANAR, host = io->memory == LWB_MEM_HOST;
-    const float *pack = chains[0].stream->setup->host.tab[1].pack;
-    size_t n_pk = 0;
-    for (size_t i = 0; i < n_chains; i++) n_pk += chains[i].n_packets;
-    cudaStream_t sm = ctx->stream;
-    if ((rc = ensure(ctx, ctx->spec, (size_t)(ext.c_hi - ext.c_lo) * 4))) return rc;
-    BatchArenas ar;
-    if ((rc = ar.open(ctx, io, ext, C, true))) return rc;
-    FrontStages fs;
-    fs.n = n_pk;
-    fs.C = C;
-    fs.smem_old = prologue_smem((int)C, kLongBs);
-    fs.n2max = kLongN2;
-    fs.c_lo = ext.c_lo;
-    fs.r_lo = ext.r_lo;
-    fs.r_hi = ext.r_hi;
-    fs.dense = ext.need_dense;
-    if (plan && plan->pro.p && plan->front.pk == plan->pro.p && plan->front.n == n_pk) {
-        // a prepared batch re-planned (host memory: every execution): the packet list of the previous execution
-        // depends only on the plan's chain and mode arrays
-        fs.pk = plan->front.pk;
-        fs.fast = plan->front.fast;
-    } else {
-        Staging *st;
-        if ((rc = acquire_staging(ctx, n_pk * sizeof(DevPacket), &st))) return rc;
-        DevBuf &db = plan ? plan->pro : ctx->desc;
-        if ((rc = ensure(ctx, db, n_pk * sizeof(DevPacket)))) return rc;
-        DevPacket *hp = (DevPacket *)st->h;
-        size_t di = 0;
-        for (size_t i = 0; i < n_chains; i++) {
-            write_front_packets(&chains[i], 0, chains[i].n_packets, chains[i].coeff_offset, hp + di);
-            di += chains[i].n_packets;
-        }
-        fs.pk = (const DevPacket *)db.p;
-        fs.fast = front_stages_fast(ctx, ar, fs, hp);
-        CU(ctx, cudaMemcpyAsync(db.p, hp, n_pk * sizeof(DevPacket), cudaMemcpyHostToDevice, sm));
-        CU(ctx, cudaEventRecord(st->ev, sm));
-        st->pending = true;
-    }
-    if (plan) plan->front = fs;
-    const uint64_t gen = ctx->state_gen;
-    const bool cap = plan && !host;
-    // Host memory: slices of chains flow through three streams -- copy_in brings a slice's inputs (dense residues, or
-    // VQ runs / entries, and its floor rows), the compute stream runs its front stages and the fused kernel, copy_out
-    // takes its PCM home -- so that H2D, kernels and D2H of consecutive slices overlap (the link is duplex).  The
-    // descriptor upload of a slice goes on copy_in: behind copy_out's PCM copies the next slice's kernels would wait
-    // for the previous slice's D2H.
-    const size_t n_sl = host ? host_chunks(n_pk * (size_t)C * kLongN2 * 4, n_chains) : 1;
-    const float *spec = (const float *)ctx->spec.p - ext.c_lo;
-    size_t pk0 = 0;
-    for (size_t sl = 0; sl < n_sl; sl++) {
-        const size_t i0 = n_chains * sl / n_sl, i1 = n_chains * (sl + 1) / n_sl;
-        BatchExtent se;
-        se.scan = false;
-        if ((rc = long_extent(ctx, io, chains, i0, i1, &se))) return rc;
-        if (se.empty()) continue;
+        if ((rc = uniform_extent(ctx, io, chains, i0, i1, kLongN2, &ke))) return rc;
+        if (ke.empty()) continue;
         size_t npk = 0;
         for (size_t i = i0; i < i1; i++) npk += chains[i].n_packets;
-        LongRuns lr;
-        if ((rc = ar.upload(sl, se)) || (rc = front_stages_launch(ctx, ar, fs, pk0, npk)) ||
-            (rc = long_build_runs(ctx, chains + i0, i1 - i0, 1, spec, ar.pcm, i16 ? 2 : 4, cap ? &plan->runs : nullptr, &lr)) ||
-            (rc = long_upload_runs(ctx, lr, host ? ctx->copy_in : ctx->copy_out)) ||
-            (rc = launch_long(ctx, lr.d, (uint32_t)(lr.n / kLongNB), pack, i16)) || (rc = ar.download(sl, chains, i0, i1, se)))
+        if ((rc = ar.upload(k, ke)) || (residue && (rc = front_stages_launch(ctx, ar, fs, pk0, npk)))) return rc;
+        if (!lr.d) {
+            if ((rc = long_build_runs(ctx, chains, n_chains, n_chunks, in, ar.pcm, i16 ? 2 : 4, cap ? &plan->runs : nullptr, &lr)) ||
+                (rc = long_upload_runs(ctx, lr, host ? ctx->copy_in : ctx->copy_out)))
+                return rc;
+            gen = ctx->state_gen;                                           // every arena the capture points into is sized
+        }
+        if ((rc = launch_long(ctx, lr.d + lr.chunks[k].r0, (uint32_t)(lr.chunks[k].nr / kLongNB), pack, i16)) ||
+            (rc = ar.download(k, chains, i0, i1, ke)))
             return rc;
-        CU(ctx, cudaEventRecord(ctx->ev_kdone[lr.par], sm));
-        if (cap) capture(plan, gen, fs, MixLaunch{nullptr, nullptr, 0, i16, pack}, {}, (uint32_t)(lr.n / kLongNB));
         pk0 += npk;
     }
+    CU(ctx, cudaEventRecord(ctx->ev_kdone[lr.par], ctx->stream));
+    if (cap) capture(plan, gen, fs, MixLaunch{nullptr, nullptr, 0, i16, pack}, {}, (uint32_t)(lr.chunks[0].nr / kLongNB));
     if ((rc = ar.finish())) return rc;
-    for (size_t i = 0; i < n_chains; i++)
-        if (chains[i].n_packets) set_stream_state(chains[i].stream, true, kLongN2);
+    commit_uniform_states(chains, n_chains, kLongN2);
     return LWB_OK;
 }

@@ -52,20 +52,12 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
     *handled = true;
 
     const bool host = io->memory == LWB_MEM_HOST;
-    cudaStream_t sm = ctx->stream;
     int rc;
     BatchExtent ext;
+    if ((rc = uniform_extent(ctx, io, chains, 0, n_chains, (uint32_t)kMidN2, &ext)) || (rc = ext.finish(ctx, io))) return rc;
     size_t n_pk = 0;
-    for (size_t i = 0; i < n_chains; i++) {
-        lwb_chain *c = &chains[i];
-        c->status = LWB_OK;
-        c->packets_done = c->n_packets;
-        c->n_samples = c->n_packets ? (uint32_t)((c->n_packets - (c->stream->has ? 0u : 1u)) * (uint32_t)kMidN2) : 0u;
-        if (residue) n_pk += c->n_packets;
-        const uint64_t coeff_end = c->coeff_offset + (uint64_t)c->n_packets * c->stream->setup->channels * kMidN2;
-        if ((rc = ext.add(ctx, io, c, c->n_packets, coeff_end, c->n_samples))) return rc;
-    }
-    if ((rc = ext.finish(ctx, io))) return rc;
+    if (residue)
+        for (size_t i = 0; i < n_chains; i++) n_pk += chains[i].n_packets;
     BatchArenas ar;
     if ((rc = ar.open(ctx, io, ext, C, false)) || (rc = ar.upload(0, ext))) return rc;
     const float *d_coeffs = ar.coeffs;
@@ -81,29 +73,9 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
         // front stages over every packet of the batch: residue (or VQ records) + floors -> spectrum arena, same element
         // offsets as the coefficient arena
         if ((rc = ensure(ctx, ctx->spec, (size_t)(ext.c_hi - ext.c_lo) * 4))) return rc;
-        DevPacket *d_pro = (DevPacket *)((char *)dbuf.p + off_pro);
-        fs.pk = d_pro;
-        fs.n = n_pk;
-        fs.C = C;
-        fs.smem_old = prologue_smem((int)C, 11 - kb);
-        fs.n2max = (int)kMidN2;
-        fs.c_lo = ext.c_lo;
-        fs.r_lo = ext.r_lo;
-        fs.r_hi = ext.r_hi;
-        fs.dense = ext.need_dense;
-        Staging *stp;
-        if ((rc = acquire_staging(ctx, n_pk * sizeof(DevPacket), &stp))) return rc;
-        DevPacket *hp = (DevPacket *)stp->h;
-        size_t di = 0;
-        for (size_t i = 0; i < n_chains; i++) {
-            write_front_packets(&chains[i], 0, chains[i].n_packets, chains[i].coeff_offset, hp + di);
-            di += chains[i].n_packets;
-        }
-        fs.fast = front_stages_fast(ctx, ar, fs, hp);
-        CU(ctx, cudaMemcpyAsync(d_pro, hp, n_pk * sizeof(DevPacket), cudaMemcpyHostToDevice, sm));
-        CU(ctx, cudaEventRecord(stp->ev, sm));
-        stp->pending = true;
-        if ((rc = front_stages_launch(ctx, ar, fs, 0, fs.n))) return rc;
+        fs = front_stages_of(ext, C, (int)(2 * kMidN2), n_pk);
+        if ((rc = stage_front_packets(ctx, ar, chains, n_chains, dbuf, off_pro, &fs)) || (rc = front_stages_launch(ctx, ar, fs, 0, fs.n)))
+            return rc;
         d_coeffs = (const float *)ctx->spec.p - ext.c_lo;       // k_mid reads the spectrum
     }
     // runs, then groups of two runs of equal length (an odd one gets a dummy partner), longest first, dealt balanced
@@ -154,9 +126,7 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
     for (size_t k = 0; k < groups.size(); k++)
         for (size_t b = 0; b < NBg; b++) h[NBg * k + b] = groups[k].r[b];
     if (bytes > off_pro) return fail(ctx, LWB_ERR_INVALID, "internal: more run groups than runs");
-    CU(ctx, cudaMemcpyAsync(dbuf.p, h, bytes, cudaMemcpyHostToDevice, sm));
-    CU(ctx, cudaEventRecord(st->ev, sm));
-    st->pending = true;
+    if ((rc = upload_staging(ctx, st, h, dbuf.p, bytes, ctx->stream))) return rc;
     const MixLaunch ml{(char *)dbuf.p, ar.pcm, io->out_format, i16, nullptr, 0, nullptr, nullptr, pack, kb};
     MixRound rd;
     std::memset(&rd, 0, sizeof(rd));
@@ -165,7 +135,6 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
     if ((rc = mixed_launch_rounds(ctx, ml, rounds))) return rc;
     if (cap) capture(plan, gen_at_entry, fs, ml, std::move(rounds));
     if ((rc = ar.download(0, chains, 0, n_chains, ext)) || (rc = ar.finish())) return rc;
-    for (size_t i = 0; i < n_chains; i++)
-        if (chains[i].n_packets) set_stream_state(chains[i].stream, true, (uint32_t)kMidN2);
+    commit_uniform_states(chains, n_chains, (uint32_t)kMidN2);
     return LWB_OK;
 }

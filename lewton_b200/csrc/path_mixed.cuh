@@ -228,7 +228,6 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
     if (!chain_sees_long) n1max = n0max;
     if (max_rounds) {
         const bool host = io->memory == LWB_MEM_HOST;
-        cudaStream_t sm = ctx->stream;
         BatchArenas ar;
         if ((rc = ar.open(ctx, io, ext, maxc, true))) return rc;
         const float *d_coeffs = ar.coeffs;
@@ -363,38 +362,24 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                         // samples packet 0 emits (0 without history; a block after a short one emits 1024 - ls)
                         const size_t first_emit = sg.has ? (sg.first_short ? (size_t)kLongN2 - ls_long : (size_t)kLongN2) : 0;
                         for (unsigned ch = 0; ch < C; ch++) {
-                            const float *in0 = (residue ? d_spec : d_coeffs) + sg.coeff + (size_t)ch * kLongN2;
-                            char *out0 = d_pcm + (c->out_offset + (size_t)ch * c->out_stride + sg.pos) * esz;
-                            for (uint32_t k = 0; k < cuts; k++) {
-                                const size_t p0 = (size_t)sg.n * k / cuts, p1 = (size_t)sg.n * (k + 1) / cuts;
-                                LongRun &lr = h_runs[wr++];
-                                std::memset(&lr, 0, sizeof(lr));
-                                lr.in_stride = (uint32_t)(C * kLongN2);
-                                lr.state = s->d_state + (size_t)ch * state_stride(su);
-                                lr.write_state = (k + 1 == cuts);
-                                lr.last_short = (k + 1 == cuts) && sg.last_short;
-                                if (chain_flat[i] && k + 1 == cuts && q + 1 < walks[i].n_seg) lr.state_out = slot_of(i, q, C, ch);
-                                if (k == 0) {
-                                    lr.in = in0;
-                                    lr.out = out0;
-                                    lr.n_packets = (uint32_t)(p1 - p0);
-                                    lr.has_prev = sg.has;
-                                    lr.first_short = sg.first_short;
-                                    if (chain_flat[i] && q) {   // the short segment in front runs later and completes the overlap
-                                        lr.first_short = 2;
-                                        lr.state_out = lr.state_out ? lr.state_out : lr.state;
-                                        lr.state = slot_of(i, q - 1, C, ch);
-                                    } else if (needs_precopy(i)) {
-                                        lr.state_out = lr.state_out ? lr.state_out : lr.state;
-                                        h_rc[wx++] = RowCopy{lr.state, pre_slot(i, C, ch), (uint32_t)(pre_units(i) * kShortN2 / 4), 0};
-                                        lr.state = pre_slot(i, C, ch);
-                                    }
-                                } else {
-                                    lr.in = in0 + (p0 - 1) * (size_t)lr.in_stride;         // primer = packet p0 - 1
-                                    lr.out = out0 + (first_emit + (p0 - 1) * (size_t)kLongN2) * esz;
-                                    lr.n_packets = (uint32_t)(p1 - p0 + 1);
-                                    lr.has_prev = 0;
-                                }
+                            LongRun *w = h_runs + wr;
+                            wr += cuts;
+                            cut_run(LongRun{(residue ? d_spec : d_coeffs) + sg.coeff + (size_t)ch * kLongN2,
+                                            d_pcm + (c->out_offset + (size_t)ch * c->out_stride + sg.pos) * esz, s->d_state + (size_t)ch * state_stride(su),
+                                            (uint32_t)(C * kLongN2), sg.n, sg.has},
+                                    cuts, first_emit, kLongN2, esz, w);
+                            LongRun &last = w[cuts - 1], &lr = w[0];         // (one piece: the same run)
+                            last.last_short = sg.last_short;
+                            if (chain_flat[i] && q + 1 < walks[i].n_seg) last.state_out = slot_of(i, q, C, ch);
+                            lr.first_short = sg.first_short;
+                            if (chain_flat[i] && q) {   // the short segment in front runs later and completes the overlap
+                                lr.first_short = 2;
+                                lr.state_out = lr.state_out ? lr.state_out : lr.state;
+                                lr.state = slot_of(i, q - 1, C, ch);
+                            } else if (needs_precopy(i)) {
+                                lr.state_out = lr.state_out ? lr.state_out : lr.state;
+                                h_rc[wx++] = RowCopy{lr.state, pre_slot(i, C, ch), (uint32_t)(pre_units(i) * kShortN2 / 4), 0};
+                                lr.state = pre_slot(i, C, ch);
                             }
                         }
                         if (residue) emit_pro(c, sg);
@@ -413,42 +398,33 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                     const unsigned C = su->channels;
                     const uint32_t cuts = cuts_of(ck, sg, r);
                     const size_t first_emit = sg.has ? (size_t)kShortN2 : 0;       // samples packet 0 emits
+                    const bool burst = bursts && chain_flat[i] && sg.n < (uint32_t)kShortOct;    // (one piece)
                     for (unsigned ch = 0; ch < C; ch++) {
-                        const float *in0 = (residue ? d_spec : d_coeffs) + sg.coeff + (size_t)ch * kShortN2;
-                        char *out0 = d_pcm + (c->out_offset + (size_t)ch * c->out_stride + sg.pos) * esz;
-                        for (uint32_t k = 0; k < cuts; k++) {
-                            const size_t p0 = (size_t)sg.n * k / cuts, p1 = (size_t)sg.n * (k + 1) / cuts;
-                            const bool burst = bursts && chain_flat[i] && sg.n < (uint32_t)kShortOct;
-                            if (burst) burst_runs.emplace_back();
-                            ShortRun &sr = burst ? burst_runs.back() : h_sr[ws++];
-                            std::memset(&sr, 0, sizeof(sr));
-                            sr.in_stride = (uint32_t)(C * kShortN2);
-                            sr.state = s->d_state + (size_t)ch * state_stride(su);
-                            sr.write_state = (k + 1 == cuts);
-                            if (chain_flat[i] && k + 1 == cuts && q + 1 < walks[i].n_seg) {      // the long block behind has run already
-                                sr.write_state = 0;
-                                sr.tail = 1;
-                                sr.end_ptr = slot_of(i, q, C, ch);
-                            }
-                            if (k == 0) {
-                                sr.in = in0;
-                                sr.out = out0;
-                                sr.n_packets = (uint32_t)(p1 - p0);
-                                sr.has_prev = sg.has;
-                                if (chain_flat[i] && q) {       // the long segment in front left its right half in the slot
-                                    if (!sr.end_ptr) sr.end_ptr = sr.state;
-                                    sr.state = slot_of(i, q - 1, C, ch);
-                                } else if (needs_precopy(i)) {
-                                    if (!sr.end_ptr) sr.end_ptr = sr.state;
-                                    h_rc[wx++] = RowCopy{sr.state, pre_slot(i, C, ch), (uint32_t)(kShortN2 / 4), 0};
-                                    sr.state = pre_slot(i, C, ch);
-                                }
-                            } else {
-                                sr.in = in0 + (p0 - 1) * (size_t)sr.in_stride;            // primer = packet p0 - 1
-                                sr.out = out0 + (first_emit + (p0 - 1) * (size_t)kShortN2) * esz;
-                                sr.n_packets = (uint32_t)(p1 - p0 + 1);
-                                sr.has_prev = 0;
-                            }
+                        ShortRun *w;
+                        if (burst) {
+                            burst_runs.resize(burst_runs.size() + cuts);
+                            w = &burst_runs[burst_runs.size() - cuts];
+                        } else {
+                            w = h_sr + ws;
+                            ws += cuts;
+                        }
+                        cut_run(ShortRun{(residue ? d_spec : d_coeffs) + sg.coeff + (size_t)ch * kShortN2,
+                                         d_pcm + (c->out_offset + (size_t)ch * c->out_stride + sg.pos) * esz, s->d_state + (size_t)ch * state_stride(su),
+                                         (uint32_t)(C * kShortN2), sg.n, sg.has},
+                                cuts, first_emit, kShortN2, esz, w);
+                        ShortRun &last = w[cuts - 1], &sr = w[0];        // (one piece: the same run)
+                        if (chain_flat[i] && q + 1 < walks[i].n_seg) {      // the long block behind has run already
+                            last.write_state = 0;
+                            last.tail = 1;
+                            last.end_ptr = slot_of(i, q, C, ch);
+                        }
+                        if (chain_flat[i] && q) {       // the long segment in front left its right half in the slot
+                            if (!sr.end_ptr) sr.end_ptr = sr.state;
+                            sr.state = slot_of(i, q - 1, C, ch);
+                        } else if (needs_precopy(i)) {
+                            if (!sr.end_ptr) sr.end_ptr = sr.state;
+                            h_rc[wx++] = RowCopy{sr.state, pre_slot(i, C, ch), (uint32_t)(kShortN2 / 4), 0};
+                            sr.state = pre_slot(i, C, ch);
                         }
                     }
                     if (residue) emit_pro(c, sg);
@@ -516,22 +492,12 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
             }
             ck.np_ = wp - ck.p0;
         }
-        CU(ctx, cudaMemcpyAsync(db, hb, total, cudaMemcpyHostToDevice, sm));
-        CU(ctx, cudaEventRecord(st->ev, sm));
-        st->pending = true;
+        if ((rc = upload_staging(ctx, st, hb, db, total, ctx->stream))) return rc;
         // (residue entry: the front stages run first, the chain kernel sees a spectrum)
         const MixLaunch ml{db, d_pcm, io->out_format, i16, pack, ls_long, w_short, spack, nullptr, 0, off_sr, off_cd, off_by, off_rc, off_sg,
                            false, chain_shape(maxc, n1max, false), residue ? d_spec : d_coeffs};
-        FrontStages fs;                         // (residue entry: every packet of the batch, chunk by chunk)
+        FrontStages fs = front_stages_of(ext, maxc, n1max_all, n_pro);         // (residue entry: every packet of the batch, chunk by chunk)
         fs.pk = (const DevPacket *)(db + off_pro);
-        fs.n = n_pro;
-        fs.C = maxc;
-        fs.smem_old = prologue_smem(maxc, kLongBs);
-        fs.n2max = n1max_all >> 1;
-        fs.c_lo = ext.c_lo;
-        fs.r_lo = ext.r_lo;
-        fs.r_hi = ext.r_hi;
-        fs.dense = ext.need_dense;
         if (fs.n) fs.fast = front_stages_fast(ctx, ar, fs, h_pro);
         for (size_t k = 0; k < n_chunks; k++) {
             Chunk &ck = chunks[k];

@@ -251,10 +251,10 @@ def must_return(path, chunks):
     """Submits of `path` that return behind the gate, from the blocking points the header lists.  The staging ring has
     three slots, all completed after the warm-up.  Paths that stage once per submit (k_long, the one-pass and segmented
     schedules, k_mid's spectrum entry, k_chain) therefore return all three.  The residue entries of k_mid and k_long
-    stage their packet list on the compute stream and then their runs: the second submit takes the first one's packet
-    list slot, which completes behind the gate.  k_long's residue entry stages runs per slice: with three slices one
-    submit wraps the ring by itself.  The four-kernel path synchronises before its first round."""
-    if path == "generic" or (path == "residue_long" and chunks > 1):
+    stage twice per submit, at any chunk count: their packet list on the compute stream, then all their runs at once.
+    The second submit takes the first one's packet list slot, which completes behind the gate.  The four-kernel path
+    synchronises before its first round."""
+    if path == "generic":
         return 0
     return 1 if path in ("residue_long", "residue_mid") else 3
 
