@@ -79,7 +79,7 @@ uint64_t lwb_ctx_launch_count(const lwb_ctx *ctx);
 enum { LWB_KERNEL_LONG = 0, LWB_KERNEL_LONG_S = 1, LWB_KERNEL_MID = 2, LWB_KERNEL_SHORT = 3, LWB_KERNEL_SHORT_G = 4,
        LWB_KERNEL_ROW_COPY = 5, LWB_KERNEL_CHAIN = 6, LWB_KERNEL_FLOOR1_SEGMENTS = 7, LWB_KERNEL_PROLOGUE_FUSED = 8,
        LWB_KERNEL_PROLOGUE = 9, LWB_KERNEL_IMDCT = 10, LWB_KERNEL_OVERLAP = 11, LWB_KERNEL_SAVE_STATE = 12,
-       LWB_KERNEL_COUNT = 13 };
+       LWB_KERNEL_FLOOR0_CURVES = 13, LWB_KERNEL_COUNT = 14 };
 /* debug: launches of kernel `kernel_id` (LWB_KERNEL_*) by this ctx since creation (0 for an unknown id); the
  * counts of all ids sum to lwb_ctx_launch_count */
 uint64_t lwb_ctx_kernel_launches(const lwb_ctx *ctx, int kernel_id);
@@ -114,7 +114,7 @@ typedef struct lwb_tables_ref {      /* IdentHeader.cached_bs_derived[i], header
 
 enum { LWB_FLOOR_TYPE_ZERO = 0, LWB_FLOOR_TYPE_ONE = 1 };
 typedef struct lwb_floor_desc {      /* header::Floor, header.rs:399-424                           */
-    uint8_t floor_type;              /* type 0 curves are computed by the host and passed dense    */
+    uint8_t floor_type;              /* type 0: dense curves, or records (lwb_setup_set_floor0)    */
     uint8_t floor1_multiplier;       /* 1..4                                                       */
     uint8_t floor1_values;           /* floor1_x_list.len(), 2..65                                 */
     uint8_t reserved;
@@ -172,6 +172,23 @@ typedef struct lwb_setup_desc {
 int lwb_setup_create(lwb_ctx *ctx, const lwb_setup_desc *desc, lwb_setup **out);
 void lwb_setup_destroy(lwb_setup *setup);
 
+/* Floor type 0 on the device (added under ABI 3: no struct above changes).  A type-0 floor described here can be sent
+ * as LWB_FLOOR_ZERO records instead of dense LWB_FLOOR_DENSE curves; the device then computes the curve
+ * (floor_zero_compute_curve, audio.rs:160-212) bit for bit.  NULL bark_cos_omega tables are generated on the host with
+ * libm cosf / atanf in the order of header_cached.rs:129-158. */
+typedef struct lwb_floor0_desc {     /* header::FloorTypeZero, header.rs:399-407                       */
+    uint8_t order;                   /* floor0_order, 2..63 (a record holds at most 63 coefficients)    */
+    uint8_t amplitude_bits;          /* 1..64                                                          */
+    uint8_t amplitude_offset;
+    uint8_t reserved;
+    uint16_t rate;                   /* floor0_rate                                                    */
+    uint16_t bark_map_size;          /* floor0_bark_map_size                                           */
+    const float *bark_cos_omega[2];  /* cached_bark_cos_omega for blocksize_0 / blocksize_1 (n/2 floats each), or NULL */
+} lwb_floor0_desc;
+/* Describes floor `floor_index` (of type LWB_FLOOR_TYPE_ZERO in the setup's lwb_floor_desc) for LWB_FLOOR_ZERO rows.
+ * Call it before the setup's first batch.  LWB_ERR_INVALID for a bad index, a floor of type 1 or a field out of range. */
+int lwb_setup_set_floor0(lwb_setup *setup, uint32_t floor_index, const lwb_floor0_desc *desc);
+
 /* ---- stream state: PreviousWindowRight, audio.rs:847-861 ---------------------------------- */
 int lwb_stream_open(lwb_ctx *ctx, const lwb_setup *setup, lwb_stream **out);
 void lwb_stream_destroy(lwb_stream *s);
@@ -194,7 +211,13 @@ int lwb_decoded_sample_count(const lwb_setup *setup, uint8_t mode_number, int pr
 /* ---- one packet (mirrors read_audio_packet_generic's back half) --------------------------- */
 enum { LWB_FLOOR_UNUSED = 0,   /* DecodedFloor::Unused  -> zero curve (audio.rs:1021-1024)        */
        LWB_FLOOR_ONE = 1,      /* DecodedFloor::TypeOne -> raw floor1_y from floor_one_decode      */
-       LWB_FLOOR_DENSE = 2 };  /* DecodedFloor::TypeZero -> curve computed by the host (n/2 f32)   */
+       LWB_FLOOR_DENSE = 2,    /* DecodedFloor::TypeZero -> curve computed by the host (n/2 f32)   */
+       LWB_FLOOR_ZERO = 3 };   /* DecodedFloor::TypeZero -> a floor-0 record in the floor1_y row:  *
+                                * words 0-1 the amplitude (u64, low word first), words 2 .. 2 + order *
+                                * - 1 the coefficient cosines as f32 bits (floor_zero_decode's        *
+                                * output); the device computes the curve.  The row's floor needs a    *
+                                * floor-0 description (lwb_setup_set_floor0): host floor arrays are   *
+                                * refused without one, device ones act as LWB_FLOOR_UNUSED.           */
 
 enum { LWB_OUT_F32_PLANAR = 0,        /* Vec<Vec<f32>>            samples.rs:20-40, 86-90          */
        LWB_OUT_I16_PLANAR = 1,        /* Vec<Vec<i16>>            samples.rs:92-103                */

@@ -66,6 +66,9 @@ int lwf_headers_info(const lwf_headers *h, lwf_info *out);
 size_t lwf_headers_comment(const lwf_headers *h, int index, char *buf, size_t cap);
 /* what lwb_setup_create needs, filled from the parsed headers (tables via lwb_tables_generate) */
 int lwf_headers_make_setup(const lwf_headers *h, lwb_ctx *ctx, lwb_setup **out);
+/* the same, and every type-0 floor that can travel as an LWB_FLOOR_ZERO record (order 2..63, nonzero rate and bark
+ * map size) described with lwb_setup_set_floor0: the setup for packets decoded with LWF_DECODE_FLOOR0_RECORDS */
+int lwf_headers_make_setup_floor0(const lwf_headers *h, lwb_ctx *ctx, lwb_setup **out);
 
 /* ---- one audio packet: front half of read_audio_packet_generic ------------------------------- */
 typedef struct lwf_decoded_packet {
@@ -83,6 +86,11 @@ typedef struct lwf_decoded_packet {
 /* Buffers in `out` must hold channels x blocksize_1/2 floats.  Returns LWB_OK, LWF_ERR_AUDIO_IS_HEADER,
  * LWF_ERR_END_OF_PACKET (header bits missing) or LWB_ERR_BAD_FORMAT (audio.rs:926-930, :975). */
 int lwf_packet_decode(const lwf_headers *h, const uint8_t *packet, size_t len, lwf_decoded_packet *out);
+/* flags: LWF_DECODE_FLOOR0_RECORDS -- type-0 floors of order <= 63 (and nonzero rate / bark map size) come out as
+ * LWB_FLOOR_ZERO records in their floor1_y row instead of dense curves, for a setup from lwf_headers_make_setup_floor0;
+ * dense_floor may then be NULL when no type-0 floor of the stream needs it.  flags == 0 is lwf_packet_decode. */
+enum { LWF_DECODE_FLOOR0_RECORDS = 1 };
+int lwf_packet_decode_ex(const lwf_headers *h, const uint8_t *packet, size_t len, lwf_decoded_packet *out, int flags);
 int lwf_decoded_sample_count(const lwf_headers *h, const uint8_t *packet, size_t len, size_t *n_samples);
 /* The same front half with the residue left as VQ runs + entries (SURVEY.md 8f rank 2; audio.rs:587-717): what
  * residue_packet_decode would have ADDED, partition by partition in decode order, for LWB_ENTRY_VQ batches (out->residue
@@ -93,6 +101,9 @@ int lwf_headers_vq_capable(const lwf_headers *h);
 int lwf_packet_decode_vq(const lwf_headers *h, const uint8_t *packet, size_t len, lwf_decoded_packet *out,
                          lwb_vq_run *runs, size_t run_capacity, size_t *n_runs, uint16_t *entries, size_t entry_capacity,
                          size_t *n_entries);
+int lwf_packet_decode_vq_ex(const lwf_headers *h, const uint8_t *packet, size_t len, lwf_decoded_packet *out,
+                            lwb_vq_run *runs, size_t run_capacity, size_t *n_runs, uint16_t *entries, size_t entry_capacity,
+                            size_t *n_entries, int flags);
 
 /* ---- Ogg paging -------------------------------------------------------------------------------- */
 typedef struct lwf_ogg lwf_ogg;             /* PacketReader over a memory buffer (not copied)      */
@@ -155,9 +166,15 @@ void lwf_batcher_destroy(lwf_batcher *b);
 /* LWB_ENTRY_RESIDUE (default: dense residue vectors cross the boundary) or LWB_ENTRY_VQ (VQ records do; needs
  * lwf_headers_vq_capable) */
 int lwf_batcher_set_entry(lwf_batcher *b, int entry);
+/* records != 0: decode with LWF_DECODE_FLOOR0_RECORDS (the jobs' streams must come from lwf_headers_make_setup_floor0);
+ * when every type-0 floor of the stream qualifies, no dense floor arena is allocated or sent */
+int lwf_batcher_set_floor0(lwf_batcher *b, int records);
 int lwf_batcher_decode(lwf_batcher *b, lwf_stream_job *jobs, size_t n_jobs, int out_format, void *pcm);
 /* wall-clock seconds of the last lwf_batcher_decode: host entropy decode, synthesis call */
 void lwf_batcher_last_timing(const lwf_batcher *b, double *entropy_seconds, double *synthesis_seconds);
+/* bytes of the host arrays the last lwf_batcher_decode handed to the synthesis (residues or VQ records, dense floor-0
+ * curves, floor kinds and floor1_y rows): what its host-memory batches copy to the device */
+uint64_t lwf_batcher_last_input_bytes(const lwf_batcher *b);
 
 /* ---- debug taps (known-answer tests of the reference's unit-test vectors) ---------------------- */
 float lwf_debug_float32_unpack(uint32_t v);                          /* bitpacking.rs:304-314        */

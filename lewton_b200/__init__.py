@@ -5,11 +5,11 @@ Importing the package loads nothing; the first call into `lewton_b200.api` loads
 lewton_b200/liblewton_b200.so and raises if it is absent (no CPU fallback).
 """
 from . import _cabi  # noqa: F401
-from .api import (AudioReadError, Batch, ChainSpec, Context, DecodedPacket, FloorTypeOne, FloorTypeZero, Mapping,  # noqa: F401
+from .api import (AudioReadError, Batch, ChainSpec, Context, DecodedPacket, Floor0Record, FloorTypeOne, FloorTypeZero, Mapping,  # noqa: F401
                   ModeInfo, PreviousWindowRight, Setup, Ticket, VorbisError, debug_taps, decode_chains, decode_spectrum,
                   generate_tables, get_decoded_sample_count, read_audio_packet, read_audio_packet_generic)
 
-__all__ = ["AudioReadError", "Batch", "ChainSpec", "Context", "DecodedPacket", "FloorTypeOne", "FloorTypeZero", "Mapping",
+__all__ = ["AudioReadError", "Batch", "ChainSpec", "Context", "DecodedPacket", "Floor0Record", "FloorTypeOne", "FloorTypeZero", "Mapping",
            "ModeInfo", "PreviousWindowRight", "Setup", "Ticket", "VorbisError", "debug_taps", "decode_chains",
            "decode_spectrum", "generate_tables", "get_decoded_sample_count", "read_audio_packet",
            "read_audio_packet_generic"]

@@ -13,13 +13,13 @@ SO_PATH = os.environ.get("LWB_LIB") or os.path.join(_HERE, "liblewton_b200.so")
 MAX_POSTS, MAX_CHANNELS, MAX_COUPLING, MAX_SUBMAPS, MAX_MODES = 65, 255, 256, 16, 64
 OK, ERR_BAD_FORMAT, ERR_BUFFER, ERR_MISMATCH, ERR_INVALID, ERR_CUDA, ERR_NO_DEVICE = range(7)
 FLOOR_TYPE_ZERO, FLOOR_TYPE_ONE = 0, 1
-FLOOR_UNUSED, FLOOR_ONE, FLOOR_DENSE = 0, 1, 2
+FLOOR_UNUSED, FLOOR_ONE, FLOOR_DENSE, FLOOR_ZERO = 0, 1, 2, 3
 OUT_F32_PLANAR, OUT_I16_PLANAR, OUT_F32_INTERLEAVED, OUT_I16_INTERLEAVED = 0, 1, 2, 3
 ENTRY_SPECTRUM, ENTRY_RESIDUE, ENTRY_VQ = 0, 1, 2
 MEM_HOST, MEM_DEVICE = 0, 1
 # LWB_KERNEL_* ids in order: KERNELS[id] is the kernel's name
 KERNELS = ("k_long", "k_long_s", "k_mid", "k_short", "k_short_g", "k_row_copy", "k_chain", "k_floor1_segments",
-           "k_prologue_fused", "k_prologue", "k_imdct", "k_overlap", "k_save_state")
+           "k_prologue_fused", "k_prologue", "k_imdct", "k_overlap", "k_save_state", "k_floor0_curves")
 
 vp, u8p, fp, u32p = C.c_void_p, C.POINTER(C.c_uint8), C.POINTER(C.c_float), C.POINTER(C.c_uint32)
 
@@ -66,6 +66,11 @@ class SetupDesc(C.Structure):
                 ("n_residues", C.c_uint32), ("residues", C.POINTER(ResidueDesc))]
 
 
+class Floor0Desc(C.Structure):
+    _fields_ = [("order", C.c_uint8), ("amplitude_bits", C.c_uint8), ("amplitude_offset", C.c_uint8), ("reserved", C.c_uint8),
+                ("rate", C.c_uint16), ("bark_map_size", C.c_uint16), ("bark_cos_omega", fp * 2)]
+
+
 class Packet(C.Structure):
     _fields_ = [("mode_number", C.c_uint8), ("prev_window_flag", C.c_uint8), ("next_window_flag", C.c_uint8),
                 ("reserved", C.c_uint8), ("floor_kind", u8p), ("floor1_y", u32p), ("dense_floor", fp),
@@ -107,6 +112,7 @@ SYMBOLS = {
     "lwb_tables_generate": (C.c_int, [C.c_int, vp, vp, vp, vp, vp]),
     "lwb_setup_create": (C.c_int, [vp, C.POINTER(SetupDesc), C.POINTER(vp)]),
     "lwb_setup_destroy": (None, [vp]),
+    "lwb_setup_set_floor0": (C.c_int, [vp, C.c_uint32, C.POINTER(Floor0Desc)]),
     "lwb_stream_open": (C.c_int, [vp, vp, C.POINTER(vp)]),
     "lwb_stream_destroy": (None, [vp]),
     "lwb_stream_reset": (C.c_int, [vp]),

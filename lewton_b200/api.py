@@ -138,7 +138,12 @@ class FloorTypeOne:
 
 
 class FloorTypeZero:
-    """header.rs:405-412: its curve is computed by the host and passed dense."""
+    """header.rs:405-412.  Without arguments its curves are computed by the host and passed dense; with the floor's
+    header fields, Setup describes it to the device (Setup.set_floor0), which then also takes floor-0 records."""
+
+    def __init__(self, order=None, rate=0, bark_map_size=0, amplitude_bits=0, amplitude_offset=0):
+        self.order, self.rate, self.bark_map_size = order, int(rate), int(bark_map_size)
+        self.amplitude_bits, self.amplitude_offset = int(amplitude_bits), int(amplitude_offset)
 
 
 class Mapping:
@@ -210,6 +215,23 @@ class Setup:
             self._h = None
             raise AudioReadError(rc, cabi.lib().lwb_last_error(ctx._h).decode())
         ctx._children.add(self)
+        for i, f in enumerate(self.floors):
+            if isinstance(f, FloorTypeZero) and f.order is not None:
+                self.set_floor0(i, f.order, f.rate, f.bark_map_size, f.amplitude_bits, f.amplitude_offset)
+
+    def set_floor0(self, floor_index, order, rate, bark_map_size, amplitude_bits, amplitude_offset, bark_cos_omega=(None, None)):
+        """lwb_setup_set_floor0: describe type-0 floor `floor_index` so that packets may carry it as a floor-0 record
+        (DecodedPacket floors given as Floor0Record); bark_cos_omega: the two cached tables (n/2 float32 each) or None
+        to generate them."""
+        d = cabi.Floor0Desc()
+        d.order, d.amplitude_bits, d.amplitude_offset = order, amplitude_bits, amplitude_offset
+        d.rate, d.bark_map_size = rate, bark_map_size
+        keep = []
+        for i, t in enumerate(bark_cos_omega):
+            if t is not None:
+                keep.append(np.ascontiguousarray(t, np.float32))
+                d.bark_cos_omega[i] = _ptr(keep[-1], cabi.fp)
+        self.ctx.check(cabi.lib().lwb_setup_set_floor0(self._h, floor_index, C.byref(d)))
 
     @classmethod
     def _adopt(cls, ctx, handle, audio_channels, blocksize_0, blocksize_1, mode_blockflags=()):
@@ -295,11 +317,29 @@ class PreviousWindowRight:
             pass
 
 
+class Floor0Record:
+    """DecodedFloor::TypeZero as floor_zero_decode returns it (audio.rs:109-158): the amplitude and the coefficient
+    cosines; packed as the LWB_FLOOR_ZERO record of a floor1_y row."""
+
+    def __init__(self, amplitude, coefficients):
+        self.amplitude = int(amplitude)
+        self.coefficients = np.ascontiguousarray(coefficients, np.float32)
+        if not 2 <= len(self.coefficients) <= cabi.MAX_POSTS - 2:
+            raise ValueError("a floor-0 record holds 2..63 coefficients")
+
+    def words(self):
+        w = np.zeros(cabi.MAX_POSTS, np.uint32)
+        w[0], w[1] = self.amplitude & 0xFFFFFFFF, self.amplitude >> 32
+        w[2: 2 + len(self.coefficients)] = self.coefficients.view(np.uint32)
+        return w
+
+
 class DecodedPacket:
     """What audio.rs:921-986 hands to the synthesis half.
 
     floors: per channel  None (DecodedFloor::Unused) | sequence of floor1 Y values
-            (DecodedFloor::TypeOne) | float32 ndarray of n/2 (a floor-0 curve computed by the host)
+            (DecodedFloor::TypeOne) | float32 ndarray of n/2 (a floor-0 curve computed by the host) |
+            Floor0Record (DecodedFloor::TypeZero: the device computes the curve)
     residue: [channels][n/2] float32
     """
 
@@ -317,6 +357,9 @@ class DecodedPacket:
         for c, f in enumerate(self.floors):
             if f is None:
                 kinds[c] = cabi.FLOOR_UNUSED
+            elif isinstance(f, Floor0Record):
+                kinds[c] = cabi.FLOOR_ZERO
+                ys[c] = f.words()
             elif isinstance(f, np.ndarray) and f.dtype.kind == "f":
                 kinds[c] = cabi.FLOOR_DENSE
                 if dense is None:

@@ -280,6 +280,7 @@ struct ModeInfo { bool blockflag = false; uint8_t mapping = 0; };
 
 struct Floor0 {                      // header.rs:399-407
     uint8_t order = 0, amplitude_bits = 0, amplitude_offset = 0, number_of_books = 0;
+    uint16_t rate = 0, bark_map_size = 0;
     std::vector<uint8_t> book_list;
     std::vector<float> bark_cos_omega[2];
 };
@@ -559,7 +560,8 @@ static inline float bark(float x)
 {
     return 13.1f * atanf(0.00074f * x) + 2.24f * atanf(0.0000000185f * x * x) + 0.0001f * x;
 }
-static std::vector<float> bark_map_cos_omega(uint16_t n, uint16_t rate, uint16_t bark_map_size)
+// (also generates the tables lwb_setup_set_floor0 is not given, lwb_api.cu)
+std::vector<float> bark_map_cos_omega(uint16_t n, uint16_t rate, uint16_t bark_map_size)
 {
     std::vector<float> res;
     res.reserve(n);
@@ -597,6 +599,8 @@ static int read_floor(BitReader &rdr, uint16_t codebook_cnt, uint8_t bs0, uint8_
         f.amplitude_bits = (uint8_t)abits;
         f.amplitude_offset = (uint8_t)aoff;
         f.number_of_books = (uint8_t)nbooks;
+        f.rate = (uint16_t)rate;
+        f.bark_map_size = (uint16_t)bms;
         for (uint32_t i = 0; i < nbooks; i++) {
             uint32_t v;
             RD(rdr.u(8, &v));
@@ -909,6 +913,14 @@ static void floor0_curve(const std::vector<float> &cosc, uint64_t amplitude, con
     for (; w < n; w++) out[w] = 0.f;
 }
 
+// Whether a type-0 floor can travel as an LWB_FLOOR_ZERO record (lwf_packet_decode_ex with LWF_DECODE_FLOOR0_RECORDS):
+// the record holds at most LWB_MAX_POSTS - 2 coefficients, and lwb_setup_set_floor0 takes the floor (a zero rate or
+// bark map size gives a NaN bark table, on which the reference's run walk never ends).
+static bool floor0_record_ok(const Floor0 &fl)
+{
+    return fl.order >= 2 && fl.order <= LWB_MAX_POSTS - 2 && fl.rate && fl.bark_map_size;
+}
+
 // floor_one_decode, audio.rs:215-251
 static int floor1_decode(BitReader &rdr, const std::vector<Codebook> &codebooks, const Floor1 &fl, uint32_t *y, uint32_t *count)
 {
@@ -1162,7 +1174,10 @@ static int packet_head(const Headers &h, BitReader &rdr, PacketHead *ph)
     return LWB_OK;
 }
 
-static int packet_decode(const Headers &h, const uint8_t *packet, size_t len, lwf_decoded_packet *out, VqSink *sink = nullptr)
+// records: type-0 floors that qualify (floor0_record_ok) come out as LWB_FLOOR_ZERO records in their floor1_y row instead
+// of dense curves.
+static int packet_decode(const Headers &h, const uint8_t *packet, size_t len, lwf_decoded_packet *out, VqSink *sink = nullptr,
+                         bool records = false)
 {
     BitReader rdr(packet, len);
     PacketHead ph;
@@ -1186,7 +1201,15 @@ static int packet_decode(const Headers &h, const uint8_t *packet, size_t len, lw
         if (fl.type == 0) {
             uint64_t amp = 0;
             fr = floor0_decode(rdr, h.codebooks, fl.f0, &cosc, &amp);
-            if (fr == FL_OK) {
+            if (fr == FL_OK && records && floor0_record_ok(fl.f0)) {
+                // the record: amplitude (low word first), then the coefficient cosines' bits (lewton_b200.h LWB_FLOOR_ZERO)
+                uint32_t *y = out->floor1_y + c * LWB_MAX_POSTS;
+                std::memset(y, 0, sizeof(uint32_t) * LWB_MAX_POSTS);
+                y[0] = (uint32_t)amp;
+                y[1] = (uint32_t)(amp >> 32);
+                std::memcpy(y + 2, cosc.data(), cosc.size() * sizeof(float));
+                out->floor_kind[c] = LWB_FLOOR_ZERO;
+            } else if (fr == FL_OK) {
                 out->floor_kind[c] = LWB_FLOOR_DENSE;
                 floor0_curve(cosc, amp, fl.f0, ph.blockflag, (uint32_t)n2, out->dense_floor + c * n2);
             }
@@ -1560,15 +1583,52 @@ extern "C" int lwf_headers_vq_capable(const lwf_headers *h)
     return 1;
 }
 
+// Whether decoding with `flags` can produce dense floor-0 curves (a type-0 floor that does not travel as a record).
+static bool needs_dense(const lwf::Headers &h, int flags)
+{
+    for (const auto &fl : h.floors)
+        if (fl.type == 0 && !((flags & LWF_DECODE_FLOOR0_RECORDS) && lwf::floor0_record_ok(fl.f0))) return true;
+    return false;
+}
+
+// The lwb_setup_set_floor0 descriptions of the headers' type-0 floors that can travel as records (floor index, desc; the
+// tables point into the headers).  lwf_headers_make_setup_floor0 (lwb_api.cu) applies them.
+namespace lwf {
+void floor0_descs(const lwf_headers *h, std::vector<uint32_t> *index, std::vector<lwb_floor0_desc> *descs)
+{
+    for (size_t i = 0; i < h->h.floors.size(); i++) {
+        const Floor &fl = h->h.floors[i];
+        if (fl.type != 0 || !floor0_record_ok(fl.f0)) continue;
+        lwb_floor0_desc d;
+        std::memset(&d, 0, sizeof(d));
+        d.order = fl.f0.order;
+        d.amplitude_bits = fl.f0.amplitude_bits;
+        d.amplitude_offset = fl.f0.amplitude_offset;
+        d.rate = fl.f0.rate;
+        d.bark_map_size = fl.f0.bark_map_size;
+        d.bark_cos_omega[0] = fl.f0.bark_cos_omega[0].data();      // the tables the dense path uses
+        d.bark_cos_omega[1] = fl.f0.bark_cos_omega[1].data();
+        index->push_back((uint32_t)i);
+        descs->push_back(d);
+    }
+}
+}  // namespace lwf
+
 extern "C" int lwf_packet_decode_vq(const lwf_headers *h, const uint8_t *packet, size_t len, lwf_decoded_packet *out,
                                     lwb_vq_run *runs, size_t run_capacity, size_t *n_runs, uint16_t *entries, size_t entry_capacity,
                                     size_t *n_entries)
 {
+    return lwf_packet_decode_vq_ex(h, packet, len, out, runs, run_capacity, n_runs, entries, entry_capacity, n_entries, 0);
+}
+
+extern "C" int lwf_packet_decode_vq_ex(const lwf_headers *h, const uint8_t *packet, size_t len, lwf_decoded_packet *out,
+                                       lwb_vq_run *runs, size_t run_capacity, size_t *n_runs, uint16_t *entries, size_t entry_capacity,
+                                       size_t *n_entries, int flags)
+{
     if (!h || (!packet && len) || !out || !out->floor_kind || !out->floor1_y || (!runs && run_capacity) || (!entries && entry_capacity) ||
-        !n_runs || !n_entries)
+        !n_runs || !n_entries || (flags & ~LWF_DECODE_FLOOR0_RECORDS))
         return LWB_ERR_INVALID;
-    for (const auto &fl : h->h.floors)
-        if (fl.type == 0 && !out->dense_floor) return LWB_ERR_INVALID;
+    if (!out->dense_floor && needs_dense(h->h, flags)) return LWB_ERR_INVALID;
     *n_runs = *n_entries = 0;
     LWF_GUARD(
         lwf::VqSink sink;
@@ -1576,7 +1636,7 @@ extern "C" int lwf_packet_decode_vq(const lwf_headers *h, const uint8_t *packet,
         sink.run_cap = run_capacity;
         sink.entries = entries;
         sink.ent_cap = entry_capacity;
-        const int rc = lwf::packet_decode(h->h, packet, len, out, &sink);
+        const int rc = lwf::packet_decode(h->h, packet, len, out, &sink, (flags & LWF_DECODE_FLOOR0_RECORDS) != 0);
         if (rc) return rc;
         if (sink.overflow) return LWB_ERR_BUFFER;
         *n_runs = sink.n_runs;
@@ -1587,10 +1647,15 @@ extern "C" int lwf_packet_decode_vq(const lwf_headers *h, const uint8_t *packet,
 
 extern "C" int lwf_packet_decode(const lwf_headers *h, const uint8_t *packet, size_t len, lwf_decoded_packet *out)
 {
-    if (!h || (!packet && len) || !out || !out->floor_kind || !out->floor1_y || !out->residue) return LWB_ERR_INVALID;
-    for (const auto &fl : h->h.floors)
-        if (fl.type == 0 && !out->dense_floor) return LWB_ERR_INVALID;
-    LWF_GUARD(return lwf::packet_decode(h->h, packet, len, out);)
+    return lwf_packet_decode_ex(h, packet, len, out, 0);
+}
+
+extern "C" int lwf_packet_decode_ex(const lwf_headers *h, const uint8_t *packet, size_t len, lwf_decoded_packet *out, int flags)
+{
+    if (!h || (!packet && len) || !out || !out->floor_kind || !out->floor1_y || !out->residue || (flags & ~LWF_DECODE_FLOOR0_RECORDS))
+        return LWB_ERR_INVALID;
+    if (!out->dense_floor && needs_dense(h->h, flags)) return LWB_ERR_INVALID;
+    LWF_GUARD(return lwf::packet_decode(h->h, packet, len, out, nullptr, (flags & LWF_DECODE_FLOOR0_RECORDS) != 0);)
 }
 
 // get_decoded_sample_count, audio.rs:874-909
@@ -1903,16 +1968,19 @@ struct BatchArena {
     std::vector<lwb_chain> chains;
     std::vector<std::vector<lwb_vq_run>> job_runs;      // LWB_ENTRY_VQ: per-job records before they are packed (kept
     std::vector<std::vector<uint16_t>> job_ents;        // across calls: their capacity is what the next batch needs too)
+    uint64_t in_bytes = 0;                              // bytes of the arrays the slice hands to lwb_decode_chains
 };
 
 struct lwf_batcher {
     lwb_ctx *ctx = nullptr;
     const lwf_headers *hdr = nullptr;
     int threads = 1;
-    bool has_floor0 = false;
+    bool has_floor0 = false;        // the decode can produce dense floor-0 curves: the dense arena is allocated and sent
+    bool floor0_records = false;    // lwf_batcher_set_floor0
     int entry = LWB_ENTRY_RESIDUE;  // LWB_ENTRY_VQ: the residue crosses the boundary as VQ records
     BatchArena arena[2];           // slice i decodes into arena[i & 1] while slice i - 1 is being synthesised
     double t_entropy = 0, t_synth = 0;
+    uint64_t in_bytes = 0;          // of the last lwf_batcher_decode, all slices
 };
 
 extern "C" int lwf_batcher_create(lwb_ctx *ctx, const lwf_headers *h, int threads, lwf_batcher **out)
@@ -1924,7 +1992,7 @@ extern "C" int lwf_batcher_create(lwb_ctx *ctx, const lwf_headers *h, int thread
     b->hdr = h;
     if (threads <= 0) threads = (int)std::thread::hardware_concurrency();
     b->threads = std::max(1, threads);
-    for (const auto &fl : h->h.floors) b->has_floor0 |= fl.type == 0;
+    b->has_floor0 = needs_dense(h->h, 0);
     *out = b;
     return LWB_OK;
 }
@@ -1936,6 +2004,16 @@ extern "C" int lwf_batcher_set_entry(lwf_batcher *b, int entry)
     if (!b || (entry != LWB_ENTRY_RESIDUE && entry != LWB_ENTRY_VQ)) return LWB_ERR_INVALID;
     if (entry == LWB_ENTRY_VQ && !lwf_headers_vq_capable(b->hdr)) return LWB_ERR_INVALID;
     b->entry = entry;
+    return LWB_OK;
+}
+
+extern "C" uint64_t lwf_batcher_last_input_bytes(const lwf_batcher *b) { return b ? b->in_bytes : 0; }
+
+extern "C" int lwf_batcher_set_floor0(lwf_batcher *b, int records)
+{
+    if (!b) return LWB_ERR_INVALID;
+    b->floor0_records = records != 0;
+    b->has_floor0 = needs_dense(b->hdr->h, b->floor0_records ? LWF_DECODE_FLOOR0_RECORDS : 0);
     return LWB_OK;
 }
 
@@ -2030,7 +2108,7 @@ int batch_entropy(lwf_batcher *b, BatchArena &ar, lwf_stream_job *jobs, size_t j
                         sink.run_cap = cap;
                         sink.entries = scratch_ents.data();
                         sink.ent_cap = cap;
-                        rc = lwf::packet_decode(H, job.packets[k], job.lengths[k], &dp, &sink);
+                        rc = lwf::packet_decode(H, job.packets[k], job.lengths[k], &dp, &sink, b->floor0_records);
                         if (!rc && sink.overflow) rc = LWB_ERR_BUFFER;
                         if (!rc) {
                             jr.insert(jr.end(), scratch_runs.data(), scratch_runs.data() + sink.n_runs);
@@ -2039,7 +2117,7 @@ int batch_entropy(lwf_batcher *b, BatchArena &ar, lwf_stream_job *jobs, size_t j
                         run_off[pi + 1] = rc ? 0 : sink.n_runs;      // counts for now; turned into offsets below
                         ent_off[pi + 1] = rc ? 0 : sink.n_ent;
                     } else {
-                        rc = lwf::packet_decode(H, job.packets[k], job.lengths[k], &dp);
+                        rc = lwf::packet_decode(H, job.packets[k], job.lengths[k], &dp, nullptr, b->floor0_records);
                     }
                     if (rc) { dec_status[j] = rc; break; }
                     ar.modes[pi] = dp.mode_number;
@@ -2099,6 +2177,9 @@ int batch_entropy(lwf_batcher *b, BatchArena &ar, lwf_stream_job *jobs, size_t j
         copier();
         for (auto &t : cpool) t.join();
     }
+    // what crosses to the device: residues or VQ records, dense floor-0 curves, floor kinds and floor1_y rows
+    ar.in_bytes = rows + rows * LWB_MAX_POSTS * 4 + (b->has_floor0 ? coeff_total * 4 : 0) +
+                  (vq ? (pkt_total + 1) * 16 + run_off[pkt_total] * sizeof(lwb_vq_run) + ent_off[pkt_total] * 2 : coeff_total * 4);
     // chains of this slice
     ar.chains.assign(j1 - j0, lwb_chain());
     for (size_t j = j0; j < j1; j++) {
@@ -2150,6 +2231,7 @@ extern "C" int lwf_batcher_decode(lwf_batcher *b, lwf_stream_job *jobs, size_t n
         // one caller at a time), the pool already entropy-decodes slice i + 1 into the other arena.
         const size_t n_slices = std::max<size_t>(1, std::min<size_t>(4, n_jobs / 8));
         double entropy_busy = 0, synth_busy = 0;
+        uint64_t in_bytes = 0;
         int synth_rc = LWB_OK, rc = LWB_OK;
         std::thread synth;
         struct Joiner { std::thread &t; ~Joiner() { if (t.joinable()) t.join(); } } joiner{synth};   // also on unwinding
@@ -2161,6 +2243,7 @@ extern "C" int lwf_batcher_decode(lwf_batcher *b, lwf_stream_job *jobs, size_t n
             const double e0 = now_s();
             rc = batch_entropy(b, ar, jobs, j0, j1, plan, decoded, dec_status);
             entropy_busy += now_s() - e0;
+            in_bytes += ar.in_bytes;
             if (synth.joinable()) synth.join();
             if (rc != LWB_OK || synth_rc != LWB_OK) break;
             synth = std::thread([b, &ar, out_format, pcm, jobs, j0, j1, &plan, &decoded, &dec_status, &synth_rc, &synth_busy]() {
@@ -2181,6 +2264,7 @@ extern "C" int lwf_batcher_decode(lwf_batcher *b, lwf_stream_job *jobs, size_t n
         if (synth.joinable()) synth.join();
         b->t_entropy = entropy_busy;
         b->t_synth = synth_busy;
+        b->in_bytes = in_bytes;
         if (rc) return rc;
         return synth_rc;
     )

@@ -59,6 +59,7 @@ struct lwb_ctx {
     std::deque<CachedTables> tables;       // (deque: setups hold copies of dt, growth never moves an entry)
     // grow-only device arenas
     DevBuf spec, segtab, magic, x, desc, chains, ticket, cdesc, cbytes;
+    DevBuf floor0;                 // floor-0 curves of LWB_FLOOR_ZERO rows (k_floor0_curves), laid out like spec
     ArenaSet host_sets[kHostSets]; // host-memory batches, in turn
     int host_next = 0;
     ArenaSet ordered;              // in compute-stream order: device-memory batches' host floor arrays, the debug taps
@@ -86,6 +87,10 @@ struct lwb_setup {
     uint32_t n_modes = 0;
     uint32_t n_mappings = 0;
     std::vector<DevMapping> mappings;   // host copy (validation)
+    std::vector<uint8_t> floor_types;   // LWB_FLOOR_TYPE_* per floor
+    std::vector<DevFloor0> floor0;      // host copy of host.floor0 (empty: no floor-0 description)
+    mutable bool streams_opened = false; // lwb_setup_set_floor0 is refused from then on
+    bool floor0_described(uint32_t fi) const { return fi < floor0.size() && floor0[fi].order != 0; }
 };
 
 struct MixRound { size_t r0, nr, s0, ns, c0, nc, x0, nx, g0, ng, flat, nm; };   // LongRun / ShortRun / ChainDesc / RowCopy / burst-group ranges of one
@@ -103,6 +108,7 @@ struct MixLaunch {
     const float *mpack; int mid_kb;                                     // k_mid
     size_t off_sr, off_cd, off_by, off_rc, off_sg;                      // ShortRun, ChainDesc, mode bytes, RowCopy, bursts in db
     bool residue; ChainShape chain; const float *coeffs, *dense; const uint8_t *kinds; const uint32_t *ys;   // k_chain
+    const float *zero;                                                  // k_chain: curves of LWB_FLOOR_ZERO rows, or nullptr
 };
 
 // One launch of the residue entry's front stages (k_floor1_segments + k_prologue_fused, or k_prologue): floor x
@@ -118,6 +124,7 @@ struct FrontStages {
     uint64_t c_lo = 0;                 // element offset of ctx->spec[0]
     uint64_t r_lo = 0, r_hi = 0;       // packet rows of the floor / VQ arrays
     bool dense = false;                // whether the dense floor arena is passed
+    bool floor0 = false;               // whether k_floor0_curves runs first (the packets may have LWB_FLOOR_ZERO rows)
 };
 
 struct lwb_plan {
@@ -137,18 +144,6 @@ struct lwb_plan {
     std::vector<MixRound> mix_rounds;
 };
 
-// Records the launches a path made for a prepared batch; lwb_plan_execute replays them while ctx->state_gen == gen.
-static void capture(lwb_plan *plan, uint64_t gen, const FrontStages &front, const MixLaunch &ml, std::vector<MixRound> rounds,
-                    uint32_t n_groups = 0)
-{
-    plan->captured = true;
-    plan->gen = gen;
-    plan->front = front;
-    plan->mix_launch = ml;
-    plan->mix_rounds = std::move(rounds);
-    plan->n_groups = n_groups;
-}
-
 struct lwb_stream {
     lwb_ctx *ctx = nullptr;
     const lwb_setup *setup = nullptr;
@@ -157,6 +152,23 @@ struct lwb_stream {
     uint32_t plen = 0;             // per-channel length of the saved right half
     uint64_t busy_epoch = 0;       // guards against one stream appearing twice in a batch
 };
+
+// Records the launches a path made for a prepared batch; lwb_plan_execute replays them while ctx->state_gen == gen.
+static void capture(lwb_plan *plan, uint64_t gen, const FrontStages &front, const MixLaunch &ml, std::vector<MixRound> rounds,
+                    uint32_t n_groups = 0)
+{
+    plan->captured = true;
+    plan->gen = gen;
+    plan->front = front;
+    // Replays upload the host floor arrays of each step without looking at them: a later step may carry floor-0 records
+    // that the captured one did not, so the floor-0 curves run whenever a chain's setup can serve records.
+    for (size_t i = 0; i < plan->n_chains && front.n; i++)
+        if (!plan->chains[i].stream->setup->floor0.empty()) plan->front.floor0 = true;
+    plan->mix_launch = ml;
+    plan->mix_rounds = std::move(rounds);
+    plan->n_groups = n_groups;
+}
+
 
 static inline void set_stream_state(lwb_stream *s, bool has, uint32_t plen)
 {

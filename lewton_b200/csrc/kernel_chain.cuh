@@ -6,7 +6,8 @@
 // The group keeps its channel's working buffers (U, V: n/2 floats each) and the previous block's right half
 // (PreviousWindowRight, audio.rs:847-861) in shared memory for the whole chain, so HBM sees only the
 // algorithmic traffic: coefficients in, PCM out, the stream state once per chain.  Per packet:
-//   residue entry: floor-1 posts per channel (one lane, serial, <= 65 posts) -> the whole CTA does
+//   residue entry: floor-1 posts per channel (one lane, serial, <= 65 posts; floor-0 curves come rendered by
+//                  k_floor0_curves) -> the whole CTA does
 //                  inverse coupling + floor x residue bin-parallel straight into the channels'
 //                  shared buffers (audio.rs:991-1039);
 //   every warp:    inverse MDCT stage by stage in shared memory (imdct.rs:291-659, literal schedule),
@@ -63,7 +64,8 @@ template <int FORMAT, int ENTRY, bool MULTI>
 __global__ void __launch_bounds__(MULTI ? 1024 : 256)
 k_chain(const ChainDesc *__restrict__ chains, const uint8_t *__restrict__ pkt_bytes, const float *__restrict__ coeffs,
         const float *__restrict__ dense_floor, const uint8_t *__restrict__ floor_kind,
-        const uint32_t *__restrict__ floor1_y, void *__restrict__ pcm, int n1max, int wpc, int np)
+        const uint32_t *__restrict__ floor1_y, void *__restrict__ pcm, int n1max, int wpc, int np,
+        const float *__restrict__ zero_floor)
 {
     extern __shared__ float ch_smem[];
     const ChainDesc cd = chains[blockIdx.x];
@@ -132,12 +134,10 @@ k_chain(const ChainDesc *__restrict__ chains, const uint8_t *__restrict__ pkt_by
                 for (int c = 0; c < 8; c++) {
                     if (c < C) {
                         const int kind = floor_kind[row + c];
-                        float f = 0.f;                          // audio.rs:1021-1024
-                        if (kind == LWB_FLOOR_ONE)
-                            f = c_inverse_db[d_floor1_y_at(s_x + c * (LWB_MAX_POSTS + 1), s_y + c * (LWB_MAX_POSTS + 1),
-                                                           s_m[c], k) & 255u];
-                        else if (kind == LWB_FLOOR_DENSE)
-                            f = dense_floor[coeff + (size_t)c * n2 + k];
+                        const float f = kind == LWB_FLOOR_ONE
+                                            ? c_inverse_db[d_floor1_y_at(s_x + c * (LWB_MAX_POSTS + 1), s_y + c * (LWB_MAX_POSTS + 1),
+                                                                         s_m[c], k) & 255u]
+                                            : d_floor_other(kind, dense_floor, zero_floor, coeff + (size_t)c * n2 + k);
                         ch_smem[(size_t)c * per_warp + k] = __fmul_rn(f, r[c]);      // channel c's U
                     }
                 }

@@ -7,7 +7,8 @@
 //                       (floor1_eval.cuh: Seg4, division-free closed form of render_line, audio.rs:503-524);
 //   k_prologue_fused  : one CTA per packet, one thread per 4 bins, all channels: the rows' segment tables and a
 //                       bin -> segment bitmap in shared memory, floor value per bin (closed form -> dB table,
-//                       audio.rs:552-554; unused floor = zero curve, :1021-1024; dense = host-computed floor-0),
+//                       audio.rs:552-554; unused floor = zero curve, :1021-1024; dense = host-computed floor-0;
+//                       zero = floor-0 curve computed by k_floor0_curves),
 //                       inverse coupling in registers / shared memory (steps in reverse, audio.rs:991-1002),
 //                       multiply (:1035-1037), float4 loads and stores.  The kernel is HBM-bound (4 B in + 4 B out per
 //                       coefficient); the per-bin floor arithmetic rides in its idle issue slots.
@@ -190,13 +191,15 @@ __device__ __forceinline__ float4 d_floor_quad_one(const float *__restrict__ s_d
     }
     return make_float4(f[0], f[1], f[2], f[3]);
 }
+// zero: the curves k_floor0_curves rendered for LWB_FLOOR_ZERO rows, or nullptr (such rows then act as unused)
 __device__ __forceinline__ float4 d_floor_quad(int kind, int cnt, const float *__restrict__ s_db, const uint4 *__restrict__ tab,
                                                const unsigned char *__restrict__ ix, int words, int k0,
-                                               const float *__restrict__ dense, uint64_t e)
+                                               const float *__restrict__ dense, const float *__restrict__ zero, uint64_t e)
 {
     if (kind == LWB_FLOOR_ONE && (cnt & 0x7f))
         return (cnt & 0x80) ? d_floor_quad_one<true>(s_db, tab, ix, words, k0) : d_floor_quad_one<false>(s_db, tab, ix, words, k0);
     if (kind == LWB_FLOOR_DENSE) return *reinterpret_cast<const float4 *>(dense + e);
+    if (kind == LWB_FLOOR_ZERO && zero) return *reinterpret_cast<const float4 *>(zero + e);
     return make_float4(0.f, 0.f, 0.f, 0.f);                       // audio.rs:1021-1024
 }
 
@@ -212,7 +215,7 @@ constexpr bool PF_SERIAL = LWB_PF_SERIAL != 0;
 template <bool VQ>
 __global__ void __launch_bounds__(kPfThreads, 4)
 k_prologue_fused(const DevPacket *__restrict__ pkts, uint32_t n_pk, const float *__restrict__ residue, const float *__restrict__ dense_floor,
-                 const uint8_t *__restrict__ floor_kind, const uint4 *__restrict__ segtab, const uint8_t *__restrict__ seg_cnt,
+                 const float *__restrict__ zero_floor, const uint8_t *__restrict__ floor_kind, const uint4 *__restrict__ segtab, const uint8_t *__restrict__ seg_cnt,
                  const unsigned char *__restrict__ seg_index, int words, float *__restrict__ spec,
                  VqDev vq)
 {
@@ -287,11 +290,11 @@ k_prologue_fused(const DevPacket *__restrict__ pkts, uint32_t n_pk, const float 
                             d_inverse_couple(r0.z, r1.z); d_inverse_couple(r0.w, r1.w);
                         }
                     }
-                    const float4 f0 = d_floor_quad(h.k0, h.c0, s_db, t0, x0, words, 4 * q, dense_floor, e0);
+                    const float4 f0 = d_floor_quad(h.k0, h.c0, s_db, t0, x0, words, 4 * q, dense_floor, zero_floor, e0);
                     __stcs(reinterpret_cast<float4 *>(spec + e0),
                            make_float4(__fmul_rn(f0.x, r0.x), __fmul_rn(f0.y, r0.y), __fmul_rn(f0.z, r0.z), __fmul_rn(f0.w, r0.w)));
                     if (C == 2) {
-                        const float4 f1 = d_floor_quad(h.k1, h.c1, s_db, t1, x1, words, 4 * q, dense_floor, e1);
+                        const float4 f1 = d_floor_quad(h.k1, h.c1, s_db, t1, x1, words, 4 * q, dense_floor, zero_floor, e1);
                         __stcs(reinterpret_cast<float4 *>(spec + e1),
                                make_float4(__fmul_rn(f1.x, r1.x), __fmul_rn(f1.y, r1.y), __fmul_rn(f1.z, r1.z), __fmul_rn(f1.w, r1.w)));
                     }
@@ -309,8 +312,8 @@ k_prologue_fused(const DevPacket *__restrict__ pkts, uint32_t n_pk, const float 
                         d_inverse_couple(m4.x, a4.x); d_inverse_couple(m4.y, a4.y);
                         d_inverse_couple(m4.z, a4.z); d_inverse_couple(m4.w, a4.w);
                     }
-                    const float4 f0 = d_floor_quad(h.k0, h.c0, s_db, t0, x0, words, 4 * q, dense_floor, e0);
-                    const float4 f1 = d_floor_quad(h.k1, h.c1, s_db, t1, x1, words, 4 * q, dense_floor, e1);
+                    const float4 f0 = d_floor_quad(h.k0, h.c0, s_db, t0, x0, words, 4 * q, dense_floor, zero_floor, e0);
+                    const float4 f1 = d_floor_quad(h.k1, h.c1, s_db, t1, x1, words, 4 * q, dense_floor, zero_floor, e1);
                     *reinterpret_cast<float4 *>(spec + e0) =
                         make_float4(__fmul_rn(f0.x, v[0].x), __fmul_rn(f0.y, v[0].y), __fmul_rn(f0.z, v[0].z), __fmul_rn(f0.w, v[0].w));
                     *reinterpret_cast<float4 *>(spec + e1) =
@@ -375,11 +378,11 @@ k_prologue_fused(const DevPacket *__restrict__ pkts, uint32_t n_pk, const float 
                         d_inverse_couple(r0.z, r1.z); d_inverse_couple(r0.w, r1.w);
                     }
                 }
-                const float4 f0 = d_floor_quad(k0, c0, s_db, t0, x0, words, 4 * q, dense_floor, e0);
+                const float4 f0 = d_floor_quad(k0, c0, s_db, t0, x0, words, 4 * q, dense_floor, zero_floor, e0);
                 *reinterpret_cast<float4 *>(spec + e0) =
                     make_float4(__fmul_rn(f0.x, r0.x), __fmul_rn(f0.y, r0.y), __fmul_rn(f0.z, r0.z), __fmul_rn(f0.w, r0.w));
                 if (C == 2) {
-                    const float4 f1 = d_floor_quad(k1, c1, s_db, t1, x1, words, 4 * q, dense_floor, e1);
+                    const float4 f1 = d_floor_quad(k1, c1, s_db, t1, x1, words, 4 * q, dense_floor, zero_floor, e1);
                     *reinterpret_cast<float4 *>(spec + e1) =
                         make_float4(__fmul_rn(f1.x, r1.x), __fmul_rn(f1.y, r1.y), __fmul_rn(f1.z, r1.z), __fmul_rn(f1.w, r1.w));
                 }
@@ -404,7 +407,7 @@ k_prologue_fused(const DevPacket *__restrict__ pkts, uint32_t n_pk, const float 
                 const uint64_t ec = e + (uint64_t)c * n2;
                 const float4 r = s_r[c * kPfThreads + tid];
                 const float4 f = d_floor_quad(kinds[c], seg_cnt[row0 + c], s_db, reinterpret_cast<const uint4 *>(pf_smem + c * rowb),
-                                              pf_smem + c * rowb + (size_t)tab_q * 16, words, 4 * q, dense_floor, ec);
+                                              pf_smem + c * rowb + (size_t)tab_q * 16, words, 4 * q, dense_floor, zero_floor, ec);
                 *reinterpret_cast<float4 *>(spec + ec) =
                     make_float4(__fmul_rn(f.x, r.x), __fmul_rn(f.y, r.y), __fmul_rn(f.z, r.z), __fmul_rn(f.w, r.w));
             }

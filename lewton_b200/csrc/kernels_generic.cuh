@@ -44,11 +44,20 @@ constexpr int kPrologueGroup = 8;            // channels whose floor posts sit i
 // dynamic shared memory of k_prologue: one curve byte per bin for up to 8 channels of the largest block
 inline size_t prologue_smem(int channels, int blocksize_1) { return (size_t)(channels < kPrologueGroup ? channels : kPrologueGroup) << (blocksize_1 - 1); }
 
+// The floor value of a row of kind `kind` (not LWB_FLOOR_ONE) at coefficient element e: the host's dense curve, the
+// curve k_floor0_curves rendered (zero_floor; nullptr: the row acts as unused), or 0 (audio.rs:1021-1024).
+__device__ __forceinline__ float d_floor_other(int kind, const float *__restrict__ dense_floor, const float *__restrict__ zero_floor, uint64_t e)
+{
+    if (kind == LWB_FLOOR_DENSE) return dense_floor[e];
+    if (kind == LWB_FLOOR_ZERO && zero_floor) return zero_floor[e];
+    return 0.f;
+}
+
 // grid.x = packets.  spec[packet] = [channels][n/2] receives floor x decoupled residue.
 __global__ void __launch_bounds__(kPrologueThreads)
 k_prologue(const DevPacket *__restrict__ pkts, const float *__restrict__ residue,
            const float *__restrict__ dense_floor, const uint8_t *__restrict__ floor_kind,
-           const uint32_t *__restrict__ floor1_y, float *__restrict__ spec)
+           const uint32_t *__restrict__ floor1_y, float *__restrict__ spec, const float *__restrict__ zero_floor)
 {
     const DevPacket &p = pkts[blockIdx.x];
     const DevSetup &su = *p.setup;
@@ -93,11 +102,9 @@ k_prologue(const DevPacket *__restrict__ pkts, const float *__restrict__ residue
                     if (swapped) d_inverse_couple(r1, r0);
                     else d_inverse_couple(r0, r1);
                 }
-                float f0 = 0.f, f1 = 0.f;                              // audio.rs:1021-1024
-                if (k0 == LWB_FLOOR_ONE) f0 = c_inverse_db[s_curve[k]];
-                else if (k0 == LWB_FLOOR_DENSE) f0 = dense_floor[p.coeff_off + k];
-                if (k1 == LWB_FLOOR_ONE) f1 = c_inverse_db[s_curve[(size_t)n2 + k]];
-                else if (k1 == LWB_FLOOR_DENSE) f1 = dense_floor[p.coeff_off + (size_t)n2 + k];
+                const float f0 = k0 == LWB_FLOOR_ONE ? c_inverse_db[s_curve[k]] : d_floor_other(k0, dense_floor, zero_floor, p.coeff_off + k);
+                const float f1 = k1 == LWB_FLOOR_ONE ? c_inverse_db[s_curve[(size_t)n2 + k]]
+                                                     : d_floor_other(k1, dense_floor, zero_floor, p.coeff_off + (size_t)n2 + k);
                 out[k] = __fmul_rn(f0, r0);                            // audio.rs:1035-1037
                 out[(size_t)n2 + k] = __fmul_rn(f1, r1);
             }
@@ -120,9 +127,8 @@ k_prologue(const DevPacket *__restrict__ pkts, const float *__restrict__ residue
             for (int c = 0; c < 8; c++) {
                 if (c < C) {
                     const int kind = kinds[c];
-                    float f = 0.f;
-                    if (kind == LWB_FLOOR_ONE) f = c_inverse_db[s_curve[(size_t)c * n2 + k]];
-                    else if (kind == LWB_FLOOR_DENSE) f = dense_floor[p.coeff_off + (size_t)c * n2 + k];
+                    const float f = kind == LWB_FLOOR_ONE ? c_inverse_db[s_curve[(size_t)c * n2 + k]]
+                                                          : d_floor_other(kind, dense_floor, zero_floor, p.coeff_off + (size_t)c * n2 + k);
                     out[(size_t)c * n2 + k] = __fmul_rn(f, r[c]);
                 }
             }
@@ -159,13 +165,8 @@ k_prologue(const DevPacket *__restrict__ pkts, const float *__restrict__ residue
             const int kind = kinds[c];
             float *oc = out + (size_t)c * n2;
             for (int k = threadIdx.x; k < n2; k += kPrologueThreads) {
-                float f;
-                if (kind == LWB_FLOOR_ONE)
-                    f = c_inverse_db[d_floor1_y_at(s_x[g], s_y[g], s_m[g], k) & 255u];
-                else if (kind == LWB_FLOOR_DENSE)
-                    f = dense_floor[p.coeff_off + (size_t)c * n2 + k];
-                else
-                    f = 0.f;                           // audio.rs:1021-1024
+                const float f = kind == LWB_FLOOR_ONE ? c_inverse_db[d_floor1_y_at(s_x[g], s_y[g], s_m[g], k) & 255u]
+                                                      : d_floor_other(kind, dense_floor, zero_floor, p.coeff_off + (size_t)c * n2 + k);
                 oc[k] = __fmul_rn(f, oc[k]);           // audio.rs:1035-1037
             }
         }

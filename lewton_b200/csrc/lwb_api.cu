@@ -25,13 +25,19 @@
 #include "kernels_generic.cuh"
 #include "kernel_chain.cuh"
 #include "kernel_prologue.cuh"
+#include "kernel_floor0.cuh"
 #include "lwb_common.h"
 #include "pcm_copy_plan.h"
+#include "../../include/lewton_frontend.h"
 
 namespace lwb {
 int generate_tables(int bs, float *a, float *b, float *c, float *window, uint32_t *bitrev);
 int prepare_floor1(const lwb_floor_desc &d, DevFloor1 *out);
 }  // namespace lwb
+namespace lwf {
+std::vector<float> bark_map_cos_omega(uint16_t n, uint16_t rate, uint16_t bark_map_size);   // frontend.cpp
+void floor0_descs(const lwf_headers *h, std::vector<uint32_t> *index, std::vector<lwb_floor0_desc> *descs);
+}  // namespace lwf
 
 using namespace lwb;
 
@@ -105,7 +111,7 @@ extern "C" void lwb_ctx_destroy(lwb_ctx *ctx)
     cudaSetDevice(ctx->device);
     sync_all_streams(ctx);
     for (DevBuf *b : {&ctx->spec, &ctx->segtab, &ctx->magic, &ctx->x, &ctx->desc, &ctx->chains, &ctx->ticket, &ctx->runs_buf[0],
-                      &ctx->runs_buf[1], &ctx->cdesc, &ctx->cbytes})
+                      &ctx->runs_buf[1], &ctx->cdesc, &ctx->cbytes, &ctx->floor0})
         if (b->p) cudaFree(b->p);
     auto free_set = [](ArenaSet &s) {
         for (DevBuf *b : {&s.coeffs, &s.dense, &s.pcm, &s.kinds, &s.ys, &s.vqoff, &s.vqrec})
@@ -368,6 +374,7 @@ extern "C" int lwb_setup_create(lwb_ctx *ctx, const lwb_setup_desc *d, lwb_setup
     }
     std::vector<DevFloor1> floors(d->n_floors);
     for (uint32_t i = 0; i < d->n_floors && rc == LWB_OK; i++) rc = prepare_floor1(d->floors[i], &floors[i]);
+    for (uint32_t i = 0; i < d->n_floors; i++) su->floor_types.push_back(d->floors[i].floor_type);
     su->mappings.resize(d->n_mappings);
     for (uint32_t i = 0; i < d->n_mappings && rc == LWB_OK; i++) {
         const lwb_mapping_desc &m = d->mappings[i];
@@ -445,6 +452,73 @@ extern "C" int lwb_setup_create(lwb_ctx *ctx, const lwb_setup_desc *d, lwb_setup
     return LWB_OK;
 }
 
+extern "C" int lwb_setup_set_floor0(lwb_setup *su, uint32_t fi, const lwb_floor0_desc *d)
+{
+    if (!su || !d) return LWB_ERR_INVALID;
+    lwb_ctx *ctx = su->ctx;
+    if (fi >= su->floor_types.size() || su->floor_types[fi] != LWB_FLOOR_TYPE_ZERO)
+        return fail(ctx, LWB_ERR_INVALID, "set_floor0: no type-0 floor at that index");
+    if (d->order < 2 || d->order > LWB_MAX_POSTS - 2 || d->amplitude_bits < 1 || d->amplitude_bits > 64 || !d->rate || !d->bark_map_size)
+        return fail(ctx, LWB_ERR_INVALID, "set_floor0: order must be 2..63, amplitude_bits 1..64, rate and bark_map_size nonzero");
+    // Streams (and the batches and plans built on them) read the setup's description as it was: it is fixed from then on.
+    if (su->streams_opened) return fail(ctx, LWB_ERR_INVALID, "set_floor0: the setup already has streams");
+    CU(ctx, cudaSetDevice(ctx->device));
+    // a floor described again: its earlier tables and the earlier description array go
+    auto release = [&](const void *p) {
+        auto it = std::find(su->allocs.begin(), su->allocs.end(), p);
+        if (p && it != su->allocs.end()) {
+            cudaFree(*it);
+            su->allocs.erase(it);
+        }
+    };
+    DevFloor0 f;
+    std::memset(&f, 0, sizeof(f));
+    f.order = d->order;
+    f.amplitude_offset = d->amplitude_offset;
+    f.max_amp = d_floor0_max_amp(d->amplitude_bits);
+    for (int i = 0; i < 2; i++) {
+        const uint16_t n2 = (uint16_t)(1u << ((i ? su->bs1 : su->bs0) - 1));
+        std::vector<float> bark = d->bark_cos_omega[i] ? std::vector<float>(d->bark_cos_omega[i], d->bark_cos_omega[i] + n2)
+                                                       : lwf::bark_map_cos_omega(n2, d->rate, d->bark_map_size);
+        int rc = upload(su, bark.data(), bark.size(), &f.bark_cos_omega[i]);
+        if (rc) return rc;
+        CU(ctx, cudaStreamSynchronize(ctx->stream));              // (the copy reads `bark`)
+    }
+    if (su->floor0.empty()) su->floor0.assign(su->floor_types.size(), DevFloor0{});
+    release(su->floor0[fi].bark_cos_omega[0]);
+    release(su->floor0[fi].bark_cos_omega[1]);
+    release(su->host.floor0);
+    su->floor0[fi] = f;
+    const DevFloor0 *dev = nullptr;
+    int rc = upload(su, su->floor0.data(), su->floor0.size(), &dev);
+    if (rc) return rc;
+    su->host.floor0 = dev;
+    CU(ctx, cudaMemcpyAsync(su->d_setup, &su->host, sizeof(su->host), cudaMemcpyHostToDevice, ctx->stream));
+    CU(ctx, cudaStreamSynchronize(ctx->stream));
+    return LWB_OK;
+}
+
+// The front half's setup with its record-capable type-0 floors described (here, beside lwb_setup_set_floor0: the front
+// half alone builds without the synthesis library).
+extern "C" int lwf_headers_make_setup_floor0(const lwf_headers *h, lwb_ctx *ctx, lwb_setup **out)
+{
+    int rc = lwf_headers_make_setup(h, ctx, out);
+    if (rc) return rc;
+    std::vector<uint32_t> index;
+    std::vector<lwb_floor0_desc> descs;
+    try {
+        lwf::floor0_descs(h, &index, &descs);
+    } catch (...) {
+        rc = LWB_ERR_BUFFER;
+    }
+    for (size_t i = 0; i < descs.size() && !rc; i++) rc = lwb_setup_set_floor0(*out, index[i], &descs[i]);
+    if (rc) {
+        lwb_setup_destroy(*out);
+        *out = nullptr;
+    }
+    return rc;
+}
+
 // ---------------------------------------------------------------------------------------------
 // stream state
 // ---------------------------------------------------------------------------------------------
@@ -456,6 +530,7 @@ extern "C" int lwb_stream_open(lwb_ctx *ctx, const lwb_setup *su, lwb_stream **o
     CU(ctx, cudaSetDevice(ctx->device));
     lwb_stream *s = new (std::nothrow) lwb_stream();
     if (!s) return LWB_ERR_BUFFER;
+    su->streams_opened = true;
     s->ctx = ctx;
     s->setup = su;
     cudaError_t e = cudaMalloc((void **)&s->d_state, su->channels * state_stride(su) * sizeof(float));
@@ -613,7 +688,7 @@ static int queue_batch(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const l
     if ((rc = ext.finish(ctx, io))) return rc;
     if (!ext.empty()) {
         BatchArenas ar;
-        if ((rc = ar.open(ctx, io, ext, C, false)) || (rc = ar.upload(0, ext)) || (rc = run_generic(ctx, plan, io, ar)) ||
+        if ((rc = ar.open(ctx, io, ext, C, false)) || (rc = ar.upload(0, ext)) || (rc = run_generic(ctx, plan, io, ar, ext.need_floor0)) ||
             (rc = ar.download(0, chains, 0, n_chains, ext)) || (rc = ar.finish()))
             return rc;
     }
@@ -798,14 +873,18 @@ extern "C" int lwb_debug_packet_taps(lwb_stream *s, const lwb_packet *pkt, float
     if (rc) return rc;
     CU(ctx, cudaSetDevice(ctx->device));
     const size_t C = su->channels, n2 = g.n >> 1;
-    bool need_dense = false, need_y = false;
+    bool need_dense = false, need_y = false, need_floor0 = false;
     for (size_t c = 0; c < C; c++) {
-        if (pkt->floor_kind[c] > LWB_FLOOR_DENSE) return LWB_ERR_INVALID;
-        need_dense |= pkt->floor_kind[c] == LWB_FLOOR_DENSE;
-        need_y |= pkt->floor_kind[c] == LWB_FLOOR_ONE;
+        const uint8_t kd = pkt->floor_kind[c];
+        if (kd > LWB_FLOOR_ZERO) return LWB_ERR_INVALID;
+        if (kd == LWB_FLOOR_ZERO && !su->floor0_described(su->mappings[g.mapping].floor_of_channel[c])) return LWB_ERR_INVALID;
+        need_dense |= kd == LWB_FLOOR_DENSE;
+        need_y |= kd == LWB_FLOOR_ONE || kd == LWB_FLOOR_ZERO;
+        need_floor0 |= kd == LWB_FLOOR_ZERO;
     }
     if ((need_dense && !pkt->dense_floor) || (need_y && !pkt->floor1_y)) return LWB_ERR_INVALID;
-    if ((rc = ensure(ctx, ctx->ordered.coeffs, C * n2 * 4)) || (rc = ensure(ctx, ctx->spec, C * n2 * 4)) ||
+    if ((need_floor0 && (rc = ensure(ctx, ctx->floor0, C * n2 * 4))) ||
+        (rc = ensure(ctx, ctx->ordered.coeffs, C * n2 * 4)) || (rc = ensure(ctx, ctx->spec, C * n2 * 4)) ||
         (rc = ensure(ctx, ctx->x, C * g.n * 4)) || (rc = ensure(ctx, ctx->ordered.kinds, C)) ||
         (rc = ensure(ctx, ctx->ordered.ys, C * LWB_MAX_POSTS * 4)) || (rc = ensure(ctx, ctx->ordered.dense, C * n2 * 4)) ||
         (rc = ensure(ctx, ctx->desc, sizeof(DevPacket))) || (rc = ensure_pinned(ctx, sizeof(DevPacket))))
@@ -841,7 +920,7 @@ extern "C" int lwb_debug_packet_taps(lwb_stream *s, const lwb_packet *pkt, float
         CU(ctx, cudaMemcpyAsync(tmp_kinds, kd.data(), C, cudaMemcpyHostToDevice, st));
         rc = launch(ctx, LWB_KERNEL_PROLOGUE, k_prologue, dim3(1), dim3(kPrologueThreads), prologue_smem(su->channels, su->bs1), dp, (const float *)ctx->ordered.coeffs.p,
                     (const float *)tmp_dense, (const uint8_t *)tmp_kinds, (const uint32_t *)ctx->ordered.ys.p,
-                    (float *)ctx->spec.p);
+                    (float *)ctx->spec.p, (const float *)nullptr);
         if (!rc) {
             cudaError_t e = cudaMemcpyAsync(post_inverse, ctx->spec.p, C * n2 * 4, cudaMemcpyDeviceToHost, st);
             if (e == cudaSuccess) e = cudaStreamSynchronize(st);
@@ -851,9 +930,12 @@ extern "C" int lwb_debug_packet_taps(lwb_stream *s, const lwb_packet *pkt, float
         cudaFree(tmp_kinds);
         if (rc) return rc;
     }
+    float *zero = need_floor0 ? (float *)ctx->floor0.p : nullptr;
+    if (zero && (rc = launch_floor0_curves(ctx, dp, 1, (unsigned)C, (const uint8_t *)ctx->ordered.kinds.p, (const uint32_t *)ctx->ordered.ys.p, zero)))
+        return rc;
     if ((rc = launch(ctx, LWB_KERNEL_PROLOGUE, k_prologue, dim3(1), dim3(kPrologueThreads), prologue_smem(su->channels, su->bs1), dp, (const float *)ctx->ordered.coeffs.p,
                      (const float *)ctx->ordered.dense.p, (const uint8_t *)ctx->ordered.kinds.p, (const uint32_t *)ctx->ordered.ys.p,
-                     (float *)ctx->spec.p)))
+                     (float *)ctx->spec.p, (const float *)zero)))
         return rc;
     if (pre_mdct) CU(ctx, cudaMemcpyAsync(pre_mdct, ctx->spec.p, C * n2 * 4, cudaMemcpyDeviceToHost, st));
     if (post_mdct) {

@@ -54,9 +54,18 @@ struct DevBook {              // Codebook (header.rs:360-368): the value table o
 };
 constexpr int kMaxResidues = 64;      // header.rs:973 residue count = read_u6 + 1
 
+struct DevFloor0 {            // FloorTypeZero (header.rs:399-407) as lwb_setup_set_floor0 describes it; order 0 = none
+    const float *bark_cos_omega[2];   // cached_bark_cos_omega of blocksize_0 / blocksize_1: n/2 floats each
+    float max_amp;            // (1 << amplitude_bits) - 1 as f32 (audio.rs:167-169)
+    uint8_t order;            // floor0_order, 2..63
+    uint8_t amplitude_offset;
+    uint8_t pad[2];
+};
+
 struct DevSetup {
     DevTables tab[2];
     const DevFloor1 *floors;
+    const DevFloor0 *floor0;  // [n_floors], or nullptr: no floor of the setup has a floor-0 description
     const DevMapping *mappings;
     uint8_t channels, bs0, bs1, n_floors;
     uint8_t mode_blockflag[LWB_MAX_MODES];

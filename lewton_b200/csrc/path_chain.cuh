@@ -32,18 +32,18 @@ static ChainShape chain_shape(unsigned maxc, int n1max, bool residue)
 template <int ENTRY>
 static int launch_chain(lwb_ctx *ctx, int fmt, unsigned n_chains, unsigned warps, size_t smem, const ChainDesc *d,
                         const uint8_t *bytes, const float *coeffs, const float *dense, const uint8_t *kinds,
-                        const uint32_t *ys, void *pcm, int n1max, int wpc, int np)
+                        const uint32_t *ys, void *pcm, int n1max, int wpc, int np, const float *zero)
 {
 #define LWB_CHAIN_CASE(F)                                                                                    \
     case F:                                                                                                  \
         if (wpc == 1) {                                                                                      \
             cudaFuncSetAttribute(k_chain<F, ENTRY, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
             return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, false>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, \
-                          kinds, ys, pcm, n1max, wpc, np);                                                    \
+                          kinds, ys, pcm, n1max, wpc, np, zero);                                              \
         }                                                                                                    \
         cudaFuncSetAttribute(k_chain<F, ENTRY, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
         return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, true>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, kinds, \
-                      ys, pcm, n1max, wpc, 1);
+                      ys, pcm, n1max, wpc, 1, zero);
     switch (fmt) {
         LWB_CHAIN_CASE(LWB_OUT_F32_PLANAR)
         LWB_CHAIN_CASE(LWB_OUT_I16_PLANAR)
@@ -105,14 +105,36 @@ static int mixed_launch_rounds(lwb_ctx *ctx, const MixLaunch &ml, const std::vec
             const uint8_t *dby = (const uint8_t *)(ml.db + ml.off_by);
             if (ml.residue)
                 rc = launch_chain<LWB_ENTRY_RESIDUE>(ctx, ml.out_format, (unsigned)rd.nc, ml.chain.warps, ml.chain.smem, dcd, dby, ml.coeffs, ml.dense,
-                                                     ml.kinds, ml.ys, ml.pcm, ml.chain.n1max, ml.chain.wpc, ml.chain.np);
+                                                     ml.kinds, ml.ys, ml.pcm, ml.chain.n1max, ml.chain.wpc, ml.chain.np, ml.zero);
             else
                 rc = launch_chain<LWB_ENTRY_SPECTRUM>(ctx, ml.out_format, (unsigned)rd.nc, ml.chain.warps, ml.chain.smem, dcd, dby, ml.coeffs, ml.dense,
-                                                      ml.kinds, ml.ys, ml.pcm, ml.chain.n1max, ml.chain.wpc, ml.chain.np);
+                                                      ml.kinds, ml.ys, ml.pcm, ml.chain.n1max, ml.chain.wpc, ml.chain.np, ml.zero);
             if (rc) return rc;
         }
     }
     return LWB_OK;
+}
+
+// k_floor0_curves over the decoded packets of a residue-entry batch the chain kernel takes: *zero addresses the curves by
+// absolute coefficient offset.  The packet list goes to ctx->desc, which only work queued on the compute stream uses.
+static int chain_floor0_curves(lwb_ctx *ctx, const BatchArenas &ar, const BatchExtent &ext, const lwb_chain *chains, size_t n_chains,
+                               const std::vector<ChainWalk> &walks, float **zero)
+{
+    size_t n_pk = 0;
+    for (size_t i = 0; i < n_chains; i++) n_pk += walks[i].done;
+    Staging *st;
+    int rc;
+    if ((rc = acquire_staging(ctx, n_pk * sizeof(DevPacket), &st)) || (rc = ensure(ctx, ctx->desc, n_pk * sizeof(DevPacket))) ||
+        (rc = ensure(ctx, ctx->floor0, (size_t)(ext.c_hi - ext.c_lo) * sizeof(float))))
+        return rc;
+    DevPacket *hp = (DevPacket *)st->h, *w = hp;
+    for (size_t i = 0; i < n_chains; i++) {
+        write_front_packets(&chains[i], 0, walks[i].done, chains[i].coeff_offset, w);
+        w += walks[i].done;
+    }
+    if ((rc = upload_staging(ctx, st, hp, ctx->desc.p, n_pk * sizeof(DevPacket), ctx->stream))) return rc;
+    *zero = (float *)ctx->floor0.p - ext.c_lo;
+    return launch_floor0_curves(ctx, (const DevPacket *)ctx->desc.p, n_pk, ar.C, ar.fl.kinds, ar.fl.ys, *zero);
 }
 
 static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, bool *handled, lwb_plan *plan)
@@ -183,8 +205,11 @@ static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         if ((rc = upload_staging(ctx, st, hd, dbuf.p, used_desc, sm)) ||
             (rc = upload_staging(ctx, st, hb, (char *)dbuf.p + used_desc, boff + 16, sm)))
             return rc;
+        // residue entry with floor-0 records: their curves first, by absolute coefficient offset like ar.coeffs
+        float *zero = nullptr;
+        if (residue && ext.need_floor0 && ar.fl.ys && (rc = chain_floor0_curves(ctx, ar, ext, chains, n_chains, walks, &zero))) return rc;
         const MixLaunch ml{(char *)dbuf.p, ar.pcm, io->out_format, false, nullptr, 0, nullptr, nullptr, nullptr, 0, 0, 0, used_desc, 0, 0,
-                           residue, chain_shape(maxc, n1max, residue), ar.coeffs, ar.dense, ar.fl.kinds, ar.fl.ys};
+                           residue, chain_shape(maxc, n1max, residue), ar.coeffs, ar.dense, ar.fl.kinds, ar.fl.ys, zero};
         std::vector<MixRound> rounds(1, MixRound{0, 0, 0, 0, 0, n_launch});
         if ((rc = mixed_launch_rounds(ctx, ml, rounds))) return rc;
         if (cap) capture(plan, gen_at_entry, FrontStages(), ml, std::move(rounds));

@@ -138,21 +138,42 @@ static bool prologue_is_fast(const DevPacket *h_pk, size_t n_pk, unsigned C, con
 // VQ views of a batch (LWB_ENTRY_VQ), device pointers biased like the floor arrays; runs == nullptr otherwise
 struct VqView { const lwb_vq_run *runs = nullptr; const uint64_t *run_off = nullptr; const uint16_t *entries = nullptr; const uint64_t *ent_off = nullptr; };
 
-// n2max: the largest n/2 among the packets (sizes the per-row bin -> segment index).
+// The curves of the LWB_FLOOR_ZERO rows of n_pk packets with C channels into `curves` (addressed like the coefficient
+// arena of the packets' coeff_off).
+static int launch_floor0_curves(lwb_ctx *ctx, const DevPacket *d_pk, size_t n_pk, unsigned C, const uint8_t *kinds, const uint32_t *ys,
+                                float *curves)
+{
+    const size_t rows = n_pk * C;
+    if (!rows) return LWB_OK;
+    return launch(ctx, LWB_KERNEL_FLOOR0_CURVES, k_floor0_curves, dim3((unsigned)((rows + kF0Rows - 1) / kF0Rows)), dim3(kF0Threads), 0, d_pk,
+                  (uint32_t)rows, (int)C, kinds, ys, curves);
+}
+
+// n2max: the largest n/2 among the packets (sizes the per-row bin -> segment index).  floor0: the packets may have
+// LWB_FLOOR_ZERO rows -- their curves are computed first, into ctx->floor0 at the offsets `spec` has in ctx->spec; without
+// it (or without floor1_y) such rows act as LWB_FLOOR_UNUSED.
 static int launch_prologue(lwb_ctx *ctx, const DevPacket *d_pk, size_t n_pk, unsigned C, bool fast, size_t smem_old, int n2max,
-                           const float *res, const float *dense, const uint8_t *kinds, const uint32_t *ys, float *spec, VqView vq = VqView())
+                           const float *res, const float *dense, const uint8_t *kinds, const uint32_t *ys, float *spec, VqView vq = VqView(),
+                           bool floor0 = false)
 {
     if (!n_pk) return LWB_OK;
     const int words = std::max(1, (n2max + 31) >> 5);
     if (vq.runs && (!fast || (size_t)C * n2max > kVqMaxElems))
         return fail(ctx, LWB_ERR_INVALID, "VQ entry needs <= 8 channels, aligned arenas and channels * n/2 <= 12288");
+    int rc;
+    float *zero = nullptr;
+    if (floor0 && ys) {
+        if ((rc = ensure(ctx, ctx->floor0, ctx->spec.cap))) return rc;
+        zero = (float *)ctx->floor0.p + (spec - (float *)ctx->spec.p);
+        if ((rc = launch_floor0_curves(ctx, d_pk, n_pk, C, kinds, ys, zero))) return rc;
+    }
     if (!fast)
-        return launch(ctx, LWB_KERNEL_PROLOGUE, k_prologue, dim3((unsigned)n_pk), dim3(kPrologueThreads), smem_old, d_pk, res, dense, kinds, ys, spec);
+        return launch(ctx, LWB_KERNEL_PROLOGUE, k_prologue, dim3((unsigned)n_pk), dim3(kPrologueThreads), smem_old, d_pk, res, dense, kinds, ys, spec,
+                      (const float *)zero);
     // per (packet, channel) row (ctx scratch): the packed flagged segments of its floor curve, the bin -> segment
     // index (bitmap + prefix counts) and the segment count
     const size_t rows = n_pk * C, tab_bytes = rows * kSegStride * sizeof(uint4), ix_bytes = rows * seg_index_stride(words);
-    int rc = ensure(ctx, ctx->segtab, tab_bytes + ix_bytes + rows + 64);
-    if (rc) return rc;
+    if ((rc = ensure(ctx, ctx->segtab, tab_bytes + ix_bytes + rows + 64))) return rc;
     if (!ctx->magic.p) {            // multiply-high magics of every segment length, once per context
         std::vector<uint32_t> mt(kFloor1MagicEntries);
         for (int adx = 0; adx < kFloor1MagicEntries; adx++) {
@@ -172,32 +193,45 @@ static int launch_prologue(lwb_ctx *ctx, const DevPacket *d_pk, size_t n_pk, uns
     const VqDev vd{vq.runs, vq.run_off, vq.entries, vq.ent_off};
     if (vq.runs)
         return launch(ctx, LWB_KERNEL_PROLOGUE_FUSED, k_prologue_fused<true>, dim3((unsigned)grid), dim3(kPfThreads), prologue_fused_smem((int)C, words, (size_t)C * n2max), d_pk,
-                      (uint32_t)n_pk, res, dense, kinds, (const uint4 *)tab, (const uint8_t *)cnt, (const unsigned char *)ix, words, spec, vd);
+                      (uint32_t)n_pk, res, dense, (const float *)zero, kinds, (const uint4 *)tab, (const uint8_t *)cnt, (const unsigned char *)ix, words, spec, vd);
     return launch(ctx, LWB_KERNEL_PROLOGUE_FUSED, k_prologue_fused<false>, dim3((unsigned)grid), dim3(kPfThreads), prologue_fused_smem((int)C, words), d_pk, (uint32_t)n_pk, res, dense,
-                  kinds, (const uint4 *)tab, (const uint8_t *)cnt, (const unsigned char *)ix, words, spec, vd);
+                  (const float *)zero, kinds, (const uint4 *)tab, (const uint8_t *)cnt, (const unsigned char *)ix, words, spec, vd);
 }
 static int launch_prologue(lwb_ctx *ctx, const DevPacket *d_pk, const DevPacket *h_pk, size_t n_pk, unsigned C, size_t smem_old,
-                           const float *res, const float *dense, const uint8_t *kinds, const uint32_t *ys, float *spec, VqView vq = VqView())
+                           const float *res, const float *dense, const uint8_t *kinds, const uint32_t *ys, float *spec, VqView vq, bool floor0)
 {
     int n2max = 32;
     for (size_t i = 0; i < n_pk; i++) n2max = std::max(n2max, h_pk[i].n >> 1);
-    return launch_prologue(ctx, d_pk, n_pk, C, prologue_is_fast(h_pk, n_pk, C, res, dense, spec), smem_old, n2max, res, dense, kinds, ys, spec, vq);
+    return launch_prologue(ctx, d_pk, n_pk, C, prologue_is_fast(h_pk, n_pk, C, res, dense, spec), smem_old, n2max, res, dense, kinds, ys, spec, vq,
+                           floor0);
 }
 
-// Host-side look at the floor kinds of rows [row_lo, row_hi) (one row per (packet, channel)).  Device-resident
+// Host-side look at the floor kinds of the `done` packets chain c decodes (one row per (packet, channel)).  Device-resident
 // floor arrays (io->floor_memory == LWB_MEM_DEVICE) cannot be looked at: they are trusted, and the batch is assumed
-// to carry dense (floor-0) curves exactly when the caller passed a dense_floor arena.
-static int scan_floor_kinds(lwb_ctx *ctx, const lwb_batch_io *io, uint64_t row_lo, uint64_t row_hi, bool *need_dense)
+// to carry dense (floor-0) curves exactly when the caller passed a dense_floor arena, and floor-0 records exactly when
+// the chain's setup has floor-0 descriptions.
+static int scan_floor_kinds(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chain *c, uint32_t done, bool *need_dense, bool *need_floor0)
 {
+    const lwb_setup *su = c->stream->setup;
     if (io->floor_memory == LWB_MEM_DEVICE) {
         if (io->dense_floor) *need_dense = true;
+        if (!su->floor0.empty()) *need_floor0 = true;
         return LWB_OK;
     }
-    for (uint64_t r = row_lo; r < row_hi; r++) {
-        const uint8_t kd = io->floor_kind[r];
-        if (kd > LWB_FLOOR_DENSE) return fail(ctx, LWB_ERR_INVALID, "floor_kind out of range");
-        if (kd == LWB_FLOOR_ONE && !io->floor1_y) return fail(ctx, LWB_ERR_INVALID, "floor1_y missing");
-        if (kd == LWB_FLOOR_DENSE) *need_dense = true;
+    const unsigned C = su->channels;
+    for (uint32_t k = 0; k < done; k++) {
+        const uint8_t *kinds = io->floor_kind + (c->packet_index + k) * C;
+        for (unsigned ch = 0; ch < C; ch++) {
+            const uint8_t kd = kinds[ch];
+            if (kd > LWB_FLOOR_ZERO) return fail(ctx, LWB_ERR_INVALID, "floor_kind out of range");
+            if ((kd == LWB_FLOOR_ONE || kd == LWB_FLOOR_ZERO) && !io->floor1_y) return fail(ctx, LWB_ERR_INVALID, "floor1_y missing");
+            if (kd == LWB_FLOOR_DENSE) *need_dense = true;
+            if (kd != LWB_FLOOR_ZERO) continue;
+            const DevMapping &mp = su->mappings[su->host.mode_mapping[c->mode_numbers[k]]];
+            if (!su->floor0_described(mp.floor_of_channel[ch]))
+                return fail(ctx, LWB_ERR_INVALID, "floor_kind out of range: LWB_FLOOR_ZERO on a floor without a floor-0 description");
+            *need_floor0 = true;
+        }
     }
     return LWB_OK;
 }
@@ -274,7 +308,8 @@ static int upload_floor_rows(lwb_ctx *ctx, const lwb_batch_io *io, uint64_t a, u
 struct BatchExtent {
     uint64_t c_lo = ~0ull, c_hi = 0, o_lo = ~0ull, o_hi = 0, r_lo = ~0ull, r_hi = 0;
     bool need_dense = false;      // a decoded row has a dense floor
-    bool scan = true;             // check the floor kinds of the rows added (a chunk's rows were checked with its batch)
+    bool need_floor0 = false;     // a decoded row may have a floor-0 record (LWB_FLOOR_ZERO)
+    bool scan = true;            // check the floor kinds of the rows added (a chunk's rows were checked with its batch)
 
     // Chain c decodes `done` packets, whose coefficients end at coeff_end, into n_samples samples per channel.
     int add(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chain *c, uint32_t done, uint64_t coeff_end, uint64_t n_samples)
@@ -290,7 +325,7 @@ struct BatchExtent {
         if (io->entry == LWB_ENTRY_SPECTRUM) return LWB_OK;
         r_lo = std::min(r_lo, c->packet_index);
         r_hi = std::max<uint64_t>(r_hi, c->packet_index + done);
-        return scan ? scan_floor_kinds(ctx, io, c->packet_index * C, (c->packet_index + done) * C, &need_dense) : LWB_OK;
+        return scan ? scan_floor_kinds(ctx, io, c, done, &need_dense, &need_floor0) : LWB_OK;
     }
     int finish(lwb_ctx *ctx, const lwb_batch_io *io) const
     {
@@ -492,6 +527,7 @@ static FrontStages front_stages_of(const BatchExtent &ext, unsigned C, int n1max
     fs.r_lo = ext.r_lo;
     fs.r_hi = ext.r_hi;
     fs.dense = ext.need_dense;
+    fs.floor0 = ext.need_floor0;
     return fs;
 }
 
@@ -518,7 +554,8 @@ static int stage_front_packets(lwb_ctx *ctx, const BatchArenas &ar, const lwb_ch
 static int front_stages_launch(lwb_ctx *ctx, const BatchArenas &ar, const FrontStages &fs, size_t k0, size_t n)
 {
     const FrontArenas a = front_arenas(ctx, ar, fs);
-    return launch_prologue(ctx, fs.pk + k0, n, fs.C, fs.fast, fs.smem_old, fs.n2max, a.res, a.dense, ar.fl.kinds, ar.fl.ys, a.spec, ar.fl.vq);
+    return launch_prologue(ctx, fs.pk + k0, n, fs.C, fs.fast, fs.smem_old, fs.n2max, a.res, a.dense, ar.fl.kinds, ar.fl.ys, a.spec, ar.fl.vq,
+                           fs.floor0);
 }
 
 // A device-memory batch's front stages alone: stages the floor and VQ arrays of fs's packet rows on the compute stream
@@ -537,8 +574,9 @@ static int front_stages_run(lwb_ctx *ctx, const lwb_batch_io *io, const FrontSta
 }
 
 // Generic path: rounds of packets bounded by the IMDCT scratch.  Its descriptors address a host-memory batch's
-// staging from its start (element c_lo / o_lo), a device-memory batch's arenas from element 0.
-static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_batch_io *io, const BatchArenas &ar)
+// staging from its start (element c_lo / o_lo), a device-memory batch's arenas from element 0.  ext_floor0: the batch may
+// have LWB_FLOOR_ZERO rows (BatchExtent::need_floor0).
+static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_batch_io *io, const BatchArenas &ar, bool ext_floor0)
 {
     size_t maxp = 0;
     for (auto &pc : plan) maxp = std::max(maxp, pc.pk.size());
@@ -627,7 +665,7 @@ static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_bat
         if (io->entry != LWB_ENTRY_SPECTRUM) {
             if ((rc = ensure(ctx, ctx->spec, spec_hi * sizeof(float)))) return rc;
             if ((rc = launch_prologue(ctx, dp, hp, n_desc, maxc, prologue_smem_of(plan), coeffs, dense, ar.fl.kinds, ar.fl.ys,
-                                      (float *)ctx->spec.p, ar.fl.vq)))
+                                      (float *)ctx->spec.p, ar.fl.vq, ext_floor0)))
                 return rc;
             spec = (const float *)ctx->spec.p;
         }

@@ -13,16 +13,17 @@ import ctypes as C
 import numpy as np
 
 from . import _cabi as cabi
-from .api import AudioReadError, DecodedPacket, Setup
+from .api import AudioReadError, DecodedPacket, Floor0Record, Setup
 
 (ERR_END_OF_PACKET, ERR_NOT_VORBIS_HEADER, ERR_UNSUPPORTED_VERSION, ERR_HEADER_BAD_FORMAT, ERR_HEADER_BAD_TYPE,
  ERR_HEADER_IS_AUDIO, ERR_UTF8, ERR_AUDIO_IS_HEADER, ERR_OGG, ERR_NO_MORE_PACKETS) = range(16, 26)
 
 SYMBOLS = ["lwf_headers_parse", "lwf_headers_destroy", "lwf_headers_info", "lwf_headers_comment", "lwf_headers_make_setup",
-           "lwf_packet_decode", "lwf_packet_decode_vq", "lwf_headers_vq_capable", "lwf_decoded_sample_count", "lwf_ogg_open", "lwf_ogg_close", "lwf_ogg_next_packet",
+           "lwf_headers_make_setup_floor0", "lwf_packet_decode", "lwf_packet_decode_ex", "lwf_packet_decode_vq", "lwf_packet_decode_vq_ex", "lwf_headers_vq_capable", "lwf_decoded_sample_count", "lwf_ogg_open", "lwf_ogg_close", "lwf_ogg_next_packet",
            "lwf_reader_open", "lwf_reader_close", "lwf_reader_headers", "lwf_reader_read_dec_packet", "lwf_reader_last_absgp",
            "lwf_reader_skip_samples_linear", "lwf_reader_seek_absgp_pg",
            "lwf_batcher_create", "lwf_batcher_destroy", "lwf_batcher_set_entry", "lwf_batcher_decode", "lwf_batcher_last_timing",
+           "lwf_batcher_last_input_bytes", "lwf_batcher_set_floor0",
            "lwf_debug_float32_unpack", "lwf_debug_lookup1_values", "lwf_debug_ilog", "lwf_debug_read_bits", "lwf_debug_huffman",
            "lwf_debug_decode_loop"]
 
@@ -88,6 +89,11 @@ def lib():
         L.lwf_headers_comment.restype = sz
         L.lwf_headers_make_setup.argtypes = [vp, vp, C.POINTER(vp)]
         L.lwf_packet_decode.argtypes = [vp, C.c_char_p, sz, C.POINTER(_DecodedPacket)]
+        L.lwf_packet_decode_ex.argtypes = [vp, C.c_char_p, sz, C.POINTER(_DecodedPacket), C.c_int]
+        L.lwf_headers_make_setup_floor0.argtypes = [vp, vp, C.POINTER(vp)]
+        L.lwf_batcher_set_floor0.argtypes = [vp, C.c_int]
+        L.lwf_batcher_last_input_bytes.argtypes = [vp]
+        L.lwf_batcher_last_input_bytes.restype = C.c_uint64
         L.lwf_decoded_sample_count.argtypes = [vp, C.c_char_p, sz, C.POINTER(sz)]
         L.lwf_ogg_open.argtypes = [C.c_char_p, sz, C.POINTER(vp)]
         L.lwf_ogg_close.argtypes = [vp]
@@ -108,6 +114,7 @@ def lib():
         L.lwf_batcher_set_entry.argtypes = [vp, C.c_int]
         L.lwf_headers_vq_capable.argtypes = [vp]
         L.lwf_packet_decode_vq.argtypes = [vp, C.c_char_p, sz, vp, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz)]
+        L.lwf_packet_decode_vq_ex.argtypes = [vp, C.c_char_p, sz, vp, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz), C.c_int]
         L.lwf_batcher_decode.argtypes = [vp, C.POINTER(_StreamJob), sz, C.c_int, vp]
         L.lwf_batcher_last_timing.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double)]
         L.lwf_batcher_last_timing.restype = None
@@ -160,14 +167,17 @@ class Headers:
             out.append((k, v))
         return out
 
-    def make_setup(self, ctx):
-        """The device-side header constants (lwb_setup) for these headers."""
+    def make_setup(self, ctx, floor0=False):
+        """The device-side header constants (lwb_setup) for these headers; floor0: with the floor-0 descriptions that
+        packets decoded with floor0_records=True need (lwf_headers_make_setup_floor0)."""
         h = C.c_void_p()
-        ctx.check(lib().lwf_headers_make_setup(self._h, ctx._h, C.byref(h)))
+        fn = lib().lwf_headers_make_setup_floor0 if floor0 else lib().lwf_headers_make_setup
+        ctx.check(fn(self._h, ctx._h, C.byref(h)))
         return Setup._adopt(ctx, h.value, self.audio_channels, self.blocksize_0, self.blocksize_1)
 
-    def decode_packet(self, packet):
-        """audio.rs:919-986: returns an api.DecodedPacket (mode, window flags, per-channel floors, residue)."""
+    def decode_packet(self, packet, floor0_records=False):
+        """audio.rs:919-986: returns an api.DecodedPacket (mode, window flags, per-channel floors, residue).
+        floor0_records: type-0 floors of order <= 63 come out as api.Floor0Record instead of dense curves."""
         Cn, n2max = self.audio_channels, (1 << self.blocksize_1) // 2
         kinds = np.zeros(Cn, np.uint8)
         ys = np.zeros((Cn, cabi.MAX_POSTS), np.uint32)
@@ -178,7 +188,7 @@ class Headers:
         dp.floor1_y = ys.ctypes.data_as(cabi.u32p)
         dp.dense_floor = dense.ctypes.data_as(cabi.fp)
         dp.residue = res.ctypes.data_as(cabi.fp)
-        rc = lib().lwf_packet_decode(self._h, bytes(packet), len(packet), C.byref(dp))
+        rc = lib().lwf_packet_decode_ex(self._h, bytes(packet), len(packet), C.byref(dp), FLOOR0_RECORDS if floor0_records else 0)
         if rc == cabi.ERR_BAD_FORMAT:
             raise AudioReadError(rc)
         if rc:
@@ -194,6 +204,8 @@ class Headers:
                 floors.append(None)
             elif kinds[c] == cabi.FLOOR_ONE:
                 floors.append(ys[c].copy())
+            elif kinds[c] == cabi.FLOOR_ZERO:
+                floors.append(_record(ys[c]))
             else:
                 floors.append(flat_dense[c * n2:(c + 1) * n2].copy())
         residue = flat_res[: Cn * n2].reshape(Cn, n2).copy()
@@ -205,7 +217,7 @@ class Headers:
         """True if LWB_ENTRY_VQ applies to this stream (lwf_headers_vq_capable)."""
         return bool(lib().lwf_headers_vq_capable(self._h))
 
-    def decode_packet_vq(self, packet):
+    def decode_packet_vq(self, packet, floor0_records=False):
         """The same front half with the residue left as VQ runs: (DecodedPacket with a zero residue, runs, entries):
         runs a structured array (lwb_vq_run), entries the uint16 codebook entries they index."""
         Cn, n2max = self.audio_channels, (1 << self.blocksize_1) // 2
@@ -219,8 +231,8 @@ class Headers:
         cap = len(packet) * 8 + 16
         runs, ents = np.zeros(cap, VQ_RUN_DTYPE), np.zeros(cap, np.uint16)
         n, ne = C.c_size_t(), C.c_size_t()
-        rc = lib().lwf_packet_decode_vq(self._h, bytes(packet), len(packet), C.byref(dp), runs.ctypes.data, cap, C.byref(n),
-                                        ents.ctypes.data, cap, C.byref(ne))
+        rc = lib().lwf_packet_decode_vq_ex(self._h, bytes(packet), len(packet), C.byref(dp), runs.ctypes.data, cap, C.byref(n),
+                                           ents.ctypes.data, cap, C.byref(ne), FLOOR0_RECORDS if floor0_records else 0)
         if rc == cabi.ERR_BAD_FORMAT:
             raise AudioReadError(rc)
         if rc:
@@ -235,6 +247,8 @@ class Headers:
                 floors.append(None)
             elif kinds[c] == cabi.FLOOR_ONE:
                 floors.append(ys[c].copy())
+            elif kinds[c] == cabi.FLOOR_ZERO:
+                floors.append(_record(ys[c]))
             else:
                 floors.append(flat_dense[c * n2:(c + 1) * n2].copy())
         out = DecodedPacket(dp.mode_number, np.zeros((Cn, n2), np.float32), floors, dp.prev_window_flag, dp.next_window_flag)
@@ -415,17 +429,30 @@ class OggStreamReader:
             pass
 
 
+FLOOR0_RECORDS = 1           # LWF_DECODE_FLOOR0_RECORDS
+
+
+def _record(row):
+    """The api.Floor0Record in an LWB_FLOOR_ZERO floor1_y row: the amplitude and all 63 coefficient slots (those past the
+    floor's order are zero, and the device does not read them)."""
+    return Floor0Record(int(row[0]) | (int(row[1]) << 32), row[2:].view(np.float32).copy())
+
+
 class StreamBatcher:
     """lwf_batcher: entropy-decode the packets of many streams (one shared set of headers) on a host
     thread pool and synthesise them with one batched call.  jobs: list of (PreviousWindowRight,
     [packet bytes, ...]); PCM lands planar in `pcm` at out_offset = job index * channels * stride."""
 
-    def __init__(self, ctx, headers, threads=0, entry=cabi.ENTRY_RESIDUE):
+    def __init__(self, ctx, headers, threads=0, entry=cabi.ENTRY_RESIDUE, floor0=False):
+        """floor0: type-0 floors travel as floor-0 records (lwf_batcher_set_floor0); the jobs' streams must then come from
+        headers.make_setup(ctx, floor0=True)."""
         self.ctx, self.headers = ctx, headers
         h = C.c_void_p()
         ctx.check(lib().lwf_batcher_create(ctx._h, headers._h, threads, C.byref(h)))
         self._h = h.value
         ctx._children.add(self)
+        if floor0:
+            ctx.check(lib().lwf_batcher_set_floor0(self._h, 1))
         if entry != cabi.ENTRY_RESIDUE:        # LWB_ENTRY_VQ: VQ records instead of dense residue vectors cross the boundary
             rc = lib().lwf_batcher_set_entry(self._h, entry)
             if rc:
@@ -456,6 +483,7 @@ class StreamBatcher:
         e, s = C.c_double(), C.c_double()
         lib().lwf_batcher_last_timing(self._h, C.byref(e), C.byref(s))
         self.entropy_seconds, self.synthesis_seconds = e.value, s.value
+        self.input_bytes = lib().lwf_batcher_last_input_bytes(self._h)
         return [(arr[j].n_samples, arr[j].packets_done, arr[j].status) for j in range(n)]
 
     def close(self):
