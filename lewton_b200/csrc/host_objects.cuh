@@ -93,22 +93,33 @@ struct lwb_setup {
     bool floor0_described(uint32_t fi) const { return fi < floor0.size() && floor0[fi].order != 0; }
 };
 
-struct MixRound { size_t r0, nr, s0, ns, c0, nc, x0, nx, g0, ng, flat, nm; };   // LongRun / ShortRun / ChainDesc / RowCopy / burst-group ranges of one
-                                                                            // round; flat: the one-pass round (static deal, k_long_s);
-                                                                            // nm: groups of k_mid (path_mid.cuh, from the buffer's start)
 struct RowCopy { const float *src; float *dst; uint32_t n4, pad; };  // n4 float4s, copied in front of the round's kernels
 struct ChainShape { unsigned warps; size_t smem; int n1max, wpc, np; };     // k_chain's block and shared memory
-// The arguments of mixed_launch_rounds (and of a captured k_long: pack and i16).  Built by aggregate initialisation;
-// the members a path leaves out are zero.
-struct MixLaunch {
-    char *db;                                   // descriptor buffer
-    void *pcm; int out_format; bool i16;
-    const float *pack; int ls; const float *w_short;                   // k_long / k_long_s
-    const float *spack;                                                 // k_short / k_short_g
-    const float *mpack; int mid_kb;                                     // k_mid
-    size_t off_sr, off_cd, off_by, off_rc, off_sg;                      // ShortRun, ChainDesc, mode bytes, RowCopy, bursts in db
-    bool residue; ChainShape chain; const float *coeffs, *dense; const uint8_t *kinds; const uint32_t *ys;   // k_chain
-    const float *zero;                                                  // k_chain: curves of LWB_FLOOR_ZERO rows, or nullptr
+
+// One launch of a batch path (run_steps, path_generic.cuh): the kernel's LWB_KERNEL_* id, a device pointer to its
+// descriptors -- runs or run groups (LongRun, ShortRun), ChainDescs or RowCopys -- their count (groups for k_long, k_mid
+// and k_short_g) and the twiddle pack it uses.
+struct Step {
+    int kernel;
+    const void *desc;
+    size_t n;
+    const float *pack;
+};
+
+// What the steps of one batch share.  Set member by member; what a path does not launch stays zero.
+struct StepArgs {
+    void *pcm = nullptr;                                    // PCM arena (k_chain; the runs carry their own pointers)
+    int out_format = LWB_OUT_F32_PLANAR;
+    const float *w_short = nullptr;                         // k_long / k_long_s: short window and ls of transitional blocks
+    int ls = 0;
+    int mid_kb = 0;                                         // k_mid: 1 for n = 1024, 2 for n = 512
+    ChainShape chain = {};                                  // k_chain
+    const uint8_t *bytes = nullptr;                         // k_chain: mode bytes (ChainDesc::byte_off)
+    bool residue = false;                                   // k_chain: its own front half on residues
+    const float *coeffs = nullptr, *dense = nullptr;
+    const uint8_t *kinds = nullptr;
+    const uint32_t *ys = nullptr;
+    const float *zero = nullptr;                            // k_chain: curves of LWB_FLOOR_ZERO rows, or nullptr
 };
 
 // One launch of the residue entry's front stages (k_floor1_segments + k_prologue_fused, or k_prologue): floor x
@@ -132,16 +143,14 @@ struct lwb_plan {
     lwb_chain *chains = nullptr;
     size_t n_chains = 0;
     lwb_batch_io io;
-    // captured launch sequence (valid while ctx->state_gen == gen): the front stages if front.n, then either the
-    // rounds of mix_launch or, when there are none, one k_long over `runs`.  Every path that captures a residue-entry
-    // batch sets `front`; a spectrum-entry plan never does.
+    // captured launch sequence (valid while ctx->state_gen == gen): the front stages if front.n, then `steps`.  Every
+    // path that captures a residue-entry batch sets `front`; a spectrum-entry plan never does.
     bool captured = false;
     uint64_t gen = 0;
     FrontStages front;
-    DevBuf runs, pro, mix;             // descriptors the capture owns: k_long runs, the long path's front stages, the rest
-    uint32_t n_groups = 0;             // k_long groups of `runs`
-    MixLaunch mix_launch;
-    std::vector<MixRound> mix_rounds;
+    DevBuf pro, mix;                   // descriptors the capture owns: the long path's front stages, the steps'
+    StepArgs args;
+    std::vector<Step> steps;
 };
 
 struct lwb_stream {
@@ -154,8 +163,7 @@ struct lwb_stream {
 };
 
 // Records the launches a path made for a prepared batch; lwb_plan_execute replays them while ctx->state_gen == gen.
-static void capture(lwb_plan *plan, uint64_t gen, const FrontStages &front, const MixLaunch &ml, std::vector<MixRound> rounds,
-                    uint32_t n_groups = 0)
+static void capture(lwb_plan *plan, uint64_t gen, const FrontStages &front, const StepArgs &args, std::vector<Step> steps)
 {
     plan->captured = true;
     plan->gen = gen;
@@ -164,9 +172,8 @@ static void capture(lwb_plan *plan, uint64_t gen, const FrontStages &front, cons
     // that the captured one did not, so the floor-0 curves run whenever a chain's setup can serve records.
     for (size_t i = 0; i < plan->n_chains && front.n; i++)
         if (!plan->chains[i].stream->setup->floor0.empty()) plan->front.floor0 = true;
-    plan->mix_launch = ml;
-    plan->mix_rounds = std::move(rounds);
-    plan->n_groups = n_groups;
+    plan->args = args;
+    plan->steps = std::move(steps);
 }
 
 
@@ -386,14 +393,19 @@ static int copy_pcm_to_host(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chai
     return LWB_OK;
 }
 
-// The fused kernels load coefficients with TMA bulk copies and store PCM with vector stores, which need 16-byte aligned
-// addresses.  Element offsets that are multiples of 4 keep that when the arenas are 16-byte aligned: the library's
-// staging of host-memory batches always is, a caller's device arena may not be (the chain kernel takes those).
-static bool device_arenas_aligned(const lwb_batch_io *io)
+// The layout the fused kernels take: planar f32 / i16 out, and 16-byte aligned addresses, which their TMA bulk loads of
+// coefficients and vector stores of PCM need.  Element offsets that are multiples of 4 keep that when the arenas are
+// 16-byte aligned: the library's staging of host-memory batches always is, a caller's device arena may not be (the chain
+// kernel takes those).
+static bool fused_layout(const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io)
 {
-    if (io->memory != LWB_MEM_DEVICE) return true;
-    return ((reinterpret_cast<uintptr_t>(io->coeffs) | reinterpret_cast<uintptr_t>(io->pcm) |
-             reinterpret_cast<uintptr_t>(io->dense_floor)) & 15) == 0;
+    if (io->out_format != LWB_OUT_F32_PLANAR && io->out_format != LWB_OUT_I16_PLANAR) return false;
+    if (io->memory == LWB_MEM_DEVICE && ((reinterpret_cast<uintptr_t>(io->coeffs) | reinterpret_cast<uintptr_t>(io->pcm) |
+                                          reinterpret_cast<uintptr_t>(io->dense_floor)) & 15))
+        return false;
+    for (size_t i = 0; i < n_chains; i++)
+        if ((chains[i].out_offset | chains[i].out_stride | chains[i].coeff_offset) & 3) return false;
+    return true;
 }
 
 static int ensure_pinned(lwb_ctx *ctx, size_t bytes)

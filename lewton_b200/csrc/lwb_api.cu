@@ -661,10 +661,7 @@ static int queue_batch(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const l
             if (!io->floor_kind) return fail(ctx, LWB_ERR_INVALID, "residue entry needs floor_kind");
         }
     }
-    if (prepared) {                           // the path that takes the batch captures it anew, if it can
-        prepared->captured = false;
-        prepared->mix_rounds.clear();
-    }
+    if (prepared) prepared->captured = false; // the path that takes the batch captures it anew, if it can
     for (size_t k = first_batch_path(); k < kNumBatchPaths; k++) {
         bool handled = false;
         const int rc = kBatchPaths[k](ctx, chains, n_chains, io, &handled, prepared);
@@ -777,10 +774,9 @@ extern "C" int lwb_plan_create(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains,
 extern "C" void lwb_plan_destroy(lwb_plan *p)
 {
     if (!p) return;
-    if (p->runs.p || p->mix.p || p->pro.p) {
+    if (p->mix.p || p->pro.p) {
         cudaSetDevice(p->ctx->device);
         cudaStreamSynchronize(p->ctx->stream);
-        if (p->runs.p) cudaFree(p->runs.p);
         if (p->mix.p) cudaFree(p->mix.p);
         if (p->pro.p) cudaFree(p->pro.p);
     }
@@ -798,9 +794,8 @@ extern "C" int lwb_plan_execute(lwb_plan *p)
     // (Host floor arrays change from step to step and are uploaded again; device floor arrays are read in place.)
     CU(ctx, cudaSetDevice(ctx->device));
     int rc;
-    if (p->front.n && (rc = front_stages_run(ctx, &p->io, p->front))) return rc;    // they write ctx->spec, which the launch reads
-    if (p->mix_rounds.empty()) return launch_long(ctx, (const LongRun *)p->runs.p, p->n_groups, p->mix_launch.pack, p->mix_launch.i16);
-    return mixed_launch_rounds(ctx, p->mix_launch, p->mix_rounds);
+    if (p->front.n && (rc = front_stages_run(ctx, &p->io, p->front))) return rc;    // they write ctx->spec, which the steps read
+    return run_steps(ctx, p->args, p->steps);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -1,5 +1,5 @@
 // path_chain.cuh -- part of the C-ABI translation unit (included by lwb_api.cu, not compiled on its own):
-// the chain-kernel path (kernel_chain.cuh) and the launch sequence shared with the mixed path.
+// the chain-kernel path (kernel_chain.cuh), and the chain descriptors and row copies the mixed path shares with it.
 #pragma once
 
 // ---------------------------------------------------------------------------------------------
@@ -29,32 +29,6 @@ static ChainShape chain_shape(unsigned maxc, int n1max, bool residue)
     return ChainShape{maxc * wpc, chain_smem(maxc, n1max, np), n1max, wpc, np};
 }
 
-template <int ENTRY>
-static int launch_chain(lwb_ctx *ctx, int fmt, unsigned n_chains, unsigned warps, size_t smem, const ChainDesc *d,
-                        const uint8_t *bytes, const float *coeffs, const float *dense, const uint8_t *kinds,
-                        const uint32_t *ys, void *pcm, int n1max, int wpc, int np, const float *zero)
-{
-#define LWB_CHAIN_CASE(F)                                                                                    \
-    case F:                                                                                                  \
-        if (wpc == 1) {                                                                                      \
-            cudaFuncSetAttribute(k_chain<F, ENTRY, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, false>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, \
-                          kinds, ys, pcm, n1max, wpc, np, zero);                                              \
-        }                                                                                                    \
-        cudaFuncSetAttribute(k_chain<F, ENTRY, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-        return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, true>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, kinds, \
-                      ys, pcm, n1max, wpc, 1, zero);
-    switch (fmt) {
-        LWB_CHAIN_CASE(LWB_OUT_F32_PLANAR)
-        LWB_CHAIN_CASE(LWB_OUT_I16_PLANAR)
-        LWB_CHAIN_CASE(LWB_OUT_F32_INTERLEAVED)
-        LWB_CHAIN_CASE(LWB_OUT_I16_INTERLEAVED)
-    }
-#undef LWB_CHAIN_CASE
-    return LWB_ERR_INVALID;
-}
-
-// one launch of the fused kernel and one of the chain kernel per round, in stream order
 // One block per row: the stream state the first segment of a chain starts from, moved out of the way of the segment of
 // the same chain that ends the batch -- in the one-pass schedule (path_mixed.cuh) that one may store the new state before
 // the first one has read the old.
@@ -65,54 +39,26 @@ __global__ void k_row_copy(const RowCopy *__restrict__ rc)
         reinterpret_cast<float4 *>(c.dst)[i] = reinterpret_cast<const float4 *>(c.src)[i];
 }
 
-static int mixed_launch_rounds(lwb_ctx *ctx, const MixLaunch &ml, const std::vector<MixRound> &rounds)
+// The chain kernel's descriptor of packets [p0, p0 + n) of chain c, which enter with stream state (has, plen), start at
+// element offset `coeff` and emit from sample `pos` of the chain's output; their mode bytes start at byte_off.
+static void chain_desc(const lwb_chain *c, uint32_t p0, uint32_t n, bool has, uint32_t plen, uint64_t coeff, uint64_t pos, uint32_t byte_off,
+                       ChainDesc *d)
 {
-    cudaStream_t sm = ctx->stream;
-    int rc = LWB_OK;
-    for (const MixRound &rd : rounds) {
-        if (rd.nm &&             // uniform 1024-point batches (path_mid.cuh)
-            (rc = launched(ctx, LWB_KERNEL_MID, mid_launch(sm, (const LongRun *)ml.db, (uint32_t)rd.nm, ml.mpack, ctx->sm_count, ml.i16, ml.mid_kb),
-                           "mid kernel launch")))
-            return rc;
-        if (rd.nx && (rc = launch(ctx, LWB_KERNEL_ROW_COPY, k_row_copy, dim3((unsigned)rd.nx), dim3(64), 0, (const RowCopy *)(ml.db + ml.off_rc) + rd.x0)))
-            return rc;
-        if (rd.nr) {
-            unsigned int *ticket;
-            if ((rc = next_ticket(ctx, &ticket))) return rc;
-            if (kLongNB != 1) return fail(ctx, LWB_ERR_INVALID, "mixed path needs one run per warp");
-            // one pass over many short runs: the static deal with its deeper lookahead (k_long_s); rounds: tickets
-            if (rd.flat)
-                rc = launched(ctx, LWB_KERNEL_LONG_S,
-                              long_launch_static(sm, (const LongRun *)ml.db + rd.r0, (uint32_t)rd.nr, ml.pack, ctx->sm_count, ml.i16, ml.w_short, ml.ls),
-                              "long kernel launch");
-            else
-                rc = launched(ctx, LWB_KERNEL_LONG,
-                              long_launch(sm, (const LongRun *)ml.db + rd.r0, (uint32_t)rd.nr, ml.pack, ticket, ctx->sm_count, ml.i16, ml.w_short, ml.ls),
-                              "long kernel launch");
-            if (rc) return rc;
-        }
-        if (rd.ns &&
-            (rc = launched(ctx, LWB_KERNEL_SHORT, short_launch(sm, (const ShortRun *)(ml.db + ml.off_sr) + rd.s0, (uint32_t)rd.ns, ml.spack, ctx->sm_count, ml.i16),
-                           "short kernel launch")))
-            return rc;
-        if (rd.ng &&             // bursts: eight short runs of equal length per warp (k_short_g)
-            (rc = launched(ctx, LWB_KERNEL_SHORT_G,
-                           short_launch_groups(sm, (const ShortRun *)(ml.db + ml.off_sg) + rd.g0 * kShortOct, (uint32_t)rd.ng, ml.spack, ctx->sm_count, ml.i16),
-                           "short burst kernel launch")))
-            return rc;
-        if (rd.nc) {
-            const ChainDesc *dcd = (const ChainDesc *)(ml.db + ml.off_cd) + rd.c0;
-            const uint8_t *dby = (const uint8_t *)(ml.db + ml.off_by);
-            if (ml.residue)
-                rc = launch_chain<LWB_ENTRY_RESIDUE>(ctx, ml.out_format, (unsigned)rd.nc, ml.chain.warps, ml.chain.smem, dcd, dby, ml.coeffs, ml.dense,
-                                                     ml.kinds, ml.ys, ml.pcm, ml.chain.n1max, ml.chain.wpc, ml.chain.np, ml.zero);
-            else
-                rc = launch_chain<LWB_ENTRY_SPECTRUM>(ctx, ml.out_format, (unsigned)rd.nc, ml.chain.warps, ml.chain.smem, dcd, dby, ml.coeffs, ml.dense,
-                                                      ml.kinds, ml.ys, ml.pcm, ml.chain.n1max, ml.chain.wpc, ml.chain.np, ml.zero);
-            if (rc) return rc;
-        }
-    }
-    return LWB_OK;
+    const lwb_stream *s = c->stream;
+    const lwb_setup *su = s->setup;
+    std::memset(d, 0, sizeof(*d));
+    d->setup = su->d_setup;
+    d->state = s->d_state;
+    d->coeff_off = coeff;
+    d->out_off = c->out_offset + pos;
+    d->out_stride = c->out_stride;
+    d->pkt_index = c->packet_index + p0;
+    d->n_packets = n;
+    d->byte_off = byte_off;
+    d->state_stride = (uint32_t)state_stride(su);
+    d->plen0 = (uint16_t)plen;
+    d->has0 = has;
+    d->channels = (uint8_t)su->channels;
 }
 
 // k_floor0_curves over the decoded packets of a residue-entry batch the chain kernel takes: *zero addresses the curves by
@@ -167,28 +113,13 @@ static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
     std::vector<ChainWalk> walks(n_chains);
     for (size_t i = 0; i < n_chains; i++) {
         lwb_chain *c = &chains[i];
-        const lwb_stream *s = c->stream;
-        const lwb_setup *su = s->setup;
         const ChainWalk &w = walks[i] = walk_chain(c, [&](uint32_t k, const Geom &, bool, uint32_t, uint64_t, uint64_t) {
             write_mode_bytes(c, k, hb + boff + 3 * k);
         });
         set_chain_result(c, w);
         if ((rc = ext.add(ctx, io, c, w.done, w.coeff_end, w.n_samples))) return rc;
         if (!w.done) continue;
-        ChainDesc &d = hd[n_launch++];
-        std::memset(&d, 0, sizeof(d));
-        d.setup = su->d_setup;
-        d.state = s->d_state;
-        d.coeff_off = c->coeff_offset;
-        d.out_off = c->out_offset;
-        d.out_stride = c->out_stride;
-        d.pkt_index = c->packet_index;
-        d.n_packets = w.done;
-        d.byte_off = (uint32_t)boff;
-        d.state_stride = (uint32_t)state_stride(su);
-        d.plen0 = (uint16_t)s->plen;
-        d.has0 = s->has;
-        d.channels = (uint8_t)su->channels;
+        chain_desc(c, 0, w.done, c->stream->has, c->stream->plen, c->coeff_offset, 0, (uint32_t)boff, &hd[n_launch++]);
         boff += (size_t)w.done * 3;
     }
     if ((rc = ext.finish(ctx, io))) return rc;
@@ -208,11 +139,20 @@ static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         // residue entry with floor-0 records: their curves first, by absolute coefficient offset like ar.coeffs
         float *zero = nullptr;
         if (residue && ext.need_floor0 && ar.fl.ys && (rc = chain_floor0_curves(ctx, ar, ext, chains, n_chains, walks, &zero))) return rc;
-        const MixLaunch ml{(char *)dbuf.p, ar.pcm, io->out_format, false, nullptr, 0, nullptr, nullptr, nullptr, 0, 0, 0, used_desc, 0, 0,
-                           residue, chain_shape(maxc, n1max, residue), ar.coeffs, ar.dense, ar.fl.kinds, ar.fl.ys, zero};
-        std::vector<MixRound> rounds(1, MixRound{0, 0, 0, 0, 0, n_launch});
-        if ((rc = mixed_launch_rounds(ctx, ml, rounds))) return rc;
-        if (cap) capture(plan, gen_at_entry, FrontStages(), ml, std::move(rounds));
+        StepArgs args;
+        args.pcm = ar.pcm;
+        args.out_format = io->out_format;
+        args.chain = chain_shape(maxc, n1max, residue);
+        args.bytes = (const uint8_t *)dbuf.p + used_desc;
+        args.residue = residue;
+        args.coeffs = ar.coeffs;
+        args.dense = ar.dense;
+        args.kinds = ar.fl.kinds;
+        args.ys = ar.fl.ys;
+        args.zero = zero;
+        std::vector<Step> steps(1, Step{LWB_KERNEL_CHAIN, dbuf.p, n_launch, nullptr});
+        if ((rc = run_steps(ctx, args, steps))) return rc;
+        if (cap) capture(plan, gen_at_entry, FrontStages(), args, std::move(steps));
         if ((rc = ar.download(0, chains, 0, n_chains, ext)) || (rc = ar.finish())) return rc;
     }
     commit_stream_states(chains, walks);

@@ -573,6 +573,84 @@ static int front_stages_run(lwb_ctx *ctx, const lwb_batch_io *io, const FrontSta
     return front_stages_launch(ctx, ar, fs, 0, fs.n);
 }
 
+// ---------------------------------------------------------------------------------------------
+// the launches of the fused paths and the chain-kernel path (Step)
+// ---------------------------------------------------------------------------------------------
+template <int ENTRY>
+static int launch_chain(lwb_ctx *ctx, int fmt, unsigned n_chains, unsigned warps, size_t smem, const ChainDesc *d,
+                        const uint8_t *bytes, const float *coeffs, const float *dense, const uint8_t *kinds,
+                        const uint32_t *ys, void *pcm, int n1max, int wpc, int np, const float *zero)
+{
+#define LWB_CHAIN_CASE(F)                                                                                    \
+    case F:                                                                                                  \
+        if (wpc == 1) {                                                                                      \
+            cudaFuncSetAttribute(k_chain<F, ENTRY, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+            return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, false>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, \
+                          kinds, ys, pcm, n1max, wpc, np, zero);                                              \
+        }                                                                                                    \
+        cudaFuncSetAttribute(k_chain<F, ENTRY, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+        return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, true>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, kinds, \
+                      ys, pcm, n1max, wpc, 1, zero);
+    switch (fmt) {
+        LWB_CHAIN_CASE(LWB_OUT_F32_PLANAR)
+        LWB_CHAIN_CASE(LWB_OUT_I16_PLANAR)
+        LWB_CHAIN_CASE(LWB_OUT_F32_INTERLEAVED)
+        LWB_CHAIN_CASE(LWB_OUT_I16_INTERLEAVED)
+    }
+#undef LWB_CHAIN_CASE
+    return LWB_ERR_INVALID;
+}
+
+__global__ void k_row_copy(const RowCopy *__restrict__ rc);   // path_chain.cuh
+
+// Launches `steps` in order on the compute stream.  Only k_long draws a ticket.
+static int run_steps(lwb_ctx *ctx, const StepArgs &a, const std::vector<Step> &steps)
+{
+    cudaStream_t sm = ctx->stream;
+    const bool i16 = a.out_format == LWB_OUT_I16_PLANAR;
+    for (const Step &s : steps) {
+        int rc;
+        unsigned int *ticket;
+        const uint32_t n = (uint32_t)s.n;
+        switch (s.kernel) {
+        case LWB_KERNEL_ROW_COPY:
+            rc = launch(ctx, LWB_KERNEL_ROW_COPY, k_row_copy, dim3(n), dim3(64), 0, (const RowCopy *)s.desc);
+            break;
+        case LWB_KERNEL_LONG:
+            if ((rc = next_ticket(ctx, &ticket))) return rc;
+            rc = launched(ctx, LWB_KERNEL_LONG, long_launch(sm, (const LongRun *)s.desc, n, s.pack, ticket, ctx->sm_count, i16, a.w_short, a.ls),
+                          "long kernel launch");
+            break;
+        case LWB_KERNEL_LONG_S:         // one pass over many short runs: the static deal with its deeper lookahead
+            rc = launched(ctx, LWB_KERNEL_LONG_S, long_launch_static(sm, (const LongRun *)s.desc, n, s.pack, ctx->sm_count, i16, a.w_short, a.ls),
+                          "long kernel launch");
+            break;
+        case LWB_KERNEL_MID:
+            rc = launched(ctx, LWB_KERNEL_MID, mid_launch(sm, (const LongRun *)s.desc, n, s.pack, ctx->sm_count, i16, a.mid_kb), "mid kernel launch");
+            break;
+        case LWB_KERNEL_SHORT:
+            rc = launched(ctx, LWB_KERNEL_SHORT, short_launch(sm, (const ShortRun *)s.desc, n, s.pack, ctx->sm_count, i16), "short kernel launch");
+            break;
+        case LWB_KERNEL_SHORT_G:        // bursts: eight short runs of equal length per warp
+            rc = launched(ctx, LWB_KERNEL_SHORT_G, short_launch_groups(sm, (const ShortRun *)s.desc, n, s.pack, ctx->sm_count, i16),
+                          "short burst kernel launch");
+            break;
+        case LWB_KERNEL_CHAIN:
+            if (a.residue)
+                rc = launch_chain<LWB_ENTRY_RESIDUE>(ctx, a.out_format, n, a.chain.warps, a.chain.smem, (const ChainDesc *)s.desc, a.bytes, a.coeffs,
+                                                     a.dense, a.kinds, a.ys, a.pcm, a.chain.n1max, a.chain.wpc, a.chain.np, a.zero);
+            else
+                rc = launch_chain<LWB_ENTRY_SPECTRUM>(ctx, a.out_format, n, a.chain.warps, a.chain.smem, (const ChainDesc *)s.desc, a.bytes, a.coeffs,
+                                                      a.dense, a.kinds, a.ys, a.pcm, a.chain.n1max, a.chain.wpc, a.chain.np, a.zero);
+            break;
+        default:
+            return fail(ctx, LWB_ERR_INVALID, "internal: no step for this kernel");
+        }
+        if (rc) return rc;
+    }
+    return LWB_OK;
+}
+
 // Generic path: rounds of packets bounded by the IMDCT scratch.  Its descriptors address a host-memory batch's
 // staging from its start (element c_lo / o_lo), a device-memory batch's arenas from element 0.  ext_floor0: the batch may
 // have LWB_FLOOR_ZERO rows (BatchExtent::need_floor0).

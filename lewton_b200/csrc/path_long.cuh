@@ -45,24 +45,35 @@ static void cut_run(const Run &whole, size_t cuts, size_t first_emit, size_t n2,
     }
 }
 
+// The run of channel ch of n packets of chain c, blocks of n2-point halves, cut into `cuts` pieces w[0, cuts): its
+// coefficients start at `in` (the packets' first one; channels n2 apart, packets C * n2 apart), its PCM at `pcm` (the
+// chain's sample of its first packet; planes out_stride apart, esz bytes per sample).  has: a state enters it;
+// first_emit: the samples its first packet emits.
+template <typename Run>
+static void channel_run(const lwb_chain *c, unsigned ch, size_t n2, const float *in, char *pcm, size_t esz, uint32_t n, bool has,
+                        size_t first_emit, size_t cuts, Run *w)
+{
+    const lwb_stream *s = c->stream;
+    const lwb_setup *su = s->setup;
+    const unsigned C = su->channels;
+    cut_run(Run{in + (size_t)ch * n2, pcm + (c->out_offset + (size_t)ch * c->out_stride) * esz, s->d_state + (size_t)ch * state_stride(su),
+                (uint32_t)(C * n2), n, has},
+            cuts, first_emit, n2, esz, w);
+}
+
 // Appends the runs of one chain, each channel cut into `cuts` pieces.  coeffs / pcm: arenas addressed by absolute
 // element offset.
 static void long_runs_of(const LongItem &it, size_t cuts, const float *coeffs, char *pcm, size_t esz, LongRun *&w)
 {
-    const lwb_stream *s = it.c->stream;
-    const lwb_setup *su = s->setup;
-    const unsigned C = su->channels;
-    for (unsigned ch = 0; ch < C; ch++, w += cuts)
-        cut_run(LongRun{coeffs + it.c->coeff_offset + (size_t)ch * kLongN2, pcm + (it.c->out_offset + (size_t)ch * it.c->out_stride) * esz,
-                        s->d_state + (size_t)ch * state_stride(su), (uint32_t)(C * kLongN2), it.P, it.has_prev},
-                cuts, it.has_prev ? kLongN2 : 0, kLongN2, esz, w);
+    for (unsigned ch = 0; ch < it.c->stream->setup->channels; ch++, w += cuts)
+        channel_run(it.c, ch, kLongN2, coeffs + it.c->coeff_offset, pcm, esz, it.P, it.has_prev, it.has_prev ? kLongN2 : 0, cuts, w);
 }
 
 // Every packet a long block of the fast blocksize with long neighbours, every stream empty or
-// holding a 1024-sample right half, arenas aligned: what the fused kernel takes.
+// holding a 1024-sample right half, the fused kernels' layout: what the fused kernel takes.
 static bool batch_is_uniform_long(const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io)
 {
-    if (io->out_format != LWB_OUT_F32_PLANAR && io->out_format != LWB_OUT_I16_PLANAR) return false;
+    if (!fused_layout(chains, n_chains, io)) return false;
     const float *pack = nullptr;
     for (size_t i = 0; i < n_chains; i++) {
         const lwb_chain *c = &chains[i];
@@ -71,7 +82,6 @@ static bool batch_is_uniform_long(const lwb_chain *chains, size_t n_chains, cons
         if (su->bs1 != kLongBs || !su->host.tab[1].pack) return false;
         if (pack && pack != su->host.tab[1].pack) return false;
         pack = su->host.tab[1].pack;
-        if ((c->out_offset & 3) || (c->out_stride & 3) || (c->coeff_offset & 3) || !device_arenas_aligned(io)) return false;
         if (s->has && s->plen != (uint32_t)kLongN2) return false;
         for (uint32_t k = 0; k < c->n_packets; k++) {
             const uint8_t m = c->mode_numbers[k];
@@ -227,15 +237,6 @@ static int long_upload_runs(lwb_ctx *ctx, const LongRuns &lr, cudaStream_t ds)
     return LWB_OK;
 }
 
-// One k_long launch over n_groups groups of runs.
-static int launch_long(lwb_ctx *ctx, const LongRun *runs, uint32_t n_groups, const float *pack, bool i16)
-{
-    unsigned int *ticket;
-    int rc = next_ticket(ctx, &ticket);
-    if (rc) return rc;
-    return launched(ctx, LWB_KERNEL_LONG, long_launch(ctx->stream, runs, n_groups, pack, ticket, ctx->sm_count, i16), "long kernel launch");
-}
-
 // The fused long-block path for all three entries.  A residue-entry batch (LWB_ENTRY_RESIDUE or LWB_ENTRY_VQ) runs
 // the front stages (k_floor1_segments + k_prologue_fused, or k_prologue) over each chunk's packets first: they form its
 // spectrum in ctx->spec, which k_long then reads instead of the coefficient arena.  Planned straight from the chain
@@ -255,7 +256,7 @@ static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_
     if ((rc = uniform_extent(ctx, io, chains, 0, n_chains, kLongN2, &ext)) || (rc = ext.finish(ctx, io))) return rc;
     if (ext.empty()) return LWB_OK;
     const unsigned C = chains[0].stream->setup->channels;                  // (residue entries: the batch's one count)
-    const bool residue = io->entry != LWB_ENTRY_SPECTRUM, i16 = io->out_format == LWB_OUT_I16_PLANAR, host = io->memory == LWB_MEM_HOST;
+    const bool residue = io->entry != LWB_ENTRY_SPECTRUM, host = io->memory == LWB_MEM_HOST;
     const float *pack = chains[0].stream->setup->host.tab[1].pack;          // one twiddle pack per launch
     const size_t n_chunks = host ? host_chunks((size_t)(ext.c_hi - ext.c_lo) * 4, n_chains) : 1;
     const bool cap = plan && !host;
@@ -279,6 +280,10 @@ static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_
         if (plan) plan->front = fs;
         in = (const float *)ctx->spec.p - ext.c_lo;                         // same element offsets as the coefficients
     }
+    StepArgs args;
+    args.pcm = ar.pcm;
+    args.out_format = io->out_format;
+    std::vector<Step> steps;                                                // the k_long of one chunk
     LongRuns lr;
     uint64_t gen = 0;
     size_t pk0 = 0;
@@ -292,18 +297,17 @@ static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_
         for (size_t i = i0; i < i1; i++) npk += chains[i].n_packets;
         if ((rc = ar.upload(k, ke)) || (residue && (rc = front_stages_launch(ctx, ar, fs, pk0, npk)))) return rc;
         if (!lr.d) {
-            if ((rc = long_build_runs(ctx, chains, n_chains, n_chunks, in, ar.pcm, i16 ? 2 : 4, cap ? &plan->runs : nullptr, &lr)) ||
+            if ((rc = long_build_runs(ctx, chains, n_chains, n_chunks, in, ar.pcm, elem_size(io->out_format), cap ? &plan->mix : nullptr, &lr)) ||
                 (rc = long_upload_runs(ctx, lr, host ? ctx->copy_in : ctx->copy_out)))
                 return rc;
             gen = ctx->state_gen;                                           // every arena the capture points into is sized
         }
-        if ((rc = launch_long(ctx, lr.d + lr.chunks[k].r0, (uint32_t)(lr.chunks[k].nr / kLongNB), pack, i16)) ||
-            (rc = ar.download(k, chains, i0, i1, ke)))
-            return rc;
+        steps.assign(1, Step{LWB_KERNEL_LONG, lr.d + lr.chunks[k].r0, lr.chunks[k].nr / kLongNB, pack});
+        if ((rc = run_steps(ctx, args, steps)) || (rc = ar.download(k, chains, i0, i1, ke))) return rc;
         pk0 += npk;
     }
     CU(ctx, cudaEventRecord(ctx->ev_kdone[lr.par], ctx->stream));
-    if (cap) capture(plan, gen, fs, MixLaunch{nullptr, nullptr, 0, i16, pack}, {}, (uint32_t)(lr.chunks[0].nr / kLongNB));
+    if (cap) capture(plan, gen, fs, args, std::move(steps));                 // (one chunk)
     if ((rc = ar.finish())) return rc;
     commit_uniform_states(chains, n_chains, kLongN2);
     return LWB_OK;

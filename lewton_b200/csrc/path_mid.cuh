@@ -2,7 +2,7 @@
 // batches whose every packet is a full-window block of n = 1024 or of n = 512 (blocksize 10 / 9) go to k_mid
 // (kernel_mid.cuh): planar f32 / i16, <= 8 channels; the residue entry runs the front stages (k_floor1_segments +
 // k_prologue_fused, kernel_prologue.cuh) over all packets first and hand k_mid the spectrum arena.  The descriptors, the staging of host arenas and the capture by a prepared
-// batch follow try_chain; the launch goes through mixed_launch_rounds (MixRound::nm).
+// batch follow try_chain; the launch is one LWB_KERNEL_MID step.
 #pragma once
 
 struct MidGroup { LongRun r[4]; uint32_t n_packets; };
@@ -12,12 +12,10 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
     *handled = false;
     const uint64_t gen_at_entry = ctx->state_gen;
     if (getenv("LWB_NO_MID")) return LWB_OK;
-    if (io->out_format != LWB_OUT_F32_PLANAR && io->out_format != LWB_OUT_I16_PLANAR) return LWB_OK;
     const bool vq = io->entry == LWB_ENTRY_VQ, residue = io->entry != LWB_ENTRY_SPECTRUM;
     if (vq) return LWB_OK;                                    // (VQ records of such streams: the general path, as before)
-    if (!device_arenas_aligned(io)) return LWB_OK;
-    const bool i16 = io->out_format == LWB_OUT_I16_PLANAR;
-    const size_t esz = i16 ? 2 : 4;
+    if (!fused_layout(chains, n_chains, io)) return LWB_OK;
+    const size_t esz = elem_size(io->out_format);
     const float *pack = nullptr;
     int kb = 0;                                              // 1: n = 1024, 2: n = 512 (one size per batch: one pack)
     // pass 1, no side effects: every packet a full-window block of that size on top of no state or an n/2-sample one
@@ -29,7 +27,6 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
         if (pack && pack != su->host.tab[1].pack) return LWB_OK;
         pack = su->host.tab[1].pack;
         kb = 11 - su->bs1;
-        if ((c->out_offset & 3) || (c->out_stride & 3) || (c->coeff_offset & 3)) return LWB_OK;
         const uint32_t n_blk = 2048u >> kb, n2_blk = n_blk >> 1;
         if (c->stream->has && c->stream->plen != n2_blk) return LWB_OK;
         for (uint32_t k = 0; k < c->n_packets; k++) {
@@ -84,20 +81,9 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
     for (size_t i = 0; i < n_chains; i++) {
         const lwb_chain *c = &chains[i];
         if (!c->n_packets) continue;
-        const lwb_stream *s = c->stream;
-        const lwb_setup *su = s->setup;
-        const unsigned C = su->channels;
-        for (unsigned ch = 0; ch < C; ch++) {
-            LongRun lr;
-            std::memset(&lr, 0, sizeof(lr));
-            lr.in = d_coeffs + c->coeff_offset + (size_t)ch * kMidN2;
-            lr.out = ar.pcm + (c->out_offset + (size_t)ch * c->out_stride) * esz;
-            lr.state = s->d_state + (size_t)ch * state_stride(su);
-            lr.in_stride = (uint32_t)(C * kMidN2);
-            lr.n_packets = c->n_packets;
-            lr.has_prev = s->has;
-            lr.write_state = 1;
-            runs.push_back(lr);
+        for (unsigned ch = 0; ch < c->stream->setup->channels; ch++) {
+            runs.emplace_back();
+            channel_run(c, ch, kMidN2, d_coeffs + c->coeff_offset, ar.pcm, esz, c->n_packets, c->stream->has, 0, 1, &runs.back());
         }
     }
     std::stable_sort(runs.begin(), runs.end(), [](const LongRun &a, const LongRun &b) { return a.n_packets > b.n_packets; });
@@ -127,13 +113,13 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
         for (size_t b = 0; b < NBg; b++) h[NBg * k + b] = groups[k].r[b];
     if (bytes > off_pro) return fail(ctx, LWB_ERR_INVALID, "internal: more run groups than runs");
     if ((rc = upload_staging(ctx, st, h, dbuf.p, bytes, ctx->stream))) return rc;
-    const MixLaunch ml{(char *)dbuf.p, ar.pcm, io->out_format, i16, nullptr, 0, nullptr, nullptr, pack, kb};
-    MixRound rd;
-    std::memset(&rd, 0, sizeof(rd));
-    rd.nm = groups.size();
-    std::vector<MixRound> rounds(1, rd);
-    if ((rc = mixed_launch_rounds(ctx, ml, rounds))) return rc;
-    if (cap) capture(plan, gen_at_entry, fs, ml, std::move(rounds));
+    StepArgs args;
+    args.pcm = ar.pcm;
+    args.out_format = io->out_format;
+    args.mid_kb = kb;
+    std::vector<Step> steps(1, Step{LWB_KERNEL_MID, dbuf.p, groups.size(), pack});
+    if ((rc = run_steps(ctx, args, steps))) return rc;
+    if (cap) capture(plan, gen_at_entry, fs, args, std::move(steps));
     if ((rc = ar.download(0, chains, 0, n_chains, ext)) || (rc = ar.finish())) return rc;
     commit_uniform_states(chains, n_chains, (uint32_t)kMidN2);
     return LWB_OK;

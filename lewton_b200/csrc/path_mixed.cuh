@@ -42,11 +42,9 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
     *handled = false;
     const uint64_t gen_at_entry = ctx->state_gen;
     if (getenv("LWB_NO_MIXED")) return LWB_OK;
-    if (io->out_format != LWB_OUT_F32_PLANAR && io->out_format != LWB_OUT_I16_PLANAR) return LWB_OK;
-    if (!device_arenas_aligned(io)) return LWB_OK;
+    if (!fused_layout(chains, n_chains, io)) return LWB_OK;
     const bool residue = io->entry != LWB_ENTRY_SPECTRUM;
-    const bool i16 = io->out_format == LWB_OUT_I16_PLANAR;
-    const size_t esz = i16 ? 2 : 4;
+    const size_t esz = elem_size(io->out_format);
     unsigned maxc = 1;
     int n1max = 64, n0max = 64, bs0 = -1;
     size_t total_packets = 0, fast_like = 0;
@@ -73,7 +71,6 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                 spack = su->host.tab[f].pack;
             }
         }
-        if ((c->out_offset & 3) || (c->out_stride & 3) || (c->coeff_offset & 3)) return LWB_OK;
         maxc = std::max<unsigned>(maxc, su->channels);
         n1max = std::max(n1max, 1 << su->bs1);
         n0max = std::max(n0max, 1 << su->bs0);
@@ -230,7 +227,6 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         const bool host = io->memory == LWB_MEM_HOST;
         BatchArenas ar;
         if ((rc = ar.open(ctx, io, ext, maxc, true))) return rc;
-        const float *d_coeffs = ar.coeffs;
         char *d_pcm = ar.pcm;
         // host memory: chunks of chains
         const size_t n_chunks = host ? host_chunks((size_t)(ext.c_hi - ext.c_lo) * 4, n_chains) : 1;
@@ -245,7 +241,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
             size_t i0, i1, p0, np_;                      // chains, prologue packets
             BatchExtent ext;
             std::vector<uint32_t> round_cut, round_cut_s;
-            std::vector<MixRound> rounds;
+            std::vector<Step> steps;
         };
         std::vector<Chunk> chunks(n_chunks);
         auto cuts_of = [&](const Chunk &ck, const Seg &sg, size_t r) {
@@ -321,10 +317,10 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         std::vector<ShortRun> burst_runs;
         std::vector<ShortGroup> groups, tmp_g;
         std::memcpy(hb + off_by, bytes.data(), boff);
-        const float *d_spec = nullptr;
+        const float *d_in = ar.coeffs;                           // what the fused kernels and the chain kernel read
         if (residue) {
             if ((rc = ensure(ctx, ctx->spec, (size_t)(ext.c_hi - ext.c_lo) * 4))) return rc;
-            d_spec = (const float *)ctx->spec.p - ext.c_lo;      // same element offsets as the coefficient arena
+            d_in = (const float *)ctx->spec.p - ext.c_lo;        // the spectrum: same element offsets as the coefficient arena
         }
         size_t wr = 0, ws = 0, wc = 0, wp = 0;
         std::vector<LongRun> tmp_lr;
@@ -335,14 +331,9 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
             wp += sg.n;
         };
         for (Chunk &ck : chunks) {
-            ck.rounds.assign(max_rounds, MixRound{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0});
             ck.p0 = wp;
             for (size_t r = 0; r < max_rounds; r++) {
-                ck.rounds[r].r0 = wr;
-                ck.rounds[r].s0 = ws;
-                ck.rounds[r].c0 = wc;
-                ck.rounds[r].x0 = wx;
-                ck.rounds[r].g0 = wg;
+                const size_t r0 = wr, s0 = ws, c0 = wc, x0 = wx, g0 = wg;
                 burst_runs.clear();
                 // fused-kernel runs first, longest first (three buckets): the kernel hands runs out in
                 // descriptor order, and a 64-packet run started last would be the whole round's tail
@@ -356,18 +347,13 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                         const uint32_t cuts = cuts_of(ck, sg, r), piece = sg.n / cuts;
                         if ((piece >= 32 ? 0 : piece >= 8 ? 1 : 2) != bucket) continue;
                         const lwb_chain *c = &chains[i];
-                        const lwb_stream *s = c->stream;
-                        const lwb_setup *su = s->setup;
-                        const unsigned C = su->channels;
+                        const unsigned C = c->stream->setup->channels;
                         // samples packet 0 emits (0 without history; a block after a short one emits 1024 - ls)
                         const size_t first_emit = sg.has ? (sg.first_short ? (size_t)kLongN2 - ls_long : (size_t)kLongN2) : 0;
                         for (unsigned ch = 0; ch < C; ch++) {
                             LongRun *w = h_runs + wr;
                             wr += cuts;
-                            cut_run(LongRun{(residue ? d_spec : d_coeffs) + sg.coeff + (size_t)ch * kLongN2,
-                                            d_pcm + (c->out_offset + (size_t)ch * c->out_stride + sg.pos) * esz, s->d_state + (size_t)ch * state_stride(su),
-                                            (uint32_t)(C * kLongN2), sg.n, sg.has},
-                                    cuts, first_emit, kLongN2, esz, w);
+                            channel_run(c, ch, kLongN2, d_in + sg.coeff, d_pcm + sg.pos * esz, esz, sg.n, sg.has, first_emit, cuts, w);
                             LongRun &last = w[cuts - 1], &lr = w[0];         // (one piece: the same run)
                             last.last_short = sg.last_short;
                             if (chain_flat[i] && q + 1 < walks[i].n_seg) last.state_out = slot_of(i, q, C, ch);
@@ -393,9 +379,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                     const Seg &sg = segs[walks[i].seg0 + q];
                     if (sg.kind != SEG_SHORT) continue;
                     const lwb_chain *c = &chains[i];
-                    const lwb_stream *s = c->stream;
-                    const lwb_setup *su = s->setup;
-                    const unsigned C = su->channels;
+                    const unsigned C = c->stream->setup->channels;
                     const uint32_t cuts = cuts_of(ck, sg, r);
                     const size_t first_emit = sg.has ? (size_t)kShortN2 : 0;       // samples packet 0 emits
                     const bool burst = bursts && chain_flat[i] && sg.n < (uint32_t)kShortOct;    // (one piece)
@@ -408,10 +392,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                             w = h_sr + ws;
                             ws += cuts;
                         }
-                        cut_run(ShortRun{(residue ? d_spec : d_coeffs) + sg.coeff + (size_t)ch * kShortN2,
-                                         d_pcm + (c->out_offset + (size_t)ch * c->out_stride + sg.pos) * esz, s->d_state + (size_t)ch * state_stride(su),
-                                         (uint32_t)(C * kShortN2), sg.n, sg.has},
-                                cuts, first_emit, kShortN2, esz, w);
+                        channel_run(c, ch, kShortN2, d_in + sg.coeff, d_pcm + sg.pos * esz, esz, sg.n, sg.has, first_emit, cuts, w);
                         ShortRun &last = w[cuts - 1], &sr = w[0];        // (one piece: the same run)
                         if (chain_flat[i] && q + 1 < walks[i].n_seg) {      // the long block behind has run already
                             last.write_state = 0;
@@ -437,26 +418,9 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                     const Seg &sg = segs[walks[i].seg0 + q0];
                     if (sg.kind != SEG_CHAIN) continue;
                     const lwb_chain *c = &chains[i];
-                    const lwb_stream *s = c->stream;
-                    const lwb_setup *su = s->setup;
                     if (residue) emit_pro(c, sg);
-                    ChainDesc &d = h_cd[wc++];
-                    std::memset(&d, 0, sizeof(d));
-                    d.setup = su->d_setup;
-                    d.state = s->d_state;
-                    d.coeff_off = sg.coeff;
-                    d.out_off = c->out_offset + sg.pos;
-                    d.out_stride = c->out_stride;
-                    d.pkt_index = c->packet_index + sg.p0;
-                    d.n_packets = sg.n;
-                    d.byte_off = walks[i].boff + 3 * sg.p0;
-                    d.state_stride = (uint32_t)state_stride(su);
-                    d.plen0 = (uint16_t)sg.plen;
-                    d.has0 = sg.has;
-                    d.channels = (uint8_t)su->channels;
+                    chain_desc(c, sg.p0, sg.n, sg.has, sg.plen, sg.coeff, sg.pos, walks[i].boff + 3 * sg.p0, &h_cd[wc++]);
                 }
-                ck.rounds[r].nr = wr - ck.rounds[r].r0;
-                ck.rounds[r].ns = ws - ck.rounds[r].s0;
                 if (!burst_runs.empty()) {
                     // length classes, longest first, each padded with dummies (in == nullptr) to whole groups
                     groups.clear();
@@ -478,24 +442,37 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                     if ((wg + groups.size()) * kShortOct > sg_cap) return fail(ctx, LWB_ERR_INVALID, "burst group area too small");
                     for (const ShortGroup &gr : groups) std::memcpy(h_sg + (wg++) * kShortOct, gr.r, sizeof(gr.r));
                 }
-                ck.rounds[r].ng = wg - ck.rounds[r].g0;
-                ck.rounds[r].flat = flat && r == 0;
+                const size_t nr = wr - r0, ns = ws - s0;
                 if (flat && r == 0 && !getenv("LWB_NO_BALANCE")) {
                     auto warps_of = [&](size_t n, int per_cta) {
                         return std::min<size_t>((n + per_cta - 1) / per_cta, (size_t)ctx->sm_count) * per_cta;
                     };
-                    balance_static_deal(h_runs + ck.rounds[r].r0, ck.rounds[r].nr, warps_of(ck.rounds[r].nr, kLongWarps), tmp_lr);
-                    balance_static_deal(h_sr + ck.rounds[r].s0, ck.rounds[r].ns, warps_of(ck.rounds[r].ns, kShortWarps), tmp_sr);
+                    balance_static_deal(h_runs + r0, nr, warps_of(nr, kLongWarps), tmp_lr);
+                    balance_static_deal(h_sr + s0, ns, warps_of(ns, kShortWarps), tmp_sr);
                 }
-                ck.rounds[r].nc = wc - ck.rounds[r].c0;
-                ck.rounds[r].nx = wx - ck.rounds[r].x0;
+                // the round's launches: the row copies go before k_long_s, and the short kernels complete the boundary
+                // slots k_long_s left
+                if (nr && kLongNB != 1) return fail(ctx, LWB_ERR_INVALID, "mixed path needs one run per warp");
+                auto step = [&](int kernel, size_t off, size_t n, const float *pk) {
+                    if (n) ck.steps.push_back(Step{kernel, db + off, n, pk});
+                };
+                step(LWB_KERNEL_ROW_COPY, off_rc + x0 * sizeof(RowCopy), wx - x0, nullptr);
+                step(flat && r == 0 ? LWB_KERNEL_LONG_S : LWB_KERNEL_LONG, r0 * sizeof(LongRun), nr, pack);
+                step(LWB_KERNEL_SHORT, off_sr + s0 * sizeof(ShortRun), ns, spack);
+                step(LWB_KERNEL_SHORT_G, off_sg + g0 * kShortOct * sizeof(ShortRun), wg - g0, spack);
+                step(LWB_KERNEL_CHAIN, off_cd + c0 * sizeof(ChainDesc), wc - c0, nullptr);
             }
             ck.np_ = wp - ck.p0;
         }
         if ((rc = upload_staging(ctx, st, hb, db, total, ctx->stream))) return rc;
-        // (residue entry: the front stages run first, the chain kernel sees a spectrum)
-        const MixLaunch ml{db, d_pcm, io->out_format, i16, pack, ls_long, w_short, spack, nullptr, 0, off_sr, off_cd, off_by, off_rc, off_sg,
-                           false, chain_shape(maxc, n1max, false), residue ? d_spec : d_coeffs};
+        StepArgs args;
+        args.pcm = d_pcm;
+        args.out_format = io->out_format;
+        args.w_short = w_short;
+        args.ls = ls_long;
+        args.chain = chain_shape(maxc, n1max, false);
+        args.bytes = (const uint8_t *)db + off_by;
+        args.coeffs = d_in;                     // (residue entry: the front stages run first, the chain kernel sees a spectrum)
         FrontStages fs = front_stages_of(ext, maxc, n1max_all, n_pro);         // (residue entry: every packet of the batch, chunk by chunk)
         fs.pk = (const DevPacket *)(db + off_pro);
         if (fs.n) fs.fast = front_stages_fast(ctx, ar, fs, h_pro);
@@ -503,10 +480,10 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
             Chunk &ck = chunks[k];
             if (ck.ext.empty()) continue;
             if ((rc = ar.upload(k, ck.ext)) || (ck.np_ && (rc = front_stages_launch(ctx, ar, fs, ck.p0, ck.np_))) ||
-                (rc = mixed_launch_rounds(ctx, ml, ck.rounds)) || (rc = ar.download(k, chains, ck.i0, ck.i1, ck.ext)))
+                (rc = run_steps(ctx, args, ck.steps)) || (rc = ar.download(k, chains, ck.i0, ck.i1, ck.ext)))
                 return rc;
         }
-        if (cap) capture(plan, gen_at_entry, fs, ml, std::move(chunks[0].rounds));
+        if (cap) capture(plan, gen_at_entry, fs, args, std::move(chunks[0].steps));
         if ((rc = ar.finish())) return rc;
     }
     commit_stream_states(chains, results);
