@@ -506,6 +506,10 @@ __device__ __forceinline__ void lds_eo(uint32_t addr, float &e, float &o)
     asm volatile("ld.shared.f32 %0, [%2];\n\tld.shared.f32 %1, [%2+2048];" : "=f"(e), "=f"(o) : "r"(addr) : "memory");
 }
 
+}  // namespace lwb
+#include "kernel_deal.cuh"       // the static-deal driver builds on the primitives above
+namespace lwb {
+
 // Twiddle residency: pack slots [kTwReg0, kTwReg1) live in registers for the whole kernel, the
 // rest is read from the CTA's shared copy of the pack when used (compile-time choice per slot).
 // Default (H100, DESIGN.md 4.1): one block per warp, 8 warps per SM (2 per scheduler, 249 registers,
@@ -1038,25 +1042,13 @@ k_long(const LongRun *__restrict__ runs, uint32_t n_groups, const float *__restr
     }
 }
 
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void *src)
-{
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
 // ---------------------------------------------------------------------------------------------
 // k_long_s: the same transform behind a different driver, for launches made of MANY SHORT runs (the one-pass
 // schedule of mixed long / short streams, path_mixed.cuh: a run is what lies between two bursts of short
 // blocks, often one to three packets).  k_long learns its next group one group ahead (ticket, then descriptor,
 // then tiles), which leaves the ring under-filled and the descriptor latency exposed when groups are shorter
-// than the ring.  Here the deal is static (run r -> warp r mod W), so a warp knows its whole future:
-//   * descriptors arrive by cp.async in a shared ring, kLongFetch runs ahead of the producer;
-//   * the producer cursor walks (run, packet) in processing order and stays exactly kLongRing tiles ahead of
-//     the consumer, across any number of run boundaries;
-//   * the state row of the next run that overlaps with one (has_prev, not exported) is requested as soon as the
-//     state tile is free and that run's descriptor has landed.
+// than the ring.  Here the deal is static: kernel_deal.cuh's driver, one run per item, one packet per unit, and the
+// state row of the next run that overlaps with one (has_prev, not exported).
 // ---------------------------------------------------------------------------------------------
 constexpr int kLongLs256 = (kLongN - 256) / 4;      // ls of a long block next to a 256-point block
 constexpr int kLongFetch = 3;
@@ -1066,13 +1058,75 @@ constexpr size_t kLongSmemBytesS = 2048 + (size_t)kLongWarps * (kLongRing + 1) *
                                    kLongWarps * (kLongRing + 2) * 8 + (size_t)kLongWarps * kLongDescSlots * sizeof(LongRun) +
                                    kLongSlopeMax * sizeof(float) + 64;
 
-template <typename OutT, int LS>
+// The three transposes of a tile, with phase B between them (k_long_s, k_mid): phase A's values leave at the lane
+// offsets lA0 / lA1, phase B's arrive and leave at lB, phase C's arrive at lC0 / lC1.  The stage is the scratch.
+__device__ __forceinline__ void transpose_abc(const TwMix &tw, uint32_t stage_s, uint32_t lA0, uint32_t lA1, uint32_t lB,
+                                              uint32_t lC0, uint32_t lC1, V O[1][8], V E[1][8])
+{
+    __syncwarp();           // every lane has consumed its quads: the tile becomes the scratch
+    {
+        const uint32_t a0 = stage_s + lA0, a1 = stage_s + lA1;
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+            sts_eo(a0 ^ LWB_KA(j), E[0][j].x, O[0][j].x);
+            sts_eo(a1 ^ LWB_KA(j), E[0][j].y, O[0][j].y);
+        }
+    }
+    __syncwarp();
+    {
+        const uint32_t b0 = stage_s + lB;
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+            lds_eo(b0 ^ LWB_KB(j, 0), E[0][j].x, O[0][j].x);
+            lds_eo(b0 ^ LWB_KB(j, 1), E[0][j].y, O[0][j].y);
+        }
+    }
+    __syncwarp();
+    phase_b<1>(tw, O, E);
+    {
+        const uint32_t b0 = stage_s + lB;
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+            sts_eo(b0 ^ LWB_KB(j, 0), E[0][j].x, O[0][j].x);
+            sts_eo(b0 ^ LWB_KB(j, 1), E[0][j].y, O[0][j].y);
+        }
+    }
+    __syncwarp();
+    {
+        const uint32_t c0 = stage_s + lC0, c1 = stage_s + lC1;
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+            lds_eo(c0 ^ LWB_KC(j), E[0][j].x, O[0][j].x);
+            lds_eo(c1 ^ LWB_KC(j), E[0][j].y, O[0][j].y);
+        }
+    }
+    __syncwarp();
+}
+
+// A run's end state (k_long_s, k_mid): the lane's 16 values of the last packet's right half, each stored twice -- at
+// m and at N2 - 1 - m, the same value (imdct.rs:622-649).  The lane's samples are m = Wd rev3(j) + hl and
+// Wd rev3(j) + Wd - 1 - hl; TOP = N2 - Wd.
+template <int Wd, int TOP>
+__device__ __forceinline__ void store_right_half(float *state, int hl, const V pe[8])
+{
+    float *s_lo = state + hl, *s_hi = state + Wd - 1 - hl;
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        const int rw = Wd * rev3(j);
+        const float vx = (j & 1) ? pe[j].x : pe[j].y, vy = (j & 1) ? pe[j].y : pe[j].x;
+        s_lo[rw] = vx; s_hi[rw] = vy;
+        s_hi[TOP - rw] = vx; s_lo[TOP - rw] = vy;
+    }
+}
+
+// Only blocksize_0 = 256 (ls = 448) is built: it is the one short size the one-pass schedule exists for (k_short), and
+// with ls a multiple of 64 every position test of the transitional packets folds per slot.
+template <typename OutT>
 __global__ void __launch_bounds__(kLongWarps * 32, 1)
-k_long_s(const LongRun *__restrict__ runs, uint32_t n_runs, const float *__restrict__ pack,
-         const float *__restrict__ w_short, int ls_arg)
+k_long_s(const LongRun *__restrict__ runs, uint32_t n_runs, const float *__restrict__ pack, const float *__restrict__ w_short)
 {
     constexpr int NB = 1;
-    const int ls = LS ? LS : ls_arg;          // LS = 448: blocksize_0 = 256, the only short size the one-pass schedule has
+    constexpr int ls = kLongLs256;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t raw_s = smem_u32(smem_raw);
@@ -1108,85 +1162,40 @@ k_long_s(const LongRun *__restrict__ runs, uint32_t n_runs, const float *__restr
     for (int s = kTwReg0; s < kTwReg1; s++) twR[s - kTwReg0] = s_pack[s * 32 + lane];
     const TwMix tw{twR, s_pack + lane};
 
-    const uint32_t tiles_s = smem_u32(tiles), bars_s = smem_u32(bars), desc_s = smem_u32(s_desc);
-    const uint32_t bar_state = bars_s + 8 * kLongRing, state_s = smem_u32(s_state);
+    const uint32_t state_s = smem_u32(s_state);
     const uint32_t lA0 = laneA(lane, 0), lA1 = laneA(lane, 1);
     const uint32_t lB = laneB(lane);
     const uint32_t lC0 = laneC(lane, 0), lC1 = laneC(lane, 1);
 
     const uint32_t W = gridDim.x * kLongWarps, gw = blockIdx.x * kLongWarps + warp;
     if (gw >= n_runs) return;
-    const uint4 *rq = reinterpret_cast<const uint4 *>(runs);
-    uint32_t f_run = gw, f_slot = 0;
-    auto fetch = [&]() {            // cp.async groups are per thread: lanes 0..2 copy one quad each, everybody commits / waits
-        if (lane < 3 && f_run < n_runs) cp_async16(desc_s + f_slot * (uint32_t)sizeof(LongRun) + lane * 16, rq + 3 * (size_t)f_run + lane);
-        cp_async_commit();
-        f_run += W;
-        f_slot = (f_slot + 1 == (uint32_t)kLongDescSlots) ? 0 : f_slot + 1;
-    };
-#pragma unroll
-    for (int i = 0; i <= kLongFetch; i++) fetch();
-    cp_async_wait<kLongFetch>();
-    __syncwarp();
-    // ---- producer (warp-uniform cursor; lane 0 issues) ----
-    uint32_t p_run = gw, p_pkt = 0, p_slot = 0, p_stage = 0;
-    const float *p_in = s_desc[0].in;
-    uint32_t p_stride = s_desc[0].in_stride, p_npk = s_desc[0].n_packets;
-    auto produce = [&]() {
+    StaticDeal<sizeof(LongRun) / 16, kLongDescSlots, kLongFetch, kLongRing, kLongTileBytes> deal(
+        runs, n_runs, W, gw, smem_u32(s_desc), smem_u32(tiles), smem_u32(bars), lane);
+    auto units = [&](uint32_t sl) { return s_desc[sl].n_packets; };
+    auto issue = [&](uint32_t sl, uint32_t pkt, uint32_t bar, uint32_t dst) {
         if (lane == 0) {
             fence_proxy_async();          // the stage was written through the generic proxy (transposes) before
-            const uint32_t bar = bars_s + 8 * p_stage;
             mbar_expect_tx(bar, kLongTileBytes);
-            tma_load_1d(tiles_s + p_stage * kLongTileBytes, p_in + (size_t)p_pkt * p_stride, kLongTileBytes, bar);
-        }
-        p_stage = (p_stage + 1 == (uint32_t)kLongRing) ? 0 : p_stage + 1;
-        if (++p_pkt >= p_npk) {
-            p_run += W;
-            p_pkt = 0;
-            p_slot = (p_slot + 1 == (uint32_t)kLongDescSlots) ? 0 : p_slot + 1;
-            fetch();                      // run p_run + kLongFetch * W
-            cp_async_wait<kLongFetch>();  // run p_run's descriptor has landed
-            __syncwarp();
-            if (p_run < n_runs) { p_in = s_desc[p_slot].in; p_stride = s_desc[p_slot].in_stride; p_npk = s_desc[p_slot].n_packets; }
+            tma_load_1d(dst, s_desc[sl].in + (size_t)pkt * s_desc[sl].in_stride, kLongTileBytes, bar);
         }
     };
-    for (int i = 0; i < kLongRing; i++)
-        if (p_run < n_runs) produce();
-
-    // ---- state rows: st_run = the run whose row is in the tile or on its way (~0: the tile is free) ----
-    uint32_t st_run = ~0u;
-    auto issue_state = [&](const float *row, uint32_t run) {
+    auto needs_state = [&](uint32_t sl) { return s_desc[sl].has_prev && s_desc[sl].first_short != 2; };
+    auto issue_state = [&](uint32_t sl, uint32_t bar) {
         if (lane == 0) {
             fence_proxy_async();
-            mbar_expect_tx(bar_state, kLongTileBytes);
-            tma_load_1d(state_s, row, kLongTileBytes, bar_state);
-        }
-        st_run = run;
-    };
-    // first run in [from_run, p_run] that reads a row; the descriptor slots between the consumer and the producer have
-    // landed and are not overwritten before the consumer has passed them
-    auto request_state = [&](uint32_t from_run, uint32_t from_slot) {
-        uint32_t r = from_run, sl = from_slot;
-        while (r < n_runs && r <= p_run) {
-            const LongRun &d = s_desc[sl];
-            if (d.has_prev && d.first_short != 2) {
-                issue_state(d.state, r);
-                return;
-            }
-            r += W;
-            sl = (sl + 1 == (uint32_t)kLongDescSlots) ? 0 : sl + 1;
+            mbar_expect_tx(bar, kLongTileBytes);
+            tma_load_1d(state_s, s_desc[sl].state, kLongTileBytes, bar);
         }
     };
+    deal.start(units, issue);
 
-    uint32_t phase_bits = 0, slot_i = 0, c_slot = 0;
     for (uint32_t c_run = gw; c_run < n_runs; c_run += W) {
+        const uint32_t my_slot = deal.take_slot();
         RunCurS cur[NB];
-        cur[0] = run_cur_s(s_desc[c_slot]);
-        const uint32_t npk = s_desc[c_slot].n_packets;
-        const uint32_t my_slot = c_slot;
-        c_slot = (c_slot + 1 == (uint32_t)kLongDescSlots) ? 0 : c_slot + 1;
+        cur[0] = run_cur_s(s_desc[my_slot]);
+        const uint32_t npk = s_desc[my_slot].n_packets;
         const bool need_state = (cur[0].flags & 33u) == 1u;
-        if (st_run == ~0u) request_state(c_run, my_slot);
+        deal.begin_state(c_run, needs_state, issue_state);
         V pe[NB][8];
 #pragma unroll
         for (int j = 0; j < 8; j++) pe[0][j] = V{0.f, 0.f};
@@ -1194,75 +1203,29 @@ k_long_s(const LongRun *__restrict__ runs, uint32_t n_runs, const float *__restr
         out[0] = static_cast<OutT *>(cur[0].out);
 
         for (uint32_t p = 0; p < npk; p++) {
-            const uint32_t stage_s = tiles_s + slot_i * kLongTileBytes;
-            mbar_wait(bars_s + 8 * slot_i, (phase_bits >> slot_i) & 1u);
-            phase_bits ^= 1u << slot_i;
+            const uint32_t stage = deal.wait_stage();
             V O[NB][8], E[NB][8];
             {
                 const float *tp[NB];
-                tp[0] = tiles + slot_i * kLongN2;
+                tp[0] = tiles + stage * kLongN2;
                 phase_a<NB>(tp, lane, tw, O, E);
             }
-            __syncwarp();           // every lane has consumed its quads: the tile becomes the scratch
-            {
-                const uint32_t a0 = stage_s + lA0, a1 = stage_s + lA1;
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    sts_eo(a0 ^ LWB_KA(j), E[0][j].x, O[0][j].x);
-                    sts_eo(a1 ^ LWB_KA(j), E[0][j].y, O[0][j].y);
-                }
-            }
-            __syncwarp();
-            {
-                const uint32_t b0 = stage_s + lB;
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    lds_eo(b0 ^ LWB_KB(j, 0), E[0][j].x, O[0][j].x);
-                    lds_eo(b0 ^ LWB_KB(j, 1), E[0][j].y, O[0][j].y);
-                }
-            }
-            __syncwarp();
-            phase_b<NB>(tw, O, E);
-            {
-                const uint32_t b0 = stage_s + lB;
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    sts_eo(b0 ^ LWB_KB(j, 0), E[0][j].x, O[0][j].x);
-                    sts_eo(b0 ^ LWB_KB(j, 1), E[0][j].y, O[0][j].y);
-                }
-            }
-            __syncwarp();
-            {
-                const uint32_t c0 = stage_s + lC0, c1 = stage_s + lC1;
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    lds_eo(c0 ^ LWB_KC(j), E[0][j].x, O[0][j].x);
-                    lds_eo(c1 ^ LWB_KC(j), E[0][j].y, O[0][j].y);
-                }
-            }
-            __syncwarp();
-            if (p_run < n_runs) produce();          // the stage is free again
+            transpose_abc(tw, deal.ring_s + stage * kLongTileBytes, lA0, lA1, lB, lC0, lC1, O, E);
+            deal.produce(units, issue);             // the stage is free again
             phase_c_fft<NB>(tw, O, E);
             if (p > 0) {
                 out_stage<NB, false, OutT, RunCurS>(tw, lane, O, E, pe, cur, out, s_state);
             } else {
-                if (need_state) {
-                    if (st_run != c_run) issue_state(cur[0].state, c_run);  // (its descriptor had not landed when the tile came free)
-                    mbar_wait(bar_state, (phase_bits >> 30) & 1u);
-                    phase_bits ^= 1u << 30;
-                }
+                if (need_state) deal.wait_state(c_run, issue_state);
                 if (cur[0].flags & 8u)
-                    out_first_short<NB, OutT, RunCurS, true, LS>(tw, lane, O, E, pe, cur, out, s_state, w_short, ls, w_s);
+                    out_first_short<NB, OutT, RunCurS, true, ls>(tw, lane, O, E, pe, cur, out, s_state, w_short, ls, w_s);
                 else
                     out_stage<NB, true, OutT, RunCurS>(tw, lane, O, E, pe, cur, out, s_state);
                 __syncwarp();
-                if (need_state) {                                           // state tile consumed: on to the next run that needs it
-                    st_run = ~0u;
-                    request_state(c_run + W, c_slot);
-                }
+                if (need_state) deal.release_state(c_run, needs_state, issue_state);   // state tile consumed
             }
             if (p > 0 || (cur[0].flags & 1u)) out[0] += (p == 0 && (cur[0].flags & 8u)) ? kLongN2 - ls : kLongN2;
-            slot_i = (slot_i + 1 == (uint32_t)kLongRing) ? 0 : slot_i + 1;
+            deal.next_stage();
         }
         if ((cur[0].flags & 16u)) {
             // the last packet precedes a short block: see k_long
@@ -1275,8 +1238,7 @@ k_long_s(const LongRun *__restrict__ runs, uint32_t n_runs, const float *__restr
                 for (int h = 0; h < 2; h++) {
                     const float v = ((j & 1) != 0) == (h == 0) ? pe[0][j].x : pe[0][j].y;
                     const int m = r64 + (h ? 63 - lane : lane);          // x[1024 + m] = x[2047 - m] = v
-                    const bool before = LS ? (r64 < LS) : (m < ls);      // (a multiple of 64: a property of the slot)
-                    if (before) {
+                    if (r64 < ls) {                                      // (a multiple of 64: a property of the slot)
                         if (emitted) st_pcm(out[0] + m, v);
                     } else if (keep && m < kLongN2 - ls) {
                         cur[0].state_out[m - ls] = v;
@@ -1285,14 +1247,7 @@ k_long_s(const LongRun *__restrict__ runs, uint32_t n_runs, const float *__restr
                 }
             }
         } else if ((cur[0].flags & 6u) == 2u) {
-            float *s_lo = cur[0].state_out + lane, *s_hi = cur[0].state_out + 63 - lane;
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const int r64 = 64 * rev3(j);
-                const float vx = (j & 1) ? pe[0][j].x : pe[0][j].y, vy = (j & 1) ? pe[0][j].y : pe[0][j].x;
-                s_lo[r64] = vx; s_hi[r64] = vy;
-                s_hi[960 - r64] = vx; s_lo[960 - r64] = vy;
-            }
+            store_right_half<64, kLongN2 - 64>(cur[0].state_out, lane, pe[0]);
         }
     }
 }
@@ -1301,13 +1256,10 @@ inline int long_launch_static(cudaStream_t stream, const LongRun *d_runs, uint32
                               bool i16_out, const float *d_w_short, int ls)
 {
     if (!n_runs) return 0;
-    const uint32_t want = (n_runs + kLongWarps - 1) / kLongWarps;
-    const uint32_t grid = want < (uint32_t)sm_count ? want : (uint32_t)sm_count;
-    // only blocksize_0 = 256 is instantiated: it is the one short size the one-pass schedule exists for (k_short), and
-    // the runtime-ls variant of this kernel makes ptxas 12.9 crash
-    if (ls != kLongLs256) return 1;
-    if (i16_out) k_long_s<int16_t, kLongLs256><<<grid, kLongWarps * 32, kLongSmemBytesS, stream>>>(d_runs, n_runs, d_pack, d_w_short, ls);
-    else k_long_s<float, kLongLs256><<<grid, kLongWarps * 32, kLongSmemBytesS, stream>>>(d_runs, n_runs, d_pack, d_w_short, ls);
+    const uint32_t grid = static_deal_grid(n_runs, kLongWarps, sm_count);
+    if (ls != kLongLs256) return 1;               // the one short size k_long_s is built for
+    if (i16_out) k_long_s<int16_t><<<grid, kLongWarps * 32, kLongSmemBytesS, stream>>>(d_runs, n_runs, d_pack, d_w_short);
+    else k_long_s<float><<<grid, kLongWarps * 32, kLongSmemBytesS, stream>>>(d_runs, n_runs, d_pack, d_w_short);
     return cudaGetLastError() != cudaSuccess;
 }
 
@@ -1315,8 +1267,8 @@ inline void long_kernel_configure()
 {
     cudaFuncSetAttribute(k_long<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLongSmemBytes);
     cudaFuncSetAttribute(k_long<int16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLongSmemBytes);
-    cudaFuncSetAttribute(k_long_s<float, kLongLs256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLongSmemBytesS);
-    cudaFuncSetAttribute(k_long_s<int16_t, kLongLs256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLongSmemBytesS);
+    cudaFuncSetAttribute(k_long_s<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLongSmemBytesS);
+    cudaFuncSetAttribute(k_long_s<int16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLongSmemBytesS);
 }
 
 // d_runs: n_groups * kLongNB descriptors.  Returns 0 on success; `ticket` must point at a zeroed

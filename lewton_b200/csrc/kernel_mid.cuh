@@ -190,10 +190,8 @@ LWB_HD void phase_a_m(const float *const tile[], int lane, TW tw, V O[8], V E[8]
 // ---------------------------------------------------------------------------------------------
 // device side: k_mid<OutT, KB>.  Descriptors: groups of NB = 2^KB LongRun (48 B each; in_stride / out in N2-sample units of
 // this blocksize, first_short / last_short unused) of equal n_packets -- the host pads a short group with dummies --,
-// dealt to the warps statically (group g -> warp g mod W) like k_long_s: descriptors by cp.async kMidFetch groups ahead,
-// the producer cursor kLongRing stages ahead of the consumer across group boundaries (a stage = the runs' tiles, 4 KB
-// together, which then serve as the E | O planes of the transposes), the state rows of a group with history requested as
-// soon as the state tile is free.
+// under kernel_deal.cuh's static-deal driver: one group per item, one packet per unit (a stage = the runs' tiles, 4 KB
+// together, which then serve as the E | O planes of the transposes), and the state rows of a group with history.
 // ---------------------------------------------------------------------------------------------
 constexpr int kMidFetch = 3;
 template <int KB>
@@ -284,184 +282,83 @@ k_mid(const LongRun *__restrict__ runs, uint32_t n_groups, const float *__restri
     for (int s = kTwReg0; s < kTwReg1; s++) twR[s - kTwReg0] = s_pack[s * 32 + lane];
     const TwMix tw{twR, s_pack + lane};
 
-    const uint32_t tiles_s = smem_u32(tiles), bars_s = smem_u32(bars), desc_s = smem_u32(s_desc);
-    const uint32_t bar_state = bars_s + 8 * kRing, state_s = smem_u32(s_state);
+    const uint32_t state_s = smem_u32(s_state);
     const uint32_t lA0 = laneA(lane, 0), lA1 = laneA(lane, 1);
     const uint32_t lB = laneB(lane);
     const uint32_t lC0 = 4u * (uint32_t)swz(elemC_m<KB>(lane, 0, 0)), lC1 = 4u * (uint32_t)swz(elemC_m<KB>(lane, 0, 1));
 
     const uint32_t W = gridDim.x * kLongWarps, gw = blockIdx.x * kLongWarps + warp;
     if (gw >= n_groups) return;
-    const uint4 *rq = reinterpret_cast<const uint4 *>(runs);
-    constexpr uint32_t kQuads = kGroupBytes / 16;              // 6 / 12 quads per group: one lane each
-    uint32_t f_grp = gw, f_slot = 0;
-    auto fetch = [&]() {
-        if ((uint32_t)lane < kQuads && f_grp < n_groups)
-            cp_async16(desc_s + f_slot * kGroupBytes + lane * 16, rq + (size_t)kQuads * f_grp + lane);
-        cp_async_commit();
-        f_grp += W;
-        f_slot = (f_slot + 1 == (uint32_t)kSlots) ? 0 : f_slot + 1;
-    };
-#pragma unroll
-    for (int i = 0; i <= kMidFetch; i++) fetch();
-    cp_async_wait<kMidFetch>();
-    __syncwarp();
-    // ---- producer (warp-uniform cursor; lanes b < NB issue run b's tile) ----
-    uint32_t p_grp = gw, p_pkt = 0, p_slot = 0, p_stage = 0;
-    uint32_t p_npk = s_desc[0].n_packets;
-    auto produce = [&]() {
-        const uint32_t bar = bars_s + 8 * p_stage, dst = tiles_s + p_stage * kLongTileBytes;
+    StaticDeal<kGroupBytes / 16, kSlots, kMidFetch, kRing, kLongTileBytes> deal(
+        runs, n_groups, W, gw, smem_u32(s_desc), smem_u32(tiles), smem_u32(bars), lane);
+    auto units = [&](uint32_t sl) { return s_desc[NB * sl].n_packets; };
+    auto issue = [&](uint32_t sl, uint32_t pkt, uint32_t bar, uint32_t dst) {     // lanes b < NB issue run b's tile
         if (lane == 0) mbar_expect_tx(bar, NB * kTile);
         __syncwarp();
         if (lane < NB) {
-            const LongRun &r = s_desc[NB * p_slot + lane];
+            const LongRun &r = s_desc[NB * sl + lane];
             fence_proxy_async();          // the stage was written through the generic proxy (transposes) before
-            tma_load_1d(dst + lane * kTile, r.in + (size_t)p_pkt * r.in_stride, kTile, bar);
-        }
-        p_stage = (p_stage + 1 == (uint32_t)kRing) ? 0 : p_stage + 1;
-        if (++p_pkt >= p_npk) {
-            p_grp += W;
-            p_pkt = 0;
-            p_slot = (p_slot + 1 == (uint32_t)kSlots) ? 0 : p_slot + 1;
-            fetch();
-            cp_async_wait<kMidFetch>();
-            __syncwarp();
-            if (p_grp < n_groups) p_npk = s_desc[NB * p_slot].n_packets;
+            tma_load_1d(dst + lane * kTile, r.in + (size_t)pkt * r.in_stride, kTile, bar);
         }
     };
-    for (int i = 0; i < kRing; i++)
-        if (p_grp < n_groups) produce();
-
-    // ---- state rows: st_grp = the group whose rows are in the tile or on their way (~0: the tile is free) ----
-    uint32_t st_grp = ~0u;
     auto group_has_state = [&](uint32_t sl) {
         bool any = false;
 #pragma unroll
         for (int b = 0; b < NB; b++) any |= s_desc[NB * sl + b].has_prev != 0;
         return any;
     };
-    auto issue_state = [&](uint32_t sl, uint32_t grp) {        // warp-uniform; lanes b < NB with history issue their row
+    auto issue_state = [&](uint32_t sl, uint32_t bar) {        // lanes b < NB with history issue their row
         const bool mine = lane < NB && s_desc[NB * sl + (lane < NB ? lane : 0)].has_prev != 0;
         const uint32_t n = (uint32_t)__popc(__ballot_sync(0xffffffffu, mine));
-        if (lane == 0) mbar_expect_tx(bar_state, n * kTile);
+        if (lane == 0) mbar_expect_tx(bar, n * kTile);
         __syncwarp();
         if (mine) {
             fence_proxy_async();
-            tma_load_1d(state_s + lane * kTile, s_desc[NB * sl + lane].state, kTile, bar_state);
-        }
-        st_grp = grp;
-    };
-    auto request_state = [&](uint32_t from_grp, uint32_t from_slot) {       // first group in [from_grp, p_grp] with history
-        uint32_t g = from_grp, sl = from_slot;
-        while (g < n_groups && g <= p_grp) {
-            if (group_has_state(sl)) {
-                issue_state(sl, g);
-                return;
-            }
-            g += W;
-            sl = (sl + 1 == (uint32_t)kSlots) ? 0 : sl + 1;
+            tma_load_1d(state_s + lane * kTile, s_desc[NB * sl + lane].state, kTile, bar);
         }
     };
+    deal.start(units, issue);
 
-    uint32_t phase_bits = 0, slot_i = 0, c_slot = 0;
     for (uint32_t c_grp = gw; c_grp < n_groups; c_grp += W) {
-        const uint32_t my_slot = c_slot;
+        const uint32_t my_slot = deal.take_slot();
         const LongRun *g = s_desc + NB * my_slot;
         const uint32_t npk = g[0].n_packets;
         const bool grp_state = group_has_state(my_slot);
-        // this lane's run (the descriptor slot of the group being consumed is never the target of a fetch: the ring has
-        // slots to spare, see kSlots)
+        // this lane's run (the descriptor slot of the group being consumed is never the target of a fetch)
         const LongRun &mr = g[blk];
         const uint32_t flags = (mr.has_prev ? 1u : 0u) | (mr.write_state ? 2u : 0u) | (mr.dummy ? 4u : 0u);
         OutT *out = static_cast<OutT *>(mr.out);
         float *state_g = mr.state;
-        c_slot = (c_slot + 1 == (uint32_t)kSlots) ? 0 : c_slot + 1;
-        if (st_grp == ~0u) request_state(c_grp, my_slot);
+        deal.begin_state(c_grp, group_has_state, issue_state);
         V pe[8];
 #pragma unroll
         for (int j = 0; j < 8; j++) pe[j] = V{0.f, 0.f};
 
         for (uint32_t p = 0; p < npk; p++) {
-            const uint32_t stage_s = tiles_s + slot_i * kLongTileBytes;
-            mbar_wait(bars_s + 8 * slot_i, (phase_bits >> slot_i) & 1u);
-            phase_bits ^= 1u << slot_i;
+            const uint32_t stage = deal.wait_stage();
             V O[1][8], E[1][8];
             {
                 const float *tp[NB];
 #pragma unroll
-                for (int b = 0; b < NB; b++) tp[b] = tiles + slot_i * kLongN2 + b * M::N2;
+                for (int b = 0; b < NB; b++) tp[b] = tiles + stage * kLongN2 + b * M::N2;
                 phase_a_m<KB>(tp, lane, tw, O[0], E[0]);
             }
-            __syncwarp();           // every lane has consumed its quads: the tiles become the scratch
-            {
-                const uint32_t a0 = stage_s + lA0, a1 = stage_s + lA1;
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    sts_eo(a0 ^ LWB_KA(j), E[0][j].x, O[0][j].x);
-                    sts_eo(a1 ^ LWB_KA(j), E[0][j].y, O[0][j].y);
-                }
-            }
-            __syncwarp();
-            {
-                const uint32_t b0 = stage_s + lB;
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    lds_eo(b0 ^ LWB_KB(j, 0), E[0][j].x, O[0][j].x);
-                    lds_eo(b0 ^ LWB_KB(j, 1), E[0][j].y, O[0][j].y);
-                }
-            }
-            __syncwarp();
-            phase_b<1>(tw, O, E);
-            {
-                const uint32_t b0 = stage_s + lB;
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    sts_eo(b0 ^ LWB_KB(j, 0), E[0][j].x, O[0][j].x);
-                    sts_eo(b0 ^ LWB_KB(j, 1), E[0][j].y, O[0][j].y);
-                }
-            }
-            __syncwarp();
-            {
-                const uint32_t c0 = stage_s + lC0, c1 = stage_s + lC1;
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    lds_eo(c0 ^ LWB_KC(j), E[0][j].x, O[0][j].x);
-                    lds_eo(c1 ^ LWB_KC(j), E[0][j].y, O[0][j].y);
-                }
-            }
-            __syncwarp();
-            if (p_grp < n_groups) produce();          // the stage is free again
+            transpose_abc(tw, deal.ring_s + stage * kLongTileBytes, lA0, lA1, lB, lC0, lC1, O, E);
+            deal.produce(units, issue);             // the stage is free again
             phase_c_fft<1>(tw, O, E);
             if (p > 0) {
                 out_stage_m<KB, false, OutT>(tw, lane, O[0], E[0], pe, flags, out, s_state + blk * M::N2);
             } else {
-                if (grp_state) {
-                    if (st_grp != c_grp) issue_state(my_slot, c_grp);
-                    mbar_wait(bar_state, (phase_bits >> 30) & 1u);
-                    phase_bits ^= 1u << 30;
-                }
+                if (grp_state) deal.wait_state(c_grp, issue_state);
                 out_stage_m<KB, true, OutT>(tw, lane, O[0], E[0], pe, flags, out, s_state + blk * M::N2);
                 __syncwarp();
-                if (grp_state) {                                            // state tile consumed: on to the next group that needs it
-                    st_grp = ~0u;
-                    request_state(c_grp + W, c_slot);
-                }
+                if (grp_state) deal.release_state(c_grp, group_has_state, issue_state);   // state tile consumed
             }
             if (p > 0 || (flags & 1u)) out += M::N2;
-            slot_i = (slot_i + 1 == (uint32_t)kRing) ? 0 : slot_i + 1;
+            deal.next_stage();
         }
-        if ((flags & 6u) == 2u) {             // write_state and not dummy: the lane's 16 values of its run's right half, twice
-            constexpr int Wd = M::W, TOP = M::N2 - M::W;
-            const int hl = lane >> KB;
-            float *s_lo = state_g + hl, *s_hi = state_g + Wd - 1 - hl;
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const int rw = Wd * rev3(j);
-                const float vx = (j & 1) ? pe[j].x : pe[j].y, vy = (j & 1) ? pe[j].y : pe[j].x;
-                s_lo[rw] = vx; s_hi[rw] = vy;                   // state[m]
-                s_hi[TOP - rw] = vx; s_lo[TOP - rw] = vy;       // state[N2 - 1 - m]: same value (imdct.rs:622-649)
-            }
-        }
+        if ((flags & 6u) == 2u)               // write_state and not dummy
+            store_right_half<M::W, M::N2 - M::W>(state_g, lane >> KB, pe);
     }
 }
 
@@ -478,8 +375,7 @@ inline void mid_kernel_configure()
 inline int mid_launch(cudaStream_t stream, const LongRun *d_runs, uint32_t n_groups, const float *d_pack, int sm_count, bool i16_out, int kb)
 {
     if (!n_groups) return 0;
-    const uint32_t want = (n_groups + kLongWarps - 1) / kLongWarps;
-    const uint32_t grid = want < (uint32_t)sm_count ? want : (uint32_t)sm_count;
+    const uint32_t grid = static_deal_grid(n_groups, kLongWarps, sm_count);
     if (kb == 1) {
         if (i16_out) k_mid<int16_t, 1><<<grid, kLongWarps * 32, MidDev<1>::Smem, stream>>>(d_runs, n_groups, d_pack);
         else k_mid<float, 1><<<grid, kLongWarps * 32, MidDev<1>::Smem, stream>>>(d_runs, n_groups, d_pack);

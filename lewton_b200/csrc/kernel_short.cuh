@@ -251,15 +251,86 @@ __device__ __forceinline__ void copy_out4(int16_t *dst, uint32_t src)
     __stcs(reinterpret_cast<uint2 *>(dst), v);
 }
 
+// Transpose addresses (bytes inside the stage; E plane at +0, O plane at +2048).  4 * swzS(b, c) splits into a lane part,
+// an additive slot part (an immediate of the access) and a slot part XORed into bits 2..3 -- the stage bases are
+// 1024-byte aligned, so that XOR can be applied to the full address:
+//   phase A, c = cl + 8 j:   lane part 4 * swzS(b, cl),   + (j << 8),         ^ 4 * (j >> 1)
+//   phase C, c = 8 T + j:    lane part 4 * swzS(b, 8 T),  + ((j >> 2) << 7),  ^ 4 * (j & 3)
+// PCM staging: sample m of block b sits in row b (128 samples) at chunk (m >> 2) ^ b, position m & 3 -- the XOR with b
+// spreads the eight blocks' equal sample indices over the banks.  Lane parts for positions l and 3 - l; the chunk of a
+// slot is a compile-time constant XORed in.
+template <typename OutT>
+struct ShortLanes {
+    uint32_t wA0, wA1, wC0, wC1, wP0, wP1;
+    __device__ __forceinline__ ShortLanes(int l, int blk)
+    {
+        constexpr uint32_t ESZ = sizeof(OutT);
+        wA0 = 4u * (uint32_t)swzS(blk, elemA_s(l, 0, 0)); wA1 = 4u * (uint32_t)swzS(blk, elemA_s(l, 0, 1));
+        wC0 = 4u * (uint32_t)swzS(blk, elemC_s(l, 0, 0)); wC1 = 4u * (uint32_t)swzS(blk, elemC_s(l, 0, 1));
+        wP0 = (128u * ESZ + 4u * ESZ) * (uint32_t)blk + ESZ * (uint32_t)l;
+        wP1 = (128u * ESZ + 4u * ESZ) * (uint32_t)blk + ESZ * (uint32_t)(3 - l);
+    }
+};
+
+// the one transpose, phase A -> phase C (k_short, k_short_g); the stage is the scratch
+template <typename OutT>
+__device__ __forceinline__ void transpose_s(const ShortLanes<OutT> &ln, uint32_t stage_s, V O[8], V E[8])
+{
+    __syncwarp();           // every lane has consumed its quads: the stage becomes the scratch
+    {
+        const uint32_t a0 = stage_s + ln.wA0, a1 = stage_s + ln.wA1;
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+            sts_eo(((a0 ^ (4u * (j >> 1))) + (j << 8)), E[j].x, O[j].x);
+            sts_eo(((a1 ^ (4u * (j >> 1))) + (j << 8)), E[j].y, O[j].y);
+        }
+    }
+    __syncwarp();
+    {
+        const uint32_t c0 = stage_s + ln.wC0, c1 = stage_s + ln.wC1;
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+            lds_eo(((c0 ^ (4u * (j & 3))) + ((j >> 2) << 7)), E[j].x, O[j].x);
+            lds_eo(((c1 ^ (4u * (j & 3))) + ((j >> 2) << 7)), E[j].y, O[j].y);
+        }
+    }
+    __syncwarp();           // scratch consumed: the same bytes now take the PCM staging
+}
+
+// stage slot j's four samples: odd slots hold sample 8 r + l in .x and 8 r + 7 - l in .y, even slots the other way round
+template <typename OutT>
+__device__ __forceinline__ void stage_pcm_slot(const ShortLanes<OutT> &ln, uint32_t stage_s, int j, V lo, V hi)
+{
+    constexpr uint32_t CH = 4u * sizeof(OutT);
+    const uint32_t p0 = stage_s + ln.wP0, p1 = stage_s + ln.wP1;
+    const int r = rev3(j);
+    const uint32_t cA = CH * (2 * r), cB = CH * (2 * r + 1), cC = CH * (31 - 2 * r), cD = CH * (30 - 2 * r);
+    if (j & 1) {
+        sts_pcm(p0 ^ cA, lo.x, (OutT *)nullptr); sts_pcm(p1 ^ cB, lo.y, (OutT *)nullptr);
+        sts_pcm(p1 ^ cC, hi.x, (OutT *)nullptr); sts_pcm(p0 ^ cD, hi.y, (OutT *)nullptr);
+    } else {
+        sts_pcm(p1 ^ cB, lo.x, (OutT *)nullptr); sts_pcm(p0 ^ cA, lo.y, (OutT *)nullptr);
+        sts_pcm(p0 ^ cD, hi.x, (OutT *)nullptr); sts_pcm(p1 ^ cC, hi.y, (OutT *)nullptr);
+    }
+}
+
+// a run's end state: the lane's share of the last block's right half, x[128+m] == x[255-m] (imdct.rs:622-649)
+__device__ __forceinline__ void store_end_state_s(float *end_ptr, int l, const V pe[8])
+{
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        const int mx = outIndex_s(l, j, 0), my = outIndex_s(l, j, 1);
+        end_ptr[mx] = pe[j].x; end_ptr[my] = pe[j].y;
+        end_ptr[127 - mx] = pe[j].x; end_ptr[127 - my] = pe[j].y;
+    }
+}
+
 // runs: one descriptor per run; pack: short_build_pack of the setup's blocksize-8 tables.
 //
-// Runs are dealt to the warps round robin (run r -> warp r mod W): short-block runs are short -- a burst between
-// long blocks is one octet -- so the per-run latencies (descriptor, state row, first tiles) must overlap with the
-// previous runs' arithmetic.  With a static deal every warp knows its future:
-//   * descriptors arrive by cp.async in a small shared ring, kShortFetch runs ahead of their first use;
-//   * the warp PRODUCES a stream of octets (TMA copies of up to eight 512-byte spectrum blocks -- one copy when the
-//     blocks are contiguous --, plus the 512-byte state row in front of a run with history, all counted on the stage's
-//     mbarrier) up to kShortRing stages ahead of where it CONSUMES them, across run boundaries.
+// Short-block runs are short -- a burst between long blocks is one octet --, so the per-run latencies must overlap with
+// the previous runs' arithmetic: kernel_deal.cuh's static-deal driver, one run per item, one octet per unit (TMA copies
+// of up to eight 512-byte spectrum blocks -- one copy when the blocks are contiguous --, plus the 512-byte state row in
+// front of a run with history, all counted on the stage's mbarrier).
 // PCM leaves through shared memory: the lanes' samples are staged (swizzled, conflict-free) and go out as one
 // 128-bit (f32) / 64-bit (i16) store per lane and packet, 512 / 256 contiguous bytes per instruction, instead of
 // 16-byte pieces of eight different lines per instruction, which made the L1 data pipe the limiter.
@@ -292,81 +363,43 @@ k_short(const ShortRun *__restrict__ runs, uint32_t n_runs, const float *__restr
 #pragma unroll
     for (int s = kSTwReg0; s < kSTwReg1; s++) twR[s - kSTwReg0] = s_pack[s * 4 + l];
     const TwShort tw{twR, s_pack + l};
-
-    const uint32_t ring_s = smem_u32(ring), bars_s = smem_u32(bars), desc_s = smem_u32(s_desc);
-    // Transpose addresses (bytes inside the stage; E plane at +0, O plane at +2048).  4 * swzS(b, c) splits into a
-    // lane part, an additive slot part (an immediate of the access) and a slot part XORed into bits 2..3 -- the stage
-    // bases are 1024-byte aligned, so that XOR can be applied to the full address:
-    //   phase A, c = cl + 8 j:   lane part 4 * swzS(b, cl),   + (j << 8),         ^ 4 * (j >> 1)
-    //   phase C, c = 8 T + j:    lane part 4 * swzS(b, 8 T),  + ((j >> 2) << 7),  ^ 4 * (j & 3)
-    const uint32_t wA0 = 4u * (uint32_t)swzS(blk, elemA_s(l, 0, 0)), wA1 = 4u * (uint32_t)swzS(blk, elemA_s(l, 0, 1));
-    const uint32_t wC0 = 4u * (uint32_t)swzS(blk, elemC_s(l, 0, 0)), wC1 = 4u * (uint32_t)swzS(blk, elemC_s(l, 0, 1));
-    // PCM staging: sample m of block b sits in row b (128 samples) at chunk (m >> 2) ^ b, position m & 3 -- the XOR
-    // with b spreads the eight blocks' equal sample indices over the banks.  Lane parts for positions l and 3 - l;
-    // the chunk of a slot is a compile-time constant XORed in.
-    const uint32_t wP0 = (128u * ESZ + 4u * ESZ) * (uint32_t)blk + ESZ * (uint32_t)l;
-    const uint32_t wP1 = (128u * ESZ + 4u * ESZ) * (uint32_t)blk + ESZ * (uint32_t)(3 - l);
+    const ShortLanes<OutT> ln(l, blk);
 
     const uint32_t W = gridDim.x * kShortWarps, gw = blockIdx.x * kShortWarps + warp;
     if (gw >= n_runs) return;
-    const uint4 *rq = reinterpret_cast<const uint4 *>(runs);
-    // ---- descriptor fetch (cp.async groups are per thread: lanes 0..2 copy one quad each, everybody commits / waits) ----
-    uint32_t f_run = gw, f_slot = 0;
-    auto fetch = [&]() {
-        if (lane < 3 && f_run < n_runs) cp_async16(desc_s + f_slot * (uint32_t)sizeof(ShortRun) + lane * 16, rq + 3 * (size_t)f_run + lane);
-        cp_async_commit();
-        f_run += W;
-        f_slot = (f_slot + 1 == (uint32_t)kShortDescSlots) ? 0 : f_slot + 1;
-    };
-#pragma unroll
-    for (int i = 0; i <= kShortFetch; i++) fetch();
-    cp_async_wait<kShortFetch>();
-    __syncwarp();
-    // ---- producer state (warp-uniform) ----
+    StaticDeal<3, kShortDescSlots, kShortFetch, kShortRing, kShortStageBytes> deal(
+        runs, n_runs, W, gw, smem_u32(s_desc), smem_u32(ring), smem_u32(bars), lane);
     // ShortRun fields inside the three quads: q0 = {in, out}, q1 = {state, in_stride, n_packets}, q2 = {has_prev | write_state << 8, ...}
-    uint32_t p_run = gw, p_oct = 0, p_slot = 0, p_stage = 0;
-    uint4 pd0 = s_desc[0], pd1 = s_desc[1], pd2 = s_desc[2];
-    auto produce = [&]() {                                   // whole warp: issue the next octet of the producer's run
-        const float *in = reinterpret_cast<const float *>(((unsigned long long)pd0.y << 32) | pd0.x);
-        const float *state = reinterpret_cast<const float *>(((unsigned long long)pd1.y << 32) | pd1.x);
-        const uint32_t in_stride = pd1.z, npk = pd1.w;
-        const bool with_state = p_oct == 0 && (pd2.x & 0xffu);
-        const uint32_t nb = min((uint32_t)kShortOct, npk - p_oct * kShortOct);
-        const uint32_t bar = bars_s + 8 * p_stage, dst = ring_s + p_stage * kShortStageBytes;
+    auto units = [&](uint32_t sl) { return (s_desc[3 * sl + 1].w + kShortOct - 1) / kShortOct; };
+    auto issue = [&](uint32_t sl, uint32_t oct, uint32_t bar, uint32_t dst) {
+        const uint4 d0 = s_desc[3 * sl], d1 = s_desc[3 * sl + 1], d2 = s_desc[3 * sl + 2];
+        const float *in = reinterpret_cast<const float *>(((unsigned long long)d0.y << 32) | d0.x);
+        const float *state = reinterpret_cast<const float *>(((unsigned long long)d1.y << 32) | d1.x);
+        const uint32_t in_stride = d1.z, npk = d1.w;
+        const bool with_state = oct == 0 && (d2.x & 0xffu);
+        const uint32_t nb = min((uint32_t)kShortOct, npk - oct * kShortOct);
         const bool contig = in_stride == (uint32_t)kShortN2;
         if (lane == 0) mbar_expect_tx(bar, (nb + (with_state ? 1u : 0u)) * (uint32_t)(kShortN2 * 4));
         __syncwarp();
         if (contig) {
             if (lane == 0) {
                 fence_proxy_async();        // the stage was written through the generic proxy (transpose, staging) before
-                tma_load_1d(dst, in + (size_t)(p_oct * kShortOct) * kShortN2, nb * (uint32_t)(kShortN2 * 4), bar);
+                tma_load_1d(dst, in + (size_t)(oct * kShortOct) * kShortN2, nb * (uint32_t)(kShortN2 * 4), bar);
             }
         } else if ((uint32_t)lane < nb) {
             fence_proxy_async();
-            tma_load_1d(dst + lane * kShortTileStride, in + (size_t)(p_oct * kShortOct + lane) * in_stride, kShortN2 * 4, bar);
+            tma_load_1d(dst + lane * kShortTileStride, in + (size_t)(oct * kShortOct + lane) * in_stride, kShortN2 * 4, bar);
         }
         if (lane == 8 && with_state) {
             fence_proxy_async();
             tma_load_1d(dst + kShortStateOff, state, kShortN2 * 4, bar);
         }
-        p_stage = (p_stage + 1 == (uint32_t)kShortRing) ? 0 : p_stage + 1;
-        if (++p_oct * kShortOct >= npk) {                    // on to the next run of this warp
-            p_run += W;
-            p_oct = 0;
-            p_slot = (p_slot + 1 == (uint32_t)kShortDescSlots) ? 0 : p_slot + 1;
-            fetch();                                         // run p_run + kShortFetch * W
-            cp_async_wait<kShortFetch>();                    // run p_run's descriptor (fetched kShortFetch runs ago) has landed
-            __syncwarp();
-            if (p_run < n_runs) { pd0 = s_desc[3 * p_slot]; pd1 = s_desc[3 * p_slot + 1]; pd2 = s_desc[3 * p_slot + 2]; }
-        }
     };
-    for (int i = 0; i < kShortRing; i++)
-        if (p_run < n_runs) produce();
+    deal.start(units, issue);
 
-    uint32_t phase_bits = 0, slot_i = 0, c_slot = 0;
     for (uint32_t c_run = gw; c_run < n_runs; c_run += W) {
-        const uint4 d0 = s_desc[3 * c_slot], d1 = s_desc[3 * c_slot + 1], d2 = s_desc[3 * c_slot + 2];
-        c_slot = (c_slot + 1 == (uint32_t)kShortDescSlots) ? 0 : c_slot + 1;
+        const uint32_t sl = deal.take_slot();
+        const uint4 d0 = s_desc[3 * sl], d1 = s_desc[3 * sl + 1], d2 = s_desc[3 * sl + 2];
         OutT *out = reinterpret_cast<OutT *>(((unsigned long long)d0.w << 32) | d0.z);
         float *state = reinterpret_cast<float *>(((unsigned long long)d1.y << 32) | d1.x);
         const uint32_t npk = d1.w;
@@ -382,34 +415,14 @@ k_short(const ShortRun *__restrict__ runs, uint32_t n_runs, const float *__restr
         for (int j = 0; j < 8; j++) carry[j] = V{0.f, 0.f};
         V pe[8];
         for (uint32_t o = 0; o < n_oct; o++) {
-            const uint32_t stage_s = ring_s + slot_i * kShortStageBytes;
-            const unsigned char *stage_p = ring + slot_i * kShortStageBytes;
-            mbar_wait(bars_s + 8 * slot_i, (phase_bits >> slot_i) & 1u);
-            phase_bits ^= 1u << slot_i;
+            const uint32_t stage = deal.wait_stage();
+            const uint32_t stage_s = deal.ring_s + stage * kShortStageBytes;
+            const unsigned char *stage_p = ring + stage * kShortStageBytes;
             V O[8], E[8];
             phase_a_s(reinterpret_cast<const float *>(stage_p + blk * (contig ? kShortN2 * 4 : kShortTileStride)), l, tw, O, E);
             const bool first0 = (o == 0 && blk == 0);
-            __syncwarp();           // every lane has consumed its quads: the stage becomes the scratch
-            {
-                const uint32_t a0 = stage_s + wA0, a1 = stage_s + wA1;
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    sts_eo(((a0 ^ (4u * (j >> 1))) + (j << 8)), E[j].x, O[j].x);
-                    sts_eo(((a1 ^ (4u * (j >> 1))) + (j << 8)), E[j].y, O[j].y);
-                }
-            }
-            __syncwarp();
-            {
-                const uint32_t c0 = stage_s + wC0, c1 = stage_s + wC1;
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    lds_eo(((c0 ^ (4u * (j & 3))) + ((j >> 2) << 7)), E[j].x, O[j].x);
-                    lds_eo(((c1 ^ (4u * (j & 3))) + ((j >> 2) << 7)), E[j].y, O[j].y);
-                }
-            }
-            __syncwarp();           // scratch consumed: the same bytes now take the PCM staging
+            transpose_s(ln, stage_s, O, E);
             phase_c_fft<1>(tw, &O, &E);
-            const uint32_t p0 = stage_s + wP0, p1 = stage_s + wP1;
 #pragma unroll
             for (int j = 0; j < 8; j++) {
                 V p_odd;
@@ -430,17 +443,7 @@ k_short(const ShortRun *__restrict__ runs, uint32_t n_runs, const float *__restr
                 }
                 V lo, hi;
                 ola_s(p_odd, tw(P_WLO + j), tw(P_WHI + j), plo, phi, lo, hi);
-                // stage: odd slots hold sample 8 r + l in .x and 8 r + 7 - l in .y, even slots the other way round
-                constexpr uint32_t CH = 4u * ESZ;
-                const int r = rev3(j);
-                const uint32_t cA = CH * (2 * r), cB = CH * (2 * r + 1), cC = CH * (31 - 2 * r), cD = CH * (30 - 2 * r);
-                if (j & 1) {
-                    sts_pcm(p0 ^ cA, lo.x, (OutT *)nullptr); sts_pcm(p1 ^ cB, lo.y, (OutT *)nullptr);
-                    sts_pcm(p1 ^ cC, hi.x, (OutT *)nullptr); sts_pcm(p0 ^ cD, hi.y, (OutT *)nullptr);
-                } else {
-                    sts_pcm(p1 ^ cB, lo.x, (OutT *)nullptr); sts_pcm(p0 ^ cA, lo.y, (OutT *)nullptr);
-                    sts_pcm(p0 ^ cD, hi.x, (OutT *)nullptr); sts_pcm(p1 ^ cC, hi.y, (OutT *)nullptr);
-                }
+                stage_pcm_slot(ln, stage_s, j, lo, hi);
             }
 #pragma unroll
             for (int j = 0; j < 8; j++) carry[j] = pe[j];
@@ -456,18 +459,12 @@ k_short(const ShortRun *__restrict__ runs, uint32_t n_runs, const float *__restr
                 }
             }
             __syncwarp();                                        // staging and state tile consumed: the stage is free
-            if (p_run < n_runs) produce();
-            slot_i = (slot_i + 1 == (uint32_t)kShortRing) ? 0 : slot_i + 1;
+            deal.produce(units, issue);
+            deal.next_stage();
         }
-        if (write_state && (uint32_t)blk == ((npk - 1) & (kShortOct - 1))) {
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const int mx = outIndex_s(l, j, 0), my = outIndex_s(l, j, 1);
-                end_ptr[mx] = pe[j].x; end_ptr[my] = pe[j].y;
-                end_ptr[127 - mx] = pe[j].x; end_ptr[127 - my] = pe[j].y;     // x[128+m] == x[255-m] (imdct.rs:622-649)
-            }
-        }
-        if (tail && (uint32_t)blk == ((npk - 1) & (kShortOct - 1))) {
+        const bool last = (uint32_t)blk == ((npk - 1) & (kShortOct - 1));
+        if (write_state && last) store_end_state_s(end_ptr, l, pe);
+        if (tail && last) {
             // pcm[i] = x_long[ls + i] w[i] + prev[i] w[127 - i]: the first product comes from the long kernel, prev is this
             // block's right half (prev[m] == prev[127 - m] == p_even)
             OutT *on = out + (size_t)(npk - koff) * kShortN2;
@@ -497,8 +494,8 @@ k_short(const ShortRun *__restrict__ runs, uint32_t n_runs, const float *__restr
 // a warp belong to EIGHT DIFFERENT runs of equal length (a "group"; the host sorts the short runs by length and pads
 // each length class with dummies) which advance in lockstep, one packet per iteration -- so block position b's previous
 // right half is simply its own p_even of the iteration before (registers, no shuffle), or its run's state tile in
-// iteration 0.  Descriptors: 8 ShortRun per group (dummy: in == nullptr).  Same static deal, descriptor ring and
-// producer / consumer stages as k_short; a stage carries the eight state tiles behind the eight spectrum tiles.
+// iteration 0.  Descriptors: 8 ShortRun per group (dummy: in == nullptr).  The static-deal driver of k_short with one
+// group per item and one packet per unit; a stage carries the eight state tiles behind the eight spectrum tiles.
 // ---------------------------------------------------------------------------------------------
 constexpr int kShortGRing = 2;
 constexpr int kShortGStageBytes = kShortOct * kShortTileStride + kShortOct * kShortN2 * 4 + 512;     // 4608 + 4096 -> 9216 (1024-aligned)
@@ -536,64 +533,32 @@ k_short_g(const ShortRun *__restrict__ runs, uint32_t n_groups, const float *__r
 #pragma unroll
     for (int s = kSTwReg0; s < kSTwReg1; s++) twR[s - kSTwReg0] = s_pack[s * 4 + l];
     const TwShort tw{twR, s_pack + l};
-
-    const uint32_t ring_s = smem_u32(ring), bars_s = smem_u32(bars), desc_s = smem_u32(s_desc);
-    const uint32_t wA0 = 4u * (uint32_t)swzS(blk, elemA_s(l, 0, 0)), wA1 = 4u * (uint32_t)swzS(blk, elemA_s(l, 0, 1));
-    const uint32_t wC0 = 4u * (uint32_t)swzS(blk, elemC_s(l, 0, 0)), wC1 = 4u * (uint32_t)swzS(blk, elemC_s(l, 0, 1));
-    const uint32_t wP0 = (128u * ESZ + 4u * ESZ) * (uint32_t)blk + ESZ * (uint32_t)l;
-    const uint32_t wP1 = (128u * ESZ + 4u * ESZ) * (uint32_t)blk + ESZ * (uint32_t)(3 - l);
+    const ShortLanes<OutT> ln(l, blk);
     constexpr uint32_t kStateOff = kShortOct * kShortTileStride;               // state tile of block b at + 512 b
 
     const uint32_t W = gridDim.x * kShortWarps, gw = blockIdx.x * kShortWarps + warp;
     if (gw >= n_groups) return;
-    const uint4 *rq = reinterpret_cast<const uint4 *>(runs);
-    constexpr uint32_t kQuads = (uint32_t)(kShortGDescBytes / 16);             // 24 quads per group: lanes 0..23 copy one each
-    uint32_t f_grp = gw, f_slot = 0;
-    auto fetch = [&]() {
-        if ((uint32_t)lane < kQuads && f_grp < n_groups)
-            cp_async16(desc_s + f_slot * (uint32_t)kShortGDescBytes + lane * 16, rq + (size_t)kQuads * f_grp + lane);
-        cp_async_commit();
-        f_grp += W;
-        f_slot = (f_slot + 1 == (uint32_t)kShortGDescSlots) ? 0 : f_slot + 1;
-    };
-#pragma unroll
-    for (int i = 0; i <= kShortGFetch; i++) fetch();
-    cp_async_wait<kShortGFetch>();
-    __syncwarp();
-    // ---- producer: iteration p_t of group p_grp; lane b < 8 issues block position b's copies ----
-    uint32_t p_grp = gw, p_t = 0, p_slot = 0, p_stage = 0;
-    auto produce = [&]() {
-        const ShortRun *g = s_desc + p_slot * kShortOct;
-        const uint32_t npk = g[0].n_packets;
+    StaticDeal<kShortGDescBytes / 16, kShortGDescSlots, kShortGFetch, kShortGRing, kShortGStageBytes> deal(
+        runs, n_groups, W, gw, smem_u32(s_desc), smem_u32(ring), smem_u32(bars), lane);
+    auto units = [&](uint32_t sl) { return s_desc[sl * kShortOct].n_packets; };
+    auto issue = [&](uint32_t sl, uint32_t t, uint32_t bar, uint32_t dst) {     // lane b < 8 issues block position b's copies
+        const ShortRun *g = s_desc + sl * kShortOct;
         const bool mine = lane < kShortOct && g[lane & 7].in != nullptr;
-        const bool st = mine && p_t == 0 && g[lane & 7].has_prev;
+        const bool st = mine && t == 0 && g[lane & 7].has_prev;
         const uint32_t n_tiles = (uint32_t)__popc(__ballot_sync(0xffffffffu, mine)) + (uint32_t)__popc(__ballot_sync(0xffffffffu, st));
-        const uint32_t bar = bars_s + 8 * p_stage, dst = ring_s + p_stage * kShortGStageBytes;
         if (lane == 0) mbar_expect_tx(bar, n_tiles * (uint32_t)(kShortN2 * 4));
         __syncwarp();
         if (mine) {
             fence_proxy_async();
-            tma_load_1d(dst + lane * kShortTileStride, g[lane].in + (size_t)p_t * g[lane].in_stride, kShortN2 * 4, bar);
+            tma_load_1d(dst + lane * kShortTileStride, g[lane].in + (size_t)t * g[lane].in_stride, kShortN2 * 4, bar);
             if (st) tma_load_1d(dst + kStateOff + lane * (kShortN2 * 4), g[lane].state, kShortN2 * 4, bar);
         }
-        p_stage = (p_stage + 1 == (uint32_t)kShortGRing) ? 0 : p_stage + 1;
-        if (++p_t >= npk) {
-            p_grp += W;
-            p_t = 0;
-            p_slot = (p_slot + 1 == (uint32_t)kShortGDescSlots) ? 0 : p_slot + 1;
-            fetch();
-            cp_async_wait<kShortGFetch>();
-            __syncwarp();
-        }
     };
-    for (int i = 0; i < kShortGRing; i++)
-        if (p_grp < n_groups) produce();
+    deal.start(units, issue);
 
-    uint32_t phase_bits = 0, slot_i = 0, c_slot = 0;
     for (uint32_t c_grp = gw; c_grp < n_groups; c_grp += W) {
-        const ShortRun *g = s_desc + c_slot * kShortOct;
-        c_slot = (c_slot + 1 == (uint32_t)kShortGDescSlots) ? 0 : c_slot + 1;
-        // (the descriptor slot of the group being consumed is never the target of a fetch: the ring has two slots to spare)
+        // (the descriptor slot of the group being consumed is never the target of a fetch)
+        const ShortRun *g = s_desc + deal.take_slot() * kShortOct;
         const uint32_t npk = g[0].n_packets;
         const bool valid = g[blk].in != nullptr, has_prev = valid && g[blk].has_prev;
         uint32_t emit0 = 0;               // bit i: position i emits in iteration 0; bit 8 + i: position i is not a dummy
@@ -604,33 +569,13 @@ k_short_g(const ShortRun *__restrict__ runs, uint32_t n_groups, const float *__r
 #pragma unroll
         for (int j = 0; j < 8; j++) pe[j] = V{0.f, 0.f};
         for (uint32_t t = 0; t < npk; t++) {
-            const uint32_t stage_s = ring_s + slot_i * kShortGStageBytes;
-            const unsigned char *stage_p = ring + slot_i * kShortGStageBytes;
-            mbar_wait(bars_s + 8 * slot_i, (phase_bits >> slot_i) & 1u);
-            phase_bits ^= 1u << slot_i;
+            const uint32_t stage = deal.wait_stage();
+            const uint32_t stage_s = deal.ring_s + stage * kShortGStageBytes;
+            const unsigned char *stage_p = ring + stage * kShortGStageBytes;
             V O[8], E[8];
             phase_a_s(reinterpret_cast<const float *>(stage_p + blk * kShortTileStride), l, tw, O, E);
-            __syncwarp();           // every lane has consumed its quads: the stage becomes the scratch
-            {
-                const uint32_t a0 = stage_s + wA0, a1 = stage_s + wA1;
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    sts_eo(((a0 ^ (4u * (j >> 1))) + (j << 8)), E[j].x, O[j].x);
-                    sts_eo(((a1 ^ (4u * (j >> 1))) + (j << 8)), E[j].y, O[j].y);
-                }
-            }
-            __syncwarp();
-            {
-                const uint32_t c0 = stage_s + wC0, c1 = stage_s + wC1;
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    lds_eo(((c0 ^ (4u * (j & 3))) + ((j >> 2) << 7)), E[j].x, O[j].x);
-                    lds_eo(((c1 ^ (4u * (j & 3))) + ((j >> 2) << 7)), E[j].y, O[j].y);
-                }
-            }
-            __syncwarp();           // scratch consumed: the same bytes now take the PCM staging
+            transpose_s(ln, stage_s, O, E);
             phase_c_fft<1>(tw, &O, &E);
-            const uint32_t p0 = stage_s + wP0, p1 = stage_s + wP1;
 #pragma unroll
             for (int j = 0; j < 8; j++) {
                 V p_odd, lo, hi;
@@ -644,16 +589,7 @@ k_short_g(const ShortRun *__restrict__ runs, uint32_t n_groups, const float *__r
                     phi = V{lds_f32(sa + 4 * (127 - mx)), lds_f32(sa + 4 * (127 - my))};
                 }
                 ola_s(p_odd, tw(P_WLO + j), tw(P_WHI + j), plo, phi, lo, hi);
-                constexpr uint32_t CH = 4u * ESZ;
-                const int r = rev3(j);
-                const uint32_t cA = CH * (2 * r), cB = CH * (2 * r + 1), cC = CH * (31 - 2 * r), cD = CH * (30 - 2 * r);
-                if (j & 1) {
-                    sts_pcm(p0 ^ cA, lo.x, (OutT *)nullptr); sts_pcm(p1 ^ cB, lo.y, (OutT *)nullptr);
-                    sts_pcm(p1 ^ cC, hi.x, (OutT *)nullptr); sts_pcm(p0 ^ cD, hi.y, (OutT *)nullptr);
-                } else {
-                    sts_pcm(p1 ^ cB, lo.x, (OutT *)nullptr); sts_pcm(p0 ^ cA, lo.y, (OutT *)nullptr);
-                    sts_pcm(p0 ^ cD, hi.x, (OutT *)nullptr); sts_pcm(p1 ^ cC, hi.y, (OutT *)nullptr);
-                }
+                stage_pcm_slot(ln, stage_s, j, lo, hi);
             }
             __syncwarp();
             // one packet per instruction: lane L copies samples [4 L, 4 L + 4) of position i's packet t
@@ -667,18 +603,11 @@ k_short_g(const ShortRun *__restrict__ runs, uint32_t n_groups, const float *__r
                 }
             }
             __syncwarp();                                        // staging consumed: the stage is free
-            if (p_grp < n_groups) produce();
-            slot_i = (slot_i + 1 == (uint32_t)kShortGRing) ? 0 : slot_i + 1;
+            deal.produce(units, issue);
+            deal.next_stage();
         }
         float *end_ptr = g[blk].end_ptr ? g[blk].end_ptr : g[blk].state;
-        if (valid && g[blk].write_state) {
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const int mx = outIndex_s(l, j, 0), my = outIndex_s(l, j, 1);
-                end_ptr[mx] = pe[j].x; end_ptr[my] = pe[j].y;
-                end_ptr[127 - mx] = pe[j].x; end_ptr[127 - my] = pe[j].y;
-            }
-        }
+        if (valid && g[blk].write_state) store_end_state_s(end_ptr, l, pe);
         if (valid && g[blk].tail) {
             OutT *on = static_cast<OutT *>(g[blk].out) + (size_t)(npk - (has_prev ? 0u : 1u)) * kShortN2;
             float cw[8][4];
@@ -704,8 +633,7 @@ k_short_g(const ShortRun *__restrict__ runs, uint32_t n_groups, const float *__r
 inline int short_launch_groups(cudaStream_t stream, const ShortRun *d_runs, uint32_t n_groups, const float *d_pack, int sm_count, bool i16_out)
 {
     if (!n_groups) return 0;
-    const uint32_t want = (n_groups + kShortWarps - 1) / kShortWarps;
-    const uint32_t grid = want < (uint32_t)sm_count ? want : (uint32_t)sm_count;
+    const uint32_t grid = static_deal_grid(n_groups, kShortWarps, sm_count);
     if (i16_out) k_short_g<int16_t><<<grid, kShortWarps * 32, kShortGSmemBytes, stream>>>(d_runs, n_groups, d_pack);
     else k_short_g<float><<<grid, kShortWarps * 32, kShortGSmemBytes, stream>>>(d_runs, n_groups, d_pack);
     return cudaGetLastError() != cudaSuccess;
@@ -722,8 +650,7 @@ inline void short_kernel_configure()
 inline int short_launch(cudaStream_t stream, const ShortRun *d_runs, uint32_t n_runs, const float *d_pack, int sm_count, bool i16_out)
 {
     if (!n_runs) return 0;
-    const uint32_t want = (n_runs + kShortWarps - 1) / kShortWarps;
-    const uint32_t grid = want < (uint32_t)sm_count ? want : (uint32_t)sm_count;
+    const uint32_t grid = static_deal_grid(n_runs, kShortWarps, sm_count);
     if (i16_out) k_short<int16_t><<<grid, kShortWarps * 32, kShortSmemBytes, stream>>>(d_runs, n_runs, d_pack);
     else k_short<float><<<grid, kShortWarps * 32, kShortSmemBytes, stream>>>(d_runs, n_runs, d_pack);
     return cudaGetLastError() != cudaSuccess;

@@ -103,7 +103,7 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
         }
         groups.push_back(g);
     }
-    const size_t Wg = std::min<size_t>((groups.size() + kLongWarps - 1) / kLongWarps, (size_t)ctx->sm_count) * kLongWarps;
+    const size_t Wg = (size_t)static_deal_grid(groups.size(), kLongWarps, ctx->sm_count) * kLongWarps;
     balance_static_deal(groups.data(), groups.size(), Wg, tmp_g);
     const size_t bytes = groups.size() * NBg * sizeof(LongRun);
     Staging *st;

@@ -437,18 +437,15 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                             groups.back().r[in_class++ % kShortOct] = br;
                         }
                     }
-                    const size_t Wg = std::min<size_t>((groups.size() + kShortWarps - 1) / kShortWarps, (size_t)ctx->sm_count) * kShortWarps;
+                    const size_t Wg = (size_t)static_deal_grid(groups.size(), kShortWarps, ctx->sm_count) * kShortWarps;
                     if (!getenv("LWB_NO_BALANCE")) balance_static_deal(groups.data(), groups.size(), Wg, tmp_g);
                     if ((wg + groups.size()) * kShortOct > sg_cap) return fail(ctx, LWB_ERR_INVALID, "burst group area too small");
                     for (const ShortGroup &gr : groups) std::memcpy(h_sg + (wg++) * kShortOct, gr.r, sizeof(gr.r));
                 }
                 const size_t nr = wr - r0, ns = ws - s0;
                 if (flat && r == 0 && !getenv("LWB_NO_BALANCE")) {
-                    auto warps_of = [&](size_t n, int per_cta) {
-                        return std::min<size_t>((n + per_cta - 1) / per_cta, (size_t)ctx->sm_count) * per_cta;
-                    };
-                    balance_static_deal(h_runs + r0, nr, warps_of(nr, kLongWarps), tmp_lr);
-                    balance_static_deal(h_sr + s0, ns, warps_of(ns, kShortWarps), tmp_sr);
+                    balance_static_deal(h_runs + r0, nr, (size_t)static_deal_grid(nr, kLongWarps, ctx->sm_count) * kLongWarps, tmp_lr);
+                    balance_static_deal(h_sr + s0, ns, (size_t)static_deal_grid(ns, kShortWarps, ctx->sm_count) * kShortWarps, tmp_sr);
                 }
                 // the round's launches: the row copies go before k_long_s, and the short kernels complete the boundary
                 // slots k_long_s left
