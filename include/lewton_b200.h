@@ -253,7 +253,10 @@ enum { LWB_ENTRY_SPECTRUM = 0,   /* coeffs = floor x residue, enters at audio.rs
                                   * (audio.rs:587-717); coeff_offset still lays out the (device-only)   *
                                   * coefficient arena.  Needs the setup's codebooks / residues, <= 8     *
                                   * channels, channels * n/2 <= 12288, VQ books of <= 65536 entries whose   *
-                                  * dimension divides their residue's partition size.                     */
+                                  * dimension divides their residue's partition size.  Every batch shape  *
+                                  * runs on the kernels of its dense LWB_ENTRY_RESIDUE twin: k_long, the  *
+                                  * segmented schedules, k_mid, and k_chain for the rest (interleaved     *
+                                  * output, other blocksizes), which accumulates in shared memory itself. */
 /* The VQ vectors of a packet's residue, in the order the entropy decoder produces them (SURVEY.md 8f rank 2), as RUNS:
  * one run = the consecutive vectors one residue_packet_read_partition call reads (audio.rs:587-618) -- same codebook,
  * same pass, positions in arithmetic progression -- plus one 16-bit codebook entry per vector in a side array.  The
@@ -363,7 +366,9 @@ int lwb_decode_chains(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lw
  *   - arena growth: a staging arena of a host set grows after that set's previous ticket has completed; the
  *     context's other arenas grow after the compute stream has drained;
  *   - staging-ring wrap: descriptors are written to pinned staging that waits for the copy three stagings back;
- *   - the four-kernel path synchronises once per round before it writes its pinned descriptors.
+ *   - the four-kernel path synchronises once per round before it writes its pinned descriptors.  It takes only batches
+ *     of more than 8 channels or with buffers beyond shared memory (LWB_ENTRY_VQ batches included: those of every
+ *     other shape run on k_chain or the fused kernels).
  * lwb_ctx_synchronize, lwb_ctx_destroy and lwb_stream_destroy wait for every queued copy as well as every kernel. */
 int lwb_submit_chains(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, uint64_t *ticket);
 /* *done = 1 once every copy and kernel of `ticket` has finished (a host-memory batch's PCM is in `pcm`), else 0.

@@ -115,11 +115,12 @@ struct StepArgs {
     int mid_kb = 0;                                         // k_mid: 1 for n = 1024, 2 for n = 512
     ChainShape chain = {};                                  // k_chain
     const uint8_t *bytes = nullptr;                         // k_chain: mode bytes (ChainDesc::byte_off)
-    bool residue = false;                                   // k_chain: its own front half on residues
+    int entry = LWB_ENTRY_SPECTRUM;                         // k_chain: else its own front half on residues / VQ records
     const float *coeffs = nullptr, *dense = nullptr;
     const uint8_t *kinds = nullptr;
     const uint32_t *ys = nullptr;
     const float *zero = nullptr;                            // k_chain: curves of LWB_FLOOR_ZERO rows, or nullptr
+    VqDev vq = {};                                          // k_chain, LWB_ENTRY_VQ: the batch's VQ arrays
 };
 
 // One launch of the residue entry's front stages (k_floor1_segments + k_prologue_fused, or k_prologue): floor x

@@ -1,11 +1,14 @@
 // kernel_chain.cuh -- the general synthesis kernel: any blocksize 6..13, mixed short/long
-// sequences, up to 8 channels, spectrum or residue entry, all output formats, in ONE launch.
+// sequences, up to 8 channels, spectrum, residue or VQ entry, all output formats, in ONE launch.
 //
 // One CTA owns one chain (consecutive packets of one stream), one group of `wpc` warps per channel
 // (1 warp for small blocks, up to 8 for n = 8192; the group synchronises on its own named barrier).
 // The group keeps its channel's working buffers (U, V: n/2 floats each) and the previous block's right half
 // (PreviousWindowRight, audio.rs:847-861) in shared memory for the whole chain, so HBM sees only the
 // algorithmic traffic: coefficients in, PCM out, the stream state once per chain.  Per packet:
+//   VQ entry:      the whole CTA accumulates the packet's residue vectors from its VQ records into a [C][n/2]
+//                  region of shared memory (d_vq_accumulate, kernel_prologue.cuh), then goes on as the residue
+//                  entry does, reading them there instead of from the coefficient arena;
 //   residue entry: floor-1 posts per channel (one lane, serial, <= 65 posts; floor-0 curves come rendered by
 //                  k_floor0_curves) -> the whole CTA does
 //                  inverse coupling + floor x residue bin-parallel straight into the channels'
@@ -21,6 +24,7 @@
 // in shared memory: a chain's buffers and state stay there instead of round-tripping HBM between kernels.
 #pragma once
 #include "kernels_generic.cuh"
+#include "kernel_prologue.cuh"
 
 namespace lwb {
 
@@ -60,12 +64,13 @@ __device__ __forceinline__ float d_x_at(const float *V, const float *__restrict_
 // MULTI = false: one warp per channel (<= 8 warps, compile-time group size, warp-level syncs);
 // MULTI = true: `wpc` warps per channel, named barriers.
 // np: blocks a channel group transforms together (spectrum entry, !MULTI; the host sizes shared memory for it).
+// vq: the batch's VQ arrays (VQ entry; `coeffs` is not read then).
 template <int FORMAT, int ENTRY, bool MULTI>
 __global__ void __launch_bounds__(MULTI ? 1024 : 256)
 k_chain(const ChainDesc *__restrict__ chains, const uint8_t *__restrict__ pkt_bytes, const float *__restrict__ coeffs,
         const float *__restrict__ dense_floor, const uint8_t *__restrict__ floor_kind,
         const uint32_t *__restrict__ floor1_y, void *__restrict__ pcm, int n1max, int wpc, int np,
-        const float *__restrict__ zero_floor)
+        const float *__restrict__ zero_floor, VqDev vq)
 {
     extern __shared__ float ch_smem[];
     const ChainDesc cd = chains[blockIdx.x];
@@ -85,6 +90,8 @@ k_chain(const ChainDesc *__restrict__ chains, const uint8_t *__restrict__ pkt_by
     uint16_t *s_x = reinterpret_cast<uint16_t *>(ch_smem + (size_t)W * per_warp);
     uint16_t *s_y = s_x + 8 * (LWB_MAX_POSTS + 1);
     int *s_m = reinterpret_cast<int *>(s_y + 8 * (LWB_MAX_POSTS + 1));
+    // VQ entry: the packet's residue vectors, [C][n/2] (the host sizes this region for C * n1max / 2 floats)
+    float *s_acc = reinterpret_cast<float *>(s_m + 8);
 
     const int n0 = 1 << su.bs0;
     bool has = cd.has0;
@@ -105,22 +112,29 @@ k_chain(const ChainDesc *__restrict__ chains, const uint8_t *__restrict__ pkt_by
         if (ENTRY == LWB_ENTRY_SPECTRUM && !MULTI)
             while (g < (uint32_t)np && p + g < cd.n_packets && su.mode_blockflag[bytes[3 * (p + g)]] == blockflag) g++;
 
-        if (ENTRY == LWB_ENTRY_RESIDUE) {
+        if (ENTRY != LWB_ENTRY_SPECTRUM) {
             const int mode = bytes[3 * p];
             const DevMapping &mp = su.mappings[su.mode_mapping[mode]];
             const uint64_t row = (cd.pkt_index + p) * C;
-            __syncthreads();              // previous packet finished with U/V and the post arrays
+            __syncthreads();              // previous packet finished with U/V, the post arrays and the accumulators
             if (active && lane == 0 && floor_kind[row + warp] == LWB_FLOOR_ONE) {
                 const DevFloor1 &fl = su.floors[mp.floor_of_channel[warp]];
                 s_m[warp] = d_floor1_posts(fl, floor1_y + (row + warp) * LWB_MAX_POSTS, n2,
                                            s_x + warp * (LWB_MAX_POSTS + 1), s_y + warp * (LWB_MAX_POSTS + 1));
+            }
+            if (ENTRY == LWB_ENTRY_VQ) {
+                const uint64_t pk = cd.pkt_index + p;
+                const uint64_t o0 = vq.run_off[pk], e0 = vq.ent_off[pk];
+                d_vq_accumulate(s_acc, C, n2, su, mp, vq.runs + o0, (uint32_t)(vq.run_off[pk + 1] - o0), vq.entries + e0,
+                                (uint32_t)(vq.ent_off[pk + 1] - e0), threadIdx.x, blockDim.x);
             }
             __syncthreads();
             const int nsteps = mp.n_coupling;
             for (int k = threadIdx.x; k < n2; k += blockDim.x) {
                 float r[8];
 #pragma unroll
-                for (int c = 0; c < 8; c++) r[c] = c < C ? coeffs[coeff + (size_t)c * n2 + k] : 0.f;
+                for (int c = 0; c < 8; c++)
+                    r[c] = c < C ? (ENTRY == LWB_ENTRY_VQ ? s_acc[c * n2 + k] : coeffs[coeff + (size_t)c * n2 + k]) : 0.f;
                 for (int s = nsteps - 1; s >= 0; s--) {       // audio.rs:991-1002
                     const int mi = mp.mag[s], ai = mp.ang[s];
                     float mv = 0.f, av = 0.f;
@@ -147,7 +161,7 @@ k_chain(const ChainDesc *__restrict__ chains, const uint8_t *__restrict__ pkt_by
 
         if (active) {
             float *V0 = U + (n1max >> 1);
-            if (ENTRY == LWB_ENTRY_RESIDUE) {
+            if (ENTRY != LWB_ENTRY_SPECTRUM) {
                 d_imdct_to_v(tb, n, U, U, V0, lane, gt, gsync);
             } else {
                 const float *X = coeffs + coeff + (size_t)warp * n2;

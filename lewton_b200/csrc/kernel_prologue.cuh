@@ -130,16 +130,17 @@ constexpr size_t kVqMaxElems = 12288;          // 48 KB of accumulators: stereo 
 // LWB_ENTRY_VQ: the packet's residue vectors, accumulated in shared memory from its VQ runs in the reference's
 // order (residue_packet_decode_inner, audio.rs:620-717; residue_packet_read_partition, :587-618): per coefficient
 // the f32 additions happen pass by pass; within a pass the vectors of a packet are disjoint, so the runs of a pass
-// go in parallel (one thread per run, its vectors in sequence).  acc: [C][n2], zeroed here.  Called by the whole CTA.
+// go in parallel (one thread per run, its vectors in sequence).  acc: [C][n2], zeroed here.  Called by the whole CTA,
+// thread tid of nthreads (k_prologue_fused, k_chain); ends on a CTA barrier.
 __device__ __forceinline__ void d_vq_accumulate(float *acc, int C, int n2, const DevSetup &su, const DevMapping &mp,
                                                 const lwb_vq_run *__restrict__ runs, uint32_t nruns,
-                                                const uint16_t *__restrict__ entries, uint32_t nent, int tid)
+                                                const uint16_t *__restrict__ entries, uint32_t nent, int tid, int nthreads)
 {
     const int total = C * n2;
-    for (int i = tid; i < total; i += kPfThreads) acc[i] = 0.f;
+    for (int i = tid; i < total; i += nthreads) acc[i] = 0.f;
     __syncthreads();
     for (uint32_t pass = 0; pass < 8; pass++) {
-        for (uint32_t i = tid; i < nruns; i += kPfThreads) {
+        for (uint32_t i = tid; i < nruns; i += nthreads) {
             const lwb_vq_run r = runs[i];
             if ((r.pass_kind & 7u) != pass || r.book >= su.n_books) continue;
             const DevBook bk = su.books[r.book];
@@ -351,7 +352,7 @@ k_prologue_fused(const DevPacket *__restrict__ pkts, uint32_t n_pk, const float 
         if (VQ) {
             const uint64_t o0 = vq.run_off[p.pkt_index], o1 = vq.run_off[p.pkt_index + 1];
             const uint64_t e0 = vq.ent_off[p.pkt_index], e1 = vq.ent_off[p.pkt_index + 1];
-            d_vq_accumulate(s_acc, C, n2, su, mp, vq.runs + o0, (uint32_t)(o1 - o0), vq.entries + e0, (uint32_t)(e1 - e0), tid);
+            d_vq_accumulate(s_acc, C, n2, su, mp, vq.runs + o0, (uint32_t)(o1 - o0), vq.entries + e0, (uint32_t)(e1 - e0), tid, kPfThreads);
         }
         __syncthreads();
         if (stereo) {

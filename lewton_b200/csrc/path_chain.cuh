@@ -6,11 +6,13 @@
 // Chain kernel path (kernel_chain.cuh): everything the fused long-block kernel does not take,
 // as long as channels <= 8 and the per-channel buffers fit in shared memory.
 // ---------------------------------------------------------------------------------------------
-// Shared memory of the chain kernel: per channel `np` blocks of U | V plus the previous right half, and the
-// floor posts of up to 8 channels.  np (blocks a channel group transforms together) is 4 where that fits.
-static size_t chain_smem(unsigned maxc, int n1max, int np)
+// Shared memory of the chain kernel: per channel `np` blocks of U | V plus the previous right half, the
+// floor posts of up to 8 channels and, VQ entry, the residue accumulators (maxc * n1max / 2 floats: <= 48 KB within
+// kVqMaxElems, 194 KB in all at most).  np (blocks a channel group transforms together) is 4 where that fits.
+static size_t chain_smem(unsigned maxc, int n1max, int np, bool vq = false)
 {
-    return (size_t)maxc * ((size_t)np * n1max + n1max / 2) * 4 + 8 * (LWB_MAX_POSTS + 1) * 2 * 2 + 64;
+    return (size_t)maxc * ((size_t)np * n1max + n1max / 2) * 4 + 8 * (LWB_MAX_POSTS + 1) * 2 * 2 + 64 +
+           (vq ? (size_t)maxc * (n1max / 2) * 4 : 0);
 }
 static int chain_np(unsigned maxc, int n1max, int wpc, bool residue)
 {
@@ -20,13 +22,13 @@ static int chain_np(unsigned maxc, int n1max, int wpc, bool residue)
     return np;
 }
 // k_chain for chains of up to maxc channels and blocks of up to n1max: one warp per channel and 1024 samples of the
-// largest block, at most 32 warps per CTA
-static ChainShape chain_shape(unsigned maxc, int n1max, bool residue)
+// largest block, at most 32 warps per CTA.  residue: the residue or the VQ entry (vq).
+static ChainShape chain_shape(unsigned maxc, int n1max, bool residue, bool vq = false)
 {
     int wpc = std::max(1, std::min(8, n1max / 1024));
     while (wpc > 1 && (unsigned)wpc * maxc > 32) wpc >>= 1;
     const int np = chain_np(maxc, n1max, wpc, residue);
-    return ChainShape{maxc * wpc, chain_smem(maxc, n1max, np), n1max, wpc, np};
+    return ChainShape{maxc * wpc, chain_smem(maxc, n1max, np, vq), n1max, wpc, np};
 }
 
 // One block per row: the stream state the first segment of a chain starts from, moved out of the way of the segment of
@@ -61,7 +63,7 @@ static void chain_desc(const lwb_chain *c, uint32_t p0, uint32_t n, bool has, ui
     d->channels = (uint8_t)su->channels;
 }
 
-// k_floor0_curves over the decoded packets of a residue-entry batch the chain kernel takes: *zero addresses the curves by
+// k_floor0_curves over the decoded packets of a residue- or VQ-entry batch the chain kernel takes: *zero addresses the curves by
 // absolute coefficient offset.  The packet list goes to ctx->desc, which only work queued on the compute stream uses.
 static int chain_floor0_curves(lwb_ctx *ctx, const BatchArenas &ar, const BatchExtent &ext, const lwb_chain *chains, size_t n_chains,
                                const std::vector<ChainWalk> &walks, float **zero)
@@ -87,8 +89,7 @@ static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
 {
     *handled = false;
     const uint64_t gen_at_entry = ctx->state_gen;
-    if (io->entry == LWB_ENTRY_VQ) return LWB_OK;            // (its residue stage runs inside the kernel, on dense vectors)
-    const bool residue = io->entry == LWB_ENTRY_RESIDUE;
+    const bool vq = io->entry == LWB_ENTRY_VQ, residue = io->entry != LWB_ENTRY_SPECTRUM;
     unsigned maxc = 1;
     int n1max = 64;
     size_t total_packets = 0;
@@ -99,7 +100,8 @@ static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         n1max = std::max(n1max, 1 << su->bs1);
         total_packets += chains[i].n_packets;
     }
-    if (chain_smem(maxc, n1max, 1) > 200 * 1024) return LWB_OK;
+    // (VQ: the accumulators of the largest block; the four-kernel path words the error of a batch beyond them)
+    if ((vq && (size_t)maxc * (n1max / 2) > kVqMaxElems) || chain_smem(maxc, n1max, 1, vq) > 200 * 1024) return LWB_OK;
     *handled = true;
 
     int rc;
@@ -128,7 +130,7 @@ static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         if ((rc = ar.open(ctx, io, ext, maxc, false)) || (rc = ar.upload(0, ext))) return rc;
         cudaStream_t sm = ctx->stream;
         // descriptors and mode bytes share one device buffer; a prepared batch (device memory, spectrum
-        // entry) owns it and replays the launch while no stream changes shape
+        // entry) owns it and replays the launch while no stream changes shape (residue and VQ entries are not captured)
         const bool cap = plan && !ar.host && !residue;
         DevBuf &dbuf = cap ? plan->mix : ctx->cdesc;
         const size_t used_desc = n_launch * sizeof(ChainDesc);
@@ -136,20 +138,21 @@ static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         if ((rc = upload_staging(ctx, st, hd, dbuf.p, used_desc, sm)) ||
             (rc = upload_staging(ctx, st, hb, (char *)dbuf.p + used_desc, boff + 16, sm)))
             return rc;
-        // residue entry with floor-0 records: their curves first, by absolute coefficient offset like ar.coeffs
+        // residue or VQ entry with floor-0 records: their curves first, by absolute coefficient offset like ar.coeffs
         float *zero = nullptr;
         if (residue && ext.need_floor0 && ar.fl.ys && (rc = chain_floor0_curves(ctx, ar, ext, chains, n_chains, walks, &zero))) return rc;
         StepArgs args;
         args.pcm = ar.pcm;
         args.out_format = io->out_format;
-        args.chain = chain_shape(maxc, n1max, residue);
+        args.chain = chain_shape(maxc, n1max, residue, vq);
         args.bytes = (const uint8_t *)dbuf.p + used_desc;
-        args.residue = residue;
+        args.entry = io->entry;
         args.coeffs = ar.coeffs;
         args.dense = ar.dense;
         args.kinds = ar.fl.kinds;
         args.ys = ar.fl.ys;
         args.zero = zero;
+        args.vq = VqDev{ar.fl.vq.runs, ar.fl.vq.run_off, ar.fl.vq.entries, ar.fl.vq.ent_off};
         std::vector<Step> steps(1, Step{LWB_KERNEL_CHAIN, dbuf.p, n_launch, nullptr});
         if ((rc = run_steps(ctx, args, steps))) return rc;
         if (cap) capture(plan, gen_at_entry, FrontStages(), args, std::move(steps));

@@ -579,18 +579,18 @@ static int front_stages_run(lwb_ctx *ctx, const lwb_batch_io *io, const FrontSta
 template <int ENTRY>
 static int launch_chain(lwb_ctx *ctx, int fmt, unsigned n_chains, unsigned warps, size_t smem, const ChainDesc *d,
                         const uint8_t *bytes, const float *coeffs, const float *dense, const uint8_t *kinds,
-                        const uint32_t *ys, void *pcm, int n1max, int wpc, int np, const float *zero)
+                        const uint32_t *ys, void *pcm, int n1max, int wpc, int np, const float *zero, VqDev vq)
 {
 #define LWB_CHAIN_CASE(F)                                                                                    \
     case F:                                                                                                  \
         if (wpc == 1) {                                                                                      \
             cudaFuncSetAttribute(k_chain<F, ENTRY, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
             return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, false>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, \
-                          kinds, ys, pcm, n1max, wpc, np, zero);                                              \
+                          kinds, ys, pcm, n1max, wpc, np, zero, vq);                                          \
         }                                                                                                    \
         cudaFuncSetAttribute(k_chain<F, ENTRY, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
         return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, true>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, kinds, \
-                      ys, pcm, n1max, wpc, 1, zero);
+                      ys, pcm, n1max, wpc, 1, zero, vq);
     switch (fmt) {
         LWB_CHAIN_CASE(LWB_OUT_F32_PLANAR)
         LWB_CHAIN_CASE(LWB_OUT_I16_PLANAR)
@@ -636,12 +636,15 @@ static int run_steps(lwb_ctx *ctx, const StepArgs &a, const std::vector<Step> &s
                           "short burst kernel launch");
             break;
         case LWB_KERNEL_CHAIN:
-            if (a.residue)
+            if (a.entry == LWB_ENTRY_VQ)
+                rc = launch_chain<LWB_ENTRY_VQ>(ctx, a.out_format, n, a.chain.warps, a.chain.smem, (const ChainDesc *)s.desc, a.bytes, a.coeffs,
+                                                a.dense, a.kinds, a.ys, a.pcm, a.chain.n1max, a.chain.wpc, a.chain.np, a.zero, a.vq);
+            else if (a.entry == LWB_ENTRY_RESIDUE)
                 rc = launch_chain<LWB_ENTRY_RESIDUE>(ctx, a.out_format, n, a.chain.warps, a.chain.smem, (const ChainDesc *)s.desc, a.bytes, a.coeffs,
-                                                     a.dense, a.kinds, a.ys, a.pcm, a.chain.n1max, a.chain.wpc, a.chain.np, a.zero);
+                                                     a.dense, a.kinds, a.ys, a.pcm, a.chain.n1max, a.chain.wpc, a.chain.np, a.zero, a.vq);
             else
                 rc = launch_chain<LWB_ENTRY_SPECTRUM>(ctx, a.out_format, n, a.chain.warps, a.chain.smem, (const ChainDesc *)s.desc, a.bytes, a.coeffs,
-                                                      a.dense, a.kinds, a.ys, a.pcm, a.chain.n1max, a.chain.wpc, a.chain.np, a.zero);
+                                                      a.dense, a.kinds, a.ys, a.pcm, a.chain.n1max, a.chain.wpc, a.chain.np, a.zero, a.vq);
             break;
         default:
             return fail(ctx, LWB_ERR_INVALID, "internal: no step for this kernel");
