@@ -1,5 +1,6 @@
 """Shared test helpers: random setups / packets, the oracle-driven reference decode, and which kernels ran."""
 import contextlib
+import os
 
 import numpy as np
 import pytest
@@ -12,6 +13,21 @@ ALL_KERNELS = frozenset(cabi.KERNELS)
 GENERIC = frozenset({"k_prologue", "k_imdct", "k_overlap", "k_save_state"})      # the four-kernel path
 FRONT = frozenset({"k_floor1_segments", "k_prologue_fused"})                     # two-kernel front stages
 FUSED = frozenset({"k_long", "k_long_s", "k_mid", "k_short", "k_short_g"})       # the fused synthesis kernels
+
+
+@contextlib.contextmanager
+def environ(env):
+    """Sets the environment variables of dict `env` (None: none) for the block, then restores them."""
+    old = {k: os.environ.get(k) for k in (env or {})}
+    os.environ.update(env or {})
+    try:
+        yield
+    finally:
+        for k, v in old.items():
+            if v is None:
+                os.environ.pop(k, None)
+            else:
+                os.environ[k] = v
 
 
 @contextlib.contextmanager

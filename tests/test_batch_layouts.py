@@ -4,15 +4,13 @@ else in the output arena, in host and device memory, for every layout the ABI al
 reversed, offsets that are not multiples of 4, empty chains and fresh streams.  The samples are bit-exact against the
 oracle (f32; i16 exact) whatever mix of setups a batch holds, each chain's output equals what it gives decoded alone,
 and misaligned device arenas give the same bytes as aligned ones."""
-import contextlib
-import os
 
 import numpy as np
 import pytest
 
 import lewton_b200 as L
 from lewton_b200 import _cabi as cabi
-from helpers import (ALL_KERNELS, FRONT, FUSED, GENERIC, RefStream, assert_contained, bits_equal, expect_kernels, fill_guard,
+from helpers import (ALL_KERNELS, FRONT, FUSED, GENERIC, RefStream, assert_contained, bits_equal, environ, expect_kernels, fill_guard,
                      launches_are_attributed, make_setup, mismatch_report, random_floor1_y, write_set)
 
 launches_are_attributed  # (autouse)
@@ -32,20 +30,6 @@ def ctx():
     c = L.Context(0)
     yield c
     c.close()
-
-
-@contextlib.contextmanager
-def environ(env):
-    old = {k: os.environ.get(k) for k in (env or {})}
-    os.environ.update(env or {})
-    try:
-        yield
-    finally:
-        for k, v in old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
 
 
 def flags(bf):

@@ -21,8 +21,6 @@ The library waits on the host in these places by design; the tests work around t
 - The four-kernel path synchronises before it writes its pinned descriptors.  It has no case here.
 - Host-memory batches return after their PCM has landed.
 - Inputs are in device arenas before the gate closes."""
-import contextlib
-import os
 import threading
 import types
 
@@ -32,7 +30,7 @@ import torch
 
 import lewton_b200 as L
 from lewton_b200 import _cabi as cabi
-from helpers import (ALL_KERNELS, FRONT, RefStream, assert_contained, bits_equal, expect_kernels, fill_guard,
+from helpers import (ALL_KERNELS, FRONT, RefStream, assert_contained, bits_equal, environ, expect_kernels, fill_guard,
                      launches_are_attributed, make_setup, mismatch_report, mode_sequence, random_floor1_y, write_set)
 
 pytestmark = pytest.mark.gpu
@@ -53,20 +51,6 @@ def ctx():
     c = L.Context(0)
     yield c
     c.close()
-
-
-@contextlib.contextmanager
-def environ(env):
-    old = {k: os.environ.get(k) for k in (env or {})}
-    os.environ.update(env or {})
-    try:
-        yield
-    finally:
-        for k, v in old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
 
 
 class Gate:

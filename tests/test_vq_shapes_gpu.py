@@ -18,13 +18,13 @@ import torch
 
 import lewton_b200 as L
 import vorbis_packer as vp
-from helpers import (ALL_KERNELS, FRONT, GENERIC, RefStream, assert_contained, bits_equal, expect_kernels, fill_guard,
+from helpers import (ALL_KERNELS, FRONT, GENERIC, RefStream, assert_contained, bits_equal, environ, expect_kernels, fill_guard,
                      launches_are_attributed, mismatch_report, write_set)
 from lewton_b200 import _cabi as cabi
 from lewton_b200 import frontend as fe
 from test_frontend_cpu import floor0_expected
 from test_frontend_gpu import consistent_modes
-from test_queued_batches import Gate, environ
+from test_queued_batches import Gate
 
 pytestmark = pytest.mark.gpu
 
