@@ -22,7 +22,8 @@
  *
  * All arithmetic is IEEE binary32, round-to-nearest, never contracted, in the
  * reference's operation order: f32 PCM is bit-identical to lewton's own output
- * (up to the sign of zero / NaN payload), i16 PCM is bit-identical.
+ * (up to the sign of zero / NaN payload), i16 PCM is bit-identical, f16 PCM is
+ * the round-to-nearest-even binary16 of that f32 PCM.
  */
 #ifndef LEWTON_B200_H
 #define LEWTON_B200_H
@@ -222,7 +223,15 @@ enum { LWB_FLOOR_UNUSED = 0,   /* DecodedFloor::Unused  -> zero curve (audio.rs:
 enum { LWB_OUT_F32_PLANAR = 0,        /* Vec<Vec<f32>>            samples.rs:20-40, 86-90          */
        LWB_OUT_I16_PLANAR = 1,        /* Vec<Vec<i16>>            samples.rs:92-103                */
        LWB_OUT_F32_INTERLEAVED = 2,   /* InterleavedSamples<f32>  samples.rs:43-79                 */
-       LWB_OUT_I16_INTERLEAVED = 3 }; /* InterleavedSamples<i16>                                   */
+       LWB_OUT_I16_INTERLEAVED = 3,   /* InterleavedSamples<i16>                                   */
+       LWB_OUT_F16_PLANAR = 4,        /* Vec<Vec<half::f16>>      a caller's `impl Sample for f16` */
+       LWB_OUT_F16_INTERLEAVED = 5 }; /* InterleavedSamples<half::f16>                             */
+/* F16 formats: each element is an IEEE binary16 (2 bytes, the layout of the F32 / I16 format of the same arrangement)
+ * equal to the binary32 sample x that the F32 format would write, rounded to nearest even: binary16 subnormals are
+ * kept (no flush to zero), |x| >= 65520 becomes +-inf, a NaN gives a NaN.  They take the same batch paths as the I16
+ * formats of the same layout.  Added under ABI 3 (no struct changes): a library without them refuses out_format 4 / 5
+ * with LWB_ERR_INVALID ("bad out_format") before it touches any chain result, stream state or arena -- as every
+ * library refuses any out_format above the last one it knows -- so a caller detects support by one refused call. */
 
 typedef struct lwb_packet {
     uint8_t mode_number;             /* audio.rs:925                                               */

@@ -15,6 +15,7 @@ OK, ERR_BAD_FORMAT, ERR_BUFFER, ERR_MISMATCH, ERR_INVALID, ERR_CUDA, ERR_NO_DEVI
 FLOOR_TYPE_ZERO, FLOOR_TYPE_ONE = 0, 1
 FLOOR_UNUSED, FLOOR_ONE, FLOOR_DENSE, FLOOR_ZERO = 0, 1, 2, 3
 OUT_F32_PLANAR, OUT_I16_PLANAR, OUT_F32_INTERLEAVED, OUT_I16_INTERLEAVED = 0, 1, 2, 3
+OUT_F16_PLANAR, OUT_F16_INTERLEAVED = 4, 5
 ENTRY_SPECTRUM, ENTRY_RESIDUE, ENTRY_VQ = 0, 1, 2
 MEM_HOST, MEM_DEVICE = 0, 1
 # LWB_KERNEL_* ids in order: KERNELS[id] is the kernel's name

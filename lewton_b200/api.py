@@ -371,8 +371,16 @@ class DecodedPacket:
         return kinds, ys, dense
 
 
+# (sample, interleaved) -> (LWB_OUT_*, numpy dtype).  "f16": IEEE binary16, the f32 sample rounded to nearest even.
 _FORMATS = {("f32", False): (cabi.OUT_F32_PLANAR, np.float32), ("i16", False): (cabi.OUT_I16_PLANAR, np.int16),
-            ("f32", True): (cabi.OUT_F32_INTERLEAVED, np.float32), ("i16", True): (cabi.OUT_I16_INTERLEAVED, np.int16)}
+            ("f32", True): (cabi.OUT_F32_INTERLEAVED, np.float32), ("i16", True): (cabi.OUT_I16_INTERLEAVED, np.int16),
+            ("f16", False): (cabi.OUT_F16_PLANAR, np.float16), ("f16", True): (cabi.OUT_F16_INTERLEAVED, np.float16)}
+
+
+def sample_format(sample, interleaved=False):
+    """(LWB_OUT_* format, numpy dtype) of sample type "f32" | "i16" | "f16" in the planar or interleaved layout (KeyError
+    for any other sample type)."""
+    return _FORMATS[(sample, bool(interleaved))]
 
 
 def get_decoded_sample_count(setup, mode_number, prev_window_flag=True, next_window_flag=True):
@@ -389,7 +397,7 @@ def read_audio_packet_generic(setup, packet, pwr, sample="f32", interleaved=Fals
     """audio.rs:919-1160 (back half).  Returns planar [channels][len] (Vec<Vec<S>>) or
     interleaved [len][channels] (InterleavedSamples<S>); len == 0 for the first packet after a reset.
     Raises AudioReadError (kind 'AudioBadFormat' for the guard at audio.rs:1107-1111)."""
-    fmt, dt = _FORMATS[(sample, interleaved)]
+    fmt, dt = sample_format(sample, interleaved)
     ch = setup.audio_channels
     cap = setup.blocksize(packet.mode_number)
     kinds, ys, dense = packet.pack()
@@ -417,7 +425,7 @@ def read_audio_packet(setup, packet, pwr):
 def decode_spectrum(setup, mode_number, spectrum, pwr, prev_window_flag=True, next_window_flag=True, sample="f32",
                     interleaved=False):
     """Entry at the record_pre_mdct tap (audio.rs:1041): spectrum [channels][n/2] = floor x residue."""
-    fmt, dt = _FORMATS[(sample, interleaved)]
+    fmt, dt = sample_format(sample, interleaved)
     ch = setup.audio_channels
     cap = setup.blocksize(mode_number)
     sp = np.ascontiguousarray(spectrum, np.float32)

@@ -368,8 +368,16 @@ static size_t host_chunks(size_t in_bytes, size_t n_chains)
     return std::min<size_t>(std::max<size_t>(1, in_bytes >> 25), std::min<size_t>(8, n_chains));
 }
 
-static size_t elem_size(int fmt) { return (fmt == LWB_OUT_F32_PLANAR || fmt == LWB_OUT_F32_INTERLEAVED) ? 4 : 2; }
-static bool is_planar(int fmt) { return fmt == LWB_OUT_F32_PLANAR || fmt == LWB_OUT_I16_PLANAR; }
+// f(std::integral_constant<int, fmt>()): how the kernels templated on an LWB_OUT_* value (k_chain, k_overlap) are picked
+// for a runtime format.  Instantiated for every format out_format_known accepts.
+template <int F = LWB_OUT_F32_PLANAR, typename Fn>
+static int with_out_format(int fmt, Fn &&f)
+{
+    if constexpr (out_format_known(F))
+        return fmt == F ? f(std::integral_constant<int, F>()) : with_out_format<F + 1>(fmt, f);
+    else
+        return LWB_ERR_INVALID;
+}
 
 // D2H of the PCM that chains [i0, i1) produced, from the staging buffer `stage`, which holds arena element `obase` at
 // its start.  Only the write set is copied (pcm_copy_plan.h): the gaps between planes and between chains are the
@@ -377,8 +385,8 @@ static bool is_planar(int fmt) { return fmt == LWB_OUT_F32_PLANAR || fmt == LWB_
 static int copy_pcm_to_host(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chain *chains, size_t i0, size_t i1,
                             const void *stage, uint64_t obase, cudaStream_t st)
 {
-    const size_t esz = elem_size(io->out_format);
-    const bool planar = is_planar(io->out_format);
+    const size_t esz = out_format_of(io->out_format).esz;
+    const bool planar = out_format_of(io->out_format).planar;
     ctx->pcm_spans.clear();
     for (size_t i = i0; i < i1; i++) {
         const lwb_chain *c = &chains[i];
@@ -394,13 +402,13 @@ static int copy_pcm_to_host(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chai
     return LWB_OK;
 }
 
-// The layout the fused kernels take: planar f32 / i16 out, and 16-byte aligned addresses, which their TMA bulk loads of
-// coefficients and vector stores of PCM need.  Element offsets that are multiples of 4 keep that when the arenas are
-// 16-byte aligned: the library's staging of host-memory batches always is, a caller's device arena may not be (the chain
-// kernel takes those).
+// The layout the fused kernels take: planar out (f32, i16 or f16), and 16-byte aligned addresses, which their TMA bulk
+// loads of coefficients and vector stores of PCM need.  Element offsets that are multiples of 4 keep that when the arenas
+// are 16-byte aligned: the library's staging of host-memory batches always is, a caller's device arena may not be (the
+// chain kernel takes those).
 static bool fused_layout(const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io)
 {
-    if (io->out_format != LWB_OUT_F32_PLANAR && io->out_format != LWB_OUT_I16_PLANAR) return false;
+    if (!out_format_of(io->out_format).planar) return false;
     if (io->memory == LWB_MEM_DEVICE && ((reinterpret_cast<uintptr_t>(io->coeffs) | reinterpret_cast<uintptr_t>(io->pcm) |
                                           reinterpret_cast<uintptr_t>(io->dense_floor)) & 15))
         return false;

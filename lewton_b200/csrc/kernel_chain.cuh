@@ -193,14 +193,7 @@ k_chain(const ChainDesc *__restrict__ chains, const uint8_t *__restrict__ pkt_by
                         float v = d_x_at(V, B, n, ls + i);
                         if (i < plen)                                  // audio.rs:1116-1118
                             v = __fadd_rn(__fmul_rn(v, __ldg(w + i)), __fmul_rn(prev[i], __ldg(w + plen - 1 - i)));
-                        if (FORMAT == LWB_OUT_F32_PLANAR)
-                            ((float *)pcm)[cd.out_off + (size_t)warp * cd.out_stride + pos + i] = v;
-                        else if (FORMAT == LWB_OUT_I16_PLANAR)
-                            ((int16_t *)pcm)[cd.out_off + (size_t)warp * cd.out_stride + pos + i] = d_sample_i16(v);
-                        else if (FORMAT == LWB_OUT_F32_INTERLEAVED)
-                            ((float *)pcm)[cd.out_off + (pos + i) * C + warp] = v;
-                        else
-                            ((int16_t *)pcm)[cd.out_off + (pos + i) * C + warp] = d_sample_i16(v);
+                        store_sample<FORMAT>(pcm, cd.out_off, cd.out_stride, C, warp, pos + i, v);
                     }
                     gsync();
                 }

@@ -32,8 +32,13 @@
 #pragma once
 #include <stdint.h>
 
+#include "lwb_common.h"
+
 #if defined(__CUDACC__)
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
+
+#include <type_traits>
 #define LWB_HD __host__ __device__ __forceinline__
 #else
 #define LWB_HD inline
@@ -48,7 +53,7 @@ constexpr int kLongN2 = 1024;
 // one run = consecutive packets of one channel of one stream
 struct alignas(16) LongRun {      // 48 bytes: fetched by the kernel with one 1-D TMA copy
     const float *in;        // first packet's spectrum (1024 floats); next packet at +in_stride
-    void *out;              // first emitted packet's PCM (f32 or i16 elements); next at +1024
+    void *out;              // first emitted packet's PCM (f32, i16 or f16 elements); next at +1024
     float *state;           // stream state row of this channel (1024 floats)
     uint32_t in_stride;
     uint32_t n_packets;     // including a primer packet if prime != 0
@@ -584,8 +589,36 @@ __device__ __forceinline__ int16_t d_sample_i16(float v)
     asm("cvt.rzi.s16.f32 %0, %1;" : "=h"(r) : "f"(__fmul_rn(v, 32768.0f)));
     return (int16_t)r;
 }
+// `Sample for f16` (LWB_OUT_F16_*): the f32 sample rounded to nearest even, binary16 subnormals kept (no .ftz),
+// overflow to +-inf, NaN -> NaN
+__device__ __forceinline__ __half d_sample_f16(float v)
+{
+    unsigned short r;
+    asm("cvt.rn.f16.f32 %0, %1;" : "=h"(r) : "f"(v));
+    return __ushort_as_half(r);
+}
+// one sample as the element type of its format
+__device__ __forceinline__ float d_sample(float v, float *) { return v; }
+__device__ __forceinline__ int16_t d_sample(float v, int16_t *) { return d_sample_i16(v); }
+__device__ __forceinline__ __half d_sample(float v, __half *) { return d_sample_f16(v); }
 __device__ __forceinline__ void st_pcm(float *p, float v) { __stcs(p, v); }    // streaming: the PCM is not read again
 __device__ __forceinline__ void st_pcm(int16_t *p, float v) { __stcs(reinterpret_cast<short *>(p), (short)d_sample_i16(v)); }
+__device__ __forceinline__ void st_pcm(__half *p, float v) { __stcs(reinterpret_cast<short *>(p), __half_as_short(d_sample_f16(v))); }
+
+// the element type of a sample kind
+template <SampleKind K>
+using sample_t = std::conditional_t<K == kSampleF32, float, std::conditional_t<K == kSampleI16, int16_t, __half>>;
+
+// Stores sample i of channel ch of a chain or packet whose PCM starts at element `off`, in format FORMAT (k_chain and
+// the four-kernel path's k_overlap)
+template <int FORMAT>
+__device__ __forceinline__ void store_sample(void *pcm, uint64_t off, uint64_t stride, unsigned channels, unsigned ch,
+                                             uint64_t i, float v)
+{
+    constexpr OutFormat F = out_format_of(FORMAT);
+    using T = sample_t<F.kind>;
+    static_cast<T *>(pcm)[off + (F.planar ? (uint64_t)ch * stride + i : i * channels + ch)] = d_sample(v, static_cast<T *>(nullptr));
+}
 
 // Step 8 + window + overlap-add + stores, all 8 slots of all NB blocks.  FIRST: packet 0 of the
 // run -- its previous right half comes from the stream state (staged in shared memory by TMA
@@ -1253,13 +1286,16 @@ k_long_s(const LongRun *__restrict__ runs, uint32_t n_runs, const float *__restr
 }
 
 inline int long_launch_static(cudaStream_t stream, const LongRun *d_runs, uint32_t n_runs, const float *d_pack, int sm_count,
-                              bool i16_out, const float *d_w_short, int ls)
+                              SampleKind kind, const float *d_w_short, int ls)
 {
     if (!n_runs) return 0;
     const uint32_t grid = static_deal_grid(n_runs, kLongWarps, sm_count);
     if (ls != kLongLs256) return 1;               // the one short size k_long_s is built for
-    if (i16_out) k_long_s<int16_t><<<grid, kLongWarps * 32, kLongSmemBytesS, stream>>>(d_runs, n_runs, d_pack, d_w_short);
-    else k_long_s<float><<<grid, kLongWarps * 32, kLongSmemBytesS, stream>>>(d_runs, n_runs, d_pack, d_w_short);
+    switch (kind) {
+    case kSampleI16: k_long_s<int16_t><<<grid, kLongWarps * 32, kLongSmemBytesS, stream>>>(d_runs, n_runs, d_pack, d_w_short); break;
+    case kSampleF16: k_long_s<__half><<<grid, kLongWarps * 32, kLongSmemBytesS, stream>>>(d_runs, n_runs, d_pack, d_w_short); break;
+    default: k_long_s<float><<<grid, kLongWarps * 32, kLongSmemBytesS, stream>>>(d_runs, n_runs, d_pack, d_w_short); break;
+    }
     return cudaGetLastError() != cudaSuccess;
 }
 
@@ -1267,19 +1303,24 @@ inline void long_kernel_configure()
 {
     cudaFuncSetAttribute(k_long<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLongSmemBytes);
     cudaFuncSetAttribute(k_long<int16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLongSmemBytes);
+    cudaFuncSetAttribute(k_long<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLongSmemBytes);
     cudaFuncSetAttribute(k_long_s<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLongSmemBytesS);
     cudaFuncSetAttribute(k_long_s<int16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLongSmemBytesS);
+    cudaFuncSetAttribute(k_long_s<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLongSmemBytesS);
 }
 
 // d_runs: n_groups * kLongNB descriptors.  Returns 0 on success; `ticket` must point at a zeroed
 // device word no other launch in flight uses.
 inline int long_launch(cudaStream_t stream, const LongRun *d_runs, uint32_t n_groups, const float *d_pack,
-                       unsigned int *ticket, int sm_count, bool i16_out, const float *d_w_short = nullptr, int ls = 0)
+                       unsigned int *ticket, int sm_count, SampleKind kind, const float *d_w_short = nullptr, int ls = 0)
 {
     const uint32_t want = (n_groups + kLongWarps - 1) / kLongWarps;
     const uint32_t grid = want < (uint32_t)sm_count ? want : (uint32_t)sm_count;
-    if (i16_out) k_long<int16_t><<<grid, kLongWarps * 32, kLongSmemBytes, stream>>>(d_runs, n_groups, d_pack, ticket, d_w_short, ls);
-    else k_long<float><<<grid, kLongWarps * 32, kLongSmemBytes, stream>>>(d_runs, n_groups, d_pack, ticket, d_w_short, ls);
+    switch (kind) {
+    case kSampleI16: k_long<int16_t><<<grid, kLongWarps * 32, kLongSmemBytes, stream>>>(d_runs, n_groups, d_pack, ticket, d_w_short, ls); break;
+    case kSampleF16: k_long<__half><<<grid, kLongWarps * 32, kLongSmemBytes, stream>>>(d_runs, n_groups, d_pack, ticket, d_w_short, ls); break;
+    default: k_long<float><<<grid, kLongWarps * 32, kLongSmemBytes, stream>>>(d_runs, n_groups, d_pack, ticket, d_w_short, ls); break;
+    }
     return cudaGetLastError() != cudaSuccess;
 }
 #endif  // __CUDACC__

@@ -366,22 +366,30 @@ inline void mid_kernel_configure()
 {
     cudaFuncSetAttribute(k_mid<float, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MidDev<1>::Smem);
     cudaFuncSetAttribute(k_mid<int16_t, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MidDev<1>::Smem);
+    cudaFuncSetAttribute(k_mid<__half, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MidDev<1>::Smem);
     cudaFuncSetAttribute(k_mid<float, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MidDev<2>::Smem);
     cudaFuncSetAttribute(k_mid<int16_t, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MidDev<2>::Smem);
+    cudaFuncSetAttribute(k_mid<__half, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MidDev<2>::Smem);
     static_assert(MidDev<1>::Smem <= 232448 && MidDev<2>::Smem <= 232448, "k_mid's shared memory must fit one SM");
 }
 
 // kb: 1 -> n = 1024 (groups of two runs), 2 -> n = 512 (groups of four)
-inline int mid_launch(cudaStream_t stream, const LongRun *d_runs, uint32_t n_groups, const float *d_pack, int sm_count, bool i16_out, int kb)
+inline int mid_launch(cudaStream_t stream, const LongRun *d_runs, uint32_t n_groups, const float *d_pack, int sm_count, SampleKind kind, int kb)
 {
     if (!n_groups) return 0;
     const uint32_t grid = static_deal_grid(n_groups, kLongWarps, sm_count);
     if (kb == 1) {
-        if (i16_out) k_mid<int16_t, 1><<<grid, kLongWarps * 32, MidDev<1>::Smem, stream>>>(d_runs, n_groups, d_pack);
-        else k_mid<float, 1><<<grid, kLongWarps * 32, MidDev<1>::Smem, stream>>>(d_runs, n_groups, d_pack);
+        switch (kind) {
+        case kSampleI16: k_mid<int16_t, 1><<<grid, kLongWarps * 32, MidDev<1>::Smem, stream>>>(d_runs, n_groups, d_pack); break;
+        case kSampleF16: k_mid<__half, 1><<<grid, kLongWarps * 32, MidDev<1>::Smem, stream>>>(d_runs, n_groups, d_pack); break;
+        default: k_mid<float, 1><<<grid, kLongWarps * 32, MidDev<1>::Smem, stream>>>(d_runs, n_groups, d_pack); break;
+        }
     } else {
-        if (i16_out) k_mid<int16_t, 2><<<grid, kLongWarps * 32, MidDev<2>::Smem, stream>>>(d_runs, n_groups, d_pack);
-        else k_mid<float, 2><<<grid, kLongWarps * 32, MidDev<2>::Smem, stream>>>(d_runs, n_groups, d_pack);
+        switch (kind) {
+        case kSampleI16: k_mid<int16_t, 2><<<grid, kLongWarps * 32, MidDev<2>::Smem, stream>>>(d_runs, n_groups, d_pack); break;
+        case kSampleF16: k_mid<__half, 2><<<grid, kLongWarps * 32, MidDev<2>::Smem, stream>>>(d_runs, n_groups, d_pack); break;
+        default: k_mid<float, 2><<<grid, kLongWarps * 32, MidDev<2>::Smem, stream>>>(d_runs, n_groups, d_pack); break;
+        }
     }
     return cudaGetLastError() != cudaSuccess;
 }

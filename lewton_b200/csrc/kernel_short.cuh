@@ -31,7 +31,7 @@ constexpr int kShortOct = 8;               // blocks a warp transforms together
 
 struct alignas(16) ShortRun {              // 48 bytes
     const float *in;        // first packet's spectrum (128 floats); next packet at +in_stride
-    void *out;              // first emitted packet's PCM (f32 or i16 elements); next at +128
+    void *out;              // first emitted packet's PCM (f32, i16 or f16 elements); next at +128
     float *state;           // stream state row of this channel (>= 128 floats)
     uint32_t in_stride;
     uint32_t n_packets;     // including a primer packet (has_prev == 0: packet 0 emits nothing)
@@ -233,22 +233,28 @@ struct TwShort {
 
 // PCM staging: one sample as OutT (samples.rs:86-103)
 __device__ __forceinline__ void sts_pcm(uint32_t addr, float v, float *) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory"); }
-__device__ __forceinline__ void sts_pcm(uint32_t addr, float v, int16_t *)
+// 2-byte samples (i16, f16) differ only in the conversion: one staging store for both
+template <typename OutT>
+__device__ __forceinline__ void sts_pcm(uint32_t addr, float v, OutT *)
 {
-    asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"((short)d_sample_i16(v)) : "memory");
+    static_assert(sizeof(OutT) == 2, "2-byte samples");
+    const OutT s = d_sample(v, static_cast<OutT *>(nullptr));
+    asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"(*reinterpret_cast<const unsigned short *>(&s)) : "memory");
 }
-// four staged samples of one lane -> global, streaming
-__device__ __forceinline__ void copy_out4(float *dst, uint32_t src)
+// four staged samples of one lane -> global, streaming: one 16-byte (f32) or 8-byte (2-byte samples) store
+template <typename OutT>
+__device__ __forceinline__ void copy_out4(OutT *dst, uint32_t src)
 {
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(src) : "memory");
-    __stcs(reinterpret_cast<float4 *>(dst), v);
-}
-__device__ __forceinline__ void copy_out4(int16_t *dst, uint32_t src)
-{
-    uint2 v;
-    asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(src) : "memory");
-    __stcs(reinterpret_cast<uint2 *>(dst), v);
+    if constexpr (sizeof(OutT) == 4) {
+        float4 v;
+        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(src) : "memory");
+        __stcs(reinterpret_cast<float4 *>(dst), v);
+    } else {
+        static_assert(sizeof(OutT) == 2, "2-byte samples");
+        uint2 v;
+        asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(src) : "memory");
+        __stcs(reinterpret_cast<uint2 *>(dst), v);
+    }
 }
 
 // Transpose addresses (bytes inside the stage; E plane at +0, O plane at +2048).  4 * swzS(b, c) splits into a lane part,
@@ -630,12 +636,15 @@ k_short_g(const ShortRun *__restrict__ runs, uint32_t n_groups, const float *__r
     }
 }
 
-inline int short_launch_groups(cudaStream_t stream, const ShortRun *d_runs, uint32_t n_groups, const float *d_pack, int sm_count, bool i16_out)
+inline int short_launch_groups(cudaStream_t stream, const ShortRun *d_runs, uint32_t n_groups, const float *d_pack, int sm_count, SampleKind kind)
 {
     if (!n_groups) return 0;
     const uint32_t grid = static_deal_grid(n_groups, kShortWarps, sm_count);
-    if (i16_out) k_short_g<int16_t><<<grid, kShortWarps * 32, kShortGSmemBytes, stream>>>(d_runs, n_groups, d_pack);
-    else k_short_g<float><<<grid, kShortWarps * 32, kShortGSmemBytes, stream>>>(d_runs, n_groups, d_pack);
+    switch (kind) {
+    case kSampleI16: k_short_g<int16_t><<<grid, kShortWarps * 32, kShortGSmemBytes, stream>>>(d_runs, n_groups, d_pack); break;
+    case kSampleF16: k_short_g<__half><<<grid, kShortWarps * 32, kShortGSmemBytes, stream>>>(d_runs, n_groups, d_pack); break;
+    default: k_short_g<float><<<grid, kShortWarps * 32, kShortGSmemBytes, stream>>>(d_runs, n_groups, d_pack); break;
+    }
     return cudaGetLastError() != cudaSuccess;
 }
 
@@ -643,16 +652,21 @@ inline void short_kernel_configure()
 {
     cudaFuncSetAttribute(k_short<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kShortSmemBytes);
     cudaFuncSetAttribute(k_short<int16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kShortSmemBytes);
+    cudaFuncSetAttribute(k_short<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kShortSmemBytes);
     cudaFuncSetAttribute(k_short_g<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kShortGSmemBytes);
     cudaFuncSetAttribute(k_short_g<int16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kShortGSmemBytes);
+    cudaFuncSetAttribute(k_short_g<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kShortGSmemBytes);
 }
 
-inline int short_launch(cudaStream_t stream, const ShortRun *d_runs, uint32_t n_runs, const float *d_pack, int sm_count, bool i16_out)
+inline int short_launch(cudaStream_t stream, const ShortRun *d_runs, uint32_t n_runs, const float *d_pack, int sm_count, SampleKind kind)
 {
     if (!n_runs) return 0;
     const uint32_t grid = static_deal_grid(n_runs, kShortWarps, sm_count);
-    if (i16_out) k_short<int16_t><<<grid, kShortWarps * 32, kShortSmemBytes, stream>>>(d_runs, n_runs, d_pack);
-    else k_short<float><<<grid, kShortWarps * 32, kShortSmemBytes, stream>>>(d_runs, n_runs, d_pack);
+    switch (kind) {
+    case kSampleI16: k_short<int16_t><<<grid, kShortWarps * 32, kShortSmemBytes, stream>>>(d_runs, n_runs, d_pack); break;
+    case kSampleF16: k_short<__half><<<grid, kShortWarps * 32, kShortSmemBytes, stream>>>(d_runs, n_runs, d_pack); break;
+    default: k_short<float><<<grid, kShortWarps * 32, kShortSmemBytes, stream>>>(d_runs, n_runs, d_pack); break;
+    }
     return cudaGetLastError() != cudaSuccess;
 }
 #endif  // __CUDACC__

@@ -521,7 +521,7 @@ k_imdct(const DevPacket *__restrict__ pkts, const float *__restrict__ spec, floa
 // ---------------------------------------------------------------------------------------------
 // window / overlap-add / slice / sample conversion, audio.rs:1079-1157 + samples.rs
 // ---------------------------------------------------------------------------------------------
-// d_sample_i16 (samples.rs:92-103) lives in kernel_long.cuh, shared by both paths
+// the sample conversions (samples.rs:86-103, and f16) and store_sample live in kernel_long.cuh, shared by every path
 
 constexpr int kOverlapThreads = 256;
 
@@ -547,14 +547,7 @@ k_overlap(const DevPacket *__restrict__ pkts, const float *__restrict__ x, void 
         float v = xc[ls + i];
         if (i < plen)                                  // audio.rs:1116-1118
             v = __fadd_rn(__fmul_rn(v, w[i]), __fmul_rn(prev[i], w[plen - 1 - i]));
-        if (FORMAT == LWB_OUT_F32_PLANAR)
-            ((float *)pcm)[p.out_off + (size_t)ch * p.out_stride + i] = v;
-        else if (FORMAT == LWB_OUT_I16_PLANAR)
-            ((int16_t *)pcm)[p.out_off + (size_t)ch * p.out_stride + i] = d_sample_i16(v);
-        else if (FORMAT == LWB_OUT_F32_INTERLEAVED)
-            ((float *)pcm)[p.out_off + (size_t)i * p.channels + ch] = v;
-        else
-            ((int16_t *)pcm)[p.out_off + (size_t)i * p.channels + ch] = d_sample_i16(v);
+        store_sample<FORMAT>(pcm, p.out_off, p.out_stride, p.channels, ch, i, v);
     }
 }
 

@@ -640,7 +640,7 @@ static int queue_batch(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const l
     if (!ctx || (!chains && n_chains) || !io) return LWB_ERR_INVALID;
     if (io->entry != LWB_ENTRY_SPECTRUM && io->entry != LWB_ENTRY_RESIDUE && io->entry != LWB_ENTRY_VQ) return fail(ctx, LWB_ERR_INVALID, "bad entry");
     if (io->memory != LWB_MEM_HOST && io->memory != LWB_MEM_DEVICE) return fail(ctx, LWB_ERR_INVALID, "bad memory space");
-    if (io->out_format < 0 || io->out_format > LWB_OUT_I16_INTERLEAVED) return fail(ctx, LWB_ERR_INVALID, "bad out_format");
+    if (!out_format_known(io->out_format)) return fail(ctx, LWB_ERR_INVALID, "bad out_format");
     if (n_chains == 0) return LWB_OK;
     if ((!io->coeffs && io->entry != LWB_ENTRY_VQ) || !io->pcm) return fail(ctx, LWB_ERR_INVALID, "null arena");
     if (io->entry == LWB_ENTRY_VQ && (!io->vq_runs || !io->vq_run_offsets || !io->vq_entries || !io->vq_entry_offsets || !io->floor_kind))

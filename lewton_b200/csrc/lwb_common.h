@@ -12,7 +12,32 @@
 
 #include "../../include/lewton_b200.h"
 
+#if defined(__CUDACC__)
+#define LWB_CHD __host__ __device__ constexpr
+#else
+#define LWB_CHD constexpr
+#endif
+
 namespace lwb {
+
+// The PCM formats (LWB_OUT_*): all that the batch paths, the launchers and the kernels know about one.  A sample kind
+// is one conversion from the f32 sample (samples.rs:86-103); kernel_long.cuh maps it to its element type.
+enum SampleKind { kSampleF32 = 0, kSampleI16 = 1, kSampleF16 = 2 };
+struct OutFormat {
+    unsigned esz;             // bytes per element
+    bool planar;              // [channel][out_stride] planes, else [t][channel]
+    SampleKind kind;
+};
+LWB_CHD bool out_format_known(int f) { return f >= LWB_OUT_F32_PLANAR && f <= LWB_OUT_F16_INTERLEAVED; }
+LWB_CHD OutFormat out_format_of(int f)
+{
+    return f == LWB_OUT_I16_PLANAR        ? OutFormat{2, true, kSampleI16}
+           : f == LWB_OUT_F32_INTERLEAVED ? OutFormat{4, false, kSampleF32}
+           : f == LWB_OUT_I16_INTERLEAVED ? OutFormat{2, false, kSampleI16}
+           : f == LWB_OUT_F16_PLANAR      ? OutFormat{2, true, kSampleF16}
+           : f == LWB_OUT_F16_INTERLEAVED ? OutFormat{2, false, kSampleF16}
+                                          : OutFormat{4, true, kSampleF32};
+}
 
 struct DevTables {            // CachedBlocksizeDerived, header_cached.rs:27-31 (device pointers)
     const float *a, *b, *c, *window;

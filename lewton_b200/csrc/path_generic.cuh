@@ -316,7 +316,7 @@ struct BatchExtent {
     {
         if (!done) return LWB_OK;
         const unsigned C = c->stream->setup->channels;
-        const bool planar = is_planar(io->out_format);
+        const bool planar = out_format_of(io->out_format).planar;
         if (planar && c->out_stride < n_samples) return fail(ctx, LWB_ERR_BUFFER, "chain: out_stride smaller than the samples produced");
         c_lo = std::min(c_lo, c->coeff_offset);
         c_hi = std::max(c_hi, coeff_end);
@@ -357,7 +357,7 @@ static int check_page_locked(lwb_ctx *ctx, const lwb_batch_io *io, const BatchEx
     const char *bad = nullptr;
     if (io->entry != LWB_ENTRY_VQ && !page_locked(io->coeffs, ext.c_lo, ext.c_hi, sizeof(float))) bad = "coeffs";
     else if (ext.need_dense && !page_locked(io->dense_floor, ext.c_lo, ext.c_hi, sizeof(float))) bad = "dense_floor";
-    else if (!page_locked(io->pcm, ext.o_lo, ext.o_hi, elem_size(io->out_format))) bad = "pcm";
+    else if (!page_locked(io->pcm, ext.o_lo, ext.o_hi, out_format_of(io->out_format).esz)) bad = "pcm";
     else if (io->entry != LWB_ENTRY_SPECTRUM && io->floor_memory == LWB_MEM_HOST && ext.r_hi > ext.r_lo) {
         const uint64_t a = ext.r_lo * C, b = ext.r_hi * C;
         if (!page_locked(io->floor_kind, a, b, 1)) bad = "floor_kind";
@@ -410,7 +410,7 @@ struct BatchArenas {
             set = &ctx->host_sets[ctx->host_next];
             ctx->host_next = (ctx->host_next + 1) % kHostSets;
             in_use = set->done;
-            const size_t esz = elem_size(io->out_format), bytes = (size_t)(ext.c_hi - ext.c_lo) * sizeof(float);
+            const size_t esz = out_format_of(io->out_format).esz, bytes = (size_t)(ext.c_hi - ext.c_lo) * sizeof(float);
             if (ext.o_hi > ext.o_lo && (rc = ensure(ctx, set->pcm, (size_t)(ext.o_hi - ext.o_lo) * esz, in_use))) return rc;
             if (!vq && (rc = ensure(ctx, set->coeffs, bytes, in_use))) return rc;
             if (ext.need_dense && (rc = ensure(ctx, set->dense, bytes, in_use))) return rc;
@@ -581,24 +581,17 @@ static int launch_chain(lwb_ctx *ctx, int fmt, unsigned n_chains, unsigned warps
                         const uint8_t *bytes, const float *coeffs, const float *dense, const uint8_t *kinds,
                         const uint32_t *ys, void *pcm, int n1max, int wpc, int np, const float *zero, VqDev vq)
 {
-#define LWB_CHAIN_CASE(F)                                                                                    \
-    case F:                                                                                                  \
-        if (wpc == 1) {                                                                                      \
-            cudaFuncSetAttribute(k_chain<F, ENTRY, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, false>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, \
-                          kinds, ys, pcm, n1max, wpc, np, zero, vq);                                          \
-        }                                                                                                    \
-        cudaFuncSetAttribute(k_chain<F, ENTRY, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-        return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, true>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, kinds, \
+    return with_out_format(fmt, [&](auto f) {
+        constexpr int F = decltype(f)::value;
+        if (wpc == 1) {
+            cudaFuncSetAttribute(k_chain<F, ENTRY, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, false>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense,
+                          kinds, ys, pcm, n1max, wpc, np, zero, vq);
+        }
+        cudaFuncSetAttribute(k_chain<F, ENTRY, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, true>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, kinds,
                       ys, pcm, n1max, wpc, 1, zero, vq);
-    switch (fmt) {
-        LWB_CHAIN_CASE(LWB_OUT_F32_PLANAR)
-        LWB_CHAIN_CASE(LWB_OUT_I16_PLANAR)
-        LWB_CHAIN_CASE(LWB_OUT_F32_INTERLEAVED)
-        LWB_CHAIN_CASE(LWB_OUT_I16_INTERLEAVED)
-    }
-#undef LWB_CHAIN_CASE
-    return LWB_ERR_INVALID;
+    });
 }
 
 __global__ void k_row_copy(const RowCopy *__restrict__ rc);   // path_chain.cuh
@@ -607,7 +600,7 @@ __global__ void k_row_copy(const RowCopy *__restrict__ rc);   // path_chain.cuh
 static int run_steps(lwb_ctx *ctx, const StepArgs &a, const std::vector<Step> &steps)
 {
     cudaStream_t sm = ctx->stream;
-    const bool i16 = a.out_format == LWB_OUT_I16_PLANAR;
+    const SampleKind kind = out_format_of(a.out_format).kind;
     for (const Step &s : steps) {
         int rc;
         unsigned int *ticket;
@@ -618,21 +611,21 @@ static int run_steps(lwb_ctx *ctx, const StepArgs &a, const std::vector<Step> &s
             break;
         case LWB_KERNEL_LONG:
             if ((rc = next_ticket(ctx, &ticket))) return rc;
-            rc = launched(ctx, LWB_KERNEL_LONG, long_launch(sm, (const LongRun *)s.desc, n, s.pack, ticket, ctx->sm_count, i16, a.w_short, a.ls),
+            rc = launched(ctx, LWB_KERNEL_LONG, long_launch(sm, (const LongRun *)s.desc, n, s.pack, ticket, ctx->sm_count, kind, a.w_short, a.ls),
                           "long kernel launch");
             break;
         case LWB_KERNEL_LONG_S:         // one pass over many short runs: the static deal with its deeper lookahead
-            rc = launched(ctx, LWB_KERNEL_LONG_S, long_launch_static(sm, (const LongRun *)s.desc, n, s.pack, ctx->sm_count, i16, a.w_short, a.ls),
+            rc = launched(ctx, LWB_KERNEL_LONG_S, long_launch_static(sm, (const LongRun *)s.desc, n, s.pack, ctx->sm_count, kind, a.w_short, a.ls),
                           "long kernel launch");
             break;
         case LWB_KERNEL_MID:
-            rc = launched(ctx, LWB_KERNEL_MID, mid_launch(sm, (const LongRun *)s.desc, n, s.pack, ctx->sm_count, i16, a.mid_kb), "mid kernel launch");
+            rc = launched(ctx, LWB_KERNEL_MID, mid_launch(sm, (const LongRun *)s.desc, n, s.pack, ctx->sm_count, kind, a.mid_kb), "mid kernel launch");
             break;
         case LWB_KERNEL_SHORT:
-            rc = launched(ctx, LWB_KERNEL_SHORT, short_launch(sm, (const ShortRun *)s.desc, n, s.pack, ctx->sm_count, i16), "short kernel launch");
+            rc = launched(ctx, LWB_KERNEL_SHORT, short_launch(sm, (const ShortRun *)s.desc, n, s.pack, ctx->sm_count, kind), "short kernel launch");
             break;
         case LWB_KERNEL_SHORT_G:        // bursts: eight short runs of equal length per warp
-            rc = launched(ctx, LWB_KERNEL_SHORT_G, short_launch_groups(sm, (const ShortRun *)s.desc, n, s.pack, ctx->sm_count, i16),
+            rc = launched(ctx, LWB_KERNEL_SHORT_G, short_launch_groups(sm, (const ShortRun *)s.desc, n, s.pack, ctx->sm_count, kind),
                           "short burst kernel launch");
             break;
         case LWB_KERNEL_CHAIN:
@@ -664,10 +657,10 @@ static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_bat
     if (maxp == 0) return LWB_OK;
     const uint64_t coeff_base = ar.host ? ar.c_lo : 0, pcm_base = ar.host ? ar.o_lo : 0;
     const float *coeffs = ar.coeffs ? ar.coeffs + coeff_base : nullptr, *dense = ar.dense ? ar.dense + coeff_base : nullptr;
-    void *pcm = ar.pcm + pcm_base * elem_size(io->out_format);
+    void *pcm = ar.pcm + pcm_base * out_format_of(io->out_format).esz;
     // x elements of one "packet column" (packet i of every chain), to size the rounds
     std::vector<uint32_t> start(plan.size(), 0);
-    const bool planar = is_planar(io->out_format);
+    const bool planar = out_format_of(io->out_format).planar;
     while (true) {
         // pick how many packets per chain go into this round
         size_t x_elems = 0, n_desc = 0, spec_lo = ~(size_t)0, spec_hi = 0;
@@ -754,12 +747,9 @@ static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_bat
                          spec, (float *)ctx->x.p)))
             return rc;
         dim3 g2((unsigned)n_desc, maxc), b2(kOverlapThreads);
-        switch (io->out_format) {
-        case LWB_OUT_F32_PLANAR: rc = launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<LWB_OUT_F32_PLANAR>, g2, b2, 0, dp, (const float *)ctx->x.p, pcm); break;
-        case LWB_OUT_I16_PLANAR: rc = launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<LWB_OUT_I16_PLANAR>, g2, b2, 0, dp, (const float *)ctx->x.p, pcm); break;
-        case LWB_OUT_F32_INTERLEAVED: rc = launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<LWB_OUT_F32_INTERLEAVED>, g2, b2, 0, dp, (const float *)ctx->x.p, pcm); break;
-        default: rc = launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<LWB_OUT_I16_INTERLEAVED>, g2, b2, 0, dp, (const float *)ctx->x.p, pcm); break;
-        }
+        rc = with_out_format(io->out_format, [&](auto f) {
+            return launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<decltype(f)::value>, g2, b2, 0, dp, (const float *)ctx->x.p, pcm);
+        });
         if (rc) return rc;
         if ((rc = launch(ctx, LWB_KERNEL_SAVE_STATE, k_save_state, g2, b2, 0, dp, (const float *)ctx->x.p))) return rc;
     }

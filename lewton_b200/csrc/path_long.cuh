@@ -3,7 +3,7 @@
 #pragma once
 
 // ---------------------------------------------------------------------------------------------
-// Fused path (kernel_long.cuh).  Eligible batches: any entry, planar f32 / i16 out, every packet a
+// Fused path (kernel_long.cuh).  Eligible batches: any entry, planar f32 / i16 / f16 out, every packet a
 // long block of blocksize 2^11 with long neighbours, every stream either empty or holding a
 // 1024-sample right half.  Planned directly from the chain list in O(chains + mode bytes) -- at
 // 0.8 G blocks/s per GPU a per-packet host plan would be the bottleneck.
@@ -297,7 +297,7 @@ static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_
         for (size_t i = i0; i < i1; i++) npk += chains[i].n_packets;
         if ((rc = ar.upload(k, ke)) || (residue && (rc = front_stages_launch(ctx, ar, fs, pk0, npk)))) return rc;
         if (!lr.d) {
-            if ((rc = long_build_runs(ctx, chains, n_chains, n_chunks, in, ar.pcm, elem_size(io->out_format), cap ? &plan->mix : nullptr, &lr)) ||
+            if ((rc = long_build_runs(ctx, chains, n_chains, n_chunks, in, ar.pcm, out_format_of(io->out_format).esz, cap ? &plan->mix : nullptr, &lr)) ||
                 (rc = long_upload_runs(ctx, lr, host ? ctx->copy_in : ctx->copy_out)))
                 return rc;
             gen = ctx->state_gen;                                           // every arena the capture points into is sized

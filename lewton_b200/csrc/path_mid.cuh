@@ -1,6 +1,6 @@
 // path_mid.cuh -- part of the C-ABI translation unit (included by lwb_api.cu, not compiled on its own):
 // batches whose every packet is a full-window block of n = 1024 or of n = 512 (blocksize 10 / 9) go to k_mid
-// (kernel_mid.cuh): planar f32 / i16, <= 8 channels; the residue and VQ entries run the front stages (k_floor1_segments +
+// (kernel_mid.cuh): planar f32 / i16 / f16, <= 8 channels; the residue and VQ entries run the front stages (k_floor1_segments +
 // k_prologue_fused, kernel_prologue.cuh) over all packets first and hand k_mid the spectrum arena.  The descriptors, the staging of host arenas and the capture by a prepared
 // batch (any entry) follow try_chain; the launch is one LWB_KERNEL_MID step.
 #pragma once
@@ -14,7 +14,7 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
     if (getenv("LWB_NO_MID")) return LWB_OK;
     const bool residue = io->entry != LWB_ENTRY_SPECTRUM;     // residue or VQ entry: the front stages run first
     if (!fused_layout(chains, n_chains, io)) return LWB_OK;
-    const size_t esz = elem_size(io->out_format);
+    const size_t esz = out_format_of(io->out_format).esz;
     const float *pack = nullptr;
     int kb = 0;                                              // 1: n = 1024, 2: n = 512 (one size per batch: one pack)
     // pass 1, no side effects: every packet a full-window block of that size on top of no state or an n/2-sample one

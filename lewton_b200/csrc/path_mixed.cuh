@@ -44,7 +44,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
     if (getenv("LWB_NO_MIXED")) return LWB_OK;
     if (!fused_layout(chains, n_chains, io)) return LWB_OK;
     const bool residue = io->entry != LWB_ENTRY_SPECTRUM;
-    const size_t esz = elem_size(io->out_format);
+    const size_t esz = out_format_of(io->out_format).esz;
     unsigned maxc = 1;
     int n1max = 64, n0max = 64, bs0 = -1;
     size_t total_packets = 0, fast_like = 0;

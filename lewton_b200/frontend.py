@@ -4,7 +4,8 @@
   Headers.decode_packet           audio.rs:919-986            (front half of read_audio_packet_generic)
   Headers.decoded_sample_count    audio.rs:874-909            (get_decoded_sample_count)
   OggPacketReader                 ogg::PacketReader as inside_ogg.rs uses it
-  OggStreamReader                 inside_ogg.rs:60-227        (read_dec_packet, read_dec_packet_itl, get_last_absgp)
+  OggStreamReader                 inside_ogg.rs:60-227        (read_dec_packet, read_dec_packet_itl, read_dec_packet_generic,
+                                                              get_last_absgp)
 
 The entropy decode is CPU work by nature and runs on the host; synthesis goes through the CUDA back
 half (lwb_decode_packet / lwb_decode_chains)."""
@@ -13,7 +14,7 @@ import ctypes as C
 import numpy as np
 
 from . import _cabi as cabi
-from .api import AudioReadError, DecodedPacket, Floor0Record, Setup
+from .api import AudioReadError, DecodedPacket, Floor0Record, Setup, sample_format
 
 (ERR_END_OF_PACKET, ERR_NOT_VORBIS_HEADER, ERR_UNSUPPORTED_VERSION, ERR_HEADER_BAD_FORMAT, ERR_HEADER_BAD_TYPE,
  ERR_HEADER_IS_AUDIO, ERR_UTF8, ERR_AUDIO_IS_HEADER, ERR_OGG, ERR_NO_MORE_PACKETS) = range(16, 26)
@@ -400,9 +401,16 @@ class OggStreamReader:
         """read_dec_packet_generic::<Vec<Vec<f32>>>"""
         return self._read(cabi.OUT_F32_PLANAR, np.float32, False)
 
+    def read_dec_packet_generic(self, sample="f32", interleaved=False):
+        """inside_ogg.rs:191-205, read_dec_packet_generic::<S>: sample "f32" | "i16" | "f16" (numpy float16: the f32
+        samples rounded to nearest even); planar [channels] arrays or one interleaved array, or None at the end."""
+        fmt, dt = sample_format(sample, interleaved)
+        return self._read(fmt, dt, bool(interleaved))
+
     def skip_samples_linear(self, to_skip, sample="f32"):
-        """inside_ogg.rs:244-283 -> (Option<S>, usize): (planar packet or None, samples left to skip inside it)."""
-        fmt, dt = (cabi.OUT_F32_PLANAR, np.float32) if sample == "f32" else (cabi.OUT_I16_PLANAR, np.int16)
+        """inside_ogg.rs:244-283 -> (Option<S>, usize): (planar packet or None, samples left to skip inside it).  sample:
+        "f32", "f16", else i16."""
+        fmt, dt = sample_format(sample if sample in ("f32", "f16") else "i16")
         pck = self._read(fmt, dt, False, skip=int(to_skip))
         return pck, self._skip_left
 
