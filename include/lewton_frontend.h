@@ -162,6 +162,7 @@ typedef struct lwf_stream_job {
 typedef struct lwf_batcher lwf_batcher;
 /* `setup` must come from lwf_headers_make_setup(h, ctx); threads <= 0: one per host CPU */
 int lwf_batcher_create(lwb_ctx *ctx, const lwf_headers *h, int threads, lwf_batcher **out);
+/* waits for the submitted batches that still read the batcher's arenas, then frees them */
 void lwf_batcher_destroy(lwf_batcher *b);
 /* LWB_ENTRY_RESIDUE (default: dense residue vectors cross the boundary) or LWB_ENTRY_VQ (VQ records do; needs
  * lwf_headers_vq_capable) */
@@ -169,11 +170,39 @@ int lwf_batcher_set_entry(lwf_batcher *b, int entry);
 /* records != 0: decode with LWF_DECODE_FLOOR0_RECORDS (the jobs' streams must come from lwf_headers_make_setup_floor0);
  * when every type-0 floor of the stream qualifies, no dense floor arena is allocated or sent */
 int lwf_batcher_set_floor0(lwf_batcher *b, int records);
+/* Returns once the PCM has landed in `pcm` (host memory, pageable or page-locked).  It first waits for every batch
+ * lwf_batcher_submit queued that still reads the batcher's arenas. */
 int lwf_batcher_decode(lwf_batcher *b, lwf_stream_job *jobs, size_t n_jobs, int out_format, void *pcm);
-/* wall-clock seconds of the last lwf_batcher_decode: host entropy decode, synthesis call */
+/* Asynchronous lwf_batcher_decode.  Entropy-decodes `jobs` like lwf_batcher_decode, queues their synthesis as ONE
+ * lwb_submit_chains batch on the batcher's ctx and returns once it is queued.  pcm_memory: LWB_MEM_HOST (`pcm` must be
+ * page-locked, as for a host-memory lwb_submit_chains) or LWB_MEM_DEVICE (`pcm` is device memory of the batcher's ctx;
+ * the PCM never crosses to the host).  *ticket is a ticket of that ctx: wait or query it with lwb_ticket_wait /
+ * lwb_ticket_query; `pcm` holds the PCM once it has completed.
+ * Before it returns:
+ *   - the entropy decode is finished: the jobs' packet buffers may be reused or freed;
+ *   - every job's n_samples, packets_done and status is written, with the values lwf_batcher_decode would give, entropy
+ *     and packet-header errors included;
+ *   - the stream states have advanced, so a stream can appear in the next submit at once.
+ * A refused submit (a NULL argument, a pcm_memory other than the two values, an unknown out_format, pageable host PCM,
+ * anything lwb_submit_chains refuses) changes no job result and no stream state, writes nothing to `pcm` and issues no
+ * ticket.
+ * Device PCM: the batch reads the residue vectors (LWB_ENTRY_RESIDUE) and dense floor-0 curves from device arenas of
+ * the batcher, into which the call copies its pinned ones on lwb_ctx_cuda_stream(); floor and VQ arrays are uploaded by
+ * the library as for any device batch with host floor arrays.  The fused kernels take it under the same alignment rule
+ * as any device batch (lwb_chain); anything else runs on the chain kernel.
+ * Arena sets: the batcher's pinned input arenas, and their device copies, form a ring of two sets.  A submit writes the
+ * set the submit two back read, after that submit's ticket has completed.
+ * A submit blocks the calling thread in these places, and in those lwb_submit_chains lists:
+ *   - the entropy decode of the jobs, on the batcher's thread pool;
+ *   - arena-set wait: with two submits in flight, a third waits for the ticket of the older one;
+ *   - arena growth: a device arena grows after the ctx's stream has drained. */
+int lwf_batcher_submit(lwf_batcher *b, lwf_stream_job *jobs, size_t n_jobs, int out_format, void *pcm, int pcm_memory,
+                       uint64_t *ticket);
+/* wall-clock seconds of the last lwf_batcher_decode: host entropy decode, synthesis call; of the last
+ * lwf_batcher_submit: entropy decode, the rest of the call (arena-set wait, uploads and lwb_submit_chains) */
 void lwf_batcher_last_timing(const lwf_batcher *b, double *entropy_seconds, double *synthesis_seconds);
-/* bytes of the host arrays the last lwf_batcher_decode handed to the synthesis (residues or VQ records, dense floor-0
- * curves, floor kinds and floor1_y rows): what its host-memory batches copy to the device */
+/* bytes of the host arrays the last lwf_batcher_decode or lwf_batcher_submit handed to the synthesis (residues or VQ
+ * records, dense floor-0 curves, floor kinds and floor1_y rows): what its batches copy to the device */
 uint64_t lwf_batcher_last_input_bytes(const lwf_batcher *b);
 
 /* ---- debug taps (known-answer tests of the reference's unit-test vectors) ---------------------- */

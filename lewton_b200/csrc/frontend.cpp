@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "../../include/lewton_frontend.h"
+#include "batcher.h"
 
 // Resource caps for header fields a hostile stream controls (BufferNotAddressable, header.rs:117-125):
 // the spec allows 2^24 codebook entries; value tables beyond 2^26 floats are refused.  The fuzz harness
@@ -1947,41 +1948,7 @@ extern "C" int lwf_reader_last_absgp(const lwf_reader *r, uint64_t *absgp)
 // ---------------------------------------------------------------------------------------------
 // lwf_batcher: parallel host entropy decode + one batched synthesis call
 // ---------------------------------------------------------------------------------------------
-struct PinnedBuf {
-    void *p = nullptr;
-    size_t cap = 0;
-    bool ensure(size_t bytes)
-    {
-        if (bytes <= cap) return true;
-        if (p) lwb_host_free(p);
-        cap = bytes + bytes / 4 + 4096;
-        p = lwb_host_alloc(cap);
-        if (!p) cap = 0;
-        return p != nullptr;
-    }
-    ~PinnedBuf() { if (p) lwb_host_free(p); }
-};
-
-struct BatchArena {
-    PinnedBuf coeffs, dense, kinds, ys, vqrun, vqent, vqroff, vqeoff;
-    std::vector<uint8_t> modes, prevs, nexts;
-    std::vector<lwb_chain> chains;
-    std::vector<std::vector<lwb_vq_run>> job_runs;      // LWB_ENTRY_VQ: per-job records before they are packed (kept
-    std::vector<std::vector<uint16_t>> job_ents;        // across calls: their capacity is what the next batch needs too)
-    uint64_t in_bytes = 0;                              // bytes of the arrays the slice hands to lwb_decode_chains
-};
-
-struct lwf_batcher {
-    lwb_ctx *ctx = nullptr;
-    const lwf_headers *hdr = nullptr;
-    int threads = 1;
-    bool has_floor0 = false;        // the decode can produce dense floor-0 curves: the dense arena is allocated and sent
-    bool floor0_records = false;    // lwf_batcher_set_floor0
-    int entry = LWB_ENTRY_RESIDUE;  // LWB_ENTRY_VQ: the residue crosses the boundary as VQ records
-    BatchArena arena[2];           // slice i decodes into arena[i & 1] while slice i - 1 is being synthesised
-    double t_entropy = 0, t_synth = 0;
-    uint64_t in_bytes = 0;          // of the last lwf_batcher_decode, all slices
-};
+using namespace lwfb;
 
 extern "C" int lwf_batcher_create(lwb_ctx *ctx, const lwf_headers *h, int threads, lwf_batcher **out)
 {
@@ -1997,7 +1964,12 @@ extern "C" int lwf_batcher_create(lwb_ctx *ctx, const lwf_headers *h, int thread
     return LWB_OK;
 }
 
-extern "C" void lwf_batcher_destroy(lwf_batcher *b) { delete b; }
+extern "C" void lwf_batcher_destroy(lwf_batcher *b)
+{
+    if (!b) return;
+    if (b->release) b->release(b, true);                // the arenas may still be read by submitted batches
+    delete b;
+}
 
 extern "C" int lwf_batcher_set_entry(lwf_batcher *b, int entry)
 {
@@ -2024,13 +1996,11 @@ extern "C" void lwf_batcher_last_timing(const lwf_batcher *b, double *e, double 
     if (s) *s = b->t_synth;
 }
 
-static double now_s()
+namespace lwfb {
+double now_s()
 {
     return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
-
-namespace {
-struct JobPlan { uint64_t coeff0, pkt0; uint32_t usable; int32_t head_status; };
 
 // entropy decode of jobs [j0, j1) into `ar` on `threads` host threads
 int batch_entropy(lwf_batcher *b, BatchArena &ar, lwf_stream_job *jobs, size_t j0, size_t j1, std::vector<JobPlan> &plan,
@@ -2180,6 +2150,7 @@ int batch_entropy(lwf_batcher *b, BatchArena &ar, lwf_stream_job *jobs, size_t j
     // what crosses to the device: residues or VQ records, dense floor-0 curves, floor kinds and floor1_y rows
     ar.in_bytes = rows + rows * LWB_MAX_POSTS * 4 + (b->has_floor0 ? coeff_total * 4 : 0) +
                   (vq ? (pkt_total + 1) * 16 + run_off[pkt_total] * sizeof(lwb_vq_run) + ent_off[pkt_total] * 2 : coeff_total * 4);
+    ar.coeff_total = coeff_total;
     // chains of this slice
     ar.chains.assign(j1 - j0, lwb_chain());
     for (size_t j = j0; j < j1; j++) {
@@ -2198,7 +2169,7 @@ int batch_entropy(lwf_batcher *b, BatchArena &ar, lwf_stream_job *jobs, size_t j
     return LWB_OK;
 }
 
-int batch_synth(lwf_batcher *b, BatchArena &ar, int out_format, void *pcm)
+lwb_batch_io batch_io(const lwf_batcher *b, const BatchArena &ar, int out_format, void *pcm)
 {
     lwb_batch_io io;
     std::memset(&io, 0, sizeof(io));
@@ -2214,16 +2185,38 @@ int batch_synth(lwf_batcher *b, BatchArena &ar, int out_format, void *pcm)
     io.floor1_y = (const uint32_t *)ar.ys.p;
     io.out_format = out_format;
     io.pcm = pcm;
-    return lwb_decode_chains(b->ctx, ar.chains.data(), ar.chains.size(), &io);
+    return io;
 }
-}  // namespace
+
+// The synthesis's results, and where it ran every packet the entropy decode passed, the entropy or header error that
+// stopped the stream there.
+void job_results(lwf_stream_job *jobs, size_t j0, size_t j1, const BatchArena &ar, const std::vector<JobPlan> &plan,
+                 const std::vector<uint32_t> &decoded, const std::vector<int32_t> &dec_status)
+{
+    for (size_t j = j0; j < j1; j++) {
+        const lwb_chain &c = ar.chains[j - j0];
+        jobs[j].n_samples = c.n_samples;
+        jobs[j].packets_done = c.packets_done;
+        jobs[j].status = c.status;
+        if (c.status == LWB_OK && c.packets_done == decoded[j] && decoded[j] < jobs[j].n_packets)
+            jobs[j].status = dec_status[j] != LWB_OK ? dec_status[j] : plan[j].head_status;
+    }
+}
+
+int check_jobs(const lwf_stream_job *jobs, size_t n_jobs)
+{
+    for (size_t j = 0; j < n_jobs; j++)
+        if (!jobs[j].stream || (jobs[j].n_packets && (!jobs[j].packets || !jobs[j].lengths))) return LWB_ERR_INVALID;
+    return LWB_OK;
+}
+}  // namespace lwfb
 
 extern "C" int lwf_batcher_decode(lwf_batcher *b, lwf_stream_job *jobs, size_t n_jobs, int out_format, void *pcm)
 {
-    if (!b || (!jobs && n_jobs) || !pcm) return LWB_ERR_INVALID;
-    for (size_t j = 0; j < n_jobs; j++)
-        if (!jobs[j].stream || (jobs[j].n_packets && (!jobs[j].packets || !jobs[j].lengths))) return LWB_ERR_INVALID;
+    if (!b || (!jobs && n_jobs) || !pcm || check_jobs(jobs, n_jobs)) return LWB_ERR_INVALID;
     LWF_GUARD(
+        int rc = b->release ? b->release(b, false) : LWB_OK;      // submitted batches may still read the arenas
+        if (rc) return rc;
         std::vector<JobPlan> plan(n_jobs);
         std::vector<uint32_t> decoded(n_jobs, 0);
         std::vector<int32_t> dec_status(n_jobs, LWB_OK);
@@ -2232,7 +2225,7 @@ extern "C" int lwf_batcher_decode(lwf_batcher *b, lwf_stream_job *jobs, size_t n
         const size_t n_slices = std::max<size_t>(1, std::min<size_t>(4, n_jobs / 8));
         double entropy_busy = 0, synth_busy = 0;
         uint64_t in_bytes = 0;
-        int synth_rc = LWB_OK, rc = LWB_OK;
+        int synth_rc = LWB_OK;
         std::thread synth;
         struct Joiner { std::thread &t; ~Joiner() { if (t.joinable()) t.join(); } } joiner{synth};   // also on unwinding
         for (size_t sl = 0; sl < n_slices && rc == LWB_OK; sl++) {
@@ -2248,17 +2241,11 @@ extern "C" int lwf_batcher_decode(lwf_batcher *b, lwf_stream_job *jobs, size_t n
             if (rc != LWB_OK || synth_rc != LWB_OK) break;
             synth = std::thread([b, &ar, out_format, pcm, jobs, j0, j1, &plan, &decoded, &dec_status, &synth_rc, &synth_busy]() {
                 const double s0 = now_s();
-                const int r = batch_synth(b, ar, out_format, pcm);
+                const lwb_batch_io io = batch_io(b, ar, out_format, pcm);
+                const int r = lwb_decode_chains(b->ctx, ar.chains.data(), ar.chains.size(), &io);
                 synth_busy += now_s() - s0;
                 if (r) { synth_rc = r; return; }
-                for (size_t j = j0; j < j1; j++) {
-                    const lwb_chain &c = ar.chains[j - j0];
-                    jobs[j].n_samples = c.n_samples;
-                    jobs[j].packets_done = c.packets_done;
-                    jobs[j].status = c.status;
-                    if (c.status == LWB_OK && c.packets_done == decoded[j] && decoded[j] < jobs[j].n_packets)
-                        jobs[j].status = dec_status[j] != LWB_OK ? dec_status[j] : plan[j].head_status;
-                }
+                job_results(jobs, j0, j1, ar, plan, decoded, dec_status);
             });
         }
         if (synth.joinable()) synth.join();

@@ -24,7 +24,7 @@ SYMBOLS = ["lwf_headers_parse", "lwf_headers_destroy", "lwf_headers_info", "lwf_
            "lwf_reader_open", "lwf_reader_close", "lwf_reader_headers", "lwf_reader_read_dec_packet", "lwf_reader_last_absgp",
            "lwf_reader_skip_samples_linear", "lwf_reader_seek_absgp_pg",
            "lwf_batcher_create", "lwf_batcher_destroy", "lwf_batcher_set_entry", "lwf_batcher_decode", "lwf_batcher_last_timing",
-           "lwf_batcher_last_input_bytes", "lwf_batcher_set_floor0",
+           "lwf_batcher_last_input_bytes", "lwf_batcher_set_floor0", "lwf_batcher_submit",
            "lwf_debug_float32_unpack", "lwf_debug_lookup1_values", "lwf_debug_ilog", "lwf_debug_read_bits", "lwf_debug_huffman",
            "lwf_debug_decode_loop"]
 
@@ -117,6 +117,7 @@ def lib():
         L.lwf_packet_decode_vq.argtypes = [vp, C.c_char_p, sz, vp, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz)]
         L.lwf_packet_decode_vq_ex.argtypes = [vp, C.c_char_p, sz, vp, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz), C.c_int]
         L.lwf_batcher_decode.argtypes = [vp, C.POINTER(_StreamJob), sz, C.c_int, vp]
+        L.lwf_batcher_submit.argtypes = [vp, C.POINTER(_StreamJob), sz, C.c_int, vp, C.c_int, C.POINTER(C.c_uint64)]
         L.lwf_batcher_last_timing.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double)]
         L.lwf_batcher_last_timing.restype = None
         L.lwf_debug_float32_unpack.argtypes = [C.c_uint32]
@@ -466,7 +467,8 @@ class StreamBatcher:
             if rc:
                 raise AudioReadError(rc, "this stream does not qualify for LWB_ENTRY_VQ (lwf_headers_vq_capable)")
 
-    def decode(self, jobs, pcm, stride, out_format=cabi.OUT_F32_PLANAR):
+    def _jobs(self, jobs, stride):
+        """The lwf_stream_job array of `jobs`, and the packet arrays it points to."""
         n = len(jobs)
         arr = (_StreamJob * n)()
         keep = []
@@ -481,18 +483,43 @@ class StreamBatcher:
             arr[j].lengths = ln
             arr[j].out_offset = j * Cn * stride
             arr[j].out_stride = stride
-        self.prepared = (arr, keep, n)
+        return arr, keep, n
+
+    def _counters(self):
+        e, s = C.c_double(), C.c_double()
+        lib().lwf_batcher_last_timing(self._h, C.byref(e), C.byref(s))
+        self.entropy_seconds, self.synthesis_seconds = e.value, s.value
+        self.input_bytes = lib().lwf_batcher_last_input_bytes(self._h)
+
+    def decode(self, jobs, pcm, stride, out_format=cabi.OUT_F32_PLANAR):
+        self.prepared = self._jobs(jobs, stride)
         return self.run(pcm, out_format)
 
     def run(self, pcm, out_format=cabi.OUT_F32_PLANAR):
         """Decode the jobs of the last decode() again (same packets; benchmarking)."""
         arr, _, n = self.prepared
         self.ctx.check(lib().lwf_batcher_decode(self._h, arr, n, out_format, pcm.ctypes.data))
-        e, s = C.c_double(), C.c_double()
-        lib().lwf_batcher_last_timing(self._h, C.byref(e), C.byref(s))
-        self.entropy_seconds, self.synthesis_seconds = e.value, s.value
-        self.input_bytes = lib().lwf_batcher_last_input_bytes(self._h)
-        return [(arr[j].n_samples, arr[j].packets_done, arr[j].status) for j in range(n)]
+        self._counters()
+        return _results(arr, n)
+
+    def submit(self, jobs, pcm, stride, out_format=cabi.OUT_F32_PLANAR):
+        """lwf_batcher_submit: entropy-decodes `jobs` (as decode()), queues their synthesis and returns a BatcherTicket
+        once it is queued.  pcm: a page-locked numpy array (Context.host_alloc), a torch CUDA tensor or an integer device
+        pointer; the memory space follows from it.  The streams may be submitted again at once; `pcm` holds the PCM once
+        the ticket is done.  entropy_seconds / synthesis_seconds / input_bytes describe this submit."""
+        if isinstance(pcm, np.ndarray):
+            addr, memory = pcm.ctypes.data, cabi.MEM_HOST
+        elif isinstance(pcm, int):
+            addr, memory = pcm, cabi.MEM_DEVICE
+        elif hasattr(pcm, "data_ptr") and getattr(pcm, "is_cuda", False):
+            addr, memory = pcm.data_ptr(), cabi.MEM_DEVICE
+        else:
+            raise TypeError("pcm: a page-locked numpy array, a torch CUDA tensor or an integer device pointer")
+        arr, keep, n = self._jobs(jobs, stride)
+        t = C.c_uint64()
+        self.ctx.check(lib().lwf_batcher_submit(self._h, arr, n, out_format, addr, memory, C.byref(t)))
+        self._counters()
+        return BatcherTicket(self.ctx, t.value, arr, n, (keep, pcm))
 
     def close(self):
         if self._h:
@@ -504,3 +531,33 @@ class StreamBatcher:
             self.close()
         except Exception:
             pass
+
+
+def _results(arr, n):
+    return [(arr[j].n_samples, arr[j].packets_done, arr[j].status) for j in range(n)]
+
+
+class BatcherTicket:
+    """A batch queued by StreamBatcher.submit, in the manner of api.Ticket.  It keeps `pcm` and the job arrays alive until
+    it is done; the job results were written before submit returned."""
+
+    def __init__(self, ctx, ticket, arr, n, keep):
+        self.ctx, self.id = ctx, ticket
+        self._arr, self._n, self._keep = arr, n, keep
+
+    def done(self):
+        """lwb_ticket_query: whether every copy and kernel of the batch has finished.  Never blocks."""
+        if self._keep is not None:
+            d = C.c_int()
+            self.ctx.check(cabi.lib().lwb_ticket_query(self.ctx._h, self.id, C.byref(d)))
+            if not d.value:
+                return False
+            self._keep = None
+        return True
+
+    def wait(self):
+        """lwb_ticket_wait; returns the job results [(n_samples, packets_done, status)], as StreamBatcher.run does."""
+        if self._keep is not None:
+            self.ctx.check(cabi.lib().lwb_ticket_wait(self.ctx._h, self.id))
+            self._keep = None
+        return _results(self._arr, self._n)
