@@ -164,20 +164,32 @@ typedef struct lwf_batcher lwf_batcher;
 int lwf_batcher_create(lwb_ctx *ctx, const lwf_headers *h, int threads, lwf_batcher **out);
 /* waits for the submitted batches that still read the batcher's arenas, then frees them */
 void lwf_batcher_destroy(lwf_batcher *b);
+/* Jobs whose stream was opened on `setup` are entropy-decoded with `h` (which, like the batcher's own headers, must
+ * outlive the batcher).  Streams of any setup not registered here keep the headers given to lwf_batcher_create, as
+ * before.  LWB_ERR_INVALID: NULL argument, a setup already registered, a setup whose channel count or blocksizes differ
+ * from h's ident header (or that was made on another context), or (LWB_ENTRY_VQ) headers that fail
+ * lwf_headers_vq_capable.
+ * Header sets are grouped by (channel count, blocksize_0, blocksize_1); the batcher's own headers form a group too.  A
+ * decode or submit entropy-decodes all its jobs in one parallel pass, then synthesises each group's jobs as one batch
+ * (a residue or VQ batch has one channel count, and a batch of one blocksize pair runs whole on that shape's fused
+ * kernel).  With no header set added there is one group, and every call makes the batches it made before. */
+int lwf_batcher_add_headers(lwf_batcher *b, const lwf_headers *h, const lwb_setup *setup);
 /* LWB_ENTRY_RESIDUE (default: dense residue vectors cross the boundary) or LWB_ENTRY_VQ (VQ records do; needs
- * lwf_headers_vq_capable) */
+ * lwf_headers_vq_capable of the batcher's headers and of every header set added) */
 int lwf_batcher_set_entry(lwf_batcher *b, int entry);
 /* records != 0: decode with LWF_DECODE_FLOOR0_RECORDS (the jobs' streams must come from lwf_headers_make_setup_floor0);
- * when every type-0 floor of the stream qualifies, no dense floor arena is allocated or sent */
+ * applies to every header set.  A group whose type-0 floors all qualify allocates and sends no dense floor arena. */
 int lwf_batcher_set_floor0(lwf_batcher *b, int records);
 /* Returns once the PCM has landed in `pcm` (host memory, pageable or page-locked).  It first waits for every batch
  * lwf_batcher_submit queued that still reads the batcher's arenas. */
 int lwf_batcher_decode(lwf_batcher *b, lwf_stream_job *jobs, size_t n_jobs, int out_format, void *pcm);
 /* Asynchronous lwf_batcher_decode.  Entropy-decodes `jobs` like lwf_batcher_decode, queues their synthesis as ONE
- * lwb_submit_chains batch on the batcher's ctx and returns once it is queued.  pcm_memory: LWB_MEM_HOST (`pcm` must be
- * page-locked, as for a host-memory lwb_submit_chains) or LWB_MEM_DEVICE (`pcm` is device memory of the batcher's ctx;
- * the PCM never crosses to the host).  *ticket is a ticket of that ctx: wait or query it with lwb_ticket_wait /
- * lwb_ticket_query; `pcm` holds the PCM once it has completed.
+ * lwb_submit_chains batch per group of header sets (lwf_batcher_add_headers), back to back, on the batcher's ctx and
+ * returns once they are queued.  pcm_memory: LWB_MEM_HOST (`pcm` must be page-locked, as for a host-memory
+ * lwb_submit_chains) or LWB_MEM_DEVICE (`pcm` is device memory of the batcher's ctx; the PCM never crosses to the
+ * host).  *ticket is a ticket of that ctx, the last group's (tickets complete in submission order, so it covers every
+ * batch of the call): wait or query it with lwb_ticket_wait / lwb_ticket_query; `pcm` holds the PCM once it has
+ * completed.
  * Before it returns:
  *   - the entropy decode is finished: the jobs' packet buffers may be reused or freed;
  *   - every job's n_samples, packets_done and status is written, with the values lwf_batcher_decode would give, entropy
@@ -185,13 +197,17 @@ int lwf_batcher_decode(lwf_batcher *b, lwf_stream_job *jobs, size_t n_jobs, int 
  *   - the stream states have advanced, so a stream can appear in the next submit at once.
  * A refused submit (a NULL argument, a pcm_memory other than the two values, an unknown out_format, pageable host PCM,
  * anything lwb_submit_chains refuses) changes no job result and no stream state, writes nothing to `pcm` and issues no
- * ticket.
+ * ticket.  With several groups, every group's batch is checked (page-locked PCM included) and every arena grown before
+ * the first is queued.  Only LWB_ERR_CUDA or LWB_ERR_BUFFER can then stop a later group's batch: the call returns it
+ * without a ticket; the groups queued before it have written their jobs' results and advanced their streams
+ * (lwb_ctx_synchronize waits for their PCM), the device-side states of the failing group's streams are undefined, and
+ * the jobs and streams of the groups after it are unchanged.
  * Device PCM: the batch reads the residue vectors (LWB_ENTRY_RESIDUE) and dense floor-0 curves from device arenas of
  * the batcher, into which the call copies its pinned ones on lwb_ctx_cuda_stream(); floor and VQ arrays are uploaded by
  * the library as for any device batch with host floor arrays.  The fused kernels take it under the same alignment rule
  * as any device batch (lwb_chain); anything else runs on the chain kernel.
- * Arena sets: the batcher's pinned input arenas, and their device copies, form a ring of two sets.  A submit writes the
- * set the submit two back read, after that submit's ticket has completed.
+ * Arena sets: the batcher's pinned input arenas, and their device copies, form a ring of two sets (each with one arena
+ * per group).  A submit writes the set the submit two back read, after that submit's ticket has completed.
  * A submit blocks the calling thread in these places, and in those lwb_submit_chains lists:
  *   - the entropy decode of the jobs, on the batcher's thread pool;
  *   - arena-set wait: with two submits in flight, a third waits for the ticket of the older one;

@@ -1,11 +1,14 @@
 // batcher.h -- internals of lwf_batcher (include/lewton_frontend.h) shared by its two halves: frontend.cpp, the
-// host entropy decode and the synchronous lwf_batcher_decode, and batcher_submit.cpp, the asynchronous lwf_batcher_submit.
+// host entropy decode and the synchronous lwf_batcher_decode, and batcher_submit.cpp, the asynchronous lwf_batcher_submit
+// and lwf_batcher_add_headers.
 // frontend.cpp needs no CUDA and calls only the synchronous back half, so that it also builds against a stub back half
-// (the fuzz harness); whatever submits use beyond that is reached through lwf_batcher::release.
+// (the fuzz harness); whatever submits and header sets use beyond that is reached through the hooks on lwf_batcher
+// (release, set_of).
 #ifndef LWF_BATCHER_H
 #define LWF_BATCHER_H
 
 #include <cstdint>
+#include <memory>
 #include <vector>
 
 #include "../../include/lewton_frontend.h"
@@ -31,13 +34,33 @@ struct BatchArena {
     PinnedBuf coeffs, dense, kinds, ys, vqrun, vqent, vqroff, vqeoff;
     std::vector<uint8_t> modes, prevs, nexts;
     std::vector<lwb_chain> chains;
-    std::vector<std::vector<lwb_vq_run>> job_runs;      // LWB_ENTRY_VQ: per-job records before they are packed (kept
+    std::vector<size_t> job;                            // the index in the caller's job array of each chain
+    std::vector<std::vector<lwb_vq_run>> job_runs;      // LWB_ENTRY_VQ: per-chain records before they are packed (kept
     std::vector<std::vector<uint16_t>> job_ents;        // across calls: their capacity is what the next batch needs too)
-    uint64_t in_bytes = 0;                              // bytes of the arrays the slice hands to lwb_decode_chains
-    uint64_t coeff_total = 0;                           // elements of the slice's coefficient (and dense floor) arena
+    uint64_t in_bytes = 0;                              // bytes of the arrays the batch hands to lwb_decode_chains
+    uint64_t coeff_total = 0;                           // elements of the batch's coefficient (and dense floor) arena
 };
 
-struct JobPlan { uint64_t coeff0, pkt0; uint32_t usable; int32_t head_status; };
+// The streams of one group share a channel count and a blocksize pair, and go to the synthesis as one batch: the
+// library takes residue batches of one channel count only, and a batch of one blocksize pair runs whole on the fused
+// kernel of that shape (k_long, the mixed schedule, k_mid) instead of falling to k_chain rounds.
+struct Group {
+    uint8_t channels = 0, bs0 = 0, bs1 = 0;
+    bool has_floor0 = false;        // a header set of the group can produce dense floor-0 curves: the dense arena is sent
+    // lwf_batcher_decode: slice i decodes into arena[i & 1] while slice i - 1 is being synthesised.
+    // lwf_batcher_submit: the two sets form a ring; a submit decodes into the set the submit two back read.
+    BatchArena arena[2];
+};
+
+// A set of headers and the setup whose streams it decodes; set 0 is lwf_batcher_create's, for the streams of every
+// setup not registered with lwf_batcher_add_headers (its setup is NULL).
+struct HeaderSet {
+    const lwf_headers *h = nullptr;
+    const lwb_setup *setup = nullptr;
+    size_t group = 0;
+};
+
+struct JobPlan { uint64_t coeff0, pkt0; uint32_t usable; int32_t head_status; size_t set, slot; };
 
 struct SubmitRing;      // batcher_submit.cpp: the tickets and device arenas of lwf_batcher_submit
 
@@ -45,20 +68,19 @@ struct SubmitRing;      // batcher_submit.cpp: the tickets and device arenas of 
 
 struct lwf_batcher {
     lwb_ctx *ctx = nullptr;
-    const lwf_headers *hdr = nullptr;
     int threads = 1;
-    bool has_floor0 = false;        // the decode can produce dense floor-0 curves: the dense arena is allocated and sent
     bool floor0_records = false;    // lwf_batcher_set_floor0
     int entry = LWB_ENTRY_RESIDUE;  // LWB_ENTRY_VQ: the residue crosses the boundary as VQ records
-    // lwf_batcher_decode: slice i decodes into arena[i & 1] while slice i - 1 is being synthesised.
-    // lwf_batcher_submit: the two sets form a ring; a submit decodes into the set the submit two back read.
-    lwfb::BatchArena arena[2];
+    std::vector<lwfb::HeaderSet> sets;
+    std::vector<std::unique_ptr<lwfb::Group>> groups;   // (not moved when a group is added: submits may read their arenas)
     double t_entropy = 0, t_synth = 0;
-    uint64_t in_bytes = 0;          // of the last lwf_batcher_decode (all slices) or lwf_batcher_submit
+    uint64_t in_bytes = 0;          // of the last lwf_batcher_decode (all slices) or lwf_batcher_submit (all groups)
     // Set by the first lwf_batcher_submit: waits for the submits that still read the arena sets (and with destroy, frees
     // the ring and its device arenas).  lwf_batcher_decode and lwf_batcher_destroy call it before they touch the arenas.
     lwfb::SubmitRing *ring = nullptr;
     int (*release)(lwf_batcher *b, bool destroy) = nullptr;
+    // Set by the first lwf_batcher_add_headers: the header set of the jobs of stream s.  Without it every job has set 0.
+    size_t (*set_of)(const lwf_batcher *b, const lwb_stream *s) = nullptr;
 };
 
 namespace lwfb {
@@ -66,14 +88,28 @@ namespace lwfb {
 double now_s();
 // any job without a stream, or with packets but no packet or length array: LWB_ERR_INVALID
 int check_jobs(const lwf_stream_job *jobs, size_t n_jobs);
-// entropy decode of jobs [j0, j1) into `ar` on the batcher's host threads; fills ar's chains
-int batch_entropy(lwf_batcher *b, BatchArena &ar, lwf_stream_job *jobs, size_t j0, size_t j1, std::vector<JobPlan> &plan,
-                  std::vector<uint32_t> &decoded, std::vector<int32_t> &dec_status);
-// the host-memory batch of arena set `ar`
-lwb_batch_io batch_io(const lwf_batcher *b, const BatchArena &ar, int out_format, void *pcm);
-// job results of chains [j0, j1) of `ar` after their synthesis
-void job_results(lwf_stream_job *jobs, size_t j0, size_t j1, const BatchArena &ar, const std::vector<JobPlan> &plan,
-                 const std::vector<uint32_t> &decoded, const std::vector<int32_t> &dec_status);
+// plan[j].set for every job
+void assign_sets(const lwf_batcher *b, const lwf_stream_job *jobs, size_t n_jobs, std::vector<JobPlan> &plan);
+// which groups have dense floor-0 curves, after a header set was added or lwf_batcher_set_floor0
+void update_floor0(lwf_batcher *b);
+// Entropy decode of jobs list[0 .. n) (plan[j].set assigned) into arena set `set` of their groups, in one parallel pass
+// on the batcher's host threads; fills the arenas' chains, each group's in list order.  *used: the groups with jobs in
+// the list, ascending, or group 0 alone if the list is empty.
+int batch_entropy(lwf_batcher *b, size_t set, lwf_stream_job *jobs, const size_t *list, size_t n, std::vector<JobPlan> &plan,
+                  std::vector<uint32_t> &decoded, std::vector<int32_t> &dec_status, std::vector<size_t> *used);
+// the host-memory batch of group g's arena set `ar`
+lwb_batch_io batch_io(const lwf_batcher *b, size_t g, const BatchArena &ar, int out_format, void *pcm);
+// job results of the chains of `ar` after their synthesis
+void job_results(lwf_stream_job *jobs, const BatchArena &ar, const std::vector<JobPlan> &plan, const std::vector<uint32_t> &decoded,
+                 const std::vector<int32_t> &dec_status);
+
+// lwb_api.cu: what the batcher needs to know of lwb_setup and lwb_stream
+struct SetupShape { const lwb_ctx *ctx; uint8_t channels, bs0, bs1; };
+SetupShape setup_shape(const lwb_setup *su);
+const lwb_setup *stream_setup(const lwb_stream *s);
+// The refusals lwb_submit_chains would make of this batch (out_format, streams, one channel count, a stream in two
+// chains, floor kinds, out_stride, page-locked host memory), made without queuing anything or changing any state.
+int check_submit(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io);
 
 }  // namespace lwfb
 

@@ -1953,15 +1953,21 @@ using namespace lwfb;
 extern "C" int lwf_batcher_create(lwb_ctx *ctx, const lwf_headers *h, int threads, lwf_batcher **out)
 {
     if (!ctx || !h || !out) return LWB_ERR_INVALID;
-    lwf_batcher *b = new (std::nothrow) lwf_batcher();
-    if (!b) return LWB_ERR_BUFFER;
-    b->ctx = ctx;
-    b->hdr = h;
-    if (threads <= 0) threads = (int)std::thread::hardware_concurrency();
-    b->threads = std::max(1, threads);
-    b->has_floor0 = needs_dense(h->h, 0);
-    *out = b;
-    return LWB_OK;
+    LWF_GUARD(
+        std::unique_ptr<lwf_batcher> b(new lwf_batcher());
+        b->ctx = ctx;
+        if (threads <= 0) threads = (int)std::thread::hardware_concurrency();
+        b->threads = std::max(1, threads);
+        b->groups.emplace_back(new Group());
+        Group &g = *b->groups[0];
+        g.channels = h->h.ident.audio_channels;
+        g.bs0 = h->h.ident.blocksize_0;
+        g.bs1 = h->h.ident.blocksize_1;
+        b->sets.push_back(HeaderSet{h, nullptr, 0});
+        update_floor0(b.get());
+        *out = b.release();
+        return LWB_OK;
+    )
 }
 
 extern "C" void lwf_batcher_destroy(lwf_batcher *b)
@@ -1974,7 +1980,9 @@ extern "C" void lwf_batcher_destroy(lwf_batcher *b)
 extern "C" int lwf_batcher_set_entry(lwf_batcher *b, int entry)
 {
     if (!b || (entry != LWB_ENTRY_RESIDUE && entry != LWB_ENTRY_VQ)) return LWB_ERR_INVALID;
-    if (entry == LWB_ENTRY_VQ && !lwf_headers_vq_capable(b->hdr)) return LWB_ERR_INVALID;
+    if (entry == LWB_ENTRY_VQ)
+        for (const HeaderSet &s : b->sets)
+            if (!lwf_headers_vq_capable(s.h)) return LWB_ERR_INVALID;
     b->entry = entry;
     return LWB_OK;
 }
@@ -1985,7 +1993,7 @@ extern "C" int lwf_batcher_set_floor0(lwf_batcher *b, int records)
 {
     if (!b) return LWB_ERR_INVALID;
     b->floor0_records = records != 0;
-    b->has_floor0 = needs_dense(b->hdr->h, b->floor0_records ? LWF_DECODE_FLOOR0_RECORDS : 0);
+    update_floor0(b);
     return LWB_OK;
 }
 
@@ -2002,62 +2010,97 @@ double now_s()
     return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
 
-// entropy decode of jobs [j0, j1) into `ar` on `threads` host threads
-int batch_entropy(lwf_batcher *b, BatchArena &ar, lwf_stream_job *jobs, size_t j0, size_t j1, std::vector<JobPlan> &plan,
-                  std::vector<uint32_t> &decoded, std::vector<int32_t> &dec_status)
+void assign_sets(const lwf_batcher *b, const lwf_stream_job *jobs, size_t n_jobs, std::vector<JobPlan> &plan)
 {
-    const lwf::Headers &H = b->hdr->h;
-    const size_t C = H.ident.audio_channels;
-    // pass 1 (cheap, serial): packet headers -> blocksizes -> arena offsets.  A packet whose header
+    for (size_t j = 0; j < n_jobs; j++) plan[j].set = b->set_of ? b->set_of(b, jobs[j].stream) : 0;
+}
+
+void update_floor0(lwf_batcher *b)
+{
+    for (auto &g : b->groups) g->has_floor0 = false;
+    for (const HeaderSet &s : b->sets)
+        if (needs_dense(s.h->h, b->floor0_records ? LWF_DECODE_FLOOR0_RECORDS : 0)) b->groups[s.group]->has_floor0 = true;
+}
+
+// entropy decode of jobs list[0 .. n) into arena set `set` of their groups on the batcher's host threads
+int batch_entropy(lwf_batcher *b, size_t set, lwf_stream_job *jobs, const size_t *list, size_t n, std::vector<JobPlan> &plan,
+                  std::vector<uint32_t> &decoded, std::vector<int32_t> &dec_status, std::vector<size_t> *used)
+{
+    const size_t n_groups = b->groups.size();
+    // pass 1 (cheap, serial): packet headers -> blocksizes -> arena offsets in the job's group.  A packet whose header
     // cannot be read ends its stream's chain there (its error is reported after the earlier ones ran).
-    uint64_t coeff_total = 0, pkt_total = 0;
-    for (size_t j = j0; j < j1; j++) {
-        lwf_stream_job &job = jobs[j];
-        plan[j] = JobPlan{coeff_total, pkt_total, 0, LWB_OK};
+    std::vector<uint64_t> coeff_total(n_groups, 0), pkt_total(n_groups, 0);
+    std::vector<std::vector<size_t>> members(n_groups);        // the jobs of each group, in list order
+    for (size_t i = 0; i < n; i++) {
+        const size_t j = list[i];
+        const lwf_stream_job &job = jobs[j];
+        JobPlan &p = plan[j];
+        const size_t g = b->sets[p.set].group;
+        const lwf::Headers &H = b->sets[p.set].h->h;
+        const size_t C = b->groups[g]->channels;
+        p.coeff0 = coeff_total[g];
+        p.pkt0 = pkt_total[g];
+        p.usable = 0;
+        p.head_status = LWB_OK;
+        p.slot = members[g].size();
+        members[g].push_back(j);
         for (uint32_t k = 0; k < job.n_packets; k++) {
             lwf::BitReader rdr(job.packets[k], job.lengths[k]);
             lwf::PacketHead ph;
             const int rc = lwf::packet_head(H, rdr, &ph);
-            if (rc) { plan[j].head_status = rc; break; }
-            coeff_total += (uint64_t)C * (ph.n / 2);
-            plan[j].usable++;
+            if (rc) { p.head_status = rc; break; }
+            coeff_total[g] += (uint64_t)C * (ph.n / 2);
+            p.usable++;
         }
-        pkt_total += plan[j].usable;
+        pkt_total[g] += p.usable;
     }
-    const size_t rows = (size_t)pkt_total * C;
+    used->clear();
+    for (size_t g = 0; g < n_groups; g++)
+        if (!members[g].empty()) used->push_back(g);
+    if (used->empty()) used->push_back(0);
     const bool vq = b->entry == LWB_ENTRY_VQ;
-    if ((!vq && !ar.coeffs.ensure((size_t)coeff_total * 4 + 16)) || !ar.kinds.ensure(rows + 16) || !ar.ys.ensure(rows * LWB_MAX_POSTS * 4 + 16) ||
-        (b->has_floor0 && !ar.dense.ensure((size_t)coeff_total * 4 + 16)) || (vq && (!ar.vqroff.ensure(((size_t)pkt_total + 1) * 8 + 16) || !ar.vqeoff.ensure(((size_t)pkt_total + 1) * 8 + 16))))
-        return LWB_ERR_BUFFER;
-    // VQ: every stream's records are collected per job first (their number is only known after the decode), then
-    // packed into one pinned arena with per-packet offsets
-    std::vector<std::vector<lwb_vq_run>> &job_runs = ar.job_runs;
-    std::vector<std::vector<uint16_t>> &job_ents = ar.job_ents;
-    if (vq) {
-        if (job_runs.size() < j1 - j0) { job_runs.resize(j1 - j0); job_ents.resize(j1 - j0); }
-        for (size_t j = 0; j < j1 - j0; j++) { job_runs[j].clear(); job_ents[j].clear(); }
+    for (size_t g : *used) {
+        BatchArena &ar = b->groups[g]->arena[set];
+        const size_t rows = (size_t)pkt_total[g] * b->groups[g]->channels;
+        if ((!vq && !ar.coeffs.ensure((size_t)coeff_total[g] * 4 + 16)) || !ar.kinds.ensure(rows + 16) || !ar.ys.ensure(rows * LWB_MAX_POSTS * 4 + 16) ||
+            (b->groups[g]->has_floor0 && !ar.dense.ensure((size_t)coeff_total[g] * 4 + 16)) ||
+            (vq && (!ar.vqroff.ensure(((size_t)pkt_total[g] + 1) * 8 + 16) || !ar.vqeoff.ensure(((size_t)pkt_total[g] + 1) * 8 + 16))))
+            return LWB_ERR_BUFFER;
+        // VQ: every stream's records are collected per job first (their number is only known after the decode), then
+        // packed into one pinned arena with per-packet offsets
+        if (vq) {
+            const size_t m = members[g].size();
+            if (ar.job_runs.size() < m) { ar.job_runs.resize(m); ar.job_ents.resize(m); }
+            for (size_t s = 0; s < m; s++) { ar.job_runs[s].clear(); ar.job_ents[s].clear(); }
+        }
+        ar.modes.resize(pkt_total[g]);
+        ar.prevs.resize(pkt_total[g]);
+        ar.nexts.resize(pkt_total[g]);
     }
-    uint64_t *run_off = vq ? (uint64_t *)ar.vqroff.p : nullptr, *ent_off = vq ? (uint64_t *)ar.vqeoff.p : nullptr;
-    ar.modes.resize(pkt_total);
-    ar.prevs.resize(pkt_total);
-    ar.nexts.resize(pkt_total);
-    float *coeffs = (float *)ar.coeffs.p, *dense = b->has_floor0 ? (float *)ar.dense.p : nullptr;
-    uint8_t *kinds = (uint8_t *)ar.kinds.p;
-    uint32_t *ys = (uint32_t *)ar.ys.p;
-    // pass 2 (parallel over streams): entropy decode straight into the arenas
-    std::atomic<size_t> next_job(j0);
+    // pass 2 (parallel over all jobs of the list): entropy decode straight into the arenas of each job's group
+    std::atomic<size_t> next_job(0);
     std::atomic<int> failed(0);
     auto worker = [&]() {
         try {
             std::vector<lwb_vq_run> scratch_runs;        // LWB_ENTRY_VQ: one packet's records (see below)
             std::vector<uint16_t> scratch_ents;
             for (;;) {
-                const size_t j = next_job.fetch_add(1);
-                if (j >= j1) break;
+                const size_t i = next_job.fetch_add(1);
+                if (i >= n) break;
+                const size_t j = list[i];
                 const lwf_stream_job &job = jobs[j];
-                uint64_t coff = plan[j].coeff0;
-                for (uint32_t k = 0; k < plan[j].usable; k++) {
-                    const uint64_t pi = plan[j].pkt0 + k;
+                const JobPlan &p = plan[j];
+                const lwf::Headers &H = b->sets[p.set].h->h;
+                Group &G = *b->groups[b->sets[p.set].group];
+                BatchArena &ar = G.arena[set];
+                const size_t C = G.channels;
+                float *coeffs = (float *)ar.coeffs.p, *dense = G.has_floor0 ? (float *)ar.dense.p : nullptr;
+                uint8_t *kinds = (uint8_t *)ar.kinds.p;
+                uint32_t *ys = (uint32_t *)ar.ys.p;
+                uint64_t *run_off = vq ? (uint64_t *)ar.vqroff.p : nullptr, *ent_off = vq ? (uint64_t *)ar.vqeoff.p : nullptr;
+                uint64_t coff = p.coeff0;
+                for (uint32_t k = 0; k < p.usable; k++) {
+                    const uint64_t pi = p.pkt0 + k;
                     lwf_decoded_packet dp;
                     std::memset(&dp, 0, sizeof(dp));
                     dp.floor_kind = kinds + pi * C;
@@ -2066,8 +2109,8 @@ int batch_entropy(lwf_batcher *b, BatchArena &ar, lwf_stream_job *jobs, size_t j
                     dp.dense_floor = dense ? dense + coff : nullptr;
                     int rc;
                     if (vq) {
-                        std::vector<lwb_vq_run> &jr = job_runs[j - j0];
-                        std::vector<uint16_t> &je = job_ents[j - j0];
+                        std::vector<lwb_vq_run> &jr = ar.job_runs[p.slot];
+                        std::vector<uint16_t> &je = ar.job_ents[p.slot];
                         // decoded into the thread's scratch (a packet of b bytes holds fewer than 8 b codewords), then only
                         // what it produced is appended (growing the job's vectors to the bound first meant zero-filling
                         // ~22 KB per 280-byte packet)
@@ -2101,7 +2144,7 @@ int batch_entropy(lwf_batcher *b, BatchArena &ar, lwf_stream_job *jobs, size_t j
             failed.store(1);
         }
     };
-    const int nt = (int)std::min<size_t>((size_t)b->threads, std::max<size_t>(1, j1 - j0));
+    const int nt = (int)std::min<size_t>((size_t)b->threads, std::max<size_t>(1, n));
     std::vector<std::thread> pool;
     try {
         pool.reserve((size_t)nt);
@@ -2115,27 +2158,33 @@ int batch_entropy(lwf_batcher *b, BatchArena &ar, lwf_stream_job *jobs, size_t j
     if (failed.load()) return LWB_ERR_BUFFER;
     if (vq) {
         // counts -> offsets (rows of packets that were not decoded own nothing), then one packed copy of each array
-        run_off[0] = ent_off[0] = 0;
-        for (size_t j = j0; j < j1; j++)
-            for (uint32_t k = 0; k < plan[j].usable; k++) {
-                const uint64_t pi = plan[j].pkt0 + k;
-                const bool ok = k < decoded[j];
-                run_off[pi + 1] = run_off[pi] + (ok ? run_off[pi + 1] : 0);
-                ent_off[pi + 1] = ent_off[pi] + (ok ? ent_off[pi + 1] : 0);
-            }
-        if (!ar.vqrun.ensure((size_t)run_off[pkt_total] * sizeof(lwb_vq_run) + 16) || !ar.vqent.ensure((size_t)ent_off[pkt_total] * 2 + 16))
-            return LWB_ERR_BUFFER;
+        for (size_t g : *used) {
+            BatchArena &ar = b->groups[g]->arena[set];
+            uint64_t *run_off = (uint64_t *)ar.vqroff.p, *ent_off = (uint64_t *)ar.vqeoff.p;
+            run_off[0] = ent_off[0] = 0;
+            for (size_t j : members[g])
+                for (uint32_t k = 0; k < plan[j].usable; k++) {
+                    const uint64_t pi = plan[j].pkt0 + k;
+                    const bool ok = k < decoded[j];
+                    run_off[pi + 1] = run_off[pi] + (ok ? run_off[pi + 1] : 0);
+                    ent_off[pi + 1] = ent_off[pi] + (ok ? ent_off[pi + 1] : 0);
+                }
+            if (!ar.vqrun.ensure((size_t)run_off[pkt_total[g]] * sizeof(lwb_vq_run) + 16) || !ar.vqent.ensure((size_t)ent_off[pkt_total[g]] * 2 + 16))
+                return LWB_ERR_BUFFER;
+        }
         // ~3 KB per stereo long packet: copied by the pool as well (one thread alone would take about as long over it as
         // the whole pool over the entropy decode)
-        std::atomic<size_t> next_copy(j0);
+        std::atomic<size_t> next_copy(0);
         auto copier = [&]() {
             for (;;) {
-                const size_t j = next_copy.fetch_add(1);
-                if (j >= j1) return;
-                const std::vector<lwb_vq_run> &jr = job_runs[j - j0];
-                const std::vector<uint16_t> &je = job_ents[j - j0];
-                if (!jr.empty()) std::memcpy((lwb_vq_run *)ar.vqrun.p + run_off[plan[j].pkt0], jr.data(), jr.size() * sizeof(lwb_vq_run));
-                if (!je.empty()) std::memcpy((uint16_t *)ar.vqent.p + ent_off[plan[j].pkt0], je.data(), je.size() * sizeof(uint16_t));
+                const size_t i = next_copy.fetch_add(1);
+                if (i >= n) return;
+                const JobPlan &p = plan[list[i]];
+                BatchArena &ar = b->groups[b->sets[p.set].group]->arena[set];
+                const std::vector<lwb_vq_run> &jr = ar.job_runs[p.slot];
+                const std::vector<uint16_t> &je = ar.job_ents[p.slot];
+                if (!jr.empty()) std::memcpy((lwb_vq_run *)ar.vqrun.p + ((uint64_t *)ar.vqroff.p)[p.pkt0], jr.data(), jr.size() * sizeof(lwb_vq_run));
+                if (!je.empty()) std::memcpy((uint16_t *)ar.vqent.p + ((uint64_t *)ar.vqeoff.p)[p.pkt0], je.data(), je.size() * sizeof(uint16_t));
             }
         };
         std::vector<std::thread> cpool;
@@ -2147,29 +2196,35 @@ int batch_entropy(lwf_batcher *b, BatchArena &ar, lwf_stream_job *jobs, size_t j
         copier();
         for (auto &t : cpool) t.join();
     }
-    // what crosses to the device: residues or VQ records, dense floor-0 curves, floor kinds and floor1_y rows
-    ar.in_bytes = rows + rows * LWB_MAX_POSTS * 4 + (b->has_floor0 ? coeff_total * 4 : 0) +
-                  (vq ? (pkt_total + 1) * 16 + run_off[pkt_total] * sizeof(lwb_vq_run) + ent_off[pkt_total] * 2 : coeff_total * 4);
-    ar.coeff_total = coeff_total;
-    // chains of this slice
-    ar.chains.assign(j1 - j0, lwb_chain());
-    for (size_t j = j0; j < j1; j++) {
-        lwb_chain &c = ar.chains[j - j0];
-        std::memset(&c, 0, sizeof(c));
-        c.stream = jobs[j].stream;
-        c.n_packets = decoded[j];
-        c.mode_numbers = ar.modes.data() + plan[j].pkt0;
-        c.prev_window_flags = ar.prevs.data() + plan[j].pkt0;
-        c.next_window_flags = ar.nexts.data() + plan[j].pkt0;
-        c.coeff_offset = plan[j].coeff0;
-        c.packet_index = plan[j].pkt0;
-        c.out_offset = jobs[j].out_offset;
-        c.out_stride = jobs[j].out_stride;
+    for (size_t g : *used) {
+        BatchArena &ar = b->groups[g]->arena[set];
+        const uint64_t rows = pkt_total[g] * b->groups[g]->channels, pk = pkt_total[g];
+        // what crosses to the device: residues or VQ records, dense floor-0 curves, floor kinds and floor1_y rows
+        ar.in_bytes = rows + rows * LWB_MAX_POSTS * 4 + (b->groups[g]->has_floor0 ? coeff_total[g] * 4 : 0) +
+                      (vq ? (pk + 1) * 16 + ((uint64_t *)ar.vqroff.p)[pk] * sizeof(lwb_vq_run) + ((uint64_t *)ar.vqeoff.p)[pk] * 2 : coeff_total[g] * 4);
+        ar.coeff_total = coeff_total[g];
+        // the group's chains
+        ar.job = members[g];
+        ar.chains.assign(members[g].size(), lwb_chain());
+        for (size_t s = 0; s < members[g].size(); s++) {
+            const size_t j = members[g][s];
+            lwb_chain &c = ar.chains[s];
+            std::memset(&c, 0, sizeof(c));
+            c.stream = jobs[j].stream;
+            c.n_packets = decoded[j];
+            c.mode_numbers = ar.modes.data() + plan[j].pkt0;
+            c.prev_window_flags = ar.prevs.data() + plan[j].pkt0;
+            c.next_window_flags = ar.nexts.data() + plan[j].pkt0;
+            c.coeff_offset = plan[j].coeff0;
+            c.packet_index = plan[j].pkt0;
+            c.out_offset = jobs[j].out_offset;
+            c.out_stride = jobs[j].out_stride;
+        }
     }
     return LWB_OK;
 }
 
-lwb_batch_io batch_io(const lwf_batcher *b, const BatchArena &ar, int out_format, void *pcm)
+lwb_batch_io batch_io(const lwf_batcher *b, size_t g, const BatchArena &ar, int out_format, void *pcm)
 {
     lwb_batch_io io;
     std::memset(&io, 0, sizeof(io));
@@ -2180,7 +2235,7 @@ lwb_batch_io batch_io(const lwf_batcher *b, const BatchArena &ar, int out_format
     io.vq_run_offsets = (const uint64_t *)ar.vqroff.p;
     io.vq_entries = (const uint16_t *)ar.vqent.p;
     io.vq_entry_offsets = (const uint64_t *)ar.vqeoff.p;
-    io.dense_floor = b->has_floor0 ? (const float *)ar.dense.p : nullptr;
+    io.dense_floor = b->groups[g]->has_floor0 ? (const float *)ar.dense.p : nullptr;
     io.floor_kind = (const uint8_t *)ar.kinds.p;
     io.floor1_y = (const uint32_t *)ar.ys.p;
     io.out_format = out_format;
@@ -2190,11 +2245,12 @@ lwb_batch_io batch_io(const lwf_batcher *b, const BatchArena &ar, int out_format
 
 // The synthesis's results, and where it ran every packet the entropy decode passed, the entropy or header error that
 // stopped the stream there.
-void job_results(lwf_stream_job *jobs, size_t j0, size_t j1, const BatchArena &ar, const std::vector<JobPlan> &plan,
-                 const std::vector<uint32_t> &decoded, const std::vector<int32_t> &dec_status)
+void job_results(lwf_stream_job *jobs, const BatchArena &ar, const std::vector<JobPlan> &plan, const std::vector<uint32_t> &decoded,
+                 const std::vector<int32_t> &dec_status)
 {
-    for (size_t j = j0; j < j1; j++) {
-        const lwb_chain &c = ar.chains[j - j0];
+    for (size_t s = 0; s < ar.chains.size(); s++) {
+        const lwb_chain &c = ar.chains[s];
+        const size_t j = ar.job[s];
         jobs[j].n_samples = c.n_samples;
         jobs[j].packets_done = c.packets_done;
         jobs[j].status = c.status;
@@ -2220,32 +2276,45 @@ extern "C" int lwf_batcher_decode(lwf_batcher *b, lwf_stream_job *jobs, size_t n
         std::vector<JobPlan> plan(n_jobs);
         std::vector<uint32_t> decoded(n_jobs, 0);
         std::vector<int32_t> dec_status(n_jobs, LWB_OK);
+        assign_sets(b, jobs, n_jobs, plan);
         // Slices of streams: while the GPU call of slice i runs (on one helper thread -- an lwb_ctx takes
-        // one caller at a time), the pool already entropy-decodes slice i + 1 into the other arena.
-        const size_t n_slices = std::max<size_t>(1, std::min<size_t>(4, n_jobs / 8));
+        // one caller at a time), the pool already entropy-decodes slice i + 1 into the other arena.  A slice holds the
+        // jobs of one group (one batch); each group is cut into up to four slices, and the slices of all groups follow
+        // each other through the pipeline.
+        std::vector<std::vector<size_t>> members(b->groups.size());
+        for (size_t j = 0; j < n_jobs; j++) members[b->sets[plan[j].set].group].push_back(j);
+        std::vector<std::vector<size_t>> slices;
+        for (size_t g = 0; g < members.size(); g++) {
+            const size_t m = members[g].size();
+            if (!m && (g || n_jobs)) continue;        // no jobs at all: one empty batch, as for any other job count
+            const size_t n_slices = std::max<size_t>(1, std::min<size_t>(4, m / 8));
+            for (size_t sl = 0; sl < n_slices; sl++)
+                slices.emplace_back(members[g].begin() + m * sl / n_slices, members[g].begin() + m * (sl + 1) / n_slices);
+        }
         double entropy_busy = 0, synth_busy = 0;
         uint64_t in_bytes = 0;
         int synth_rc = LWB_OK;
+        std::vector<size_t> used;
         std::thread synth;
         struct Joiner { std::thread &t; ~Joiner() { if (t.joinable()) t.join(); } } joiner{synth};   // also on unwinding
-        for (size_t sl = 0; sl < n_slices && rc == LWB_OK; sl++) {
-            const size_t j0 = n_jobs * sl / n_slices, j1 = n_jobs * (sl + 1) / n_slices;
-            // arena[sl & 1] was last read by the synthesis of slice sl - 2, which finished before that of
-            // slice sl - 1 was started
-            BatchArena &ar = b->arena[sl & 1];
+        for (size_t sl = 0; sl < slices.size() && rc == LWB_OK; sl++) {
+            // arena set sl & 1 of the slice's group was last read by the synthesis of slice sl - 2 or earlier, which
+            // finished before that of slice sl - 1 was started
             const double e0 = now_s();
-            rc = batch_entropy(b, ar, jobs, j0, j1, plan, decoded, dec_status);
+            rc = batch_entropy(b, sl & 1, jobs, slices[sl].data(), slices[sl].size(), plan, decoded, dec_status, &used);
             entropy_busy += now_s() - e0;
-            in_bytes += ar.in_bytes;
             if (synth.joinable()) synth.join();
             if (rc != LWB_OK || synth_rc != LWB_OK) break;
-            synth = std::thread([b, &ar, out_format, pcm, jobs, j0, j1, &plan, &decoded, &dec_status, &synth_rc, &synth_busy]() {
+            const size_t g = used[0];
+            BatchArena &ar = b->groups[g]->arena[sl & 1];
+            in_bytes += ar.in_bytes;
+            synth = std::thread([b, g, &ar, out_format, pcm, jobs, &plan, &decoded, &dec_status, &synth_rc, &synth_busy]() {
                 const double s0 = now_s();
-                const lwb_batch_io io = batch_io(b, ar, out_format, pcm);
+                const lwb_batch_io io = batch_io(b, g, ar, out_format, pcm);
                 const int r = lwb_decode_chains(b->ctx, ar.chains.data(), ar.chains.size(), &io);
                 synth_busy += now_s() - s0;
                 if (r) { synth_rc = r; return; }
-                job_results(jobs, j0, j1, ar, plan, decoded, dec_status);
+                job_results(jobs, ar, plan, decoded, dec_status);
             });
         }
         if (synth.joinable()) synth.join();

@@ -29,6 +29,7 @@
 #include "lwb_common.h"
 #include "pcm_copy_plan.h"
 #include "../../include/lewton_frontend.h"
+#include "batcher.h"
 
 namespace lwb {
 int generate_tables(int bs, float *a, float *b, float *c, float *window, uint32_t *bitrev);
@@ -634,10 +635,10 @@ static size_t first_batch_path()
     return std::strcmp(fg, "1") == 0 ? kNumBatchPaths : kNumBatchPaths - 1;
 }
 
-// Checks, plans and queues one batch; a host-memory batch that queues work issues its ticket (BatchArenas::finish).
-static int queue_batch(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, lwb_plan *prepared)
+// The argument checks of a batch and what every path relies on: valid chains, each stream in one chain, and the residue
+// entries' floor kinds and single channel count.  Shared by queue_batch and lwfb::check_submit.
+static int check_batch_args(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io)
 {
-    if (!ctx || (!chains && n_chains) || !io) return LWB_ERR_INVALID;
     if (io->entry != LWB_ENTRY_SPECTRUM && io->entry != LWB_ENTRY_RESIDUE && io->entry != LWB_ENTRY_VQ) return fail(ctx, LWB_ERR_INVALID, "bad entry");
     if (io->memory != LWB_MEM_HOST && io->memory != LWB_MEM_DEVICE) return fail(ctx, LWB_ERR_INVALID, "bad memory space");
     if (!out_format_known(io->out_format)) return fail(ctx, LWB_ERR_INVALID, "bad out_format");
@@ -645,13 +646,10 @@ static int queue_batch(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const l
     if ((!io->coeffs && io->entry != LWB_ENTRY_VQ) || !io->pcm) return fail(ctx, LWB_ERR_INVALID, "null arena");
     if (io->entry == LWB_ENTRY_VQ && (!io->vq_runs || !io->vq_run_offsets || !io->vq_entries || !io->vq_entry_offsets || !io->floor_kind))
         return fail(ctx, LWB_ERR_INVALID, "VQ entry needs vq_runs, vq_entries, their offsets and floor_kind");
-    CU(ctx, cudaSetDevice(ctx->device));
-    // what every path relies on: valid chains, each stream in one chain, and the residue entries' floor kinds and
-    // single channel count
     const uint64_t epoch = ++ctx->epoch;      // per context: concurrent calls on different contexts share nothing
     const unsigned C = chains[0].stream ? chains[0].stream->setup->channels : 0;
     for (size_t i = 0; i < n_chains; i++) {
-        lwb_chain *c = &chains[i];
+        const lwb_chain *c = &chains[i];
         if (!c->stream || c->stream->ctx != ctx || (c->n_packets && !c->mode_numbers))
             return fail(ctx, LWB_ERR_INVALID, "chain: bad stream or mode list");
         if (c->stream->busy_epoch == epoch) return fail(ctx, LWB_ERR_INVALID, "a stream appears in two chains of one batch");
@@ -661,16 +659,28 @@ static int queue_batch(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const l
             if (!io->floor_kind) return fail(ctx, LWB_ERR_INVALID, "residue entry needs floor_kind");
         }
     }
+    return LWB_OK;
+}
+
+// Checks, plans and queues one batch; a host-memory batch that queues work issues its ticket (BatchArenas::finish).
+// Every argument refusal of a batch must be one lwfb::check_submit also makes without queuing anything: the stream
+// batcher relies on it to refuse a submit of several batches before it queues the first.  A new refusal goes into
+// check_batch_args, or, if a path makes it while it walks the chains, into check_submit as well.
+static int queue_batch(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, lwb_plan *prepared)
+{
+    if (!ctx || (!chains && n_chains) || !io) return LWB_ERR_INVALID;
+    int rc = check_batch_args(ctx, chains, n_chains, io);
+    if (rc || n_chains == 0) return rc;
+    CU(ctx, cudaSetDevice(ctx->device));
+    const unsigned C = chains[0].stream->setup->channels;
     if (prepared) prepared->captured = false; // the path that takes the batch captures it anew, if it can
     for (size_t k = first_batch_path(); k < kNumBatchPaths; k++) {
         bool handled = false;
-        const int rc = kBatchPaths[k](ctx, chains, n_chains, io, &handled, prepared);
-        if (rc || handled) return rc;
+        if ((rc = kBatchPaths[k](ctx, chains, n_chains, io, &handled, prepared)) || handled) return rc;
     }
     std::vector<PlanChain> plan(n_chains);
     std::vector<ChainWalk> walks(n_chains);
     BatchExtent ext;
-    int rc;
     for (size_t i = 0; i < n_chains; i++) {
         lwb_chain *c = &chains[i];
         PlanChain &pc = plan[i];
@@ -754,6 +764,32 @@ extern "C" int lwb_ticket_wait(lwb_ctx *ctx, uint64_t ticket)
     CU(ctx, cudaSetDevice(ctx->device));
     return retire_tickets(ctx, ticket, true);
 }
+
+// ---------------------------------------------------------------------------------------------
+// what the stream batcher (batcher.h) needs of setups and streams
+// ---------------------------------------------------------------------------------------------
+namespace lwfb {
+SetupShape setup_shape(const lwb_setup *su) { return SetupShape{su->ctx, su->channels, su->bs0, su->bs1}; }
+
+const lwb_setup *stream_setup(const lwb_stream *s) { return s->setup; }
+
+// queue_batch's argument checks (check_batch_args), then what the paths refuse while they walk the chains: the extent
+// checks of BatchExtent (out_stride, floor kinds, a missing dense arena) and, for host memory, the page-locked check of
+// BatchArenas::open -- on the chain walks alone, queuing nothing.
+int check_submit(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io)
+{
+    int rc = check_batch_args(ctx, chains, n_chains, io);
+    if (rc || n_chains == 0) return rc;
+    const unsigned C = chains[0].stream->setup->channels;
+    BatchExtent ext;
+    for (size_t i = 0; i < n_chains; i++) {
+        const ChainWalk w = walk_chain(&chains[i], [](uint32_t, const Geom &, bool, uint32_t, uint64_t, uint64_t) {});
+        if ((rc = ext.add(ctx, io, &chains[i], w.done, w.coeff_end, w.n_samples))) return rc;
+    }
+    if ((rc = ext.finish(ctx, io))) return rc;
+    return io->memory == LWB_MEM_HOST && !ext.empty() ? check_page_locked(ctx, io, ext, C) : LWB_OK;
+}
+}  // namespace lwfb
 
 // ---------------------------------------------------------------------------------------------
 // prepared batches

@@ -24,7 +24,7 @@ SYMBOLS = ["lwf_headers_parse", "lwf_headers_destroy", "lwf_headers_info", "lwf_
            "lwf_reader_open", "lwf_reader_close", "lwf_reader_headers", "lwf_reader_read_dec_packet", "lwf_reader_last_absgp",
            "lwf_reader_skip_samples_linear", "lwf_reader_seek_absgp_pg",
            "lwf_batcher_create", "lwf_batcher_destroy", "lwf_batcher_set_entry", "lwf_batcher_decode", "lwf_batcher_last_timing",
-           "lwf_batcher_last_input_bytes", "lwf_batcher_set_floor0", "lwf_batcher_submit",
+           "lwf_batcher_last_input_bytes", "lwf_batcher_set_floor0", "lwf_batcher_submit", "lwf_batcher_add_headers",
            "lwf_debug_float32_unpack", "lwf_debug_lookup1_values", "lwf_debug_ilog", "lwf_debug_read_bits", "lwf_debug_huffman",
            "lwf_debug_decode_loop"]
 
@@ -113,6 +113,7 @@ def lib():
         L.lwf_batcher_destroy.argtypes = [vp]
         L.lwf_batcher_destroy.restype = None
         L.lwf_batcher_set_entry.argtypes = [vp, C.c_int]
+        L.lwf_batcher_add_headers.argtypes = [vp, vp, vp]
         L.lwf_headers_vq_capable.argtypes = [vp]
         L.lwf_packet_decode_vq.argtypes = [vp, C.c_char_p, sz, vp, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz)]
         L.lwf_packet_decode_vq_ex.argtypes = [vp, C.c_char_p, sz, vp, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz), C.c_int]
@@ -448,9 +449,10 @@ def _record(row):
 
 
 class StreamBatcher:
-    """lwf_batcher: entropy-decode the packets of many streams (one shared set of headers) on a host
-    thread pool and synthesise them with one batched call.  jobs: list of (PreviousWindowRight,
-    [packet bytes, ...]); PCM lands planar in `pcm` at out_offset = job index * channels * stride."""
+    """lwf_batcher: entropy-decode the packets of many streams on a host thread pool and synthesise them with one
+    batched call per group of header sets (one group unless add_headers registered more).  jobs: list of
+    (PreviousWindowRight, [packet bytes, ...]); job j's PCM lands in `pcm` behind the jobs before it, each taking its
+    stream's channels * stride elements (out_offset = job index * channels * stride for one set of headers)."""
 
     def __init__(self, ctx, headers, threads=0, entry=cabi.ENTRY_RESIDUE, floor0=False):
         """floor0: type-0 floors travel as floor-0 records (lwf_batcher_set_floor0); the jobs' streams must then come from
@@ -459,6 +461,7 @@ class StreamBatcher:
         h = C.c_void_p()
         ctx.check(lib().lwf_batcher_create(ctx._h, headers._h, threads, C.byref(h)))
         self._h = h.value
+        self._sets = []
         ctx._children.add(self)
         if floor0:
             ctx.check(lib().lwf_batcher_set_floor0(self._h, 1))
@@ -467,12 +470,18 @@ class StreamBatcher:
             if rc:
                 raise AudioReadError(rc, "this stream does not qualify for LWB_ENTRY_VQ (lwf_headers_vq_capable)")
 
+    def add_headers(self, headers, setup):
+        """lwf_batcher_add_headers: the jobs of streams opened on `setup` (an api.Setup made from `headers`) are decoded
+        with `headers`; both are kept alive with the batcher."""
+        self.ctx.check(lib().lwf_batcher_add_headers(self._h, headers._h, setup._h))
+        self._sets.append((headers, setup))
+
     def _jobs(self, jobs, stride):
         """The lwf_stream_job array of `jobs`, and the packet arrays it points to."""
         n = len(jobs)
         arr = (_StreamJob * n)()
         keep = []
-        Cn = self.headers.audio_channels
+        off = 0
         for j, (pwr, packets) in enumerate(jobs):
             pk = (C.c_char_p * len(packets))(*packets)
             ln = (C.c_size_t * len(packets))(*[len(p) for p in packets])
@@ -481,8 +490,9 @@ class StreamBatcher:
             arr[j].n_packets = len(packets)
             arr[j].packets = pk
             arr[j].lengths = ln
-            arr[j].out_offset = j * Cn * stride
+            arr[j].out_offset = off
             arr[j].out_stride = stride
+            off += pwr.setup.audio_channels * stride
         return arr, keep, n
 
     def _counters(self):
