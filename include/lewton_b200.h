@@ -190,6 +190,24 @@ typedef struct lwb_floor0_desc {     /* header::FloorTypeZero, header.rs:399-407
  * Call it before the setup's first batch.  LWB_ERR_INVALID for a bad index, a floor of type 1 or a field out of range. */
 int lwb_setup_set_floor0(lwb_setup *setup, uint32_t floor_index, const lwb_floor0_desc *desc);
 
+/* Output channel mix (added under ABI 3: no struct above changes).  Every chain of a stream opened on the setup then
+ * writes K = n_out output channels instead of the stream's C = audio_channels (Vorbis I section 4.3.9 order):
+ * reordering (e.g. to the WAV / WAVEFORMATEXTENSIBLE order), selection, mono / stereo downmix and duplication.
+ *   matrix: [n_out][C] row-major f32, 1 <= n_out <= 8; n_out == 0 with matrix == NULL clears the mix.
+ *   Refused with LWB_ERR_INVALID, nothing changed: a NULL setup, n_out out of range, a non-finite coefficient, a call
+ *   after any stream has been opened on the setup.
+ * Value, bit for bit and without FMA: with x_c[t] the f32 sample the F32 formats write without a mix, y_k[t] is the
+ * left-to-right f32 sum, over ascending c with M[k][c] != 0, of the rounded products M[k][c] * x_c[t] (the first term
+ * is not added to a zero; a row without a nonzero coefficient gives +0.0f); y is then converted like any f32 sample.
+ * A row with a single 1.0f copies its channel exactly, so permutations and selections are bit-exact.
+ * Layout: planar, n_samples per plane at out_offset + k * out_stride; interleaved, n_samples * K elements at out_offset;
+ * lwb_decode_packet / lwb_decode_spectrum write [K][capacity] or [capacity][K].  Nothing else changes: n_samples,
+ * packets_done, status and the stream state (still C channels) are what the same batch gives without a mix.  Setups with
+ * and without a mix may share a batch; such a batch runs on the chain kernel or the four-kernel path. */
+int lwb_setup_set_output_mix(lwb_setup *setup, uint32_t n_out, const float *matrix);
+/* K: n_out of the setup's mix, or audio_channels without one (0 for a NULL setup) */
+uint32_t lwb_setup_output_channels(const lwb_setup *setup);
+
 /* ---- stream state: PreviousWindowRight, audio.rs:847-861 ---------------------------------- */
 int lwb_stream_open(lwb_ctx *ctx, const lwb_setup *setup, lwb_stream **out);
 void lwb_stream_destroy(lwb_stream *s);
@@ -245,7 +263,7 @@ typedef struct lwb_packet {
 } lwb_packet;
 
 /* Synchronous convenience = submit + flush + fetch.  out: planar [channels][capacity] or
- * interleaved [capacity][channels]; *n_samples = samples per channel written (0 for the first
+ * interleaved [capacity][channels] (channels: lwb_setup_output_channels); *n_samples = samples per channel written (0 for the first
  * packet after a reset).  Host buffers. */
 int lwb_decode_packet(lwb_stream *s, const lwb_packet *pkt, int out_format, void *out,
                       size_t capacity_per_channel, size_t *n_samples);
@@ -291,7 +309,8 @@ enum { LWB_MEM_HOST = 0, LWB_MEM_DEVICE = 1 };
 /* One stream's run of consecutive packets.  Input arenas are chain-major: the chain's packets
  * follow each other, each packet as [channels][n/2 of that packet].
  * Output: a chain writes exactly n_samples elements per channel plane at out_offset + c * out_stride
- * (planar), or n_samples * channels elements at out_offset (interleaved), and nothing else in `pcm`,
+ * (planar), or n_samples * channels elements at out_offset (interleaved), and nothing else in `pcm`
+ * (channels: lwb_setup_output_channels of the stream's setup),
  * in either memory space: the gaps between planes and between chains keep what the caller put there.
  * Any element offsets and any pointer alignment are accepted.  The fused kernels take device-memory
  * batches whose coeffs / dense_floor / pcm are 16-byte aligned and whose coeff_offset, out_offset and

@@ -114,6 +114,8 @@ SYMBOLS = {
     "lwb_setup_create": (C.c_int, [vp, C.POINTER(SetupDesc), C.POINTER(vp)]),
     "lwb_setup_destroy": (None, [vp]),
     "lwb_setup_set_floor0": (C.c_int, [vp, C.c_uint32, C.POINTER(Floor0Desc)]),
+    "lwb_setup_set_output_mix": (C.c_int, [vp, C.c_uint32, fp]),
+    "lwb_setup_output_channels": (C.c_uint32, [vp]),
     "lwb_stream_open": (C.c_int, [vp, vp, C.POINTER(vp)]),
     "lwb_stream_destroy": (None, [vp]),
     "lwb_stream_reset": (C.c_int, [vp]),

@@ -233,6 +233,24 @@ class Setup:
                 d.bark_cos_omega[i] = _ptr(keep[-1], cabi.fp)
         self.ctx.check(cabi.lib().lwb_setup_set_floor0(self._h, floor_index, C.byref(d)))
 
+    def set_output_mix(self, matrix):
+        """lwb_setup_set_output_mix: chains of this setup's streams write K = len(matrix) output channels, output k the
+        f32 sum over input channels c (ascending, zero coefficients skipped) of matrix[k][c] * sample_c; None clears the
+        mix.  matrix: [K][audio_channels], 1 <= K <= 8 (mix_mono, mix_select, mix_wav_order build the common ones).  Only
+        before the setup's first stream is opened."""
+        if matrix is None:
+            self.ctx.check(cabi.lib().lwb_setup_set_output_mix(self._h, 0, None))
+            return
+        m = np.ascontiguousarray(matrix, np.float32)
+        if m.ndim != 2 or m.shape[1] != self.audio_channels:
+            raise ValueError(f"matrix: [K][{self.audio_channels}] expected, got shape {m.shape}")
+        self.ctx.check(cabi.lib().lwb_setup_set_output_mix(self._h, m.shape[0], _ptr(m, cabi.fp)))
+
+    @property
+    def output_channels(self):
+        """K: the channels a chain of this setup writes (lwb_setup_output_channels); audio_channels without a mix."""
+        return cabi.lib().lwb_setup_output_channels(self._h)
+
     @classmethod
     def _adopt(cls, ctx, handle, audio_channels, blocksize_0, blocksize_1, mode_blockflags=()):
         """Wrap an lwb_setup built by the library itself (lwf_headers_make_setup)."""
@@ -383,6 +401,40 @@ def sample_format(sample, interleaved=False):
     return _FORMATS[(sample, bool(interleaved))]
 
 
+def mix_mono(channels):
+    """The output mix (Setup.set_output_mix) of a mono downmix: one row of weights 1/channels (f32)."""
+    return np.full((1, channels), np.float32(1) / np.float32(channels), np.float32)
+
+
+def mix_select(channels, outputs):
+    """The output mix that writes input channels `outputs` (indices, in Vorbis order; repeats duplicate a channel) as the
+    output channels, in that order: bit-exact copies."""
+    m = np.zeros((len(outputs), channels), np.float32)
+    for k, c in enumerate(outputs):
+        if not 0 <= c < channels:
+            raise ValueError(f"channel {c} out of range for {channels} channels")
+        m[k, c] = 1
+    return m
+
+
+# Vorbis I section 4.3.9 channel order -> the WAVEFORMATEXTENSIBLE channel-mask order (FL FR FC LFE BL BR FLC FRC BC SL SR)
+# that WAV files, ALSA and most PCM pipelines use: entry k is the Vorbis channel that becomes output channel k.
+_WAV_ORDER = {1: (0,), 2: (0, 1),
+              3: (0, 2, 1),                     # L C R -> L R C
+              4: (0, 1, 2, 3),                  # FL FR RL RR (already in mask order)
+              5: (0, 2, 1, 3, 4),               # FL C FR RL RR -> FL FR FC BL BR
+              6: (0, 2, 1, 5, 3, 4),            # FL C FR RL RR LFE -> FL FR FC LFE BL BR
+              7: (0, 2, 1, 6, 5, 3, 4),         # FL C FR SL SR RC LFE -> FL FR FC LFE BC SL SR
+              8: (0, 2, 1, 7, 5, 6, 3, 4)}      # FL C FR SL SR RL RR LFE -> FL FR FC LFE BL BR SL SR
+
+
+def mix_wav_order(channels):
+    """The output mix that reorders 1 to 8 channels from Vorbis order to WAV order (a permutation: bit-exact)."""
+    if channels not in _WAV_ORDER:
+        raise ValueError("WAV order is defined for 1 to 8 channels")
+    return mix_select(channels, _WAV_ORDER[channels])
+
+
 def get_decoded_sample_count(setup, mode_number, prev_window_flag=True, next_window_flag=True):
     """audio.rs:874-909 for an already parsed packet header."""
     n = C.c_uint32()
@@ -395,10 +447,11 @@ def get_decoded_sample_count(setup, mode_number, prev_window_flag=True, next_win
 
 def read_audio_packet_generic(setup, packet, pwr, sample="f32", interleaved=False):
     """audio.rs:919-1160 (back half).  Returns planar [channels][len] (Vec<Vec<S>>) or
-    interleaved [len][channels] (InterleavedSamples<S>); len == 0 for the first packet after a reset.
+    interleaved [len][channels] (InterleavedSamples<S>), channels = setup.output_channels; len == 0 for the first packet
+    after a reset.
     Raises AudioReadError (kind 'AudioBadFormat' for the guard at audio.rs:1107-1111)."""
     fmt, dt = sample_format(sample, interleaved)
-    ch = setup.audio_channels
+    ch = setup.output_channels
     cap = setup.blocksize(packet.mode_number)
     kinds, ys, dense = packet.pack()
     p = cabi.Packet()
@@ -426,7 +479,7 @@ def decode_spectrum(setup, mode_number, spectrum, pwr, prev_window_flag=True, ne
                     interleaved=False):
     """Entry at the record_pre_mdct tap (audio.rs:1041): spectrum [channels][n/2] = floor x residue."""
     fmt, dt = sample_format(sample, interleaved)
-    ch = setup.audio_channels
+    ch = setup.output_channels
     cap = setup.blocksize(mode_number)
     sp = np.ascontiguousarray(spectrum, np.float32)
     out = np.zeros((cap, ch) if interleaved else (ch, cap), dt)

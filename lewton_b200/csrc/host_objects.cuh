@@ -89,8 +89,10 @@ struct lwb_setup {
     std::vector<DevMapping> mappings;   // host copy (validation)
     std::vector<uint8_t> floor_types;   // LWB_FLOOR_TYPE_* per floor
     std::vector<DevFloor0> floor0;      // host copy of host.floor0 (empty: no floor-0 description)
-    mutable bool streams_opened = false; // lwb_setup_set_floor0 is refused from then on
+    mutable bool streams_opened = false; // lwb_setup_set_floor0 and lwb_setup_set_output_mix are refused from then on
     bool floor0_described(uint32_t fi) const { return fi < floor0.size() && floor0[fi].order != 0; }
+    // K: the channels a chain of this setup writes (lwb_setup_set_output_mix)
+    unsigned out_channels() const { return host.n_out ? host.n_out : channels; }
 };
 
 struct RowCopy { const float *src; float *dst; uint32_t n4, pad; };  // n4 float4s, copied in front of the round's kernels
@@ -121,6 +123,7 @@ struct StepArgs {
     const uint32_t *ys = nullptr;
     const float *zero = nullptr;                            // k_chain: curves of LWB_FLOOR_ZERO rows, or nullptr
     VqDev vq = {};                                          // k_chain, LWB_ENTRY_VQ: the batch's VQ arrays
+    bool mix = false;                                       // k_chain: a chain's setup has an output mix
 };
 
 // One launch of the residue entry's front stages (k_floor1_segments + k_prologue_fused, or k_prologue): floor x
@@ -390,7 +393,7 @@ static int copy_pcm_to_host(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chai
     ctx->pcm_spans.clear();
     for (size_t i = i0; i < i1; i++) {
         const lwb_chain *c = &chains[i];
-        pcm_chain_spans(planar, c->stream->setup->channels, c->out_offset, c->out_stride, c->n_samples, ctx->pcm_spans);
+        pcm_chain_spans(planar, c->stream->setup->out_channels(), c->out_offset, c->out_stride, c->n_samples, ctx->pcm_spans);
     }
     plan_pcm_copies(ctx->pcm_spans, (uint64_t)INT32_MAX / esz, ctx->pcm_copies);
     for (const PcmCopy &cp : ctx->pcm_copies) {

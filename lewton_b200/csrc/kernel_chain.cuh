@@ -65,7 +65,11 @@ __device__ __forceinline__ float d_x_at(const float *V, const float *__restrict_
 // MULTI = true: `wpc` warps per channel, named barriers.
 // np: blocks a channel group transforms together (spectrum entry, !MULTI; the host sizes shared memory for it).
 // vq: the batch's VQ arrays (VQ entry; `coeffs` is not read then).
-template <int FORMAT, int ENTRY, bool MULTI>
+// MIX: the chain's setup may have an output mix (lwb_setup_set_output_mix).  The channel groups then write their
+// overlap-added samples into a [C][n1max/2] tile -- each group's U half of the block, free once its transform is done --
+// and after a CTA barrier the whole CTA forms the K output channels from it and stores them; a setup without a mix has
+// K = C and copies its channels.  Every group, active or not, reaches the barriers (olen is the same for every channel).
+template <int FORMAT, int ENTRY, bool MULTI, bool MIX = false>
 __global__ void __launch_bounds__(MULTI ? 1024 : 256)
 k_chain(const ChainDesc *__restrict__ chains, const uint8_t *__restrict__ pkt_bytes, const float *__restrict__ coeffs,
         const float *__restrict__ dense_floor, const uint8_t *__restrict__ floor_kind,
@@ -183,7 +187,39 @@ k_chain(const ChainDesc *__restrict__ chains, const uint8_t *__restrict__ pkt_by
             const int slope_sel = pf ? blockflag : 0;
             const int rs = nf ? n2 : (n * 3 - n0) >> 2;
             const int re = nf ? n : (n * 3 + n0) >> 2;
-            if (active) {
+            if constexpr (MIX) {
+                constexpr bool planar = out_format_of(FORMAT).planar;
+                const float *V = U + q * n1max + (n1max >> 1);
+                const float *__restrict__ B = tb.b;
+                const int olen = rs - ls, T = n1max >> 1, K = su.n_out ? su.n_out : C;
+                if (has) {
+                    const float *__restrict__ w = su.tab[slope_sel].window;
+                    for (int t0 = 0; t0 < olen; t0 += T) {
+                        const int tn = min(T, olen - t0);
+                        if (active)
+                            for (int i = lane; i < tn; i += gt) {
+                                const int j = t0 + i;
+                                float v = d_x_at(V, B, n, ls + j);
+                                if (j < plen)                          // audio.rs:1116-1118
+                                    v = __fadd_rn(__fmul_rn(v, __ldg(w + j)), __fmul_rn(prev[j], __ldg(w + plen - 1 - j)));
+                                U[q * n1max + i] = v;
+                            }
+                        __syncthreads();
+                        for (int e = threadIdx.x; e < K * tn; e += blockDim.x) {
+                            const int k = planar ? e / tn : e % K, t = planar ? e % tn : e / K;
+                            auto x = [&](int c) { return ch_smem[(size_t)c * per_warp + q * n1max + t]; };
+                            store_sample<FORMAT>(pcm, cd.out_off, cd.out_stride, K, k, pos + t0 + t, su.n_out ? d_mix_sample(su, k, x) : x(k));
+                        }
+                        __syncthreads();
+                    }
+                }
+                plen = re - rs;                                        // audio.rs:1121
+                if (active) {
+                    for (int i = lane; i < plen; i += gt) prev[i] = d_x_at(V, B, n, rs + i);
+                    gsync();
+                }
+                if (has) pos += olen;
+            } else if (active) {
                 const float *V = U + q * n1max + (n1max >> 1);
                 const float *__restrict__ B = tb.b;
                 const int olen = rs - ls;

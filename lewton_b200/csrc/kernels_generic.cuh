@@ -525,12 +525,47 @@ k_imdct(const DevPacket *__restrict__ pkts, const float *__restrict__ spec, floa
 
 constexpr int kOverlapThreads = 256;
 
-template <int FORMAT>
+// Output channel k of the setup's mix (lwb_setup_set_output_mix) at one sample; x(c) gives input channel c's f32 sample.
+// The rounded products are summed left to right in ascending channel order, the first one not added to a zero; a row
+// without terms gives +0.0f.
+template <class X>
+__device__ __forceinline__ float d_mix_sample(const DevSetup &su, int k, X x)
+{
+    const int a = su.mix_row[k], b = su.mix_row[k + 1];
+    if (a == b) return 0.f;
+    float y = __fmul_rn(__ldg(su.mix_w + a), x(su.mix_ch[a]));
+    for (int j = a + 1; j < b; j++) y = __fadd_rn(y, __fmul_rn(__ldg(su.mix_w + j), x(su.mix_ch[j])));
+    return y;
+}
+
+// MIX: grid.y is the output channel k of the packet's setup (its input channels without a mix); each block recomputes
+// the overlap-add of the input channels row k uses, from x and the previous right half, and stores their mix.
+template <int FORMAT, bool MIX = false>
 __global__ void __launch_bounds__(kOverlapThreads)
 k_overlap(const DevPacket *__restrict__ pkts, const float *__restrict__ x, void *__restrict__ pcm)
 {
     const DevPacket &p = pkts[blockIdx.x];
     const int ch = blockIdx.y;
+    if constexpr (MIX) {
+        const DevSetup &su = *p.setup;
+        const int K = su.n_out ? su.n_out : p.channels;
+        if (ch >= K || p.plen == 0) return;
+        const int n = p.n, plen = p.plen, ls = p.ls, olen = p.rs - p.ls;
+        const float *__restrict__ w = su.tab[p.slope_sel].window;
+        const DevPacket *q = p.prev_packet >= 0 ? &pkts[p.prev_packet] : nullptr;
+        for (int i = threadIdx.x; i < olen; i += kOverlapThreads) {
+            auto ola = [&](int c) {                        // the unmixed path's sample of channel c
+                float v = x[p.x_off + (size_t)c * n + ls + i];
+                if (i < plen) {
+                    const float pv = q ? x[q->x_off + (size_t)c * q->n + p.prev_rs + i] : p.state[(size_t)c * p.state_stride + i];
+                    v = __fadd_rn(__fmul_rn(v, w[i]), __fmul_rn(pv, w[plen - 1 - i]));
+                }
+                return v;
+            };
+            store_sample<FORMAT>(pcm, p.out_off, p.out_stride, K, ch, i, su.n_out ? d_mix_sample(su, ch, ola) : ola(ch));
+        }
+        return;
+    }
     if (ch >= p.channels || p.plen == 0) return;      // audio.rs:1140-1151: no previous -> no output
     const int n = p.n;
     const float *__restrict__ xc = x + p.x_off + (size_t)ch * n;

@@ -11,6 +11,7 @@
 
 #include <algorithm>
 #include <cctype>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -499,6 +500,52 @@ extern "C" int lwb_setup_set_floor0(lwb_setup *su, uint32_t fi, const lwb_floor0
     return LWB_OK;
 }
 
+extern "C" int lwb_setup_set_output_mix(lwb_setup *su, uint32_t n_out, const float *m)
+{
+    if (!su) return LWB_ERR_INVALID;
+    lwb_ctx *ctx = su->ctx;
+    const unsigned C = su->channels;
+    if ((n_out == 0) != (m == nullptr) || n_out > 8) return fail(ctx, LWB_ERR_INVALID, "set_output_mix: n_out must be 1..8 with a matrix, or 0 with none");
+    for (size_t i = 0; i < (size_t)n_out * C; i++)
+        if (!std::isfinite(m[i])) return fail(ctx, LWB_ERR_INVALID, "set_output_mix: a coefficient is not finite");
+    // Streams (and the batches and plans built on them) lay out their PCM by the setup's output channels: fixed from then on.
+    if (su->streams_opened) return fail(ctx, LWB_ERR_INVALID, "set_output_mix: the setup already has streams");
+    CU(ctx, cudaSetDevice(ctx->device));
+    // per output row, its nonzero coefficients in ascending channel order
+    std::vector<uint8_t> ch;
+    std::vector<float> w;
+    DevSetup h = su->host;
+    h.mix_ch = nullptr;
+    h.mix_w = nullptr;
+    std::memset(h.mix_row, 0, sizeof(h.mix_row));
+    h.n_out = (uint8_t)n_out;
+    for (uint32_t k = 0; k < n_out; k++) {
+        for (unsigned c = 0; c < C; c++)
+            if (m[(size_t)k * C + c] != 0.f) {
+                ch.push_back((uint8_t)c);
+                w.push_back(m[(size_t)k * C + c]);
+            }
+        h.mix_row[k + 1] = (uint16_t)ch.size();
+    }
+    for (uint32_t k = n_out; k < 8; k++) h.mix_row[k + 1] = h.mix_row[n_out];
+    int rc;
+    if (n_out && ((rc = upload(su, ch.data(), ch.size(), &h.mix_ch)) || (rc = upload(su, w.data(), w.size(), &h.mix_w)))) return rc;
+    CU(ctx, cudaMemcpyAsync(su->d_setup, &h, sizeof(h), cudaMemcpyHostToDevice, ctx->stream));
+    CU(ctx, cudaStreamSynchronize(ctx->stream));           // (the copies read `ch`, `w` and `h`)
+    // the previous mix's term lists go
+    for (const void *p : {(const void *)su->host.mix_ch, (const void *)su->host.mix_w}) {
+        auto it = std::find(su->allocs.begin(), su->allocs.end(), p);
+        if (p && it != su->allocs.end()) {
+            cudaFree(*it);
+            su->allocs.erase(it);
+        }
+    }
+    su->host = h;
+    return LWB_OK;
+}
+
+extern "C" uint32_t lwb_setup_output_channels(const lwb_setup *su) { return su ? su->out_channels() : 0; }
+
 // The front half's setup with its record-capable type-0 floors described (here, beside lwb_setup_set_floor0: the front
 // half alone builds without the synthesis library).
 extern "C" int lwf_headers_make_setup_floor0(const lwf_headers *h, lwb_ctx *ctx, lwb_setup **out)
@@ -674,7 +721,12 @@ static int queue_batch(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const l
     CU(ctx, cudaSetDevice(ctx->device));
     const unsigned C = chains[0].stream->setup->channels;
     if (prepared) prepared->captured = false; // the path that takes the batch captures it anew, if it can
-    for (size_t k = first_batch_path(); k < kNumBatchPaths; k++) {
+    // An output mix is applied where one CTA holds every channel of a packet (k_chain) or by the four-kernel path: a batch
+    // with a mixed chain skips the fused paths, as interleaved output does.
+    size_t first = first_batch_path();
+    for (size_t i = 0; i < n_chains && first < kNumBatchPaths - 1; i++)
+        if (chains[i].stream->setup->host.n_out) first = kNumBatchPaths - 1;
+    for (size_t k = first; k < kNumBatchPaths; k++) {
         bool handled = false;
         if ((rc = kBatchPaths[k](ctx, chains, n_chains, io, &handled, prepared)) || handled) return rc;
     }

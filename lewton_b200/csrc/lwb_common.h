@@ -99,6 +99,12 @@ struct DevSetup {
     const DevBook *books;
     uint32_t n_books, n_residues;
     uint32_t res_psize[kMaxResidues];  // residue_partition_size
+    // output mix (lwb_setup_set_output_mix); n_out == 0: none.  Output channel k sums the terms
+    // [mix_row[k], mix_row[k + 1]): input channel mix_ch[j] times mix_w[j], in ascending channel order.
+    const uint8_t *mix_ch;
+    const float *mix_w;
+    uint16_t mix_row[9];
+    uint8_t n_out;
 };
 
 // One packet of a batch; every index/geometry decision is made on the host

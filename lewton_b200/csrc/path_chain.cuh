@@ -93,9 +93,11 @@ static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
     unsigned maxc = 1;
     int n1max = 64;
     size_t total_packets = 0;
+    bool mix = false;
     for (size_t i = 0; i < n_chains; i++) {
         const lwb_setup *su = chains[i].stream->setup;
         if (su->channels > 8) return LWB_OK;
+        mix |= su->host.n_out != 0;
         maxc = std::max<unsigned>(maxc, su->channels);
         n1max = std::max(n1max, 1 << su->bs1);
         total_packets += chains[i].n_packets;
@@ -153,6 +155,7 @@ static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         args.ys = ar.fl.ys;
         args.zero = zero;
         args.vq = VqDev{ar.fl.vq.runs, ar.fl.vq.run_off, ar.fl.vq.entries, ar.fl.vq.ent_off};
+        args.mix = mix;
         std::vector<Step> steps(1, Step{LWB_KERNEL_CHAIN, dbuf.p, n_launch, nullptr});
         if ((rc = run_steps(ctx, args, steps))) return rc;
         if (cap) capture(plan, gen_at_entry, FrontStages(), args, std::move(steps));

@@ -315,7 +315,7 @@ struct BatchExtent {
     int add(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chain *c, uint32_t done, uint64_t coeff_end, uint64_t n_samples)
     {
         if (!done) return LWB_OK;
-        const unsigned C = c->stream->setup->channels;
+        const unsigned C = c->stream->setup->out_channels();
         const bool planar = out_format_of(io->out_format).planar;
         if (planar && c->out_stride < n_samples) return fail(ctx, LWB_ERR_BUFFER, "chain: out_stride smaller than the samples produced");
         c_lo = std::min(c_lo, c->coeff_offset);
@@ -576,7 +576,7 @@ static int front_stages_run(lwb_ctx *ctx, const lwb_batch_io *io, const FrontSta
 // ---------------------------------------------------------------------------------------------
 // the launches of the fused paths and the chain-kernel path (Step)
 // ---------------------------------------------------------------------------------------------
-template <int ENTRY>
+template <int ENTRY, bool MIX>
 static int launch_chain(lwb_ctx *ctx, int fmt, unsigned n_chains, unsigned warps, size_t smem, const ChainDesc *d,
                         const uint8_t *bytes, const float *coeffs, const float *dense, const uint8_t *kinds,
                         const uint32_t *ys, void *pcm, int n1max, int wpc, int np, const float *zero, VqDev vq)
@@ -584,14 +584,22 @@ static int launch_chain(lwb_ctx *ctx, int fmt, unsigned n_chains, unsigned warps
     return with_out_format(fmt, [&](auto f) {
         constexpr int F = decltype(f)::value;
         if (wpc == 1) {
-            cudaFuncSetAttribute(k_chain<F, ENTRY, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, false>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense,
+            cudaFuncSetAttribute(k_chain<F, ENTRY, false, MIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, false, MIX>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense,
                           kinds, ys, pcm, n1max, wpc, np, zero, vq);
         }
-        cudaFuncSetAttribute(k_chain<F, ENTRY, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, true>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, kinds,
+        cudaFuncSetAttribute(k_chain<F, ENTRY, true, MIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, true, MIX>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, kinds,
                       ys, pcm, n1max, wpc, 1, zero, vq);
     });
+}
+template <int ENTRY>
+static int launch_chain(lwb_ctx *ctx, bool mix, int fmt, unsigned n_chains, unsigned warps, size_t smem, const ChainDesc *d,
+                        const uint8_t *bytes, const float *coeffs, const float *dense, const uint8_t *kinds,
+                        const uint32_t *ys, void *pcm, int n1max, int wpc, int np, const float *zero, VqDev vq)
+{
+    return mix ? launch_chain<ENTRY, true>(ctx, fmt, n_chains, warps, smem, d, bytes, coeffs, dense, kinds, ys, pcm, n1max, wpc, np, zero, vq)
+               : launch_chain<ENTRY, false>(ctx, fmt, n_chains, warps, smem, d, bytes, coeffs, dense, kinds, ys, pcm, n1max, wpc, np, zero, vq);
 }
 
 __global__ void k_row_copy(const RowCopy *__restrict__ rc);   // path_chain.cuh
@@ -630,13 +638,13 @@ static int run_steps(lwb_ctx *ctx, const StepArgs &a, const std::vector<Step> &s
             break;
         case LWB_KERNEL_CHAIN:
             if (a.entry == LWB_ENTRY_VQ)
-                rc = launch_chain<LWB_ENTRY_VQ>(ctx, a.out_format, n, a.chain.warps, a.chain.smem, (const ChainDesc *)s.desc, a.bytes, a.coeffs,
+                rc = launch_chain<LWB_ENTRY_VQ>(ctx, a.mix, a.out_format, n, a.chain.warps, a.chain.smem, (const ChainDesc *)s.desc, a.bytes, a.coeffs,
                                                 a.dense, a.kinds, a.ys, a.pcm, a.chain.n1max, a.chain.wpc, a.chain.np, a.zero, a.vq);
             else if (a.entry == LWB_ENTRY_RESIDUE)
-                rc = launch_chain<LWB_ENTRY_RESIDUE>(ctx, a.out_format, n, a.chain.warps, a.chain.smem, (const ChainDesc *)s.desc, a.bytes, a.coeffs,
+                rc = launch_chain<LWB_ENTRY_RESIDUE>(ctx, a.mix, a.out_format, n, a.chain.warps, a.chain.smem, (const ChainDesc *)s.desc, a.bytes, a.coeffs,
                                                      a.dense, a.kinds, a.ys, a.pcm, a.chain.n1max, a.chain.wpc, a.chain.np, a.zero, a.vq);
             else
-                rc = launch_chain<LWB_ENTRY_SPECTRUM>(ctx, a.out_format, n, a.chain.warps, a.chain.smem, (const ChainDesc *)s.desc, a.bytes, a.coeffs,
+                rc = launch_chain<LWB_ENTRY_SPECTRUM>(ctx, a.mix, a.out_format, n, a.chain.warps, a.chain.smem, (const ChainDesc *)s.desc, a.bytes, a.coeffs,
                                                       a.dense, a.kinds, a.ys, a.pcm, a.chain.n1max, a.chain.wpc, a.chain.np, a.zero, a.vq);
             break;
         default:
@@ -694,12 +702,17 @@ static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_bat
         CU(ctx, cudaStreamSynchronize(ctx->stream));
         DevPacket *hp = (DevPacket *)ctx->h_desc;
         size_t di = 0, xo = 0;
-        unsigned maxc = 1, maxn = 64;
+        unsigned maxc = 1, maxn = 64, maxk = 1;
+        bool mix = false;
         for (size_t ci = 0; ci < plan.size(); ci++) {
             PlanChain &pc = plan[ci];
             const lwb_stream *s = pc.c->stream;
             const lwb_setup *su = s->setup;
-            const unsigned C = su->channels;
+            const unsigned C = su->channels, K = su->out_channels();
+            if (take[ci]) {
+                maxk = std::max(maxk, K);
+                mix |= su->host.n_out != 0;
+            }
             for (uint32_t k = 0; k < take[ci]; k++) {
                 const PlanPacket &pp = pc.pk[start[ci] + k];
                 DevPacket &d = hp[di];
@@ -709,7 +722,7 @@ static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_bat
                 d.coeff_off = pp.coeff_off - coeff_base;
                 d.x_off = xo;
                 d.out_stride = pc.c->out_stride;
-                d.out_off = pc.c->out_offset - pcm_base + (planar ? pp.sample_pos : pp.sample_pos * C);
+                d.out_off = pc.c->out_offset - pcm_base + (planar ? pp.sample_pos : pp.sample_pos * K);
                 d.pkt_index = pc.c->packet_index + start[ci] + k;
                 d.prev_packet = k ? (int32_t)(di - 1) : -1;
                 d.prev_rs = k ? hp[di - 1].rs : 0;
@@ -748,6 +761,9 @@ static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_bat
             return rc;
         dim3 g2((unsigned)n_desc, maxc), b2(kOverlapThreads);
         rc = with_out_format(io->out_format, [&](auto f) {
+            if (mix)        // grid.y: output channels
+                return launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<decltype(f)::value, true>, dim3((unsigned)n_desc, maxk), b2, 0, dp,
+                              (const float *)ctx->x.p, pcm);
             return launch(ctx, LWB_KERNEL_OVERLAP, k_overlap<decltype(f)::value>, g2, b2, 0, dp, (const float *)ctx->x.p, pcm);
         });
         if (rc) return rc;

@@ -452,7 +452,8 @@ class StreamBatcher:
     """lwf_batcher: entropy-decode the packets of many streams on a host thread pool and synthesise them with one
     batched call per group of header sets (one group unless add_headers registered more).  jobs: list of
     (PreviousWindowRight, [packet bytes, ...]); job j's PCM lands in `pcm` behind the jobs before it, each taking its
-    stream's channels * stride elements (out_offset = job index * channels * stride for one set of headers)."""
+    stream's output channels * stride elements (Setup.output_channels: audio_channels unless the setup has an output mix;
+    out_offset = job index * channels * stride for one set of headers)."""
 
     def __init__(self, ctx, headers, threads=0, entry=cabi.ENTRY_RESIDUE, floor0=False):
         """floor0: type-0 floors travel as floor-0 records (lwf_batcher_set_floor0); the jobs' streams must then come from
@@ -492,7 +493,7 @@ class StreamBatcher:
             arr[j].lengths = ln
             arr[j].out_offset = off
             arr[j].out_stride = stride
-            off += pwr.setup.audio_channels * stride
+            off += pwr.setup.output_channels * stride
         return arr, keep, n
 
     def _counters(self):
