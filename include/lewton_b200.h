@@ -393,10 +393,9 @@ int lwb_decode_chains(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lw
  * A submit still blocks the calling thread in these places, and nowhere else:
  *   - arena growth: a staging arena of a host set grows after that set's previous ticket has completed; the
  *     context's other arenas grow after the compute stream has drained;
- *   - staging-ring wrap: descriptors are written to pinned staging that waits for the copy three stagings back;
- *   - the four-kernel path synchronises once per round before it writes its pinned descriptors.  It takes only batches
- *     of more than 8 channels or with buffers beyond shared memory (LWB_ENTRY_VQ batches included: those of every
- *     other shape run on k_chain or the fused kernels).
+ *   - staging-ring wrap: descriptors are written to pinned staging that waits for the copy three stagings back.  The
+ *     four-kernel path (batches of more than 8 channels or with buffers beyond shared memory) stages once per round of
+ *     its IMDCT scratch, so a batch of more than three rounds waits at its fourth round for its own first copy.
  * lwb_ctx_synchronize, lwb_ctx_destroy and lwb_stream_destroy wait for every queued copy as well as every kernel. */
 int lwb_submit_chains(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, uint64_t *ticket);
 /* *done = 1 once every copy and kernel of `ticket` has finished (a host-memory batch's PCM is in `pcm`), else 0.

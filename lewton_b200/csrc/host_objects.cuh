@@ -11,7 +11,7 @@ struct DevBuf {
     size_t cap = 0;
 };
 
-// pinned staging for one batch's descriptors; `ev` marks the end of the copy that reads it
+// pinned staging for one batch's descriptors (the four-kernel path: one round's); `ev` marks the end of the copy that reads it
 struct Staging {
     void *h = nullptr;
     size_t cap = 0;
@@ -72,9 +72,6 @@ struct lwb_ctx {
     std::deque<cudaEvent_t> ticket_events;
     std::vector<cudaEvent_t> spare_events;
     bool pinned_only = false;      // set while a host-memory lwb_submit_chains queues its batch
-    // pinned staging for descriptors (four-kernel path)
-    void *h_desc = nullptr;
-    size_t h_desc_cap = 0;
     size_t x_cap_elems = (size_t)64 << 20;     // IMDCT scratch per round of the generic path (256 MiB)
 };
 
@@ -418,21 +415,6 @@ static bool fused_layout(const lwb_chain *chains, size_t n_chains, const lwb_bat
     for (size_t i = 0; i < n_chains; i++)
         if ((chains[i].out_offset | chains[i].out_stride | chains[i].coeff_offset) & 3) return false;
     return true;
-}
-
-static int ensure_pinned(lwb_ctx *ctx, size_t bytes)
-{
-    if (bytes <= ctx->h_desc_cap) return LWB_OK;
-    if (ctx->h_desc) {
-        CU(ctx, cudaStreamSynchronize(ctx->stream));
-        cudaFreeHost(ctx->h_desc);
-        ctx->h_desc = nullptr;
-        ctx->h_desc_cap = 0;
-    }
-    size_t want = bytes * 2 + 4096;
-    CU(ctx, cudaHostAlloc(&ctx->h_desc, want, cudaHostAllocDefault));
-    ctx->h_desc_cap = want;
-    return LWB_OK;
 }
 
 // ---------------------------------------------------------------------------------------------

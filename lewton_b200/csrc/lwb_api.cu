@@ -126,7 +126,6 @@ extern "C" void lwb_ctx_destroy(lwb_ctx *ctx)
     for (cudaEvent_t e : ctx->spare_events) cudaEventDestroy(e);
     for (CachedTables &ct : ctx->tables)
         for (void *p : ct.allocs) cudaFree(p);
-    if (ctx->h_desc) cudaFreeHost(ctx->h_desc);
     for (void *h : ctx->stage_old) cudaFreeHost(h);
     for (Staging &st : ctx->stage) {
         if (st.h) cudaFreeHost(st.h);
@@ -668,10 +667,12 @@ extern "C" int lwb_decoded_sample_count(const lwb_setup *su, uint8_t mode, int p
 #include "path_mixed.cuh"
 #include "path_mid.cuh"
 
-// The batch paths in the order they are tried; what none of them takes goes to the four-kernel path (run_generic).
+// The batch paths in the order they are tried.  The last, the four-kernel path, takes every batch that reaches it.
 using BatchPath = int (*)(lwb_ctx *, lwb_chain *, size_t, const lwb_batch_io *, bool *, lwb_plan *);
-static const BatchPath kBatchPaths[] = {try_long, try_mid, try_mixed, try_chain};
-constexpr size_t kNumBatchPaths = sizeof(kBatchPaths) / sizeof(kBatchPaths[0]);
+static constexpr BatchPath kBatchPaths[] = {try_long, try_mid, try_mixed, try_chain, try_generic};
+constexpr size_t kChainPath = 3, kGenericPath = 4;
+static_assert(kBatchPaths[kChainPath] == try_chain && kBatchPaths[kGenericPath] == try_generic && std::size(kBatchPaths) == kGenericPath + 1,
+              "kChainPath / kGenericPath name the chain-kernel and the four-kernel path, the last one");
 
 // Index of the first batch path to try.  LWB_FORCE_GENERIC is a test switch that sends batches to the reference
 // paths: "1" to the four-kernel path only, any other value to the chain kernel and then the four-kernel path.
@@ -679,7 +680,7 @@ static size_t first_batch_path()
 {
     const char *fg = getenv("LWB_FORCE_GENERIC");
     if (!fg) return 0;
-    return std::strcmp(fg, "1") == 0 ? kNumBatchPaths : kNumBatchPaths - 1;
+    return std::strcmp(fg, "1") == 0 ? kGenericPath : kChainPath;
 }
 
 // The argument checks of a batch and what every path relies on: valid chains, each stream in one chain, and the residue
@@ -719,40 +720,17 @@ static int queue_batch(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const l
     int rc = check_batch_args(ctx, chains, n_chains, io);
     if (rc || n_chains == 0) return rc;
     CU(ctx, cudaSetDevice(ctx->device));
-    const unsigned C = chains[0].stream->setup->channels;
     if (prepared) prepared->captured = false; // the path that takes the batch captures it anew, if it can
     // An output mix is applied where one CTA holds every channel of a packet (k_chain) or by the four-kernel path: a batch
     // with a mixed chain skips the fused paths, as interleaved output does.
     size_t first = first_batch_path();
-    for (size_t i = 0; i < n_chains && first < kNumBatchPaths - 1; i++)
-        if (chains[i].stream->setup->host.n_out) first = kNumBatchPaths - 1;
-    for (size_t k = first; k < kNumBatchPaths; k++) {
+    for (size_t i = 0; i < n_chains && first < kChainPath; i++)
+        if (chains[i].stream->setup->host.n_out) first = kChainPath;
+    for (size_t k = first; k < std::size(kBatchPaths); k++) {
         bool handled = false;
         if ((rc = kBatchPaths[k](ctx, chains, n_chains, io, &handled, prepared)) || handled) return rc;
     }
-    std::vector<PlanChain> plan(n_chains);
-    std::vector<ChainWalk> walks(n_chains);
-    BatchExtent ext;
-    for (size_t i = 0; i < n_chains; i++) {
-        lwb_chain *c = &chains[i];
-        PlanChain &pc = plan[i];
-        pc.c = c;
-        pc.pk.reserve(c->n_packets);
-        walks[i] = walk_chain(c, [&](uint32_t, const Geom &g, bool has, uint32_t plen, uint64_t coeff, uint64_t pos) {
-            pc.pk.push_back(PlanPacket{g, has ? plen : 0, coeff, pos});
-        });
-        set_chain_result(c, walks[i]);
-        if ((rc = ext.add(ctx, io, c, walks[i].done, walks[i].coeff_end, walks[i].n_samples))) return rc;
-    }
-    if ((rc = ext.finish(ctx, io))) return rc;
-    if (!ext.empty()) {
-        BatchArenas ar;
-        if ((rc = ar.open(ctx, io, ext, C, false)) || (rc = ar.upload(0, ext)) || (rc = run_generic(ctx, plan, io, ar, ext.need_floor0)) ||
-            (rc = ar.download(0, chains, 0, n_chains, ext)) || (rc = ar.finish()))
-            return rc;
-    }
-    commit_stream_states(chains, walks);
-    return LWB_OK;
+    return fail(ctx, LWB_ERR_INVALID, "internal: no batch path took the batch");
 }
 
 // One batch.  ticket == nullptr: the synchronous entry points, which return once a host-memory batch's PCM has landed
@@ -966,14 +944,14 @@ extern "C" int lwb_debug_packet_taps(lwb_stream *s, const lwb_packet *pkt, float
         need_floor0 |= kd == LWB_FLOOR_ZERO;
     }
     if ((need_dense && !pkt->dense_floor) || (need_y && !pkt->floor1_y)) return LWB_ERR_INVALID;
+    Staging *slot;
     if ((need_floor0 && (rc = ensure(ctx, ctx->floor0, C * n2 * 4))) ||
         (rc = ensure(ctx, ctx->ordered.coeffs, C * n2 * 4)) || (rc = ensure(ctx, ctx->spec, C * n2 * 4)) ||
         (rc = ensure(ctx, ctx->x, C * g.n * 4)) || (rc = ensure(ctx, ctx->ordered.kinds, C)) ||
         (rc = ensure(ctx, ctx->ordered.ys, C * LWB_MAX_POSTS * 4)) || (rc = ensure(ctx, ctx->ordered.dense, C * n2 * 4)) ||
-        (rc = ensure(ctx, ctx->desc, sizeof(DevPacket))) || (rc = ensure_pinned(ctx, sizeof(DevPacket))))
+        (rc = ensure(ctx, ctx->desc, sizeof(DevPacket))) || (rc = acquire_staging(ctx, sizeof(DevPacket), &slot)))
         return rc;
-    CU(ctx, cudaStreamSynchronize(ctx->stream));
-    DevPacket *d = (DevPacket *)ctx->h_desc;
+    DevPacket *d = (DevPacket *)slot->h;
     std::memset(d, 0, sizeof(*d));
     d->setup = su->d_setup;
     d->state = s->d_state;
@@ -984,7 +962,7 @@ extern "C" int lwb_debug_packet_taps(lwb_stream *s, const lwb_packet *pkt, float
     d->blockflag = g.blockflag; d->mapping = g.mapping; d->slope_sel = g.slope_sel;
     d->channels = (uint8_t)C;
     cudaStream_t st = ctx->stream;
-    CU(ctx, cudaMemcpyAsync(ctx->desc.p, d, sizeof(*d), cudaMemcpyHostToDevice, st));
+    if ((rc = upload_staging(ctx, slot, d, ctx->desc.p, sizeof(*d), st))) return rc;
     CU(ctx, cudaMemcpyAsync(ctx->ordered.coeffs.p, pkt->residue, C * n2 * 4, cudaMemcpyHostToDevice, st));
     CU(ctx, cudaMemcpyAsync(ctx->ordered.kinds.p, pkt->floor_kind, C, cudaMemcpyHostToDevice, st));
     if (need_y) CU(ctx, cudaMemcpyAsync(ctx->ordered.ys.p, pkt->floor1_y, C * LWB_MAX_POSTS * 4, cudaMemcpyHostToDevice, st));

@@ -5,18 +5,6 @@
 // ---------------------------------------------------------------------------------------------
 // batch planning
 // ---------------------------------------------------------------------------------------------
-struct PlanPacket {
-    Geom g;
-    uint32_t plen;          // 0: no previous half -> 0 samples out
-    uint64_t coeff_off;     // absolute element offset
-    uint64_t sample_pos;    // samples (per channel) produced by the chain before this packet
-};
-
-struct PlanChain {
-    lwb_chain *c;
-    std::vector<PlanPacket> pk;
-};
-
 // What one chain decodes: the packets up to the first with a bad mode or an overlap the reference refuses, the samples
 // they produce and the stream state they leave (audio.rs:1056-1073, 1083-1154).
 struct ChainWalk {
@@ -90,15 +78,6 @@ static void write_mode_bytes(const lwb_chain *c, uint32_t k, uint8_t *out)
     out[0] = c->mode_numbers[k];
     out[1] = c->prev_window_flags ? c->prev_window_flags[k] : 1;
     out[2] = c->next_window_flags ? c->next_window_flags[k] : 1;
-}
-
-// dynamic shared memory k_prologue needs for the chains of a batch (curve bytes of the largest block)
-static size_t prologue_smem_of(const std::vector<PlanChain> &plan)
-{
-    size_t m = 0;
-    for (const PlanChain &pc : plan)
-        if (pc.c && pc.c->stream) m = std::max(m, prologue_smem(pc.c->stream->setup->channels, pc.c->stream->setup->bs1));
-    return m;
 }
 
 // Every launch of the library goes through launch() or launched(), which count it under its kernel's LWB_KERNEL_* id.
@@ -655,9 +634,34 @@ static int run_steps(lwb_ctx *ctx, const StepArgs &a, const std::vector<Step> &s
     return LWB_OK;
 }
 
-// Generic path: rounds of packets bounded by the IMDCT scratch.  Its descriptors address a host-memory batch's
-// staging from its start (element c_lo / o_lo), a device-memory batch's arenas from element 0.  ext_floor0: the batch may
-// have LWB_FLOOR_ZERO rows (BatchExtent::need_floor0).
+// ---------------------------------------------------------------------------------------------
+// four-kernel path (kernels_generic.cuh): the last batch path, which takes every batch that reaches it
+// ---------------------------------------------------------------------------------------------
+struct PlanPacket {
+    Geom g;
+    uint32_t plen;          // 0: no previous half -> 0 samples out
+    uint64_t coeff_off;     // absolute element offset
+    uint64_t sample_pos;    // samples (per channel) produced by the chain before this packet
+};
+
+struct PlanChain {
+    lwb_chain *c;
+    std::vector<PlanPacket> pk;
+};
+
+// dynamic shared memory k_prologue needs for the chains of a batch (curve bytes of the largest block)
+static size_t prologue_smem_of(const std::vector<PlanChain> &plan)
+{
+    size_t m = 0;
+    for (const PlanChain &pc : plan)
+        if (pc.c && pc.c->stream) m = std::max(m, prologue_smem(pc.c->stream->setup->channels, pc.c->stream->setup->bs1));
+    return m;
+}
+
+// Rounds of packets bounded by the IMDCT scratch.  Each round stages its descriptors in the next slot of the staging
+// ring; ctx->desc, ctx->x and ctx->spec are reused from round to round in compute-stream order.  The descriptors
+// address a host-memory batch's staging from its start (element c_lo / o_lo), a device-memory batch's arenas from
+// element 0.  ext_floor0: the batch may have LWB_FLOOR_ZERO rows (BatchExtent::need_floor0).
 static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_batch_io *io, const BatchArenas &ar, bool ext_floor0)
 {
     size_t maxp = 0;
@@ -695,12 +699,11 @@ static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_bat
         }
         if (!any) break;
         int rc;
-        if ((rc = ensure_pinned(ctx, n_desc * sizeof(DevPacket)))) return rc;
-        if ((rc = ensure(ctx, ctx->desc, n_desc * sizeof(DevPacket)))) return rc;
-        if ((rc = ensure(ctx, ctx->x, x_elems * sizeof(float)))) return rc;
-        // the pinned descriptor staging is reused every round: wait for the previous upload
-        CU(ctx, cudaStreamSynchronize(ctx->stream));
-        DevPacket *hp = (DevPacket *)ctx->h_desc;
+        Staging *st;
+        if ((rc = acquire_staging(ctx, n_desc * sizeof(DevPacket), &st)) || (rc = ensure(ctx, ctx->desc, n_desc * sizeof(DevPacket))) ||
+            (rc = ensure(ctx, ctx->x, x_elems * sizeof(float))))
+            return rc;
+        DevPacket *hp = (DevPacket *)st->h;
         size_t di = 0, xo = 0;
         unsigned maxc = 1, maxn = 64, maxk = 1;
         bool mix = false;
@@ -746,7 +749,7 @@ static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_bat
             }
             start[ci] += take[ci];
         }
-        CU(ctx, cudaMemcpyAsync(ctx->desc.p, hp, n_desc * sizeof(DevPacket), cudaMemcpyHostToDevice, ctx->stream));
+        if ((rc = upload_staging(ctx, st, hp, ctx->desc.p, n_desc * sizeof(DevPacket), ctx->stream))) return rc;
         const DevPacket *dp = (const DevPacket *)ctx->desc.p;
         const float *spec = coeffs;
         if (io->entry != LWB_ENTRY_SPECTRUM) {
@@ -769,6 +772,37 @@ static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_bat
         if (rc) return rc;
         if ((rc = launch(ctx, LWB_KERNEL_SAVE_STATE, k_save_state, g2, b2, 0, dp, (const float *)ctx->x.p))) return rc;
     }
+    return LWB_OK;
+}
+
+// Any batch: not captured by a prepared batch, which plans it again on every execution.
+static int try_generic(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, bool *handled, lwb_plan *)
+{
+    *handled = true;
+    const unsigned C = chains[0].stream->setup->channels;
+    std::vector<PlanChain> plan(n_chains);
+    std::vector<ChainWalk> walks(n_chains);
+    BatchExtent ext;
+    int rc;
+    for (size_t i = 0; i < n_chains; i++) {
+        lwb_chain *c = &chains[i];
+        PlanChain &pc = plan[i];
+        pc.c = c;
+        pc.pk.reserve(c->n_packets);
+        walks[i] = walk_chain(c, [&](uint32_t, const Geom &g, bool has, uint32_t plen, uint64_t coeff, uint64_t pos) {
+            pc.pk.push_back(PlanPacket{g, has ? plen : 0, coeff, pos});
+        });
+        set_chain_result(c, walks[i]);
+        if ((rc = ext.add(ctx, io, c, walks[i].done, walks[i].coeff_end, walks[i].n_samples))) return rc;
+    }
+    if ((rc = ext.finish(ctx, io))) return rc;
+    if (!ext.empty()) {
+        BatchArenas ar;
+        if ((rc = ar.open(ctx, io, ext, C, false)) || (rc = ar.upload(0, ext)) || (rc = run_generic(ctx, plan, io, ar, ext.need_floor0)) ||
+            (rc = ar.download(0, chains, 0, n_chains, ext)) || (rc = ar.finish()))
+            return rc;
+    }
+    commit_stream_states(chains, walks);
     return LWB_OK;
 }
 

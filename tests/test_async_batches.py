@@ -9,9 +9,9 @@ submission order -- f32 PCM bit for bit, i16 PCM exactly, nothing outside the wr
 arena changed, and every stream's final state bit for bit.  Each sequence runs ungated first, so that no arena grows in
 the gated run, and every call names the kernels that must (and must not) run.
 
-A submit still waits on the host in the places the header lists (arena growth, staging-ring wrap, the four-kernel path's
-per-round synchronise); must_return() says how many submits of each path return behind the gate.  Page-locked arrays
-are freed before a gate closes: cudaFreeHost waits for the device."""
+A submit still waits on the host in the places the header lists (arena growth, staging-ring wrap); must_return() says
+how many submits of each path return behind the gate.  Page-locked arrays are freed before a gate closes: cudaFreeHost
+waits for the device."""
 import ctypes
 import threading
 
@@ -250,12 +250,10 @@ def submit_gated(ctx, gate, calls, what, must_return=3):
 def must_return(path, chunks):
     """Submits of `path` that return behind the gate, from the blocking points the header lists.  The staging ring has
     three slots, all completed after the warm-up.  Paths that stage once per submit (k_long, the one-pass and segmented
-    schedules, k_mid's spectrum entry, k_chain) therefore return all three.  The residue entries of k_mid and k_long
-    stage twice per submit, at any chunk count: their packet list on the compute stream, then all their runs at once.
-    The second submit takes the first one's packet list slot, which completes behind the gate.  The four-kernel path
-    synchronises before its first round."""
-    if path == "generic":
-        return 0
+    schedules, k_mid's spectrum entry, k_chain, and the four-kernel path, whose 6-packet batches take one round)
+    therefore return all three.  The residue entries of k_mid and k_long stage twice per submit, at any chunk count:
+    their packet list on the compute stream, then all their runs at once.  The second submit takes the first one's
+    packet list slot, which completes behind the gate."""
     return 1 if path in ("residue_long", "residue_mid") else 3
 
 

@@ -14,11 +14,10 @@ state bit for bit.  A prepared batch writes the same arenas every step, so each 
 the context's stream: the final state alone depends on the last packet only.
 
 The library waits on the host in these places by design; the tests work around them:
-- Arena growth.  ensure() and ensure_pinned() synchronise when they grow an arena.  Each sequence first runs ungated, on
-  other streams and output arenas of the same sizes, so that no queued call grows one.
+- Arena growth.  ensure() synchronises when it grows an arena.  Each sequence first runs ungated, on other streams and
+  output arenas of the same sizes, so that no queued call grows one.
 - Staging ring wrap.  acquire_staging waits for the copy three stagings back, so only the first two or three calls that
   stage descriptors return while the gate is closed.  The later ones wait for it to open, and they still reuse the ring.
-- The four-kernel path synchronises before it writes its pinned descriptors.  It has no case here.
 - Host-memory batches return after their PCM has landed.
 - Inputs are in device arenas before the gate closes."""
 import threading
