@@ -362,7 +362,7 @@ typedef struct lwb_batch_io {
  * floor / VQ arrays (floor_memory == LWB_MEM_HOST) are uploaded by copies queued on that stream, which read them when
  * the stream reaches them, as cudaMemcpyAsync reads pinned memory: keep them unchanged until the batch's work has run
  * (lwb_ctx_synchronize, or an event recorded on the stream after the call).  The chain array and the mode and flag
- * arrays are read before the call returns. */
+ * arrays are read before the call returns.  A batch that is refused changes no chain result and no stream state. */
 int lwb_decode_chains(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io);
 
 /* Asynchronous batches.  A decode server that feeds the GPU from host memory queues batch k + 1 (and entropy-decodes
@@ -377,7 +377,7 @@ int lwb_decode_chains(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lw
  *   - the stream states advance, so a stream can appear in the next submit at once, with its packets in order;
  *   - the chain array and the mode and flag arrays have been read.
  * A submit that is refused (an argument or memory check, a batch lwb_decode_chains would refuse) changes no chain
- * result, no stream state and no arena.  After LWB_ERR_CUDA the chain results are restored and no stream state is
+ * result, no stream state and no arena.  After LWB_ERR_CUDA the chain results are not written and no stream state is
  * committed on the host, but kernels already queued may have run: the device-side state of the batch's streams is
  * undefined (reset or re-import them).  The staging a failed batch took is reused only behind what it had queued.
  * Until the ticket completes:

@@ -108,7 +108,7 @@ struct SetupShape { const lwb_ctx *ctx; uint8_t channels, bs0, bs1; };
 SetupShape setup_shape(const lwb_setup *su);
 const lwb_setup *stream_setup(const lwb_stream *s);
 // The refusals lwb_submit_chains would make of this batch (out_format, streams, one channel count, a stream in two
-// chains, floor kinds, out_stride, page-locked host memory), made without queuing anything or changing any state.
+// chains, floor kinds, out_stride, VQ offsets, page-locked host memory), made without queuing anything or changing any state.
 int check_submit(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io);
 
 }  // namespace lwfb

@@ -71,7 +71,6 @@ struct lwb_ctx {
     uint64_t tickets_issued = 0, tickets_done = 0;
     std::deque<cudaEvent_t> ticket_events;
     std::vector<cudaEvent_t> spare_events;
-    bool pinned_only = false;      // set while a host-memory lwb_submit_chains queues its batch
     size_t x_cap_elems = (size_t)64 << 20;     // IMDCT scratch per round of the generic path (256 MiB)
 };
 
@@ -377,29 +376,6 @@ static int with_out_format(int fmt, Fn &&f)
         return fmt == F ? f(std::integral_constant<int, F>()) : with_out_format<F + 1>(fmt, f);
     else
         return LWB_ERR_INVALID;
-}
-
-// D2H of the PCM that chains [i0, i1) produced, from the staging buffer `stage`, which holds arena element `obase` at
-// its start.  Only the write set is copied (pcm_copy_plan.h): the gaps between planes and between chains are the
-// caller's memory, and the kernels never wrote them in the staging buffer.
-static int copy_pcm_to_host(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chain *chains, size_t i0, size_t i1,
-                            const void *stage, uint64_t obase, cudaStream_t st)
-{
-    const size_t esz = out_format_of(io->out_format).esz;
-    const bool planar = out_format_of(io->out_format).planar;
-    ctx->pcm_spans.clear();
-    for (size_t i = i0; i < i1; i++) {
-        const lwb_chain *c = &chains[i];
-        pcm_chain_spans(planar, c->stream->setup->out_channels(), c->out_offset, c->out_stride, c->n_samples, ctx->pcm_spans);
-    }
-    plan_pcm_copies(ctx->pcm_spans, (uint64_t)INT32_MAX / esz, ctx->pcm_copies);
-    for (const PcmCopy &cp : ctx->pcm_copies) {
-        char *dst = (char *)io->pcm + cp.off * esz;
-        const char *src = (const char *)stage + (cp.off - obase) * esz;
-        if (cp.height == 1) CU(ctx, cudaMemcpyAsync(dst, src, cp.width * esz, cudaMemcpyDeviceToHost, st));
-        else CU(ctx, cudaMemcpy2DAsync(dst, cp.pitch * esz, src, cp.pitch * esz, cp.width * esz, cp.height, cudaMemcpyDeviceToHost, st));
-    }
-    return LWB_OK;
 }
 
 // The layout the fused kernels take: planar out (f32, i16 or f16), and 16-byte aligned addresses, which their TMA bulk

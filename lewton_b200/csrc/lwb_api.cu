@@ -668,7 +668,7 @@ extern "C" int lwb_decoded_sample_count(const lwb_setup *su, uint8_t mode, int p
 #include "path_mid.cuh"
 
 // The batch paths in the order they are tried.  The last, the four-kernel path, takes every batch that reaches it.
-using BatchPath = int (*)(lwb_ctx *, lwb_chain *, size_t, const lwb_batch_io *, bool *, lwb_plan *);
+using BatchPath = int (*)(lwb_ctx *, const lwb_chain *, size_t, const lwb_batch_io *, const BatchWalk &, bool *, lwb_plan *);
 static constexpr BatchPath kBatchPaths[] = {try_long, try_mid, try_mixed, try_chain, try_generic};
 constexpr size_t kChainPath = 3, kGenericPath = 4;
 static_assert(kBatchPaths[kChainPath] == try_chain && kBatchPaths[kGenericPath] == try_generic && std::size(kBatchPaths) == kGenericPath + 1,
@@ -684,7 +684,7 @@ static size_t first_batch_path()
 }
 
 // The argument checks of a batch and what every path relies on: valid chains, each stream in one chain, and the residue
-// entries' floor kinds and single channel count.  Shared by queue_batch and lwfb::check_submit.
+// entries' floor kinds and single channel count.
 static int check_batch_args(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io)
 {
     if (io->entry != LWB_ENTRY_SPECTRUM && io->entry != LWB_ENTRY_RESIDUE && io->entry != LWB_ENTRY_VQ) return fail(ctx, LWB_ERR_INVALID, "bad entry");
@@ -710,14 +710,42 @@ static int check_batch_args(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chai
     return LWB_OK;
 }
 
-// Checks, plans and queues one batch; a host-memory batch that queues work issues its ticket (BatchArenas::finish).
-// Every argument refusal of a batch must be one lwfb::check_submit also makes without queuing anything: the stream
-// batcher relies on it to refuse a submit of several batches before it queues the first.  A new refusal goes into
-// check_batch_args, or, if a path makes it while it walks the chains, into check_submit as well.
-static int queue_batch(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, lwb_plan *prepared)
+// The one walk of a batch, made before a path is chosen: the argument checks, every chain's walk and the batch's extent,
+// and every refusal a batch gets from its arguments and arrays -- an out_stride below the samples a chain produces,
+// host floor kinds out of range or without floor1_y, a dense floor without dense_floor, decreasing host VQ offsets
+// and, with pinned_only (a submit), host arrays that are not page-locked.  It writes nothing into the chain array and
+// queues nothing.  The paths refuse a batch only on a CUDA error, and in one more case: the VQ entry's front-stage
+// limits (channels, alignment, channels * n/2), which launch_prologue checks on the path that takes the batch.
+static int walk_batch(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, bool pinned_only, BatchWalk *bw)
+{
+    int rc = check_batch_args(ctx, chains, n_chains, io);
+    if (rc || n_chains == 0) return rc;
+    BatchExtent &ext = bw->ext;
+    bw->walks.resize(n_chains);
+    const bool planar = out_format_of(io->out_format).planar;
+    for (size_t i = 0; i < n_chains; i++) {
+        const lwb_chain *c = &chains[i];
+        const ChainWalk &w = bw->walks[i] = walk_chain(c, [](uint32_t, const Geom &, bool, uint32_t, uint64_t, uint64_t) {});
+        if (!w.done) continue;
+        if (planar && c->out_stride < w.n_samples) return fail(ctx, LWB_ERR_BUFFER, "chain: out_stride smaller than the samples produced");
+        ext.add(io, c, w);
+        if (io->entry != LWB_ENTRY_SPECTRUM && (rc = scan_floor_kinds(ctx, io, c, w.done, &ext.need_dense, &ext.need_floor0))) return rc;
+    }
+    if (ext.need_dense && !io->dense_floor) return fail(ctx, LWB_ERR_INVALID, "dense_floor missing");
+    if ((rc = check_vq_offsets(ctx, io, ext.r_lo, ext.r_hi))) return rc;
+    if (!pinned_only || io->memory != LWB_MEM_HOST || ext.empty()) return LWB_OK;
+    CU(ctx, cudaSetDevice(ctx->device));
+    return check_page_locked(ctx, io, ext, chains[0].stream->setup->channels);
+}
+
+// Walks one batch (walk_batch) and queues it on the first path that takes it.  Once the path has queued its work, the
+// chain results and stream states of the walk are written; a refused batch changes neither.  A host-memory batch that
+// queues work issues its ticket (BatchArenas::finish).
+static int queue_batch(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, lwb_plan *prepared, bool pinned_only)
 {
     if (!ctx || (!chains && n_chains) || !io) return LWB_ERR_INVALID;
-    int rc = check_batch_args(ctx, chains, n_chains, io);
+    BatchWalk bw;
+    int rc = walk_batch(ctx, chains, n_chains, io, pinned_only, &bw);
     if (rc || n_chains == 0) return rc;
     CU(ctx, cudaSetDevice(ctx->device));
     if (prepared) prepared->captured = false; // the path that takes the batch captures it anew, if it can
@@ -728,20 +756,24 @@ static int queue_batch(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const l
         if (chains[i].stream->setup->host.n_out) first = kChainPath;
     for (size_t k = first; k < std::size(kBatchPaths); k++) {
         bool handled = false;
-        if ((rc = kBatchPaths[k](ctx, chains, n_chains, io, &handled, prepared)) || handled) return rc;
+        if ((rc = kBatchPaths[k](ctx, chains, n_chains, io, bw, &handled, prepared))) return rc;
+        if (!handled) continue;
+        for (size_t i = 0; i < n_chains; i++) set_chain_result(&chains[i], bw.walks[i]);
+        commit_stream_states(chains, bw.walks);
+        return LWB_OK;
     }
     return fail(ctx, LWB_ERR_INVALID, "internal: no batch path took the batch");
 }
 
 // One batch.  ticket == nullptr: the synchronous entry points, which return once a host-memory batch's PCM has landed
 // (they wait for the ticket it issued).  Else lwb_submit_chains: *ticket identifies the batch's work, whatever its
-// memory space, and nothing is waited for.
+// memory space, and nothing is waited for; a host-memory submit's arrays must be page-locked.
 static int decode_chains_impl(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, lwb_plan *prepared,
                               uint64_t *ticket = nullptr)
 {
     if (!ctx) return LWB_ERR_INVALID;
     const uint64_t issued = ctx->tickets_issued;
-    int rc = queue_batch(ctx, chains, n_chains, io, prepared);
+    int rc = queue_batch(ctx, chains, n_chains, io, prepared, ticket != nullptr);
     if (rc) return rc;
     if (!ticket) return ctx->tickets_issued != issued ? retire_tickets(ctx, ctx->tickets_issued, true) : LWB_OK;
     if (ctx->tickets_issued == issued) {        // a device-memory or empty batch (which may not have set the device)
@@ -763,20 +795,7 @@ extern "C" int lwb_decode_chains(lwb_ctx *ctx, lwb_chain *chains, size_t n_chain
 extern "C" int lwb_submit_chains(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, uint64_t *ticket)
 {
     if (!ctx || !ticket || (!chains && n_chains) || !io) return LWB_ERR_INVALID;
-    // a submit that fails leaves every chain result as it was (stream states are committed only by a batch that queued)
-    struct Result { uint32_t n_samples, packets_done; int32_t status; };
-    std::vector<Result> saved(n_chains);
-    for (size_t i = 0; i < n_chains; i++) saved[i] = Result{chains[i].n_samples, chains[i].packets_done, chains[i].status};
-    ctx->pinned_only = io->memory == LWB_MEM_HOST;
-    const int rc = decode_chains_impl(ctx, chains, n_chains, io, nullptr, ticket);
-    ctx->pinned_only = false;
-    if (rc)
-        for (size_t i = 0; i < n_chains; i++) {
-            chains[i].n_samples = saved[i].n_samples;
-            chains[i].packets_done = saved[i].packets_done;
-            chains[i].status = saved[i].status;
-        }
-    return rc;
+    return decode_chains_impl(ctx, chains, n_chains, io, nullptr, ticket);
 }
 
 extern "C" int lwb_ticket_query(lwb_ctx *ctx, uint64_t ticket, int *done)
@@ -803,21 +822,11 @@ SetupShape setup_shape(const lwb_setup *su) { return SetupShape{su->ctx, su->cha
 
 const lwb_setup *stream_setup(const lwb_stream *s) { return s->setup; }
 
-// queue_batch's argument checks (check_batch_args), then what the paths refuse while they walk the chains: the extent
-// checks of BatchExtent (out_stride, floor kinds, a missing dense arena) and, for host memory, the page-locked check of
-// BatchArenas::open -- on the chain walks alone, queuing nothing.
+// The walk lwb_submit_chains makes of this batch (walk_batch), queuing nothing.
 int check_submit(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io)
 {
-    int rc = check_batch_args(ctx, chains, n_chains, io);
-    if (rc || n_chains == 0) return rc;
-    const unsigned C = chains[0].stream->setup->channels;
-    BatchExtent ext;
-    for (size_t i = 0; i < n_chains; i++) {
-        const ChainWalk w = walk_chain(&chains[i], [](uint32_t, const Geom &, bool, uint32_t, uint64_t, uint64_t) {});
-        if ((rc = ext.add(ctx, io, &chains[i], w.done, w.coeff_end, w.n_samples))) return rc;
-    }
-    if ((rc = ext.finish(ctx, io))) return rc;
-    return io->memory == LWB_MEM_HOST && !ext.empty() ? check_page_locked(ctx, io, ext, C) : LWB_OK;
+    BatchWalk bw;
+    return walk_batch(ctx, chains, n_chains, io, true, &bw);
 }
 }  // namespace lwfb
 

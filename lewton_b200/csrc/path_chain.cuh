@@ -85,7 +85,8 @@ static int chain_floor0_curves(lwb_ctx *ctx, const BatchArenas &ar, const BatchE
     return launch_floor0_curves(ctx, (const DevPacket *)ctx->desc.p, n_pk, ar.C, ar.fl.kinds, ar.fl.ys, *zero);
 }
 
-static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, bool *handled, lwb_plan *plan)
+static int try_chain(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, const BatchWalk &bw, bool *handled,
+                     lwb_plan *plan)
 {
     *handled = false;
     const uint64_t gen_at_entry = ctx->state_gen;
@@ -112,21 +113,16 @@ static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
     if ((rc = acquire_staging(ctx, desc_bytes + byte_bytes, &st))) return rc;
     ChainDesc *hd = (ChainDesc *)st->h;
     uint8_t *hb = (uint8_t *)st->h + desc_bytes;
-    BatchExtent ext;
+    const BatchExtent &ext = bw.ext;
     size_t boff = 0, n_launch = 0;
-    std::vector<ChainWalk> walks(n_chains);
     for (size_t i = 0; i < n_chains; i++) {
-        lwb_chain *c = &chains[i];
-        const ChainWalk &w = walks[i] = walk_chain(c, [&](uint32_t k, const Geom &, bool, uint32_t, uint64_t, uint64_t) {
-            write_mode_bytes(c, k, hb + boff + 3 * k);
-        });
-        set_chain_result(c, w);
-        if ((rc = ext.add(ctx, io, c, w.done, w.coeff_end, w.n_samples))) return rc;
-        if (!w.done) continue;
-        chain_desc(c, 0, w.done, c->stream->has, c->stream->plen, c->coeff_offset, 0, (uint32_t)boff, &hd[n_launch++]);
-        boff += (size_t)w.done * 3;
+        const lwb_chain *c = &chains[i];
+        const uint32_t done = bw.walks[i].done;
+        if (!done) continue;
+        for (uint32_t k = 0; k < done; k++) write_mode_bytes(c, k, hb + boff + 3 * k);
+        chain_desc(c, 0, done, c->stream->has, c->stream->plen, c->coeff_offset, 0, (uint32_t)boff, &hd[n_launch++]);
+        boff += (size_t)done * 3;
     }
-    if ((rc = ext.finish(ctx, io))) return rc;
     if (n_launch) {
         BatchArenas ar;
         if ((rc = ar.open(ctx, io, ext, maxc, false)) || (rc = ar.upload(0, ext))) return rc;
@@ -142,7 +138,7 @@ static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
             return rc;
         // residue or VQ entry with floor-0 records: their curves first, by absolute coefficient offset like ar.coeffs
         float *zero = nullptr;
-        if (residue && ext.need_floor0 && ar.fl.ys && (rc = chain_floor0_curves(ctx, ar, ext, chains, n_chains, walks, &zero))) return rc;
+        if (residue && ext.need_floor0 && ar.fl.ys && (rc = chain_floor0_curves(ctx, ar, ext, chains, n_chains, bw.walks, &zero))) return rc;
         StepArgs args;
         args.pcm = ar.pcm;
         args.out_format = io->out_format;
@@ -159,9 +155,8 @@ static int try_chain(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         std::vector<Step> steps(1, Step{LWB_KERNEL_CHAIN, dbuf.p, n_launch, nullptr});
         if ((rc = run_steps(ctx, args, steps))) return rc;
         if (cap) capture(plan, gen_at_entry, FrontStages(), args, std::move(steps));
-        if ((rc = ar.download(0, chains, 0, n_chains, ext)) || (rc = ar.finish())) return rc;
+        if ((rc = ar.download(0, chains, bw, 0, n_chains, ext)) || (rc = ar.finish())) return rc;
     }
-    commit_stream_states(chains, walks);
     return LWB_OK;
 }
 

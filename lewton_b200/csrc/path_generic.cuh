@@ -15,6 +15,8 @@ struct ChainWalk {
     uint32_t end_plen = 0;
     bool clear_after = false;     // the OLA guard fired on packet `done`: the state becomes empty
     uint64_t coeff_end = 0;       // element offset behind the last decoded packet
+    uint32_t full_n = 0;          // n of every decoded packet when all are full-window blocks of one size, else 0
+    bool long_only = true;        // every decoded packet a long block between long neighbours (both window flags set)
 };
 
 // Walks chain c from its stream's state, with no side effects.  on_packet(k, g, has, plen, coeff, pos) sees every packet
@@ -28,9 +30,9 @@ static ChainWalk walk_chain(const lwb_chain *c, F &&on_packet)
     uint32_t plen = c->stream->plen;
     uint64_t coeff = c->coeff_offset, pos = 0;
     for (uint32_t k = 0; k < c->n_packets; k++) {
+        const int pf = c->prev_window_flags ? c->prev_window_flags[k] : 1, nf = c->next_window_flags ? c->next_window_flags[k] : 1;
         Geom g;
-        const int rc = geometry(su, c->mode_numbers[k], c->prev_window_flags ? c->prev_window_flags[k] : 1,
-                                c->next_window_flags ? c->next_window_flags[k] : 1, &g);
+        const int rc = geometry(su, c->mode_numbers[k], pf, nf, &g);
         if (rc) { w.status = rc; break; }
         if (has) {
             const uint32_t slope_len = 1u << ((g.slope_sel ? su->bs1 : su->bs0) - 1);
@@ -45,6 +47,8 @@ static ChainWalk walk_chain(const lwb_chain *c, F &&on_packet)
             }
         }
         on_packet(k, g, has, plen, coeff, pos);
+        w.full_n = g.ls == 0 && g.rs == g.n >> 1 && g.re == g.n && (!w.done || w.full_n == g.n) ? g.n : 0;
+        w.long_only = w.long_only && g.blockflag && pf && nf;
         coeff += (uint64_t)su->channels * (g.n >> 1);
         if (has) pos += g.rs - g.ls;
         has = true;
@@ -66,7 +70,7 @@ static void set_chain_result(lwb_chain *c, const ChainWalk &w)
 }
 
 // The stream states the walks of a batch leave, committed once the batch's work is queued.
-static void commit_stream_states(lwb_chain *chains, const std::vector<ChainWalk> &walks)
+static void commit_stream_states(const lwb_chain *chains, const std::vector<ChainWalk> &walks)
 {
     for (size_t i = 0; i < walks.size(); i++)
         if (walks[i].done || walks[i].clear_after) set_stream_state(chains[i].stream, walks[i].end_has, walks[i].end_plen);
@@ -215,9 +219,20 @@ static int scan_floor_kinds(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chai
     return LWB_OK;
 }
 
+// Host VQ offsets (LWB_ENTRY_VQ) bound the records of packet rows [r_lo, r_hi), which floor_views stages: they must not
+// decrease across them.  Device arrays cannot be looked at.
+static int check_vq_offsets(lwb_ctx *ctx, const lwb_batch_io *io, uint64_t r_lo, uint64_t r_hi)
+{
+    if (io->entry != LWB_ENTRY_VQ || io->floor_memory == LWB_MEM_DEVICE || r_hi <= r_lo) return LWB_OK;
+    if (io->vq_run_offsets[r_hi] < io->vq_run_offsets[r_lo] || io->vq_entry_offsets[r_hi] < io->vq_entry_offsets[r_lo])
+        return fail(ctx, LWB_ERR_INVALID, "vq offsets must be non-decreasing");
+    return LWB_OK;
+}
+
 // The floor and VQ arrays (LWB_ENTRY_VQ) of packet rows [r_lo, r_hi) of a batch with C channels as the device sees
 // them, biased so that ABSOLUTE rows and offsets address them.  Host arrays get room in the kinds / ys / vqoff / vqrec
 // arenas of `set` (grown behind `in_use`, see ensure()), which upload_floor_rows fills; device arrays are used in place.
+// The caller has checked the VQ offsets (check_vq_offsets).
 struct FloorViews {
     const uint8_t *kinds = nullptr;
     const uint32_t *ys = nullptr;
@@ -248,7 +263,6 @@ static int floor_views(lwb_ctx *ctx, const lwb_batch_io *io, ArenaSet &set, cuda
     if (!vq) return LWB_OK;
     const uint64_t o_lo = io->vq_run_offsets[r_lo], o_hi = io->vq_run_offsets[r_hi];
     const uint64_t e_lo = io->vq_entry_offsets[r_lo], e_hi = io->vq_entry_offsets[r_hi];
-    if (o_hi < o_lo || e_hi < e_lo) return fail(ctx, LWB_ERR_INVALID, "vq offsets must be non-decreasing");
     const size_t b_off = ((size_t)(r_hi - r_lo) + 1) * sizeof(uint64_t), b_run = std::max<size_t>((size_t)(o_hi - o_lo), 1) * sizeof(lwb_vq_run);
     if ((rc = ensure(ctx, set.vqoff, 2 * b_off, in_use)) ||
         (rc = ensure(ctx, set.vqrec, b_run + std::max<size_t>((size_t)(e_hi - e_lo), 1) * sizeof(uint16_t) + 16, in_use)))
@@ -288,30 +302,38 @@ struct BatchExtent {
     uint64_t c_lo = ~0ull, c_hi = 0, o_lo = ~0ull, o_hi = 0, r_lo = ~0ull, r_hi = 0;
     bool need_dense = false;      // a decoded row has a dense floor
     bool need_floor0 = false;     // a decoded row may have a floor-0 record (LWB_FLOOR_ZERO)
-    bool scan = true;            // check the floor kinds of the rows added (a chunk's rows were checked with its batch)
 
-    // Chain c decodes `done` packets, whose coefficients end at coeff_end, into n_samples samples per channel.
-    int add(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chain *c, uint32_t done, uint64_t coeff_end, uint64_t n_samples)
+    // The ranges of chain c, whose walk w decodes w.done packets.
+    void add(const lwb_batch_io *io, const lwb_chain *c, const ChainWalk &w)
     {
-        if (!done) return LWB_OK;
+        if (!w.done) return;
         const unsigned C = c->stream->setup->out_channels();
         const bool planar = out_format_of(io->out_format).planar;
-        if (planar && c->out_stride < n_samples) return fail(ctx, LWB_ERR_BUFFER, "chain: out_stride smaller than the samples produced");
         c_lo = std::min(c_lo, c->coeff_offset);
-        c_hi = std::max(c_hi, coeff_end);
+        c_hi = std::max(c_hi, w.coeff_end);
         o_lo = std::min(o_lo, c->out_offset);
-        o_hi = std::max(o_hi, c->out_offset + (planar ? (uint64_t)(C - 1) * c->out_stride + n_samples : n_samples * C));
-        if (io->entry == LWB_ENTRY_SPECTRUM) return LWB_OK;
+        o_hi = std::max(o_hi, c->out_offset + (planar ? (uint64_t)(C - 1) * c->out_stride + w.n_samples : w.n_samples * C));
+        if (io->entry == LWB_ENTRY_SPECTRUM) return;
         r_lo = std::min(r_lo, c->packet_index);
-        r_hi = std::max<uint64_t>(r_hi, c->packet_index + done);
-        return scan ? scan_floor_kinds(ctx, io, c, done, &need_dense, &need_floor0) : LWB_OK;
-    }
-    int finish(lwb_ctx *ctx, const lwb_batch_io *io) const
-    {
-        return need_dense && !io->dense_floor ? fail(ctx, LWB_ERR_INVALID, "dense_floor missing") : LWB_OK;
+        r_hi = std::max<uint64_t>(r_hi, c->packet_index + w.done);
     }
     bool empty() const { return c_hi <= c_lo; }
 };
+
+// A batch walked once, before a path is chosen (walk_batch, lwb_api.cu): every chain's walk and the batch's extent.
+// The paths read it; queue_batch writes the chain results and stream states from it once a path has queued the batch.
+struct BatchWalk {
+    std::vector<ChainWalk> walks;
+    BatchExtent ext;
+};
+
+// The extent of chains [i0, i1) of a walked batch: one chunk of a chunked host-memory batch.
+static BatchExtent chunk_extent(const lwb_batch_io *io, const lwb_chain *chains, const BatchWalk &bw, size_t i0, size_t i1)
+{
+    BatchExtent e;
+    for (size_t i = i0; i < i1; i++) e.add(io, &chains[i], bw.walks[i]);
+    return e;
+}
 
 // Whether host bytes [lo, hi) * esz of `base` begin and end in page-locked memory (the runtime tells; pageable memory
 // is "unregistered").
@@ -353,6 +375,29 @@ static int check_page_locked(lwb_ctx *ctx, const lwb_batch_io *io, const BatchEx
                                        " is not page-locked (lwb_host_alloc, cudaHostAlloc or cudaHostRegister)").c_str());
 }
 
+// D2H of the PCM that chains [i0, i1), walked as walks[i0, i1), produced, from the staging buffer `stage`, which holds
+// arena element `obase` at its start.  Only the write set is copied (pcm_copy_plan.h): the gaps between planes and
+// between chains are the caller's memory, and the kernels never wrote them in the staging buffer.
+static int copy_pcm_to_host(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chain *chains, const ChainWalk *walks, size_t i0, size_t i1,
+                            const void *stage, uint64_t obase, cudaStream_t st)
+{
+    const size_t esz = out_format_of(io->out_format).esz;
+    const bool planar = out_format_of(io->out_format).planar;
+    ctx->pcm_spans.clear();
+    for (size_t i = i0; i < i1; i++) {
+        const lwb_chain *c = &chains[i];
+        pcm_chain_spans(planar, c->stream->setup->out_channels(), c->out_offset, c->out_stride, walks[i].n_samples, ctx->pcm_spans);
+    }
+    plan_pcm_copies(ctx->pcm_spans, (uint64_t)INT32_MAX / esz, ctx->pcm_copies);
+    for (const PcmCopy &cp : ctx->pcm_copies) {
+        char *dst = (char *)io->pcm + cp.off * esz;
+        const char *src = (const char *)stage + (cp.off - obase) * esz;
+        if (cp.height == 1) CU(ctx, cudaMemcpyAsync(dst, src, cp.width * esz, cudaMemcpyDeviceToHost, st));
+        else CU(ctx, cudaMemcpy2DAsync(dst, cp.pitch * esz, src, cp.pitch * esz, cp.width * esz, cp.height, cudaMemcpyDeviceToHost, st));
+    }
+    return LWB_OK;
+}
+
 // The arenas of a batch as its kernels address them: coefficients, dense floors and PCM by absolute element offset,
 // floor and VQ arrays by absolute packet row (FloorViews).  A host-memory batch is staged in the next of the context's
 // host sets, chunk by chunk: upload(k) brings chunk k's inputs, download(k) takes its PCM home behind its kernels.  Its
@@ -385,7 +430,6 @@ struct BatchArenas {
         int rc;
         cudaEvent_t in_use = nullptr;
         if (host) {
-            if (ctx->pinned_only && (rc = check_page_locked(ctx, io, ext, C))) return rc;
             set = &ctx->host_sets[ctx->host_next];
             ctx->host_next = (ctx->host_next + 1) % kHostSets;
             in_use = set->done;
@@ -421,14 +465,14 @@ struct BatchArenas {
         return LWB_OK;
     }
     // chains [i0, i1) of the batch make up chunk k
-    int download(size_t k, const lwb_chain *chains, size_t i0, size_t i1, const BatchExtent &ck)
+    int download(size_t k, const lwb_chain *chains, const BatchWalk &bw, size_t i0, size_t i1, const BatchExtent &ck)
     {
         if (!host || ck.o_hi <= ck.o_lo) return LWB_OK;
         if (down != ctx->stream) {
             CU(ctx, cudaEventRecord(ctx->ev_done[k], ctx->stream));
             CU(ctx, cudaStreamWaitEvent(down, ctx->ev_done[k], 0));
         }
-        return copy_pcm_to_host(ctx, io, chains, i0, i1, set->pcm.p, o_lo, down);
+        return copy_pcm_to_host(ctx, io, chains, bw.walks.data(), i0, i1, set->pcm.p, o_lo, down);
     }
     // The batch is queued: a host-memory batch records its ticket, which also releases its set to the next user.
     int finish()
@@ -548,7 +592,7 @@ static int front_stages_run(lwb_ctx *ctx, const lwb_batch_io *io, const FrontSta
     ext.need_dense = fs.dense;
     BatchArenas ar;
     int rc;
-    if ((rc = ar.open(ctx, io, ext, fs.C, false)) || (rc = ar.upload(0, ext))) return rc;
+    if ((rc = check_vq_offsets(ctx, io, fs.r_lo, fs.r_hi)) || (rc = ar.open(ctx, io, ext, fs.C, false)) || (rc = ar.upload(0, ext))) return rc;
     return front_stages_launch(ctx, ar, fs, 0, fs.n);
 }
 
@@ -645,7 +689,7 @@ struct PlanPacket {
 };
 
 struct PlanChain {
-    lwb_chain *c;
+    const lwb_chain *c;
     std::vector<PlanPacket> pk;
 };
 
@@ -776,33 +820,26 @@ static int run_generic(lwb_ctx *ctx, std::vector<PlanChain> &plan, const lwb_bat
 }
 
 // Any batch: not captured by a prepared batch, which plans it again on every execution.
-static int try_generic(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, bool *handled, lwb_plan *)
+static int try_generic(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, const BatchWalk &bw, bool *handled, lwb_plan *)
 {
     *handled = true;
+    const BatchExtent &ext = bw.ext;
+    if (ext.empty()) return LWB_OK;
     const unsigned C = chains[0].stream->setup->channels;
     std::vector<PlanChain> plan(n_chains);
-    std::vector<ChainWalk> walks(n_chains);
-    BatchExtent ext;
-    int rc;
     for (size_t i = 0; i < n_chains; i++) {
-        lwb_chain *c = &chains[i];
         PlanChain &pc = plan[i];
-        pc.c = c;
-        pc.pk.reserve(c->n_packets);
-        walks[i] = walk_chain(c, [&](uint32_t, const Geom &g, bool has, uint32_t plen, uint64_t coeff, uint64_t pos) {
+        pc.c = &chains[i];
+        pc.pk.reserve(bw.walks[i].done);
+        walk_chain(pc.c, [&](uint32_t, const Geom &g, bool has, uint32_t plen, uint64_t coeff, uint64_t pos) {
             pc.pk.push_back(PlanPacket{g, has ? plen : 0, coeff, pos});
         });
-        set_chain_result(c, walks[i]);
-        if ((rc = ext.add(ctx, io, c, walks[i].done, walks[i].coeff_end, walks[i].n_samples))) return rc;
     }
-    if ((rc = ext.finish(ctx, io))) return rc;
-    if (!ext.empty()) {
-        BatchArenas ar;
-        if ((rc = ar.open(ctx, io, ext, C, false)) || (rc = ar.upload(0, ext)) || (rc = run_generic(ctx, plan, io, ar, ext.need_floor0)) ||
-            (rc = ar.download(0, chains, 0, n_chains, ext)) || (rc = ar.finish()))
-            return rc;
-    }
-    commit_stream_states(chains, walks);
-    return LWB_OK;
+    BatchArenas ar;
+    int rc;
+    if ((rc = ar.open(ctx, io, ext, C, false)) || (rc = ar.upload(0, ext)) || (rc = run_generic(ctx, plan, io, ar, ext.need_floor0)) ||
+        (rc = ar.download(0, chains, bw, 0, n_chains, ext)))
+        return rc;
+    return ar.finish();
 }
 

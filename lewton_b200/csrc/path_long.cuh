@@ -69,9 +69,9 @@ static void long_runs_of(const LongItem &it, size_t cuts, const float *coeffs, c
         channel_run(it.c, ch, kLongN2, coeffs + it.c->coeff_offset, pcm, esz, it.P, it.has_prev, it.has_prev ? kLongN2 : 0, cuts, w);
 }
 
-// Every packet a long block of the fast blocksize with long neighbours, every stream empty or
-// holding a 1024-sample right half, the fused kernels' layout: what the fused kernel takes.
-static bool batch_is_uniform_long(const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io)
+// Every packet decodes, a long block of the fast blocksize between long neighbours, every stream empty or holding a
+// 1024-sample right half, the fused kernels' layout: what the fused kernel takes.
+static bool batch_is_uniform_long(const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, const BatchWalk &bw)
 {
     if (!fused_layout(chains, n_chains, io)) return false;
     const float *pack = nullptr;
@@ -83,40 +83,9 @@ static bool batch_is_uniform_long(const lwb_chain *chains, size_t n_chains, cons
         if (pack && pack != su->host.tab[1].pack) return false;
         pack = su->host.tab[1].pack;
         if (s->has && s->plen != (uint32_t)kLongN2) return false;
-        for (uint32_t k = 0; k < c->n_packets; k++) {
-            const uint8_t m = c->mode_numbers[k];
-            if (m >= su->n_modes || !su->host.mode_blockflag[m]) return false;
-            if (c->prev_window_flags && !c->prev_window_flags[k]) return false;
-            if (c->next_window_flags && !c->next_window_flags[k]) return false;
-        }
+        if (bw.walks[i].done != c->n_packets || !bw.walks[i].long_only) return false;
     }
     return true;
-}
-
-// A uniform batch (k_long, k_mid: every packet a full-window block of one size n = 2 * n2) in closed form.  Sets the
-// results of chains [i0, i1) -- all their packets decode, each emits n2 samples but the first of an empty stream --
-// and adds them to `ext`.
-static int uniform_extent(lwb_ctx *ctx, const lwb_batch_io *io, lwb_chain *chains, size_t i0, size_t i1, uint32_t n2, BatchExtent *ext)
-{
-    for (size_t i = i0; i < i1; i++) {
-        lwb_chain *c = &chains[i];
-        c->status = LWB_OK;
-        c->packets_done = c->n_packets;
-        c->n_samples = c->n_packets ? (c->n_packets - (c->stream->has ? 0u : 1u)) * n2 : 0u;
-    }
-    int rc = LWB_OK;
-    for (size_t i = i0; i < i1 && !rc; i++) {
-        const lwb_chain *c = &chains[i];
-        rc = ext->add(ctx, io, c, c->n_packets, c->coeff_offset + (uint64_t)c->n_packets * c->stream->setup->channels * n2, c->n_samples);
-    }
-    return rc;
-}
-
-// ... and once it is queued, the state it leaves: every stream that decoded a packet holds its last n2-sample right half.
-static void commit_uniform_states(lwb_chain *chains, size_t n_chains, uint32_t n2)
-{
-    for (size_t i = 0; i < n_chains; i++)
-        if (chains[i].n_packets) set_stream_state(chains[i].stream, true, n2);
 }
 
 // The k_long runs of a batch in pinned staging: chunk k (chains [n_chains * k / n_chunks, n_chains * (k + 1) / n_chunks))
@@ -246,15 +215,15 @@ static int long_upload_runs(lwb_ctx *ctx, const LongRuns &lr, cudaStream_t ds)
 // stream runs its kernels, copy_out takes its PCM home -- so that H2D, kernels and D2H of consecutive chunks overlap
 // (the link is duplex).  The runs of all chunks are built while the first chunk's inputs copy and go up once, on
 // copy_in behind those inputs: behind copy_out's PCM copies the kernels would wait for the D2H of the batch before.
-static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, bool *handled, lwb_plan *plan)
+static int try_long(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, const BatchWalk &bw, bool *handled,
+                    lwb_plan *plan)
 {
     *handled = false;
-    if (!batch_is_uniform_long(chains, n_chains, io)) return LWB_OK;
+    if (!batch_is_uniform_long(chains, n_chains, io, bw)) return LWB_OK;
     *handled = true;
-    BatchExtent ext;
-    int rc;
-    if ((rc = uniform_extent(ctx, io, chains, 0, n_chains, kLongN2, &ext)) || (rc = ext.finish(ctx, io))) return rc;
+    const BatchExtent &ext = bw.ext;
     if (ext.empty()) return LWB_OK;
+    int rc;
     const unsigned C = chains[0].stream->setup->channels;                  // (residue entries: the batch's one count)
     const bool residue = io->entry != LWB_ENTRY_SPECTRUM, host = io->memory == LWB_MEM_HOST;
     const float *pack = chains[0].stream->setup->host.tab[1].pack;          // one twiddle pack per launch
@@ -289,9 +258,7 @@ static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_
     size_t pk0 = 0;
     for (size_t k = 0; k < n_chunks; k++) {
         const size_t i0 = n_chains * k / n_chunks, i1 = n_chains * (k + 1) / n_chunks;
-        BatchExtent ke;
-        ke.scan = false;
-        if ((rc = uniform_extent(ctx, io, chains, i0, i1, kLongN2, &ke))) return rc;
+        const BatchExtent ke = chunk_extent(io, chains, bw, i0, i1);
         if (ke.empty()) continue;
         size_t npk = 0;
         for (size_t i = i0; i < i1; i++) npk += chains[i].n_packets;
@@ -303,12 +270,10 @@ static int try_long(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_
             gen = ctx->state_gen;                                           // every arena the capture points into is sized
         }
         steps.assign(1, Step{LWB_KERNEL_LONG, lr.d + lr.chunks[k].r0, lr.chunks[k].nr / kLongNB, pack});
-        if ((rc = run_steps(ctx, args, steps)) || (rc = ar.download(k, chains, i0, i1, ke))) return rc;
+        if ((rc = run_steps(ctx, args, steps)) || (rc = ar.download(k, chains, bw, i0, i1, ke))) return rc;
         pk0 += npk;
     }
     CU(ctx, cudaEventRecord(ctx->ev_kdone[lr.par], ctx->stream));
     if (cap) capture(plan, gen, fs, args, std::move(steps));                 // (one chunk)
-    if ((rc = ar.finish())) return rc;
-    commit_uniform_states(chains, n_chains, kLongN2);
-    return LWB_OK;
+    return ar.finish();
 }

@@ -7,7 +7,8 @@
 
 struct MidGroup { LongRun r[4]; uint32_t n_packets; };
 
-static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, bool *handled, lwb_plan *plan)
+static int try_mid(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, const BatchWalk &bw, bool *handled,
+                   lwb_plan *plan)
 {
     *handled = false;
     const uint64_t gen_at_entry = ctx->state_gen;
@@ -17,30 +18,21 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
     const size_t esz = out_format_of(io->out_format).esz;
     const float *pack = nullptr;
     int kb = 0;                                              // 1: n = 1024, 2: n = 512 (one size per batch: one pack)
-    // pass 1, no side effects: every packet a full-window block of that size on top of no state or an n/2-sample one
+    // every packet decodes, a full-window block of that size on top of no state or an n/2-sample one (a bad mode
+    // number: the chain kernel reports it in place)
     size_t n_runs = 0;
     for (size_t i = 0; i < n_chains; i++) {
         const lwb_chain *c = &chains[i];
         const lwb_setup *su = c->stream->setup;
+        const ChainWalk &w = bw.walks[i];
         if (su->channels > 8 || (su->bs1 != 10 && su->bs1 != 9) || !su->host.tab[1].pack) return LWB_OK;
         if (pack && pack != su->host.tab[1].pack) return LWB_OK;
         pack = su->host.tab[1].pack;
         kb = 11 - su->bs1;
-        const uint32_t n_blk = 2048u >> kb, n2_blk = n_blk >> 1;
-        if (c->stream->has && c->stream->plen != n2_blk) return LWB_OK;
-        for (uint32_t k = 0; k < c->n_packets; k++) {
-            Geom g;
-            if (geometry(su, c->mode_numbers[k], c->prev_window_flags ? c->prev_window_flags[k] : 1,
-                         c->next_window_flags ? c->next_window_flags[k] : 1, &g))
-                return LWB_OK;                                  // a bad mode number: the chain kernel reports it in place
-            if (g.n != n_blk || g.ls != 0 || g.rs != n2_blk || g.re != n_blk) return LWB_OK;
-        }
-        if (c->n_packets) {
-            // the planes hold the samples the chain produces: none for the first packet of an empty stream
-            const uint64_t produced = (uint64_t)(c->n_packets - (c->stream->has ? 0u : 1u)) * n2_blk;
-            if (c->out_stride < produced) return LWB_OK;     // (the chain kernel words the error)
-            n_runs += su->channels;
-        }
+        const uint32_t n_blk = 2048u >> kb;
+        if (c->stream->has && c->stream->plen != n_blk >> 1) return LWB_OK;
+        if (w.done != c->n_packets || (w.done && w.full_n != n_blk)) return LWB_OK;
+        if (w.done) n_runs += su->channels;
     }
     if (!pack || !n_runs) return LWB_OK;
     const size_t kMidN2 = 1024u >> kb, NBg = (size_t)1 << kb;
@@ -49,8 +41,7 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
 
     const bool host = io->memory == LWB_MEM_HOST;
     int rc;
-    BatchExtent ext;
-    if ((rc = uniform_extent(ctx, io, chains, 0, n_chains, (uint32_t)kMidN2, &ext)) || (rc = ext.finish(ctx, io))) return rc;
+    const BatchExtent &ext = bw.ext;
     size_t n_pk = 0;
     if (residue)
         for (size_t i = 0; i < n_chains; i++) n_pk += chains[i].n_packets;
@@ -119,7 +110,6 @@ static int try_mid(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_b
     std::vector<Step> steps(1, Step{LWB_KERNEL_MID, dbuf.p, groups.size(), pack});
     if ((rc = run_steps(ctx, args, steps))) return rc;
     if (cap) capture(plan, gen_at_entry, fs, args, std::move(steps));
-    if ((rc = ar.download(0, chains, 0, n_chains, ext)) || (rc = ar.finish())) return rc;
-    commit_uniform_states(chains, n_chains, (uint32_t)kMidN2);
-    return LWB_OK;
+    if ((rc = ar.download(0, chains, bw, 0, n_chains, ext))) return rc;
+    return ar.finish();
 }

@@ -37,7 +37,8 @@ static void balance_static_deal(Run *runs, size_t n, size_t W, std::vector<Run> 
 // a group of k_short_g: eight runs of one length (the deal above moves it as a unit)
 struct ShortGroup { ShortRun r[kShortOct]; uint32_t n_packets; };
 
-static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, bool *handled, lwb_plan *plan)
+static int try_mixed(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, const BatchWalk &bw, bool *handled,
+                     lwb_plan *plan)
 {
     *handled = false;
     const uint64_t gen_at_entry = ctx->state_gen;
@@ -94,18 +95,17 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
     bool chain_sees_long = false;       // the chain kernel's shared memory is sized for what it actually gets
     struct Walk { uint32_t seg0, n_seg; uint32_t boff; size_t slot0; };
     std::vector<Walk> walks(n_chains);
-    std::vector<ChainWalk> results(n_chains);
     std::vector<Seg> segs;
     segs.reserve(n_chains * 2);
     struct Pk { bool has; uint32_t plen; uint64_t coeff, pos; };
     std::vector<Pk> pk;
     std::vector<uint8_t> bytes(total_packets * 3 + 16);
     size_t boff = 0, max_rounds = 0;
-    BatchExtent ext;
+    const BatchExtent &ext = bw.ext;
     int rc = LWB_OK;
     std::vector<uint8_t> is_l;           // bit0 k_long packet, bit1 follows a short block, bit2 precedes one; bit3 k_short packet
     for (size_t i = 0; i < n_chains; i++) {
-        lwb_chain *c = &chains[i];
+        const lwb_chain *c = &chains[i];
         const lwb_setup *su = c->stream->setup;
         Walk &w = walks[i];
         w.boff = (uint32_t)boff;
@@ -113,7 +113,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         if (pk.size() < c->n_packets) { pk.resize(c->n_packets); is_l.resize(c->n_packets); }
         w.seg0 = (uint32_t)segs.size();
         w.n_seg = 0;
-        const ChainWalk &cw = results[i] = walk_chain(c, [&](uint32_t k, const Geom &g, bool has, uint32_t plen, uint64_t coeff, uint64_t pos) {
+        walk_chain(c, [&](uint32_t k, const Geom &g, bool has, uint32_t plen, uint64_t coeff, uint64_t pos) {
             pk[k] = Pk{has, plen, coeff, pos};
             is_l[k] = 0;
             if (g.blockflag && g.n == (uint32_t)kLongN && su->host.tab[1].pack == pack && pack) {
@@ -125,10 +125,8 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
             }
             write_mode_bytes(c, k, &bytes[boff + 3 * k]);
         });
-        const uint32_t done = cw.done;
-        set_chain_result(c, cw);
+        const uint32_t done = bw.walks[i].done;
         boff += (size_t)done * 3;
-        if ((rc = ext.add(ctx, io, c, done, cw.coeff_end, cw.n_samples))) return rc;
         if (!done) continue;
         // pass 2: segments.  A fused-kernel run starts at a long block that follows a short one and ends at
         // one that precedes a short one; everything else is handed to the chain kernel.
@@ -153,7 +151,6 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
         w.n_seg = (uint32_t)segs.size() - w.seg0;
         max_rounds = std::max<size_t>(max_rounds, w.n_seg);
     }
-    if ((rc = ext.finish(ctx, io))) return rc;
     // One pass instead of rounds: where every chain alternates strictly between long and short segments, the only
     // thing a segment needs from its predecessor is the pl = 128 samples the two blocks overlap in, and the sum
     // x[ls + i] w[i] + prev[i] w[pl-1-i] (audio.rs:1112-1118) does not care which of its two products exists first.
@@ -184,8 +181,8 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
     {
         size_t pk_flat = 0, pk_all = 0;
         for (size_t i = 0; i < n_chains; i++) {
-            pk_all += chains[i].packets_done;
-            if (chain_flat[i]) pk_flat += chains[i].packets_done;
+            pk_all += bw.walks[i].done;
+            if (chain_flat[i]) pk_flat += bw.walks[i].done;
         }
         if (!flat_enabled || pk_flat * 2 < pk_all) {
             std::fill(chain_flat.begin(), chain_flat.end(), 0);
@@ -255,7 +252,7 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
             Chunk &ck = chunks[k];
             ck.i0 = n_chains * k / n_chunks;
             ck.i1 = n_chains * (k + 1) / n_chunks;
-            ck.ext.scan = false;
+            ck.ext = chunk_extent(io, chains, bw, ck.i0, ck.i1);
             std::vector<size_t> round_long(max_rounds, 0), round_short(max_rounds, 0);
             for (size_t i = ck.i0; i < ck.i1; i++) {
                 const unsigned C = chains[i].stream->setup->channels;
@@ -263,7 +260,6 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
                     if (segs[walks[i].seg0 + q].kind == SEG_LONG) round_long[round_of(i, q)] += C;
                     if (segs[walks[i].seg0 + q].kind == SEG_SHORT) round_short[round_of(i, q)] += C;
                 }
-                if ((rc = ck.ext.add(ctx, io, &chains[i], results[i].done, results[i].coeff_end, results[i].n_samples))) return rc;
             }
             ck.round_cut.assign(max_rounds, 1);
             ck.round_cut_s.assign(max_rounds, 1);
@@ -477,13 +473,12 @@ static int try_mixed(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const lwb
             Chunk &ck = chunks[k];
             if (ck.ext.empty()) continue;
             if ((rc = ar.upload(k, ck.ext)) || (ck.np_ && (rc = front_stages_launch(ctx, ar, fs, ck.p0, ck.np_))) ||
-                (rc = run_steps(ctx, args, ck.steps)) || (rc = ar.download(k, chains, ck.i0, ck.i1, ck.ext)))
+                (rc = run_steps(ctx, args, ck.steps)) || (rc = ar.download(k, chains, bw, ck.i0, ck.i1, ck.ext)))
                 return rc;
         }
         if (cap) capture(plan, gen_at_entry, fs, args, std::move(chunks[0].steps));
         if ((rc = ar.finish())) return rc;
     }
-    commit_stream_states(chains, results);
     return LWB_OK;
 }
 
