@@ -148,7 +148,7 @@ struct lwb_plan {
     bool captured = false;
     uint64_t gen = 0;
     FrontStages front;
-    DevBuf pro, mix;                   // descriptors the capture owns: the long path's front stages, the steps'
+    DevBuf pro, desc;                  // descriptors the capture owns: the long path's front stages, the steps'
     StepArgs args;
     std::vector<Step> steps;
 };

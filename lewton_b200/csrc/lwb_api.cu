@@ -849,10 +849,10 @@ extern "C" int lwb_plan_create(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains,
 extern "C" void lwb_plan_destroy(lwb_plan *p)
 {
     if (!p) return;
-    if (p->mix.p || p->pro.p) {
+    if (p->desc.p || p->pro.p) {
         cudaSetDevice(p->ctx->device);
         cudaStreamSynchronize(p->ctx->stream);
-        if (p->mix.p) cudaFree(p->mix.p);
+        if (p->desc.p) cudaFree(p->desc.p);
         if (p->pro.p) cudaFree(p->pro.p);
     }
     delete p;

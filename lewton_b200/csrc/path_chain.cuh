@@ -130,7 +130,7 @@ static int try_chain(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, con
         // descriptors and mode bytes share one device buffer; a prepared batch (device memory, spectrum
         // entry) owns it and replays the launch while no stream changes shape (residue and VQ entries are not captured)
         const bool cap = plan && !ar.host && !residue;
-        DevBuf &dbuf = cap ? plan->mix : ctx->cdesc;
+        DevBuf &dbuf = cap ? plan->desc : ctx->cdesc;
         const size_t used_desc = n_launch * sizeof(ChainDesc);
         if ((rc = ensure(ctx, dbuf, used_desc + boff + 16))) return rc;
         if ((rc = upload_staging(ctx, st, hd, dbuf.p, used_desc, sm)) ||

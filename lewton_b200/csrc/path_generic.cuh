@@ -1,5 +1,5 @@
 // path_generic.cuh -- part of the C-ABI translation unit (included by lwb_api.cu, not compiled on its own):
-// the chain walk, extent and host-memory pipeline every batch path shares, and the four-kernel path (kernels_generic.cuh).
+// the chain walk, run helpers, extent and host-memory pipeline every batch path shares, and the four-kernel path (kernels_generic.cuh).
 #pragma once
 
 // ---------------------------------------------------------------------------------------------
@@ -82,6 +82,97 @@ static void write_mode_bytes(const lwb_chain *c, uint32_t k, uint8_t *out)
     out[0] = c->mode_numbers[k];
     out[1] = c->prev_window_flags ? c->prev_window_flags[k] : 1;
     out[2] = c->next_window_flags ? c->next_window_flags[k] : 1;
+}
+
+// Cuts `whole`, the run of one channel (a LongRun or a ShortRun: in, out, state, in_stride, n_packets, has_prev), into
+// `cuts` pieces w[0, cuts), for when there are too few runs to fill the machine.  Every piece after the first
+// re-transforms the packet before its first one as a primer (its right half is all the piece needs), which keeps the
+// pieces independent at the cost of one extra transform per cut.  Packet 0 of the run emits first_emit samples, every
+// later one n2, of esz bytes each.  Only the last piece stores the state.
+template <typename Run>
+static void cut_run(const Run &whole, size_t cuts, size_t first_emit, size_t n2, size_t esz, Run *w)
+{
+    const size_t P = whole.n_packets;
+    for (size_t k = 0; k < cuts; k++) {
+        const size_t p0 = P * k / cuts, p1 = P * (k + 1) / cuts;   // this piece emits packets [p0, p1)
+        Run &r = w[k];
+        std::memset(&r, 0, sizeof(r));
+        r.in_stride = whole.in_stride;
+        r.state = whole.state;
+        r.write_state = (k + 1 == cuts);
+        if (k == 0) {
+            r.in = whole.in;
+            r.out = whole.out;
+            r.n_packets = (uint32_t)(p1 - p0);
+            r.has_prev = whole.has_prev;
+        } else {
+            const size_t primer = p0 - 1;
+            r.in = whole.in + primer * whole.in_stride;
+            r.out = (char *)whole.out + (first_emit + primer * n2) * esz;          // behind the samples before packet p0
+            r.n_packets = (uint32_t)(p1 - p0 + 1);
+            r.has_prev = 0;
+        }
+    }
+}
+
+// The run of channel ch of n packets of chain c, blocks of n2-point halves, cut into `cuts` pieces w[0, cuts): its
+// coefficients start at `in` (the packets' first one; channels n2 apart, packets C * n2 apart), its PCM at `pcm` (the
+// chain's sample of its first packet; planes out_stride apart, esz bytes per sample).  has: a state enters it;
+// first_emit: the samples its first packet emits.
+template <typename Run>
+static void channel_run(const lwb_chain *c, unsigned ch, size_t n2, const float *in, char *pcm, size_t esz, uint32_t n, bool has,
+                        size_t first_emit, size_t cuts, Run *w)
+{
+    const lwb_stream *s = c->stream;
+    const lwb_setup *su = s->setup;
+    const unsigned C = su->channels;
+    cut_run(Run{in + (size_t)ch * n2, pcm + (c->out_offset + (size_t)ch * c->out_stride) * esz, s->d_state + (size_t)ch * state_stride(su),
+                (uint32_t)(C * n2), n, has},
+            cuts, first_emit, n2, esz, w);
+}
+
+// Static deals (run r -> warp r mod W: k_long_s, k_mid, k_short, k_short_g) finish with their most loaded warp: order the
+// runs so that the W columns carry equal packet counts -- longest first, dealt boustrophedon (row 0 left to right, row 1
+// right to left, ...).  With random run lengths an unordered deal leaves the slowest of 1184 warps a third above the mean.
+// W: the warps of the launch of n runs, `warps` per CTA.
+template <typename Run>
+static void balance_static_deal(Run *runs, size_t n, int warps, int sm_count)
+{
+    const size_t W = (size_t)static_deal_grid(n, warps, sm_count) * warps;
+    if (n <= W || W < 2) return;
+    uint32_t maxp = 0;
+    for (size_t i = 0; i < n; i++) maxp = std::max(maxp, runs[i].n_packets);
+    std::vector<size_t> start(maxp + 2, 0);
+    for (size_t i = 0; i < n; i++) start[maxp - runs[i].n_packets + 1]++;          // counting sort, descending
+    for (size_t k = 1; k < start.size(); k++) start[k] += start[k - 1];
+    std::vector<Run> tmp(n);
+    const size_t full_rows = n / W;
+    for (size_t i = 0; i < n; i++) {
+        const size_t k = start[maxp - runs[i].n_packets]++;
+        const size_t row = k / W, col = k % W;
+        tmp[(row & 1) && row < full_rows ? row * W + (W - 1 - col) : k] = runs[i];
+    }
+    std::memcpy(runs, tmp.data(), n * sizeof(Run));
+}
+
+// Up to G runs of one length that a warp transforms in lockstep (k_mid, k_short_g); the deal above moves it as a unit.
+template <typename Run, int G>
+struct RunGroup { Run r[G]; uint32_t n_packets; };
+
+// Cuts `runs` into groups of g <= G runs of equal length: longest first, in their order within a length.  The last group
+// of a length is filled up with pad(its first run), a dummy of the kernel's own kind.  Sorts `runs`.
+template <int G, typename Run, typename Pad>
+static std::vector<RunGroup<Run, G>> group_runs(std::vector<Run> &runs, size_t g, Pad &&pad)
+{
+    std::stable_sort(runs.begin(), runs.end(), [](const Run &a, const Run &b) { return a.n_packets > b.n_packets; });
+    std::vector<RunGroup<Run, G>> groups;
+    for (size_t i = 0; i < runs.size();) {
+        RunGroup<Run, G> &gr = groups.emplace_back();
+        std::memset(&gr, 0, sizeof(gr));
+        gr.n_packets = runs[i].n_packets;
+        for (size_t k = 0; k < g; k++) gr.r[k] = i < runs.size() && runs[i].n_packets == gr.n_packets ? runs[i++] : pad(gr.r[0]);
+    }
+    return groups;
 }
 
 // Every launch of the library goes through launch() or launched(), which count it under its kernel's LWB_KERNEL_* id.

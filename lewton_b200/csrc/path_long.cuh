@@ -1,5 +1,5 @@
 // path_long.cuh -- part of the C-ABI translation unit (included by lwb_api.cu, not compiled on its own):
-// the fused long-block path (kernel_long.cuh): run cutting and descriptor staging, for the spectrum and the residue entries.
+// the fused long-block path (kernel_long.cuh): its runs and their staging, for the spectrum and the residue entries.
 #pragma once
 
 // ---------------------------------------------------------------------------------------------
@@ -13,53 +13,6 @@ struct LongItem {
     uint32_t P;
     bool has_prev;
 };
-
-// Cuts `whole`, the run of one channel (a LongRun or a ShortRun: in, out, state, in_stride, n_packets, has_prev), into
-// `cuts` pieces w[0, cuts), for when there are too few runs to fill the machine.  Every piece after the first
-// re-transforms the packet before its first one as a primer (its right half is all the piece needs), which keeps the
-// pieces independent at the cost of one extra transform per cut.  Packet 0 of the run emits first_emit samples, every
-// later one n2, of esz bytes each.  Only the last piece stores the state.
-template <typename Run>
-static void cut_run(const Run &whole, size_t cuts, size_t first_emit, size_t n2, size_t esz, Run *w)
-{
-    const size_t P = whole.n_packets;
-    for (size_t k = 0; k < cuts; k++) {
-        const size_t p0 = P * k / cuts, p1 = P * (k + 1) / cuts;   // this piece emits packets [p0, p1)
-        Run &r = w[k];
-        std::memset(&r, 0, sizeof(r));
-        r.in_stride = whole.in_stride;
-        r.state = whole.state;
-        r.write_state = (k + 1 == cuts);
-        if (k == 0) {
-            r.in = whole.in;
-            r.out = whole.out;
-            r.n_packets = (uint32_t)(p1 - p0);
-            r.has_prev = whole.has_prev;
-        } else {
-            const size_t primer = p0 - 1;
-            r.in = whole.in + primer * whole.in_stride;
-            r.out = (char *)whole.out + (first_emit + primer * n2) * esz;          // behind the samples before packet p0
-            r.n_packets = (uint32_t)(p1 - p0 + 1);
-            r.has_prev = 0;
-        }
-    }
-}
-
-// The run of channel ch of n packets of chain c, blocks of n2-point halves, cut into `cuts` pieces w[0, cuts): its
-// coefficients start at `in` (the packets' first one; channels n2 apart, packets C * n2 apart), its PCM at `pcm` (the
-// chain's sample of its first packet; planes out_stride apart, esz bytes per sample).  has: a state enters it;
-// first_emit: the samples its first packet emits.
-template <typename Run>
-static void channel_run(const lwb_chain *c, unsigned ch, size_t n2, const float *in, char *pcm, size_t esz, uint32_t n, bool has,
-                        size_t first_emit, size_t cuts, Run *w)
-{
-    const lwb_stream *s = c->stream;
-    const lwb_setup *su = s->setup;
-    const unsigned C = su->channels;
-    cut_run(Run{in + (size_t)ch * n2, pcm + (c->out_offset + (size_t)ch * c->out_stride) * esz, s->d_state + (size_t)ch * state_stride(su),
-                (uint32_t)(C * n2), n, has},
-            cuts, first_emit, n2, esz, w);
-}
 
 // Appends the runs of one chain, each channel cut into `cuts` pieces.  coeffs / pcm: arenas addressed by absolute
 // element offset.
@@ -264,7 +217,7 @@ static int try_long(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, cons
         for (size_t i = i0; i < i1; i++) npk += chains[i].n_packets;
         if ((rc = ar.upload(k, ke)) || (residue && (rc = front_stages_launch(ctx, ar, fs, pk0, npk)))) return rc;
         if (!lr.d) {
-            if ((rc = long_build_runs(ctx, chains, n_chains, n_chunks, in, ar.pcm, out_format_of(io->out_format).esz, cap ? &plan->mix : nullptr, &lr)) ||
+            if ((rc = long_build_runs(ctx, chains, n_chains, n_chunks, in, ar.pcm, out_format_of(io->out_format).esz, cap ? &plan->desc : nullptr, &lr)) ||
                 (rc = long_upload_runs(ctx, lr, host ? ctx->copy_in : ctx->copy_out)))
                 return rc;
             gen = ctx->state_gen;                                           // every arena the capture points into is sized

@@ -5,8 +5,6 @@
 // batch (any entry) follow try_chain; the launch is one LWB_KERNEL_MID step.
 #pragma once
 
-struct MidGroup { LongRun r[4]; uint32_t n_packets; };
-
 static int try_mid(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, const BatchWalk &bw, bool *handled,
                    lwb_plan *plan)
 {
@@ -51,9 +49,8 @@ static int try_mid(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const
     // A prepared batch in device memory owns its descriptors (run groups, then the front stages' packet list) and replays
     // them while no stream changes shape (lwb_plan_execute).
     const bool cap = plan && !host;
-    DevBuf &dbuf = cap ? plan->mix : ctx->cdesc;
-    const size_t NBcap = (size_t)1 << kb;
-    const size_t off_pro = (n_runs * NBcap * sizeof(LongRun) + 15) & ~(size_t)15;      // (an upper bound: every run its own group)
+    DevBuf &dbuf = cap ? plan->desc : ctx->cdesc;
+    const size_t off_pro = (n_runs * NBg * sizeof(LongRun) + 15) & ~(size_t)15;      // (an upper bound: every run its own group)
     if ((rc = ensure(ctx, dbuf, off_pro + n_pk * sizeof(DevPacket) + 16))) return rc;
     FrontStages fs;
     if (residue) {
@@ -65,7 +62,7 @@ static int try_mid(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const
             return rc;
         d_coeffs = (const float *)ctx->spec.p - ext.c_lo;       // k_mid reads the spectrum
     }
-    // runs, then groups of two runs of equal length (an odd one gets a dummy partner), longest first, dealt balanced
+    // runs, then groups of NBg runs of equal length (filled up with dummies), longest first, dealt balanced
     std::vector<LongRun> runs;
     runs.reserve(n_runs);
     for (size_t i = 0; i < n_chains; i++) {
@@ -76,25 +73,9 @@ static int try_mid(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const
             channel_run(c, ch, kMidN2, d_coeffs + c->coeff_offset, ar.pcm, esz, c->n_packets, c->stream->has, 0, 1, &runs.back());
         }
     }
-    std::stable_sort(runs.begin(), runs.end(), [](const LongRun &a, const LongRun &b) { return a.n_packets > b.n_packets; });
-    std::vector<MidGroup> groups, tmp_g;
-    groups.reserve(runs.size() / NBg + 8);
-    for (size_t i = 0; i < runs.size();) {
-        MidGroup g;
-        std::memset(&g, 0, sizeof(g));
-        g.n_packets = runs[i].n_packets;
-        size_t k = 0;
-        while (k < NBg && i < runs.size() && runs[i].n_packets == g.n_packets) g.r[k++] = runs[i++];
-        for (; k < NBg; k++) {                    // dummies: read valid memory, store nothing
-            g.r[k] = g.r[0];
-            g.r[k].dummy = 1;
-            g.r[k].write_state = 0;
-            g.r[k].has_prev = 0;
-        }
-        groups.push_back(g);
-    }
-    const size_t Wg = (size_t)static_deal_grid(groups.size(), kLongWarps, ctx->sm_count) * kLongWarps;
-    balance_static_deal(groups.data(), groups.size(), Wg, tmp_g);
+    // dummies: read valid memory, store nothing
+    auto groups = group_runs<4>(runs, NBg, [](LongRun d) { d.dummy = 1; d.write_state = 0; d.has_prev = 0; return d; });
+    balance_static_deal(groups.data(), groups.size(), kLongWarps, ctx->sm_count);
     const size_t bytes = groups.size() * NBg * sizeof(LongRun);
     Staging *st;
     if ((rc = acquire_staging(ctx, bytes, &st))) return rc;
