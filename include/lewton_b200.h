@@ -312,7 +312,10 @@ enum { LWB_MEM_HOST = 0, LWB_MEM_DEVICE = 1 };
  * (planar), or n_samples * channels elements at out_offset (interleaved), and nothing else in `pcm`
  * (channels: lwb_setup_output_channels of the stream's setup),
  * in either memory space: the gaps between planes and between chains keep what the caller put there.
- * Any element offsets and any pointer alignment are accepted.  The fused kernels take device-memory
+ * Any element offsets and any pointer alignment are accepted, as long as every range a chain touches ends
+ * inside the 64-bit address space: a chain whose PCM write set (out_offset + (channels - 1) * out_stride +
+ * n_samples, or out_offset + n_samples * channels), coefficient range or packet-row range, counted in bytes,
+ * would wrap past 2^64 is refused with LWB_ERR_BUFFER before anything is queued.  The fused kernels take device-memory
  * batches whose coeffs / dense_floor / pcm are 16-byte aligned and whose coeff_offset, out_offset and
  * out_stride are multiples of 4 (host-memory batches: the offsets only); anything else runs on the
  * chain kernel, which gives the same results more slowly. */
@@ -332,6 +335,11 @@ typedef struct lwb_chain {
     int32_t status;                   /* LWB_OK or the error of packet `packets_done`              */
 } lwb_chain;
 
+/* A host-memory batch (memory == LWB_MEM_HOST) is staged on the device as its extent: coefficient elements from the
+ * lowest coeff_offset to the highest coefficient end, PCM elements from the lowest out_offset to the highest end of a
+ * write set, gaps included.  Its device memory grows with that span, not with the samples decoded: two chains 2^33
+ * elements apart, or one planar chain with an out_stride of 2^32, stage 32 GiB of f32 PCM.  Keep the chains of one
+ * host-memory batch close together in the arenas. */
 typedef struct lwb_batch_io {
     int entry;                        /* LWB_ENTRY_*                                               */
     int memory;                       /* LWB_MEM_*: where coeffs/dense_floor/pcm live              */

@@ -710,9 +710,31 @@ static int check_batch_args(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chai
     return LWB_OK;
 }
 
+// Whether the ranges chain c's walk w touches end inside the 64-bit address space, in bytes: its PCM write set, its
+// coefficient (and dense floor) elements and, for the residue entries, its packet rows of floor1_y, the widest per-row
+// array.  BatchExtent::add and the run descriptors sum these offsets in uint64_t; an offset near 2^64 would wrap to a
+// small one and address memory the caller never named.
+static bool chain_ranges_fit(const lwb_batch_io *io, const lwb_chain *c, const ChainWalk &w)
+{
+    const lwb_setup *su = c->stream->setup;
+    const uint64_t K = su->out_channels(), esz = out_format_of(io->out_format).esz;
+    uint64_t span, end;
+    if (out_format_of(io->out_format).planar) {
+        if (__builtin_mul_overflow(K - 1, c->out_stride, &span) || __builtin_add_overflow(span, w.n_samples, &span)) return false;
+    } else if (__builtin_mul_overflow(w.n_samples, K, &span)) {
+        return false;
+    }
+    if (__builtin_add_overflow(c->out_offset, span, &end) || __builtin_mul_overflow(end, esz, &end)) return false;
+    // walk_chain sums the packets' C * n/2 (below 2^52) onto coeff_offset: coeff_end is below it exactly when that wrapped
+    if (w.coeff_end < c->coeff_offset || __builtin_mul_overflow(w.coeff_end, (uint64_t)sizeof(float), &end)) return false;
+    if (io->entry == LWB_ENTRY_SPECTRUM) return true;
+    return !__builtin_add_overflow(c->packet_index, (uint64_t)w.done, &end) &&
+           !__builtin_mul_overflow(end, (uint64_t)su->channels * LWB_MAX_POSTS * sizeof(uint32_t), &end);
+}
+
 // The one walk of a batch, made before a path is chosen: the argument checks, every chain's walk and the batch's extent,
 // and every refusal a batch gets from its arguments and arrays -- an out_stride below the samples a chain produces,
-// host floor kinds out of range or without floor1_y, a dense floor without dense_floor, decreasing host VQ offsets
+// a chain range that does not fit in 64 bits (chain_ranges_fit), host floor kinds out of range or without floor1_y, a dense floor without dense_floor, decreasing host VQ offsets
 // and, with pinned_only (a submit), host arrays that are not page-locked.  It writes nothing into the chain array and
 // queues nothing.  The paths refuse a batch only on a CUDA error, and in one more case: the VQ entry's front-stage
 // limits (channels, alignment, channels * n/2), which launch_prologue checks on the path that takes the batch.
@@ -728,6 +750,7 @@ static int walk_batch(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, co
         const ChainWalk &w = bw->walks[i] = walk_chain(c, [](uint32_t, const Geom &, bool, uint32_t, uint64_t, uint64_t) {});
         if (!w.done) continue;
         if (planar && c->out_stride < w.n_samples) return fail(ctx, LWB_ERR_BUFFER, "chain: out_stride smaller than the samples produced");
+        if (!chain_ranges_fit(io, c, w)) return fail(ctx, LWB_ERR_BUFFER, "chain: a PCM, coefficient or packet-row range does not fit in 64 bits");
         ext.add(io, c, w);
         if (io->entry != LWB_ENTRY_SPECTRUM && (rc = scan_floor_kinds(ctx, io, c, w.done, &ext.need_dense, &ext.need_floor0))) return rc;
     }

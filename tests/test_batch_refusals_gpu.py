@@ -3,7 +3,11 @@ batch can get from its arguments and arrays.  For a batch shaped for each of the
 called through lwb_decode_chains, lwb_submit_chains and lwb_plan_execute: the call returns the refusal's code and
 message, launches no kernel, issues no ticket and changes no PCM element, chain result or stream state.  The same batch,
 unbroken, then decodes on its path as the oracle does.  A stream-batcher submit of two groups whose later group has too
-small an out_stride is refused before the first group is queued."""
+small an out_stride is refused before the first group is queued.  A chain whose PCM write set, coefficient range or
+packet-row range would wrap past 2^64 is refused the same way, with the batch in host or in device memory: a wrapped sum
+would otherwise give an extent that ends before it starts, and kernels queued against the wrapped address.
+
+Do not run the wrap cases against a library without the wrap check: it queues kernels at the wrapped addresses."""
 import ctypes as C
 
 import numpy as np
@@ -22,7 +26,7 @@ pytestmark = pytest.mark.gpu
 
 launches_are_attributed  # (autouse)
 
-F32P, RESIDUE, VQ, HOST = cabi.OUT_F32_PLANAR, cabi.ENTRY_RESIDUE, cabi.ENTRY_VQ, cabi.MEM_HOST
+F32P, RESIDUE, VQ, HOST, DEVICE = cabi.OUT_F32_PLANAR, cabi.ENTRY_RESIDUE, cabi.ENTRY_VQ, cabi.MEM_HOST, cabi.MEM_DEVICE
 MIXED = {"k_long_s", "k_short_g"}
 # shape: (setup kind, sequence kind, packets per chain, kernels the unbroken residue batch runs, kernels it may add)
 SHAPES = {
@@ -33,6 +37,8 @@ SHAPES = {
     "generic": ("wide", "mixed", 6, GENERIC, set()),
 }
 OUT_STRIDE = "chain: out_stride smaller than the samples produced"
+WRAP = "chain: a PCM, coefficient or packet-row range does not fit in 64 bits"
+U64 = 1 << 64
 # case: (entry points, code, message).  lwb_decode_chains and lwb_plan_execute take pageable host memory.
 CASES = {
     "out_stride": (("decode", "submit", "plan"), cabi.ERR_BUFFER, OUT_STRIDE),
@@ -41,6 +47,13 @@ CASES = {
     "floor1_y_missing": (("decode", "submit", "plan"), cabi.ERR_INVALID, "floor1_y missing"),
     "floor_kind_range": (("decode", "submit", "plan"), cabi.ERR_INVALID, "floor_kind out of range"),
     "vq_offsets": (("decode", "submit", "plan"), cabi.ERR_INVALID, "vq offsets must be non-decreasing"),
+    "wrap_out_offset": (("decode", "submit", "plan"), cabi.ERR_BUFFER, WRAP),
+    "wrap_out_stride": (("decode", "submit", "plan"), cabi.ERR_BUFFER, WRAP),
+    "wrap_coeff_offset": (("decode", "submit", "plan"), cabi.ERR_BUFFER, WRAP),
+    "wrap_packet_index": (("decode", "submit", "plan"), cabi.ERR_BUFFER, WRAP),
+    "wrap_out_bytes": (("decode", "submit", "plan"), cabi.ERR_BUFFER, WRAP),
+    "wrap_coeff_bytes": (("decode", "submit", "plan"), cabi.ERR_BUFFER, WRAP),
+    "wrap_packet_bytes": (("decode", "submit", "plan"), cabi.ERR_BUFFER, WRAP),
     "pageable": (("submit",), cabi.ERR_INVALID,
                  "host-memory submit: coeffs is not page-locked (lwb_host_alloc, cudaHostAlloc or cudaHostRegister)"),
 }
@@ -61,8 +74,23 @@ def sus(ctx):
 def break_batch(ctx, call, case, arr, io):
     """Breaks the marshalled batch (arr, io) of `call` as `case` says; returns the arrays io now points to."""
     kinds = call.kinds.copy()                     # [packet row][channel]
+    last = arr[len(call.chains) - 1]
     if case == "out_stride":
-        arr[len(call.chains) - 1].out_stride = 4
+        last.out_stride = 4
+    elif case == "wrap_out_offset":               # out_offset + out_stride + n_samples passes 2^64
+        last.out_offset = U64 - last.out_stride - 8
+    elif case == "wrap_out_stride":               # (C - 1) * out_stride (+ n_samples) passes 2^64
+        last.out_stride = U64 - 4
+    elif case == "wrap_coeff_offset":             # the coefficient end passes 2^64
+        last.coeff_offset = U64 - 16
+    elif case == "wrap_packet_index":             # packet_index + packets passes 2^64
+        last.packet_index = U64 - 2
+    elif case == "wrap_out_bytes":                # the PCM end fits in elements, not in bytes (f32: * 4)
+        last.out_offset = 1 << 62
+    elif case == "wrap_coeff_bytes":              # the coefficient end fits in elements, not in bytes
+        last.coeff_offset = 1 << 62
+    elif case == "wrap_packet_bytes":             # the packet-row end fits, its floor1_y bytes (* C * LWB_MAX_POSTS * 4) do not
+        last.packet_index = 1 << 60
     elif case == "stream_twice":
         arr[1].stream = arr[0].stream
     elif case == "dense_floor_missing":
@@ -109,16 +137,31 @@ def empty_submit(ctx, io):
 @pytest.mark.parametrize("case,way", [(case, way) for case, (ways, _, _) in CASES.items() for way in ways])
 @pytest.mark.parametrize("shape", list(SHAPES))
 def test_refused_batch_changes_nothing(ctx, oracle, sus, shape, case, way):
+    refused_batch_changes_nothing(ctx, oracle, sus, shape, case, way, HOST)
+
+
+@pytest.mark.parametrize("way", ["decode", "submit", "plan"])
+@pytest.mark.parametrize("case", [case for case in CASES if case.startswith("wrap_")])
+@pytest.mark.parametrize("shape", ["long", "chain", "generic"])
+def test_wrapping_range_refused_in_device_memory(ctx, oracle, sus, shape, case, way):
+    """The wrap refusals with coefficients, dense floors and PCM in device memory, where a wrapped address would be
+    written in place."""
+    refused_batch_changes_nothing(ctx, oracle, sus, shape, case, way, DEVICE)
+
+
+def refused_batch_changes_nothing(ctx, oracle, sus, shape, case, way, memory):
     _, code, message = CASES[case]
     kind, seq_kind, P, ran, extra = SHAPES[shape]
-    rng = np.random.default_rng([list(SHAPES).index(shape), list(CASES).index(case), ["decode", "submit", "plan"].index(way)])
+    rng = np.random.default_rng([list(SHAPES).index(shape), list(CASES).index(case), ["decode", "submit", "plan"].index(way), memory])
     tws = twins(oracle, sus, kind, 2)
-    call = AsyncCall(ctx, rng, [(tw, sequence(rng, seq_kind, P)) for tw in tws], RESIDUE, F32P, HOST,
+    call = AsyncCall(ctx, rng, [(tw, sequence(rng, seq_kind, P)) for tw in tws], RESIDUE, F32P, memory,
                      (ran, ALL_KERNELS - ran - extra))
     if shape == "chain":
         for c in call.chains:
             c.out_offset += 1
-    arr, io = L.api._marshal(call.chains, RESIDUE, HOST, call.coeffs, call.pcm, F32P, call.kinds, call.ys, call.dense, HOST, None)
+    coeffs, pcm = call.arenas()
+    dense = call.kw["dense_floor"] if memory == DEVICE else call.dense
+    arr, io = L.api._marshal(call.chains, RESIDUE, memory, coeffs, pcm, F32P, call.kinds, call.ys, dense, HOST, None)
     t0 = empty_submit(ctx, io)
     keep = break_batch(ctx, call, case, arr, io)
     n = len(call.chains)
