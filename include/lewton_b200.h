@@ -222,6 +222,45 @@ uint32_t lwb_stream_state_len(const lwb_stream *s);
 int lwb_stream_export_state(lwb_stream *s, float *out /* [channels][len] */);
 int lwb_stream_import_state(lwb_stream *s, const float *data /* [channels][len] */, uint32_t len);
 
+/* Many streams' states in one call (added under ABI 3: no struct above changes).  A decode server checkpoints thousands
+ * of streams per step, restores them after LWB_ERR_CUDA, and moves them to another context or GPU; one export / import
+ * per stream costs a synchronisation each.  Slot i names a stream and where its state lies in `buf`.
+ *   Values: slot i of a save holds exactly what lwb_stream_export_state gives for its stream: [channels][len] f32 rows,
+ *     contiguous at buf + offset.  Loading those values gives a stream that decodes every later packet exactly as the
+ *     saved one would (f32 bit for bit, i16 and f16 exactly, on every batch path).  has = 1 with len = 0 is a state (what
+ *     lwb_stream_import_state(s, NULL, 0) makes) and round-trips; has = 0 is PreviousWindowRight::new().
+ *   Ordering: both calls are stream-ordered on lwb_ctx_cuda_stream(ctx), like lwb_submit_chains, and draw *ticket from the
+ *     same sequence.  A save queued after a submit sees the states that submit leaves; a load queued before a submit is
+ *     what that submit starts from.  The host (has, len) of a stream moves at call time, as a submit's does: a save writes
+ *     the slots' len and has before it returns, a load sets the streams' (has, len) and makes prepared batches
+ *     (lwb_plan_execute) plan again.  A save's rows are in `buf` once its ticket completes; a load reads `buf` until its
+ *     ticket completes.
+ *   Memory: LWB_MEM_DEVICE: `buf` is device memory of ctx's device, used in place (any alignment; 16-byte aligned rows of
+ *     a multiple of 4 floats move as float4s).  LWB_MEM_HOST: `buf` must be page-locked at the first and the last byte
+ *     the slots touch, as for a host-memory lwb_submit_chains; pageable memory is refused.  A host-memory call is staged
+ *     in the context's device arenas: a load uploads the extent of its slots (lowest offset to highest end, gaps
+ *     included) in one copy, a save downloads exactly the slots' rows, in one copy when they are adjacent.
+ *   Refusals, before anything changes (no stream state, no slot, no buffer, no ticket):
+ *     LWB_ERR_INVALID: a NULL ctx, buf or ticket (slots may be NULL when n == 0), a bad memory space, a slot without a
+ *       stream or with a stream of another context, a stream in two slots, a load slot with has == 0 and len != 0,
+ *       host memory that is not page-locked;
+ *     LWB_ERR_BUFFER: a load slot's len above blocksize_1 / 2 of its stream's setup, or a slot whose range
+ *       (offset + channels * len elements, in bytes) would wrap past 2^64.
+ *   Across contexts: a buffer saved by one context may be loaded by another, on the same or another device (moving the
+ *     bytes between devices is the caller's).  Nothing orders the two contexts' streams: the caller waits on the save's
+ *     ticket before it queues the load.  The load reads `channels` rows of len floats per slot, channels of the loading
+ *     stream's setup, so the two streams need equal channel counts; their setups need only len <= blocksize_1 / 2 of the
+ *     loading one, the rule of lwb_stream_import_state. */
+typedef struct lwb_state_slot {
+    lwb_stream *stream;
+    uint64_t offset;     /* element offset of this stream's [channels][len] f32 rows in `buf`                     */
+    uint32_t len;        /* save: written (lwb_stream_state_len); load: read, <= blocksize_1 / 2                  */
+    uint8_t has;         /* save: written (!lwb_stream_is_empty); load: read (0 = PreviousWindowRight::new())     */
+    uint8_t reserved[3];
+} lwb_state_slot;
+int lwb_streams_save(lwb_ctx *ctx, lwb_state_slot *slots, size_t n, int memory, float *buf, uint64_t *ticket);
+int lwb_streams_load(lwb_ctx *ctx, const lwb_state_slot *slots, size_t n, int memory, const float *buf, uint64_t *ticket);
+
 /* audio::get_decoded_sample_count (audio.rs:874-909) for an already-parsed packet header:
  * right_win_start - left_win_start; does not look at the stream state. */
 int lwb_decoded_sample_count(const lwb_setup *setup, uint8_t mode_number, int prev_window_flag,

@@ -92,6 +92,10 @@ class BatchIo(C.Structure):
                 ("vq_runs", vp), ("vq_run_offsets", vp), ("vq_entries", vp), ("vq_entry_offsets", vp), ("floor_memory", C.c_int)]
 
 
+class StateSlot(C.Structure):
+    _fields_ = [("stream", vp), ("offset", C.c_uint64), ("len", C.c_uint32), ("has", C.c_uint8), ("reserved", C.c_uint8 * 3)]
+
+
 # name -> (restype, argtypes); every symbol include/lewton_b200.h declares
 SYMBOLS = {
     "lwb_abi_version": (C.c_int, []),
@@ -124,6 +128,8 @@ SYMBOLS = {
     "lwb_stream_state_len": (C.c_uint32, [vp]),
     "lwb_stream_export_state": (C.c_int, [vp, vp]),
     "lwb_stream_import_state": (C.c_int, [vp, vp, C.c_uint32]),
+    "lwb_streams_save": (C.c_int, [vp, C.POINTER(StateSlot), C.c_size_t, C.c_int, vp, C.POINTER(C.c_uint64)]),
+    "lwb_streams_load": (C.c_int, [vp, C.POINTER(StateSlot), C.c_size_t, C.c_int, vp, C.POINTER(C.c_uint64)]),
     "lwb_decoded_sample_count": (C.c_int, [vp, C.c_uint8, C.c_int, C.c_int, C.POINTER(C.c_uint32)]),
     "lwb_decode_packet": (C.c_int, [vp, C.POINTER(Packet), C.c_int, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
     "lwb_decode_spectrum": (C.c_int, [vp, C.c_uint8, C.c_int, C.c_int, vp, C.c_int, vp, C.c_size_t,

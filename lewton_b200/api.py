@@ -97,6 +97,33 @@ class Context:
         self.check(cabi.lib().lwb_submit_chains(self._h, arr, len(chains), C.byref(io), C.byref(t)))
         return Ticket(self, t.value, chains, arr, (coeffs, pcm, floor_kind, floor1_y, dense_floor, vq, io))
 
+    def save_states(self, pwrs, buf, memory=cabi.MEM_DEVICE, offsets=None):
+        """lwb_streams_save: queues copies of the states of streams `pwrs` into `buf` and returns (slots, Ticket) at once.
+        Slot i (StateSlot) holds stream i's (has, len), known now, and its element offset; its [channels][len] f32 rows are
+        in buf at that offset once the ticket is done.  buf: a page-locked numpy array (MEM_HOST, host_alloc) or device
+        memory of this context's device (MEM_DEVICE: an integer pointer or a torch tensor).  offsets: the slots' element
+        offsets, default state_offsets(pwrs) (back to back, as the states stand after every batch queued so far)."""
+        pwrs = list(pwrs)
+        if offsets is None:
+            offsets = state_offsets(pwrs)[0]
+        slots = [StateSlot(p, o) for p, o in zip(pwrs, offsets, strict=True)]
+        arr = _slot_array(slots)
+        t = C.c_uint64()
+        self.check(cabi.lib().lwb_streams_save(self._h, arr, len(slots), memory, _addr(buf), C.byref(t)))
+        for sl, a in zip(slots, arr):
+            sl.len, sl.has = int(a.len), bool(a.has)
+        return slots, Ticket(self, t.value, [], None, (buf, arr))
+
+    def load_states(self, slots, buf, memory=cabi.MEM_DEVICE):
+        """lwb_streams_load: queues copies of the states `slots` describe from `buf` into their streams (StateSlot.pwr, of
+        this context) and returns the Ticket at once; batches queued afterwards start from them.  buf as for save_states,
+        unchanged until the ticket is done.  A buffer another context saved is waited for (its save ticket) first."""
+        slots = list(slots)
+        arr = _slot_array(slots)
+        t = C.c_uint64()
+        self.check(cabi.lib().lwb_streams_load(self._h, arr, len(slots), memory, _addr(buf), C.byref(t)))
+        return Ticket(self, t.value, [], None, (buf, arr))
+
     def close(self):
         if self._h:
             # readers (frontend.OggStreamReader) own streams and setups of their own: they go first
@@ -333,6 +360,50 @@ class PreviousWindowRight:
             self.close()
         except Exception:
             pass
+
+
+class StateSlot:
+    """One stream's state in a state buffer (lwb_state_slot): [channels][len] f32 rows at element `offset`; has False is
+    the empty state of PreviousWindowRight::new().  Context.save_states fills len and has; Context.load_states reads them
+    into `pwr`."""
+
+    def __init__(self, pwr, offset, len=0, has=False):
+        self.pwr, self.offset, self.len, self.has = pwr, int(offset), int(len), bool(has)
+
+    def __repr__(self):
+        return f"StateSlot(offset={self.offset}, len={self.len}, has={self.has})"
+
+
+def state_offsets(pwrs, lengths=None):
+    """Element offsets that lay the states of streams `pwrs` out back to back in one state buffer, each starting at a
+    multiple of 4 floats (so the copies move float4s), and the buffer's size in elements: (offsets, total).
+    lengths: the state length of each stream; by default its len() now, which is what a save queued now writes.  Pass
+    blocksize_1 // 2 of each stream's setup for a layout that holds any state the streams may have later."""
+    pwrs = list(pwrs)
+    lengths = [len(p) for p in pwrs] if lengths is None else [int(n) for n in lengths]
+    offsets, total = [], 0
+    for p, n in zip(pwrs, lengths, strict=True):
+        offsets.append(total)
+        total += (p.setup.audio_channels * n + 3) // 4 * 4
+    return offsets, total
+
+
+def _slot_array(slots):
+    arr = (cabi.StateSlot * len(slots))()
+    for a, sl in zip(arr, slots):
+        a.stream, a.offset, a.len, a.has = sl.pwr._h, sl.offset, sl.len, int(sl.has)
+    return arr
+
+
+def _addr(x):
+    """The address of an arena: a numpy array's data, a torch tensor's data_ptr(), or an integer pointer (None: NULL)."""
+    if x is None:
+        return None
+    if isinstance(x, np.ndarray):
+        return x.ctypes.data
+    if hasattr(x, "data_ptr"):
+        return x.data_ptr()
+    return int(x)
 
 
 class Floor0Record:
@@ -601,7 +672,7 @@ class Ticket:
         return True
 
     def wait(self):
-        """lwb_ticket_wait; returns the chains with their results."""
+        """lwb_ticket_wait; returns the chains with their results (none for a save_states or load_states ticket)."""
         if self._keep is not None:
             self.ctx.check(cabi.lib().lwb_ticket_wait(self.ctx._h, self.id))
             self._keep = None
@@ -622,13 +693,7 @@ def _marshal(chains, entry, memory, coeffs, pcm, out_format, floor_kind, floor1_
         arr[i].coeff_offset, arr[i].packet_index = c.coeff_offset, c.packet_index
         arr[i].out_offset, arr[i].out_stride = c.out_offset, c.out_stride
 
-    def addr(x):
-        if x is None:
-            return None
-        if isinstance(x, np.ndarray):
-            return x.ctypes.data
-        return int(x)
-
+    addr = _addr
     io = cabi.BatchIo()
     io.entry, io.memory, io.out_format = entry, memory, out_format
     io.coeffs, io.pcm, io.dense_floor = addr(coeffs), addr(pcm), addr(dense_floor)

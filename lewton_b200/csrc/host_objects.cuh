@@ -60,6 +60,7 @@ struct lwb_ctx {
     // grow-only device arenas
     DevBuf spec, segtab, magic, x, desc, chains, ticket, cdesc, cbytes;
     DevBuf floor0;                 // floor-0 curves of LWB_FLOOR_ZERO rows (k_floor0_curves), laid out like spec
+    DevBuf state_rows;             // RowCopy descriptors of lwb_streams_save / lwb_streams_load, in compute-stream order
     ArenaSet host_sets[kHostSets]; // host-memory batches, in turn
     int host_next = 0;
     ArenaSet ordered;              // in compute-stream order: device-memory batches' host floor arrays, the debug taps
@@ -91,7 +92,8 @@ struct lwb_setup {
     unsigned out_channels() const { return host.n_out ? host.n_out : channels; }
 };
 
-struct RowCopy { const float *src; float *dst; uint32_t n4, pad; };  // n4 float4s, copied in front of the round's kernels
+// One row for k_row_copy: n float4s, or with `scalar` set n floats (rows of any alignment and length)
+struct RowCopy { const float *src; float *dst; uint32_t n, scalar; };
 struct ChainShape { unsigned warps; size_t smem; int n1max, wpc, np; };     // k_chain's block and shared memory
 
 // One launch of a batch path (run_steps, path_generic.cuh): the kernel's LWB_KERNEL_* id, a device pointer to its

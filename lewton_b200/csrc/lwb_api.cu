@@ -113,7 +113,7 @@ extern "C" void lwb_ctx_destroy(lwb_ctx *ctx)
     cudaSetDevice(ctx->device);
     sync_all_streams(ctx);
     for (DevBuf *b : {&ctx->spec, &ctx->segtab, &ctx->magic, &ctx->x, &ctx->desc, &ctx->chains, &ctx->ticket, &ctx->runs_buf[0],
-                      &ctx->runs_buf[1], &ctx->cdesc, &ctx->cbytes, &ctx->floor0})
+                      &ctx->runs_buf[1], &ctx->cdesc, &ctx->cbytes, &ctx->floor0, &ctx->state_rows})
         if (b->p) cudaFree(b->p);
     auto free_set = [](ArenaSet &s) {
         for (DevBuf *b : {&s.coeffs, &s.dense, &s.pcm, &s.kinds, &s.ys, &s.vqoff, &s.vqrec})
@@ -835,6 +835,151 @@ extern "C" int lwb_ticket_wait(lwb_ctx *ctx, uint64_t ticket)
     if (!ctx || ticket == 0 || ticket > ctx->tickets_issued) return LWB_ERR_INVALID;
     CU(ctx, cudaSetDevice(ctx->device));
     return retire_tickets(ctx, ticket, true);
+}
+
+// ---------------------------------------------------------------------------------------------
+// many streams' states (lwb_streams_save / lwb_streams_load)
+// ---------------------------------------------------------------------------------------------
+// The state length slot `sl` moves: the stream's at call time for a save, the slot's for a load.
+static uint32_t slot_len(const lwb_state_slot &sl, bool load)
+{
+    return load ? sl.len : (sl.stream->has ? sl.stream->plen : 0);
+}
+
+// Every refusal of a save or a load, before anything changes, and the element extent [*lo, *hi) of the slots' rows
+// (empty: *hi <= *lo).  A slot's range must end inside the 64-bit address space in bytes, as chain_ranges_fit asks of a
+// chain's ranges.
+static int check_state_slots(lwb_ctx *ctx, const lwb_state_slot *slots, size_t n, int memory, const float *buf, const uint64_t *ticket,
+                             bool load, uint64_t *lo, uint64_t *hi)
+{
+    if (!ctx) return LWB_ERR_INVALID;
+    if ((!slots && n) || !buf || !ticket) return fail(ctx, LWB_ERR_INVALID, "streams_save / streams_load: a NULL argument");
+    if (memory != LWB_MEM_HOST && memory != LWB_MEM_DEVICE) return fail(ctx, LWB_ERR_INVALID, "bad memory space");
+    const uint64_t epoch = ++ctx->epoch;
+    *lo = ~0ull;
+    *hi = 0;
+    for (size_t i = 0; i < n; i++) {
+        const lwb_state_slot &sl = slots[i];
+        lwb_stream *s = sl.stream;
+        if (!s || s->ctx != ctx) return fail(ctx, LWB_ERR_INVALID, "slot: no stream, or a stream of another context");
+        if (s->busy_epoch == epoch) return fail(ctx, LWB_ERR_INVALID, "a stream appears in two slots");
+        s->busy_epoch = epoch;
+        if (load && !sl.has && sl.len) return fail(ctx, LWB_ERR_INVALID, "slot: has == 0 with len != 0");
+        if (load && sl.len > state_stride(s->setup)) return fail(ctx, LWB_ERR_BUFFER, "slot: len above blocksize_1 / 2 of the stream's setup");
+        const uint64_t len = slot_len(sl, load);
+        uint64_t end, bytes;
+        if (__builtin_add_overflow(sl.offset, (uint64_t)s->setup->channels * len, &end) || __builtin_mul_overflow(end, (uint64_t)sizeof(float), &bytes))
+            return fail(ctx, LWB_ERR_BUFFER, "slot: its range does not fit in 64 bits");
+        if (!len) continue;
+        *lo = std::min(*lo, sl.offset);
+        *hi = std::max(*hi, end);
+    }
+    if (memory != LWB_MEM_HOST || *hi <= *lo) return LWB_OK;
+    CU(ctx, cudaSetDevice(ctx->device));
+    if (!page_locked(buf, *lo, *hi, sizeof(float)))
+        return fail(ctx, LWB_ERR_INVALID, "host-memory streams_save / streams_load: buf is not page-locked (lwb_host_alloc, cudaHostAlloc or cudaHostRegister)");
+    return LWB_OK;
+}
+
+// Queues one k_row_copy launch over the (slot, channel) rows of nonzero length: stream state row c <-> dev + offset - base
+// + c * len.  Its descriptors go through the staging ring like a batch's.
+static int queue_state_rows(lwb_ctx *ctx, const lwb_state_slot *slots, size_t n, float *dev, uint64_t base, bool load)
+{
+    size_t rows = 0;
+    for (size_t i = 0; i < n; i++)
+        if (slot_len(slots[i], load)) rows += slots[i].stream->setup->channels;
+    if (!rows) return LWB_OK;
+    Staging *st;
+    int rc;
+    if ((rc = acquire_staging(ctx, rows * sizeof(RowCopy), &st)) || (rc = ensure(ctx, ctx->state_rows, rows * sizeof(RowCopy)))) return rc;
+    RowCopy *h = (RowCopy *)st->h;
+    size_t k = 0;
+    for (size_t i = 0; i < n; i++) {
+        const lwb_stream *s = slots[i].stream;
+        const uint32_t len = slot_len(slots[i], load);
+        for (unsigned c = 0; len && c < s->setup->channels; c++) {
+            float *row = s->d_state + (size_t)c * state_stride(s->setup), *b = dev + (slots[i].offset - base) + (uint64_t)c * len;
+            const float *src = load ? b : row;
+            float *dst = load ? row : b;
+            const bool vec = len % 4 == 0 && ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0;
+            h[k++] = RowCopy{src, dst, vec ? len / 4 : len, vec ? 0u : 1u};
+        }
+    }
+    if ((rc = upload_staging(ctx, st, h, ctx->state_rows.p, rows * sizeof(RowCopy), ctx->stream))) return rc;
+    return run_steps(ctx, StepArgs(), std::vector<Step>(1, Step{LWB_KERNEL_ROW_COPY, ctx->state_rows.p, rows, nullptr}));
+}
+
+// A save (load == false) or a load, queued on the compute stream with its ticket.  Host memory is staged in the next host
+// arena set, which the set's previous user releases on the GPU (ArenaSet::done) and this call's ticket releases in turn.
+// slots_w: the save's slots, written once the work is queued (nullptr for a load).
+static int move_states(lwb_ctx *ctx, bool load, lwb_state_slot *slots_w, const lwb_state_slot *slots, size_t n, int memory, float *buf,
+                       uint64_t *ticket)
+{
+    uint64_t lo, hi;
+    int rc = check_state_slots(ctx, slots, n, memory, buf, ticket, load, &lo, &hi);
+    if (rc) return rc;
+    CU(ctx, cudaSetDevice(ctx->device));
+    ArenaSet *set = nullptr;
+    if (memory == LWB_MEM_DEVICE || hi <= lo) {
+        if ((rc = queue_state_rows(ctx, slots, n, buf, 0, load))) return rc;
+    } else {
+        set = &ctx->host_sets[ctx->host_next];
+        ctx->host_next = (ctx->host_next + 1) % kHostSets;
+        const size_t bytes = (size_t)(hi - lo) * sizeof(float);
+        if ((rc = ensure(ctx, set->coeffs, bytes, set->done))) return rc;
+        CU(ctx, cudaStreamWaitEvent(ctx->stream, set->done, 0));
+        float *stage = (float *)set->coeffs.p;
+        if (load) CU(ctx, cudaMemcpyAsync(stage, buf + lo, bytes, cudaMemcpyHostToDevice, ctx->stream));
+        rc = queue_state_rows(ctx, slots, n, stage, lo, load);
+        if (!rc && !load) {       // exactly the slots' rows go home: the gaps between them are the caller's
+            std::vector<PcmSpan> spans;
+            std::vector<PcmCopy> copies;
+            for (size_t i = 0; i < n; i++)
+                if (const uint32_t len = slot_len(slots[i], false)) spans.push_back(PcmSpan{slots[i].offset, (uint64_t)slots[i].stream->setup->channels * len});
+            plan_pcm_copies(spans, (uint64_t)INT32_MAX / sizeof(float), copies);
+            for (const PcmCopy &cp : copies) {
+                float *dst = buf + cp.off;
+                const float *src = stage + (cp.off - lo);
+                cudaError_t e = cp.height == 1 ? cudaMemcpyAsync(dst, src, cp.width * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream)
+                                               : cudaMemcpy2DAsync(dst, cp.pitch * sizeof(float), src, cp.pitch * sizeof(float), cp.width * sizeof(float),
+                                                                   cp.height, cudaMemcpyDeviceToHost, ctx->stream);
+                if (e != cudaSuccess) {
+                    rc = fail(ctx, LWB_ERR_CUDA, "streams_save: copy to host", e);
+                    break;
+                }
+            }
+        }
+        if (rc) {               // the set's next user still waits behind whatever this call queued
+            cudaEventRecord(set->done, ctx->stream);
+            cudaGetLastError();
+            return rc;
+        }
+    }
+    if ((rc = issue_ticket(ctx, set))) return rc;
+    *ticket = ctx->tickets_issued;
+    for (size_t i = 0; i < n; i++) {
+        lwb_stream *s = slots[i].stream;
+        if (load) {
+            s->has = slots[i].has != 0;
+            s->plen = slots[i].len;
+        } else {
+            slots_w[i].len = slot_len(slots[i], false);
+            slots_w[i].has = s->has ? 1 : 0;
+        }
+    }
+    if (load) ctx->state_gen++;     // contents changed even where the shape did not: prepared batches plan again
+    return LWB_OK;
+}
+
+extern "C" int lwb_streams_save(lwb_ctx *ctx, lwb_state_slot *slots, size_t n, int memory, float *buf, uint64_t *ticket)
+{
+    return move_states(ctx, false, slots, slots, n, memory, buf, ticket);
+}
+
+extern "C" int lwb_streams_load(lwb_ctx *ctx, const lwb_state_slot *slots, size_t n, int memory, const float *buf, uint64_t *ticket)
+{
+    // (a load only reads buf: move_states writes through it on a save alone)
+    return move_states(ctx, true, nullptr, slots, n, memory, const_cast<float *>(buf), ticket);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -33,11 +33,16 @@ static ChainShape chain_shape(unsigned maxc, int n1max, bool residue, bool vq = 
 
 // One block per row: the stream state the first segment of a chain starts from, moved out of the way of the segment of
 // the same chain that ends the batch -- in the one-pass schedule (path_mixed.cuh) that one may store the new state before
-// the first one has read the old.
+// the first one has read the old; and the state rows lwb_streams_save / lwb_streams_load move, whose offsets in the
+// caller's buffer may leave a row unaligned or of a length that is not a multiple of 4 (the scalar form).
 __global__ void k_row_copy(const RowCopy *__restrict__ rc)
 {
     const RowCopy c = rc[blockIdx.x];
-    for (uint32_t i = threadIdx.x; i < c.n4; i += blockDim.x)
+    if (c.scalar) {
+        for (uint32_t i = threadIdx.x; i < c.n; i += blockDim.x) c.dst[i] = c.src[i];
+        return;
+    }
+    for (uint32_t i = threadIdx.x; i < c.n; i += blockDim.x)
         reinterpret_cast<float4 *>(c.dst)[i] = reinterpret_cast<const float4 *>(c.src)[i];
 }
 

@@ -76,3 +76,60 @@ def gather_streams(local_tensor, root_tensor, n_streams, root=0):
         lo, hi = stream_range(n_streams, world, rank)
         if hi > lo:
             _p2p([dist.P2POp(dist.isend, local_tensor, root)])
+
+
+def migrate_streams(ctx, src, dst, pwrs=(), setups=()):
+    """Moves live streams from rank `src` to rank `dst` mid-decode, without a gap or a changed sample: a long-lived server
+    rebalances its ranks, or hands a context's streams over before it goes.  Both ranks call it; any other rank returns []
+    at once.  ctx: this rank's Context.
+      src: pwrs are the streams to move, in order, called after the batches that decoded them so far have been queued.
+        Their states are saved in one call (Context.save_states) and waited for; the streams may be closed afterwards.
+        Returns [].
+      dst: setups holds one Setup of ctx per stream, in the same order, each with the channel count of the stream it
+        receives and a blocksize_1 whose half holds its state.  Returns the new streams, loaded (Context.load_states): the
+        next batch queued on ctx decodes from them exactly as the source streams would have.
+    The state buffer crosses with its slot metadata in grouped point-to-point transfers, as scatter_streams' rows do: in
+    device memory over NCCL, in page-locked host memory over gloo."""
+    import numpy as np
+    import torch
+    import torch.distributed as dist
+
+    from . import _cabi as cabi
+    from .api import PreviousWindowRight, StateSlot, state_offsets
+    rank = dist.get_rank()
+    if rank not in (src, dst) or src == dst:
+        return []
+    nccl = dist.get_backend() == "nccl"
+    dev = torch.device("cuda", ctx.device) if nccl else torch.device("cpu")
+    memory = cabi.MEM_DEVICE if nccl else cabi.MEM_HOST
+
+    def state_buffer(n):
+        if nccl:
+            return torch.empty(max(n, 1), dtype=torch.float32, device=dev)
+        return torch.from_numpy(ctx.host_alloc(max(n, 1), np.float32))
+
+    if rank == src:
+        pwrs = list(pwrs)
+        offsets, total = state_offsets(pwrs)
+        buf = state_buffer(total)
+        slots, ticket = ctx.save_states(pwrs, buf, memory, offsets)
+        ticket.wait()                         # the transfers below run on torch's streams, not on ctx's
+        meta = torch.tensor([[s.offset, s.len, int(s.has)] for s in slots] or [[0, 0, 0]], dtype=torch.int64, device=dev)
+        _p2p([dist.P2POp(dist.isend, torch.tensor([len(slots), total], dtype=torch.int64, device=dev), dst)])
+        _p2p([dist.P2POp(dist.isend, meta, dst), dist.P2POp(dist.isend, buf, dst)])
+        return []
+    setups = list(setups)
+    head = torch.zeros(2, dtype=torch.int64, device=dev)
+    _p2p([dist.P2POp(dist.irecv, head, src)])
+    n, total = (int(v) for v in head.tolist())
+    if n != len(setups):
+        raise ValueError(f"migrate_streams: rank {src} sends {n} streams, rank {dst} has {len(setups)} setups for them")
+    meta = torch.zeros((max(n, 1), 3), dtype=torch.int64, device=dev)
+    buf = state_buffer(total)
+    _p2p([dist.P2POp(dist.irecv, meta, src), dist.P2POp(dist.irecv, buf, src)])
+    if nccl:
+        torch.cuda.current_stream(dev).synchronize()      # the load runs on ctx's stream
+    new = [PreviousWindowRight(su) for su in setups]
+    slots = [StateSlot(p, o, ln, h) for p, (o, ln, h) in zip(new, meta.tolist())]
+    ctx.load_states(slots, buf, memory).wait()
+    return new
