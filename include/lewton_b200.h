@@ -217,6 +217,34 @@ int lwb_stream_reset(lwb_stream *s);
 int lwb_stream_is_empty(const lwb_stream *s);
 /* #[derive(Clone)]: an independent copy of the state */
 int lwb_stream_clone(const lwb_stream *s, lwb_stream **out);
+/* Output window of a stream (added under ABI 3: no struct or existing call changes).  Of the samples its packets produce
+ * from the next queued packet on, the first `skip` per channel are not written, the next `limit` are, and none after
+ * that (limit = UINT64_MAX: no end).  Decoding and the stream state are unchanged: every packet still decodes and
+ * advances PreviousWindowRight exactly as without a window.  skip = 0, limit = UINT64_MAX is the default and is what
+ * every existing caller gets.  It is how a caller gets lewton's sample count at the end of a stream (the last packet
+ * truncated to the page's granule position, inside_ogg.rs:219-222) and sample-exact starts after a seek, without a pass
+ * of its own over the PCM.
+ *   Placement: written sample j of a chain (0-based among the written ones) goes to out_offset + k * out_stride + j
+ *     (planar) or to out_offset + j * K + k (interleaved), K = lwb_setup_output_channels.  lwb_chain.n_samples is the
+ *     number of samples written, and the out_stride and range checks of a batch use that number.  Nothing outside the
+ *     written set changes, in either memory space.
+ *   When it moves: the counters advance where the stream state's (has, len) does -- when a batch is queued, at call
+ *     time, for lwb_decode_chains, lwb_submit_chains and lwb_plan_execute alike -- so consecutive submits, and windows
+ *     that span several batches, behave as one stream.  A refused batch moves no counter; after LWB_ERR_CUDA the counters
+ *     are handled like the states: not committed on the host.
+ *   lwb_stream_reset leaves the window alone (a seek is a reset followed by lwb_stream_set_window); lwb_stream_clone
+ *   copies it; lwb_streams_save / lwb_streams_load do not carry it (the slot format is fixed).  Setting a window makes
+ *   prepared batches that hold the stream plan again; lwb_plan_execute replays a prepared batch only while none of its
+ *   streams has a window other than the default, so a stream whose limit has run out to 0 keeps its batches planning
+ *   every execution until lwb_stream_set_window(s, 0, UINT64_MAX).  lwb_decode_packet and lwb_decode_spectrum honour
+ *   the window too.
+ *   Memory: a clipped chain decodes its full output into scratch first.  Host-memory batches stage it beside their PCM;
+ *   device-memory batches keep it in a device buffer of the context that grows to the largest batch's clipped output
+ *   (all chains of a batch clipped: about the size of its PCM) and is freed with the context.
+ *   A NULL stream is refused with LWB_ERR_INVALID. */
+int lwb_stream_set_window(lwb_stream *s, uint64_t skip, uint64_t limit);
+/* what is left of the window: skip still to drop, limit still to write (UINT64_MAX: no end); either pointer may be NULL */
+int lwb_stream_window(const lwb_stream *s, uint64_t *skip_left, uint64_t *limit_left);
 /* debug / checkpoint: per-channel length of the saved right half (0 if empty), and its data */
 uint32_t lwb_stream_state_len(const lwb_stream *s);
 int lwb_stream_export_state(lwb_stream *s, float *out /* [channels][len] */);
@@ -369,7 +397,8 @@ typedef struct lwb_chain {
     uint64_t out_offset;              /* element offset of the chain's PCM in `pcm`                 */
     uint64_t out_stride;              /* planar: elements between channel planes (>= total samples)*/
     /* results */
-    uint32_t n_samples;               /* samples per channel produced by this chain                */
+    uint32_t n_samples;               /* samples per channel written by this chain (produced, less what the stream's
+                                       * window, lwb_stream_set_window, leaves out)                 */
     uint32_t packets_done;            /* == n_packets unless status != 0                           */
     int32_t status;                   /* LWB_OK or the error of packet `packets_done`              */
 } lwb_chain;

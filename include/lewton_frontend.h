@@ -154,7 +154,7 @@ typedef struct lwf_stream_job {
     uint64_t out_offset;              /* element offset of this stream's PCM in `pcm`                */
     uint64_t out_stride;              /* planar formats: elements between channel planes             */
     /* results */
-    uint32_t n_samples;               /* samples per channel produced                                */
+    uint32_t n_samples;               /* samples per channel written (less what the stream window, lwb_stream_set_window, drops) */
     uint32_t packets_done;            /* packets synthesised (== n_packets unless status != 0)       */
     int32_t status;                   /* LWB_OK, or the error of packet `packets_done`               */
 } lwf_stream_job;

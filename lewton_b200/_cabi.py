@@ -125,6 +125,8 @@ SYMBOLS = {
     "lwb_stream_reset": (C.c_int, [vp]),
     "lwb_stream_is_empty": (C.c_int, [vp]),
     "lwb_stream_clone": (C.c_int, [vp, C.POINTER(vp)]),
+    "lwb_stream_set_window": (C.c_int, [vp, C.c_uint64, C.c_uint64]),
+    "lwb_stream_window": (C.c_int, [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "lwb_stream_state_len": (C.c_uint32, [vp]),
     "lwb_stream_export_state": (C.c_int, [vp, vp]),
     "lwb_stream_import_state": (C.c_int, [vp, vp, C.c_uint32]),

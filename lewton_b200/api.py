@@ -309,6 +309,9 @@ class Setup:
             pass
 
 
+NO_LIMIT = (1 << 64) - 1      # lwb_stream_set_window: a window without an end
+
+
 class PreviousWindowRight:
     """audio.rs:847-861 -- the only inter-packet state, resident on the device (lwb_stream)."""
 
@@ -333,6 +336,23 @@ class PreviousWindowRight:
         h = C.c_void_p()
         self.setup.ctx.check(cabi.lib().lwb_stream_clone(self._h, C.byref(h)))
         return PreviousWindowRight(self.setup, h)
+
+    def set_window(self, skip=0, limit=None):
+        """Output window (lwb_stream_set_window): of the samples the next packets produce, drop the first `skip` per
+        channel, write the next `limit` (None: no end) and none after them.  The state advances as without a window;
+        reset() leaves the window alone, so a seek is reset() then set_window(skip).  Batches report the samples
+        written."""
+        limit = NO_LIMIT if limit is None else int(limit)
+        if skip < 0 or not 0 <= limit <= NO_LIMIT:
+            raise ValueError("skip and limit must be >= 0 (limit None: no end)")
+        self.setup.ctx.check(cabi.lib().lwb_stream_set_window(self._h, int(skip), limit))
+
+    @property
+    def window(self):
+        """What is left of the window: (skip still to drop, limit still to write or None for no end)."""
+        skip, limit = C.c_uint64(), C.c_uint64()
+        self.setup.ctx.check(cabi.lib().lwb_stream_window(self._h, C.byref(skip), C.byref(limit)))
+        return skip.value, None if limit.value == NO_LIMIT else limit.value
 
     def __len__(self):
         return cabi.lib().lwb_stream_state_len(self._h)

@@ -51,6 +51,7 @@ struct lwb_ctx {
     uint32_t ticket_next = 0;
     uint64_t epoch = 0;            // batch counter: lwb_stream::busy_epoch == epoch <=> the stream already sits in this batch
     uint64_t state_gen = 1;        // bumped whenever any stream's (has, len) changes: plans key on it
+    bool windows_set = false;      // lwb_stream_set_window has been called on a stream of this ctx
     std::string err;
     uint64_t launches = 0;
     uint64_t kernel_launches[LWB_KERNEL_COUNT] = {};   // per LWB_KERNEL_* id; they sum to `launches`
@@ -60,7 +61,8 @@ struct lwb_ctx {
     // grow-only device arenas
     DevBuf spec, segtab, magic, x, desc, chains, ticket, cdesc, cbytes;
     DevBuf floor0;                 // floor-0 curves of LWB_FLOOR_ZERO rows (k_floor0_curves), laid out like spec
-    DevBuf state_rows;             // RowCopy descriptors of lwb_streams_save / lwb_streams_load, in compute-stream order
+    DevBuf state_rows;             // RowCopy descriptors, in compute-stream order: lwb_streams_save / load, clipped chains
+    DevBuf win;                    // device-memory batches: the full output of their clipped chains (BatchWalk::clip)
     ArenaSet host_sets[kHostSets]; // host-memory batches, in turn
     int host_next = 0;
     ArenaSet ordered;              // in compute-stream order: device-memory batches' host floor arrays, the debug taps
@@ -92,8 +94,9 @@ struct lwb_setup {
     unsigned out_channels() const { return host.n_out ? host.n_out : channels; }
 };
 
-// One row for k_row_copy: n float4s, or with `scalar` set n floats (rows of any alignment and length)
-struct RowCopy { const float *src; float *dst; uint32_t n, scalar; };
+// One row for k_row_copy: `bytes` (even) from src to dst, both 2-byte aligned (rows of any sample type and alignment)
+struct RowCopy { const void *src; void *dst; uint64_t bytes; };
+constexpr int kRowCopyThreads = 256;
 struct ChainShape { unsigned warps; size_t smem; int n1max, wpc, np; };     // k_chain's block and shared memory
 
 // One launch of a batch path (run_steps, path_generic.cuh): the kernel's LWB_KERNEL_* id, a device pointer to its
@@ -162,6 +165,8 @@ struct lwb_stream {
     bool has = false;              // PreviousWindowRight.data.is_some()
     uint32_t plen = 0;             // per-channel length of the saved right half
     uint64_t busy_epoch = 0;       // guards against one stream appearing twice in a batch
+    uint64_t skip_left = 0;        // the output window (lwb_stream_set_window): samples still to drop ...
+    uint64_t limit_left = ~0ull;   // ... and still to write after them (~0: no end)
 };
 
 // Records the launches a path made for a prepared batch; lwb_plan_execute replays them while ctx->state_gen == gen.

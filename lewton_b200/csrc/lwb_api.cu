@@ -113,7 +113,7 @@ extern "C" void lwb_ctx_destroy(lwb_ctx *ctx)
     cudaSetDevice(ctx->device);
     sync_all_streams(ctx);
     for (DevBuf *b : {&ctx->spec, &ctx->segtab, &ctx->magic, &ctx->x, &ctx->desc, &ctx->chains, &ctx->ticket, &ctx->runs_buf[0],
-                      &ctx->runs_buf[1], &ctx->cdesc, &ctx->cbytes, &ctx->floor0, &ctx->state_rows})
+                      &ctx->runs_buf[1], &ctx->cdesc, &ctx->cbytes, &ctx->floor0, &ctx->state_rows, &ctx->win})
         if (b->p) cudaFree(b->p);
     auto free_set = [](ArenaSet &s) {
         for (DevBuf *b : {&s.coeffs, &s.dense, &s.pcm, &s.kinds, &s.ys, &s.vqoff, &s.vqrec})
@@ -604,6 +604,22 @@ extern "C" int lwb_stream_reset(lwb_stream *s)
     set_stream_state(s, false, 0);
     return LWB_OK;
 }
+extern "C" int lwb_stream_set_window(lwb_stream *s, uint64_t skip, uint64_t limit)
+{
+    if (!s) return LWB_ERR_INVALID;
+    s->skip_left = skip;
+    s->limit_left = limit;
+    s->ctx->windows_set = true;
+    s->ctx->state_gen++;           // prepared batches holding the stream plan again
+    return LWB_OK;
+}
+extern "C" int lwb_stream_window(const lwb_stream *s, uint64_t *skip_left, uint64_t *limit_left)
+{
+    if (!s) return LWB_ERR_INVALID;
+    if (skip_left) *skip_left = s->skip_left;
+    if (limit_left) *limit_left = s->limit_left;
+    return LWB_OK;
+}
 extern "C" int lwb_stream_is_empty(const lwb_stream *s) { return (!s || !s->has) ? 1 : 0; }
 extern "C" uint32_t lwb_stream_state_len(const lwb_stream *s) { return (s && s->has) ? s->plen : 0; }
 
@@ -614,6 +630,8 @@ extern "C" int lwb_stream_clone(const lwb_stream *s, lwb_stream **out)
     if (rc) return rc;
     (*out)->has = s->has;
     (*out)->plen = s->plen;
+    (*out)->skip_left = s->skip_left;
+    (*out)->limit_left = s->limit_left;
     lwb_ctx *ctx = s->ctx;
     CU(ctx, cudaMemcpyAsync((*out)->d_state, s->d_state,
                             s->setup->channels * state_stride(s->setup) * sizeof(float),
@@ -710,7 +728,8 @@ static int check_batch_args(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chai
     return LWB_OK;
 }
 
-// Whether the ranges chain c's walk w touches end inside the 64-bit address space, in bytes: its PCM write set, its
+// Whether the ranges chain c's walk w touches end inside the 64-bit address space, in bytes: its PCM write set (the
+// samples it writes, w.written), its
 // coefficient (and dense floor) elements and, for the residue entries, its packet rows of floor1_y, the widest per-row
 // array.  BatchExtent::add and the run descriptors sum these offsets in uint64_t; an offset near 2^64 would wrap to a
 // small one and address memory the caller never named.
@@ -720,8 +739,8 @@ static bool chain_ranges_fit(const lwb_batch_io *io, const lwb_chain *c, const C
     const uint64_t K = su->out_channels(), esz = out_format_of(io->out_format).esz;
     uint64_t span, end;
     if (out_format_of(io->out_format).planar) {
-        if (__builtin_mul_overflow(K - 1, c->out_stride, &span) || __builtin_add_overflow(span, w.n_samples, &span)) return false;
-    } else if (__builtin_mul_overflow(w.n_samples, K, &span)) {
+        if (__builtin_mul_overflow(K - 1, c->out_stride, &span) || __builtin_add_overflow(span, w.written, &span)) return false;
+    } else if (__builtin_mul_overflow(w.written, K, &span)) {
         return false;
     }
     if (__builtin_add_overflow(c->out_offset, span, &end) || __builtin_mul_overflow(end, esz, &end)) return false;
@@ -733,7 +752,7 @@ static bool chain_ranges_fit(const lwb_batch_io *io, const lwb_chain *c, const C
 }
 
 // The one walk of a batch, made before a path is chosen: the argument checks, every chain's walk and the batch's extent,
-// and every refusal a batch gets from its arguments and arrays -- an out_stride below the samples a chain produces,
+// and every refusal a batch gets from its arguments and arrays -- an out_stride below the samples a chain writes,
 // a chain range that does not fit in 64 bits (chain_ranges_fit), host floor kinds out of range or without floor1_y, a dense floor without dense_floor, decreasing host VQ offsets
 // and, with pinned_only (a submit), host arrays that are not page-locked.  It writes nothing into the chain array and
 // queues nothing.  The paths refuse a batch only on a CUDA error, and in one more case: the VQ entry's front-stage
@@ -743,13 +762,15 @@ static int walk_batch(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, co
     int rc = check_batch_args(ctx, chains, n_chains, io);
     if (rc || n_chains == 0) return rc;
     BatchExtent &ext = bw->ext;
+    bw->chains = chains;
     bw->walks.resize(n_chains);
     const bool planar = out_format_of(io->out_format).planar;
     for (size_t i = 0; i < n_chains; i++) {
         const lwb_chain *c = &chains[i];
-        const ChainWalk &w = bw->walks[i] = walk_chain(c, [](uint32_t, const Geom &, bool, uint32_t, uint64_t, uint64_t) {});
+        ChainWalk &w = bw->walks[i] = walk_chain(c, [](uint32_t, const Geom &, bool, uint32_t, uint64_t, uint64_t) {});
+        clip_to_window(c->stream, &w);
         if (!w.done) continue;
-        if (planar && c->out_stride < w.n_samples) return fail(ctx, LWB_ERR_BUFFER, "chain: out_stride smaller than the samples produced");
+        if (planar && c->out_stride < w.written) return fail(ctx, LWB_ERR_BUFFER, "chain: out_stride smaller than the samples produced");
         if (!chain_ranges_fit(io, c, w)) return fail(ctx, LWB_ERR_BUFFER, "chain: a PCM, coefficient or packet-row range does not fit in 64 bits");
         ext.add(io, c, w);
         if (io->entry != LWB_ENTRY_SPECTRUM && (rc = scan_floor_kinds(ctx, io, c, w.done, &ext.need_dense, &ext.need_floor0))) return rc;
@@ -759,6 +780,52 @@ static int walk_batch(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, co
     if (!pinned_only || io->memory != LWB_MEM_HOST || ext.empty()) return LWB_OK;
     CU(ctx, cudaSetDevice(ctx->device));
     return check_page_locked(ctx, io, ext, chains[0].stream->setup->channels);
+}
+
+// Output windows (lwb_stream_set_window).  A clipped chain (ChainWalk::clipped) keeps the path its batch would take
+// without a window: at end of stream nearly every step of a decode server has some stream ending, and routing those to
+// the chain kernel would take most batches off k_long.  So it decodes its full output, laid out as the fused kernels
+// want it -- planes of a multiple of 8 elements, 16-byte aligned -- into scratch, and BatchArenas::download moves the
+// samples it writes to their place with k_row_copy.  This writes bw->clip, the chain array the paths then decode: the
+// clipped chains point into the scratch, the others are the caller's.  A host-memory batch's scratch follows the PCM
+// extent in its staging (whose start moves down to an 8-element boundary), so only written samples cross PCIe.  A
+// device-memory batch's scratch is ctx->win, addressed from io->pcm by a wrapping element offset -- as the staged arenas
+// are addressed from bases biased by their first element -- and placed at io->pcm's offset mod 16.
+static int place_clipped_chains(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, BatchWalk *bw)
+{
+    const OutFormat of = out_format_of(io->out_format);
+    auto region = [&](size_t i, uint64_t *stride) {
+        const uint64_t K = chains[i].stream->setup->out_channels(), n = bw->walks[i].n_samples;
+        *stride = (n + 7) & ~7ull;
+        return of.planar ? K * *stride : (n * K + 7) & ~7ull;
+    };
+    uint64_t total = 0, stride;
+    for (size_t i = 0; i < n_chains; i++)
+        if (bw->walks[i].clipped()) total += region(i, &stride);
+    if (!total) return LWB_OK;
+    uint64_t at, end;
+    if (io->memory == LWB_MEM_HOST) {
+        BatchExtent &ext = bw->ext;
+        at = (ext.o_hi + 7) & ~7ull;
+        if (at < ext.o_hi || __builtin_add_overflow(at, total, &end) || __builtin_mul_overflow(end, (uint64_t)of.esz, &end))
+            return fail(ctx, LWB_ERR_BUFFER, "chain: the staged PCM of a windowed batch does not fit in 64 bits");
+        ext.o_lo &= ~7ull;
+        ext.o_hi = at + total;
+    } else {
+        int rc;
+        if ((rc = ensure(ctx, ctx->win, total * of.esz + 16))) return rc;
+        const uintptr_t pcm = reinterpret_cast<uintptr_t>(io->pcm), win = reinterpret_cast<uintptr_t>(ctx->win.p) + (pcm & 15);
+        at = (uint64_t)(win - pcm) / of.esz;
+    }
+    bw->clip.assign(chains, chains + n_chains);
+    for (size_t i = 0; i < n_chains; i++) {
+        if (!bw->walks[i].clipped()) continue;
+        const uint64_t size = region(i, &stride);
+        bw->clip[i].out_offset = at;
+        bw->clip[i].out_stride = stride;
+        at += size;
+    }
+    return LWB_OK;
 }
 
 // Walks one batch (walk_batch) and queues it on the first path that takes it.  Once the path has queued its work, the
@@ -771,6 +838,8 @@ static int queue_batch(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const l
     int rc = walk_batch(ctx, chains, n_chains, io, pinned_only, &bw);
     if (rc || n_chains == 0) return rc;
     CU(ctx, cudaSetDevice(ctx->device));
+    if ((rc = place_clipped_chains(ctx, chains, n_chains, io, &bw))) return rc;
+    const lwb_chain *decode = bw.clip.empty() ? chains : bw.clip.data();
     if (prepared) prepared->captured = false; // the path that takes the batch captures it anew, if it can
     // An output mix is applied where one CTA holds every channel of a packet (k_chain) or by the four-kernel path: a batch
     // with a mixed chain skips the fused paths, as interleaved output does.
@@ -779,8 +848,9 @@ static int queue_batch(lwb_ctx *ctx, lwb_chain *chains, size_t n_chains, const l
         if (chains[i].stream->setup->host.n_out) first = kChainPath;
     for (size_t k = first; k < std::size(kBatchPaths); k++) {
         bool handled = false;
-        if ((rc = kBatchPaths[k](ctx, chains, n_chains, io, bw, &handled, prepared))) return rc;
+        if ((rc = kBatchPaths[k](ctx, decode, n_chains, io, bw, &handled, prepared))) return rc;
         if (!handled) continue;
+        if (prepared && !bw.clip.empty()) prepared->captured = false;   // a replay would not move the clipped samples
         for (size_t i = 0; i < n_chains; i++) set_chain_result(&chains[i], bw.walks[i]);
         commit_stream_states(chains, bw.walks);
         return LWB_OK;
@@ -899,10 +969,7 @@ static int queue_state_rows(lwb_ctx *ctx, const lwb_state_slot *slots, size_t n,
         const uint32_t len = slot_len(slots[i], load);
         for (unsigned c = 0; len && c < s->setup->channels; c++) {
             float *row = s->d_state + (size_t)c * state_stride(s->setup), *b = dev + (slots[i].offset - base) + (uint64_t)c * len;
-            const float *src = load ? b : row;
-            float *dst = load ? row : b;
-            const bool vec = len % 4 == 0 && ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0;
-            h[k++] = RowCopy{src, dst, vec ? len / 4 : len, vec ? 0u : 1u};
+            h[k++] = load ? RowCopy{b, row, len * sizeof(float)} : RowCopy{row, b, len * sizeof(float)};
         }
     }
     if ((rc = upload_staging(ctx, st, h, ctx->state_rows.p, rows * sizeof(RowCopy), ctx->stream))) return rc;
@@ -1026,11 +1093,20 @@ extern "C" void lwb_plan_destroy(lwb_plan *p)
     delete p;
 }
 
+// Whether a stream of the plan has an output window that may clip it: its counters move at every execution, which a
+// replay would not do.
+static bool plan_has_window(const lwb_plan *p)
+{
+    for (size_t i = 0; i < p->n_chains; i++)
+        if (p->chains[i].stream->skip_left || p->chains[i].stream->limit_left != ~0ull) return true;
+    return false;
+}
+
 extern "C" int lwb_plan_execute(lwb_plan *p)
 {
     if (!p) return LWB_ERR_INVALID;
     lwb_ctx *ctx = p->ctx;
-    if (!p->captured || p->gen != ctx->state_gen || first_batch_path() != 0)
+    if (!p->captured || p->gen != ctx->state_gen || first_batch_path() != 0 || (ctx->windows_set && plan_has_window(p)))
         return decode_chains_impl(ctx, p->chains, p->n_chains, &p->io, p);
     // steady state: nothing about the batch or the stream states has changed shape since the descriptors were
     // built -- the per-chain results in the caller's array and the stream states are still right: just launch.

@@ -34,16 +34,50 @@ static ChainShape chain_shape(unsigned maxc, int n1max, bool residue, bool vq = 
 // One block per row: the stream state the first segment of a chain starts from, moved out of the way of the segment of
 // the same chain that ends the batch -- in the one-pass schedule (path_mixed.cuh) that one may store the new state before
 // the first one has read the old; and the state rows lwb_streams_save / lwb_streams_load move, whose offsets in the
-// caller's buffer may leave a row unaligned or of a length that is not a multiple of 4 (the scalar form).
-__global__ void k_row_copy(const RowCopy *__restrict__ rc)
+// caller's buffer may leave a row unaligned or of a length that is not a multiple of 4; and the written samples of a
+// clipped chain (BatchWalk::clip), f32, i16 or f16 rows from its full output to their place at any 2-byte alignment.
+// Every row is stored in full 16-byte lines between a 2-byte head (up to dst's next 16-byte boundary) and a 2-byte tail.
+// Where source and destination agree mod 16 the lines are plain vector copies; otherwise each line is funnel-shifted
+// out of the two aligned 16-byte source lines it straddles (Q: its offset in words, r: the 0 or 16 bits left over).
+// Those lines hold at least one byte of the row each, so the loads stay inside the row's 16-byte lines.
+template <int Q>
+__device__ __forceinline__ void row_copy_shifted(const uint4 *__restrict__ a, uint4 *__restrict__ d, uint64_t nv, unsigned r)
+{
+    for (uint64_t v = threadIdx.x; v < nv; v += blockDim.x) {
+        const uint4 A = a[v], B = a[v + 1];
+        const uint32_t w[8] = {A.x, A.y, A.z, A.w, B.x, B.y, B.z, B.w};
+        d[v] = make_uint4(__funnelshift_r(w[Q], w[Q + 1], r), __funnelshift_r(w[Q + 1], w[Q + 2], r), __funnelshift_r(w[Q + 2], w[Q + 3], r),
+                          __funnelshift_r(w[Q + 3], w[Q + 4], r));
+    }
+}
+
+__global__ void __launch_bounds__(kRowCopyThreads) k_row_copy(const RowCopy *__restrict__ rc)
 {
     const RowCopy c = rc[blockIdx.x];
-    if (c.scalar) {
-        for (uint32_t i = threadIdx.x; i < c.n; i += blockDim.x) c.dst[i] = c.src[i];
+    const char *src = static_cast<const char *>(c.src);
+    char *dst = static_cast<char *>(c.dst);
+    const uint64_t head = min(c.bytes, (uint64_t)((16 - (reinterpret_cast<uintptr_t>(dst) & 15)) & 15));
+    const uint64_t nv = (c.bytes - head) >> 4;
+    for (uint64_t i = 2 * threadIdx.x; i < head; i += 2 * blockDim.x)
+        *reinterpret_cast<uint16_t *>(dst + i) = *reinterpret_cast<const uint16_t *>(src + i);
+    for (uint64_t i = head + nv * 16 + 2 * threadIdx.x; i < c.bytes; i += 2 * blockDim.x)
+        *reinterpret_cast<uint16_t *>(dst + i) = *reinterpret_cast<const uint16_t *>(src + i);
+    uint4 *d = reinterpret_cast<uint4 *>(dst + head);
+    const char *s = src + head;
+    const unsigned sh = reinterpret_cast<uintptr_t>(s) & 15, r = (sh & 3) * 8;
+    const uint4 *a = reinterpret_cast<const uint4 *>(s - sh);
+    switch (sh >> 2) {
+    case 0:
+        if (!sh) {
+            for (uint64_t v = threadIdx.x; v < nv; v += blockDim.x) d[v] = a[v];
+            return;
+        }
+        row_copy_shifted<0>(a, d, nv, r);
         return;
+    case 1: row_copy_shifted<1>(a, d, nv, r); return;
+    case 2: row_copy_shifted<2>(a, d, nv, r); return;
+    default: row_copy_shifted<3>(a, d, nv, r); return;
     }
-    for (uint32_t i = threadIdx.x; i < c.n; i += blockDim.x)
-        reinterpret_cast<float4 *>(c.dst)[i] = reinterpret_cast<const float4 *>(c.src)[i];
 }
 
 // The chain kernel's descriptor of packets [p0, p0 + n) of chain c, which enter with stream state (has, plen), start at
@@ -160,7 +194,7 @@ static int try_chain(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, con
         std::vector<Step> steps(1, Step{LWB_KERNEL_CHAIN, dbuf.p, n_launch, nullptr});
         if ((rc = run_steps(ctx, args, steps))) return rc;
         if (cap) capture(plan, gen_at_entry, FrontStages(), args, std::move(steps));
-        if ((rc = ar.download(0, chains, bw, 0, n_chains, ext)) || (rc = ar.finish())) return rc;
+        if ((rc = ar.download(0, bw, 0, n_chains, ext)) || (rc = ar.finish())) return rc;
     }
     return LWB_OK;
 }

@@ -11,12 +11,15 @@ struct ChainWalk {
     uint32_t done = 0;            // packets decoded
     int status = LWB_OK;
     uint64_t n_samples = 0;       // per channel
+    uint64_t skip = 0;            // the stream's window (clip_to_window): of those samples, the first `skip` are dropped
+    uint64_t written = 0;         // and the next `written` written (== n_samples without a window)
     bool end_has = false;         // stream state after them
     uint32_t end_plen = 0;
     bool clear_after = false;     // the OLA guard fired on packet `done`: the state becomes empty
     uint64_t coeff_end = 0;       // element offset behind the last decoded packet
     uint32_t full_n = 0;          // n of every decoded packet when all are full-window blocks of one size, else 0
     bool long_only = true;        // every decoded packet a long block between long neighbours (both window flags set)
+    bool clipped() const { return skip || written != n_samples; }
 };
 
 // Walks chain c from its stream's state, with no side effects.  on_packet(k, g, has, plen, coeff, pos) sees every packet
@@ -62,18 +65,28 @@ static ChainWalk walk_chain(const lwb_chain *c, F &&on_packet)
     return w;
 }
 
+// The samples of w that stream s's output window (lwb_stream_set_window) lets through: w.skip and w.written.
+static void clip_to_window(const lwb_stream *s, ChainWalk *w)
+{
+    window_clip(s->skip_left, s->limit_left, w->n_samples, &w->skip, &w->written);
+}
+
 static void set_chain_result(lwb_chain *c, const ChainWalk &w)
 {
     c->status = w.status;
     c->packets_done = w.done;
-    c->n_samples = (uint32_t)w.n_samples;
+    c->n_samples = (uint32_t)w.written;
 }
 
-// The stream states the walks of a batch leave, committed once the batch's work is queued.
+// The stream states and output windows the walks of a batch leave, committed once the batch's work is queued.
 static void commit_stream_states(const lwb_chain *chains, const std::vector<ChainWalk> &walks)
 {
-    for (size_t i = 0; i < walks.size(); i++)
-        if (walks[i].done || walks[i].clear_after) set_stream_state(chains[i].stream, walks[i].end_has, walks[i].end_plen);
+    for (size_t i = 0; i < walks.size(); i++) {
+        lwb_stream *s = chains[i].stream;
+        if (walks[i].done || walks[i].clear_after) set_stream_state(s, walks[i].end_has, walks[i].end_plen);
+        s->skip_left -= walks[i].skip;
+        if (s->limit_left != ~0ull) s->limit_left -= walks[i].written;
+    }
 }
 
 // The three mode bytes (mode, previous and next window flag) of packet k of chain c, as the chain kernel reads them.
@@ -394,7 +407,7 @@ struct BatchExtent {
     bool need_dense = false;      // a decoded row has a dense floor
     bool need_floor0 = false;     // a decoded row may have a floor-0 record (LWB_FLOOR_ZERO)
 
-    // The ranges of chain c, whose walk w decodes w.done packets.
+    // The ranges of chain c, whose walk w decodes w.done packets and writes w.written samples per channel.
     void add(const lwb_batch_io *io, const lwb_chain *c, const ChainWalk &w)
     {
         if (!w.done) return;
@@ -403,7 +416,7 @@ struct BatchExtent {
         c_lo = std::min(c_lo, c->coeff_offset);
         c_hi = std::max(c_hi, w.coeff_end);
         o_lo = std::min(o_lo, c->out_offset);
-        o_hi = std::max(o_hi, c->out_offset + (planar ? (uint64_t)(C - 1) * c->out_stride + w.n_samples : w.n_samples * C));
+        o_hi = std::max(o_hi, c->out_offset + (planar ? (uint64_t)(C - 1) * c->out_stride + w.written : w.written * C));
         if (io->entry == LWB_ENTRY_SPECTRUM) return;
         r_lo = std::min(r_lo, c->packet_index);
         r_hi = std::max<uint64_t>(r_hi, c->packet_index + w.done);
@@ -413,9 +426,14 @@ struct BatchExtent {
 
 // A batch walked once, before a path is chosen (walk_batch, lwb_api.cu): every chain's walk and the batch's extent.
 // The paths read it; queue_batch writes the chain results and stream states from it once a path has queued the batch.
+// `clip` (place_clipped_chains, lwb_api.cu) is empty unless a chain's window clips it: it is then the chain array the
+// paths decode, in which each clipped chain writes its full output to scratch; BatchArenas::download moves the written
+// samples to their place in the caller's chains.
 struct BatchWalk {
+    const lwb_chain *chains = nullptr;      // the caller's
     std::vector<ChainWalk> walks;
     BatchExtent ext;
+    std::vector<lwb_chain> clip;
 };
 
 // The extent of chains [i0, i1) of a walked batch: one chunk of a chunked host-memory batch.
@@ -466,7 +484,7 @@ static int check_page_locked(lwb_ctx *ctx, const lwb_batch_io *io, const BatchEx
                                        " is not page-locked (lwb_host_alloc, cudaHostAlloc or cudaHostRegister)").c_str());
 }
 
-// D2H of the PCM that chains [i0, i1), walked as walks[i0, i1), produced, from the staging buffer `stage`, which holds
+// D2H of the PCM that chains [i0, i1), walked as walks[i0, i1), wrote, from the staging buffer `stage`, which holds
 // arena element `obase` at its start.  Only the write set is copied (pcm_copy_plan.h): the gaps between planes and
 // between chains are the caller's memory, and the kernels never wrote them in the staging buffer.
 static int copy_pcm_to_host(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chain *chains, const ChainWalk *walks, size_t i0, size_t i1,
@@ -477,7 +495,7 @@ static int copy_pcm_to_host(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chai
     ctx->pcm_spans.clear();
     for (size_t i = i0; i < i1; i++) {
         const lwb_chain *c = &chains[i];
-        pcm_chain_spans(planar, c->stream->setup->out_channels(), c->out_offset, c->out_stride, walks[i].n_samples, ctx->pcm_spans);
+        pcm_chain_spans(planar, c->stream->setup->out_channels(), c->out_offset, c->out_stride, walks[i].written, ctx->pcm_spans);
     }
     plan_pcm_copies(ctx->pcm_spans, (uint64_t)INT32_MAX / esz, ctx->pcm_copies);
     for (const PcmCopy &cp : ctx->pcm_copies) {
@@ -495,6 +513,8 @@ static int copy_pcm_to_host(lwb_ctx *ctx, const lwb_batch_io *io, const lwb_chai
 // uploads wait on the GPU for the batch that used the set before (ArenaSet::done) and nothing else.  With the copy
 // streams (copy_in / copy_out, ordered by ev_in[k] / ev_done[k]) the copies of one chunk overlap the kernels of
 // another; otherwise everything runs on the compute stream.  A device-memory batch uses the caller's arenas in place.
+static int run_steps(lwb_ctx *ctx, const StepArgs &a, const std::vector<Step> &steps);
+
 struct BatchArenas {
     const float *coeffs = nullptr, *dense = nullptr;
     char *pcm = nullptr;
@@ -555,15 +575,47 @@ struct BatchArenas {
         CU(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_in[k], 0));
         return LWB_OK;
     }
-    // chains [i0, i1) of the batch make up chunk k
-    int download(size_t k, const lwb_chain *chains, const BatchWalk &bw, size_t i0, size_t i1, const BatchExtent &ck)
+    // Chains [i0, i1) of the batch make up chunk k, whose kernels are queued: the written samples of its clipped chains
+    // go to their place, then a host-memory batch's PCM goes home.
+    int download(size_t k, const BatchWalk &bw, size_t i0, size_t i1, const BatchExtent &ck)
     {
+        int rc;
+        if (!bw.clip.empty() && (rc = move_clipped(bw, i0, i1))) return rc;
         if (!host || ck.o_hi <= ck.o_lo) return LWB_OK;
         if (down != ctx->stream) {
             CU(ctx, cudaEventRecord(ctx->ev_done[k], ctx->stream));
             CU(ctx, cudaStreamWaitEvent(down, ctx->ev_done[k], 0));
         }
-        return copy_pcm_to_host(ctx, io, chains, bw.walks.data(), i0, i1, set->pcm.p, o_lo, down);
+        return copy_pcm_to_host(ctx, io, bw.chains, bw.walks.data(), i0, i1, set->pcm.p, o_lo, down);
+    }
+    // One k_row_copy launch on the compute stream: per clipped chain of [i0, i1) with written samples, per plane (or the
+    // one interleaved range), samples [skip, skip + written) of its full output (bw.clip) to the caller's place.
+    int move_clipped(const BatchWalk &bw, size_t i0, size_t i1)
+    {
+        const OutFormat of = out_format_of(io->out_format);
+        size_t n = 0;
+        for (size_t i = i0; i < i1; i++)
+            if (bw.walks[i].clipped() && bw.walks[i].written) n += of.planar ? bw.chains[i].stream->setup->out_channels() : 1;
+        if (!n) return LWB_OK;
+        Staging *st;
+        int rc;
+        if ((rc = acquire_staging(ctx, n * sizeof(RowCopy), &st)) || (rc = ensure(ctx, ctx->state_rows, n * sizeof(RowCopy)))) return rc;
+        RowCopy *h = (RowCopy *)st->h, *w = h;
+        for (size_t i = i0; i < i1; i++) {
+            const ChainWalk &cw = bw.walks[i];
+            if (!cw.clipped() || !cw.written) continue;
+            const lwb_chain &c = bw.chains[i], &full = bw.clip[i];
+            const uint64_t K = c.stream->setup->out_channels();
+            if (!of.planar) {
+                *w++ = RowCopy{pcm + (full.out_offset + cw.skip * K) * of.esz, pcm + c.out_offset * of.esz, cw.written * K * of.esz};
+                continue;
+            }
+            for (uint64_t k = 0; k < K; k++)
+                *w++ = RowCopy{pcm + (full.out_offset + k * full.out_stride + cw.skip) * of.esz, pcm + (c.out_offset + k * c.out_stride) * of.esz,
+                               cw.written * of.esz};
+        }
+        if ((rc = upload_staging(ctx, st, h, ctx->state_rows.p, n * sizeof(RowCopy), ctx->stream))) return rc;
+        return run_steps(ctx, StepArgs(), std::vector<Step>(1, Step{LWB_KERNEL_ROW_COPY, ctx->state_rows.p, n, nullptr}));
     }
     // The batch is queued: a host-memory batch records its ticket, which also releases its set to the next user.
     int finish()
@@ -716,7 +768,7 @@ static int launch_chain(lwb_ctx *ctx, bool mix, int fmt, unsigned n_chains, unsi
                : launch_chain<ENTRY, false>(ctx, fmt, n_chains, warps, smem, d, bytes, coeffs, dense, kinds, ys, pcm, n1max, wpc, np, zero, vq);
 }
 
-__global__ void k_row_copy(const RowCopy *__restrict__ rc);   // path_chain.cuh
+__global__ void __launch_bounds__(kRowCopyThreads) k_row_copy(const RowCopy *__restrict__ rc);   // path_chain.cuh
 
 // Launches `steps` in order on the compute stream.  Only k_long draws a ticket.
 static int run_steps(lwb_ctx *ctx, const StepArgs &a, const std::vector<Step> &steps)
@@ -729,7 +781,7 @@ static int run_steps(lwb_ctx *ctx, const StepArgs &a, const std::vector<Step> &s
         const uint32_t n = (uint32_t)s.n;
         switch (s.kernel) {
         case LWB_KERNEL_ROW_COPY:
-            rc = launch(ctx, LWB_KERNEL_ROW_COPY, k_row_copy, dim3(n), dim3(64), 0, (const RowCopy *)s.desc);
+            rc = launch(ctx, LWB_KERNEL_ROW_COPY, k_row_copy, dim3(n), dim3(kRowCopyThreads), 0, (const RowCopy *)s.desc);
             break;
         case LWB_KERNEL_LONG:
             if ((rc = next_ticket(ctx, &ticket))) return rc;
@@ -929,7 +981,7 @@ static int try_generic(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, c
     BatchArenas ar;
     int rc;
     if ((rc = ar.open(ctx, io, ext, C, false)) || (rc = ar.upload(0, ext)) || (rc = run_generic(ctx, plan, io, ar, ext.need_floor0)) ||
-        (rc = ar.download(0, chains, bw, 0, n_chains, ext)))
+        (rc = ar.download(0, bw, 0, n_chains, ext)))
         return rc;
     return ar.finish();
 }

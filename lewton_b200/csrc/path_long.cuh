@@ -223,7 +223,7 @@ static int try_long(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, cons
             gen = ctx->state_gen;                                           // every arena the capture points into is sized
         }
         steps.assign(1, Step{LWB_KERNEL_LONG, lr.d + lr.chunks[k].r0, lr.chunks[k].nr / kLongNB, pack});
-        if ((rc = run_steps(ctx, args, steps)) || (rc = ar.download(k, chains, bw, i0, i1, ke))) return rc;
+        if ((rc = run_steps(ctx, args, steps)) || (rc = ar.download(k, bw, i0, i1, ke))) return rc;
         pk0 += npk;
     }
     CU(ctx, cudaEventRecord(ctx->ev_kdone[lr.par], ctx->stream));

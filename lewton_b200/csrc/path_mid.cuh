@@ -91,6 +91,6 @@ static int try_mid(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const
     std::vector<Step> steps(1, Step{LWB_KERNEL_MID, dbuf.p, groups.size(), pack});
     if ((rc = run_steps(ctx, args, steps))) return rc;
     if (cap) capture(plan, gen_at_entry, fs, args, std::move(steps));
-    if ((rc = ar.download(0, chains, bw, 0, n_chains, ext))) return rc;
+    if ((rc = ar.download(0, bw, 0, n_chains, ext))) return rc;
     return ar.finish();
 }

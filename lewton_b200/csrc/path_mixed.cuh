@@ -291,7 +291,7 @@ struct MixedWriter {
         if (!(sc.chain[i].pass && q) && !sc.needs_precopy(i)) return;
         if (!end) end = first.state;
         float *from = slot(q ? sc.slot_of(i, q - 1, C, ch) : sc.pre_slot(i, C, ch));
-        if (!q) ((RowCopy *)(hb + ly.off_rc))[wx++] = RowCopy{first.state, from, (uint32_t)(sc.pre_units(i) * kShortN2 / 4), 0};
+        if (!q) ((RowCopy *)(hb + ly.off_rc))[wx++] = RowCopy{first.state, from, sc.pre_units(i) * kShortN2 * sizeof(float)};
         first.state = from;
     }
     // k_long's runs of long segment q of chain i.  In the pass, a run after a short segment leaves its left slope in the
@@ -451,7 +451,7 @@ static int try_mixed(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, con
         MixedChunk &ck = chunks[k];
         if (ck.ext.empty()) continue;
         if ((rc = ar.upload(k, ck.ext)) || (ck.np_ && (rc = front_stages_launch(ctx, ar, fs, ck.p0, ck.np_))) ||
-            (rc = run_steps(ctx, args, ck.steps)) || (rc = ar.download(k, chains, bw, ck.i0, ck.i1, ck.ext)))
+            (rc = run_steps(ctx, args, ck.steps)) || (rc = ar.download(k, bw, ck.i0, ck.i1, ck.ext)))
             return rc;
     }
     if (cap) capture(plan, gen_at_entry, fs, args, std::move(chunks[0].steps));

@@ -1,4 +1,4 @@
-// pcm_copy_plan.h -- which elements of the PCM arena a batch's chains produce, and the copies that move exactly those
+// pcm_copy_plan.h -- which elements of the PCM arena a batch's chains write, and the copies that move exactly those
 // from a device staging buffer laid out like the arena.  Host code without CUDA types, so that
 // tests/emu/copy_plan_emu.cpp can run this source on the CPU.
 #pragma once
@@ -22,6 +22,14 @@ inline void pcm_chain_spans(bool planar, unsigned C, uint64_t out_offset, uint64
         return;
     }
     for (unsigned c = 0; c < C; c++) spans.push_back(PcmSpan{out_offset + (uint64_t)c * out_stride, n});
+}
+
+// An output window (lwb_stream_set_window) with skip_left samples still to drop and limit_left still to write, over a
+// chain that produces n per channel: the chain drops its first *skip samples and writes the next *written.
+inline void window_clip(uint64_t skip_left, uint64_t limit_left, uint64_t n, uint64_t *skip, uint64_t *written)
+{
+    *skip = std::min(skip_left, n);
+    *written = std::min(limit_left, n - *skip);
 }
 
 // Sorts the spans, merges those that touch or overlap, and emits each run of consecutive merged spans of equal width
