@@ -148,3 +148,30 @@ def test_window_clip_edges(emu):
     for (n, s, lim), want in cases:
         skip, written, _ = _plan(emu, True, [2], [0], [n], [n], [s], [lim])
         assert (int(skip[0]), int(written[0])) == want, (n, s, lim)
+
+
+@pytest.mark.parametrize("seed", range(4))
+def test_window_counters_over_stopped_chains(emu, seed):
+    """A window over batches whose chains stop: each batch produces the samples of its decoded packets only (none for a
+    chain that stops at packet 0, none for the packet after the overlap guard emptied the state).  window_clip of each
+    batch, with the counters moved as commit_stream_states moves them (skip_left by the samples dropped, limit_left by
+    those written), writes exactly the window's slice of everything the batches produced, whatever the stops."""
+    rng = np.random.default_rng(seed)
+    for _ in range(50):
+        produced = [int(rng.choice([0, 0, 1, 7, 128, 1024, int(rng.integers(0, 4000))])) for _ in range(int(rng.integers(1, 8)))]
+        total = sum(produced)
+        skip = int(rng.integers(0, total + 50))
+        limit = [NO_LIMIT, int(rng.integers(0, total + 50)), 0][int(rng.integers(0, 3))]
+        skip_left, limit_left, pos, got = skip, limit, 0, []
+        for n in produced:
+            s, w, _ = _plan(emu, True, [2], [0], [n], [n], [skip_left], [limit_left])
+            s, w = int(s[0]), int(w[0])
+            got += list(range(pos + s, pos + s + w))
+            skip_left -= s
+            if limit_left != NO_LIMIT:
+                limit_left -= w
+            pos += n
+        end = total if limit == NO_LIMIT else min(total, skip + limit)
+        assert got == list(range(min(skip, total), max(min(skip, total), end))), (produced, skip, limit)
+        assert skip_left == max(skip - total, 0)
+        assert limit_left == (NO_LIMIT if limit == NO_LIMIT else limit - len(got))
