@@ -139,15 +139,7 @@ k_chain(const ChainDesc *__restrict__ chains, const uint8_t *__restrict__ pkt_by
 #pragma unroll
                 for (int c = 0; c < 8; c++)
                     r[c] = c < C ? (ENTRY == LWB_ENTRY_VQ ? s_acc[c * n2 + k] : coeffs[coeff + (size_t)c * n2 + k]) : 0.f;
-                for (int s = nsteps - 1; s >= 0; s--) {       // audio.rs:991-1002
-                    const int mi = mp.mag[s], ai = mp.ang[s];
-                    float mv = 0.f, av = 0.f;
-#pragma unroll
-                    for (int c = 0; c < 8; c++) { if (c == mi) mv = r[c]; if (c == ai) av = r[c]; }
-                    d_inverse_couple(mv, av);
-#pragma unroll
-                    for (int c = 0; c < 8; c++) { if (c == mi) r[c] = mv; if (c == ai) r[c] = av; }
-                }
+                d_inverse_couple_regs(r, mp, nsteps);
 #pragma unroll
                 for (int c = 0; c < 8; c++) {
                     if (c < C) {

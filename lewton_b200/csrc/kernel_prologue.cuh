@@ -204,15 +204,47 @@ __device__ __forceinline__ float4 d_floor_quad(int kind, int cnt, const float *_
     return make_float4(0.f, 0.f, 0.f, 0.f);                       // audio.rs:1021-1024
 }
 
+// Header fields of a packet with <= 2 channels and at most one coupling step; kinds, cnt: its rows' floor kinds and
+// segment counts
+struct PfStereo { int n2, nsteps, k0, k1, c0, c1; bool swapped; uint64_t base; };
+__device__ __forceinline__ PfStereo d_pf_stereo_head(const DevPacket &p, const DevMapping &mp, int C, const uint8_t *__restrict__ kinds,
+                                                     const uint8_t *__restrict__ cnt)
+{
+    PfStereo h;
+    h.n2 = p.n >> 1;
+    h.nsteps = mp.n_coupling;
+    h.swapped = h.nsteps == 1 && mp.mag[0] == 1;
+    h.base = p.coeff_off;
+    h.k0 = kinds[0]; h.k1 = C == 2 ? kinds[1] : LWB_FLOOR_UNUSED;
+    h.c0 = cnt[0]; h.c1 = C == 2 ? cnt[1] : 0;
+    return h;
+}
+// Quad q of such a packet: couple the residue quads r0, r1 (audio.rs:991-1002), multiply by the floor values out of
+// the rows' tables at `tabs` (row stride rowb), store -- at evict-first priority (STREAM) or plainly.
+template <bool STREAM>
+__device__ __forceinline__ void d_pf_stereo_quad(const PfStereo &h, int C, int q, float4 r0, float4 r1, const unsigned char *tabs,
+                                                 size_t rowb, int words, const float *__restrict__ s_db, const float *__restrict__ dense,
+                                                 const float *__restrict__ zero, float *__restrict__ spec)
+{
+    const uint64_t e0 = h.base + 4 * (uint64_t)q, e1 = e0 + h.n2;
+    d_inverse_couple_stereo(h.nsteps, h.swapped, r0, r1);
+    const unsigned char *tabs1 = tabs + rowb;
+    const float4 f0 = d_floor_quad(h.k0, h.c0, s_db, reinterpret_cast<const uint4 *>(tabs), tabs + kSegStride * 16, words, 4 * q, dense, zero, e0);
+    if (STREAM) __stcs(reinterpret_cast<float4 *>(spec + e0), d_floor_mul(f0, r0));
+    else *reinterpret_cast<float4 *>(spec + e0) = d_floor_mul(f0, r0);
+    if (C == 2) {
+        const float4 f1 = d_floor_quad(h.k1, h.c1, s_db, reinterpret_cast<const uint4 *>(tabs1), tabs1 + kSegStride * 16, words, 4 * q,
+                                       dense, zero, e1);
+        if (STREAM) __stcs(reinterpret_cast<float4 *>(spec + e1), d_floor_mul(f1, r1));
+        else *reinterpret_cast<float4 *>(spec + e1) = d_floor_mul(f1, r1);
+    }
+}
+
 // Persistent CTAs striding over the packets (grid = min(packets, a few CTAs per SM)).  Requires every coeff_off
 // (and the arena bases) to be multiples of 4 elements, <= 8 channels, a uniform channel count C.
 // Per packet: every global read the packet needs -- residue quads, the rows' segment tables and indices -- is issued
 // at the top (one exposed memory latency), the tables land in shared memory, and the per-bin work runs out of it.
 // VQ: the residue does not come from `residue` but from the packet's VQ records (d_vq_accumulate).
-#ifndef LWB_PF_SERIAL
-#define LWB_PF_SERIAL 0
-#endif
-constexpr bool PF_SERIAL = LWB_PF_SERIAL != 0;
 template <bool VQ>
 __global__ void __launch_bounds__(kPfThreads, 4)
 k_prologue_fused(const DevPacket *__restrict__ pkts, uint32_t n_pk, const float *__restrict__ residue, const float *__restrict__ dense_floor,
@@ -230,16 +262,14 @@ k_prologue_fused(const DevPacket *__restrict__ pkts, uint32_t n_pk, const float 
     const int row_q = (int)(rowb >> 4), tab_q = kSegStride;       // 16-byte quads per row: table, then index
     float4 *s_r = reinterpret_cast<float4 *>(pf_smem + (size_t)C * rowb);     // [C][kPfThreads] when C > 1
     float *s_acc = reinterpret_cast<float *>(pf_smem + (size_t)C * rowb + (C > 1 ? (size_t)C * kPfThreads * sizeof(float4) : 0));   // VQ: [C][n2]
-    if (!VQ && C <= 2 && !PF_SERIAL) {
+    if (!VQ && C <= 2) {
         // One or two channels, dense residue: the packets are software-pipelined.  While packet k is computed out of one
         // table buffer, everything packet k + 1 needs is already on its way: its rows' tables by cp.async into the other
         // buffer, its residue quads and header fields into registers.  One CTA barrier per packet.
-        struct Head { int n2, nsteps, k0, k1, c0, c1; bool swapped; uint64_t base; };
         const int row_q2 = C * row_q;                                 // quads of one table buffer
         unsigned char *bufs[2] = {pf_smem, pf_smem + (size_t)C * rowb};
         const uint32_t bufs_s[2] = {smem_u32(bufs[0]), smem_u32(bufs[1])};
-        auto prefetch = [&](uint32_t pk, int b, Head &h, float4 &a0, float4 &a1) {
-            const DevPacket &p = pkts[pk];
+        auto prefetch = [&](uint32_t pk, int b, PfStereo &h, float4 &a0, float4 &a1) {
             const size_t row0 = (size_t)pk * C;
             for (int i = tid; i < row_q2; i += kPfThreads) {        // (one pass: <= 2 rows of <= 109 quads)
                 const int c = i >= row_q ? 1 : 0, j = i - (c ? row_q : 0);
@@ -248,22 +278,15 @@ k_prologue_fused(const DevPacket *__restrict__ pkts, uint32_t n_pk, const float 
                 cp_async16(bufs_s[b] + 16u * (uint32_t)i, src);
             }
             cp_async_commit();
-            const DevSetup &su = *p.setup;
-            const DevMapping &mp = su.mappings[p.mapping];
-            h.n2 = p.n >> 1;
-            h.nsteps = mp.n_coupling;
-            h.swapped = h.nsteps == 1 && mp.mag[0] == 1;
-            h.base = p.coeff_off;
-            const uint8_t *kinds = floor_kind + p.pkt_index * C;
-            h.k0 = kinds[0]; h.k1 = C == 2 ? kinds[1] : LWB_FLOOR_UNUSED;
-            h.c0 = seg_cnt[row0]; h.c1 = C == 2 ? seg_cnt[row0 + 1] : 0;
+            const DevPacket &p = pkts[pk];
+            h = d_pf_stereo_head(p, p.setup->mappings[p.mapping], C, floor_kind + p.pkt_index * C, seg_cnt + row0);
             a0 = make_float4(0.f, 0.f, 0.f, 0.f); a1 = a0;
             if (tid < (h.n2 >> 2)) {
                 a0 = __ldcs(reinterpret_cast<const float4 *>(residue + h.base + 4 * (uint64_t)tid));
                 if (C == 2) a1 = __ldcs(reinterpret_cast<const float4 *>(residue + h.base + h.n2 + 4 * (uint64_t)tid));
             }
         };
-        Head h, hn;
+        PfStereo h, hn;
         float4 r0, r1, rn0, rn1;
         int b = 0;
         prefetch(blockIdx.x, 0, h, r0, r1);
@@ -272,53 +295,30 @@ k_prologue_fused(const DevPacket *__restrict__ pkts, uint32_t n_pk, const float 
             __syncthreads();              // this packet's tables are in; everybody is done with the other buffer
             const uint32_t nx = pk + gridDim.x;
             if (nx < n_pk) prefetch(nx, b ^ 1, hn, rn0, rn1);
-            const uint4 *t0 = reinterpret_cast<const uint4 *>(bufs[b]), *t1 = reinterpret_cast<const uint4 *>(bufs[b] + rowb);
-            const unsigned char *x0 = bufs[b] + (size_t)tab_q * 16, *x1 = x0 + rowb;
             const int n2 = h.n2;
             if (h.nsteps <= 1) {
                 for (int q = tid; q < (n2 >> 2); q += kPfThreads) {
-                    const uint64_t e0 = h.base + 4 * (uint64_t)q, e1 = e0 + n2;
                     if (q != tid) {                               // blocks of more than 1024 bins: further passes
-                        r0 = *reinterpret_cast<const float4 *>(residue + e0);
-                        if (C == 2) r1 = *reinterpret_cast<const float4 *>(residue + e1);
+                        r0 = *reinterpret_cast<const float4 *>(residue + h.base + 4 * (uint64_t)q);
+                        if (C == 2) r1 = *reinterpret_cast<const float4 *>(residue + h.base + n2 + 4 * (uint64_t)q);
                     }
-                    if (h.nsteps == 1) {
-                        if (h.swapped) {
-                            d_inverse_couple(r1.x, r0.x); d_inverse_couple(r1.y, r0.y);
-                            d_inverse_couple(r1.z, r0.z); d_inverse_couple(r1.w, r0.w);
-                        } else {
-                            d_inverse_couple(r0.x, r1.x); d_inverse_couple(r0.y, r1.y);
-                            d_inverse_couple(r0.z, r1.z); d_inverse_couple(r0.w, r1.w);
-                        }
-                    }
-                    const float4 f0 = d_floor_quad(h.k0, h.c0, s_db, t0, x0, words, 4 * q, dense_floor, zero_floor, e0);
-                    __stcs(reinterpret_cast<float4 *>(spec + e0),
-                           make_float4(__fmul_rn(f0.x, r0.x), __fmul_rn(f0.y, r0.y), __fmul_rn(f0.z, r0.z), __fmul_rn(f0.w, r0.w)));
-                    if (C == 2) {
-                        const float4 f1 = d_floor_quad(h.k1, h.c1, s_db, t1, x1, words, 4 * q, dense_floor, zero_floor, e1);
-                        __stcs(reinterpret_cast<float4 *>(spec + e1),
-                               make_float4(__fmul_rn(f1.x, r1.x), __fmul_rn(f1.y, r1.y), __fmul_rn(f1.z, r1.z), __fmul_rn(f1.w, r1.w)));
-                    }
+                    d_pf_stereo_quad<true>(h, C, q, r0, r1, bufs[b], rowb, words, s_db, dense_floor, zero_floor, spec);
                 }
             } else {
                 // several coupling steps over two channels (legal, never seen): in order, one bin at a time
                 const DevMapping &mp = pkts[pk].setup->mappings[pkts[pk].mapping];
+                const uint4 *t0 = reinterpret_cast<const uint4 *>(bufs[b]), *t1 = reinterpret_cast<const uint4 *>(bufs[b] + rowb);
+                const unsigned char *x0 = bufs[b] + (size_t)tab_q * 16, *x1 = x0 + rowb;
                 for (int q = tid; q < (n2 >> 2); q += kPfThreads) {
                     const uint64_t e0 = h.base + 4 * (uint64_t)q, e1 = e0 + n2;
                     float4 v[2];
                     v[0] = *reinterpret_cast<const float4 *>(residue + e0);
                     v[1] = *reinterpret_cast<const float4 *>(residue + e1);
-                    for (int s2 = h.nsteps - 1; s2 >= 0; s2--) {
-                        float4 &m4 = v[mp.mag[s2] & 1], &a4 = v[mp.ang[s2] & 1];
-                        d_inverse_couple(m4.x, a4.x); d_inverse_couple(m4.y, a4.y);
-                        d_inverse_couple(m4.z, a4.z); d_inverse_couple(m4.w, a4.w);
-                    }
+                    for (int s2 = h.nsteps - 1; s2 >= 0; s2--) d_inverse_couple(v[mp.mag[s2] & 1], v[mp.ang[s2] & 1]);
                     const float4 f0 = d_floor_quad(h.k0, h.c0, s_db, t0, x0, words, 4 * q, dense_floor, zero_floor, e0);
                     const float4 f1 = d_floor_quad(h.k1, h.c1, s_db, t1, x1, words, 4 * q, dense_floor, zero_floor, e1);
-                    *reinterpret_cast<float4 *>(spec + e0) =
-                        make_float4(__fmul_rn(f0.x, v[0].x), __fmul_rn(f0.y, v[0].y), __fmul_rn(f0.z, v[0].z), __fmul_rn(f0.w, v[0].w));
-                    *reinterpret_cast<float4 *>(spec + e1) =
-                        make_float4(__fmul_rn(f1.x, v[1].x), __fmul_rn(f1.y, v[1].y), __fmul_rn(f1.z, v[1].z), __fmul_rn(f1.w, v[1].w));
+                    *reinterpret_cast<float4 *>(spec + e0) = d_floor_mul(f0, v[0]);
+                    *reinterpret_cast<float4 *>(spec + e1) = d_floor_mul(f1, v[1]);
                 }
             }
             h = hn; r0 = rn0; r1 = rn1;
@@ -333,13 +333,6 @@ k_prologue_fused(const DevPacket *__restrict__ pkts, uint32_t n_pk, const float 
         const uint8_t *kinds = floor_kind + p.pkt_index * C;
         const uint64_t base = p.coeff_off;
         const size_t row0 = (size_t)pk * C;
-        const bool stereo = C <= 2 && nsteps <= 1;
-        // residue quads of this thread (first pass of the bin loop) -- issued before the table copy
-        float4 r0 = make_float4(0.f, 0.f, 0.f, 0.f), r1 = r0;
-        if (!VQ && stereo && tid < (n2 >> 2)) {
-            r0 = *reinterpret_cast<const float4 *>(residue + base + 4 * (uint64_t)tid);
-            if (C == 2) r1 = *reinterpret_cast<const float4 *>(residue + base + n2 + 4 * (uint64_t)tid);
-        }
         __syncthreads();                                          // the previous packet is done with the shared tables
         for (int i = tid; i < C * row_q; i += kPfThreads) {
             const int c = i / row_q, j = i - c * row_q;
@@ -355,38 +348,12 @@ k_prologue_fused(const DevPacket *__restrict__ pkts, uint32_t n_pk, const float 
             d_vq_accumulate(s_acc, C, n2, su, mp, vq.runs + o0, (uint32_t)(o1 - o0), vq.entries + e0, (uint32_t)(e1 - e0), tid, kPfThreads);
         }
         __syncthreads();
-        if (stereo) {
-            const int k0 = kinds[0], k1 = C == 2 ? kinds[1] : LWB_FLOOR_UNUSED;
-            const int c0 = seg_cnt[row0], c1 = C == 2 ? seg_cnt[row0 + 1] : 0;
-            const bool swapped = nsteps == 1 && mp.mag[0] == 1;          // (magnitude, angle) = (1, 0)
-            const uint4 *t0 = reinterpret_cast<const uint4 *>(pf_smem), *t1 = reinterpret_cast<const uint4 *>(pf_smem + rowb);
-            const unsigned char *x0 = pf_smem + (size_t)tab_q * 16, *x1 = x0 + rowb;
+        if (VQ && C <= 2 && nsteps <= 1) {                        // (dense residue of this shape: the pipelined loop above)
+            const PfStereo h = d_pf_stereo_head(p, mp, C, kinds, seg_cnt + row0);
             for (int q = tid; q < (n2 >> 2); q += kPfThreads) {
-                const uint64_t e0 = base + 4 * (uint64_t)q, e1 = e0 + n2;
-                if (VQ) {
-                    r0 = *reinterpret_cast<const float4 *>(s_acc + 4 * q);
-                    if (C == 2) r1 = *reinterpret_cast<const float4 *>(s_acc + n2 + 4 * q);
-                } else if (q != tid) {                            // blocks of more than 1024 bins: further passes
-                    r0 = *reinterpret_cast<const float4 *>(residue + e0);
-                    if (C == 2) r1 = *reinterpret_cast<const float4 *>(residue + e1);
-                }
-                if (nsteps == 1) {
-                    if (swapped) {
-                        d_inverse_couple(r1.x, r0.x); d_inverse_couple(r1.y, r0.y);
-                        d_inverse_couple(r1.z, r0.z); d_inverse_couple(r1.w, r0.w);
-                    } else {
-                        d_inverse_couple(r0.x, r1.x); d_inverse_couple(r0.y, r1.y);
-                        d_inverse_couple(r0.z, r1.z); d_inverse_couple(r0.w, r1.w);
-                    }
-                }
-                const float4 f0 = d_floor_quad(k0, c0, s_db, t0, x0, words, 4 * q, dense_floor, zero_floor, e0);
-                *reinterpret_cast<float4 *>(spec + e0) =
-                    make_float4(__fmul_rn(f0.x, r0.x), __fmul_rn(f0.y, r0.y), __fmul_rn(f0.z, r0.z), __fmul_rn(f0.w, r0.w));
-                if (C == 2) {
-                    const float4 f1 = d_floor_quad(k1, c1, s_db, t1, x1, words, 4 * q, dense_floor, zero_floor, e1);
-                    *reinterpret_cast<float4 *>(spec + e1) =
-                        make_float4(__fmul_rn(f1.x, r1.x), __fmul_rn(f1.y, r1.y), __fmul_rn(f1.z, r1.z), __fmul_rn(f1.w, r1.w));
-                }
+                const float4 r0 = *reinterpret_cast<const float4 *>(s_acc + 4 * q);
+                const float4 r1 = C == 2 ? *reinterpret_cast<const float4 *>(s_acc + n2 + 4 * q) : make_float4(0.f, 0.f, 0.f, 0.f);
+                d_pf_stereo_quad<false>(h, C, q, r0, r1, pf_smem, rowb, words, s_db, dense_floor, zero_floor, spec);
             }
             continue;
         }
@@ -399,18 +366,15 @@ k_prologue_fused(const DevPacket *__restrict__ pkts, uint32_t n_pk, const float 
                                                : *reinterpret_cast<const float4 *>(residue + e + (uint64_t)c * n2);
             for (int s = nsteps - 1; s >= 0; s--) {                      // audio.rs:991-1002
                 float4 m4 = s_r[mp.mag[s] * kPfThreads + tid], a4 = s_r[mp.ang[s] * kPfThreads + tid];
-                d_inverse_couple(m4.x, a4.x); d_inverse_couple(m4.y, a4.y);
-                d_inverse_couple(m4.z, a4.z); d_inverse_couple(m4.w, a4.w);
+                d_inverse_couple(m4, a4);
                 s_r[mp.mag[s] * kPfThreads + tid] = m4;
                 s_r[mp.ang[s] * kPfThreads + tid] = a4;
             }
             for (int c = 0; c < C; c++) {
                 const uint64_t ec = e + (uint64_t)c * n2;
-                const float4 r = s_r[c * kPfThreads + tid];
                 const float4 f = d_floor_quad(kinds[c], seg_cnt[row0 + c], s_db, reinterpret_cast<const uint4 *>(pf_smem + c * rowb),
                                               pf_smem + c * rowb + (size_t)tab_q * 16, words, 4 * q, dense_floor, zero_floor, ec);
-                *reinterpret_cast<float4 *>(spec + ec) =
-                    make_float4(__fmul_rn(f.x, r.x), __fmul_rn(f.y, r.y), __fmul_rn(f.z, r.z), __fmul_rn(f.w, r.w));
+                *reinterpret_cast<float4 *>(spec + ec) = d_floor_mul(f, s_r[c * kPfThreads + tid]);
             }
         }
     }

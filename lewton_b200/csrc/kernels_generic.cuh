@@ -38,6 +38,41 @@ __device__ __forceinline__ void d_inverse_couple(float &m, float &a)
     m = s ? m0 : v;
     a = s ? v : m0;
 }
+// the same on each of four consecutive bins
+__device__ __forceinline__ void d_inverse_couple(float4 &m, float4 &a)
+{
+    d_inverse_couple(m.x, a.x); d_inverse_couple(m.y, a.y);
+    d_inverse_couple(m.z, a.z); d_inverse_couple(m.w, a.w);
+}
+// floor x residue of four consecutive bins (audio.rs:1035-1037)
+__device__ __forceinline__ float4 d_floor_mul(float4 f, float4 r)
+{
+    return make_float4(__fmul_rn(f.x, r.x), __fmul_rn(f.y, r.y), __fmul_rn(f.z, r.z), __fmul_rn(f.w, r.w));
+}
+// At most one coupling step over two channels (r0, r1: channels 0 and 1); swapped: (magnitude, angle) = (1, 0).
+// T is float or float4.
+template <typename T>
+__device__ __forceinline__ void d_inverse_couple_stereo(int nsteps, bool swapped, T &r0, T &r1)
+{
+    if (nsteps == 1) {
+        if (swapped) d_inverse_couple(r1, r0);
+        else d_inverse_couple(r0, r1);
+    }
+}
+// The nsteps coupling steps of mp, in reverse (audio.rs:991-1002), on one bin of up to 8 channels held in registers.
+// The channel indices are dynamic, so each step reads and writes its pair through predicated selects.
+__device__ __forceinline__ void d_inverse_couple_regs(float (&r)[8], const DevMapping &mp, int nsteps)
+{
+    for (int s = nsteps - 1; s >= 0; s--) {
+        const int mi = mp.mag[s], ai = mp.ang[s];
+        float mv = 0.f, av = 0.f;
+#pragma unroll
+        for (int c = 0; c < 8; c++) { if (c == mi) mv = r[c]; if (c == ai) av = r[c]; }
+        d_inverse_couple(mv, av);
+#pragma unroll
+        for (int c = 0; c < 8; c++) { if (c == mi) r[c] = mv; if (c == ai) r[c] = av; }
+    }
+}
 
 constexpr int kPrologueThreads = 256;
 constexpr int kPrologueGroup = 8;            // channels whose floor posts sit in smem at once
@@ -98,10 +133,7 @@ k_prologue(const DevPacket *__restrict__ pkts, const float *__restrict__ residue
             const int k0 = kinds[0], k1 = kinds[1];
             for (int k = threadIdx.x; k < n2; k += kPrologueThreads) {
                 float r0 = res[k], r1 = res[(size_t)n2 + k];
-                if (nsteps == 1) {
-                    if (swapped) d_inverse_couple(r1, r0);
-                    else d_inverse_couple(r0, r1);
-                }
+                d_inverse_couple_stereo(nsteps, swapped, r0, r1);
                 const float f0 = k0 == LWB_FLOOR_ONE ? c_inverse_db[s_curve[k]] : d_floor_other(k0, dense_floor, zero_floor, p.coeff_off + k);
                 const float f1 = k1 == LWB_FLOOR_ONE ? c_inverse_db[s_curve[(size_t)n2 + k]]
                                                      : d_floor_other(k1, dense_floor, zero_floor, p.coeff_off + (size_t)n2 + k);
@@ -114,15 +146,7 @@ k_prologue(const DevPacket *__restrict__ pkts, const float *__restrict__ residue
             float r[8];
 #pragma unroll
             for (int c = 0; c < 8; c++) r[c] = c < C ? res[(size_t)c * n2 + k] : 0.f;
-            for (int s = nsteps - 1; s >= 0; s--) {
-                const int mi = mp.mag[s], ai = mp.ang[s];
-                float mv = 0.f, av = 0.f;
-#pragma unroll
-                for (int c = 0; c < 8; c++) { if (c == mi) mv = r[c]; if (c == ai) av = r[c]; }
-                d_inverse_couple(mv, av);
-#pragma unroll
-                for (int c = 0; c < 8; c++) { if (c == mi) r[c] = mv; if (c == ai) r[c] = av; }
-            }
+            d_inverse_couple_regs(r, mp, nsteps);
 #pragma unroll
             for (int c = 0; c < 8; c++) {
                 if (c < C) {

@@ -1222,27 +1222,19 @@ extern "C" int lwb_debug_packet_taps(lwb_stream *s, const lwb_packet *pkt, float
     if (need_dense) CU(ctx, cudaMemcpyAsync(ctx->ordered.dense.p, pkt->dense_floor, C * n2 * 4, cudaMemcpyHostToDevice, st));
     const DevPacket *dp = (const DevPacket *)ctx->desc.p;
     if (post_inverse) {
-        // audio.rs:1004 tap: coupling only -- run the prologue with every floor "dense = 1.0"?  No:
-        // the tap is taken by running the prologue on a copy with all floors unused replaced by a
-        // unit curve, so that floor x residue leaves the decoupled residue unchanged.
-        std::vector<float> ones(C * n2, 1.0f);
-        std::vector<uint8_t> kd(C, LWB_FLOOR_DENSE);
-        void *tmp_dense = nullptr, *tmp_kinds = nullptr;
-        CU(ctx, cudaMalloc(&tmp_dense, C * n2 * 4));
-        CU(ctx, cudaMalloc(&tmp_kinds, C));
-        CU(ctx, cudaMemcpyAsync(tmp_dense, ones.data(), C * n2 * 4, cudaMemcpyHostToDevice, st));
-        CU(ctx, cudaMemcpyAsync(tmp_kinds, kd.data(), C, cudaMemcpyHostToDevice, st));
-        rc = launch(ctx, LWB_KERNEL_PROLOGUE, k_prologue, dim3(1), dim3(kPrologueThreads), prologue_smem(su->channels, su->bs1), dp, (const float *)ctx->ordered.coeffs.p,
-                    (const float *)tmp_dense, (const uint8_t *)tmp_kinds, (const uint32_t *)ctx->ordered.ys.p,
-                    (float *)ctx->spec.p, (const float *)nullptr);
-        if (!rc) {
-            cudaError_t e = cudaMemcpyAsync(post_inverse, ctx->spec.p, C * n2 * 4, cudaMemcpyDeviceToHost, st);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-            if (e != cudaSuccess) rc = fail(ctx, LWB_ERR_CUDA, "tap copy", e);
-        }
-        cudaFree(tmp_dense);
-        cudaFree(tmp_kinds);
-        if (rc) return rc;
+        // audio.rs:1004 tap: coupling only.  The prologue runs with every channel's floor a dense unit curve, so that
+        // floor x residue leaves the decoupled residue unchanged.  Curve and kinds sit in the IMDCT scratch ctx->x
+        // (C * n floats), which the tap uses again only after this prologue.
+        float *unit = (float *)ctx->x.p;
+        uint8_t *unit_kinds = (uint8_t *)(unit + C * n2);
+        const std::vector<float> ones(C * n2, 1.0f);
+        CU(ctx, cudaMemcpyAsync(unit, ones.data(), C * n2 * 4, cudaMemcpyHostToDevice, st));
+        CU(ctx, cudaMemsetAsync(unit_kinds, LWB_FLOOR_DENSE, C, st));
+        if ((rc = launch(ctx, LWB_KERNEL_PROLOGUE, k_prologue, dim3(1), dim3(kPrologueThreads), prologue_smem(su->channels, su->bs1), dp,
+                         (const float *)ctx->ordered.coeffs.p, (const float *)unit, (const uint8_t *)unit_kinds,
+                         (const uint32_t *)ctx->ordered.ys.p, (float *)ctx->spec.p, (const float *)nullptr)))
+            return rc;
+        CU(ctx, cudaMemcpyAsync(post_inverse, ctx->spec.p, C * n2 * 4, cudaMemcpyDeviceToHost, st));
     }
     float *zero = need_floor0 ? (float *)ctx->floor0.p : nullptr;
     if (zero && (rc = launch_floor0_curves(ctx, dp, 1, (unsigned)C, (const uint8_t *)ctx->ordered.kinds.p, (const uint32_t *)ctx->ordered.ys.p, zero)))
