@@ -451,7 +451,9 @@ class StreamSpec:
     """A random valid set of headers.  channels, blocksizes (log2), and knobs for which features appear."""
 
     def __init__(self, rng, channels=2, bs0=8, bs1=11, floor0=False, n_modes=None, sample_rate=44100, residue_types=None,
-                 cascade_p=0.5):
+                 cascade_p=0.5, couplings=None):
+        """couplings: one fixed coupling list [(magnitude, angle), ...] per mapping; the modes are then mode 2i short and
+        mode 2i + 1 long of mapping i.  None: 1-2 mappings with random coupling lists and random modes."""
         self.rng = rng
         self.channels, self.bs0, self.bs1, self.sample_rate = channels, bs0, bs1, sample_rate
         # codebooks: scalar books first (floor-1 values / class words), then VQ books
@@ -484,10 +486,12 @@ class StreamSpec:
         for rt in rts:
             self.residues.append(Residue(rng, self.books, vq_ids, class_ids, n2_long, rt, cascade_p))
         self.mappings = []
-        for _ in range(int(rng.integers(1, 3))):
+        for k in range(int(rng.integers(1, 3)) if couplings is None else len(couplings)):
             submaps = int(rng.integers(1, min(3, channels) + 1))
             steps = []
-            if channels > 1:
+            if couplings is not None:
+                steps = [(int(m), int(a)) for m, a in couplings[k]]
+            elif channels > 1:
                 for _ in range(int(rng.integers(0, channels + 1))):
                     m, a = rng.choice(channels, 2, replace=False)
                     steps.append((int(m), int(a)))
@@ -495,10 +499,13 @@ class StreamSpec:
             self.mappings.append({"submaps": submaps, "coupling": steps, "mux": mux,
                                   "floors": rng.integers(0, len(self.floors), submaps).tolist(),
                                   "residues": rng.integers(0, len(self.residues), submaps).tolist()})
-        n_modes = n_modes or int(rng.integers(2, 5))
-        self.modes = [(0, int(rng.integers(0, len(self.mappings)))), (1, int(rng.integers(0, len(self.mappings))))]
-        while len(self.modes) < n_modes:
-            self.modes.append((int(rng.integers(0, 2)), int(rng.integers(0, len(self.mappings)))))
+        if couplings is not None:
+            self.modes = [(bf, i) for i in range(len(couplings)) for bf in (0, 1)]
+        else:
+            n_modes = n_modes or int(rng.integers(2, 5))
+            self.modes = [(0, int(rng.integers(0, len(self.mappings)))), (1, int(rng.integers(0, len(self.mappings))))]
+            while len(self.modes) < n_modes:
+                self.modes.append((int(rng.integers(0, 2)), int(rng.integers(0, len(self.mappings)))))
         self.vendor = "lewton_b200 synthetic packer"
         self.comments = [("TITLE", "synthetic"), ("ARTIST", "packer éè")]
 
