@@ -202,48 +202,6 @@ struct MidDev {           // n = 512: four descriptors per group -- one ring sta
                                    kLongWarps * (Ring + 2) * 8 + (size_t)kLongWarps * Slots * Mid<KB>::NB * sizeof(LongRun) + 64;
 };
 
-// step 8 + window + overlap-add + stores of the lane's block, all 8 slots.  FIRST: packet 0 of the run (its previous right
-// half comes from the state tile if has_prev, else nothing is emitted).  flags: bit0 has_prev, bit2 dummy.
-template <int KB, bool FIRST, typename OutT>
-__device__ __forceinline__ void out_stage_m(const TwMix &tw, int lane, const V O[8], const V E[8], V pe[8], uint32_t flags,
-                                            OutT *out, const float *s_state)
-{
-    using M = Mid<KB>;
-    constexpr int Wd = M::W, TOP = M::N2 - M::W;       // sample m = Wd r + hl (or + Wd - 1 - hl); N2 - 1 - m = TOP - Wd r + ...
-    const int hl = lane >> KB;
-#pragma unroll
-    for (int j = 0; j < 8; j++) {
-        const int rw = Wd * rev3(j);
-        const bool nat = (j & 1);             // odd slots: half x -> hl, half y -> Wd - 1 - hl
-        V plo = pe[j], phi = pe[j];
-        bool emit = !(flags & 4u);
-        if (FIRST) {
-            emit = emit && (flags & 1u);
-            if (flags & 1u) {                 // prev[m] and prev[N2 - 1 - m] read separately: an imported state need not be symmetric
-                const float *s_lo = s_state + hl, *s_hi = s_state + Wd - 1 - hl;
-                const float ax = nat ? s_lo[rw] : s_hi[rw], ay = nat ? s_hi[rw] : s_lo[rw];
-                const float bx = nat ? s_hi[TOP - rw] : s_lo[TOP - rw];
-                const float by = nat ? s_lo[TOP - rw] : s_hi[TOP - rw];
-                plo = V{ax, ay};
-                phi = V{bx, by};
-            }
-        }
-        V lo, hi, pev;
-        step8_ola(tw(P_B0 + j), tw(P_B1 + j), tw(P_WLO + j), tw(P_WHI + j), O[j], E[j], plo, phi, lo, hi, pev);
-        pe[j] = pev;
-        if (emit) {
-            OutT *o_lo = out + hl, *o_hi = out + Wd - 1 - hl;
-            if (nat) {
-                st_pcm(o_lo + rw, lo.x); st_pcm(o_hi + rw, lo.y);
-                st_pcm(o_hi + TOP - rw, hi.x); st_pcm(o_lo + TOP - rw, hi.y);
-            } else {
-                st_pcm(o_hi + rw, lo.x); st_pcm(o_lo + rw, lo.y);
-                st_pcm(o_lo + TOP - rw, hi.x); st_pcm(o_hi + TOP - rw, hi.y);
-            }
-        }
-    }
-}
-
 template <typename OutT, int KB>
 __global__ void __launch_bounds__(kLongWarps * 32, 1)
 k_mid(const LongRun *__restrict__ runs, uint32_t n_groups, const float *__restrict__ pack)
@@ -256,31 +214,12 @@ k_mid(const LongRun *__restrict__ runs, uint32_t n_groups, const float *__restri
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int blk = blockC_m<KB>(lane);                        // the run of the group whose samples this lane ends up with
-    const uint32_t raw_s = smem_u32(smem_raw);
-    const uint32_t align_pad = (2048u - (raw_s & 2047u)) & 2047u;
-    unsigned char *base = smem_raw + align_pad;
-    constexpr size_t kTilesBytes = (size_t)kLongWarps * kRing * kLongTileBytes;
-    constexpr size_t kStateBytes = (size_t)kLongWarps * kLongTileBytes;
-    float *tiles = reinterpret_cast<float *>(base) + (size_t)warp * kRing * kLongN2;
-    float *s_state = reinterpret_cast<float *>(base + kTilesBytes) + (size_t)warp * kLongN2;      // [NB][N2]
-    V *s_pack = reinterpret_cast<V *>(base + kTilesBytes + kStateBytes);
-    unsigned char *tail = base + kTilesBytes + kStateBytes + (size_t)kLongPackFloats * 4;
-    LongRun *s_desc = reinterpret_cast<LongRun *>(tail) + warp * kSlots * NB;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(tail + (size_t)kLongWarps * kSlots * NB * sizeof(LongRun)) + warp * (kRing + 2);
-    {
-        const float4 *src = reinterpret_cast<const float4 *>(pack);
-        float4 *dst = reinterpret_cast<float4 *>(s_pack);
-        for (int i = threadIdx.x; i < kLongPackFloats / 4; i += blockDim.x) dst[i] = __ldg(src + i);
-    }
-    if (lane == 0) {
-        for (int i = 0; i < kRing + 1; i++) mbar_init(smem_u32(&bars[i]), 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    V twR[kTwReg1 - kTwReg0 > 0 ? kTwReg1 - kTwReg0 : 1];
-#pragma unroll
-    for (int s = kTwReg0; s < kTwReg1; s++) twR[s - kTwReg0] = s_pack[s * 32 + lane];
-    const TwMix tw{twR, s_pack + lane};
+    const LongSmem<kRing, kLongTileBytes, kSlots * NB> sm(smem_raw, warp);
+    const float *tiles = sm.tiles, *s_state = sm.s_state;     // s_state: [NB][N2]
+    LongRun *s_desc = sm.s_desc;
+    V twR[kTwRegs];
+    long_cta_setup(pack, sm.s_pack, sm.bars, kRing + 1, lane, twR);
+    const TwMix tw{twR, sm.s_pack + lane};
 
     const uint32_t state_s = smem_u32(s_state);
     const uint32_t lA0 = laneA(lane, 0), lA1 = laneA(lane, 1);
@@ -290,7 +229,7 @@ k_mid(const LongRun *__restrict__ runs, uint32_t n_groups, const float *__restri
     const uint32_t W = gridDim.x * kLongWarps, gw = blockIdx.x * kLongWarps + warp;
     if (gw >= n_groups) return;
     StaticDeal<kGroupBytes / 16, kSlots, kMidFetch, kRing, kLongTileBytes> deal(
-        runs, n_groups, W, gw, smem_u32(s_desc), smem_u32(tiles), smem_u32(bars), lane);
+        runs, n_groups, W, gw, smem_u32(s_desc), smem_u32(tiles), smem_u32(sm.bars), lane);
     auto units = [&](uint32_t sl) { return s_desc[NB * sl].n_packets; };
     auto issue = [&](uint32_t sl, uint32_t pkt, uint32_t bar, uint32_t dst) {     // lanes b < NB issue run b's tile
         if (lane == 0) mbar_expect_tx(bar, NB * kTile);
@@ -343,14 +282,14 @@ k_mid(const LongRun *__restrict__ runs, uint32_t n_groups, const float *__restri
                 for (int b = 0; b < NB; b++) tp[b] = tiles + stage * kLongN2 + b * M::N2;
                 phase_a_m<KB>(tp, lane, tw, O[0], E[0]);
             }
-            transpose_abc(tw, deal.ring_s + stage * kLongTileBytes, lA0, lA1, lB, lC0, lC1, O, E);
+            transpose_abc<1>(tw, deal.ring_s + stage * kLongTileBytes, lA0, lA1, lB, lC0, lC1, O, E);
             deal.produce(units, issue);             // the stage is free again
             phase_c_fft<1>(tw, O, E);
             if (p > 0) {
-                out_stage_m<KB, false, OutT>(tw, lane, O[0], E[0], pe, flags, out, s_state + blk * M::N2);
+                out_block<M::W, M::N2 - M::W, false>(tw, lane >> KB, O[0], E[0], pe, flags, out, s_state + blk * M::N2);
             } else {
                 if (grp_state) deal.wait_state(c_grp, issue_state);
-                out_stage_m<KB, true, OutT>(tw, lane, O[0], E[0], pe, flags, out, s_state + blk * M::N2);
+                out_block<M::W, M::N2 - M::W, true>(tw, lane >> KB, O[0], E[0], pe, flags, out, s_state + blk * M::N2);
                 __syncwarp();
                 if (grp_state) deal.release_state(c_grp, group_has_state, issue_state);   // state tile consumed
             }
@@ -364,13 +303,13 @@ k_mid(const LongRun *__restrict__ runs, uint32_t n_groups, const float *__restri
 
 inline void mid_kernel_configure()
 {
-    cudaFuncSetAttribute(k_mid<float, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MidDev<1>::Smem);
-    cudaFuncSetAttribute(k_mid<int16_t, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MidDev<1>::Smem);
-    cudaFuncSetAttribute(k_mid<__half, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MidDev<1>::Smem);
-    cudaFuncSetAttribute(k_mid<float, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MidDev<2>::Smem);
-    cudaFuncSetAttribute(k_mid<int16_t, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MidDev<2>::Smem);
-    cudaFuncSetAttribute(k_mid<__half, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MidDev<2>::Smem);
     static_assert(MidDev<1>::Smem <= 232448 && MidDev<2>::Smem <= 232448, "k_mid's shared memory must fit one SM");
+    for (SampleKind k : {kSampleF32, kSampleI16, kSampleF16})
+        with_sample_type(k, [](auto t) {
+            using T = typename decltype(t)::type;
+            cudaFuncSetAttribute(k_mid<T, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MidDev<1>::Smem);
+            cudaFuncSetAttribute(k_mid<T, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MidDev<2>::Smem);
+        });
 }
 
 // kb: 1 -> n = 1024 (groups of two runs), 2 -> n = 512 (groups of four)

@@ -231,6 +231,42 @@ struct TwShort {
     }
 };
 
+// The CTA's shared window of k_short and k_short_g, 1 KB aligned: [ring: warps x Ring stages of StageBytes][pack]
+// [descriptors: DescBytes per warp][mbarriers: Ring per warp]
+template <int Ring, size_t StageBytes, size_t DescBytes>
+struct ShortSmem {
+    static constexpr size_t kRingBytes = (size_t)kShortWarps * Ring * StageBytes;
+    unsigned char *ring, *s_desc;
+    V *s_pack;
+    uint64_t *bars;
+    __device__ __forceinline__ ShortSmem(unsigned char *smem_raw, int warp)
+    {
+        unsigned char *base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+        unsigned char *tail = base + kRingBytes + (size_t)kShortPackFloats * 4;
+        ring = base + (size_t)warp * Ring * StageBytes;
+        s_pack = reinterpret_cast<V *>(base + kRingBytes);
+        s_desc = tail + (size_t)warp * DescBytes;
+        bars = reinterpret_cast<uint64_t *>(tail + (size_t)kShortWarps * DescBytes) + warp * Ring;
+    }
+};
+
+// The CTA set-up of k_short and k_short_g: stage the pack, init the first n_bars mbarriers of every warp, and load the
+// lane's resident twiddles (short-pack slots [kSTwReg0, kSTwReg1)) into twR.  The pack depends on l = lane & 3 only: the
+// shared copy keeps 4 lanes per slot (32 bytes), so that a warp's twiddle read is one multicast wavefront instead of two.
+__device__ __forceinline__ void short_cta_setup(const float *pack, V *s_pack, uint64_t *bars, int n_bars, int lane, V *twR)
+{
+    for (int i = threadIdx.x; i < SP_END * 4; i += blockDim.x)
+        s_pack[i] = reinterpret_cast<const V *>(pack)[(i >> 2) * 32 + (i & 3)];
+    if (lane == 0) {
+        for (int i = 0; i < n_bars; i++) mbar_init(smem_u32(&bars[i]), 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+#pragma unroll
+    for (int s = kSTwReg0; s < kSTwReg1; s++) twR[s - kSTwReg0] = s_pack[s * 4 + (lane & 3)];
+}
+constexpr int kSTwRegs = kSTwReg1 - kSTwReg0 > 0 ? kSTwReg1 - kSTwReg0 : 1;
+
 // PCM staging: one sample as OutT (samples.rs:86-103)
 __device__ __forceinline__ void sts_pcm(uint32_t addr, float v, float *) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory"); }
 // 2-byte samples (i16, f16) differ only in the conversion: one staging store for both
@@ -331,6 +367,30 @@ __device__ __forceinline__ void store_end_state_s(float *end_ptr, int l, const V
     }
 }
 
+// The end of a run whose last block a long block follows, the long block's kernel having run BEFORE this one
+// (ShortRun::tail): pcm[i] = x_long[ls + i] w[i] + prev[i] w[127 - i].  The first product comes from the long kernel at
+// end_ptr, prev is this block's right half (prev[m] == prev[127 - m] == p_even); the 128 samples go to `on`.
+template <typename OutT>
+__device__ __forceinline__ void short_tail(const TwShort &tw, int l, const V pe[8], const float *end_ptr, OutT *on)
+{
+    float cw[8][4];                              // all loads first: the stores below may alias them as far as the compiler knows
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        const int mx = outIndex_s(l, j, 0), my = outIndex_s(l, j, 1);
+        cw[j][0] = __ldcg(end_ptr + mx); cw[j][1] = __ldcg(end_ptr + my);
+        cw[j][2] = __ldcg(end_ptr + 127 - mx); cw[j][3] = __ldcg(end_ptr + 127 - my);
+    }
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        const int mx = outIndex_s(l, j, 0), my = outIndex_s(l, j, 1);
+        const V wlo = tw(P_WLO + j), whi = tw(P_WHI + j);
+        st_pcm(on + mx, __fadd_rn(cw[j][0], __fmul_rn(pe[j].x, whi.x)));
+        st_pcm(on + my, __fadd_rn(cw[j][1], __fmul_rn(pe[j].y, whi.y)));
+        st_pcm(on + 127 - mx, __fadd_rn(cw[j][2], __fmul_rn(pe[j].x, wlo.x)));
+        st_pcm(on + 127 - my, __fadd_rn(cw[j][3], __fmul_rn(pe[j].y, wlo.y)));
+    }
+}
+
 // runs: one descriptor per run; pack: short_build_pack of the setup's blocksize-8 tables.
 //
 // Short-block runs are short -- a burst between long blocks is one octet --, so the per-run latencies must overlap with
@@ -348,33 +408,18 @@ k_short(const ShortRun *__restrict__ runs, uint32_t n_runs, const float *__restr
     constexpr uint32_t ESZ = sizeof(OutT);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int l = lane & 3, blk = lane >> 2;
-    const uint32_t raw_s = smem_u32(smem_s);
-    unsigned char *base = smem_s + ((1024u - (raw_s & 1023u)) & 1023u);
-    constexpr size_t kRingBytes = (size_t)kShortWarps * kShortRing * kShortStageBytes;
-    unsigned char *ring = base + (size_t)warp * kShortRing * kShortStageBytes;
-    V *s_pack = reinterpret_cast<V *>(base + kRingBytes);
-    uint4 *s_desc = reinterpret_cast<uint4 *>(base + kRingBytes + (size_t)kShortPackFloats * 4) + warp * kShortDescSlots * 3;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(base + kRingBytes + (size_t)kShortPackFloats * 4 +
-                                                  (size_t)kShortWarps * kShortDescSlots * sizeof(ShortRun)) + warp * kShortRing;
-    // the pack depends on l = lane & 3 only: the shared copy keeps 4 lanes per slot (32 bytes), so that a warp's
-    // twiddle read is one multicast wavefront instead of two
-    for (int i = threadIdx.x; i < SP_END * 4; i += blockDim.x)
-        s_pack[i] = reinterpret_cast<const V *>(pack)[(i >> 2) * 32 + (i & 3)];
-    if (lane == 0) {
-        for (int i = 0; i < kShortRing; i++) mbar_init(smem_u32(&bars[i]), 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    V twR[kSTwReg1 - kSTwReg0 > 0 ? kSTwReg1 - kSTwReg0 : 1];
-#pragma unroll
-    for (int s = kSTwReg0; s < kSTwReg1; s++) twR[s - kSTwReg0] = s_pack[s * 4 + l];
-    const TwShort tw{twR, s_pack + l};
+    const ShortSmem<kShortRing, kShortStageBytes, kShortDescSlots * sizeof(ShortRun)> sm(smem_s, warp);
+    unsigned char *ring = sm.ring;
+    uint4 *s_desc = reinterpret_cast<uint4 *>(sm.s_desc);
+    V twR[kSTwRegs];
+    short_cta_setup(pack, sm.s_pack, sm.bars, kShortRing, lane, twR);
+    const TwShort tw{twR, sm.s_pack + l};
     const ShortLanes<OutT> ln(l, blk);
 
     const uint32_t W = gridDim.x * kShortWarps, gw = blockIdx.x * kShortWarps + warp;
     if (gw >= n_runs) return;
     StaticDeal<3, kShortDescSlots, kShortFetch, kShortRing, kShortStageBytes> deal(
-        runs, n_runs, W, gw, smem_u32(s_desc), smem_u32(ring), smem_u32(bars), lane);
+        runs, n_runs, W, gw, smem_u32(s_desc), smem_u32(ring), smem_u32(sm.bars), lane);
     // ShortRun fields inside the three quads: q0 = {in, out}, q1 = {state, in_stride, n_packets}, q2 = {has_prev | write_state << 8, ...}
     auto units = [&](uint32_t sl) { return (s_desc[3 * sl + 1].w + kShortOct - 1) / kShortOct; };
     auto issue = [&](uint32_t sl, uint32_t oct, uint32_t bar, uint32_t dst) {
@@ -470,27 +515,7 @@ k_short(const ShortRun *__restrict__ runs, uint32_t n_runs, const float *__restr
         }
         const bool last = (uint32_t)blk == ((npk - 1) & (kShortOct - 1));
         if (write_state && last) store_end_state_s(end_ptr, l, pe);
-        if (tail && last) {
-            // pcm[i] = x_long[ls + i] w[i] + prev[i] w[127 - i]: the first product comes from the long kernel, prev is this
-            // block's right half (prev[m] == prev[127 - m] == p_even)
-            OutT *on = out + (size_t)(npk - koff) * kShortN2;
-            float cw[8][4];                              // all loads first: the stores below may alias them as far as the compiler knows
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const int mx = outIndex_s(l, j, 0), my = outIndex_s(l, j, 1);
-                cw[j][0] = __ldcg(end_ptr + mx); cw[j][1] = __ldcg(end_ptr + my);
-                cw[j][2] = __ldcg(end_ptr + 127 - mx); cw[j][3] = __ldcg(end_ptr + 127 - my);
-            }
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const int mx = outIndex_s(l, j, 0), my = outIndex_s(l, j, 1);
-                const V wlo = tw(P_WLO + j), whi = tw(P_WHI + j);
-                st_pcm(on + mx, __fadd_rn(cw[j][0], __fmul_rn(pe[j].x, whi.x)));
-                st_pcm(on + my, __fadd_rn(cw[j][1], __fmul_rn(pe[j].y, whi.y)));
-                st_pcm(on + 127 - mx, __fadd_rn(cw[j][2], __fmul_rn(pe[j].x, wlo.x)));
-                st_pcm(on + 127 - my, __fadd_rn(cw[j][3], __fmul_rn(pe[j].y, wlo.y)));
-            }
-        }
+        if (tail && last) short_tail(tw, l, pe, end_ptr, out + (size_t)(npk - koff) * kShortN2);
     }
 }
 
@@ -520,32 +545,19 @@ k_short_g(const ShortRun *__restrict__ runs, uint32_t n_groups, const float *__r
     constexpr uint32_t ESZ = sizeof(OutT);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int l = lane & 3, blk = lane >> 2;
-    const uint32_t raw_s = smem_u32(smem_s);
-    unsigned char *base = smem_s + ((1024u - (raw_s & 1023u)) & 1023u);
-    constexpr size_t kRingBytes = (size_t)kShortWarps * kShortGRing * kShortGStageBytes;
-    unsigned char *ring = base + (size_t)warp * kShortGRing * kShortGStageBytes;
-    V *s_pack = reinterpret_cast<V *>(base + kRingBytes);
-    ShortRun *s_desc = reinterpret_cast<ShortRun *>(base + kRingBytes + (size_t)kShortPackFloats * 4) + warp * kShortGDescSlots * kShortOct;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(base + kRingBytes + (size_t)kShortPackFloats * 4 +
-                                                  (size_t)kShortWarps * kShortGDescSlots * kShortGDescBytes) + warp * kShortGRing;
-    for (int i = threadIdx.x; i < SP_END * 4; i += blockDim.x)
-        s_pack[i] = reinterpret_cast<const V *>(pack)[(i >> 2) * 32 + (i & 3)];
-    if (lane == 0) {
-        for (int i = 0; i < kShortGRing; i++) mbar_init(smem_u32(&bars[i]), 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    V twR[kSTwReg1 - kSTwReg0 > 0 ? kSTwReg1 - kSTwReg0 : 1];
-#pragma unroll
-    for (int s = kSTwReg0; s < kSTwReg1; s++) twR[s - kSTwReg0] = s_pack[s * 4 + l];
-    const TwShort tw{twR, s_pack + l};
+    const ShortSmem<kShortGRing, kShortGStageBytes, kShortGDescSlots * kShortGDescBytes> sm(smem_s, warp);
+    unsigned char *ring = sm.ring;
+    ShortRun *s_desc = reinterpret_cast<ShortRun *>(sm.s_desc);
+    V twR[kSTwRegs];
+    short_cta_setup(pack, sm.s_pack, sm.bars, kShortGRing, lane, twR);
+    const TwShort tw{twR, sm.s_pack + l};
     const ShortLanes<OutT> ln(l, blk);
     constexpr uint32_t kStateOff = kShortOct * kShortTileStride;               // state tile of block b at + 512 b
 
     const uint32_t W = gridDim.x * kShortWarps, gw = blockIdx.x * kShortWarps + warp;
     if (gw >= n_groups) return;
     StaticDeal<kShortGDescBytes / 16, kShortGDescSlots, kShortGFetch, kShortGRing, kShortGStageBytes> deal(
-        runs, n_groups, W, gw, smem_u32(s_desc), smem_u32(ring), smem_u32(bars), lane);
+        runs, n_groups, W, gw, smem_u32(s_desc), smem_u32(ring), smem_u32(sm.bars), lane);
     auto units = [&](uint32_t sl) { return s_desc[sl * kShortOct].n_packets; };
     auto issue = [&](uint32_t sl, uint32_t t, uint32_t bar, uint32_t dst) {     // lane b < 8 issues block position b's copies
         const ShortRun *g = s_desc + sl * kShortOct;
@@ -614,25 +626,7 @@ k_short_g(const ShortRun *__restrict__ runs, uint32_t n_groups, const float *__r
         }
         float *end_ptr = g[blk].end_ptr ? g[blk].end_ptr : g[blk].state;
         if (valid && g[blk].write_state) store_end_state_s(end_ptr, l, pe);
-        if (valid && g[blk].tail) {
-            OutT *on = static_cast<OutT *>(g[blk].out) + (size_t)(npk - (has_prev ? 0u : 1u)) * kShortN2;
-            float cw[8][4];
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const int mx = outIndex_s(l, j, 0), my = outIndex_s(l, j, 1);
-                cw[j][0] = __ldcg(end_ptr + mx); cw[j][1] = __ldcg(end_ptr + my);
-                cw[j][2] = __ldcg(end_ptr + 127 - mx); cw[j][3] = __ldcg(end_ptr + 127 - my);
-            }
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const int mx = outIndex_s(l, j, 0), my = outIndex_s(l, j, 1);
-                const V wlo = tw(P_WLO + j), whi = tw(P_WHI + j);
-                st_pcm(on + mx, __fadd_rn(cw[j][0], __fmul_rn(pe[j].x, whi.x)));
-                st_pcm(on + my, __fadd_rn(cw[j][1], __fmul_rn(pe[j].y, whi.y)));
-                st_pcm(on + 127 - mx, __fadd_rn(cw[j][2], __fmul_rn(pe[j].x, wlo.x)));
-                st_pcm(on + 127 - my, __fadd_rn(cw[j][3], __fmul_rn(pe[j].y, wlo.y)));
-            }
-        }
+        if (valid && g[blk].tail) short_tail(tw, l, pe, end_ptr, static_cast<OutT *>(g[blk].out) + (size_t)(npk - (has_prev ? 0u : 1u)) * kShortN2);
     }
 }
 
@@ -650,12 +644,12 @@ inline int short_launch_groups(cudaStream_t stream, const ShortRun *d_runs, uint
 
 inline void short_kernel_configure()
 {
-    cudaFuncSetAttribute(k_short<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kShortSmemBytes);
-    cudaFuncSetAttribute(k_short<int16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kShortSmemBytes);
-    cudaFuncSetAttribute(k_short<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kShortSmemBytes);
-    cudaFuncSetAttribute(k_short_g<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kShortGSmemBytes);
-    cudaFuncSetAttribute(k_short_g<int16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kShortGSmemBytes);
-    cudaFuncSetAttribute(k_short_g<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kShortGSmemBytes);
+    for (SampleKind k : {kSampleF32, kSampleI16, kSampleF16})
+        with_sample_type(k, [](auto t) {
+            using T = typename decltype(t)::type;
+            cudaFuncSetAttribute(k_short<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kShortSmemBytes);
+            cudaFuncSetAttribute(k_short_g<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kShortGSmemBytes);
+        });
 }
 
 inline int short_launch(cudaStream_t stream, const ShortRun *d_runs, uint32_t n_runs, const float *d_pack, int sm_count, SampleKind kind)

@@ -742,30 +742,31 @@ static int front_stages_run(lwb_ctx *ctx, const lwb_batch_io *io, const FrontSta
 // ---------------------------------------------------------------------------------------------
 // the launches of the fused paths and the chain-kernel path (Step)
 // ---------------------------------------------------------------------------------------------
-template <int ENTRY, bool MIX>
-static int launch_chain(lwb_ctx *ctx, int fmt, unsigned n_chains, unsigned warps, size_t smem, const ChainDesc *d,
-                        const uint8_t *bytes, const float *coeffs, const float *dense, const uint8_t *kinds,
-                        const uint32_t *ys, void *pcm, int n1max, int wpc, int np, const float *zero, VqDev vq)
+// k_chain for the batch's entry, output format, mix and warps per chain
+static int launch_chain(lwb_ctx *ctx, const StepArgs &a, uint32_t n_chains, const ChainDesc *d)
 {
-    return with_out_format(fmt, [&](auto f) {
-        constexpr int F = decltype(f)::value;
-        if (wpc == 1) {
-            cudaFuncSetAttribute(k_chain<F, ENTRY, false, MIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, false, MIX>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense,
-                          kinds, ys, pcm, n1max, wpc, np, zero, vq);
+    auto entry = [&](auto go) {
+        switch (a.entry) {
+        case LWB_ENTRY_VQ: return go(std::integral_constant<int, LWB_ENTRY_VQ>());
+        case LWB_ENTRY_RESIDUE: return go(std::integral_constant<int, LWB_ENTRY_RESIDUE>());
+        default: return go(std::integral_constant<int, LWB_ENTRY_SPECTRUM>());
         }
-        cudaFuncSetAttribute(k_chain<F, ENTRY, true, MIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, true, MIX>, dim3(n_chains), dim3(warps * 32), smem, d, bytes, coeffs, dense, kinds,
-                      ys, pcm, n1max, wpc, 1, zero, vq);
+    };
+    return entry([&](auto e) {
+        return with_out_format(a.out_format, [&](auto f) {
+            constexpr int ENTRY = decltype(e)::value, F = decltype(f)::value;
+            auto go = [&](auto wide, auto mix) {         // wide: more than one warp per chain
+                constexpr bool WIDE = decltype(wide)::value, MIX = decltype(mix)::value;
+                cudaFuncSetAttribute(k_chain<F, ENTRY, WIDE, MIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)a.chain.smem);
+                return launch(ctx, LWB_KERNEL_CHAIN, k_chain<F, ENTRY, WIDE, MIX>, dim3(n_chains), dim3(a.chain.warps * 32), a.chain.smem, d,
+                              a.bytes, a.coeffs, a.dense, a.kinds, a.ys, a.pcm, a.chain.n1max, a.chain.wpc, WIDE ? 1 : a.chain.np, a.zero, a.vq);
+            };
+            const std::true_type yes;
+            const std::false_type no;
+            if (a.chain.wpc == 1) return a.mix ? go(no, yes) : go(no, no);
+            return a.mix ? go(yes, yes) : go(yes, no);
+        });
     });
-}
-template <int ENTRY>
-static int launch_chain(lwb_ctx *ctx, bool mix, int fmt, unsigned n_chains, unsigned warps, size_t smem, const ChainDesc *d,
-                        const uint8_t *bytes, const float *coeffs, const float *dense, const uint8_t *kinds,
-                        const uint32_t *ys, void *pcm, int n1max, int wpc, int np, const float *zero, VqDev vq)
-{
-    return mix ? launch_chain<ENTRY, true>(ctx, fmt, n_chains, warps, smem, d, bytes, coeffs, dense, kinds, ys, pcm, n1max, wpc, np, zero, vq)
-               : launch_chain<ENTRY, false>(ctx, fmt, n_chains, warps, smem, d, bytes, coeffs, dense, kinds, ys, pcm, n1max, wpc, np, zero, vq);
 }
 
 __global__ void __launch_bounds__(kRowCopyThreads) k_row_copy(const RowCopy *__restrict__ rc);   // path_chain.cuh
@@ -803,15 +804,7 @@ static int run_steps(lwb_ctx *ctx, const StepArgs &a, const std::vector<Step> &s
                           "short burst kernel launch");
             break;
         case LWB_KERNEL_CHAIN:
-            if (a.entry == LWB_ENTRY_VQ)
-                rc = launch_chain<LWB_ENTRY_VQ>(ctx, a.mix, a.out_format, n, a.chain.warps, a.chain.smem, (const ChainDesc *)s.desc, a.bytes, a.coeffs,
-                                                a.dense, a.kinds, a.ys, a.pcm, a.chain.n1max, a.chain.wpc, a.chain.np, a.zero, a.vq);
-            else if (a.entry == LWB_ENTRY_RESIDUE)
-                rc = launch_chain<LWB_ENTRY_RESIDUE>(ctx, a.mix, a.out_format, n, a.chain.warps, a.chain.smem, (const ChainDesc *)s.desc, a.bytes, a.coeffs,
-                                                     a.dense, a.kinds, a.ys, a.pcm, a.chain.n1max, a.chain.wpc, a.chain.np, a.zero, a.vq);
-            else
-                rc = launch_chain<LWB_ENTRY_SPECTRUM>(ctx, a.mix, a.out_format, n, a.chain.warps, a.chain.smem, (const ChainDesc *)s.desc, a.bytes, a.coeffs,
-                                                      a.dense, a.kinds, a.ys, a.pcm, a.chain.n1max, a.chain.wpc, a.chain.np, a.zero, a.vq);
+            rc = launch_chain(ctx, a, n, (const ChainDesc *)s.desc);
             break;
         default:
             return fail(ctx, LWB_ERR_INVALID, "internal: no step for this kernel");

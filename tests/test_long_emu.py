@@ -92,7 +92,7 @@ def test_emulated_kernel_special_values(emu, pack, oracle):
 
 @pytest.mark.parametrize("seed,npk,prev", [(20, 4, (0, 0)), (21, 3, (1, 0)), (22, 1, (0, 1)), (23, 5, (1, 1))])
 def test_emulated_dual_block_matches_oracle(emu, pack, oracle, seed, npk, prev):
-    """NB = 2: a warp transforms two runs in lockstep (the shipped configuration)."""
+    """NB = 2: a warp transforms two runs in lockstep (LWB_LONG_NB=2; the shipped configuration is NB = 1)."""
     rng = np.random.default_rng(seed)
     spec = rng.standard_normal((2, npk, 1024)).astype(np.float32)
     states = rng.standard_normal((2, 1024)).astype(np.float32)
