@@ -119,7 +119,7 @@ LWB_HD void d_floor1_render_segment(const uint16_t *sx, const uint16_t *sy, int 
     }
 }
 
-// ---- chunked closed-form render (k_floor1_curves) -------------------------------------------
+// ---- division-free closed form (d_floor1_pack_segment, k_floor1_segments) ----------------------
 // floor(N / adx) for N = |dy| * (k - x0) < 2^20 (|dy| < 2^8, k - x0 < n/2 <= 2^12) by one multiply-high, no
 // division anywhere:  M = floor((2^(32+s) - 1) / adx) + 1,  floor(N / adx) == mulhi(N, M) >> s  whenever
 // N * adx < 2^(32+s)  (M * adx = 2^(32+s) + e with 0 < e <= adx, and the error term N * e / (adx * 2^(32+s)) stays
@@ -175,53 +175,6 @@ LWB_HD uint32_t d_floor1_seg_y(const Seg4 &s, int k)
     if (SHIFT) q >>= (s.y & 2u) ? 12 : 0;
     const uint32_t y0 = (s.y >> 8) & 255u, neg = 0u - (s.y & 1u);
     return y0 + ((q ^ neg) - neg);
-}
-
-// Prepares segment j of a row for d_floor1_render16: magic multiplier into sm[j], its shift into the (unused) high
-// byte of sy[j] (curve values are <= 255: posts are clamped to range - 1 and range * multiplier <= 256).
-LWB_HD void d_floor1_prepare_segment(const uint16_t *sx, uint16_t *sy, uint32_t *sm, int j)
-{
-    int sh;
-    sm[j] = d_floor1_magic((int)sx[j + 1] - (int)sx[j], &sh);
-    sy[j] = (uint16_t)((sy[j] & 255u) | ((uint32_t)sh << 8));
-}
-
-// 16 consecutive bins [k0, k0 + 16) of the rendered curve (k0 + 16 <= n2 <= last sx), one byte each, as four
-// little-endian words: the closed form of render_line (audio.rs:503-524) per bin, segment found once per chunk
-// and advanced when a bin reaches the next flagged post.  Segments prepared by d_floor1_prepare_segment.
-LWB_HD void d_floor1_render16(const uint16_t *sx, const uint16_t *sy, const uint32_t *sm, int m, int k0, uint32_t out[4])
-{
-    int lo = 0, hi = m - 1;                  // sx[lo] <= k0 < sx[hi]
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if ((int)sx[mid] <= k0) lo = mid; else hi = mid;
-    }
-    int x1 = sx[lo + 1], y0 = sy[lo] & 255, sh = sy[lo] >> 8;
-    int dy = (int)(sy[lo + 1] & 255) - y0;
-    uint32_t mg = sm[lo];
-    uint32_t ady = (uint32_t)(dy < 0 ? -dy : dy);
-    int sgn = dy < 0 ? -1 : 1;
-    uint32_t nn = ady * (uint32_t)(k0 - (int)sx[lo]);
-#pragma unroll
-    for (int w = 0; w < 4; w++) {
-        uint32_t word = 0;
-#pragma unroll
-        for (int b = 0; b < 4; b++) {
-            if (k0 + 4 * w + b >= x1) {      // posts are strictly increasing in x: one step is enough
-                lo++;
-                x1 = sx[lo + 1]; y0 = sy[lo] & 255; sh = sy[lo] >> 8;
-                dy = (int)(sy[lo + 1] & 255) - y0;
-                mg = sm[lo];
-                ady = (uint32_t)(dy < 0 ? -dy : dy);
-                sgn = dy < 0 ? -1 : 1;
-                nn = 0;
-            }
-            const int y = y0 + sgn * (int)(d_mulhi_u32(nn, mg) >> sh);      // 0 <= y <= 255
-            word |= (uint32_t)y << (8 * b);
-            nn += ady;
-        }
-        out[w] = word;
-    }
 }
 
 }  // namespace lwb

@@ -180,8 +180,9 @@ template <bool SHIFT>
 __device__ __forceinline__ float4 d_floor_quad_one(const float *__restrict__ s_db, const uint4 *__restrict__ tab,
                                                    const unsigned char *__restrict__ ix, int words, int k0)
 {
-    // segment of bin k = (number of flagged posts with x <= k) - 1; the post at x = 0 is always flagged.  The four
-    // bins of a quad share one bitmap word and look their segments up independently of one another.
+    // segment of bin k = (number of flagged posts with x <= k) - 1.  Post 0 is always flagged (d_floor1_posts), and
+    // prepare_floor1 refuses every x list whose post 0 is not at x = 0, so every bin has a segment.  The four bins of a
+    // quad share one bitmap word and look their segments up independently of one another.
     const uint32_t bits = reinterpret_cast<const uint32_t *>(ix)[k0 >> 5];
     const int pre = (int)ix[(size_t)words * 4 + (k0 >> 5)] - 1;
     float f[4];

@@ -78,8 +78,10 @@ int generate_tables(int bs, float *a, float *b, float *c, float *window, uint32_
 
 // Fills sorted order (header.rs:887-889) and the low/high neighbour of every post i >= 2
 // (audio.rs:253-292: the closest smaller / larger x among posts 0..i).  Returns LWB_OK, or
-// LWB_ERR_BAD_FORMAT for lists the header parser rejects (duplicates, header.rs:890-901) or
-// for which the reference's neighbour search would panic.
+// LWB_ERR_BAD_FORMAT for lists the header parser cannot produce (post 0 not at x = 0: it always
+// makes [0, 1 << rangebits, ...], header.rs:877-879; duplicates, :890-901) or for which the
+// reference's neighbour search would panic.  Post 0 at x = 0 is what lets every kernel start the
+// curve at its first flagged post: render_line covers bins from lx = 0 (audio.rs:532-541).
 int prepare_floor1(const lwb_floor_desc &d, DevFloor1 *out)
 {
     std::memset(out, 0, sizeof(*out));
@@ -88,6 +90,7 @@ int prepare_floor1(const lwb_floor_desc &d, DevFloor1 *out)
     const int np = d.floor1_values;
     if (np < 2 || np > LWB_MAX_POSTS) return LWB_ERR_BAD_FORMAT;
     if (d.floor1_multiplier < 1 || d.floor1_multiplier > 4) return LWB_ERR_BAD_FORMAT;
+    if (d.floor1_x_list[0] != 0) return LWB_ERR_BAD_FORMAT;
     out->mult = d.floor1_multiplier;
     out->nposts = static_cast<uint8_t>(np);
     for (int i = 0; i < np; i++) {

@@ -8,7 +8,7 @@
 #include "../../lewton_b200/csrc/tables_host.cpp"
 
 extern "C" int lwb_emu_floor1(int mult, const uint32_t *xs, int nposts, const uint32_t *y, int n2,
-                              uint32_t *curve_closed, uint8_t *curve_render, uint8_t *curve_chunks, uint8_t *curve_packed)
+                              uint32_t *curve_closed, uint8_t *curve_render, uint8_t *curve_packed)
 {
     lwb_floor_desc d;
     std::memset(&d, 0, sizeof(d));
@@ -24,14 +24,6 @@ extern "C" int lwb_emu_floor1(int mult, const uint32_t *xs, int nposts, const ui
     for (int k = 0; k < n2; k++) curve_closed[k] = lwb::d_floor1_y_at(sx, sy, m, k);
     std::memset(curve_render, 0xee, (size_t)n2);
     for (int seg = 0; seg + 1 < m; seg++) lwb::d_floor1_render_segment(sx, sy, seg, n2, curve_render);
-    // the chunked closed-form render of k_floor1_curves (16 bins per work item, multiply-high division)
-    uint32_t sm[LWB_MAX_POSTS + 1];
-    for (int j = 0; j + 1 < m; j++) lwb::d_floor1_prepare_segment(sx, sy, sm, j);
-    for (int k0 = 0; k0 < n2; k0 += 16) {
-        uint32_t w[4];
-        lwb::d_floor1_render16(sx, sy, sm, m, k0, w);
-        std::memcpy(curve_chunks + k0, w, 16);
-    }
     // the packed-segment evaluation of k_prologue_fused: per bin, segment advanced without branches
     {
         lwb::Seg4 tab[LWB_MAX_POSTS + 2];
@@ -48,7 +40,7 @@ extern "C" int lwb_emu_floor1(int mult, const uint32_t *xs, int nposts, const ui
     return 0;
 }
 
-// exactness of the multiply-high division used by d_floor1_render16: every adx up to 2^15, every |dy|, dense t
+// exactness of the multiply-high division d_floor1_pack_segment packs into each segment: every adx up to 2^15, every |dy|, dense t
 extern "C" long lwb_emu_magic_mismatches(int adx_lo, int adx_hi)
 {
     long bad = 0;

@@ -1,6 +1,6 @@
 """CPU emulation of the GPU's floor-1 evaluation (tests/emu/floor1_emu.cpp compiles
-lewton_b200/csrc/floor1_eval.cuh for the host): post unwrap + closed-form curve + DDA segment render
-against the oracle's literal restatement of audio.rs:391-555, on random floors incl. wild post values,
+lewton_b200/csrc/floor1_eval.cuh for the host): post unwrap + closed-form curve + DDA segment render +
+the packed segments of k_prologue_fused against the oracle's literal restatement of audio.rs:391-555, on random floors incl. wild post values,
 posts beyond n/2 and early-ending x lists."""
 import ctypes as C
 import os
@@ -25,7 +25,7 @@ def build():
 
 
 @pytest.mark.parametrize("seed", range(8))
-def test_floor1_posts_closed_form_and_dda_render_match_the_oracle(oracle, seed):
+def test_floor1_posts_closed_form_dda_and_packed_segments_match_the_oracle(oracle, seed):
     L = C.CDLL(build())
     rng = np.random.default_rng(1000 + seed)
     for case in range(150):
@@ -38,20 +38,19 @@ def test_floor1_posts_closed_form_and_dda_render_match_the_oracle(oracle, seed):
         xa, ya = np.array(xs, np.uint32), np.array(y, np.uint32)
         closed = np.zeros(n2, np.uint32)
         render = np.zeros(n2, np.uint8)
-        chunks = np.zeros(n2, np.uint8)
         packed = np.zeros(n2, np.uint8)
         rc = L.lwb_emu_floor1(mult, xa.ctypes.data_as(C.c_void_p), len(xs), ya.ctypes.data_as(C.c_void_p), n2,
                               closed.ctypes.data_as(C.c_void_p), render.ctypes.data_as(C.c_void_p),
-                              chunks.ctypes.data_as(C.c_void_p), packed.ctypes.data_as(C.c_void_p))
+                              packed.ctypes.data_as(C.c_void_p))
         assert rc == 0
         assert np.array_equal(packed.astype(np.uint32), want & 255), (seed, case, np.nonzero(packed != (want & 255))[0][:5])
-        assert np.array_equal(chunks.astype(np.uint32), want & 255), (seed, case, np.nonzero(chunks != (want & 255))[0][:5])
         assert np.array_equal(closed & 255, want & 255), (seed, case)
         assert np.array_equal(render.astype(np.uint32), want & 255), (seed, case, np.nonzero(render != (want & 255))[0][:5])
 
 
-def test_multiply_high_division_is_exact():
-    """d_floor1_magic / d_mulhi_u32 == integer division for every segment length it is used for."""
+def test_packed_segment_multiply_high_division_is_exact():
+    """d_floor1_magic / d_mulhi_u32, the division d_floor1_pack_segment packs into each segment for k_prologue_fused,
+    == integer division for every segment length it is used for."""
     L = C.CDLL(build())
     L.lwb_emu_magic_mismatches.restype = C.c_long
     assert L.lwb_emu_magic_mismatches(1, 32768) == 0

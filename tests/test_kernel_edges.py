@@ -16,6 +16,7 @@ and the final stream state bit for bit.  Each case names the kernel that must ha
 import numpy as np
 import pytest
 
+import floor1_cases as fc
 import lewton_b200 as L
 from lewton_b200 import _cabi as cabi
 from helpers import (ALL_KERNELS, FRONT, RefStream, bits_equal, expect_kernels, launches_are_attributed,
@@ -263,34 +264,6 @@ def _long_segment_xs(rng, rangebits, n2):
     return xs, above - below
 
 
-def _unwrap(xs, mult, y):
-    """Floor-1 step 1 (audio.rs:391-435, like the oracle's lwo_floor1_amplitude) in Python integers.  Returns the
-    products ady * (x - x0) render_point forms (u32 in the reference: >= 2^32 wraps) and the final y values before the
-    clamp to range - 1 (as u32).  Asserts that the signed step-2 arithmetic stays inside i32, where the reference and
-    the oracle agree."""
-    rng_y = [256, 128, 86, 64][mult - 1]
-    i32 = lambda v: ((v + (1 << 31)) & 0xffffffff) - (1 << 31)
-    fy, prods = [y[0], y[1]], []
-    for i in range(2, len(xs)):
-        lo = max((j for j in range(i) if xs[j] < xs[i]), key=lambda j: xs[j])
-        hi = min((j for j in range(i) if xs[j] > xs[i]), key=lambda j: xs[j])
-        dy = i32(fy[hi] - fy[lo])
-        prods.append(abs(dy) * (xs[i] - xs[lo]))
-        off = (prods[-1] & 0xffffffff) // (xs[hi] - xs[lo])
-        pred = i32(fy[lo] - off if dy < 0 else fy[lo] + off)
-        val, highroom, lowroom = y[i], rng_y - pred, pred
-        room = min(highroom, lowroom) * 2
-        if val <= 0:
-            r = pred
-        elif val >= room:
-            r = pred + val - lowroom if highroom > lowroom else pred - val + highroom - 1
-        else:
-            r = pred + ((-val - 1 if val % 2 == 1 else val) >> 1)
-        assert all(-(1 << 31) <= v < (1 << 31) for v in (highroom, room, r)), "beyond the reference's i32 arithmetic"
-        fy.append(r & 0xffffffff)
-    return prods, fy
-
-
 def _wild_y(rng, mult, nposts):
     rng_y = [256, 128, 86, 64][mult - 1]
     y = [int(rng.integers(rng_y - 1, 256)), int(rng.integers(0, 256))]      # posts 0 / 1: at range - 1 and above
@@ -330,7 +303,7 @@ def test_floor1_long_segments_and_wild_posts(ctx, oracle, n, rangebits):
             for c in range(C):
                 mult = floors[mappings[mode_ids[i]]["floor_of_channel"][c]][0]
                 y = _wild_y(rng, mult, 65)
-                prods, fy = _unwrap(floors[mappings[mode_ids[i]]["floor_of_channel"][c]][1], mult, y)
+                prods, fy, _ = fc.unwrap(floors[mappings[mode_ids[i]]["floor_of_channel"][c]][1], mult, y)
                 wraps += sum(v >= 1 << 32 for v in prods)
                 at_edge += sum(v == [256, 128, 86, 64][mult - 1] - 1 for v in fy)
                 above += sum(v > [256, 128, 86, 64][mult - 1] - 1 for v in fy)
