@@ -221,6 +221,77 @@ void lwf_batcher_last_timing(const lwf_batcher *b, double *entropy_seconds, doub
  * records, dense floor-0 curves, floor kinds and floor1_y rows): what its batches copy to the device */
 uint64_t lwf_batcher_last_input_bytes(const lwf_batcher *b);
 
+/* ---- many OggStreamReaders at once: the reader's semantics on the batcher's synthesis ---------- */
+/* Each reader is an lwf_reader over its own bytes; one lwf_readers_read advances many of them.  Their Ogg de-paging and
+ * sample counting, then their entropy decode, run on the host thread pool; their synthesis is one lwb_submit_chains
+ * batch per group of equal channel count and blocksize pair, as lwf_batcher_submit makes it (residue entry, dense
+ * floor-0 curves, as lwf_reader decodes).  Each reader returns exactly what a single lwf_reader would return for the
+ * same bytes.  Seeking and skipping stay on lwf_reader. */
+typedef struct lwf_readers lwf_readers;     /* many OggStreamReaders on one ctx, one host thread pool */
+int lwf_readers_create(lwb_ctx *ctx, int threads, lwf_readers **out);       /* threads <= 0: one per host CPU */
+void lwf_readers_destroy(lwf_readers *rs);                                   /* waits for its queued reads */
+/* lwf_reader_open for one more reader: reads its headers; `data` is not copied and must outlive the reader.  Readers whose
+ * ident and setup header bytes are equal share one parsed setup header (parsed once), one lwb_setup and one header set of
+ * the entropy decode; each reader's own lwf_headers holds its comments and gives the shared set's info and decode.  The
+ * device setup and the reader's stream state are made by the first lwf_readers_read that reads it. */
+int lwf_readers_add(lwf_readers *rs, const uint8_t *data, size_t len, uint32_t *index);
+const lwf_headers *lwf_readers_headers(const lwf_readers *rs, uint32_t index); /* the stream its NEXT packet belongs to */
+int lwf_readers_last_absgp(const lwf_readers *rs, uint32_t index, uint64_t *absgp); /* as lwf_reader_last_absgp */
+/* distinct (ident, setup) header byte pairs among the streams the readers have opened: one lwb_setup each */
+uint32_t lwf_readers_setup_count(const lwf_readers *rs);
+/* wall-clock seconds of the last accepted lwf_readers_read: the de-paging and sample counting pass, and the
+ * internal batcher's entropy decode and rest of its submit (lwf_batcher_last_timing) */
+void lwf_readers_last_timing(const lwf_readers *rs, double *paging_seconds, double *entropy_seconds, double *synthesis_seconds);
+
+typedef struct lwf_read_job {
+    uint32_t reader;          /* index from lwf_readers_add; a reader may appear in at most one job per call */
+    uint32_t max_packets;     /* read at most this many audio packets (calls of lwf_reader_read_dec_packet)  */
+    uint64_t out_offset;      /* element offset of this job's PCM in `pcm`                                  */
+    uint64_t out_stride;      /* planar: elements between channel planes                                    */
+    uint32_t *packet_samples; /* optional [max_packets]: samples each returned packet wrote (NULL: not wanted) */
+    /* results */
+    uint32_t n_packets;       /* packets returned (what that many single-reader calls would have returned)   */
+    uint32_t n_samples;       /* samples per channel written: the concatenation of those packets' PCM       */
+    uint8_t  channels;        /* channel count of the stream the packets belong to                           */
+    uint8_t  next_chained;    /* 1: the reader now stands at a new logical stream (headers already read)     */
+    uint8_t  ended;           /* 1: no packet left (the single reader's LWF_ERR_NO_MORE_PACKETS)             */
+    uint8_t  reserved;
+    int32_t  status;          /* LWB_OK, or the code the single reader's call for packet n_packets returned  */
+} lwf_read_job;
+/* Reads up to max_packets audio packets from each job's reader and queues their synthesis, asynchronously, in the manner
+ * of lwf_batcher_submit.
+ * Equivalence: the PCM a job writes, and packet_samples, are those of n_packets consecutive lwf_reader_read_dec_packet
+ * calls on a single reader over the same bytes, concatenated: written sample j of the job goes to out_offset + c *
+ * out_stride + j (planar) or out_offset + j * channels + c (interleaved).  f32 is bit for bit the single reader's (up to
+ * the sign of zero and NaN payloads), i16 and f16 exactly.  status, lwf_readers_last_absgp and the absgp accounting, and
+ * (but for a chained stream, below) lwf_readers_headers are that reader's after those calls.  Nothing outside the
+ * job's n_samples samples per channel is written.
+ * Errors: a job stops at its first failing packet.  That packet is consumed, as in the single reader; its code
+ * (LWB_ERR_BAD_FORMAT, LWF_ERR_END_OF_PACKET, LWF_ERR_AUDIO_IS_HEADER, an Ogg or header error) goes to status, and the
+ * reader's next call continues after it.  A job that reads past the last packet sets ended and keeps status LWB_OK.
+ * LWB_ERR_MISMATCH in status: the samples the batch wrote differ from the sum of packet_samples, which come from the
+ * packets' headers (window flags that disagree with the block before, and that the synthesis did not refuse); the
+ * reader has advanced as the other results say.
+ * Chained streams: a job never spans two logical streams, so its layout has one channel count (`channels`).  When the
+ * next packet begins a new stream the job stops there and reads the new headers (a header error goes to status), and
+ * next_chained is set: lwf_readers_headers then gives the new stream, whose channel count and blocksizes lay out the next
+ * job.  That next job decodes and drops the new stream's first audio packet first, as read_next_audio_packet does.
+ * End of stream: the last packet is truncated to its page's granule position by the stream's output window
+ * (lwb_stream_set_window) set for that job alone: the batch keeps its fused kernel and there is no host pass over PCM.
+ * Before it returns, the de-paging and entropy decode are done, every job's results are written and the readers have
+ * advanced, so they can be read again at once; *ticket (as lwf_batcher_submit's) completes once the PCM is in `pcm`.
+ * pcm_memory, page-locked host memory, tickets, the ring of two arena sets and the places the call blocks are
+ * lwf_batcher_submit's.
+ * Refusals -- LWB_ERR_INVALID for a NULL rs, jobs, pcm or ticket, n_jobs == 0, a pcm_memory other than LWB_MEM_HOST and
+ * LWB_MEM_DEVICE, an unknown out_format, an unknown reader index, a reader in two jobs, a planar job whose out_stride is
+ * below max_packets * blocksize_1 / 2 + (blocksize_1 - blocksize_0) / 4 of its reader's stream (the most max_packets
+ * packets can return: a long block before a short one returns (3 blocksize_1 - blocksize_0) / 4), and anything
+ * lwf_batcher_submit refuses (pageable host PCM among them); or the error of making a reader's device setup or stream -- change no job, reader or PCM element and issue
+ * no ticket.  After LWB_ERR_CUDA or LWB_ERR_BUFFER from a later group's batch, the jobs of the groups queued before it
+ * have their results and their readers have advanced; the others are unchanged. */
+int lwf_readers_read(lwf_readers *rs, lwf_read_job *jobs, size_t n_jobs, int out_format, void *pcm, int pcm_memory,
+                     uint64_t *ticket);
+
 /* ---- debug taps (known-answer tests of the reference's unit-test vectors) ---------------------- */
 float lwf_debug_float32_unpack(uint32_t v);                          /* bitpacking.rs:304-314        */
 uint32_t lwf_debug_lookup1_values(uint32_t entries, uint16_t dims);  /* header.rs:616-649            */

@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "liblewton_b200.so")
 K_LONG_REGS = 249          # k_long's registers per thread in the measured H100 build (DESIGN.md 4.1)
 SOURCES = ["lwb_api.cu", "host_objects.cuh", "path_generic.cuh", "path_long.cuh", "path_chain.cuh", "path_mixed.cuh", "path_mid.cuh",
-           "tables_host.cpp", "frontend.cpp", "batcher_submit.cpp", "batcher.h", "lwb_common.h", "pcm_copy_plan.h", "kernels_generic.cuh", "kernel_long.cuh", "kernel_deal.cuh", "kernel_short.cuh", "kernel_mid.cuh", "kernel_chain.cuh", "kernel_prologue.cuh", "kernel_floor0.cuh", "floor1_eval.cuh",
+           "tables_host.cpp", "frontend.cpp", "batcher_submit.cpp", "readers.cpp", "batcher.h", "lwb_common.h", "pcm_copy_plan.h", "kernels_generic.cuh", "kernel_long.cuh", "kernel_deal.cuh", "kernel_short.cuh", "kernel_mid.cuh", "kernel_chain.cuh", "kernel_prologue.cuh", "kernel_floor0.cuh", "floor1_eval.cuh",
            "floor1_inverse_db.inc", "Makefile"]
 
 

@@ -8,6 +8,7 @@
 #define LWF_BATCHER_H
 
 #include <cstdint>
+#include <functional>
 #include <memory>
 #include <vector>
 
@@ -86,6 +87,16 @@ struct lwf_batcher {
 namespace lwfb {
 
 double now_s();
+// The batcher's host thread pool: `worker` on the calling thread and on up to min(threads, n) - 1 more, all joined
+// before it returns.  The workers share the work through a counter of their own; a thread that cannot be started leaves
+// the work to the others.
+void run_pool(int threads, size_t n, const std::function<void()> &worker);
+// An independent copy of a pager's position and buffered packets (nullptr without memory)
+lwf_ogg *ogg_clone(const lwf_ogg *o);
+// Headers with the comments of `comment` (a comment header packet; lwf_headers_parse's errors for it) that share the
+// ident header, codebooks, floors, residues, mappings and modes of `shared`, which must outlive them.  What
+// lwf_headers_info, the packet decode and lwf_headers_make_setup give for them is what they give for `shared`.
+int headers_sharing(const lwf_headers *shared, const uint8_t *comment, size_t comment_len, lwf_headers **out);
 // any job without a stream, or with packets but no packet or length array: LWB_ERR_INVALID
 int check_jobs(const lwf_stream_job *jobs, size_t n_jobs);
 // plan[j].set for every job

@@ -1438,7 +1438,13 @@ struct Ogg {
         return LWB_ERR_INVALID;                 \
     }
 
-struct lwf_headers { lwf::Headers h; };
+// setup_of: headers that only hold an ident header and comments (lwfb::headers_sharing), whose codebooks, floors, residues,
+// mappings and modes are those of setup_of; body() is what every use but the comments reads.
+struct lwf_headers {
+    lwf::Headers h;
+    const lwf_headers *setup_of = nullptr;
+    const lwf::Headers &body() const { return setup_of ? setup_of->h : h; }
+};
 struct lwf_ogg { lwf::Ogg o; };
 
 extern "C" int lwf_headers_parse(const uint8_t *ident, size_t ident_len, const uint8_t *comment, size_t comment_len,
@@ -1462,7 +1468,7 @@ extern "C" void lwf_headers_destroy(lwf_headers *h) { delete h; }
 extern "C" int lwf_headers_info(const lwf_headers *h, lwf_info *out)
 {
     if (!h || !out) return LWB_ERR_INVALID;
-    const lwf::Headers &s = h->h;
+    const lwf::Headers &s = h->body();
     out->audio_channels = s.ident.audio_channels;
     out->blocksize_0 = s.ident.blocksize_0;
     out->blocksize_1 = s.ident.blocksize_1;
@@ -1475,7 +1481,7 @@ extern "C" int lwf_headers_info(const lwf_headers *h, lwf_info *out)
     out->n_residues = (uint32_t)s.residues.size();
     out->n_mappings = (uint32_t)s.mappings.size();
     out->n_modes = (uint32_t)s.modes.size();
-    out->n_comments = (uint32_t)s.comments.size();
+    out->n_comments = (uint32_t)h->h.comments.size();
     return LWB_OK;
 }
 
@@ -1502,7 +1508,7 @@ extern "C" int lwf_headers_make_setup(const lwf_headers *h, lwb_ctx *ctx, lwb_se
 {
     if (!h || !ctx || !out) return LWB_ERR_INVALID;
     LWF_GUARD(
-    const lwf::Headers &s = h->h;
+    const lwf::Headers &s = h->body();
     std::vector<lwb_floor_desc> floors(s.floors.size());
     for (size_t i = 0; i < s.floors.size(); i++) {
         std::memset(&floors[i], 0, sizeof(lwb_floor_desc));
@@ -1569,7 +1575,7 @@ extern "C" int lwf_headers_make_setup(const lwf_headers *h, lwb_ctx *ctx, lwb_se
 extern "C" int lwf_headers_vq_capable(const lwf_headers *h)
 {
     if (!h) return 0;
-    const lwf::Headers &s = h->h;
+    const lwf::Headers &s = h->body();
     if (s.ident.audio_channels > 8 || s.codebooks.size() > 256 || s.residues.size() > 64) return 0;
     if ((size_t)s.ident.audio_channels << (s.ident.blocksize_1 - 1) > 12288) return 0;       // the device accumulators
     for (const lwf::Residue &r : s.residues)
@@ -1597,8 +1603,8 @@ static bool needs_dense(const lwf::Headers &h, int flags)
 namespace lwf {
 void floor0_descs(const lwf_headers *h, std::vector<uint32_t> *index, std::vector<lwb_floor0_desc> *descs)
 {
-    for (size_t i = 0; i < h->h.floors.size(); i++) {
-        const Floor &fl = h->h.floors[i];
+    for (size_t i = 0; i < h->body().floors.size(); i++) {
+        const Floor &fl = h->body().floors[i];
         if (fl.type != 0 || !floor0_record_ok(fl.f0)) continue;
         lwb_floor0_desc d;
         std::memset(&d, 0, sizeof(d));
@@ -1629,7 +1635,7 @@ extern "C" int lwf_packet_decode_vq_ex(const lwf_headers *h, const uint8_t *pack
     if (!h || (!packet && len) || !out || !out->floor_kind || !out->floor1_y || (!runs && run_capacity) || (!entries && entry_capacity) ||
         !n_runs || !n_entries || (flags & ~LWF_DECODE_FLOOR0_RECORDS))
         return LWB_ERR_INVALID;
-    if (!out->dense_floor && needs_dense(h->h, flags)) return LWB_ERR_INVALID;
+    if (!out->dense_floor && needs_dense(h->body(), flags)) return LWB_ERR_INVALID;
     *n_runs = *n_entries = 0;
     LWF_GUARD(
         lwf::VqSink sink;
@@ -1637,7 +1643,7 @@ extern "C" int lwf_packet_decode_vq_ex(const lwf_headers *h, const uint8_t *pack
         sink.run_cap = run_capacity;
         sink.entries = entries;
         sink.ent_cap = entry_capacity;
-        const int rc = lwf::packet_decode(h->h, packet, len, out, &sink, (flags & LWF_DECODE_FLOOR0_RECORDS) != 0);
+        const int rc = lwf::packet_decode(h->body(), packet, len, out, &sink, (flags & LWF_DECODE_FLOOR0_RECORDS) != 0);
         if (rc) return rc;
         if (sink.overflow) return LWB_ERR_BUFFER;
         *n_runs = sink.n_runs;
@@ -1655,8 +1661,8 @@ extern "C" int lwf_packet_decode_ex(const lwf_headers *h, const uint8_t *packet,
 {
     if (!h || (!packet && len) || !out || !out->floor_kind || !out->floor1_y || !out->residue || (flags & ~LWF_DECODE_FLOOR0_RECORDS))
         return LWB_ERR_INVALID;
-    if (!out->dense_floor && needs_dense(h->h, flags)) return LWB_ERR_INVALID;
-    LWF_GUARD(return lwf::packet_decode(h->h, packet, len, out, nullptr, (flags & LWF_DECODE_FLOOR0_RECORDS) != 0);)
+    if (!out->dense_floor && needs_dense(h->body(), flags)) return LWB_ERR_INVALID;
+    LWF_GUARD(return lwf::packet_decode(h->body(), packet, len, out, nullptr, (flags & LWF_DECODE_FLOOR0_RECORDS) != 0);)
 }
 
 // get_decoded_sample_count, audio.rs:874-909
@@ -1665,9 +1671,9 @@ extern "C" int lwf_decoded_sample_count(const lwf_headers *h, const uint8_t *pac
     if (!h || (!packet && len) || !n_samples) return LWB_ERR_INVALID;
     lwf::BitReader rdr(packet, len);
     lwf::PacketHead ph;
-    const int rc = lwf::packet_head(h->h, rdr, &ph);
+    const int rc = lwf::packet_head(h->body(), rdr, &ph);
     if (rc) return rc;
-    const uint32_t n = ph.n, n0 = 1u << h->h.ident.blocksize_0;
+    const uint32_t n = ph.n, n0 = 1u << h->body().ident.blocksize_0;
     const uint32_t ls = ph.prev ? 0 : (n - n0) >> 2;
     const uint32_t rs = ph.next ? n >> 1 : (n * 3 - n0) >> 2;
     *n_samples = rs - ls;
@@ -1751,7 +1757,7 @@ static int reader_read_headers(lwf_reader *r, const lwf_ogg_packet *first)
     r->serial = serial;
     r->has_absgp = false;
     r->audio_start = r->ogg->o.at;
-    const size_t C = h->h.ident.audio_channels, n2 = (size_t)1 << (h->h.ident.blocksize_1 - 1);
+    const size_t C = h->body().ident.audio_channels, n2 = (size_t)1 << (h->body().ident.blocksize_1 - 1);
     r->kinds.assign(C, 0);
     r->ys.assign(C * LWB_MAX_POSTS, 0);
     r->dense.assign(C * n2, 0.f);
@@ -1960,9 +1966,9 @@ extern "C" int lwf_batcher_create(lwb_ctx *ctx, const lwf_headers *h, int thread
         b->threads = std::max(1, threads);
         b->groups.emplace_back(new Group());
         Group &g = *b->groups[0];
-        g.channels = h->h.ident.audio_channels;
-        g.bs0 = h->h.ident.blocksize_0;
-        g.bs1 = h->h.ident.blocksize_1;
+        g.channels = h->body().ident.audio_channels;
+        g.bs0 = h->body().ident.blocksize_0;
+        g.bs1 = h->body().ident.blocksize_1;
         b->sets.push_back(HeaderSet{h, nullptr, 0});
         update_floor0(b.get());
         *out = b.release();
@@ -2010,6 +2016,44 @@ double now_s()
     return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
 
+void run_pool(int threads, size_t n, const std::function<void()> &worker)
+{
+    const int nt = (int)std::min<size_t>((size_t)std::max(1, threads), std::max<size_t>(1, n));
+    std::vector<std::thread> pool;
+    try {
+        pool.reserve((size_t)nt);
+        for (int t = 1; t < nt; t++) pool.emplace_back(worker);
+    } catch (...) {
+        // no more threads to be had (std::system_error) or no memory for the vector: go on with the workers that did
+        // start -- they share the job counter, so the work is the same -- instead of unwinding past joinable threads
+    }
+    worker();
+    for (auto &t : pool) t.join();
+}
+
+lwf_ogg *ogg_clone(const lwf_ogg *o)
+{
+    try {
+        return new lwf_ogg(*o);
+    } catch (...) {
+        return nullptr;
+    }
+}
+
+int headers_sharing(const lwf_headers *shared, const uint8_t *comment, size_t comment_len, lwf_headers **out)
+{
+    if (!comment && comment_len) return LWB_ERR_INVALID;
+    LWF_GUARD(
+        std::unique_ptr<lwf_headers> h(new lwf_headers());
+        const int rc = lwf::read_comment(comment, comment_len, &h->h);
+        if (rc) return rc;
+        h->h.ident = shared->body().ident;
+        h->setup_of = shared->setup_of ? shared->setup_of : shared;
+        *out = h.release();
+        return LWB_OK;
+    )
+}
+
 void assign_sets(const lwf_batcher *b, const lwf_stream_job *jobs, size_t n_jobs, std::vector<JobPlan> &plan)
 {
     for (size_t j = 0; j < n_jobs; j++) plan[j].set = b->set_of ? b->set_of(b, jobs[j].stream) : 0;
@@ -2019,7 +2063,7 @@ void update_floor0(lwf_batcher *b)
 {
     for (auto &g : b->groups) g->has_floor0 = false;
     for (const HeaderSet &s : b->sets)
-        if (needs_dense(s.h->h, b->floor0_records ? LWF_DECODE_FLOOR0_RECORDS : 0)) b->groups[s.group]->has_floor0 = true;
+        if (needs_dense(s.h->body(), b->floor0_records ? LWF_DECODE_FLOOR0_RECORDS : 0)) b->groups[s.group]->has_floor0 = true;
 }
 
 // entropy decode of jobs list[0 .. n) into arena set `set` of their groups on the batcher's host threads
@@ -2036,7 +2080,7 @@ int batch_entropy(lwf_batcher *b, size_t set, lwf_stream_job *jobs, const size_t
         const lwf_stream_job &job = jobs[j];
         JobPlan &p = plan[j];
         const size_t g = b->sets[p.set].group;
-        const lwf::Headers &H = b->sets[p.set].h->h;
+        const lwf::Headers &H = b->sets[p.set].h->body();
         const size_t C = b->groups[g]->channels;
         p.coeff0 = coeff_total[g];
         p.pkt0 = pkt_total[g];
@@ -2090,7 +2134,7 @@ int batch_entropy(lwf_batcher *b, size_t set, lwf_stream_job *jobs, const size_t
                 const size_t j = list[i];
                 const lwf_stream_job &job = jobs[j];
                 const JobPlan &p = plan[j];
-                const lwf::Headers &H = b->sets[p.set].h->h;
+                const lwf::Headers &H = b->sets[p.set].h->body();
                 Group &G = *b->groups[b->sets[p.set].group];
                 BatchArena &ar = G.arena[set];
                 const size_t C = G.channels;
@@ -2144,17 +2188,7 @@ int batch_entropy(lwf_batcher *b, size_t set, lwf_stream_job *jobs, const size_t
             failed.store(1);
         }
     };
-    const int nt = (int)std::min<size_t>((size_t)b->threads, std::max<size_t>(1, n));
-    std::vector<std::thread> pool;
-    try {
-        pool.reserve((size_t)nt);
-        for (int t = 1; t < nt; t++) pool.emplace_back(worker);
-    } catch (...) {
-        // no more threads to be had (std::system_error) or no memory for the vector: go on with the workers that did
-        // start -- they share the job counter, so the work is the same -- instead of unwinding past joinable threads
-    }
-    worker();
-    for (auto &t : pool) t.join();
+    run_pool(b->threads, n, worker);
     if (failed.load()) return LWB_ERR_BUFFER;
     if (vq) {
         // counts -> offsets (rows of packets that were not decoded own nothing), then one packed copy of each array
@@ -2187,14 +2221,7 @@ int batch_entropy(lwf_batcher *b, size_t set, lwf_stream_job *jobs, const size_t
                 if (!je.empty()) std::memcpy((uint16_t *)ar.vqent.p + ((uint64_t *)ar.vqeoff.p)[p.pkt0], je.data(), je.size() * sizeof(uint16_t));
             }
         };
-        std::vector<std::thread> cpool;
-        try {
-            cpool.reserve((size_t)nt);
-            for (int t = 1; t < nt; t++) cpool.emplace_back(copier);
-        } catch (...) {
-        }
-        copier();
-        for (auto &t : cpool) t.join();
+        run_pool(b->threads, n, copier);
     }
     for (size_t g : *used) {
         BatchArena &ar = b->groups[g]->arena[set];
@@ -2336,7 +2363,7 @@ extern "C" double lwf_debug_decode_loop(const lwf_headers *h, const uint8_t *con
 {
     if (!h || !packets || !lens) return -1.0;
     try {
-        const size_t C = h->h.ident.audio_channels, n2 = (size_t)1 << (h->h.ident.blocksize_1 - 1);
+        const size_t C = h->body().ident.audio_channels, n2 = (size_t)1 << (h->body().ident.blocksize_1 - 1);
         std::vector<uint8_t> kinds(C);
         std::vector<uint32_t> ys(C * LWB_MAX_POSTS);
         std::vector<float> dense(C * n2), res(C * n2);
@@ -2355,7 +2382,7 @@ extern "C" double lwf_debug_decode_loop(const lwf_headers *h, const uint8_t *con
                 dp.residue = vq ? nullptr : res.data();
                 lwf::VqSink sink;
                 sink.runs = runs.data(); sink.run_cap = cap; sink.entries = ents.data(); sink.ent_cap = cap;
-                if (lwf::packet_decode(h->h, packets[i], lens[i], &dp, vq ? &sink : nullptr)) return -2.0;
+                if (lwf::packet_decode(h->body(), packets[i], lens[i], &dp, vq ? &sink : nullptr)) return -2.0;
             }
         return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     } catch (...) {

@@ -6,6 +6,7 @@
   OggPacketReader                 ogg::PacketReader as inside_ogg.rs uses it
   OggStreamReader                 inside_ogg.rs:60-227        (read_dec_packet, read_dec_packet_itl, read_dec_packet_generic,
                                                               get_last_absgp)
+  OggStreamReaders                many OggStreamReaders advanced by one batched call (lwf_readers)
 
 The entropy decode is CPU work by nature and runs on the host; synthesis goes through the CUDA back
 half (lwb_decode_packet / lwb_decode_chains)."""
@@ -25,6 +26,8 @@ SYMBOLS = ["lwf_headers_parse", "lwf_headers_destroy", "lwf_headers_info", "lwf_
            "lwf_reader_skip_samples_linear", "lwf_reader_seek_absgp_pg",
            "lwf_batcher_create", "lwf_batcher_destroy", "lwf_batcher_set_entry", "lwf_batcher_decode", "lwf_batcher_last_timing",
            "lwf_batcher_last_input_bytes", "lwf_batcher_set_floor0", "lwf_batcher_submit", "lwf_batcher_add_headers",
+           "lwf_readers_create", "lwf_readers_destroy", "lwf_readers_add", "lwf_readers_headers", "lwf_readers_last_absgp",
+           "lwf_readers_setup_count", "lwf_readers_last_timing", "lwf_readers_read",
            "lwf_debug_float32_unpack", "lwf_debug_lookup1_values", "lwf_debug_ilog", "lwf_debug_read_bits", "lwf_debug_huffman",
            "lwf_debug_decode_loop"]
 
@@ -74,6 +77,12 @@ class _StreamJob(C.Structure):
                 ("n_samples", C.c_uint32), ("packets_done", C.c_uint32), ("status", C.c_int32)]
 
 
+class _ReadJob(C.Structure):
+    _fields_ = [("reader", C.c_uint32), ("max_packets", C.c_uint32), ("out_offset", C.c_uint64), ("out_stride", C.c_uint64),
+                ("packet_samples", cabi.u32p), ("n_packets", C.c_uint32), ("n_samples", C.c_uint32), ("channels", C.c_uint8),
+                ("next_chained", C.c_uint8), ("ended", C.c_uint8), ("reserved", C.c_uint8), ("status", C.c_int32)]
+
+
 _declared = False
 
 
@@ -121,6 +130,18 @@ def lib():
         L.lwf_batcher_submit.argtypes = [vp, C.POINTER(_StreamJob), sz, C.c_int, vp, C.c_int, C.POINTER(C.c_uint64)]
         L.lwf_batcher_last_timing.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double)]
         L.lwf_batcher_last_timing.restype = None
+        L.lwf_readers_create.argtypes = [vp, C.c_int, C.POINTER(vp)]
+        L.lwf_readers_destroy.argtypes = [vp]
+        L.lwf_readers_destroy.restype = None
+        L.lwf_readers_add.argtypes = [vp, C.c_char_p, sz, C.POINTER(C.c_uint32)]
+        L.lwf_readers_headers.argtypes = [vp, C.c_uint32]
+        L.lwf_readers_headers.restype = vp
+        L.lwf_readers_last_absgp.argtypes = [vp, C.c_uint32, C.POINTER(C.c_uint64)]
+        L.lwf_readers_setup_count.argtypes = [vp]
+        L.lwf_readers_setup_count.restype = C.c_uint32
+        L.lwf_readers_last_timing.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double)]
+        L.lwf_readers_last_timing.restype = None
+        L.lwf_readers_read.argtypes = [vp, C.POINTER(_ReadJob), sz, C.c_int, vp, C.c_int, C.POINTER(C.c_uint64)]
         L.lwf_debug_float32_unpack.argtypes = [C.c_uint32]
         L.lwf_debug_float32_unpack.restype = C.c_float
         L.lwf_debug_lookup1_values.argtypes = [C.c_uint32, C.c_uint16]
@@ -372,17 +393,9 @@ class OggStreamReader:
                 return None
         if rc == ERR_NO_MORE_PACKETS:
             return None
-        if rc == cabi.ERR_BAD_FORMAT:
-            raise AudioReadError(rc)
-        if rc in (ERR_END_OF_PACKET, ERR_AUDIO_IS_HEADER):
-            e = AudioReadError(rc)
-            e.kind = {ERR_END_OF_PACKET: "EndOfPacket", ERR_AUDIO_IS_HEADER: "AudioIsHeader"}[rc]
+        e = read_error(self.ctx, rc)
+        if e is not None:
             raise e
-        if 16 <= rc <= 23:               # the headers of a chained stream (inside_ogg.rs:118-137): VorbisError::BadHeader
-            raise HeaderReadError(rc)
-        if rc >= ERR_OGG:
-            raise OggReadError("code %d" % rc)
-        self.ctx.check(rc)
         if lib().lwf_reader_headers(self._h) != self.headers._h:
             self._refresh()                      # a chained stream started
         Cn = self.headers.audio_channels
@@ -518,14 +531,7 @@ class StreamBatcher:
         once it is queued.  pcm: a page-locked numpy array (Context.host_alloc), a torch CUDA tensor or an integer device
         pointer; the memory space follows from it.  The streams may be submitted again at once; `pcm` holds the PCM once
         the ticket is done.  entropy_seconds / synthesis_seconds / input_bytes describe this submit."""
-        if isinstance(pcm, np.ndarray):
-            addr, memory = pcm.ctypes.data, cabi.MEM_HOST
-        elif isinstance(pcm, int):
-            addr, memory = pcm, cabi.MEM_DEVICE
-        elif hasattr(pcm, "data_ptr") and getattr(pcm, "is_cuda", False):
-            addr, memory = pcm.data_ptr(), cabi.MEM_DEVICE
-        else:
-            raise TypeError("pcm: a page-locked numpy array, a torch CUDA tensor or an integer device pointer")
+        addr, memory = _pcm_address(pcm)
         arr, keep, n = self._jobs(jobs, stride)
         t = C.c_uint64()
         self.ctx.check(lib().lwf_batcher_submit(self._h, arr, n, out_format, addr, memory, C.byref(t)))
@@ -572,3 +578,201 @@ class BatcherTicket:
             self.ctx.check(cabi.lib().lwb_ticket_wait(self.ctx._h, self.id))
             self._keep = None
         return _results(self._arr, self._n)
+
+
+def _pcm_address(pcm):
+    """(address, LWB_MEM_*) of a page-locked numpy array, a torch CUDA tensor or an integer device pointer."""
+    if isinstance(pcm, np.ndarray):
+        return pcm.ctypes.data, cabi.MEM_HOST
+    if isinstance(pcm, int):
+        return pcm, cabi.MEM_DEVICE
+    if hasattr(pcm, "data_ptr") and getattr(pcm, "is_cuda", False):
+        return pcm.data_ptr(), cabi.MEM_DEVICE
+    raise TypeError("pcm: a page-locked numpy array, a torch CUDA tensor or an integer device pointer")
+
+
+def read_error(ctx, rc):
+    """The exception OggStreamReader raises for status `rc` of a packet (None for LWB_OK; LWF_ERR_NO_MORE_PACKETS, the
+    end, is the caller's to handle)."""
+    if rc == 0:
+        return None
+    if rc == cabi.ERR_BAD_FORMAT:
+        return AudioReadError(rc)
+    if rc in (ERR_END_OF_PACKET, ERR_AUDIO_IS_HEADER):
+        e = AudioReadError(rc)
+        e.kind = {ERR_END_OF_PACKET: "EndOfPacket", ERR_AUDIO_IS_HEADER: "AudioIsHeader"}[rc]
+        return e
+    if 16 <= rc <= 23:               # the headers of a chained stream (inside_ogg.rs:118-137): VorbisError::BadHeader
+        return HeaderReadError(rc)
+    if rc >= ERR_OGG:
+        return OggReadError("code %d" % rc)
+    try:
+        ctx.check(rc)
+    except Exception as e:      # noqa: BLE001 -- the exception object is the result
+        return e
+    return None
+
+
+class ReadResult:
+    """One job of OggStreamReaders.read: the packets it returned (n_packets, and packet_samples, the samples each wrote),
+    n_samples per channel written at out_offset (planar: channel c at out_offset + c * out_stride; interleaved: `channels`
+    samples per frame), and how the reader stopped: status (LWB_OK or the code the single reader's next call returned),
+    ended (no packet left) and next_chained (the reader stands at a new logical stream)."""
+
+    def __init__(self, job, packet_samples):
+        for f, _ in _ReadJob._fields_:
+            if f not in ("packet_samples", "reserved"):
+                setattr(self, f, getattr(job, f))
+        self.next_chained, self.ended = bool(self.next_chained), bool(self.ended)
+        self.packet_samples = packet_samples[: self.n_packets].copy()
+
+    def __repr__(self):
+        return ("ReadResult(reader=%d, n_packets=%d, n_samples=%d, channels=%d, status=%d, ended=%s, next_chained=%s)" %
+                (self.reader, self.n_packets, self.n_samples, self.channels, self.status, self.ended, self.next_chained))
+
+
+class ReadTicket:
+    """A read queued by OggStreamReaders.read, in the manner of BatcherTicket: the job results (`results`) were written
+    before read returned; `pcm` holds the PCM once the ticket is done, and the ticket keeps it alive until then."""
+
+    def __init__(self, ctx, ticket, results, keep):
+        self.ctx, self.id, self.results, self._keep = ctx, ticket, results, keep
+
+    def done(self):
+        """lwb_ticket_query; never blocks."""
+        if self._keep is not None:
+            d = C.c_int()
+            self.ctx.check(cabi.lib().lwb_ticket_query(self.ctx._h, self.id, C.byref(d)))
+            if not d.value:
+                return False
+            self._keep = None
+        return True
+
+    def wait(self):
+        """lwb_ticket_wait; returns the job results [ReadResult]."""
+        if self._keep is not None:
+            self.ctx.check(cabi.lib().lwb_ticket_wait(self.ctx._h, self.id))
+            self._keep = None
+        return self.results
+
+
+class OggStreamReaders:
+    """Many OggStreamReaders on one context (lwf_readers): read() advances any of them by up to max_packets audio packets
+    in one call -- de-paging and entropy decode on a host thread pool, synthesis as one batch per channel count and
+    blocksize pair on the fused kernels -- and each returns exactly what OggStreamReader.read_dec_packet_generic returns,
+    packet for packet.  Readers whose ident and setup headers are byte-equal share one device setup."""
+
+    def __init__(self, ctx, threads=0):
+        self.ctx = ctx
+        h = C.c_void_p()
+        ctx.check(lib().lwf_readers_create(ctx._h, threads, C.byref(h)))
+        self._h = h.value
+        self._data = []                          # the bytes of each reader: lwf_readers_add does not copy them
+        self._headers = {}
+        ctx._children.add(self)
+
+    def add(self, data):
+        """A reader over `data` (OggStreamReader(ctx, data)): its headers are read now.  Returns its index."""
+        data = bytes(data)
+        i = C.c_uint32()
+        rc = lib().lwf_readers_add(self._h, data, len(data), C.byref(i))
+        if rc:
+            e = read_error(self.ctx, rc)
+            raise e if e is not None else AudioReadError(rc)
+        self._data.append(data)
+        return i.value
+
+    def stride(self, index, max_packets):
+        """The least planar stride of a job of max_packets packets of reader `index` (lwf_readers_read refuses a smaller
+        one): max_packets * blocksize_1 / 2 + (blocksize_1 - blocksize_0) / 4 of its stream."""
+        h = self.headers(index)
+        n1, n0 = 1 << h.blocksize_1, 1 << h.blocksize_0
+        return max_packets * n1 // 2 + (n1 - n0) // 4 if max_packets else 0
+
+    def __len__(self):
+        return len(self._data)
+
+    def headers(self, index):
+        """Headers of the stream reader `index`'s next packet belongs to (after a job with next_chained: the new one's)."""
+        h = lib().lwf_readers_headers(self._h, index)
+        if not h:
+            raise IndexError(index)
+        if self._headers.get(index, (None,))[0] != h:
+            self._headers[index] = (h, Headers(None, None, None, _handle=h))
+        return self._headers[index][1]
+
+    def get_last_absgp(self, index):
+        v = C.c_uint64()
+        return v.value if lib().lwf_readers_last_absgp(self._h, index, C.byref(v)) == 0 else None
+
+    @property
+    def setup_count(self):
+        """Distinct (ident, setup) header pairs among the streams opened: one device setup each."""
+        return lib().lwf_readers_setup_count(self._h)
+
+    def read(self, jobs, pcm, stride, sample="f32", interleaved=False):
+        """lwf_readers_read.  jobs: [(reader index, max_packets)], each reader at most once.  Job j's PCM lands in `pcm`
+        behind the jobs before it, each taking its reader's channels * stride elements (planar: channel c at
+        offset + c * stride; stride >= self.stride(index, max_packets) of every job).  pcm: a page-locked numpy array
+        (Context.host_alloc), a torch CUDA tensor or an integer device pointer, as for StreamBatcher.submit.  Returns a
+        ReadTicket; its results are known at once, its PCM once it is done.  paging_seconds, entropy_seconds and
+        synthesis_seconds describe this read (lwf_readers_last_timing)."""
+        fmt, _ = sample_format(sample, interleaved)
+        addr, memory = _pcm_address(pcm)
+        n = len(jobs)
+        arr = (_ReadJob * n)()
+        counts = []
+        off = 0
+        for j, (index, max_packets) in enumerate(jobs):
+            ps = np.zeros(max(1, max_packets), np.uint32)
+            counts.append(ps)
+            arr[j].reader, arr[j].max_packets = index, max_packets
+            arr[j].out_offset, arr[j].out_stride = off, stride
+            arr[j].packet_samples = ps.ctypes.data_as(cabi.u32p)
+            off += self.headers(index).audio_channels * stride
+        t = C.c_uint64()
+        self.ctx.check(lib().lwf_readers_read(self._h, arr, n, fmt, addr, memory, C.byref(t)))
+        p, e, s = C.c_double(), C.c_double(), C.c_double()
+        lib().lwf_readers_last_timing(self._h, C.byref(p), C.byref(e), C.byref(s))
+        self.paging_seconds, self.entropy_seconds, self.synthesis_seconds = p.value, e.value, s.value
+        return ReadTicket(self.ctx, t.value, [ReadResult(arr[j], counts[j]) for j in range(n)], (arr, counts, pcm))
+
+    def read_dec_packets(self, indices, max_packets, sample="f32", interleaved=False):
+        """read() into page-locked host memory and wait: per reader, the packets it returned, each in the form
+        OggStreamReader.read_dec_packet_generic returns it (planar: a list of per-channel arrays; interleaved: one array),
+        then None if it reached the end, or the exception the single reader's next call would have raised."""
+        fmt, dt = sample_format(sample, interleaved)
+        if not indices:
+            return []
+        stride = max([1] + [self.stride(i, max_packets) for i in indices])
+        total = sum(self.headers(i).audio_channels for i in indices) * stride
+        pcm = self.ctx.host_alloc(max(1, total), dt)
+        results = self.read([(i, max_packets) for i in indices], pcm, stride, sample, interleaved).wait()
+        out = []
+        for r in results:
+            pkts, s0 = [], 0
+            for n in r.packet_samples:
+                n = int(n)
+                if interleaved:
+                    pkts.append(pcm[r.out_offset + s0 * r.channels: r.out_offset + (s0 + n) * r.channels].copy())
+                else:
+                    pkts.append([pcm[r.out_offset + c * stride + s0: r.out_offset + c * stride + s0 + n].copy()
+                                 for c in range(r.channels)])
+                s0 += n
+            if r.status:
+                pkts.append(read_error(self.ctx, r.status))
+            elif r.ended:
+                pkts.append(None)
+            out.append(pkts)
+        return out
+
+    def close(self):
+        if self._h:
+            lib().lwf_readers_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
