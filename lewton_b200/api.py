@@ -95,7 +95,9 @@ class Context:
         arr, io = _marshal(chains, entry, memory, coeffs, pcm, out_format, floor_kind, floor1_y, dense_floor, floor_memory, vq)
         t = C.c_uint64()
         self.check(cabi.lib().lwb_submit_chains(self._h, arr, len(chains), C.byref(io), C.byref(t)))
-        return Ticket(self, t.value, chains, arr, (coeffs, pcm, floor_kind, floor1_y, dense_floor, vq, io))
+        ticket = Ticket(self, t.value, (coeffs, pcm, floor_kind, floor1_y, dense_floor, vq, io), lambda: _collect(chains, arr))
+        ticket.chains, ticket._arr = chains, arr
+        return ticket
 
     def save_states(self, pwrs, buf, memory=cabi.MEM_DEVICE, offsets=None):
         """lwb_streams_save: queues copies of the states of streams `pwrs` into `buf` and returns (slots, Ticket) at once.
@@ -112,7 +114,7 @@ class Context:
         self.check(cabi.lib().lwb_streams_save(self._h, arr, len(slots), memory, _addr(buf), C.byref(t)))
         for sl, a in zip(slots, arr):
             sl.len, sl.has = int(a.len), bool(a.has)
-        return slots, Ticket(self, t.value, [], None, (buf, arr))
+        return slots, Ticket(self, t.value, (buf, arr))
 
     def load_states(self, slots, buf, memory=cabi.MEM_DEVICE):
         """lwb_streams_load: queues copies of the states `slots` describe from `buf` into their streams (StateSlot.pwr, of
@@ -122,7 +124,7 @@ class Context:
         arr = _slot_array(slots)
         t = C.c_uint64()
         self.check(cabi.lib().lwb_streams_load(self._h, arr, len(slots), memory, _addr(buf), C.byref(t)))
-        return Ticket(self, t.value, [], None, (buf, arr))
+        return Ticket(self, t.value, (buf, arr))
 
     def close(self):
         if self._h:
@@ -674,15 +676,15 @@ class _PinnedBlock:
 
 
 class Ticket:
-    """A batch queued by Context.submit_chains.  It keeps every array of the batch alive until it is done; wait() copies
-    the chain results into the ChainSpecs (the library wrote them before submit_chains returned)."""
+    """Work queued on a context: a batch (Context.submit_chains, StreamBatcher.submit, OggStreamReaders.read) or a copy
+    of stream states (save_states, load_states).  It keeps every array the work reads or writes (`keep`) alive until it
+    is done; wait() returns result(), built from the results the library wrote before the queuing call returned."""
 
-    def __init__(self, ctx, ticket, chains, arr, keep):
-        self.ctx, self.id, self.chains = ctx, ticket, chains
-        self._arr, self._keep = arr, keep
+    def __init__(self, ctx, ticket, keep, result=list):
+        self.ctx, self.id, self._keep, self._result = ctx, ticket, keep, result
 
     def done(self):
-        """lwb_ticket_query: whether every copy and kernel of the batch has finished.  Never blocks."""
+        """lwb_ticket_query: whether every copy and kernel of the work has finished.  Never blocks."""
         if self._keep is not None:
             d = C.c_int()
             self.ctx.check(cabi.lib().lwb_ticket_query(self.ctx._h, self.id, C.byref(d)))
@@ -692,11 +694,12 @@ class Ticket:
         return True
 
     def wait(self):
-        """lwb_ticket_wait; returns the chains with their results (none for a save_states or load_states ticket)."""
+        """lwb_ticket_wait; returns the results: submit_chains' chains with theirs, StreamBatcher.submit's
+        [(n_samples, packets_done, status)], OggStreamReaders.read's [ReadResult], none for save_states and load_states."""
         if self._keep is not None:
             self.ctx.check(cabi.lib().lwb_ticket_wait(self.ctx._h, self.id))
             self._keep = None
-        return _collect(self.chains, self._arr)
+        return self._result()
 
 
 def _marshal(chains, entry, memory, coeffs, pcm, out_format, floor_kind, floor1_y, dense_floor, floor_memory, vq):

@@ -1,6 +1,7 @@
 // batcher.h -- internals of lwf_batcher (include/lewton_frontend.h) shared by its two halves: frontend.cpp, the
 // host entropy decode and the synchronous lwf_batcher_decode, and batcher_submit.cpp, the asynchronous lwf_batcher_submit
-// and lwf_batcher_add_headers.
+// and lwf_batcher_add_headers; and the rules of OggStreamReader, which frontend.cpp's lwf_reader and readers.cpp's
+// lwf_readers share.
 // frontend.cpp needs no CUDA and calls only the synchronous back half, so that it also builds against a stub back half
 // (the fuzz harness); whatever submits and header sets use beyond that is reached through the hooks on lwf_batcher
 // (release, set_of).
@@ -10,11 +11,28 @@
 #include <cstdint>
 #include <functional>
 #include <memory>
+#include <new>
+#include <stdexcept>
 #include <vector>
 
 #include "../../include/lewton_frontend.h"
 
 namespace lwfb {
+
+// f() behind the C ABI, which nothing may unwind across: allocation failures (bad_alloc, length_error) become
+// LWB_ERR_BUFFER, any other exception LWB_ERR_INVALID.
+template <class F> int guarded(F &&f)
+{
+    try {
+        return f();
+    } catch (const std::bad_alloc &) {
+        return LWB_ERR_BUFFER;
+    } catch (const std::length_error &) {
+        return LWB_ERR_BUFFER;
+    } catch (...) {
+        return LWB_ERR_INVALID;
+    }
+}
 
 struct PinnedBuf {
     void *p = nullptr;
@@ -97,6 +115,33 @@ lwf_ogg *ogg_clone(const lwf_ogg *o);
 // ident header, codebooks, floors, residues, mappings and modes of `shared`, which must outlive them.  What
 // lwf_headers_info, the packet decode and lwf_headers_make_setup give for them is what they give for `shared`.
 int headers_sharing(const lwf_headers *shared, const uint8_t *comment, size_t comment_len, lwf_headers **out);
+
+// OggStreamReader's granule position (inside_ogg.rs:219-227): absgp after the packets returned so far, if known.
+struct Granule {
+    bool has = false;
+    uint64_t absgp = 0;
+    // of the n samples packet pk decodes to, those it returns: a stream's last packet is cut to its page's granule
+    // position (inside_ogg.rs:219-222)
+    size_t cut(const lwf_ogg_packet &pk, size_t n) const;
+    // after pk returned n samples: the page's granule position at its last packet, else n further on if known (:223-227)
+    void step(const lwf_ogg_packet &pk, size_t n);
+};
+
+// The header packets of a logical stream, as read_headers (inside_ogg.rs:19-39) gathers them
+struct HeaderPackets {
+    std::vector<uint8_t> ident, comment;
+    lwf_ogg_packet setup;              // a pager packet: valid until the pager's next read
+    uint32_t serial = 0;               // the stream's serial, to be adopted
+};
+// Reads the ident (unless `chained`: a chained stream's, already read into hp.ident), comment and setup packets from o.
+// At the start of the data packets of other serials are skipped until those of the ident packet's stream arrive; in
+// front of a chained stream the next two packets are taken whatever their serial, and the setup packet's serial is
+// adopted (:124-137).  The end of the data is LWF_ERR_OGG.
+int read_header_packets(lwf_ogg *o, bool chained, HeaderPackets &hp);
+// The serial filter of read_next_audio_packet (inside_ogg.rs:107-117): the next packet of `serial`, or of another
+// serial if it begins a logical stream (a chained stream: pk->stream_serial != serial); other packets are skipped.
+// *reads (if not NULL) counts the pager reads.
+int next_packet_of(lwf_ogg *o, uint32_t serial, lwf_ogg_packet *pk, size_t *reads);
 // any job without a stream, or with packets but no packet or length array: LWB_ERR_INVALID
 int check_jobs(const lwf_stream_job *jobs, size_t n_jobs);
 // plan[j].set for every job

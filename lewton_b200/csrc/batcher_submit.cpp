@@ -3,8 +3,6 @@
 // which registers those header sets.  The entropy decode and the batches' arrays are frontend.cpp's (batcher.h); this
 // file adds the ring of arena sets, with the ticket of the submit that last read each set, and the device copies of the
 // coefficient and dense floor arenas that device-PCM batches read.
-#include <new>
-#include <stdexcept>
 #include <vector>
 
 #include <cuda_runtime.h>
@@ -248,15 +246,7 @@ extern "C" int lwf_batcher_submit(lwf_batcher *b, lwf_stream_job *jobs, size_t n
     if (!b || (!jobs && n_jobs) || !pcm || !ticket || (pcm_memory != LWB_MEM_HOST && pcm_memory != LWB_MEM_DEVICE) ||
         lwfb::check_jobs(jobs, n_jobs))
         return LWB_ERR_INVALID;
-    try {
-        return lwfb::submit(b, jobs, n_jobs, out_format, pcm, pcm_memory, ticket);
-    } catch (const std::bad_alloc &) {
-        return LWB_ERR_BUFFER;
-    } catch (const std::length_error &) {
-        return LWB_ERR_BUFFER;
-    } catch (...) {
-        return LWB_ERR_INVALID;
-    }
+    return lwfb::guarded([&] { return lwfb::submit(b, jobs, n_jobs, out_format, pcm, pcm_memory, ticket); });
 }
 
 // The NULL and LWB_ENTRY_VQ checks come before anything reads the setup or the batcher's context.
@@ -266,13 +256,5 @@ extern "C" int lwf_batcher_add_headers(lwf_batcher *b, const lwf_headers *h, con
     if (b->entry == LWB_ENTRY_VQ && !lwf_headers_vq_capable(h)) return LWB_ERR_INVALID;
     for (const lwfb::HeaderSet &s : b->sets)
         if (s.setup == setup) return LWB_ERR_INVALID;
-    try {
-        return lwfb::add_headers(b, h, setup);
-    } catch (const std::bad_alloc &) {
-        return LWB_ERR_BUFFER;
-    } catch (const std::length_error &) {
-        return LWB_ERR_BUFFER;
-    } catch (...) {
-        return LWB_ERR_INVALID;
-    }
+    return lwfb::guarded([&] { return lwfb::add_headers(b, h, setup); });
 }

@@ -1303,34 +1303,50 @@ struct Ogg {
         return streams.back().second;
     }
 
+    struct PageHead { uint8_t htype; uint64_t absgp; uint32_t serial, crc; size_t nseg, total; };
+
+    // The header of the page at byte `pos`: LWF_ERR_OGG unless its capture pattern, version, segment table and body are
+    // all there
+    int page_head(size_t pos, PageHead *h) const
+    {
+        if (pos + 27 > len) return LWF_ERR_OGG;
+        const uint8_t *p = d + pos;
+        if (std::memcmp(p, "OggS", 4) != 0 || p[4] != 0) return LWF_ERR_OGG;
+        auto le = [p](int at, int n) {
+            uint64_t v = 0;
+            for (int i = n - 1; i >= 0; i--) v = (v << 8) | p[at + i];
+            return v;
+        };
+        h->htype = p[5];
+        h->absgp = le(6, 8);
+        h->serial = (uint32_t)le(14, 4);
+        h->crc = (uint32_t)le(22, 4);
+        h->nseg = p[26];
+        if (pos + 27 + h->nseg > len) return LWF_ERR_OGG;
+        size_t body = 0;
+        for (size_t i = 0; i < h->nseg; i++) body += p[27 + i];
+        h->total = 27 + h->nseg + body;
+        if (pos + h->total > len) return LWF_ERR_OGG;
+        return LWB_OK;
+    }
+
     // parse one page into the queue; LWF_ERR_NO_MORE_PACKETS at the end of the data
     int read_page()
     {
         if (at >= len) return LWF_ERR_NO_MORE_PACKETS;
-        if (at + 27 > len) return LWF_ERR_OGG;
+        PageHead h;
+        if (page_head(at, &h)) return LWF_ERR_OGG;
         const uint8_t *p = d + at;
-        if (std::memcmp(p, "OggS", 4) != 0 || p[4] != 0) return LWF_ERR_OGG;
-        const uint8_t htype = p[5];
-        uint64_t absgp = 0;
-        for (int i = 7; i >= 0; i--) absgp = (absgp << 8) | p[6 + i];
-        const uint32_t serial = (uint32_t)p[14] | ((uint32_t)p[15] << 8) | ((uint32_t)p[16] << 16) | ((uint32_t)p[17] << 24);
-        const uint32_t crc = (uint32_t)p[22] | ((uint32_t)p[23] << 8) | ((uint32_t)p[24] << 16) | ((uint32_t)p[25] << 24);
-        const size_t nseg = p[26];
-        if (at + 27 + nseg > len) return LWF_ERR_OGG;
-        size_t body = 0;
-        for (size_t i = 0; i < nseg; i++) body += p[27 + i];
-        const size_t total = 27 + nseg + body;
-        if (at + total > len) return LWF_ERR_OGG;
-        if (ogg_crc(p, total, 22) != crc) return LWF_ERR_OGG;
-        OggStreamState &st = state(serial);
-        const bool bos = htype & 2, eos = htype & 4, continued = htype & 1;
+        if (ogg_crc(p, h.total, 22) != h.crc) return LWF_ERR_OGG;
+        OggStreamState &st = state(h.serial);
+        const bool bos = h.htype & 2, eos = h.htype & 4, continued = h.htype & 1;
         if (!continued) { st.partial.clear(); st.in_packet = false; }
-        const uint8_t *bp = p + 27 + nseg;
+        const uint8_t *bp = p + 27 + h.nseg;
         const size_t q0 = queue.size();
         bool first_in_page = true;
         bool dropping = st.drop_continued && continued;
         st.drop_continued = false;
-        for (size_t i = 0; i < nseg; i++) {
+        for (size_t i = 0; i < h.nseg; i++) {
             const uint8_t l = p[27 + i];
             if (dropping) {                    // still inside the packet that began before the seek target
                 bp += l;
@@ -1343,8 +1359,8 @@ struct Ogg {
             if (l < 255) {
                 Pending pk;
                 pk.data.swap(st.partial);
-                pk.serial = serial;
-                pk.absgp = absgp;
+                pk.serial = h.serial;
+                pk.absgp = h.absgp;
                 pk.first_stream = bos && first_in_page && !st.seen;
                 pk.last_stream = false;
                 pk.first_page = first_in_page;
@@ -1360,7 +1376,7 @@ struct Ogg {
             queue.back().last_page = true;
             if (eos) queue.back().last_stream = true;
         }
-        at += total;
+        at += h.total;
         return LWB_OK;
     }
 
@@ -1372,22 +1388,14 @@ struct Ogg {
     {
         size_t pos = from, best = (size_t)-1, first = (size_t)-1;
         while (pos + 27 <= len) {
-            const uint8_t *p = d + pos;
-            if (std::memcmp(p, "OggS", 4) != 0 || p[4] != 0) return LWF_ERR_OGG;
-            const size_t nseg = p[26];
-            if (pos + 27 + nseg > len) return LWF_ERR_OGG;
-            size_t body = 0;
-            for (size_t i = 0; i < nseg; i++) body += p[27 + i];
-            if (pos + 27 + nseg + body > len) return LWF_ERR_OGG;
-            const uint32_t ps = (uint32_t)p[14] | ((uint32_t)p[15] << 8) | ((uint32_t)p[16] << 16) | ((uint32_t)p[17] << 24);
-            uint64_t g = 0;
-            for (int i = 7; i >= 0; i--) g = (g << 8) | p[6 + i];
-            if (ps == serial) {
+            PageHead h;
+            if (page_head(pos, &h)) return LWF_ERR_OGG;
+            if (h.serial == serial) {
                 if (first == (size_t)-1) first = pos;
-                if (g != ~0ull && g <= goal) best = pos;       // (-1: no packet finishes on this page)
-                else if (g != ~0ull && g > goal) break;
+                if (h.absgp != ~0ull && h.absgp <= goal) best = pos;       // (-1: no packet finishes on this page)
+                else if (h.absgp != ~0ull && h.absgp > goal) break;
             }
-            pos += 27 + nseg + body;
+            pos += h.total;
         }
         if (first == (size_t)-1) return LWF_ERR_OGG;
         at = best != (size_t)-1 ? best : first;
@@ -1425,18 +1433,9 @@ struct Ogg {
 }  // namespace lwf
 
 // ---------------------------------------------------------------------------------------------
-// C ABI.  Nothing may unwind across it: allocation failures become LWB_ERR_BUFFER.
+// C ABI.  Nothing may unwind across it (lwfb::guarded): allocation failures become LWB_ERR_BUFFER.
 // ---------------------------------------------------------------------------------------------
-#define LWF_GUARD(...)                          \
-    try {                                       \
-        __VA_ARGS__                             \
-    } catch (const std::bad_alloc &) {          \
-        return LWB_ERR_BUFFER;                  \
-    } catch (const std::length_error &) {       \
-        return LWB_ERR_BUFFER;                  \
-    } catch (...) {                             \
-        return LWB_ERR_INVALID;                 \
-    }
+using lwfb::guarded;
 
 // setup_of: headers that only hold an ident header and comments (lwfb::headers_sharing), whose codebooks, floors, residues,
 // mappings and modes are those of setup_of; body() is what every use but the comments reads.
@@ -1451,7 +1450,7 @@ extern "C" int lwf_headers_parse(const uint8_t *ident, size_t ident_len, const u
                                  const uint8_t *setup, size_t setup_len, lwf_headers **out)
 {
     if (!ident || !comment || !setup || !out) return LWB_ERR_INVALID;
-    LWF_GUARD(
+    return guarded([&]() -> int {
         std::unique_ptr<lwf_headers> h(new (std::nothrow) lwf_headers());
         if (!h) return LWB_ERR_BUFFER;
         int rc;
@@ -1460,7 +1459,7 @@ extern "C" int lwf_headers_parse(const uint8_t *ident, size_t ident_len, const u
         if ((rc = lwf::read_setup(setup, setup_len, &h->h))) return rc;
         *out = h.release();
         return LWB_OK;
-    )
+    });
 }
 
 extern "C" void lwf_headers_destroy(lwf_headers *h) { delete h; }
@@ -1507,7 +1506,7 @@ extern "C" size_t lwf_headers_comment(const lwf_headers *h, int index, char *buf
 extern "C" int lwf_headers_make_setup(const lwf_headers *h, lwb_ctx *ctx, lwb_setup **out)
 {
     if (!h || !ctx || !out) return LWB_ERR_INVALID;
-    LWF_GUARD(
+    return guarded([&]() -> int {
     const lwf::Headers &s = h->body();
     std::vector<lwb_floor_desc> floors(s.floors.size());
     for (size_t i = 0; i < s.floors.size(); i++) {
@@ -1567,7 +1566,7 @@ extern "C" int lwf_headers_make_setup(const lwf_headers *h, lwb_ctx *ctx, lwb_se
         d.residues = resids.data();
     }
     return lwb_setup_create(ctx, &d, out);
-    )
+    });
 }
 
 // What LWB_ENTRY_VQ needs from a stream: <= 8 channels, and every VQ book a residue uses has a dimension that divides
@@ -1637,7 +1636,7 @@ extern "C" int lwf_packet_decode_vq_ex(const lwf_headers *h, const uint8_t *pack
         return LWB_ERR_INVALID;
     if (!out->dense_floor && needs_dense(h->body(), flags)) return LWB_ERR_INVALID;
     *n_runs = *n_entries = 0;
-    LWF_GUARD(
+    return guarded([&]() -> int {
         lwf::VqSink sink;
         sink.runs = runs;
         sink.run_cap = run_capacity;
@@ -1649,7 +1648,7 @@ extern "C" int lwf_packet_decode_vq_ex(const lwf_headers *h, const uint8_t *pack
         *n_runs = sink.n_runs;
         *n_entries = sink.n_ent;
         return LWB_OK;
-    )
+    });
 }
 
 extern "C" int lwf_packet_decode(const lwf_headers *h, const uint8_t *packet, size_t len, lwf_decoded_packet *out)
@@ -1662,7 +1661,7 @@ extern "C" int lwf_packet_decode_ex(const lwf_headers *h, const uint8_t *packet,
     if (!h || (!packet && len) || !out || !out->floor_kind || !out->floor1_y || !out->residue || (flags & ~LWF_DECODE_FLOOR0_RECORDS))
         return LWB_ERR_INVALID;
     if (!out->dense_floor && needs_dense(h->body(), flags)) return LWB_ERR_INVALID;
-    LWF_GUARD(return lwf::packet_decode(h->body(), packet, len, out, nullptr, (flags & LWF_DECODE_FLOOR0_RECORDS) != 0);)
+    return guarded([&] { return lwf::packet_decode(h->body(), packet, len, out, nullptr, (flags & LWF_DECODE_FLOOR0_RECORDS) != 0); });
 }
 
 // get_decoded_sample_count, audio.rs:874-909
@@ -1694,7 +1693,7 @@ extern "C" void lwf_ogg_close(lwf_ogg *o) { delete o; }
 extern "C" int lwf_ogg_next_packet(lwf_ogg *o, lwf_ogg_packet *pkt)
 {
     if (!o || !pkt) return LWB_ERR_INVALID;
-    LWF_GUARD(return o->o.next(pkt);)
+    return guarded([&] { return o->o.next(pkt); });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1707,8 +1706,7 @@ struct lwf_reader {
     lwb_setup *setup = nullptr;
     lwb_stream *pwr = nullptr;
     uint32_t serial = 0;
-    bool has_absgp = false;
-    uint64_t absgp = 0;
+    lwfb::Granule gp;
     size_t audio_start = 0;        // byte offset of the first page after the current stream's headers
     std::vector<uint8_t> kinds;
     std::vector<uint32_t> ys;
@@ -1728,34 +1726,19 @@ static void reader_drop_stream(lwf_reader *r)
 // read_headers, inside_ogg.rs:19-39 (`first`: the ident packet has already been read)
 static int reader_read_headers(lwf_reader *r, const lwf_ogg_packet *first)
 {
-    lwf_ogg_packet pk;
-    int rc;
-    std::vector<uint8_t> ident, comment;
-    if (first) pk = *first;
-    else if ((rc = lwf_ogg_next_packet(r->ogg, &pk))) return rc == LWF_ERR_NO_MORE_PACKETS ? LWF_ERR_OGG : rc;
-    ident.assign(pk.data, pk.data + pk.len);
-    // At the start of the data packets of other logical streams are skipped until the comment and the setup header of
-    // the ident packet's stream arrive (read_headers, inside_ogg.rs:30-47).  In front of a chained stream the reference
-    // takes the NEXT TWO packets, whatever their serial, and then adopts the setup packet's serial (:124-137): a foreign
-    // packet in between fails there as a bad header, and so it does here.
-    const bool chained = first != nullptr;
-    uint32_t serial = pk.stream_serial;
-    do {
-        if ((rc = lwf_ogg_next_packet(r->ogg, &pk))) return rc == LWF_ERR_NO_MORE_PACKETS ? LWF_ERR_OGG : rc;
-    } while (!chained && pk.stream_serial != serial);
-    comment.assign(pk.data, pk.data + pk.len);
-    do {
-        if ((rc = lwf_ogg_next_packet(r->ogg, &pk))) return rc == LWF_ERR_NO_MORE_PACKETS ? LWF_ERR_OGG : rc;
-    } while (!chained && pk.stream_serial != serial);
-    if (chained) serial = pk.stream_serial;
+    lwfb::HeaderPackets hp;
+    if (first) hp.ident.assign(first->data, first->data + first->len);
+    int rc = lwfb::read_header_packets(r->ogg, first != nullptr, hp);
+    if (rc) return rc;
     lwf_headers *h = nullptr;
-    if ((rc = lwf_headers_parse(ident.data(), ident.size(), comment.data(), comment.size(), pk.data, pk.len, &h))) return rc;
+    if ((rc = lwf_headers_parse(hp.ident.data(), hp.ident.size(), hp.comment.data(), hp.comment.size(), hp.setup.data, hp.setup.len, &h)))
+        return rc;
     reader_drop_stream(r);
     r->hdr = h;
     if ((rc = lwf_headers_make_setup(h, r->ctx, &r->setup))) return rc;
     if ((rc = lwb_stream_open(r->ctx, r->setup, &r->pwr))) return rc;
-    r->serial = serial;
-    r->has_absgp = false;
+    r->serial = hp.serial;
+    r->gp.has = false;
     r->audio_start = r->ogg->o.at;
     const size_t C = h->body().ident.audio_channels, n2 = (size_t)1 << (h->body().ident.blocksize_1 - 1);
     r->kinds.assign(C, 0);
@@ -1773,16 +1756,7 @@ extern "C" int lwf_reader_open(lwb_ctx *ctx, const uint8_t *data, size_t len, lw
     r->ctx = ctx;
     int rc = lwf_ogg_open(data, len, &r->ogg);
     if (rc) return rc;
-    try {
-        rc = reader_read_headers(r.get(), nullptr);
-    } catch (const std::bad_alloc &) {
-        rc = LWB_ERR_BUFFER;
-    } catch (const std::length_error &) {
-        rc = LWB_ERR_BUFFER;
-    } catch (...) {
-        rc = LWB_ERR_INVALID;
-    }
-    if (rc) {
+    if ((rc = guarded([&] { return reader_read_headers(r.get(), nullptr); }))) {
         reader_drop_stream(r.get());
         lwf_ogg_close(r->ogg);
         return rc;
@@ -1827,22 +1801,17 @@ static int reader_decode(lwf_reader *r, const lwf_ogg_packet &pk, int out_format
 // read_next_audio_packet, inside_ogg.rs:107-143
 static int reader_next_audio_packet(lwf_reader *r, lwf_ogg_packet *pk)
 {
-    int rc;
-    for (;;) {
-        if ((rc = lwf_ogg_next_packet(r->ogg, pk))) return rc;
-        if (pk->stream_serial == r->serial) return LWB_OK;
-        if (!pk->first_in_stream) continue;
-        // a chained stream begins: new headers, new state; its first audio packet is decoded and dropped
-        if ((rc = reader_read_headers(r, pk))) return rc;
-        if ((rc = lwf_ogg_next_packet(r->ogg, pk))) return rc;
-        const size_t C = r->hdr->h.ident.audio_channels, n1 = (size_t)1 << r->hdr->h.ident.blocksize_1;
-        r->scratch.resize(C * n1);
-        size_t dropped = 0;
-        if ((rc = reader_decode(r, *pk, LWB_OUT_F32_PLANAR, r->scratch.data(), n1, &dropped))) return rc;
-        r->has_absgp = true;
-        r->absgp = pk->absgp_page;
-        return lwf_ogg_next_packet(r->ogg, pk);
-    }
+    int rc = lwfb::next_packet_of(r->ogg, r->serial, pk, nullptr);
+    if (rc || pk->stream_serial == r->serial) return rc;
+    // a chained stream begins: new headers, new state; its first audio packet is decoded and dropped
+    if ((rc = reader_read_headers(r, pk))) return rc;
+    if ((rc = lwf_ogg_next_packet(r->ogg, pk))) return rc;
+    const size_t C = r->hdr->h.ident.audio_channels, n1 = (size_t)1 << r->hdr->h.ident.blocksize_1;
+    r->scratch.resize(C * n1);
+    size_t dropped = 0;
+    if ((rc = reader_decode(r, *pk, LWB_OUT_F32_PLANAR, r->scratch.data(), n1, &dropped))) return rc;
+    r->gp = lwfb::Granule{true, pk->absgp_page};
+    return lwf_ogg_next_packet(r->ogg, pk);
 }
 
 // dec_packet_generic, inside_ogg.rs:207-229: decode, truncate at the end of the stream, account the granule position
@@ -1852,16 +1821,8 @@ static int reader_dec_packet(lwf_reader *r, const lwf_ogg_packet &pk, int out_fo
     const size_t cap = cap_total / r->hdr->h.ident.audio_channels;
     int rc = reader_decode(r, pk, out_format, out, cap, &n);
     if (rc) return rc;
-    if (r->has_absgp && pk.last_in_stream) {                      // inside_ogg.rs:219-222
-        const uint64_t target = pk.absgp_page > r->absgp ? pk.absgp_page - r->absgp : 0;
-        if (target < n) n = (size_t)target;
-    }
-    if (pk.last_in_page) {                                        // :223-227
-        r->has_absgp = true;
-        r->absgp = pk.absgp_page;
-    } else if (r->has_absgp) {
-        r->absgp += n;
-    }
+    n = r->gp.cut(pk, n);
+    r->gp.step(pk, n);
     *n_samples = n;
     return LWB_OK;
 }
@@ -1871,12 +1832,12 @@ extern "C" int lwf_reader_read_dec_packet(lwf_reader *r, int out_format, void *o
 {
     if (!r || !out || !n_samples) return LWB_ERR_INVALID;
     *n_samples = 0;
-    LWF_GUARD(
+    return guarded([&] {
         lwf_ogg_packet pk;
         int rc = reader_next_audio_packet(r, &pk);
         if (rc) return rc;
         return reader_dec_packet(r, pk, out_format, out, cap_total, n_samples);
-    )
+    });
 }
 
 // skip_samples_linear, inside_ogg.rs:244-283: packets are only measured (get_decoded_sample_count) until the one that
@@ -1889,7 +1850,7 @@ extern "C" int lwf_reader_skip_samples_linear(lwf_reader *r, size_t to_skip, int
     *n_samples = 0;
     *got_packet = 0;
     *left_to_skip = to_skip;
-    LWF_GUARD(
+    return guarded([&]() -> int {
         std::vector<uint8_t> last;             // Option<Packet>: the packet read before `next`
         bool have_last = false;
         lwf_ogg_packet last_pk;
@@ -1901,11 +1862,8 @@ extern "C" int lwf_reader_skip_samples_linear(lwf_reader *r, size_t to_skip, int
             if (rc) return rc;
             size_t cnt = 0;
             if ((rc = lwf_decoded_sample_count(r->hdr, next.data, next.len, &cnt))) return rc;
-            if (r->has_absgp && next.last_in_stream) {             // :258-262
-                have_last = false;
-                const uint64_t target = next.absgp_page > r->absgp ? next.absgp_page - r->absgp : 0;
-                if (target < cnt) cnt = (size_t)target;
-            }
+            if (r->gp.has && next.last_in_stream) have_last = false;       // :258-262
+            cnt = r->gp.cut(next, cnt);
             if (to_skip < cnt) {                                   // :263-271
                 if (have_last) {
                     lwb_stream_reset(r->pwr);
@@ -1923,31 +1881,31 @@ extern "C" int lwf_reader_skip_samples_linear(lwf_reader *r, size_t to_skip, int
                 return LWB_OK;
             }
             to_skip -= cnt;
-            if (r->has_absgp) r->absgp += cnt;                     // :275-277
+            if (r->gp.has) r->gp.absgp += cnt;                     // :275-277, whatever the page
             last.assign(next.data, next.data + next.len);
             last_pk = next;
             have_last = true;
         }
-    )
+    });
 }
 
 // seek_absgp_pg, inside_ogg.rs:307-313: page-granular seek, then cur_absgp = None and a fresh PreviousWindowRight
 extern "C" int lwf_reader_seek_absgp_pg(lwf_reader *r, uint64_t absgp)
 {
     if (!r) return LWB_ERR_INVALID;
-    LWF_GUARD(
+    return guarded([&] {
         const int rc = r->ogg->o.seek_absgp(r->serial, absgp, r->audio_start);
         if (rc) return rc;
-        r->has_absgp = false;
+        r->gp.has = false;
         return lwb_stream_reset(r->pwr);
-    )
+    });
 }
 
 extern "C" int lwf_reader_last_absgp(const lwf_reader *r, uint64_t *absgp)
 {
     if (!r || !absgp) return LWB_ERR_INVALID;
-    if (!r->has_absgp) return 1;
-    *absgp = r->absgp;
+    if (!r->gp.has) return 1;
+    *absgp = r->gp.absgp;
     return 0;
 }
 
@@ -1959,7 +1917,7 @@ using namespace lwfb;
 extern "C" int lwf_batcher_create(lwb_ctx *ctx, const lwf_headers *h, int threads, lwf_batcher **out)
 {
     if (!ctx || !h || !out) return LWB_ERR_INVALID;
-    LWF_GUARD(
+    return guarded([&]() -> int {
         std::unique_ptr<lwf_batcher> b(new lwf_batcher());
         b->ctx = ctx;
         if (threads <= 0) threads = (int)std::thread::hardware_concurrency();
@@ -1973,7 +1931,7 @@ extern "C" int lwf_batcher_create(lwb_ctx *ctx, const lwf_headers *h, int thread
         update_floor0(b.get());
         *out = b.release();
         return LWB_OK;
-    )
+    });
 }
 
 extern "C" void lwf_batcher_destroy(lwf_batcher *b)
@@ -2043,7 +2001,7 @@ lwf_ogg *ogg_clone(const lwf_ogg *o)
 int headers_sharing(const lwf_headers *shared, const uint8_t *comment, size_t comment_len, lwf_headers **out)
 {
     if (!comment && comment_len) return LWB_ERR_INVALID;
-    LWF_GUARD(
+    return guarded([&]() -> int {
         std::unique_ptr<lwf_headers> h(new lwf_headers());
         const int rc = lwf::read_comment(comment, comment_len, &h->h);
         if (rc) return rc;
@@ -2051,7 +2009,57 @@ int headers_sharing(const lwf_headers *shared, const uint8_t *comment, size_t co
         h->setup_of = shared->setup_of ? shared->setup_of : shared;
         *out = h.release();
         return LWB_OK;
-    )
+    });
+}
+
+size_t Granule::cut(const lwf_ogg_packet &pk, size_t n) const
+{
+    if (!has || !pk.last_in_stream) return n;
+    const uint64_t target = pk.absgp_page > absgp ? pk.absgp_page - absgp : 0;
+    return target < n ? (size_t)target : n;
+}
+
+void Granule::step(const lwf_ogg_packet &pk, size_t n)
+{
+    if (pk.last_in_page) {
+        has = true;
+        absgp = pk.absgp_page;
+    } else if (has) {
+        absgp += n;
+    }
+}
+
+int read_header_packets(lwf_ogg *o, bool chained, HeaderPackets &hp)
+{
+    lwf_ogg_packet &pk = hp.setup;
+    auto next = [&]() {
+        const int rc = lwf_ogg_next_packet(o, &pk);
+        return rc == LWF_ERR_NO_MORE_PACKETS ? (int)LWF_ERR_OGG : rc;
+    };
+    int rc;
+    if (!chained) {
+        if ((rc = next())) return rc;
+        hp.ident.assign(pk.data, pk.data + pk.len);
+        hp.serial = pk.stream_serial;
+    }
+    do {
+        if ((rc = next())) return rc;
+    } while (!chained && pk.stream_serial != hp.serial);
+    hp.comment.assign(pk.data, pk.data + pk.len);
+    do {
+        if ((rc = next())) return rc;
+    } while (!chained && pk.stream_serial != hp.serial);
+    hp.serial = pk.stream_serial;
+    return LWB_OK;
+}
+
+int next_packet_of(lwf_ogg *o, uint32_t serial, lwf_ogg_packet *pk, size_t *reads)
+{
+    for (;;) {
+        if (reads) ++*reads;
+        const int rc = lwf_ogg_next_packet(o, pk);
+        if (rc || pk->stream_serial == serial || pk->first_in_stream) return rc;
+    }
 }
 
 void assign_sets(const lwf_batcher *b, const lwf_stream_job *jobs, size_t n_jobs, std::vector<JobPlan> &plan)
@@ -2297,7 +2305,7 @@ int check_jobs(const lwf_stream_job *jobs, size_t n_jobs)
 extern "C" int lwf_batcher_decode(lwf_batcher *b, lwf_stream_job *jobs, size_t n_jobs, int out_format, void *pcm)
 {
     if (!b || (!jobs && n_jobs) || !pcm || check_jobs(jobs, n_jobs)) return LWB_ERR_INVALID;
-    LWF_GUARD(
+    return guarded([&] {
         int rc = b->release ? b->release(b, false) : LWB_OK;      // submitted batches may still read the arenas
         if (rc) return rc;
         std::vector<JobPlan> plan(n_jobs);
@@ -2350,7 +2358,7 @@ extern "C" int lwf_batcher_decode(lwf_batcher *b, lwf_stream_job *jobs, size_t n
         b->in_bytes = in_bytes;
         if (rc) return rc;
         return synth_rc;
-    )
+    });
 }
 
 // ---------------------------------------------------------------------------------------------

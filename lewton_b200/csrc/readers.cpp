@@ -1,23 +1,21 @@
 // readers.cpp -- lwf_readers (include/lewton_frontend.h): many OggStreamReaders advanced by one call.  Each reader keeps
-// what lwf_reader keeps on the host (pager, serial, absgp accounting) and its own stream state; a call de-pages and
+// what lwf_reader keeps on the host (pager, serial, granule position) and its own stream state; a call de-pages and
 // counts each job's packets on the batcher's thread pool, then hands the packets to an internal lwf_batcher's submit, so
-// that their entropy decode and synthesis are exactly lwf_batcher_submit's.  The rules of frontend.cpp's single reader
-// (reader_next_audio_packet, reader_dec_packet) are restated here per job, with the packet results of the batch:
-//   - a fresh stream state (first stream, chained stream) makes its first packet return 0 samples;
-//   - the first audio packet of a chained stream is decoded and dropped, and sets absgp to its page's;
-//   - the last packet of a stream is truncated to its page's granule position (here: by the stream's output window);
-//   - absgp moves with the samples of packets that do not end a page, and to the page's at the last one;
-//   - packets of other serials are skipped unless they begin a new stream.
+// that their entropy decode and synthesis are exactly lwf_batcher_submit's.  The header walk, the serial filter and the
+// granule position rules are the single reader's own (batcher.h); what is this file's is applying them ahead of the
+// batch, per job, and committing the reader state of the packets the batch ran.  A fresh stream state (first stream,
+// chained stream) makes its first packet return 0 samples, a chained stream's first audio packet is decoded and
+// dropped, and the cut of a stream's last packet is made by the stream's output window.
 #include <algorithm>
 #include <atomic>
 #include <cstring>
 #include <new>
-#include <stdexcept>
 #include <thread>
 #include <vector>
 
 #include "batcher.h"
 
+using lwfb::Granule;
 using lwfb::ogg_clone;
 using lwfb::run_pool;
 
@@ -37,8 +35,7 @@ struct Reader {
     size_t set = 0;                    // its SharedSet
     lwb_stream *pwr = nullptr;         // made by the first read of the stream
     uint32_t serial = 0;
-    bool has_absgp = false;
-    uint64_t absgp = 0;
+    Granule gp;
     bool fresh = true;                 // the stream state is empty: the next packet returns 0 samples
     bool pending_drop = false;         // a chained stream's headers were read: its first audio packet is dropped next
     uint8_t channels = 0, bs0 = 0, bs1 = 0;
@@ -49,8 +46,7 @@ struct Pkt {
     size_t off, len;                   // in Job::bytes
     uint32_t samples;                  // what it returns (0 for the dropped packet)
     size_t calls;                      // pager reads up to and including this packet, from the job's start
-    bool has_absgp;
-    uint64_t absgp;
+    Granule gp;
 };
 
 struct Job {
@@ -84,57 +80,41 @@ namespace {
 
 bool same(const std::vector<uint8_t> &v, const uint8_t *p, size_t n) { return v.size() == n && (n == 0 || !std::memcmp(v.data(), p, n)); }
 
-// The shared set of these header bytes; a new pair is parsed here, the only parse of its setup header (with
+// The shared set of these header packets; a new pair is parsed here, the only parse of its setup header (with
 // lwf_headers_parse's errors, those of the comment header included)
-int find_set(lwf_readers *rs, const std::vector<uint8_t> &ident, const std::vector<uint8_t> &comment, const lwf_ogg_packet &setup,
-             size_t *out)
+int find_set(lwf_readers *rs, const lwfb::HeaderPackets &hp, size_t *out)
 {
+    const lwf_ogg_packet &setup = hp.setup;
     for (size_t k = 0; k < rs->sets.size(); k++)
-        if (same(rs->sets[k]->ident, ident.data(), ident.size()) && same(rs->sets[k]->setup, setup.data, setup.len)) {
+        if (same(rs->sets[k]->ident, hp.ident.data(), hp.ident.size()) && same(rs->sets[k]->setup, setup.data, setup.len)) {
             *out = k;
             return LWB_OK;
         }
     std::unique_ptr<SharedSet> s(new SharedSet());
-    s->ident = ident;
+    s->ident = hp.ident;
     s->setup.assign(setup.data, setup.data + setup.len);
-    const int rc = lwf_headers_parse(ident.data(), ident.size(), comment.data(), comment.size(), setup.data, setup.len, &s->h);
+    const int rc =
+        lwf_headers_parse(hp.ident.data(), hp.ident.size(), hp.comment.data(), hp.comment.size(), setup.data, setup.len, &s->h);
     if (rc) return rc;
     rs->sets.push_back(std::move(s));
     *out = rs->sets.size() - 1;
     return LWB_OK;
 }
 
-// read_headers, inside_ogg.rs:19-39, as frontend.cpp's reader_read_headers (`first`: the ident packet of a chained
-// stream, already read).  The absgp accounting is left alone: a chained stream's dropped packet resets it.
+// read_headers, inside_ogg.rs:19-39 (`first`: the ident packet of a chained stream, already read).  The granule
+// position is left alone: a chained stream's dropped packet resets it.
 int read_headers(lwf_readers *rs, Reader &r, const std::vector<uint8_t> *first)
 {
-    lwf_ogg_packet pk;
-    int rc;
-    std::vector<uint8_t> ident, comment;
-    const bool chained = first != nullptr;
-    uint32_t serial = 0;
-    if (chained) {
-        ident = *first;
-        serial = r.serial;
-    } else {
-        if ((rc = lwf_ogg_next_packet(r.ogg, &pk))) return rc == LWF_ERR_NO_MORE_PACKETS ? LWF_ERR_OGG : rc;
-        ident.assign(pk.data, pk.data + pk.len);
-        serial = pk.stream_serial;
-    }
-    do {
-        if ((rc = lwf_ogg_next_packet(r.ogg, &pk))) return rc == LWF_ERR_NO_MORE_PACKETS ? LWF_ERR_OGG : rc;
-    } while (!chained && pk.stream_serial != serial);
-    comment.assign(pk.data, pk.data + pk.len);
-    do {
-        if ((rc = lwf_ogg_next_packet(r.ogg, &pk))) return rc == LWF_ERR_NO_MORE_PACKETS ? LWF_ERR_OGG : rc;
-    } while (!chained && pk.stream_serial != serial);
-    if (chained) serial = pk.stream_serial;
+    lwfb::HeaderPackets hp;
+    if (first) hp.ident = *first;
+    int rc = lwfb::read_header_packets(r.ogg, first != nullptr, hp);
+    if (rc) return rc;
     size_t set = 0;
-    if ((rc = find_set(rs, ident, comment, pk, &set))) return rc;
+    if ((rc = find_set(rs, hp, &set))) return rc;
     // the reader's own headers hold its comments only: an equal (ident, setup) pair parsed before cannot fail, so the
     // comment header is all that can, with the code the whole parse gives
     lwf_headers *h = nullptr;
-    if ((rc = lwfb::headers_sharing(rs->sets[set]->h, comment.data(), comment.size(), &h))) return rc;
+    if ((rc = lwfb::headers_sharing(rs->sets[set]->h, hp.comment.data(), hp.comment.size(), &h))) return rc;
     lwf_info info;
     lwf_headers_info(h, &info);
     if (r.hdr) lwf_headers_destroy(r.hdr);
@@ -142,9 +122,9 @@ int read_headers(lwf_readers *rs, Reader &r, const std::vector<uint8_t> *first)
     r.hdr = h;
     r.set = set;
     r.pwr = nullptr;
-    r.serial = serial;
+    r.serial = hp.serial;
     r.fresh = true;
-    r.pending_drop = chained;
+    r.pending_drop = first != nullptr;
     r.channels = info.audio_channels;
     r.bs0 = info.blocksize_0;
     r.bs1 = info.blocksize_1;
@@ -174,22 +154,22 @@ int ensure_device(lwf_readers *rs, Reader &r)
 }
 
 // De-pages up to max_packets returned packets of reader r into job j and counts the samples each returns, with the
-// reader's absgp accounting after each.  The pager advances (j.snap holds it as it was); the rest of the reader is
+// reader's granule position after each.  The pager advances (j.snap holds it as it was); the rest of the reader is
 // left to the commit, which knows which packets the batch ran.
 void depage(const lwf_readers *rs, Reader &r, uint32_t max_packets, Job &j)
 {
     if (!max_packets) return;
-    bool has_absgp = r.has_absgp, fresh = r.fresh, direct = false;
-    uint64_t absgp = r.absgp, sum = 0;
-    size_t calls = 0;
+    bool fresh = r.fresh, direct = false;
+    Granule gp = r.gp;
+    uint64_t sum = 0;
     lwf_ogg_packet pk;
     int rc = LWB_OK;
     auto next = [&]() {
-        j.calls = ++calls;
+        j.calls++;
         return lwf_ogg_next_packet(r.ogg, &pk);
     };
     auto add = [&](uint32_t samples) {
-        j.pkts.push_back(Pkt{j.bytes.size(), pk.len, samples, calls, has_absgp, absgp});
+        j.pkts.push_back(Pkt{j.bytes.size(), pk.len, samples, j.calls, gp});
         j.bytes.insert(j.bytes.end(), pk.data, pk.data + pk.len);
     };
     if (r.pending_drop) {
@@ -197,14 +177,12 @@ void depage(const lwf_readers *rs, Reader &r, uint32_t max_packets, Job &j)
         // (a fresh state: it returns nothing), absgp becomes its page's, and the packet after it is returned whatever
         // its serial
         j.drop_tried = true;
-        has_absgp = false;
         if ((rc = next())) {
             if (rc == LWF_ERR_NO_MORE_PACKETS) j.ended = true;
             else j.stop = rc;
             return;
         }
-        has_absgp = true;
-        absgp = pk.absgp_page;
+        gp = Granule{true, pk.absgp_page};
         add(0);
         j.dropped = true;
         fresh = false;
@@ -213,10 +191,7 @@ void depage(const lwf_readers *rs, Reader &r, uint32_t max_packets, Job &j)
     const lwf_headers *H = rs->sets[r.set]->h;
     bool truncated = false;
     for (uint32_t returned = 0; returned < max_packets; returned++) {
-        for (;;) {
-            if ((rc = next())) break;
-            if (direct || pk.stream_serial == r.serial || pk.first_in_stream) break;
-        }
+        rc = direct ? next() : lwfb::next_packet_of(r.ogg, r.serial, &pk, &j.calls);
         if (rc) {
             if (rc == LWF_ERR_NO_MORE_PACKETS) j.ended = true;
             else j.stop = rc;
@@ -240,22 +215,12 @@ void depage(const lwf_readers *rs, Reader &r, uint32_t max_packets, Job &j)
             break;
         }
         if (fresh) cnt = 0;
-        if (has_absgp && pk.last_in_stream) {         // inside_ogg.rs:219-222
-            const uint64_t target = pk.absgp_page > absgp ? pk.absgp_page - absgp : 0;
-            if (target < cnt) {
-                cnt = (size_t)target;
-                truncated = true;
-            }
-        }
-        if (pk.last_in_page) {                        // :223-227
-            has_absgp = true;
-            absgp = pk.absgp_page;
-        } else if (has_absgp) {
-            absgp += cnt;
-        }
+        const size_t kept = gp.cut(pk, cnt);
+        truncated = kept < cnt;
+        gp.step(pk, kept);
         fresh = false;
-        add((uint32_t)cnt);
-        sum += cnt;
+        add((uint32_t)kept);
+        sum += kept;
     }
     if (truncated) j.limit = sum;
 }
@@ -280,11 +245,10 @@ void commit(lwf_readers *rs, Reader &r, Job &j, const lwf_stream_job &sj, lwf_re
     const size_t keep = failed && f < n ? j.pkts[f].calls : j.keep_calls;
     if (keep < j.calls) rewind(r, j, keep);
     if (f > 0) {
-        r.has_absgp = j.pkts[f - 1].has_absgp;
-        r.absgp = j.pkts[f - 1].absgp;
+        r.gp = j.pkts[f - 1].gp;
         r.fresh = false;
     } else if (j.drop_tried) {
-        r.has_absgp = false;
+        r.gp.has = false;
     }
     if (j.drop_tried) r.pending_drop = false;
     out.n_packets = (uint32_t)(f > D ? f - D : 0);
@@ -440,21 +404,14 @@ extern "C" int lwf_readers_add(lwf_readers *rs, const uint8_t *data, size_t len,
     if (!r) return LWB_ERR_BUFFER;
     int rc = lwf_ogg_open(data, len, &r->ogg);
     if (rc) return rc;
-    try {
-        rc = read_headers(rs, *r, nullptr);
-        if (!rc) {
-            rs->readers.push_back(std::move(r));
-            *index = (uint32_t)(rs->readers.size() - 1);
-            return LWB_OK;
-        }
-    } catch (const std::bad_alloc &) {
-        rc = LWB_ERR_BUFFER;
-    } catch (const std::length_error &) {
-        rc = LWB_ERR_BUFFER;
-    } catch (...) {
-        rc = LWB_ERR_INVALID;
-    }
-    destroy_reader(*r);
+    rc = lwfb::guarded([&]() -> int {
+        const int hrc = read_headers(rs, *r, nullptr);
+        if (hrc) return hrc;
+        rs->readers.push_back(std::move(r));
+        *index = (uint32_t)(rs->readers.size() - 1);
+        return LWB_OK;
+    });
+    if (rc) destroy_reader(*r);     // (r is still held: the push_back failed or was not made)
     return rc;
 }
 
@@ -467,8 +424,8 @@ extern "C" int lwf_readers_last_absgp(const lwf_readers *rs, uint32_t index, uin
 {
     if (!rs || index >= rs->readers.size() || !absgp) return LWB_ERR_INVALID;
     const Reader &r = *rs->readers[index];
-    if (!r.has_absgp) return 1;
-    *absgp = r.absgp;
+    if (!r.gp.has) return 1;
+    *absgp = r.gp.absgp;
     return 0;
 }
 
@@ -488,13 +445,5 @@ extern "C" int lwf_readers_read(lwf_readers *rs, lwf_read_job *jobs, size_t n_jo
     if (!rs || !jobs || !n_jobs || !pcm || !ticket || (pcm_memory != LWB_MEM_HOST && pcm_memory != LWB_MEM_DEVICE) || out_format < 0 ||
         out_format > LWB_OUT_F16_INTERLEAVED)
         return LWB_ERR_INVALID;
-    try {
-        return read(rs, jobs, n_jobs, out_format, pcm, pcm_memory, ticket);
-    } catch (const std::bad_alloc &) {
-        return LWB_ERR_BUFFER;
-    } catch (const std::length_error &) {
-        return LWB_ERR_BUFFER;
-    } catch (...) {
-        return LWB_ERR_INVALID;
-    }
+    return lwfb::guarded([&] { return read(rs, jobs, n_jobs, out_format, pcm, pcm_memory, ticket); });
 }

@@ -15,7 +15,7 @@ import ctypes as C
 import numpy as np
 
 from . import _cabi as cabi
-from .api import AudioReadError, DecodedPacket, Floor0Record, Setup, sample_format
+from .api import AudioReadError, DecodedPacket, Floor0Record, Setup, Ticket, sample_format
 
 (ERR_END_OF_PACKET, ERR_NOT_VORBIS_HEADER, ERR_UNSUPPORTED_VERSION, ERR_HEADER_BAD_FORMAT, ERR_HEADER_BAD_TYPE,
  ERR_HEADER_IS_AUDIO, ERR_UTF8, ERR_AUDIO_IS_HEADER, ERR_OGG, ERR_NO_MORE_PACKETS) = range(16, 26)
@@ -527,16 +527,18 @@ class StreamBatcher:
         return _results(arr, n)
 
     def submit(self, jobs, pcm, stride, out_format=cabi.OUT_F32_PLANAR):
-        """lwf_batcher_submit: entropy-decodes `jobs` (as decode()), queues their synthesis and returns a BatcherTicket
-        once it is queued.  pcm: a page-locked numpy array (Context.host_alloc), a torch CUDA tensor or an integer device
-        pointer; the memory space follows from it.  The streams may be submitted again at once; `pcm` holds the PCM once
-        the ticket is done.  entropy_seconds / synthesis_seconds / input_bytes describe this submit."""
+        """lwf_batcher_submit: entropy-decodes `jobs` (as decode()), queues their synthesis and returns an api.Ticket
+        once it is queued; its wait() returns the job results [(n_samples, packets_done, status)], as run() does.  pcm: a
+        page-locked numpy array (Context.host_alloc), a torch CUDA tensor or an integer device pointer; the memory space
+        follows from it.  The streams may be submitted again at once; `pcm` holds the PCM once the ticket is done, and
+        the ticket keeps it and the job arrays alive until then.  entropy_seconds / synthesis_seconds / input_bytes
+        describe this submit."""
         addr, memory = _pcm_address(pcm)
         arr, keep, n = self._jobs(jobs, stride)
         t = C.c_uint64()
         self.ctx.check(lib().lwf_batcher_submit(self._h, arr, n, out_format, addr, memory, C.byref(t)))
         self._counters()
-        return BatcherTicket(self.ctx, t.value, arr, n, (keep, pcm))
+        return Ticket(self.ctx, t.value, (keep, pcm), lambda: _results(arr, n))
 
     def close(self):
         if self._h:
@@ -552,32 +554,6 @@ class StreamBatcher:
 
 def _results(arr, n):
     return [(arr[j].n_samples, arr[j].packets_done, arr[j].status) for j in range(n)]
-
-
-class BatcherTicket:
-    """A batch queued by StreamBatcher.submit, in the manner of api.Ticket.  It keeps `pcm` and the job arrays alive until
-    it is done; the job results were written before submit returned."""
-
-    def __init__(self, ctx, ticket, arr, n, keep):
-        self.ctx, self.id = ctx, ticket
-        self._arr, self._n, self._keep = arr, n, keep
-
-    def done(self):
-        """lwb_ticket_query: whether every copy and kernel of the batch has finished.  Never blocks."""
-        if self._keep is not None:
-            d = C.c_int()
-            self.ctx.check(cabi.lib().lwb_ticket_query(self.ctx._h, self.id, C.byref(d)))
-            if not d.value:
-                return False
-            self._keep = None
-        return True
-
-    def wait(self):
-        """lwb_ticket_wait; returns the job results [(n_samples, packets_done, status)], as StreamBatcher.run does."""
-        if self._keep is not None:
-            self.ctx.check(cabi.lib().lwb_ticket_wait(self.ctx._h, self.id))
-            self._keep = None
-        return _results(self._arr, self._n)
 
 
 def _pcm_address(pcm):
@@ -629,31 +605,6 @@ class ReadResult:
     def __repr__(self):
         return ("ReadResult(reader=%d, n_packets=%d, n_samples=%d, channels=%d, status=%d, ended=%s, next_chained=%s)" %
                 (self.reader, self.n_packets, self.n_samples, self.channels, self.status, self.ended, self.next_chained))
-
-
-class ReadTicket:
-    """A read queued by OggStreamReaders.read, in the manner of BatcherTicket: the job results (`results`) were written
-    before read returned; `pcm` holds the PCM once the ticket is done, and the ticket keeps it alive until then."""
-
-    def __init__(self, ctx, ticket, results, keep):
-        self.ctx, self.id, self.results, self._keep = ctx, ticket, results, keep
-
-    def done(self):
-        """lwb_ticket_query; never blocks."""
-        if self._keep is not None:
-            d = C.c_int()
-            self.ctx.check(cabi.lib().lwb_ticket_query(self.ctx._h, self.id, C.byref(d)))
-            if not d.value:
-                return False
-            self._keep = None
-        return True
-
-    def wait(self):
-        """lwb_ticket_wait; returns the job results [ReadResult]."""
-        if self._keep is not None:
-            self.ctx.check(cabi.lib().lwb_ticket_wait(self.ctx._h, self.id))
-            self._keep = None
-        return self.results
 
 
 class OggStreamReaders:
@@ -714,9 +665,10 @@ class OggStreamReaders:
         """lwf_readers_read.  jobs: [(reader index, max_packets)], each reader at most once.  Job j's PCM lands in `pcm`
         behind the jobs before it, each taking its reader's channels * stride elements (planar: channel c at
         offset + c * stride; stride >= self.stride(index, max_packets) of every job).  pcm: a page-locked numpy array
-        (Context.host_alloc), a torch CUDA tensor or an integer device pointer, as for StreamBatcher.submit.  Returns a
-        ReadTicket; its results are known at once, its PCM once it is done.  paging_seconds, entropy_seconds and
-        synthesis_seconds describe this read (lwf_readers_last_timing)."""
+        (Context.host_alloc), a torch CUDA tensor or an integer device pointer, as for StreamBatcher.submit.  Returns an
+        api.Ticket; its results ([ReadResult], `results` and what wait() returns) are known at once, its PCM once it is
+        done, and it keeps `pcm` alive until then.  paging_seconds, entropy_seconds and synthesis_seconds describe this
+        read (lwf_readers_last_timing)."""
         fmt, _ = sample_format(sample, interleaved)
         addr, memory = _pcm_address(pcm)
         n = len(jobs)
@@ -735,7 +687,10 @@ class OggStreamReaders:
         p, e, s = C.c_double(), C.c_double(), C.c_double()
         lib().lwf_readers_last_timing(self._h, C.byref(p), C.byref(e), C.byref(s))
         self.paging_seconds, self.entropy_seconds, self.synthesis_seconds = p.value, e.value, s.value
-        return ReadTicket(self.ctx, t.value, [ReadResult(arr[j], counts[j]) for j in range(n)], (arr, counts, pcm))
+        results = [ReadResult(arr[j], counts[j]) for j in range(n)]
+        ticket = Ticket(self.ctx, t.value, (arr, counts, pcm), lambda: results)
+        ticket.results = results
+        return ticket
 
     def read_dec_packets(self, indices, max_packets, sample="f32", interleaved=False):
         """read() into page-locked host memory and wait: per reader, the packets it returned, each in the form
