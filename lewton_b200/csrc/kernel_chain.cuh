@@ -43,22 +43,17 @@ struct ChainDesc {
     uint8_t channels;
 };
 
-// x[j] of the IMDCT output, from the post-step-7 buffer V (step 8, imdct.rs:589-658):
-//   out[m] = p_odd, out[n2-1-m] = -p_odd, out[n2+m] = p_even, out[n-1-m] = p_even,  m < n/4
+// x[j] of the IMDCT output, from the post-step-7 buffer V: the one step-8 product (d_imdct_step8) that gives it
 __device__ __forceinline__ float d_x_at(const float *V, const float *__restrict__ B, int n, int j)
 {
     const int n2 = n >> 1, n4 = n >> 2;
     if (j < n2) {
         const bool mir = j >= n4;
-        const int m = mir ? n2 - 1 - j : j;
-        const int ee = n2 - 2 - 2 * m;
-        const float p_odd = __fsub_rn(__fmul_rn(V[ee], __ldg(B + ee + 1)), __fmul_rn(V[ee + 1], __ldg(B + ee)));
+        const float p_odd = d_imdct_step8(V, B, n2, mir ? n2 - 1 - j : j).x;
         return mir ? -p_odd : p_odd;
     }
     const int jj = j - n2;
-    const int m = jj >= n4 ? n2 - 1 - jj : jj;
-    const int ee = n2 - 2 - 2 * m;
-    return __fsub_rn(__fmul_rn(-V[ee], __ldg(B + ee)), __fmul_rn(V[ee + 1], __ldg(B + ee + 1)));
+    return d_imdct_step8(V, B, n2, jj >= n4 ? n2 - 1 - jj : jj).y;
 }
 
 // MULTI = false: one warp per channel (<= 8 warps, compile-time group size, warp-level syncs);
@@ -158,16 +153,16 @@ k_chain(const ChainDesc *__restrict__ chains, const uint8_t *__restrict__ pkt_by
         if (active) {
             float *V0 = U + (n1max >> 1);
             if (ENTRY != LWB_ENTRY_SPECTRUM) {
-                d_imdct_to_v(tb, n, U, U, V0, lane, gt, gsync);
+                d_imdct_to_v<1>(tb, n, U, 0, U, V0, 0, lane, gt, gsync);
             } else {
                 const float *X = coeffs + coeff + (size_t)warp * n2;
                 const size_t xs = (size_t)C * n2;
                 uint32_t q = 0;
                 while (q < g) {                                  // pieces of 4, 2, 1 blocks
                     const uint32_t rem = g - q;
-                    if (rem >= 4) { d_imdct_to_v_np<4>(tb, n, X + q * xs, xs, U + q * n1max, V0 + q * n1max, n1max, lane, gt, gsync); q += 4; }
-                    else if (rem >= 2) { d_imdct_to_v_np<2>(tb, n, X + q * xs, xs, U + q * n1max, V0 + q * n1max, n1max, lane, gt, gsync); q += 2; }
-                    else { d_imdct_to_v(tb, n, X + q * xs, U + q * n1max, V0 + q * n1max, lane, gt, gsync); q += 1; }
+                    if (rem >= 4) { d_imdct_to_v<4>(tb, n, X + q * xs, xs, U + q * n1max, V0 + q * n1max, n1max, lane, gt, gsync); q += 4; }
+                    else if (rem >= 2) { d_imdct_to_v<2>(tb, n, X + q * xs, xs, U + q * n1max, V0 + q * n1max, n1max, lane, gt, gsync); q += 2; }
+                    else { d_imdct_to_v<1>(tb, n, X + q * xs, xs, U + q * n1max, V0 + q * n1max, n1max, lane, gt, gsync); q += 1; }
                 }
             }
         }
@@ -179,21 +174,21 @@ k_chain(const ChainDesc *__restrict__ chains, const uint8_t *__restrict__ pkt_by
             const int slope_sel = pf ? blockflag : 0;
             const int rs = nf ? n2 : (n * 3 - n0) >> 2;
             const int re = nf ? n : (n * 3 + n0) >> 2;
-            if constexpr (MIX) {
-                constexpr bool planar = out_format_of(FORMAT).planar;
-                const float *V = U + q * n1max + (n1max >> 1);
-                const float *__restrict__ B = tb.b;
-                const int olen = rs - ls, T = n1max >> 1, K = su.n_out ? su.n_out : C;
-                if (has) {
-                    const float *__restrict__ w = su.tab[slope_sel].window;
+            const int olen = rs - ls;
+            const float *V = U + q * n1max + (n1max >> 1);
+            const float *__restrict__ B = tb.b;
+            if (has) {
+                const float *__restrict__ w = su.tab[slope_sel].window;
+                if constexpr (MIX) {
+                    constexpr bool planar = out_format_of(FORMAT).planar;
+                    const int T = n1max >> 1, K = su.n_out ? su.n_out : C;
                     for (int t0 = 0; t0 < olen; t0 += T) {
                         const int tn = min(T, olen - t0);
                         if (active)
                             for (int i = lane; i < tn; i += gt) {
                                 const int j = t0 + i;
                                 float v = d_x_at(V, B, n, ls + j);
-                                if (j < plen)                          // audio.rs:1116-1118
-                                    v = __fadd_rn(__fmul_rn(v, __ldg(w + j)), __fmul_rn(prev[j], __ldg(w + plen - 1 - j)));
+                                if (j < plen) v = d_overlap_add(v, prev[j], w, plen, j);
                                 U[q * n1max + i] = v;
                             }
                         __syncthreads();
@@ -204,35 +199,21 @@ k_chain(const ChainDesc *__restrict__ chains, const uint8_t *__restrict__ pkt_by
                         }
                         __syncthreads();
                     }
-                }
-                plen = re - rs;                                        // audio.rs:1121
-                if (active) {
-                    for (int i = lane; i < plen; i += gt) prev[i] = d_x_at(V, B, n, rs + i);
-                    gsync();
-                }
-                if (has) pos += olen;
-            } else if (active) {
-                const float *V = U + q * n1max + (n1max >> 1);
-                const float *__restrict__ B = tb.b;
-                const int olen = rs - ls;
-                if (has) {
-                    const float *__restrict__ w = su.tab[slope_sel].window;
+                } else if (active) {
                     for (int i = lane; i < olen; i += gt) {
                         float v = d_x_at(V, B, n, ls + i);
-                        if (i < plen)                                  // audio.rs:1116-1118
-                            v = __fadd_rn(__fmul_rn(v, __ldg(w + i)), __fmul_rn(prev[i], __ldg(w + plen - 1 - i)));
+                        if (i < plen) v = d_overlap_add(v, prev[i], w, plen, i);
                         store_sample<FORMAT>(pcm, cd.out_off, cd.out_stride, C, warp, pos + i, v);
                     }
-                    gsync();
+                    gsync();                                   // every lane has read prev before it is refilled
                 }
-                plen = re - rs;                                        // audio.rs:1121
+            }
+            plen = re - rs;                                    // audio.rs:1121
+            if (active) {
                 for (int i = lane; i < plen; i += gt) prev[i] = d_x_at(V, B, n, rs + i);
                 gsync();
-                if (has) pos += olen;
-            } else {
-                plen = re - rs;
-                if (has) pos += rs - ls;
             }
+            if (has) pos += olen;
             has = true;
             coeff += (uint64_t)C * n2;
         }

@@ -200,18 +200,6 @@ k_prologue(const DevPacket *__restrict__ pkts, const float *__restrict__ residue
 // ---------------------------------------------------------------------------------------------
 // inverse MDCT, imdct.rs:291-659, stage by stage in shared memory
 // ---------------------------------------------------------------------------------------------
-// One rotate-and-sum butterfly of step 3 (imdct.rs:36-41 / 94-99 / 161-166): `hi` is the odd
-// index of the upper pair, `lo` of the lower pair.
-__device__ __forceinline__ void d_bfly(float *e, int hi, int lo, float w0, float w1)
-{
-    const float k00 = __fsub_rn(e[hi], e[lo]);
-    const float k01 = __fsub_rn(e[hi - 1], e[lo - 1]);
-    e[hi] = __fadd_rn(e[hi], e[lo]);
-    e[hi - 1] = __fadd_rn(e[hi - 1], e[lo - 1]);
-    e[lo] = __fsub_rn(__fmul_rn(k00, w0), __fmul_rn(k01, w1));
-    e[lo - 1] = __fadd_rn(__fmul_rn(k01, w0), __fmul_rn(k00, w1));
-}
-
 // imdct.rs:201-232, z7 = &zm7[7]
 __device__ __forceinline__ void d_iter_54(float *z7)
 {
@@ -235,132 +223,22 @@ __device__ __forceinline__ void d_iter_54(float *z7)
 
 constexpr int kImdctThreads = 128;
 
-// Steps 0-7 of inverse_mdct (imdct.rs:337-580) for one block, cooperatively by NT threads (`tid` in
-// [0, NT)) that `sync()` synchronises (a warp, a named-barrier group, or the CTA).
-// X: n/2 spectrum coefficients (global or shared; may alias U); on return V holds the post-step-7
-// buffer that step 8 reads.  Literal schedule, including the reference's behaviour for n = 64/128.
-template <class Sync>
-__device__ __forceinline__ void d_imdct_to_v(const DevTables &tb, int n, const float *X, float *U, float *V, int tid,
-                                             int NT, Sync sync)
-{
-    const int n2 = n >> 1, n4 = n >> 2, n8 = n >> 3;
-    const int ld = tb.bs;
-    const float *__restrict__ A = tb.a;
-    const float *__restrict__ Cc = tb.c;
-
-    // step 0 (imdct.rs:337-371): V <- rotated, reflected spectrum
-    for (int t = tid; t < n8; t += NT) {
-        const float x0 = X[4 * t], x2 = X[4 * t + 2];
-        const float a0 = A[2 * t], a1 = A[2 * t + 1];
-        const int d = n4 - 2 - 2 * t, ao = n4 + 2 * t, e = n2 - 3 - 4 * t;
-        const float ne2 = -X[e + 2], ne0 = -X[e];
-        const float b0 = A[ao], b1 = A[ao + 1];
-        V[n2 - 1 - 2 * t] = __fsub_rn(__fmul_rn(x0, a0), __fmul_rn(x2, a1));
-        V[n2 - 2 - 2 * t] = __fadd_rn(__fmul_rn(x0, a1), __fmul_rn(x2, a0));
-        V[d + 1] = __fsub_rn(__fmul_rn(ne2, b0), __fmul_rn(ne0, b1));
-        V[d] = __fadd_rn(__fmul_rn(ne2, b1), __fmul_rn(ne0, b0));
-    }
-    sync();
-    // step 2 (imdct.rs:385-430): U <- V
-    for (int t = tid; t < (n >> 4); t += NT) {
-        const int ao = n2 - 8 - 8 * t, hi = n4 + 4 * t, lo = 4 * t;
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-            const int o = 2 * h;                  // pair (0,1) uses A[ao+4..5], pair (2,3) A[ao..ao+1]
-            const float w0 = A[ao + 4 - 4 * h], w1 = A[ao + 5 - 4 * h];
-            const float v1 = __fsub_rn(V[hi + o + 1], V[lo + o + 1]);
-            const float v0 = __fsub_rn(V[hi + o], V[lo + o]);
-            U[hi + o + 1] = __fadd_rn(V[hi + o + 1], V[lo + o + 1]);
-            U[hi + o] = __fadd_rn(V[hi + o], V[lo + o]);
-            U[lo + o + 1] = __fsub_rn(__fmul_rn(v1, w0), __fmul_rn(v0, w1));
-            U[lo + o] = __fadd_rn(__fmul_rn(v0, w0), __fmul_rn(v1, w1));
-        }
-    }
-    sync();
-    // step 3 (imdct.rs:445-477), literal schedule: stage 0, stage 1 (a no-op for n = 64),
-    // stages 2..ld-7.  For n = 64/128 this overlaps what ld654 does again below -- the
-    // reference's behaviour, kept bit for bit.
-    for (int l = 0; l < 2 || l <= ld - 7; l++) {
-        if (l == 1 && n < 128) continue;          // r_loop(lim = n >> 5 = 2): lim >> 2 == 0 iterations
-        const int k0 = n >> (l + 2), k1 = 1 << (l + 3);
-        const int rbits = ld - l - 4;             // r < n >> (l+4)
-        for (int q = tid; q < n8; q += NT) {
-            const int r = q & ((1 << rbits) - 1), s = q >> rbits;
-            const int i = n2 - 1 - k0 * s - 2 * r;
-            d_bfly(U, i, i - (k0 >> 1), A[r * k1], A[r * k1 + 1]);
-        }
-        sync();
-    }
-    // imdct.rs:234-288 (ld654): last three stages per 16-float group
-    {
-        const float a2 = A[n >> 3];
-        for (int g = tid; g < (n >> 5); g += NT) {
-            float *z = U + (n2 - 1 - 16 * g);
-            float k00, k11;
-            k00 = __fsub_rn(z[0], z[-8]);   k11 = __fsub_rn(z[-1], z[-9]);
-            z[0] = __fadd_rn(z[0], z[-8]);  z[-1] = __fadd_rn(z[-1], z[-9]);
-            z[-8] = k00;                    z[-9] = k11;
-            k00 = __fsub_rn(z[-2], z[-10]); k11 = __fsub_rn(z[-3], z[-11]);
-            z[-2] = __fadd_rn(z[-2], z[-10]); z[-3] = __fadd_rn(z[-3], z[-11]);
-            z[-10] = __fmul_rn(__fadd_rn(k00, k11), a2);
-            z[-11] = __fmul_rn(__fsub_rn(k11, k00), a2);
-            k00 = __fsub_rn(z[-12], z[-4]); k11 = __fsub_rn(z[-5], z[-13]);
-            z[-4] = __fadd_rn(z[-4], z[-12]); z[-5] = __fadd_rn(z[-5], z[-13]);
-            z[-12] = k11;                   z[-13] = k00;
-            k00 = __fsub_rn(z[-14], z[-6]); k11 = __fsub_rn(z[-7], z[-15]);
-            z[-6] = __fadd_rn(z[-6], z[-14]); z[-7] = __fadd_rn(z[-7], z[-15]);
-            z[-14] = __fmul_rn(__fadd_rn(k00, k11), a2);
-            z[-15] = __fmul_rn(__fsub_rn(k00, k11), a2);
-            d_iter_54(z);
-            d_iter_54(z - 8);
-        }
-    }
-    sync();
-    // steps 4-6 (imdct.rs:490-528): bit-reverse shuffle U -> V
-    for (int q = tid; q < (n >> 4); q += NT) {
-        const int d0 = n4 - 4 - 4 * q, d1 = n2 - 4 - 4 * q;
-        int k4 = tb.bitrev[2 * q];
-        V[d1 + 3] = U[k4 + 0]; V[d1 + 2] = U[k4 + 1]; V[d0 + 3] = U[k4 + 2]; V[d0 + 2] = U[k4 + 3];
-        k4 = tb.bitrev[2 * q + 1];
-        V[d1 + 1] = U[k4 + 0]; V[d1 + 0] = U[k4 + 1]; V[d0 + 1] = U[k4 + 2]; V[d0 + 0] = U[k4 + 3];
-    }
-    sync();
-    // step 7 (imdct.rs:533-580), in place on V
-    for (int t = tid; t < (n >> 4); t += NT) {
-        const int d = 4 * t, e = n2 - 4 - 4 * t, co = 4 * t;
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-            const int dd = d + 2 * h, ee = e + 2 - 2 * h;
-            const float c0 = Cc[co + 2 * h], c1 = Cc[co + 2 * h + 1];
-            const float a02 = __fsub_rn(V[dd], V[ee]);
-            const float a11 = __fadd_rn(V[dd + 1], V[ee + 1]);
-            const float b0 = __fadd_rn(__fmul_rn(c1, a02), __fmul_rn(c0, a11));
-            const float b1 = __fsub_rn(__fmul_rn(c1, a11), __fmul_rn(c0, a02));
-            const float b2 = __fadd_rn(V[dd], V[ee]);
-            const float b3 = __fsub_rn(V[dd + 1], V[ee + 1]);
-            V[dd] = __fadd_rn(b2, b0);
-            V[dd + 1] = __fadd_rn(b3, b1);
-            V[ee] = __fsub_rn(b2, b0);
-            V[ee + 1] = __fsub_rn(b1, b3);
-        }
-    }
-    sync();
-}
-
-// The same transform for NP independent blocks of one size at once (block q: spectrum X + q * xs,
-// buffers U + q * bs and V + q * bs).  Arithmetic per block is identical to d_imdct_to_v; every stage
-// first loads the operands of all NP blocks, then computes, then stores, so that a thread has NP
-// independent dependency chains in flight instead of one -- the transform is latency-bound for small
-// n, where a stage is a single butterfly per lane and each instruction waits on the one before it.
+// Steps 0-7 of inverse_mdct (imdct.rs:337-580) for NP independent blocks of one size, cooperatively by NT threads (`tid`
+// in [0, NT)) that `sync()` synchronises (a warp, a named-barrier group, or the CTA).  Block q: spectrum X + q * xs (n/2
+// coefficients, global or shared; may alias U when NP = 1), buffers U + q * bs and V + q * bs; on return V holds the
+// post-step-7 buffer that step 8 (d_imdct_step8) reads.  Literal schedule, including the reference's behaviour for
+// n = 64/128.  Every stage first loads the operands of all NP blocks, then computes, then stores, so that a thread has
+// NP independent dependency chains in flight instead of one -- the transform is latency-bound for small n, where a
+// stage is a single butterfly per lane and each instruction waits on the one before it.
 template <int NP, class Sync>
-__device__ __forceinline__ void d_imdct_to_v_np(const DevTables &tb, int n, const float *X, size_t xs, float *U, float *V, int bs,
-                                                int tid, int NT, Sync sync)
+__device__ __forceinline__ void d_imdct_to_v(const DevTables &tb, int n, const float *X, size_t xs, float *U, float *V, int bs,
+                                             int tid, int NT, Sync sync)
 {
     const int n2 = n >> 1, n4 = n >> 2, n8 = n >> 3;
     const int ld = tb.bs;
     const float *__restrict__ A = tb.a;
     const float *__restrict__ Cc = tb.c;
-    // step 0
+    // step 0 (imdct.rs:337-371): V <- rotated, reflected spectrum
     for (int t = tid; t < n8; t += NT) {
         const float a0 = A[2 * t], a1 = A[2 * t + 1];
         const int d = n4 - 2 - 2 * t, ao = n4 + 2 * t, e = n2 - 3 - 4 * t;
@@ -381,12 +259,12 @@ __device__ __forceinline__ void d_imdct_to_v_np(const DevTables &tb, int n, cons
         }
     }
     sync();
-    // step 2
+    // step 2 (imdct.rs:385-430): U <- V
     for (int t = tid; t < (n >> 4); t += NT) {
         const int ao = n2 - 8 - 8 * t, hi = n4 + 4 * t, lo = 4 * t;
 #pragma unroll
         for (int h = 0; h < 2; h++) {
-            const int o = 2 * h;
+            const int o = 2 * h;                  // pair (0,1) uses A[ao+4..5], pair (2,3) A[ao..ao+1]
             const float w0 = A[ao + 4 - 4 * h], w1 = A[ao + 5 - 4 * h];
             float h1[NP], l1[NP], h0[NP], l0[NP];
 #pragma unroll
@@ -406,11 +284,13 @@ __device__ __forceinline__ void d_imdct_to_v_np(const DevTables &tb, int n, cons
         }
     }
     sync();
-    // step 3, literal schedule
+    // step 3 (imdct.rs:445-477), literal schedule: stage 0, stage 1 (a no-op for n = 64),
+    // stages 2..ld-7.  For n = 64/128 this overlaps what ld654 does again below -- the
+    // reference's behaviour, kept bit for bit.  Each butterfly is imdct.rs:36-41 / 94-99 / 161-166.
     for (int l = 0; l < 2 || l <= ld - 7; l++) {
-        if (l == 1 && n < 128) continue;
+        if (l == 1 && n < 128) continue;          // r_loop(lim = n >> 5 = 2): lim >> 2 == 0 iterations
         const int k0 = n >> (l + 2), k1 = 1 << (l + 3);
-        const int rbits = ld - l - 4;
+        const int rbits = ld - l - 4;             // r < n >> (l+4)
         for (int qq = tid; qq < n8; qq += NT) {
             const int r = qq & ((1 << rbits) - 1), s = qq >> rbits;
             const int i = n2 - 1 - k0 * s - 2 * r, lo = i - (k0 >> 1);
@@ -433,12 +313,12 @@ __device__ __forceinline__ void d_imdct_to_v_np(const DevTables &tb, int n, cons
         }
         sync();
     }
-    // ld654: 16-float groups; NP blocks x (n >> 5) groups share the threads
+    // imdct.rs:234-288 (ld654): last three stages per 16-float group; NP blocks x (n >> 5) groups share the threads
     {
         const float a2 = A[n >> 3];
         const int groups = n >> 5;
         for (int gq = tid; gq < groups * NP; gq += NT) {
-            const int q = gq / groups, g = gq - q * groups;
+            const int q = NP == 1 ? 0 : gq / groups, g = gq - q * groups;
             float *z = U + q * bs + (n2 - 1 - 16 * g);
             float k00, k11;
             k00 = __fsub_rn(z[0], z[-8]);   k11 = __fsub_rn(z[-1], z[-9]);
@@ -460,7 +340,7 @@ __device__ __forceinline__ void d_imdct_to_v_np(const DevTables &tb, int n, cons
         }
     }
     sync();
-    // steps 4-6: bit-reverse shuffle U -> V
+    // steps 4-6 (imdct.rs:490-528): bit-reverse shuffle U -> V
     for (int qq = tid; qq < (n >> 4); qq += NT) {
         const int d0 = n4 - 4 - 4 * qq, d1 = n2 - 4 - 4 * qq;
         const int ka = tb.bitrev[2 * qq], kb = tb.bitrev[2 * qq + 1];
@@ -479,7 +359,7 @@ __device__ __forceinline__ void d_imdct_to_v_np(const DevTables &tb, int n, cons
         }
     }
     sync();
-    // step 7, in place on V
+    // step 7 (imdct.rs:533-580), in place on V
     for (int t = tid; t < (n >> 4); t += NT) {
         const int d = 4 * t, e = n2 - 4 - 4 * t, co = 4 * t;
 #pragma unroll
@@ -511,6 +391,16 @@ __device__ __forceinline__ void d_imdct_to_v_np(const DevTables &tb, int n, cons
     sync();
 }
 
+// Step 8 of inverse_mdct (imdct.rs:589-658) for output index m < n/4, from the post-step-7 buffer V: (p_odd, p_even),
+// which give x[m] = p_odd, x[n2-1-m] = -p_odd, x[n2+m] = p_even, x[n-1-m] = p_even.
+__device__ __forceinline__ float2 d_imdct_step8(const float *V, const float *__restrict__ B, int n2, int m)
+{
+    const int ee = n2 - 2 - 2 * m;                // V/B pair consumed for output index m
+    const float v0 = V[ee], v1 = V[ee + 1];
+    const float b0 = __ldg(B + ee), b1 = __ldg(B + ee + 1);
+    return make_float2(__fsub_rn(__fmul_rn(v0, b1), __fmul_rn(v1, b0)), __fsub_rn(__fmul_rn(-v0, b0), __fmul_rn(v1, b1)));
+}
+
 // grid = (packets, max channels); dynamic smem = n floats (U and V halves).
 // in: spectrum [channels][n/2] at coeff_off; out: x [channels][n] at x_off.
 __global__ void __launch_bounds__(kImdctThreads)
@@ -527,18 +417,13 @@ k_imdct(const DevPacket *__restrict__ pkts, const float *__restrict__ spec, floa
     extern __shared__ float smem[];
     float *U = smem, *V = smem + n2;
     const int tid = threadIdx.x;
-    d_imdct_to_v(tb, n, X, U, V, tid, kImdctThreads, [] { __syncthreads(); });
-    // step 8 + decode (imdct.rs:589-658)
+    d_imdct_to_v<1>(tb, n, X, 0, U, V, 0, tid, kImdctThreads, [] { __syncthreads(); });
     for (int m = tid; m < n4; m += kImdctThreads) {
-        const int ee = n2 - 2 - 2 * m;            // V/B pair consumed for output index m
-        const float v0 = V[ee], v1 = V[ee + 1];
-        const float b0 = B[ee], b1 = B[ee + 1];
-        const float p_odd = __fsub_rn(__fmul_rn(v0, b1), __fmul_rn(v1, b0));
-        const float p_even = __fsub_rn(__fmul_rn(-v0, b0), __fmul_rn(v1, b1));
-        out[m] = p_odd;
-        out[n2 - 1 - m] = -p_odd;
-        out[n2 + m] = p_even;
-        out[n - 1 - m] = p_even;
+        const float2 pp = d_imdct_step8(V, B, n2, m);
+        out[m] = pp.x;
+        out[n2 - 1 - m] = -pp.x;
+        out[n2 + m] = pp.y;
+        out[n - 1 - m] = pp.y;
     }
 }
 
@@ -562,51 +447,38 @@ __device__ __forceinline__ float d_mix_sample(const DevSetup &su, int k, X x)
     return y;
 }
 
-// MIX: grid.y is the output channel k of the packet's setup (its input channels without a mix); each block recomputes
-// the overlap-add of the input channels row k uses, from x and the previous right half, and stores their mix.
+// Sample i < plen of a block's left part, x, overlap-added with sample i of the previous block's right half, pv
+// (audio.rs:1116-1118): x windowed by w, pv by w in reverse, summed.  Samples from plen on pass unchanged.
+__device__ __forceinline__ float d_overlap_add(float x, float pv, const float *__restrict__ w, int plen, int i)
+{
+    return __fadd_rn(__fmul_rn(x, w[i]), __fmul_rn(pv, w[plen - 1 - i]));
+}
+
+// grid.y is the output channel k of the packet's setup: its input channel without MIX or without a mix.  MIX: each block
+// recomputes the overlap-add of the input channels row k uses, from x and the previous right half, and stores their mix.
 template <int FORMAT, bool MIX = false>
 __global__ void __launch_bounds__(kOverlapThreads)
 k_overlap(const DevPacket *__restrict__ pkts, const float *__restrict__ x, void *__restrict__ pcm)
 {
     const DevPacket &p = pkts[blockIdx.x];
+    const DevSetup &su = *p.setup;
     const int ch = blockIdx.y;
-    if constexpr (MIX) {
-        const DevSetup &su = *p.setup;
-        const int K = su.n_out ? su.n_out : p.channels;
-        if (ch >= K || p.plen == 0) return;
-        const int n = p.n, plen = p.plen, ls = p.ls, olen = p.rs - p.ls;
-        const float *__restrict__ w = su.tab[p.slope_sel].window;
-        const DevPacket *q = p.prev_packet >= 0 ? &pkts[p.prev_packet] : nullptr;
-        for (int i = threadIdx.x; i < olen; i += kOverlapThreads) {
-            auto ola = [&](int c) {                        // the unmixed path's sample of channel c
-                float v = x[p.x_off + (size_t)c * n + ls + i];
-                if (i < plen) {
-                    const float pv = q ? x[q->x_off + (size_t)c * q->n + p.prev_rs + i] : p.state[(size_t)c * p.state_stride + i];
-                    v = __fadd_rn(__fmul_rn(v, w[i]), __fmul_rn(pv, w[plen - 1 - i]));
-                }
-                return v;
-            };
-            store_sample<FORMAT>(pcm, p.out_off, p.out_stride, K, ch, i, su.n_out ? d_mix_sample(su, ch, ola) : ola(ch));
-        }
-        return;
-    }
-    if (ch >= p.channels || p.plen == 0) return;      // audio.rs:1140-1151: no previous -> no output
-    const int n = p.n;
-    const float *__restrict__ xc = x + p.x_off + (size_t)ch * n;
-    const float *__restrict__ prev;
-    if (p.prev_packet >= 0) {
-        const DevPacket &q = pkts[p.prev_packet];
-        prev = x + q.x_off + (size_t)ch * q.n + p.prev_rs;
-    } else {
-        prev = p.state + (size_t)ch * p.state_stride;
-    }
-    const float *__restrict__ w = p.setup->tab[p.slope_sel].window;
-    const int plen = p.plen, ls = p.ls, olen = p.rs - p.ls;
+    const bool mix = MIX && su.n_out;
+    const int K = mix ? su.n_out : p.channels;
+    if (ch >= K || p.plen == 0) return;                // audio.rs:1140-1151: no previous -> no output
+    const int n = p.n, plen = p.plen, ls = p.ls, olen = p.rs - p.ls;
+    const float *__restrict__ w = su.tab[p.slope_sel].window;
+    const DevPacket *q = p.prev_packet >= 0 ? &pkts[p.prev_packet] : nullptr;
+    auto prev_of = [&](int c) {                        // channel c's previous right half
+        return q ? x + q->x_off + (size_t)c * q->n + p.prev_rs : p.state + (size_t)c * p.state_stride;
+    };
+    const float *__restrict__ prev_ch = prev_of(ch);   // without MIX, every sample's channel is ch
     for (int i = threadIdx.x; i < olen; i += kOverlapThreads) {
-        float v = xc[ls + i];
-        if (i < plen)                                  // audio.rs:1116-1118
-            v = __fadd_rn(__fmul_rn(v, w[i]), __fmul_rn(prev[i], w[plen - 1 - i]));
-        store_sample<FORMAT>(pcm, p.out_off, p.out_stride, p.channels, ch, i, v);
+        auto ola = [&](int c) {                        // the unmixed sample of channel c
+            const float v = x[p.x_off + (size_t)c * n + ls + i];
+            return i < plen ? d_overlap_add(v, (MIX ? prev_of(c) : prev_ch)[i], w, plen, i) : v;
+        };
+        store_sample<FORMAT>(pcm, p.out_off, p.out_stride, K, ch, i, mix ? d_mix_sample(su, ch, ola) : ola(ch));
     }
 }
 

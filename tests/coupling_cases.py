@@ -15,7 +15,7 @@ below):
       front stages refuse (a residue row off a 16-byte boundary), 2 channels, <= 1 step;
   S7  k_prologue through d_inverse_couple_regs (kernels_generic.cuh:145-159): the same, every other shape of <= 8 channels;
   S8  k_prologue's two passes (kernels_generic.cuh:163-174): more than 8 channels, any path;
-  S9  k_chain's front half (kernel_chain.cuh:136-154, d_inverse_couple_regs): interleaved output, <= 8 channels;
+  S9  k_chain's front half (kernel_chain.cuh:131-149, d_inverse_couple_regs): interleaved output, <= 8 channels;
   S10 lwb_debug_packet_taps' post_inverse (lwb_api.cu:1224-1238): k_prologue on one packet under unit dense floors.
 
 Which kernels prove a site ran are in SITES; the GPU modules hold every batch to them with expect_kernels.
