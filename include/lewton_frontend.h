@@ -226,7 +226,8 @@ uint64_t lwf_batcher_last_input_bytes(const lwf_batcher *b);
  * sample counting, then their entropy decode, run on the host thread pool; their synthesis is one lwb_submit_chains
  * batch per group of equal channel count and blocksize pair, as lwf_batcher_submit makes it (residue entry, dense
  * floor-0 curves, as lwf_reader decodes).  Each reader returns exactly what a single lwf_reader would return for the
- * same bytes.  Seeking and skipping stay on lwf_reader. */
+ * same bytes, for reads (lwf_readers_read), page-granular seeks (lwf_readers_seek_absgp_pg) and linear skips
+ * (lwf_readers_skip_samples_linear) in any order. */
 typedef struct lwf_readers lwf_readers;     /* many OggStreamReaders on one ctx, one host thread pool */
 int lwf_readers_create(lwb_ctx *ctx, int threads, lwf_readers **out);       /* threads <= 0: one per host CPU */
 void lwf_readers_destroy(lwf_readers *rs);                                   /* waits for its queued reads */
@@ -239,8 +240,9 @@ const lwf_headers *lwf_readers_headers(const lwf_readers *rs, uint32_t index); /
 int lwf_readers_last_absgp(const lwf_readers *rs, uint32_t index, uint64_t *absgp); /* as lwf_reader_last_absgp */
 /* distinct (ident, setup) header byte pairs among the streams the readers have opened: one lwb_setup each */
 uint32_t lwf_readers_setup_count(const lwf_readers *rs);
-/* wall-clock seconds of the last accepted lwf_readers_read: the de-paging and sample counting pass, and the
- * internal batcher's entropy decode and rest of its submit (lwf_batcher_last_timing) */
+/* wall-clock seconds of the last accepted lwf_readers_read or lwf_readers_skip_samples_linear: the de-paging and sample
+ * counting pass (all rounds of a skip's walk), and the internal batcher's entropy decode and rest of its submit
+ * (lwf_batcher_last_timing) */
 void lwf_readers_last_timing(const lwf_readers *rs, double *paging_seconds, double *entropy_seconds, double *synthesis_seconds);
 
 typedef struct lwf_read_job {
@@ -291,6 +293,58 @@ typedef struct lwf_read_job {
  * have their results and their readers have advanced; the others are unchanged. */
 int lwf_readers_read(lwf_readers *rs, lwf_read_job *jobs, size_t n_jobs, int out_format, void *pcm, int pcm_memory,
                      uint64_t *ticket);
+
+/* lwf_reader_seek_absgp_pg for each listed reader: a page-granular seek inside the logical stream the single reader
+ * stands in, to the last page whose granule position is <= absgps[k]; afterwards lwf_readers_last_absgp is None and the
+ * next packet returns 0 samples.  status[k] gets the single reader's code (LWF_ERR_OGG for a bad page on the way or no
+ * page of the stream; the reader's position is then unchanged).  A reader whose last read job ended with next_chained
+ * seeks where the single reader would: in the stream before, whose headers lwf_readers_headers gives again.
+ * The pages are walked on the host thread pool, one task per reader.  Only host state changes: no GPU work is queued, no
+ * ticket is issued, and reads still queued are not waited for (they keep the PCM and states they were queued with).
+ * Refusals -- LWB_ERR_INVALID for a NULL rs, readers, absgps or status, n == 0, an unknown reader index or a reader
+ * listed twice -- change no reader and no status element. */
+int (lwf_readers_seek_absgp_pg)(lwf_readers *rs, const uint32_t *readers, const uint64_t *absgps, size_t n, int32_t *status);
+
+typedef struct lwf_skip_job {
+    uint32_t reader;          /* index from lwf_readers_add; a reader may appear in at most one job per call           */
+    uint32_t out_channels;    /* channels of room at out_offset (0: the reader's current stream's channel count)      */
+    uint64_t to_skip;         /* samples per channel to skip                                                           */
+    uint64_t out_offset;      /* element offset of this job's PCM in `pcm`                                             */
+    uint64_t out_stride;      /* planar: elements between channel planes; interleaved: room per channel               */
+    /* results */
+    uint64_t left_to_skip;    /* the second element of skip_samples_linear's tuple                                     */
+    uint32_t n_samples;       /* samples per channel of the returned packet                                            */
+    uint8_t  got_packet;      /* 1: a packet was returned (Ok((Some, _))); 0: the stream ended first, or status != 0   */
+    uint8_t  channels;        /* channel count of the stream the reader stands in afterwards                           */
+    uint8_t  reserved[2];
+    int32_t  status;          /* LWB_OK or the code the single reader's call returned                                  */
+} lwf_skip_job;
+/* lwf_reader_skip_samples_linear for each job's reader, with the target packets' synthesis queued asynchronously in the
+ * manner of lwf_readers_read.
+ * Equivalence: each job returns what one lwf_reader_skip_samples_linear call returns on the same bytes: the target
+ * packet's PCM (written sample j goes to out_offset + c * out_stride + j planar, out_offset + j * channels + c
+ * interleaved; f32 bit for bit, i16 and f16 exactly), n_samples, left_to_skip (to_skip itself when status != 0), the end
+ * of the stream (got_packet = 0, status LWB_OK), errors, and lwf_readers_last_absgp, lwf_readers_headers and the overlap
+ * state afterwards.  Nothing outside the job's n_samples samples per channel is written.
+ * Passes: the walk that only counts samples runs on the host thread pool.  It stops at a chained stream, whose headers
+ * are read between rounds of the pool (they change the readers' shared header sets); it then continues in the new
+ * stream after decoding and dropping its first audio packet, as the single reader does.  The synthesis is one batch per
+ * group, through the internal batcher, as a read's: a job's chain is the packet before the target and the target on a
+ * reset stream state (the packet before returns nothing), or, where the single reader has no packet before it (the
+ * first packet of the walk, or a stream's last packet with a known granule position), the target alone on the state the
+ * reader stands in -- behind a chained stream's dropped packet if the walk entered one.  A target that is its stream's
+ * truncated last packet is cut by the stream's output window, as reads cut it.  A job whose walk ends without a target
+ * but after dropping a chained stream's first packet synthesises that packet alone, writing nothing.
+ * A job that crossed into a chained stream lays its target out with that stream's channel count and blocksizes; it
+ * needs out_channels >= that count, and out_stride >= blocksize_1 / 2 + (blocksize_1 - blocksize_0) / 4 of that stream
+ * (planar) or (interleaved) out_channels * out_stride >= its channels times that: otherwise the whole call is refused.
+ * pcm_memory, page-locked host memory, tickets, the ring of two arena sets and the places the call blocks are
+ * lwf_readers_read's.
+ * Refusals -- lwf_readers_read's, with max_packets = 1 for the planar stride rule, out_channels (if not 0) below the
+ * reader's channel count, and the crossing rule above -- change no job, reader, stream state or PCM element and issue no
+ * ticket (a chained stream's headers read by the refused walk may stay parsed for a later call). */
+int (lwf_readers_skip_samples_linear)(lwf_readers *rs, lwf_skip_job *jobs, size_t n_jobs, int out_format, void *pcm,
+                                      int pcm_memory, uint64_t *ticket);
 
 /* ---- debug taps (known-answer tests of the reference's unit-test vectors) ---------------------- */
 float lwf_debug_float32_unpack(uint32_t v);                          /* bitpacking.rs:304-314        */

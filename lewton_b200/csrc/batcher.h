@@ -127,6 +127,24 @@ struct Granule {
     void step(const lwf_ogg_packet &pk, size_t n);
 };
 
+// skip_samples_linear's walk (inside_ogg.rs:244-283) over packets measured by their sample counts only
+struct SkipWalk {
+    size_t to_skip = 0;
+    bool have_last = false;            // last_pck: a packet was measured and passed over before the current one
+    // Feeds the next packet pk, whose header says it decodes to n samples.  True: pk is the target (to_skip < its
+    // samples after the end-of-stream cut; gp is left for its decode).  False: pk is passed over -- to_skip and gp's
+    // absgp (if known, whatever the page, :275-277) go past its samples, and it becomes last_pck.  A stream's last
+    // packet, if gp is known, clears last_pck first (:258-262).
+    bool target(Granule &gp, const lwf_ogg_packet &pk, size_t n);
+};
+
+// The pager's byte offset: where its next page begins
+size_t pager_offset(const lwf_ogg *o);
+// seek_absgp_pg's page walk (inside_ogg.rs:307-313): the pager moves to the start of the last page of logical stream
+// `serial`, at or after byte `from`, whose granule position is <= absgp (its first page if none is).  LWF_ERR_OGG, and
+// the pager unchanged, for a bad page on the way or no page of the stream.
+int pager_seek(lwf_ogg *o, uint32_t serial, uint64_t absgp, size_t from);
+
 // The header packets of a logical stream, as read_headers (inside_ogg.rs:19-39) gathers them
 struct HeaderPackets {
     std::vector<uint8_t> ident, comment;
@@ -163,6 +181,11 @@ void job_results(lwf_stream_job *jobs, const BatchArena &ar, const std::vector<J
 struct SetupShape { const lwb_ctx *ctx; uint8_t channels, bs0, bs1; };
 SetupShape setup_shape(const lwb_setup *su);
 const lwb_setup *stream_setup(const lwb_stream *s);
+// A stream's PreviousWindowRight flags (host only): read before lwb_stream_reset, and put back to undo it while no
+// batch has been queued on the stream since
+struct StreamFlags { bool has; uint32_t plen; };
+StreamFlags stream_flags(const lwb_stream *s);
+void set_stream_flags(lwb_stream *s, StreamFlags f);
 // The refusals lwb_submit_chains would make of this batch (out_format, streams, one channel count, a stream in two
 // chains, floor kinds, out_stride, VQ offsets, page-locked host memory), made without queuing anything or changing any state.
 int check_submit(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io);

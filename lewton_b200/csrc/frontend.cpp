@@ -1739,7 +1739,7 @@ static int reader_read_headers(lwf_reader *r, const lwf_ogg_packet *first)
     if ((rc = lwb_stream_open(r->ctx, r->setup, &r->pwr))) return rc;
     r->serial = hp.serial;
     r->gp.has = false;
-    r->audio_start = r->ogg->o.at;
+    r->audio_start = lwfb::pager_offset(r->ogg);
     const size_t C = h->body().ident.audio_channels, n2 = (size_t)1 << (h->body().ident.blocksize_1 - 1);
     r->kinds.assign(C, 0);
     r->ys.assign(C * LWB_MAX_POSTS, 0);
@@ -1852,20 +1852,19 @@ extern "C" int lwf_reader_skip_samples_linear(lwf_reader *r, size_t to_skip, int
     *left_to_skip = to_skip;
     return guarded([&]() -> int {
         std::vector<uint8_t> last;             // Option<Packet>: the packet read before `next`
-        bool have_last = false;
         lwf_ogg_packet last_pk;
         std::memset(&last_pk, 0, sizeof(last_pk));
+        lwfb::SkipWalk walk;
+        walk.to_skip = to_skip;
         for (;;) {
             lwf_ogg_packet next;
             int rc = reader_next_audio_packet(r, &next);
-            if (rc == LWF_ERR_NO_MORE_PACKETS) { *left_to_skip = to_skip; return LWB_OK; }      // Ok((None, to_skip))
+            if (rc == LWF_ERR_NO_MORE_PACKETS) { *left_to_skip = walk.to_skip; return LWB_OK; }      // Ok((None, to_skip))
             if (rc) return rc;
             size_t cnt = 0;
             if ((rc = lwf_decoded_sample_count(r->hdr, next.data, next.len, &cnt))) return rc;
-            if (r->gp.has && next.last_in_stream) have_last = false;       // :258-262
-            cnt = r->gp.cut(next, cnt);
-            if (to_skip < cnt) {                                   // :263-271
-                if (have_last) {
+            if (walk.target(r->gp, next, cnt)) {                  // :263-271
+                if (walk.have_last) {
                     lwb_stream_reset(r->pwr);
                     const size_t C = r->hdr->h.ident.audio_channels, n1 = (size_t)1 << r->hdr->h.ident.blocksize_1;
                     r->scratch.resize(C * n1);
@@ -1877,14 +1876,11 @@ extern "C" int lwf_reader_skip_samples_linear(lwf_reader *r, size_t to_skip, int
                 }
                 if ((rc = reader_dec_packet(r, next, out_format, out, cap_total, n_samples))) return rc;
                 *got_packet = 1;
-                *left_to_skip = to_skip;
+                *left_to_skip = walk.to_skip;
                 return LWB_OK;
             }
-            to_skip -= cnt;
-            if (r->gp.has) r->gp.absgp += cnt;                     // :275-277, whatever the page
             last.assign(next.data, next.data + next.len);
             last_pk = next;
-            have_last = true;
         }
     });
 }
@@ -1894,7 +1890,7 @@ extern "C" int lwf_reader_seek_absgp_pg(lwf_reader *r, uint64_t absgp)
 {
     if (!r) return LWB_ERR_INVALID;
     return guarded([&] {
-        const int rc = r->ogg->o.seek_absgp(r->serial, absgp, r->audio_start);
+        const int rc = lwfb::pager_seek(r->ogg, r->serial, absgp, r->audio_start);
         if (rc) return rc;
         r->gp.has = false;
         return lwb_stream_reset(r->pwr);
@@ -2028,6 +2024,21 @@ void Granule::step(const lwf_ogg_packet &pk, size_t n)
         absgp += n;
     }
 }
+
+bool SkipWalk::target(Granule &gp, const lwf_ogg_packet &pk, size_t n)
+{
+    if (gp.has && pk.last_in_stream) have_last = false;
+    n = gp.cut(pk, n);
+    if (to_skip < n) return true;
+    to_skip -= n;
+    if (gp.has) gp.absgp += n;
+    have_last = true;
+    return false;
+}
+
+size_t pager_offset(const lwf_ogg *o) { return o->o.at; }
+
+int pager_seek(lwf_ogg *o, uint32_t serial, uint64_t absgp, size_t from) { return o->o.seek_absgp(serial, absgp, from); }
 
 int read_header_packets(lwf_ogg *o, bool chained, HeaderPackets &hp)
 {

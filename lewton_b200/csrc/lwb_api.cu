@@ -1057,6 +1057,10 @@ SetupShape setup_shape(const lwb_setup *su) { return SetupShape{su->ctx, su->cha
 
 const lwb_setup *stream_setup(const lwb_stream *s) { return s->setup; }
 
+StreamFlags stream_flags(const lwb_stream *s) { return StreamFlags{s->has, s->plen}; }
+
+void set_stream_flags(lwb_stream *s, StreamFlags f) { set_stream_state(s, f.has, f.plen); }
+
 // The walk lwb_submit_chains makes of this batch (walk_batch), queuing nothing.
 int check_submit(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io)
 {

@@ -1,11 +1,13 @@
 // readers.cpp -- lwf_readers (include/lewton_frontend.h): many OggStreamReaders advanced by one call.  Each reader keeps
-// what lwf_reader keeps on the host (pager, serial, granule position) and its own stream state; a call de-pages and
-// counts each job's packets on the batcher's thread pool, then hands the packets to an internal lwf_batcher's submit, so
-// that their entropy decode and synthesis are exactly lwf_batcher_submit's.  The header walk, the serial filter and the
-// granule position rules are the single reader's own (batcher.h); what is this file's is applying them ahead of the
-// batch, per job, and committing the reader state of the packets the batch ran.  A fresh stream state (first stream,
-// chained stream) makes its first packet return 0 samples, a chained stream's first audio packet is decoded and
-// dropped, and the cut of a stream's last packet is made by the stream's output window.
+// what lwf_reader keeps on the host (pager, serial, granule position, where its stream's audio starts) and its own stream
+// state; a read de-pages and counts each job's packets on the batcher's thread pool, then hands the packets to an
+// internal lwf_batcher's submit, so that their entropy decode and synthesis are exactly lwf_batcher_submit's.  A skip
+// walks the packets by their sample counts on the pool and submits each job's target the same way; a seek walks pages on
+// the pool and touches host state only.  The header walk, the serial filter, the granule position and skip rules are the
+// single reader's own (batcher.h); what is this file's is applying them ahead of the batch, per job, and committing the
+// reader state of the packets the batch ran.  A fresh stream state (first stream, chained stream, after a seek) makes
+// its first packet return 0 samples, a chained stream's first audio packet is decoded and dropped, and the cut of a
+// stream's last packet is made by the stream's output window.
 #include <algorithm>
 #include <atomic>
 #include <cstring>
@@ -17,6 +19,7 @@
 
 using lwfb::Granule;
 using lwfb::ogg_clone;
+using lwfb::pager_offset;
 using lwfb::run_pool;
 
 namespace {
@@ -39,6 +42,11 @@ struct Reader {
     bool fresh = true;                 // the stream state is empty: the next packet returns 0 samples
     bool pending_drop = false;         // a chained stream's headers were read: its first audio packet is dropped next
     uint8_t channels = 0, bs0 = 0, bs1 = 0;
+    size_t audio_start = 0;            // pager offset of the first page after the stream's headers (where seeks start)
+    // While pending_drop after a read job stopped at a chained stream: the reader as the single reader still stands, in
+    // the stream before, with its pager where the single reader's next call reads the new stream's ident.  A seek goes
+    // back to it; the drop releases it.  (Readers are copied shallowly: which copy owns what is said where they are.)
+    Reader *before_chain = nullptr;
 };
 
 // One packet of a job's chain and the reader's accounting once it has been returned
@@ -73,7 +81,7 @@ struct lwf_readers {
     std::vector<std::unique_ptr<SharedSet>> sets;
     lwf_batcher *batcher = nullptr;    // made with the first device setup
     std::vector<lwb_stream *> retired; // stream states of streams that a chained stream replaced (queued reads may use them)
-    double t_paging = 0, t_entropy = 0, t_synth = 0;   // of the last lwf_readers_read
+    double t_paging = 0, t_entropy = 0, t_synth = 0;   // of the last lwf_readers_read or lwf_readers_skip_samples_linear
 };
 
 namespace {
@@ -102,7 +110,8 @@ int find_set(lwf_readers *rs, const lwfb::HeaderPackets &hp, size_t *out)
 }
 
 // read_headers, inside_ogg.rs:19-39 (`first`: the ident packet of a chained stream, already read).  The granule
-// position is left alone: a chained stream's dropped packet resets it.
+// position is left alone: a chained stream's dropped packet resets it.  The headers and stream state r held are not
+// released: the caller, which keeps a copy of r from before, decides what becomes of them.
 int read_headers(lwf_readers *rs, Reader &r, const std::vector<uint8_t> *first)
 {
     lwfb::HeaderPackets hp;
@@ -117,8 +126,6 @@ int read_headers(lwf_readers *rs, Reader &r, const std::vector<uint8_t> *first)
     if ((rc = lwfb::headers_sharing(rs->sets[set]->h, hp.comment.data(), hp.comment.size(), &h))) return rc;
     lwf_info info;
     lwf_headers_info(h, &info);
-    if (r.hdr) lwf_headers_destroy(r.hdr);
-    if (r.pwr) rs->retired.push_back(r.pwr);
     r.hdr = h;
     r.set = set;
     r.pwr = nullptr;
@@ -128,6 +135,50 @@ int read_headers(lwf_readers *rs, Reader &r, const std::vector<uint8_t> *first)
     r.channels = info.audio_channels;
     r.bs0 = info.blocksize_0;
     r.bs1 = info.blocksize_1;
+    r.audio_start = pager_offset(r.ogg);
+    return LWB_OK;
+}
+
+// Releases what reader state `old` holds and `now` does not: headers, stream state (retired: queued batches may still
+// use it), pager and the reader before a chain.
+void release_unshared(lwf_readers *rs, Reader &old, const Reader &now)
+{
+    if (old.hdr && old.hdr != now.hdr) lwf_headers_destroy(old.hdr);
+    if (old.pwr && old.pwr != now.pwr) rs->retired.push_back(old.pwr);
+    if (old.ogg != now.ogg) lwf_ogg_close(old.ogg);
+    if (old.before_chain && old.before_chain != now.before_chain) {
+        release_unshared(rs, *old.before_chain, Reader());
+        delete old.before_chain;
+    }
+}
+
+// The reader enters the chained stream whose headers it has read: the stream before is given up
+void drop_before_chain(lwf_readers *rs, Reader &r)
+{
+    if (!r.before_chain) return;
+    Reader *b = r.before_chain;
+    r.before_chain = nullptr;
+    release_unshared(rs, *b, r);
+    delete b;
+}
+
+// A read job stopped at a chained stream's ident (`calls` pager reads after the job's start): its headers are read now,
+// which the single reader does at its next call, and the reader as the single reader stands is kept until the drop.
+int read_chained(lwf_readers *rs, Reader &r, const Job &j, size_t calls)
+{
+    Reader before = r;
+    before.before_chain = nullptr;
+    if (!(before.ogg = ogg_clone(j.snap))) return LWB_ERR_BUFFER;
+    lwf_ogg_packet pk;
+    for (size_t k = 0; k < calls; k++) lwf_ogg_next_packet(before.ogg, &pk);
+    Reader *b = new (std::nothrow) Reader(before);
+    int rc = b ? read_headers(rs, r, &j.chain_ident) : LWB_ERR_BUFFER;
+    if (rc) {
+        lwf_ogg_close(before.ogg);
+        delete b;
+        return rc;
+    }
+    r.before_chain = b;
     return LWB_OK;
 }
 
@@ -244,13 +295,14 @@ void commit(lwf_readers *rs, Reader &r, Job &j, const lwf_stream_job &sj, lwf_re
     const size_t f = failed ? sj.packets_done : n;
     const size_t keep = failed && f < n ? j.pkts[f].calls : j.keep_calls;
     if (keep < j.calls) rewind(r, j, keep);
-    if (f > 0) {
-        r.gp = j.pkts[f - 1].gp;
-        r.fresh = false;
-    } else if (j.drop_tried) {
-        r.gp.has = false;
+    if (f > 0) r.gp = j.pkts[f - 1].gp;
+    else if (j.drop_tried) r.gp.has = false;
+    // the state the batch left, read from the stream's host flags: a failing packet may also have cleared it
+    r.fresh = lwb_stream_state_len(r.pwr) == 0;
+    if (j.drop_tried) {
+        r.pending_drop = false;
+        drop_before_chain(rs, r);
     }
-    if (j.drop_tried) r.pending_drop = false;
     out.n_packets = (uint32_t)(f > D ? f - D : 0);
     out.n_samples = sj.n_samples;
     out.channels = r.channels;
@@ -263,7 +315,7 @@ void commit(lwf_readers *rs, Reader &r, Job &j, const lwf_stream_job &sj, lwf_re
     if (j.chained) {
         int rc;
         try {
-            rc = read_headers(rs, r, &j.chain_ident);
+            rc = read_chained(rs, r, j, f ? j.pkts[f - 1].calls : 0);
         } catch (...) {
             rc = LWB_ERR_BUFFER;
         }
@@ -363,11 +415,311 @@ int read(lwf_readers *rs, lwf_read_job *jobs, size_t n_jobs, int out_format, voi
     return LWB_OK;
 }
 
+// Unknown or repeated reader indices among n entries `reader(k)`
+template <class F> bool bad_readers(const lwf_readers *rs, size_t n, F reader)
+{
+    std::vector<char> seen(rs->readers.size(), 0);
+    for (size_t k = 0; k < n; k++) {
+        const uint32_t i = reader(k);
+        if (i >= rs->readers.size() || seen[i]) return true;
+        seen[i] = 1;
+    }
+    return false;
+}
+
+int seek(lwf_readers *rs, const uint32_t *readers, const uint64_t *absgps, size_t n, int32_t *status)
+{
+    if (bad_readers(rs, n, [&](size_t k) { return readers[k]; })) return LWB_ERR_INVALID;
+    rs->retired.reserve(rs->retired.size() + n);       // (release_unshared below cannot fail)
+    // a reader whose headers a read took ahead of the single reader goes back to the stream the single reader stands in
+    for (size_t k = 0; k < n; k++) {
+        Reader &r = *rs->readers[readers[k]];
+        if (!r.before_chain) continue;
+        Reader *b = r.before_chain;
+        Reader now = r;
+        r = *b;
+        delete b;
+        now.before_chain = nullptr;
+        release_unshared(rs, now, r);
+    }
+    std::atomic<size_t> next(0);
+    run_pool(rs->threads, n, [&]() {
+        for (size_t k; (k = next.fetch_add(1)) < n;) {
+            Reader &r = *rs->readers[readers[k]];
+            status[k] = lwfb::pager_seek(r.ogg, r.serial, absgps[k], r.audio_start);
+        }
+    });
+    // cur_absgp = None and a fresh PreviousWindowRight: host flags only (the ctx's state counter is not the pool's to touch)
+    for (size_t k = 0; k < n; k++) {
+        if (status[k]) continue;
+        Reader &r = *rs->readers[readers[k]];
+        r.gp.has = false;
+        r.fresh = true;
+        if (r.pwr) lwb_stream_reset(r.pwr);
+    }
+    return LWB_OK;
+}
+
+// One skip job: the reader as it was, to restore it if the call is refused, and skip_samples_linear's walk over it
+struct Skip {
+    Reader saved;                      // (its resources stay the reader's; those the walk replaced are released at commit)
+    lwf_ogg *snap = nullptr;           // the pager before the walk
+    lwfb::SkipWalk walk;
+    uint64_t to_skip0 = 0;
+    std::vector<uint8_t> last, drop, target, ident;
+    lwf_ogg_packet tpk;                // the target's page facts (its data is `target`)
+    size_t tcount = 0;                 // the target's samples by its header
+    bool found = false;                // the target was read
+    bool has_drop = false;             // the walk dropped the first packet of the chained stream it stands in
+    bool boundary = false;             // the walk stopped at a chained stream's ident: its headers are read next
+    bool ended = false, reset = false;
+    int32_t stop = LWB_OK;             // the error that ended the walk
+    lwfb::StreamFlags flags{false, 0}; // reset: the stream state's flags before it
+    size_t kept = 0, limit = SIZE_MAX; // the samples the target returns, and the window if that cuts it
+    ~Skip() { lwf_ogg_close(snap); }
+};
+
+// The entropy decode of a chained stream's first audio packet, the part of its decode and drop that can fail on the
+// fresh state it is decoded on
+int entropy_check(const lwf_headers *h, const lwf_ogg_packet &pk)
+{
+    lwf_info info;
+    lwf_headers_info(h, &info);
+    const size_t C = info.audio_channels, n2 = (size_t)1 << (info.blocksize_1 - 1);
+    std::vector<uint8_t> kinds(C);
+    std::vector<uint32_t> ys(C * LWB_MAX_POSTS);
+    std::vector<float> dense(C * n2), residue(C * n2);
+    lwf_decoded_packet dp;
+    std::memset(&dp, 0, sizeof(dp));
+    dp.floor_kind = kinds.data();
+    dp.floor1_y = ys.data();
+    dp.dense_floor = dense.data();
+    dp.residue = residue.data();
+    return lwf_packet_decode(h, pk.data, pk.len, &dp);
+}
+
+// skip_samples_linear's walk of one job (inside_ogg.rs:244-283 with read_next_audio_packet, :107-143), on the pool:
+// until the target is read, the stream ends, a packet fails or a chained stream begins (its headers are read between
+// rounds, off the pool, since they change the shared sets; the next round drops its first packet and walks on)
+void skip_walk(const lwf_readers *rs, Reader &r, Skip &s)
+{
+    s.boundary = false;
+    lwf_ogg_packet pk;
+    int rc;
+    auto end = [&](int code) {
+        if (code == LWF_ERR_NO_MORE_PACKETS) s.ended = true;
+        else s.stop = code;
+    };
+    for (;;) {
+        const lwf_headers *H = rs->sets[r.set]->h;
+        if (r.pending_drop) {
+            r.pending_drop = false;
+            r.before_chain = nullptr;          // (released at commit: the walk entered the chained stream)
+            r.gp.has = false;
+            s.has_drop = false;
+            if ((rc = lwf_ogg_next_packet(r.ogg, &pk))) return end(rc);
+            if ((rc = entropy_check(H, pk))) return end(rc);
+            s.drop.assign(pk.data, pk.data + pk.len);
+            s.has_drop = true;
+            r.gp = Granule{true, pk.absgp_page};
+            if ((rc = lwf_ogg_next_packet(r.ogg, &pk))) return end(rc);     // returned whatever its serial
+        } else {
+            if ((rc = lwfb::next_packet_of(r.ogg, r.serial, &pk, nullptr))) return end(rc);
+            if (pk.stream_serial != r.serial) {
+                s.boundary = true;
+                s.ident.assign(pk.data, pk.data + pk.len);
+                return;
+            }
+        }
+        size_t cnt = 0;
+        if ((rc = lwf_decoded_sample_count(H, pk.data, pk.len, &cnt))) return end(rc);
+        if (s.walk.target(r.gp, pk, cnt)) {
+            s.found = true;
+            s.target.assign(pk.data, pk.data + pk.len);
+            s.tpk = pk;
+            s.tpk.data = nullptr;
+            s.tcount = cnt;
+            return;
+        }
+        s.last.assign(pk.data, pk.data + pk.len);
+    }
+}
+
+// Puts reader r back as it was before job s: the stream state's flags, the pager, and the headers and stream state
+// the walk made released (nothing was queued on them)
+void restore_skip(Reader &r, Skip &s)
+{
+    if (s.reset) lwfb::set_stream_flags(r.pwr, s.flags);
+    const Reader now = r;
+    r = s.saved;
+    std::swap(r.ogg, s.snap);
+    if (now.hdr != r.hdr) lwf_headers_destroy(now.hdr);
+    if (now.pwr && now.pwr != r.pwr) lwb_stream_destroy(now.pwr);
+}
+
+// The job's results and reader r's state from the batch's result for its chain
+void commit_skip(lwf_readers *rs, Reader &r, Skip &s, const lwf_stream_job &sj, lwf_skip_job &out)
+{
+    const bool failed = sj.status != LWB_OK;
+    r.fresh = lwb_stream_state_len(r.pwr) == 0;         // as the batch left it, a failing packet's clearing included
+    out.channels = r.channels;
+    out.got_packet = 0;
+    out.n_samples = 0;
+    out.left_to_skip = s.to_skip0;
+    out.status = failed ? sj.status : s.stop;
+    if (!failed && s.found) {
+        r.gp.step(s.tpk, s.kept);
+        out.got_packet = 1;
+        out.n_samples = sj.n_samples;
+        out.left_to_skip = s.walk.to_skip;
+        if (sj.n_samples != s.kept) out.status = LWB_ERR_MISMATCH;
+    } else if (!failed && s.ended) {
+        out.left_to_skip = s.walk.to_skip;
+    }
+    release_unshared(rs, s.saved, r);
+}
+
+int skip(lwf_readers *rs, lwf_skip_job *jobs, size_t n_jobs, int out_format, void *pcm, int pcm_memory, uint64_t *ticket)
+{
+    if (bad_readers(rs, n_jobs, [&](size_t k) { return jobs[k].reader; })) return LWB_ERR_INVALID;
+    for (size_t k = 0; k < n_jobs; k++) {
+        const Reader &r = *rs->readers[jobs[k].reader];
+        if (planar(out_format) && jobs[k].out_stride < most_samples(r, 1)) return LWB_ERR_INVALID;
+        if (jobs[k].out_channels && jobs[k].out_channels < r.channels) return LWB_ERR_INVALID;
+    }
+    std::vector<Skip> S(n_jobs);
+    rs->retired.reserve(rs->retired.size() + 2 * n_jobs);      // (the commits cannot fail)
+    for (size_t k = 0; k < n_jobs; k++) {
+        Reader &r = *rs->readers[jobs[k].reader];
+        if (!(S[k].snap = ogg_clone(r.ogg))) return LWB_ERR_BUFFER;
+        S[k].saved = r;
+        S[k].walk.to_skip = S[k].to_skip0 = jobs[k].to_skip;
+    }
+    // From here a refusal puts every reader back.  The walk, in rounds split at chained streams' headers.
+    auto restore_all = [&]() {
+        for (size_t k = 0; k < n_jobs; k++) restore_skip(*rs->readers[jobs[k].reader], S[k]);
+    };
+    const double p0 = lwfb::now_s();
+    std::vector<size_t> todo(n_jobs);
+    for (size_t k = 0; k < n_jobs; k++) todo[k] = k;
+    int rc = LWB_OK;
+    while (!todo.empty() && !rc) {
+        std::atomic<size_t> next(0);
+        std::atomic<int> pool_failed(0);
+        run_pool(rs->threads, todo.size(), [&]() {
+            try {
+                for (size_t t; (t = next.fetch_add(1)) < todo.size();) skip_walk(rs, *rs->readers[jobs[todo[t]].reader], S[todo[t]]);
+            } catch (...) {
+                pool_failed.store(1);
+            }
+        });
+        if (pool_failed.load()) rc = LWB_ERR_BUFFER;
+        // the chained streams' headers, off the pool.  read_headers changes the reader only once nothing can fail, so
+        // after an allocation failure every reader is put back as the others are
+        std::vector<size_t> again;
+        try {
+            again.reserve(todo.size());
+            for (size_t t = 0; t < todo.size() && !rc; t++) {
+                Skip &s = S[todo[t]];
+                if (!s.boundary) continue;
+                Reader &r = *rs->readers[jobs[todo[t]].reader];
+                const Reader before = r;
+                const int hrc = read_headers(rs, r, &s.ident);
+                if (hrc) {
+                    s.stop = hrc;
+                    continue;
+                }
+                if (before.hdr != s.saved.hdr) lwf_headers_destroy(before.hdr);     // a stream the walk passed through
+                again.push_back(todo[t]);
+            }
+        } catch (...) {
+            rc = LWB_ERR_BUFFER;
+        }
+        todo.swap(again);
+    }
+    const double paging = lwfb::now_s() - p0;
+    // the room of a job whose walk entered a chained stream
+    for (size_t k = 0; k < n_jobs && !rc; k++) {
+        const Reader &r = *rs->readers[jobs[k].reader];
+        if (r.hdr == S[k].saved.hdr) continue;
+        const uint64_t room = jobs[k].out_channels ? jobs[k].out_channels : S[k].saved.channels, most = most_samples(r, 1);
+        if (r.channels > room || (planar(out_format) ? jobs[k].out_stride < most : room * jobs[k].out_stride < r.channels * most))
+            rc = LWB_ERR_INVALID;
+    }
+    for (size_t k = 0; k < n_jobs && !rc; k++) rc = ensure_device(rs, *rs->readers[jobs[k].reader]);
+    if (rc) {
+        restore_all();
+        return rc;
+    }
+    // each job's chain: [packet before, target] on a reset state, [dropped packet, target] on the chained stream's
+    // fresh state, the target alone on the reader's state, or the dropped packet alone
+    std::vector<lwf_stream_job> sj(n_jobs);
+    std::vector<std::vector<const uint8_t *>> ptrs(n_jobs);
+    std::vector<std::vector<size_t>> lens(n_jobs);
+    try {
+        for (size_t k = 0; k < n_jobs; k++) {
+            Skip &s = S[k];
+            const Reader &r = *rs->readers[jobs[k].reader];
+            s.reset = s.found && s.walk.have_last;
+            auto add = [&](const std::vector<uint8_t> &p) {
+                ptrs[k].push_back(p.data());
+                lens[k].push_back(p.size());
+            };
+            if (s.reset) add(s.last);
+            else if (s.has_drop) add(s.drop);
+            if (s.found) {
+                add(s.target);
+                const size_t expect = s.reset || s.has_drop || !r.fresh ? s.tcount : 0;
+                s.kept = r.gp.cut(s.tpk, expect);
+                if (s.kept < expect) s.limit = s.kept;
+            }
+            std::memset(&sj[k], 0, sizeof(sj[k]));
+            sj[k].stream = r.pwr;
+            sj[k].n_packets = (uint32_t)ptrs[k].size();
+            sj[k].packets = ptrs[k].data();
+            sj[k].lengths = lens[k].data();
+            sj[k].out_offset = jobs[k].out_offset;
+            sj[k].out_stride = jobs[k].out_stride;
+        }
+    } catch (...) {
+        restore_all();
+        return LWB_ERR_BUFFER;
+    }
+    for (lwf_stream_job &q : sj) q.packets_done = UINT32_MAX;   // still so after the call: the job's batch was not queued
+    for (size_t k = 0; k < n_jobs; k++) {
+        Reader &r = *rs->readers[jobs[k].reader];
+        if (S[k].reset) {
+            S[k].flags = lwfb::stream_flags(r.pwr);
+            lwb_stream_reset(r.pwr);
+        }
+    }
+    uint64_t t = 0;
+    for (size_t k = 0; k < n_jobs && !rc; k++)
+        if (S[k].limit != SIZE_MAX) rc = lwb_stream_set_window(rs->readers[jobs[k].reader]->pwr, 0, S[k].limit);
+    if (!rc) rc = lwf_batcher_submit(rs->batcher, sj.data(), n_jobs, out_format, pcm, pcm_memory, &t);
+    for (size_t k = 0; k < n_jobs; k++)
+        if (S[k].limit != SIZE_MAX) lwb_stream_set_window(rs->readers[jobs[k].reader]->pwr, 0, UINT64_MAX);
+    for (size_t k = 0; k < n_jobs; k++) {
+        Reader &r = *rs->readers[jobs[k].reader];
+        if (sj[k].packets_done == UINT32_MAX) restore_skip(r, S[k]);
+        else commit_skip(rs, r, S[k], sj[k], jobs[k]);
+    }
+    if (rc) return rc;
+    rs->t_paging = paging;
+    lwf_batcher_last_timing(rs->batcher, &rs->t_entropy, &rs->t_synth);
+    *ticket = t;
+    return LWB_OK;
+}
+
 void destroy_reader(Reader &r)
 {
     if (r.pwr) lwb_stream_destroy(r.pwr);
     if (r.hdr) lwf_headers_destroy(r.hdr);
     lwf_ogg_close(r.ogg);
+    if (r.before_chain) {
+        destroy_reader(*r.before_chain);
+        delete r.before_chain;
+    }
 }
 
 }  // namespace
@@ -446,4 +798,19 @@ extern "C" int lwf_readers_read(lwf_readers *rs, lwf_read_job *jobs, size_t n_jo
         out_format > LWB_OUT_F16_INTERLEAVED)
         return LWB_ERR_INVALID;
     return lwfb::guarded([&] { return read(rs, jobs, n_jobs, out_format, pcm, pcm_memory, ticket); });
+}
+
+extern "C" int lwf_readers_seek_absgp_pg(lwf_readers *rs, const uint32_t *readers, const uint64_t *absgps, size_t n, int32_t *status)
+{
+    if (!rs || !readers || !absgps || !n || !status) return LWB_ERR_INVALID;
+    return lwfb::guarded([&] { return seek(rs, readers, absgps, n, status); });
+}
+
+extern "C" int lwf_readers_skip_samples_linear(lwf_readers *rs, lwf_skip_job *jobs, size_t n_jobs, int out_format, void *pcm,
+                                               int pcm_memory, uint64_t *ticket)
+{
+    if (!rs || !jobs || !n_jobs || !pcm || !ticket || (pcm_memory != LWB_MEM_HOST && pcm_memory != LWB_MEM_DEVICE) || out_format < 0 ||
+        out_format > LWB_OUT_F16_INTERLEAVED)
+        return LWB_ERR_INVALID;
+    return lwfb::guarded([&] { return skip(rs, jobs, n_jobs, out_format, pcm, pcm_memory, ticket); });
 }

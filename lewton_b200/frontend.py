@@ -6,7 +6,7 @@
   OggPacketReader                 ogg::PacketReader as inside_ogg.rs uses it
   OggStreamReader                 inside_ogg.rs:60-227        (read_dec_packet, read_dec_packet_itl, read_dec_packet_generic,
                                                               get_last_absgp)
-  OggStreamReaders                many OggStreamReaders advanced by one batched call (lwf_readers)
+  OggStreamReaders                many OggStreamReaders advanced, sought and skipped by batched calls (lwf_readers)
 
 The entropy decode is CPU work by nature and runs on the host; synthesis goes through the CUDA back
 half (lwb_decode_packet / lwb_decode_chains)."""
@@ -83,6 +83,12 @@ class _ReadJob(C.Structure):
                 ("next_chained", C.c_uint8), ("ended", C.c_uint8), ("reserved", C.c_uint8), ("status", C.c_int32)]
 
 
+class _SkipJob(C.Structure):
+    _fields_ = [("reader", C.c_uint32), ("out_channels", C.c_uint32), ("to_skip", C.c_uint64), ("out_offset", C.c_uint64),
+                ("out_stride", C.c_uint64), ("left_to_skip", C.c_uint64), ("n_samples", C.c_uint32), ("got_packet", C.c_uint8),
+                ("channels", C.c_uint8), ("reserved", C.c_uint8 * 2), ("status", C.c_int32)]
+
+
 _declared = False
 
 
@@ -142,6 +148,8 @@ def lib():
         L.lwf_readers_last_timing.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double)]
         L.lwf_readers_last_timing.restype = None
         L.lwf_readers_read.argtypes = [vp, C.POINTER(_ReadJob), sz, C.c_int, vp, C.c_int, C.POINTER(C.c_uint64)]
+        L.lwf_readers_seek_absgp_pg.argtypes = [vp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64), sz, C.POINTER(C.c_int32)]
+        L.lwf_readers_skip_samples_linear.argtypes = [vp, C.POINTER(_SkipJob), sz, C.c_int, vp, C.c_int, C.POINTER(C.c_uint64)]
         L.lwf_debug_float32_unpack.argtypes = [C.c_uint32]
         L.lwf_debug_float32_unpack.restype = C.c_float
         L.lwf_debug_lookup1_values.argtypes = [C.c_uint32, C.c_uint16]
@@ -607,11 +615,47 @@ class ReadResult:
                 (self.reader, self.n_packets, self.n_samples, self.channels, self.status, self.ended, self.next_chained))
 
 
+class SkipResult:
+    """One job of OggStreamReaders.skip_samples_linear: got_packet (a packet was returned), its n_samples per channel at
+    out_offset (planar: channel c at out_offset + c * out_stride; interleaved: `channels` samples per frame),
+    left_to_skip, the channel count of the stream the reader stands in, and status (LWB_OK or the code the single
+    reader's call returned)."""
+
+    def __init__(self, job):
+        for f, _ in _SkipJob._fields_:
+            if f != "reserved":
+                setattr(self, f, getattr(job, f))
+        self.got_packet = bool(self.got_packet)
+
+    def __repr__(self):
+        return ("SkipResult(reader=%d, got_packet=%s, n_samples=%d, left_to_skip=%d, channels=%d, status=%d)" %
+                (self.reader, self.got_packet, self.n_samples, self.left_to_skip, self.channels, self.status))
+
+
+def _stream_shapes(data):
+    """(channels, blocksize_0, blocksize_1) of every logical stream of Ogg Vorbis bytes whose first page holds a Vorbis
+    ident header, from the beginning-of-stream pages; the walk stops at the first page it cannot parse."""
+    out, at = [], 0
+    while at + 27 <= len(data) and data[at:at + 4] == b"OggS":
+        nseg = data[at + 26]
+        body = at + 27 + nseg
+        end = body + sum(data[at + 27: body])
+        if end > len(data):
+            break
+        first = data[body: body + 30]
+        if data[at + 5] & 2 and len(first) == 30 and first[:7] == b"\x01vorbis":
+            out.append((first[11], first[28] & 15, first[28] >> 4))
+        at = end
+    return out
+
+
 class OggStreamReaders:
     """Many OggStreamReaders on one context (lwf_readers): read() advances any of them by up to max_packets audio packets
     in one call -- de-paging and entropy decode on a host thread pool, synthesis as one batch per channel count and
     blocksize pair on the fused kernels -- and each returns exactly what OggStreamReader.read_dec_packet_generic returns,
-    packet for packet.  Readers whose ident and setup headers are byte-equal share one device setup."""
+    packet for packet.  seek_absgp_pg() and skip_samples_linear() do the single reader's seek and skip for many readers
+    in one call, holding each to what OggStreamReader returns too.  Readers whose ident and setup headers are byte-equal
+    share one device setup."""
 
     def __init__(self, ctx, threads=0):
         self.ctx = ctx
@@ -619,6 +663,7 @@ class OggStreamReaders:
         ctx.check(lib().lwf_readers_create(ctx._h, threads, C.byref(h)))
         self._h = h.value
         self._data = []                          # the bytes of each reader: lwf_readers_add does not copy them
+        self._shapes = []                        # (channels, blocksize_0, blocksize_1) of each file's logical streams
         self._headers = {}
         ctx._children.add(self)
 
@@ -631,6 +676,7 @@ class OggStreamReaders:
             e = read_error(self.ctx, rc)
             raise e if e is not None else AudioReadError(rc)
         self._data.append(data)
+        self._shapes.append(_stream_shapes(data))       # the bytes never change: walked once, for skip_room
         return i.value
 
     def stride(self, index, max_packets):
@@ -719,6 +765,77 @@ class OggStreamReaders:
             elif r.ended:
                 pkts.append(None)
             out.append(pkts)
+        return out
+
+    def seek_absgp_pg(self, indices, absgps):
+        """lwf_readers_seek_absgp_pg: OggStreamReader.seek_absgp_pg(absgps[k]) on reader indices[k], each reader at most
+        once; the pages are walked on the host thread pool and nothing is queued on the GPU.  Returns per reader None, or
+        the exception the single reader would have raised (its position is then unchanged)."""
+        n = len(indices)
+        if not n:
+            return []
+        idx = (C.c_uint32 * n)(*indices)
+        gps = (C.c_uint64 * n)(*[int(g) for g in absgps])
+        st = (C.c_int32 * n)()
+        self.ctx.check(lib().lwf_readers_seek_absgp_pg(self._h, idx, gps, n, st))
+        return [read_error(self.ctx, rc) for rc in st]
+
+    def skip_room(self, index):
+        """(channels, stride): the room a skip job of reader `index` takes -- the most channels of any logical stream of
+        its file, and the planar stride that one packet of any of them needs (blocksize_1 / 2 + (blocksize_1 -
+        blocksize_0) / 4), so that a skip into a chained stream fits too."""
+        h = self.headers(index)
+        shapes = self._shapes[index] + [(h.audio_channels, h.blocksize_0, h.blocksize_1)]
+        return (max(c for c, _, _ in shapes), max((1 << b1) // 2 + ((1 << b1) - (1 << b0)) // 4 for _, b0, b1 in shapes))
+
+    def skip_samples_linear(self, jobs, pcm, stride, sample="f32", interleaved=False):
+        """lwf_readers_skip_samples_linear.  jobs: [(reader index, to_skip)], each reader at most once.  Job j's target
+        packet lands in `pcm` behind the jobs before it, each taking skip_room(index)[0] * stride elements (planar: channel
+        c at offset + c * stride; stride >= skip_room(index)[1] of every job).  pcm as for read().  Returns an api.Ticket
+        whose results ([SkipResult], `results` and what wait() returns) are known at once and its PCM once it is done;
+        paging_seconds (the walk), entropy_seconds and synthesis_seconds describe this call."""
+        fmt, _ = sample_format(sample, interleaved)
+        addr, memory = _pcm_address(pcm)
+        n = len(jobs)
+        arr = (_SkipJob * n)()
+        off = 0
+        for j, (index, to_skip) in enumerate(jobs):
+            room = self.skip_room(index)[0]
+            arr[j].reader, arr[j].to_skip, arr[j].out_channels = index, int(to_skip), room
+            arr[j].out_offset, arr[j].out_stride = off, stride
+            off += room * stride
+        t = C.c_uint64()
+        self.ctx.check(lib().lwf_readers_skip_samples_linear(self._h, arr, n, fmt, addr, memory, C.byref(t)))
+        p, e, s = C.c_double(), C.c_double(), C.c_double()
+        lib().lwf_readers_last_timing(self._h, C.byref(p), C.byref(e), C.byref(s))
+        self.paging_seconds, self.entropy_seconds, self.synthesis_seconds = p.value, e.value, s.value
+        results = [SkipResult(arr[j]) for j in range(n)]
+        ticket = Ticket(self.ctx, t.value, (arr, pcm), lambda: results)
+        ticket.results = results
+        return ticket
+
+    def skip_samples_linear_dec(self, indices, to_skip, sample="f32", interleaved=False):
+        """skip_samples_linear() into page-locked host memory and wait: per reader what OggStreamReader.skip_samples_linear
+        returns -- (packet or None, left_to_skip), the packet planar (a list of per-channel arrays) or interleaved (one
+        array) -- or the exception it would have raised.  to_skip: one count for every reader, or one per reader."""
+        fmt, dt = sample_format(sample, interleaved)
+        if not indices:
+            return []
+        counts = list(to_skip) if hasattr(to_skip, "__len__") else [to_skip] * len(indices)
+        rooms = [self.skip_room(i) for i in indices]
+        stride = max(s for _, s in rooms)
+        pcm = self.ctx.host_alloc(max(1, sum(c for c, _ in rooms) * stride), dt)
+        out = []
+        for r in self.skip_samples_linear(list(zip(indices, counts)), pcm, stride, sample, interleaved).wait():
+            if r.status:
+                out.append(read_error(self.ctx, r.status))
+            elif not r.got_packet:
+                out.append((None, r.left_to_skip))
+            elif interleaved:
+                out.append((pcm[r.out_offset: r.out_offset + r.n_samples * r.channels].copy(), r.left_to_skip))
+            else:
+                out.append(([pcm[r.out_offset + c * stride: r.out_offset + c * stride + r.n_samples].copy()
+                             for c in range(r.channels)], r.left_to_skip))
         return out
 
     def close(self):
