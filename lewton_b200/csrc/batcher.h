@@ -105,10 +105,21 @@ struct lwf_batcher {
 namespace lwfb {
 
 double now_s();
-// The batcher's host thread pool: `worker` on the calling thread and on up to min(threads, n) - 1 more, all joined
-// before it returns.  The workers share the work through a counter of their own; a thread that cannot be started leaves
-// the work to the others.
-void run_pool(int threads, size_t n, const std::function<void()> &worker);
+// The batcher's host thread pool: item(k, w) once for every k in [0, n), on the calling thread (w = 0) and on up to
+// min(threads, n) - 1 more (w = 1, 2, ...: a worker's items run one after another), all joined before it returns.  A
+// thread that cannot be started leaves its items to the others.  An item that throws ends its worker, whose remaining
+// items the others take; the pool then returns LWB_ERR_BUFFER, else LWB_OK.
+int run_pool(int threads, size_t n, const std::function<void(size_t k, int w)> &item);
+// The buffers one audio packet of a stream decodes into, sized from the stream's headers (floor kinds [C], floor-1 posts
+// [C * LWB_MAX_POSTS], dense floor and residue [C * blocksize_1 / 2]), and an lwf_decoded_packet pointing at them
+struct PacketScratch {
+    std::vector<uint8_t> kinds;
+    std::vector<uint32_t> ys;
+    std::vector<float> dense, residue;
+    PacketScratch() = default;
+    explicit PacketScratch(const lwf_headers *h);
+    lwf_decoded_packet packet();
+};
 // An independent copy of a pager's position and buffered packets (nullptr without memory)
 lwf_ogg *ogg_clone(const lwf_ogg *o);
 // Headers with the comments of `comment` (a comment header packet; lwf_headers_parse's errors for it) that share the

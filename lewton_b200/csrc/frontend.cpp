@@ -1708,9 +1708,8 @@ struct lwf_reader {
     uint32_t serial = 0;
     lwfb::Granule gp;
     size_t audio_start = 0;        // byte offset of the first page after the current stream's headers
-    std::vector<uint8_t> kinds;
-    std::vector<uint32_t> ys;
-    std::vector<float> dense, residue, scratch;
+    lwfb::PacketScratch pkt;
+    std::vector<float> dropped;    // the PCM of packets decoded and dropped
 };
 
 static void reader_drop_stream(lwf_reader *r)
@@ -1740,11 +1739,7 @@ static int reader_read_headers(lwf_reader *r, const lwf_ogg_packet *first)
     r->serial = hp.serial;
     r->gp.has = false;
     r->audio_start = lwfb::pager_offset(r->ogg);
-    const size_t C = h->body().ident.audio_channels, n2 = (size_t)1 << (h->body().ident.blocksize_1 - 1);
-    r->kinds.assign(C, 0);
-    r->ys.assign(C * LWB_MAX_POSTS, 0);
-    r->dense.assign(C * n2, 0.f);
-    r->residue.assign(C * n2, 0.f);
+    r->pkt = lwfb::PacketScratch(h);
     return LWB_OK;
 }
 
@@ -1778,12 +1773,7 @@ extern "C" const lwf_headers *lwf_reader_headers(const lwf_reader *r) { return r
 // read_audio_packet_generic through the CUDA back half
 static int reader_decode(lwf_reader *r, const lwf_ogg_packet &pk, int out_format, void *out, size_t cap, size_t *n)
 {
-    lwf_decoded_packet dp;
-    std::memset(&dp, 0, sizeof(dp));
-    dp.floor_kind = r->kinds.data();
-    dp.floor1_y = r->ys.data();
-    dp.dense_floor = r->dense.data();
-    dp.residue = r->residue.data();
+    lwf_decoded_packet dp = r->pkt.packet();
     int rc = lwf_packet_decode(r->hdr, pk.data, pk.len, &dp);
     if (rc) return rc;
     lwb_packet p;
@@ -1798,6 +1788,15 @@ static int reader_decode(lwf_reader *r, const lwf_ogg_packet &pk, int out_format
     return lwb_decode_packet(r->pwr, &p, out_format, out, cap, n);
 }
 
+// Decodes pk on the reader's stream state and drops its PCM
+static int reader_decode_drop(lwf_reader *r, const lwf_ogg_packet &pk)
+{
+    const size_t C = r->hdr->h.ident.audio_channels, n1 = (size_t)1 << r->hdr->h.ident.blocksize_1;
+    r->dropped.resize(C * n1);
+    size_t n = 0;
+    return reader_decode(r, pk, LWB_OUT_F32_PLANAR, r->dropped.data(), n1, &n);
+}
+
 // read_next_audio_packet, inside_ogg.rs:107-143
 static int reader_next_audio_packet(lwf_reader *r, lwf_ogg_packet *pk)
 {
@@ -1806,10 +1805,7 @@ static int reader_next_audio_packet(lwf_reader *r, lwf_ogg_packet *pk)
     // a chained stream begins: new headers, new state; its first audio packet is decoded and dropped
     if ((rc = reader_read_headers(r, pk))) return rc;
     if ((rc = lwf_ogg_next_packet(r->ogg, pk))) return rc;
-    const size_t C = r->hdr->h.ident.audio_channels, n1 = (size_t)1 << r->hdr->h.ident.blocksize_1;
-    r->scratch.resize(C * n1);
-    size_t dropped = 0;
-    if ((rc = reader_decode(r, *pk, LWB_OUT_F32_PLANAR, r->scratch.data(), n1, &dropped))) return rc;
+    if ((rc = reader_decode_drop(r, *pk))) return rc;
     r->gp = lwfb::Granule{true, pk->absgp_page};
     return lwf_ogg_next_packet(r->ogg, pk);
 }
@@ -1866,13 +1862,10 @@ extern "C" int lwf_reader_skip_samples_linear(lwf_reader *r, size_t to_skip, int
             if (walk.target(r->gp, next, cnt)) {                  // :263-271
                 if (walk.have_last) {
                     lwb_stream_reset(r->pwr);
-                    const size_t C = r->hdr->h.ident.audio_channels, n1 = (size_t)1 << r->hdr->h.ident.blocksize_1;
-                    r->scratch.resize(C * n1);
-                    size_t dropped = 0;
                     last_pk.data = last.data();
                     last_pk.len = last.size();
                     // `next.data` points into the pager's current buffer, which stays valid: nothing is read in between
-                    if ((rc = reader_decode(r, last_pk, LWB_OUT_F32_PLANAR, r->scratch.data(), n1, &dropped))) return rc;
+                    if ((rc = reader_decode_drop(r, last_pk))) return rc;
                 }
                 if ((rc = reader_dec_packet(r, next, out_format, out, cap_total, n_samples))) return rc;
                 *got_packet = 1;
@@ -1970,19 +1963,46 @@ double now_s()
     return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
 
-void run_pool(int threads, size_t n, const std::function<void()> &worker)
+int run_pool(int threads, size_t n, const std::function<void(size_t k, int w)> &item)
 {
     const int nt = (int)std::min<size_t>((size_t)std::max(1, threads), std::max<size_t>(1, n));
+    std::atomic<size_t> next(0);
+    std::atomic<bool> failed(false);
+    auto worker = [&](int w) {
+        try {
+            for (size_t k; (k = next.fetch_add(1)) < n;) item(k, w);
+        } catch (...) {
+            failed.store(true);
+        }
+    };
     std::vector<std::thread> pool;
     try {
         pool.reserve((size_t)nt);
-        for (int t = 1; t < nt; t++) pool.emplace_back(worker);
+        for (int t = 1; t < nt; t++) pool.emplace_back(worker, t);
     } catch (...) {
         // no more threads to be had (std::system_error) or no memory for the vector: go on with the workers that did
-        // start -- they share the job counter, so the work is the same -- instead of unwinding past joinable threads
+        // start -- they share the item counter, so the work is the same -- instead of unwinding past joinable threads
     }
-    worker();
+    worker(0);
     for (auto &t : pool) t.join();
+    return failed.load() ? LWB_ERR_BUFFER : LWB_OK;
+}
+
+PacketScratch::PacketScratch(const lwf_headers *h)
+    : kinds(h->body().ident.audio_channels), ys(kinds.size() * LWB_MAX_POSTS),
+      dense(kinds.size() << (h->body().ident.blocksize_1 - 1)), residue(dense.size())
+{
+}
+
+lwf_decoded_packet PacketScratch::packet()
+{
+    lwf_decoded_packet dp;
+    std::memset(&dp, 0, sizeof(dp));
+    dp.floor_kind = kinds.data();
+    dp.floor1_y = ys.data();
+    dp.dense_floor = dense.data();
+    dp.residue = residue.data();
+    return dp;
 }
 
 lwf_ogg *ogg_clone(const lwf_ogg *o)
@@ -2141,74 +2161,65 @@ int batch_entropy(lwf_batcher *b, size_t set, lwf_stream_job *jobs, const size_t
         ar.nexts.resize(pkt_total[g]);
     }
     // pass 2 (parallel over all jobs of the list): entropy decode straight into the arenas of each job's group
-    std::atomic<size_t> next_job(0);
-    std::atomic<int> failed(0);
-    auto worker = [&]() {
-        try {
-            std::vector<lwb_vq_run> scratch_runs;        // LWB_ENTRY_VQ: one packet's records (see below)
-            std::vector<uint16_t> scratch_ents;
-            for (;;) {
-                const size_t i = next_job.fetch_add(1);
-                if (i >= n) break;
-                const size_t j = list[i];
-                const lwf_stream_job &job = jobs[j];
-                const JobPlan &p = plan[j];
-                const lwf::Headers &H = b->sets[p.set].h->body();
-                Group &G = *b->groups[b->sets[p.set].group];
-                BatchArena &ar = G.arena[set];
-                const size_t C = G.channels;
-                float *coeffs = (float *)ar.coeffs.p, *dense = G.has_floor0 ? (float *)ar.dense.p : nullptr;
-                uint8_t *kinds = (uint8_t *)ar.kinds.p;
-                uint32_t *ys = (uint32_t *)ar.ys.p;
-                uint64_t *run_off = vq ? (uint64_t *)ar.vqroff.p : nullptr, *ent_off = vq ? (uint64_t *)ar.vqeoff.p : nullptr;
-                uint64_t coff = p.coeff0;
-                for (uint32_t k = 0; k < p.usable; k++) {
-                    const uint64_t pi = p.pkt0 + k;
-                    lwf_decoded_packet dp;
-                    std::memset(&dp, 0, sizeof(dp));
-                    dp.floor_kind = kinds + pi * C;
-                    dp.floor1_y = ys + pi * C * LWB_MAX_POSTS;
-                    dp.residue = vq ? nullptr : coeffs + coff;
-                    dp.dense_floor = dense ? dense + coff : nullptr;
-                    int rc;
-                    if (vq) {
-                        std::vector<lwb_vq_run> &jr = ar.job_runs[p.slot];
-                        std::vector<uint16_t> &je = ar.job_ents[p.slot];
-                        // decoded into the thread's scratch (a packet of b bytes holds fewer than 8 b codewords), then only
-                        // what it produced is appended (growing the job's vectors to the bound first meant zero-filling
-                        // ~22 KB per 280-byte packet)
-                        const size_t cap = (size_t)job.lengths[k] * 8 + 16;
-                        if (scratch_runs.size() < cap) { scratch_runs.resize(cap); scratch_ents.resize(cap); }
-                        lwf::VqSink sink;
-                        sink.runs = scratch_runs.data();
-                        sink.run_cap = cap;
-                        sink.entries = scratch_ents.data();
-                        sink.ent_cap = cap;
-                        rc = lwf::packet_decode(H, job.packets[k], job.lengths[k], &dp, &sink, b->floor0_records);
-                        if (!rc && sink.overflow) rc = LWB_ERR_BUFFER;
-                        if (!rc) {
-                            jr.insert(jr.end(), scratch_runs.data(), scratch_runs.data() + sink.n_runs);
-                            je.insert(je.end(), scratch_ents.data(), scratch_ents.data() + sink.n_ent);
-                        }
-                        run_off[pi + 1] = rc ? 0 : sink.n_runs;      // counts for now; turned into offsets below
-                        ent_off[pi + 1] = rc ? 0 : sink.n_ent;
-                    } else {
-                        rc = lwf::packet_decode(H, job.packets[k], job.lengths[k], &dp, nullptr, b->floor0_records);
-                    }
-                    if (rc) { dec_status[j] = rc; break; }
-                    ar.modes[pi] = dp.mode_number;
-                    ar.prevs[pi] = dp.prev_window_flag;
-                    ar.nexts[pi] = dp.next_window_flag;
-                    coff += (uint64_t)C * (dp.n / 2);
-                    decoded[j]++;
+    std::vector<std::vector<lwb_vq_run>> scratch_runs(vq ? b->threads : 0);    // LWB_ENTRY_VQ: one packet's records
+    std::vector<std::vector<uint16_t>> scratch_ents(scratch_runs.size());       // (see below), per worker
+    auto decode = [&](size_t i, int w) {
+        const size_t j = list[i];
+        const lwf_stream_job &job = jobs[j];
+        const JobPlan &p = plan[j];
+        const lwf::Headers &H = b->sets[p.set].h->body();
+        Group &G = *b->groups[b->sets[p.set].group];
+        BatchArena &ar = G.arena[set];
+        const size_t C = G.channels;
+        float *coeffs = (float *)ar.coeffs.p, *dense = G.has_floor0 ? (float *)ar.dense.p : nullptr;
+        uint8_t *kinds = (uint8_t *)ar.kinds.p;
+        uint32_t *ys = (uint32_t *)ar.ys.p;
+        uint64_t *run_off = vq ? (uint64_t *)ar.vqroff.p : nullptr, *ent_off = vq ? (uint64_t *)ar.vqeoff.p : nullptr;
+        uint64_t coff = p.coeff0;
+        for (uint32_t k = 0; k < p.usable; k++) {
+            const uint64_t pi = p.pkt0 + k;
+            lwf_decoded_packet dp;
+            std::memset(&dp, 0, sizeof(dp));
+            dp.floor_kind = kinds + pi * C;
+            dp.floor1_y = ys + pi * C * LWB_MAX_POSTS;
+            dp.residue = vq ? nullptr : coeffs + coff;
+            dp.dense_floor = dense ? dense + coff : nullptr;
+            int rc;
+            if (vq) {
+                std::vector<lwb_vq_run> &jr = ar.job_runs[p.slot];
+                std::vector<uint16_t> &je = ar.job_ents[p.slot];
+                std::vector<lwb_vq_run> &runs = scratch_runs[w];
+                std::vector<uint16_t> &ents = scratch_ents[w];
+                // decoded into the worker's scratch (a packet of b bytes holds fewer than 8 b codewords), then only what
+                // it produced is appended (growing the job's vectors to the bound first meant zero-filling ~22 KB per
+                // 280-byte packet)
+                const size_t cap = (size_t)job.lengths[k] * 8 + 16;
+                if (runs.size() < cap) { runs.resize(cap); ents.resize(cap); }
+                lwf::VqSink sink;
+                sink.runs = runs.data();
+                sink.run_cap = cap;
+                sink.entries = ents.data();
+                sink.ent_cap = cap;
+                rc = lwf::packet_decode(H, job.packets[k], job.lengths[k], &dp, &sink, b->floor0_records);
+                if (!rc && sink.overflow) rc = LWB_ERR_BUFFER;
+                if (!rc) {
+                    jr.insert(jr.end(), runs.data(), runs.data() + sink.n_runs);
+                    je.insert(je.end(), ents.data(), ents.data() + sink.n_ent);
                 }
+                run_off[pi + 1] = rc ? 0 : sink.n_runs;      // counts for now; turned into offsets below
+                ent_off[pi + 1] = rc ? 0 : sink.n_ent;
+            } else {
+                rc = lwf::packet_decode(H, job.packets[k], job.lengths[k], &dp, nullptr, b->floor0_records);
             }
-        } catch (...) {
-            failed.store(1);
+            if (rc) { dec_status[j] = rc; break; }
+            ar.modes[pi] = dp.mode_number;
+            ar.prevs[pi] = dp.prev_window_flag;
+            ar.nexts[pi] = dp.next_window_flag;
+            coff += (uint64_t)C * (dp.n / 2);
+            decoded[j]++;
         }
     };
-    run_pool(b->threads, n, worker);
-    if (failed.load()) return LWB_ERR_BUFFER;
+    if (const int rc = run_pool(b->threads, n, decode)) return rc;
     if (vq) {
         // counts -> offsets (rows of packets that were not decoded own nothing), then one packed copy of each array
         for (size_t g : *used) {
@@ -2227,20 +2238,15 @@ int batch_entropy(lwf_batcher *b, size_t set, lwf_stream_job *jobs, const size_t
         }
         // ~3 KB per stereo long packet: copied by the pool as well (one thread alone would take about as long over it as
         // the whole pool over the entropy decode)
-        std::atomic<size_t> next_copy(0);
-        auto copier = [&]() {
-            for (;;) {
-                const size_t i = next_copy.fetch_add(1);
-                if (i >= n) return;
-                const JobPlan &p = plan[list[i]];
-                BatchArena &ar = b->groups[b->sets[p.set].group]->arena[set];
-                const std::vector<lwb_vq_run> &jr = ar.job_runs[p.slot];
-                const std::vector<uint16_t> &je = ar.job_ents[p.slot];
-                if (!jr.empty()) std::memcpy((lwb_vq_run *)ar.vqrun.p + ((uint64_t *)ar.vqroff.p)[p.pkt0], jr.data(), jr.size() * sizeof(lwb_vq_run));
-                if (!je.empty()) std::memcpy((uint16_t *)ar.vqent.p + ((uint64_t *)ar.vqeoff.p)[p.pkt0], je.data(), je.size() * sizeof(uint16_t));
-            }
+        auto copy = [&](size_t i, int) {
+            const JobPlan &p = plan[list[i]];
+            BatchArena &ar = b->groups[b->sets[p.set].group]->arena[set];
+            const std::vector<lwb_vq_run> &jr = ar.job_runs[p.slot];
+            const std::vector<uint16_t> &je = ar.job_ents[p.slot];
+            if (!jr.empty()) std::memcpy((lwb_vq_run *)ar.vqrun.p + ((uint64_t *)ar.vqroff.p)[p.pkt0], jr.data(), jr.size() * sizeof(lwb_vq_run));
+            if (!je.empty()) std::memcpy((uint16_t *)ar.vqent.p + ((uint64_t *)ar.vqeoff.p)[p.pkt0], je.data(), je.size() * sizeof(uint16_t));
         };
-        run_pool(b->threads, n, copier);
+        if (const int rc = run_pool(b->threads, n, copy)) return rc;
     }
     for (size_t g : *used) {
         BatchArena &ar = b->groups[g]->arena[set];
@@ -2382,10 +2388,7 @@ extern "C" double lwf_debug_decode_loop(const lwf_headers *h, const uint8_t *con
 {
     if (!h || !packets || !lens) return -1.0;
     try {
-        const size_t C = h->body().ident.audio_channels, n2 = (size_t)1 << (h->body().ident.blocksize_1 - 1);
-        std::vector<uint8_t> kinds(C);
-        std::vector<uint32_t> ys(C * LWB_MAX_POSTS);
-        std::vector<float> dense(C * n2), res(C * n2);
+        lwfb::PacketScratch s(h);
         size_t cap = 16;
         for (size_t i = 0; i < n; i++) cap = std::max(cap, lens[i] * 8 + 16);
         std::vector<lwb_vq_run> runs(cap);
@@ -2393,12 +2396,8 @@ extern "C" double lwf_debug_decode_loop(const lwf_headers *h, const uint8_t *con
         const auto t0 = std::chrono::steady_clock::now();
         for (int r = 0; r < reps; r++)
             for (size_t i = 0; i < n; i++) {
-                lwf_decoded_packet dp;
-                std::memset(&dp, 0, sizeof(dp));
-                dp.floor_kind = kinds.data();
-                dp.floor1_y = ys.data();
-                dp.dense_floor = dense.data();
-                dp.residue = vq ? nullptr : res.data();
+                lwf_decoded_packet dp = s.packet();
+                if (vq) dp.residue = nullptr;
                 lwf::VqSink sink;
                 sink.runs = runs.data(); sink.run_cap = cap; sink.entries = ents.data(); sink.ent_cap = cap;
                 if (lwf::packet_decode(h->body(), packets[i], lens[i], &dp, vq ? &sink : nullptr)) return -2.0;

@@ -1,15 +1,15 @@
 // readers.cpp -- lwf_readers (include/lewton_frontend.h): many OggStreamReaders advanced by one call.  Each reader keeps
 // what lwf_reader keeps on the host (pager, serial, granule position, where its stream's audio starts) and its own stream
-// state; a read de-pages and counts each job's packets on the batcher's thread pool, then hands the packets to an
-// internal lwf_batcher's submit, so that their entropy decode and synthesis are exactly lwf_batcher_submit's.  A skip
-// walks the packets by their sample counts on the pool and submits each job's target the same way; a seek walks pages on
-// the pool and touches host state only.  The header walk, the serial filter, the granule position and skip rules are the
-// single reader's own (batcher.h); what is this file's is applying them ahead of the batch, per job, and committing the
-// reader state of the packets the batch ran.  A fresh stream state (first stream, chained stream, after a seek) makes
+// state.  A read de-pages and counts each job's packets on the batcher's thread pool; a skip walks the packets by their
+// sample counts on the pool.  Both then run one batch step (submit_step): each job becomes one chain of an internal
+// lwf_batcher's submit, so that its entropy decode and synthesis are exactly lwf_batcher_submit's, and each reader is
+// committed from its chain's result or, if the chain was not queued, put back as it was.  A seek walks pages on the pool
+// and touches host state only.  The header walk, the serial filter, the granule position and skip rules are the single
+// reader's own (batcher.h); what is this file's is applying them ahead of the batch, per job, and committing the reader
+// state of the packets the batch ran.  A fresh stream state (first stream, chained stream, after a seek) makes
 // its first packet return 0 samples, a chained stream's first audio packet is decoded and dropped, and the cut of a
 // stream's last packet is made by the stream's output window.
 #include <algorithm>
-#include <atomic>
 #include <cstring>
 #include <new>
 #include <thread>
@@ -340,80 +340,8 @@ uint64_t most_samples(const Reader &r, uint32_t n)
     return n ? n * (n1 / 2) + (n1 - n0) / 4 : 0;
 }
 
-int read(lwf_readers *rs, lwf_read_job *jobs, size_t n_jobs, int out_format, void *pcm, int pcm_memory, uint64_t *ticket)
-{
-    std::vector<char> seen(rs->readers.size(), 0);
-    for (size_t k = 0; k < n_jobs; k++) {
-        const lwf_read_job &q = jobs[k];
-        if (q.reader >= rs->readers.size() || seen[q.reader]) return LWB_ERR_INVALID;
-        seen[q.reader] = 1;
-        const Reader &r = *rs->readers[q.reader];
-        if (planar(out_format) && q.out_stride < most_samples(r, q.max_packets)) return LWB_ERR_INVALID;
-    }
-    int rc;
-    for (size_t k = 0; k < n_jobs; k++)
-        if ((rc = ensure_device(rs, *rs->readers[jobs[k].reader]))) return rc;
-    std::vector<Job> J(n_jobs);
-    for (size_t k = 0; k < n_jobs; k++)
-        if (!(J[k].snap = ogg_clone(rs->readers[jobs[k].reader]->ogg))) return LWB_ERR_BUFFER;
-    // the readers' de-paging and sample counting on the pool
-    const double p0 = lwfb::now_s();
-    std::atomic<size_t> next_job(0);
-    std::atomic<int> pool_failed(0);
-    run_pool(rs->threads, n_jobs, [&]() {
-        try {
-            for (size_t k; (k = next_job.fetch_add(1)) < n_jobs;) depage(rs, *rs->readers[jobs[k].reader], jobs[k].max_packets, J[k]);
-        } catch (...) {
-            pool_failed.store(1);
-        }
-    });
-    const double paging = lwfb::now_s() - p0;
-    std::vector<lwf_stream_job> sj(n_jobs);
-    for (lwf_stream_job &q : sj) q.packets_done = UINT32_MAX;   // still so after the call: the job's batch was not queued
-    std::vector<std::vector<const uint8_t *>> ptrs(n_jobs);
-    std::vector<std::vector<size_t>> lens(n_jobs);
-    rc = pool_failed.load() ? LWB_ERR_BUFFER : LWB_OK;
-    uint64_t t = 0;
-    if (!rc) {
-        try {
-            for (size_t k = 0; k < n_jobs; k++) {
-                const Job &j = J[k];
-                for (const Pkt &p : j.pkts) {
-                    ptrs[k].push_back(j.bytes.data() + p.off);
-                    lens[k].push_back(p.len);
-                }
-                std::memset(&sj[k], 0, sizeof(sj[k]));
-                sj[k].stream = rs->readers[jobs[k].reader]->pwr;
-                sj[k].n_packets = (uint32_t)j.pkts.size();
-                sj[k].packets = ptrs[k].data();
-                sj[k].lengths = lens[k].data();
-                sj[k].out_offset = jobs[k].out_offset;
-                sj[k].out_stride = jobs[k].out_stride;
-                sj[k].packets_done = UINT32_MAX;
-            }
-        } catch (...) {
-            rc = LWB_ERR_BUFFER;
-        }
-    }
-    if (!rc) {
-        // end-of-stream truncation: the job's last packet is cut by its stream's window, for this batch only
-        for (size_t k = 0; k < n_jobs && !rc; k++)
-            if (J[k].limit != SIZE_MAX) rc = lwb_stream_set_window(rs->readers[jobs[k].reader]->pwr, 0, J[k].limit);
-        if (!rc) rc = lwf_batcher_submit(rs->batcher, sj.data(), n_jobs, out_format, pcm, pcm_memory, &t);
-        for (size_t k = 0; k < n_jobs; k++)
-            if (J[k].limit != SIZE_MAX) lwb_stream_set_window(rs->readers[jobs[k].reader]->pwr, 0, UINT64_MAX);
-    }
-    for (size_t k = 0; k < n_jobs; k++) {
-        Reader &r = *rs->readers[jobs[k].reader];
-        if (sj[k].packets_done == UINT32_MAX) std::swap(r.ogg, J[k].snap);     // not queued: the pager as it was
-        else commit(rs, r, J[k], sj[k], jobs[k]);
-    }
-    if (rc) return rc;
-    rs->t_paging = paging;
-    lwf_batcher_last_timing(rs->batcher, &rs->t_entropy, &rs->t_synth);
-    *ticket = t;
-    return LWB_OK;
-}
+// A planar out_stride too short for n packets of reader r's stream
+bool short_stride(int fmt, uint64_t stride, const Reader &r, uint32_t n) { return planar(fmt) && stride < most_samples(r, n); }
 
 // Unknown or repeated reader indices among n entries `reader(k)`
 template <class F> bool bad_readers(const lwf_readers *rs, size_t n, F reader)
@@ -425,6 +353,116 @@ template <class F> bool bad_readers(const lwf_readers *rs, size_t n, F reader)
         seen[i] = 1;
     }
     return false;
+}
+
+// ensure_device for the readers `reader(k)` of n jobs
+template <class F> int ensure_devices(lwf_readers *rs, size_t n, F reader)
+{
+    int rc = LWB_OK;
+    for (size_t k = 0; k < n && !rc; k++) rc = ensure_device(rs, *rs->readers[reader(k)]);
+    return rc;
+}
+
+// One job's chain in a batch step
+struct StepJob {
+    Reader *r = nullptr;               // whose stream state runs the chain
+    std::vector<const uint8_t *> packets;
+    std::vector<size_t> lengths;
+    uint64_t out_offset = 0, out_stride = 0;
+    size_t limit = SIZE_MAX;           // the samples the job may write, if its stream's window cuts its last packet
+    bool reset = false;                // the chain runs on a reset stream state
+    lwfb::StreamFlags flags{false, 0}; // reset: the stream state's flags before it
+};
+
+// The batch step of a read or a skip, after its pass on the pool.  `chain(k, c)` gives job k's chain c, whose packet
+// bytes the caller keeps; each chain is one job of the internal batcher's lwf_batcher_submit.  A chain on a reset state
+// has its stream reset first, and a chain with a limit has its stream's output window set for this submit only.  Then
+// settle(k, sj) runs for every job, with its result if it was queued and NULL if not: a job not queued has had its
+// stream's flags put back, and the caller puts its reader back.  `rc` is an error already met: nothing is submitted.
+// The chains are all made before any stream is reset, so a failure to make one leaves every stream as it was.
+template <class Chain, class Settle>
+int submit_step(lwf_readers *rs, size_t n, int rc, double paging, int out_format, void *pcm, int pcm_memory, uint64_t *ticket,
+                Chain chain, Settle settle)
+{
+    std::vector<StepJob> c;
+    std::vector<lwf_stream_job> sj;
+    bool built = false;
+    if (!rc) {
+        try {
+            c.resize(n);
+            sj.resize(n);
+            for (size_t k = 0; k < n; k++) {
+                chain(k, c[k]);
+                std::memset(&sj[k], 0, sizeof(sj[k]));
+                sj[k].stream = c[k].r->pwr;
+                sj[k].n_packets = (uint32_t)c[k].packets.size();
+                sj[k].packets = c[k].packets.data();
+                sj[k].lengths = c[k].lengths.data();
+                sj[k].out_offset = c[k].out_offset;
+                sj[k].out_stride = c[k].out_stride;
+                sj[k].packets_done = UINT32_MAX;       // still so after the call: the job's batch was not queued
+            }
+            built = true;
+        } catch (...) {
+            rc = LWB_ERR_BUFFER;
+        }
+    }
+    uint64_t t = 0;
+    if (built) {
+        for (size_t k = 0; k < n; k++)
+            if (c[k].reset) {
+                c[k].flags = lwfb::stream_flags(c[k].r->pwr);
+                lwb_stream_reset(c[k].r->pwr);
+            }
+        for (size_t k = 0; k < n && !rc; k++)
+            if (c[k].limit != SIZE_MAX) rc = lwb_stream_set_window(c[k].r->pwr, 0, c[k].limit);
+        if (!rc) rc = lwf_batcher_submit(rs->batcher, sj.data(), n, out_format, pcm, pcm_memory, &t);
+        for (size_t k = 0; k < n; k++)
+            if (c[k].limit != SIZE_MAX) lwb_stream_set_window(c[k].r->pwr, 0, UINT64_MAX);
+    }
+    for (size_t k = 0; k < n; k++) {
+        const bool queued = built && sj[k].packets_done != UINT32_MAX;
+        if (built && !queued && c[k].reset) lwfb::set_stream_flags(c[k].r->pwr, c[k].flags);
+        settle(k, queued ? &sj[k] : nullptr);
+    }
+    if (rc) return rc;
+    rs->t_paging = paging;
+    lwf_batcher_last_timing(rs->batcher, &rs->t_entropy, &rs->t_synth);
+    *ticket = t;
+    return LWB_OK;
+}
+
+int read(lwf_readers *rs, lwf_read_job *jobs, size_t n_jobs, int out_format, void *pcm, int pcm_memory, uint64_t *ticket)
+{
+    auto reader = [&](size_t k) { return jobs[k].reader; };
+    if (bad_readers(rs, n_jobs, reader)) return LWB_ERR_INVALID;
+    for (size_t k = 0; k < n_jobs; k++)
+        if (short_stride(out_format, jobs[k].out_stride, *rs->readers[jobs[k].reader], jobs[k].max_packets)) return LWB_ERR_INVALID;
+    int rc = ensure_devices(rs, n_jobs, reader);
+    if (rc) return rc;
+    std::vector<Job> J(n_jobs);
+    for (size_t k = 0; k < n_jobs; k++)
+        if (!(J[k].snap = ogg_clone(rs->readers[jobs[k].reader]->ogg))) return LWB_ERR_BUFFER;
+    // the readers' de-paging and sample counting on the pool
+    const double p0 = lwfb::now_s();
+    rc = run_pool(rs->threads, n_jobs, [&](size_t k, int) { depage(rs, *rs->readers[jobs[k].reader], jobs[k].max_packets, J[k]); });
+    const double paging = lwfb::now_s() - p0;
+    auto chain = [&](size_t k, StepJob &c) {
+        const Job &j = J[k];
+        c.r = rs->readers[jobs[k].reader].get();
+        for (const Pkt &p : j.pkts) {
+            c.packets.push_back(j.bytes.data() + p.off);
+            c.lengths.push_back(p.len);
+        }
+        c.out_offset = jobs[k].out_offset;
+        c.out_stride = jobs[k].out_stride;
+        c.limit = j.limit;              // end-of-stream truncation: the job's last packet is cut by its stream's window
+    };
+    return submit_step(rs, n_jobs, rc, paging, out_format, pcm, pcm_memory, ticket, chain, [&](size_t k, const lwf_stream_job *sj) {
+        Reader &r = *rs->readers[jobs[k].reader];
+        if (sj) commit(rs, r, J[k], *sj, jobs[k]);
+        else std::swap(r.ogg, J[k].snap);                 // the pager as it was
+    });
 }
 
 int seek(lwf_readers *rs, const uint32_t *readers, const uint64_t *absgps, size_t n, int32_t *status)
@@ -442,13 +480,11 @@ int seek(lwf_readers *rs, const uint32_t *readers, const uint64_t *absgps, size_
         now.before_chain = nullptr;
         release_unshared(rs, now, r);
     }
-    std::atomic<size_t> next(0);
-    run_pool(rs->threads, n, [&]() {
-        for (size_t k; (k = next.fetch_add(1)) < n;) {
-            Reader &r = *rs->readers[readers[k]];
-            status[k] = lwfb::pager_seek(r.ogg, r.serial, absgps[k], r.audio_start);
-        }
+    const int rc = run_pool(rs->threads, n, [&](size_t k, int) {
+        Reader &r = *rs->readers[readers[k]];
+        status[k] = lwfb::pager_seek(r.ogg, r.serial, absgps[k], r.audio_start);
     });
+    if (rc) return rc;
     // cur_absgp = None and a fresh PreviousWindowRight: host flags only (the ctx's state counter is not the pool's to touch)
     for (size_t k = 0; k < n; k++) {
         if (status[k]) continue;
@@ -472,10 +508,9 @@ struct Skip {
     bool found = false;                // the target was read
     bool has_drop = false;             // the walk dropped the first packet of the chained stream it stands in
     bool boundary = false;             // the walk stopped at a chained stream's ident: its headers are read next
-    bool ended = false, reset = false;
+    bool ended = false;
     int32_t stop = LWB_OK;             // the error that ended the walk
-    lwfb::StreamFlags flags{false, 0}; // reset: the stream state's flags before it
-    size_t kept = 0, limit = SIZE_MAX; // the samples the target returns, and the window if that cuts it
+    size_t kept = 0;                   // the samples the target returns
     ~Skip() { lwf_ogg_close(snap); }
 };
 
@@ -483,18 +518,8 @@ struct Skip {
 // fresh state it is decoded on
 int entropy_check(const lwf_headers *h, const lwf_ogg_packet &pk)
 {
-    lwf_info info;
-    lwf_headers_info(h, &info);
-    const size_t C = info.audio_channels, n2 = (size_t)1 << (info.blocksize_1 - 1);
-    std::vector<uint8_t> kinds(C);
-    std::vector<uint32_t> ys(C * LWB_MAX_POSTS);
-    std::vector<float> dense(C * n2), residue(C * n2);
-    lwf_decoded_packet dp;
-    std::memset(&dp, 0, sizeof(dp));
-    dp.floor_kind = kinds.data();
-    dp.floor1_y = ys.data();
-    dp.dense_floor = dense.data();
-    dp.residue = residue.data();
+    lwfb::PacketScratch scratch(h);
+    lwf_decoded_packet dp = scratch.packet();
     return lwf_packet_decode(h, pk.data, pk.len, &dp);
 }
 
@@ -545,11 +570,10 @@ void skip_walk(const lwf_readers *rs, Reader &r, Skip &s)
     }
 }
 
-// Puts reader r back as it was before job s: the stream state's flags, the pager, and the headers and stream state
-// the walk made released (nothing was queued on them)
+// Puts reader r back as it was before job s: the pager, and the headers and stream state the walk made released
+// (nothing was queued on them)
 void restore_skip(Reader &r, Skip &s)
 {
-    if (s.reset) lwfb::set_stream_flags(r.pwr, s.flags);
     const Reader now = r;
     r = s.saved;
     std::swap(r.ogg, s.snap);
@@ -581,10 +605,11 @@ void commit_skip(lwf_readers *rs, Reader &r, Skip &s, const lwf_stream_job &sj, 
 
 int skip(lwf_readers *rs, lwf_skip_job *jobs, size_t n_jobs, int out_format, void *pcm, int pcm_memory, uint64_t *ticket)
 {
-    if (bad_readers(rs, n_jobs, [&](size_t k) { return jobs[k].reader; })) return LWB_ERR_INVALID;
+    auto reader = [&](size_t k) { return jobs[k].reader; };
+    if (bad_readers(rs, n_jobs, reader)) return LWB_ERR_INVALID;
     for (size_t k = 0; k < n_jobs; k++) {
         const Reader &r = *rs->readers[jobs[k].reader];
-        if (planar(out_format) && jobs[k].out_stride < most_samples(r, 1)) return LWB_ERR_INVALID;
+        if (short_stride(out_format, jobs[k].out_stride, r, 1)) return LWB_ERR_INVALID;
         if (jobs[k].out_channels && jobs[k].out_channels < r.channels) return LWB_ERR_INVALID;
     }
     std::vector<Skip> S(n_jobs);
@@ -596,24 +621,12 @@ int skip(lwf_readers *rs, lwf_skip_job *jobs, size_t n_jobs, int out_format, voi
         S[k].walk.to_skip = S[k].to_skip0 = jobs[k].to_skip;
     }
     // From here a refusal puts every reader back.  The walk, in rounds split at chained streams' headers.
-    auto restore_all = [&]() {
-        for (size_t k = 0; k < n_jobs; k++) restore_skip(*rs->readers[jobs[k].reader], S[k]);
-    };
     const double p0 = lwfb::now_s();
     std::vector<size_t> todo(n_jobs);
     for (size_t k = 0; k < n_jobs; k++) todo[k] = k;
     int rc = LWB_OK;
     while (!todo.empty() && !rc) {
-        std::atomic<size_t> next(0);
-        std::atomic<int> pool_failed(0);
-        run_pool(rs->threads, todo.size(), [&]() {
-            try {
-                for (size_t t; (t = next.fetch_add(1)) < todo.size();) skip_walk(rs, *rs->readers[jobs[todo[t]].reader], S[todo[t]]);
-            } catch (...) {
-                pool_failed.store(1);
-            }
-        });
-        if (pool_failed.load()) rc = LWB_ERR_BUFFER;
+        rc = run_pool(rs->threads, todo.size(), [&](size_t t, int) { skip_walk(rs, *rs->readers[jobs[todo[t]].reader], S[todo[t]]); });
         // the chained streams' headers, off the pool.  read_headers changes the reader only once nothing can fail, so
         // after an allocation failure every reader is put back as the others are
         std::vector<size_t> again;
@@ -646,69 +659,33 @@ int skip(lwf_readers *rs, lwf_skip_job *jobs, size_t n_jobs, int out_format, voi
         if (r.channels > room || (planar(out_format) ? jobs[k].out_stride < most : room * jobs[k].out_stride < r.channels * most))
             rc = LWB_ERR_INVALID;
     }
-    for (size_t k = 0; k < n_jobs && !rc; k++) rc = ensure_device(rs, *rs->readers[jobs[k].reader]);
-    if (rc) {
-        restore_all();
-        return rc;
-    }
+    if (!rc) rc = ensure_devices(rs, n_jobs, reader);
     // each job's chain: [packet before, target] on a reset state, [dropped packet, target] on the chained stream's
     // fresh state, the target alone on the reader's state, or the dropped packet alone
-    std::vector<lwf_stream_job> sj(n_jobs);
-    std::vector<std::vector<const uint8_t *>> ptrs(n_jobs);
-    std::vector<std::vector<size_t>> lens(n_jobs);
-    try {
-        for (size_t k = 0; k < n_jobs; k++) {
-            Skip &s = S[k];
-            const Reader &r = *rs->readers[jobs[k].reader];
-            s.reset = s.found && s.walk.have_last;
-            auto add = [&](const std::vector<uint8_t> &p) {
-                ptrs[k].push_back(p.data());
-                lens[k].push_back(p.size());
-            };
-            if (s.reset) add(s.last);
-            else if (s.has_drop) add(s.drop);
-            if (s.found) {
-                add(s.target);
-                const size_t expect = s.reset || s.has_drop || !r.fresh ? s.tcount : 0;
-                s.kept = r.gp.cut(s.tpk, expect);
-                if (s.kept < expect) s.limit = s.kept;
-            }
-            std::memset(&sj[k], 0, sizeof(sj[k]));
-            sj[k].stream = r.pwr;
-            sj[k].n_packets = (uint32_t)ptrs[k].size();
-            sj[k].packets = ptrs[k].data();
-            sj[k].lengths = lens[k].data();
-            sj[k].out_offset = jobs[k].out_offset;
-            sj[k].out_stride = jobs[k].out_stride;
+    auto chain = [&](size_t k, StepJob &c) {
+        Skip &s = S[k];
+        c.r = rs->readers[jobs[k].reader].get();
+        c.reset = s.found && s.walk.have_last;
+        auto add = [&](const std::vector<uint8_t> &p) {
+            c.packets.push_back(p.data());
+            c.lengths.push_back(p.size());
+        };
+        if (c.reset) add(s.last);
+        else if (s.has_drop) add(s.drop);
+        if (s.found) {
+            add(s.target);
+            const size_t expect = c.reset || s.has_drop || !c.r->fresh ? s.tcount : 0;
+            s.kept = c.r->gp.cut(s.tpk, expect);
+            if (s.kept < expect) c.limit = s.kept;
         }
-    } catch (...) {
-        restore_all();
-        return LWB_ERR_BUFFER;
-    }
-    for (lwf_stream_job &q : sj) q.packets_done = UINT32_MAX;   // still so after the call: the job's batch was not queued
-    for (size_t k = 0; k < n_jobs; k++) {
+        c.out_offset = jobs[k].out_offset;
+        c.out_stride = jobs[k].out_stride;
+    };
+    return submit_step(rs, n_jobs, rc, paging, out_format, pcm, pcm_memory, ticket, chain, [&](size_t k, const lwf_stream_job *sj) {
         Reader &r = *rs->readers[jobs[k].reader];
-        if (S[k].reset) {
-            S[k].flags = lwfb::stream_flags(r.pwr);
-            lwb_stream_reset(r.pwr);
-        }
-    }
-    uint64_t t = 0;
-    for (size_t k = 0; k < n_jobs && !rc; k++)
-        if (S[k].limit != SIZE_MAX) rc = lwb_stream_set_window(rs->readers[jobs[k].reader]->pwr, 0, S[k].limit);
-    if (!rc) rc = lwf_batcher_submit(rs->batcher, sj.data(), n_jobs, out_format, pcm, pcm_memory, &t);
-    for (size_t k = 0; k < n_jobs; k++)
-        if (S[k].limit != SIZE_MAX) lwb_stream_set_window(rs->readers[jobs[k].reader]->pwr, 0, UINT64_MAX);
-    for (size_t k = 0; k < n_jobs; k++) {
-        Reader &r = *rs->readers[jobs[k].reader];
-        if (sj[k].packets_done == UINT32_MAX) restore_skip(r, S[k]);
-        else commit_skip(rs, r, S[k], sj[k], jobs[k]);
-    }
-    if (rc) return rc;
-    rs->t_paging = paging;
-    lwf_batcher_last_timing(rs->batcher, &rs->t_entropy, &rs->t_synth);
-    *ticket = t;
-    return LWB_OK;
+        if (sj) commit_skip(rs, r, S[k], *sj, jobs[k]);
+        else restore_skip(r, S[k]);
+    });
 }
 
 void destroy_reader(Reader &r)

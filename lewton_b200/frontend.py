@@ -632,6 +632,14 @@ class SkipResult:
                 (self.reader, self.got_packet, self.n_samples, self.left_to_skip, self.channels, self.status))
 
 
+def _packet_pcm(pcm, offset, stride, channels, s0, n, interleaved):
+    """A copy of samples [s0, s0 + n) of the job PCM at `offset` in `pcm`, in the form OggStreamReader returns a
+    packet: one interleaved array, or a list of per-channel arrays (planes `stride` apart)"""
+    if interleaved:
+        return pcm[offset + s0 * channels: offset + (s0 + n) * channels].copy()
+    return [pcm[offset + c * stride + s0: offset + c * stride + s0 + n].copy() for c in range(channels)]
+
+
 def _stream_shapes(data):
     """(channels, blocksize_0, blocksize_1) of every logical stream of Ogg Vorbis bytes whose first page holds a Vorbis
     ident header, from the beginning-of-stream pages; the walk stops at the first page it cannot parse."""
@@ -707,6 +715,19 @@ class OggStreamReaders:
         """Distinct (ident, setup) header pairs among the streams opened: one device setup each."""
         return lib().lwf_readers_setup_count(self._h)
 
+    def _queue(self, call, arr, fmt, addr, memory, result, keep):
+        """call (lwf_readers_read or lwf_readers_skip_samples_linear) on the job array arr; records its timings and
+        returns an api.Ticket that keeps `keep` alive, with results [result(j)] for every job j"""
+        t = C.c_uint64()
+        self.ctx.check(call(self._h, arr, len(arr), fmt, addr, memory, C.byref(t)))
+        p, e, s = C.c_double(), C.c_double(), C.c_double()
+        lib().lwf_readers_last_timing(self._h, C.byref(p), C.byref(e), C.byref(s))
+        self.paging_seconds, self.entropy_seconds, self.synthesis_seconds = p.value, e.value, s.value
+        results = [result(j) for j in range(len(arr))]
+        ticket = Ticket(self.ctx, t.value, keep, lambda: results)
+        ticket.results = results
+        return ticket
+
     def read(self, jobs, pcm, stride, sample="f32", interleaved=False):
         """lwf_readers_read.  jobs: [(reader index, max_packets)], each reader at most once.  Job j's PCM lands in `pcm`
         behind the jobs before it, each taking its reader's channels * stride elements (planar: channel c at
@@ -728,15 +749,8 @@ class OggStreamReaders:
             arr[j].out_offset, arr[j].out_stride = off, stride
             arr[j].packet_samples = ps.ctypes.data_as(cabi.u32p)
             off += self.headers(index).audio_channels * stride
-        t = C.c_uint64()
-        self.ctx.check(lib().lwf_readers_read(self._h, arr, n, fmt, addr, memory, C.byref(t)))
-        p, e, s = C.c_double(), C.c_double(), C.c_double()
-        lib().lwf_readers_last_timing(self._h, C.byref(p), C.byref(e), C.byref(s))
-        self.paging_seconds, self.entropy_seconds, self.synthesis_seconds = p.value, e.value, s.value
-        results = [ReadResult(arr[j], counts[j]) for j in range(n)]
-        ticket = Ticket(self.ctx, t.value, (arr, counts, pcm), lambda: results)
-        ticket.results = results
-        return ticket
+        return self._queue(lib().lwf_readers_read, arr, fmt, addr, memory, lambda j: ReadResult(arr[j], counts[j]),
+                           (arr, counts, pcm))
 
     def read_dec_packets(self, indices, max_packets, sample="f32", interleaved=False):
         """read() into page-locked host memory and wait: per reader, the packets it returned, each in the form
@@ -752,13 +766,8 @@ class OggStreamReaders:
         out = []
         for r in results:
             pkts, s0 = [], 0
-            for n in r.packet_samples:
-                n = int(n)
-                if interleaved:
-                    pkts.append(pcm[r.out_offset + s0 * r.channels: r.out_offset + (s0 + n) * r.channels].copy())
-                else:
-                    pkts.append([pcm[r.out_offset + c * stride + s0: r.out_offset + c * stride + s0 + n].copy()
-                                 for c in range(r.channels)])
+            for n in map(int, r.packet_samples):
+                pkts.append(_packet_pcm(pcm, r.out_offset, stride, r.channels, s0, n, interleaved))
                 s0 += n
             if r.status:
                 pkts.append(read_error(self.ctx, r.status))
@@ -804,15 +813,8 @@ class OggStreamReaders:
             arr[j].reader, arr[j].to_skip, arr[j].out_channels = index, int(to_skip), room
             arr[j].out_offset, arr[j].out_stride = off, stride
             off += room * stride
-        t = C.c_uint64()
-        self.ctx.check(lib().lwf_readers_skip_samples_linear(self._h, arr, n, fmt, addr, memory, C.byref(t)))
-        p, e, s = C.c_double(), C.c_double(), C.c_double()
-        lib().lwf_readers_last_timing(self._h, C.byref(p), C.byref(e), C.byref(s))
-        self.paging_seconds, self.entropy_seconds, self.synthesis_seconds = p.value, e.value, s.value
-        results = [SkipResult(arr[j]) for j in range(n)]
-        ticket = Ticket(self.ctx, t.value, (arr, pcm), lambda: results)
-        ticket.results = results
-        return ticket
+        return self._queue(lib().lwf_readers_skip_samples_linear, arr, fmt, addr, memory, lambda j: SkipResult(arr[j]),
+                           (arr, pcm))
 
     def skip_samples_linear_dec(self, indices, to_skip, sample="f32", interleaved=False):
         """skip_samples_linear() into page-locked host memory and wait: per reader what OggStreamReader.skip_samples_linear
@@ -831,11 +833,8 @@ class OggStreamReaders:
                 out.append(read_error(self.ctx, r.status))
             elif not r.got_packet:
                 out.append((None, r.left_to_skip))
-            elif interleaved:
-                out.append((pcm[r.out_offset: r.out_offset + r.n_samples * r.channels].copy(), r.left_to_skip))
             else:
-                out.append(([pcm[r.out_offset + c * stride: r.out_offset + c * stride + r.n_samples].copy()
-                             for c in range(r.channels)], r.left_to_skip))
+                out.append((_packet_pcm(pcm, r.out_offset, stride, r.channels, 0, r.n_samples, interleaved), r.left_to_skip))
         return out
 
     def close(self):
