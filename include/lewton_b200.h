@@ -110,6 +110,9 @@ int lwb_tables_generate(int blocksize_log2, float *a, float *b, float *c, float 
 typedef struct lwb_tables_ref {      /* IdentHeader.cached_bs_derived[i], header.rs:210           */
     const float *a, *b, *c;          /* TwiddleFactors, header_cached.rs:20-24                     */
     const float *window;             /* window_slope                                               */
+    /* compute_bitreverse(bs) (header_cached.rs:101-110), the only table the crate makes: the fused kernels build that
+     * permutation into their index maps, so lwb_setup_create refuses any other with LWB_ERR_INVALID (no setup is
+     * created; lwb_last_error says which table).  a, b, c and window may hold any values. */
     const uint32_t *bitrev;
 } lwb_tables_ref;
 

@@ -293,6 +293,19 @@ extern "C" int lwb_setup_create(lwb_ctx *ctx, const lwb_setup_desc *d, lwb_setup
     if (d->n_modes == 0 || d->n_modes > LWB_MAX_MODES || d->n_mappings == 0 || d->n_mappings > 64 ||
         d->n_floors == 0 || d->n_floors > 64 || !d->modes || !d->mappings || !d->floors)
         return fail(ctx, LWB_ERR_INVALID, "setup: counts out of range");
+    // A caller's bit-reversal table must be compute_bitreverse(bs) (header_cached.rs:101-110), the only one the crate
+    // makes: k_long, k_mid and k_short build that permutation into their index maps, so any other table would give PCM
+    // that depends on the batch path.
+    for (int i = 0; i < 2; i++) {
+        const lwb_tables_ref &t = d->tables[i];
+        if (!t.a || !t.bitrev) continue;
+        const int bs = i ? d->blocksize_1 : d->blocksize_0;
+        std::vector<uint32_t> br(((size_t)1 << bs) / 8);
+        generate_tables(bs, nullptr, nullptr, nullptr, nullptr, br.data());
+        if (!std::equal(br.begin(), br.end(), t.bitrev))
+            return fail(ctx, LWB_ERR_INVALID, i ? "setup: tables[1].bitrev is not compute_bitreverse(blocksize_1)"
+                                                : "setup: tables[0].bitrev is not compute_bitreverse(blocksize_0)");
+    }
     CU(ctx, cudaSetDevice(ctx->device));
     lwb_setup *su = new (std::nothrow) lwb_setup();
     if (!su) return LWB_ERR_BUFFER;

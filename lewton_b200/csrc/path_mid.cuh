@@ -24,6 +24,9 @@ static int try_mid(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const
         const lwb_setup *su = c->stream->setup;
         const ChainWalk &w = bw.walks[i];
         if (su->channels > 8 || (su->bs1 != 10 && su->bs1 != 9) || !su->host.tab[1].pack) return LWB_OK;
+        // blocksize_0 == blocksize_1: short packets and the left slope of long ones after a short block read tab[0] (audio.rs:
+        // 1048, 1059-1088), which k_mid's one pack holds only when both tables are the same (the context shares equal tables)
+        if (su->bs0 == su->bs1 && su->host.tab[0].pack != su->host.tab[1].pack) return LWB_OK;
         if (pack && pack != su->host.tab[1].pack) return LWB_OK;
         pack = su->host.tab[1].pack;
         kb = 11 - su->bs1;

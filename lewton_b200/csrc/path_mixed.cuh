@@ -163,7 +163,11 @@ static uint32_t segment_chain(const lwb_chain *c, const MixedShape &sh, size_t b
     sc.chain.push_back(MixedSchedule::Chain{(uint32_t)sc.segs.size(), 0, (uint32_t)boff});
     const uint32_t done = walk_chain(c, [&](uint32_t k, const Geom &g, bool has, uint32_t plen, uint64_t coeff, uint64_t pos) {
         MixedSeg &p = pk[k] = MixedSeg{SEG_CHAIN, false, false, k, 1, has, plen, coeff, pos};
-        if (g.blockflag && g.n == (uint32_t)kLongN && su->host.tab[1].pack == sh.pack && sh.pack) {
+        // A long block after a short one of the same size (blocksize_0 == blocksize_1: ls == 0, slope_sel == 0) slopes its
+        // whole left half with tab[0]'s window (audio.rs:1059-1088), which k_long's pack holds only when both tables are
+        // the same (the context shares equal tables).
+        const bool left_ok = g.ls != 0 || g.slope_sel || su->host.tab[0].pack == su->host.tab[1].pack;
+        if (g.blockflag && g.n == (uint32_t)kLongN && su->host.tab[1].pack == sh.pack && sh.pack && left_ok) {
             const bool fs = g.ls != 0;
             if (!has || plen == (fs ? (uint32_t)sh.pl_short : (uint32_t)kLongN2)) {     // on the state the block before leaves
                 p.kind = SEG_LONG;

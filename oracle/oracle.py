@@ -104,12 +104,19 @@ def _ptr(a):
     return a.ctypes.data_as(C.c_void_p)
 
 
+class _TablesStruct(C.Structure):
+    """lwo_tables (lewton_oracle.h), for tables held by numpy arrays."""
+    _fields_ = [("bs", C.c_int), ("n", C.c_int), ("a", C.POINTER(C.c_float)), ("b", C.POINTER(C.c_float)),
+                ("c", C.POINTER(C.c_float)), ("window", C.POINTER(C.c_float)), ("bitrev", C.POINTER(C.c_uint32))]
+
+
 class Tables:
     """header_cached.rs:27-41 CachedBlocksizeDerived for one blocksize."""
 
     def __init__(self, bs):
         self.bs, self.n = bs, 1 << bs
         self._h = lib().lwo_tables_new(bs)
+        self._owned = True
         if not self._h:
             raise ValueError("blocksize out of range")
         n = self.n
@@ -120,9 +127,35 @@ class Tables:
         self.window = np.ctypeslib.as_array(L.lwo_tables_window(self._h), (n // 2,)).copy()
         self.bitrev = np.ctypeslib.as_array(L.lwo_tables_bitrev(self._h), (n // 8,)).copy()
 
+    @classmethod
+    def from_arrays(cls, bs, a, b, c, window, bitrev):
+        """Tables of the caller's own (a Rust caller's cached_bs_derived, or any other values): the oracle computes with
+        exactly these arrays (copied; the attributes a, b, c, window and bitrev are read-only views of them, and the
+        object keeps them alive for as long as the oracle reads them).  Not entered in the tables() cache."""
+        if not 6 <= bs <= 13:
+            raise ValueError("blocksize out of range")
+        t = cls.__new__(cls)
+        t.bs, t.n, t._owned = bs, 1 << bs, False
+        n = t.n
+        arrs = {}
+        for name, arr, size, dt in (("a", a, n // 2, np.float32), ("b", b, n // 2, np.float32), ("c", c, n // 4, np.float32),
+                                    ("window", window, n // 2, np.float32), ("bitrev", bitrev, n // 8, np.uint32)):
+            x = np.array(arr, dt, copy=True).ravel()
+            if x.size != size:
+                raise ValueError(f"{name}: {size} entries expected for blocksize {bs}, got {x.size}")
+            arrs[name] = x
+            view = x.view()
+            view.flags.writeable = False
+            setattr(t, name, view)
+        t._arrays = arrs                  # what _st points into, whatever becomes of the attributes
+        t._st = _TablesStruct(bs, n, *(arrs[k].ctypes.data_as(C.POINTER(C.c_float)) for k in ("a", "b", "c", "window")),
+                              arrs["bitrev"].ctypes.data_as(C.POINTER(C.c_uint32)))
+        t._h = C.addressof(t._st)
+        return t
+
     def __del__(self):
         try:
-            if getattr(self, "_h", None) and _lib is not None:
+            if getattr(self, "_owned", False) and getattr(self, "_h", None) and _lib is not None:
                 _lib.lwo_tables_free(self._h)
                 self._h = None
         except Exception:
@@ -138,9 +171,19 @@ def tables(bs):
     return _tables[bs]
 
 
-def inverse_mdct(spectrum, bs):
-    """imdct.rs:291: n/2 coefficients -> n samples (float32)."""
-    t = tables(bs)
+def _pair(bs0, bs1, given):
+    """The (blocksize_0, blocksize_1) tables: `given` (a pair of Tables) or the generated ones."""
+    if given is None:
+        return tables(bs0), tables(bs1)
+    t0, t1 = given
+    if (t0.bs, t1.bs) != (bs0, bs1):
+        raise ValueError(f"tables of blocksizes {(t0.bs, t1.bs)} for a ({bs0}, {bs1}) stream")
+    return t0, t1
+
+
+def inverse_mdct(spectrum, bs, tables=None):
+    """imdct.rs:291: n/2 coefficients -> n samples (float32).  tables: a Tables of blocksize bs (default: generated)."""
+    t = _pair(bs, bs, None if tables is None else (tables, tables))[0]
     buf = np.zeros(t.n, np.float32)
     buf[: t.n // 2] = np.asarray(spectrum, np.float32)
     lib().lwo_inverse_mdct(t._h, _ptr(buf))
@@ -290,10 +333,10 @@ class Pwr:
             pass
 
 
-def synth_spectrum(bs0, bs1, blockflag, prev_flag, next_flag, spectrum, pwr):
-    """audio.rs:1041-1157 from the pre-MDCT tap.  spectrum [ch][n/2].
+def synth_spectrum(bs0, bs1, blockflag, prev_flag, next_flag, spectrum, pwr, tables=None):
+    """audio.rs:1041-1157 from the pre-MDCT tap.  spectrum [ch][n/2]; tables: (t0, t1) Tables (default: generated).
     Returns (rc, pcm[ch][len])."""
-    t0, t1 = tables(bs0), tables(bs1)
+    t0, t1 = _pair(bs0, bs1, tables)
     n = (1 << bs1) if blockflag else (1 << bs0)
     sp = np.ascontiguousarray(spectrum, np.float32)
     ch = sp.shape[0]
@@ -305,11 +348,11 @@ def synth_spectrum(bs0, bs1, blockflag, prev_flag, next_flag, spectrum, pwr):
     return rc, out[:, : olen.value].copy()
 
 
-def synth_packet(bs0, bs1, blockflag, prev_flag, next_flag, coupling, floors, residues, pwr):
+def synth_packet(bs0, bs1, blockflag, prev_flag, next_flag, coupling, floors, residues, pwr, tables=None):
     """audio.rs:988-1157.  coupling = [(mag, ang), ...] in header order;
     floors = per channel None | (Floor1, y[]) | ndarray(dense curve);
-    residues [ch][n/2] (not modified).  Returns (rc, pcm[ch][len])."""
-    t0, t1 = tables(bs0), tables(bs1)
+    residues [ch][n/2] (not modified); tables: (t0, t1) Tables (default: generated).  Returns (rc, pcm[ch][len])."""
+    t0, t1 = _pair(bs0, bs1, tables)
     n = (1 << bs1) if blockflag else (1 << bs0)
     res = np.array(residues, np.float32, copy=True)
     ch = res.shape[0]

@@ -160,8 +160,9 @@ def random_floor1_y(rng, mult, nposts, wild=False):
 class RefStream:
     """Oracle-side twin of one stream: decodes packet by packet with oracle.synth_*."""
 
-    def __init__(self, oracle, channels, bs0, bs1, modes, mappings=None, floors=None):
-        self.o, self.ch, self.bs0, self.bs1 = oracle, channels, bs0, bs1
+    def __init__(self, oracle, channels, bs0, bs1, modes, mappings=None, floors=None, tables=None):
+        """tables: the oracle's (t0, t1) Tables the setup was given (default: generated)."""
+        self.o, self.ch, self.bs0, self.bs1, self.tables = oracle, channels, bs0, bs1, tables
         self.modes = modes                      # [(blockflag, mapping)]
         self.mappings = mappings or [{"coupling": [], "floor_of_channel": [0] * channels}]
         self.floors = floors or []              # [(mult, xs)] -> oracle Floor1 objects
@@ -170,7 +171,7 @@ class RefStream:
 
     def spectrum(self, mode, prev, nxt, spec):
         bf = self.modes[mode][0]
-        return self.o.synth_spectrum(self.bs0, self.bs1, bf, prev, nxt, spec, self.pwr)
+        return self.o.synth_spectrum(self.bs0, self.bs1, bf, prev, nxt, spec, self.pwr, tables=self.tables)
 
     def packet(self, mode, prev, nxt, residue, floors):
         """floors: per channel None | list y | ndarray dense"""
@@ -182,7 +183,7 @@ class RefStream:
                 fl.append(f)
             else:
                 fl.append((self.ofloors[mp["floor_of_channel"][c]], f))
-        return self.o.synth_packet(self.bs0, self.bs1, bf, prev, nxt, mp["coupling"], fl, residue, self.pwr)
+        return self.o.synth_packet(self.bs0, self.bs1, bf, prev, nxt, mp["coupling"], fl, residue, self.pwr, tables=self.tables)
 
 
 def make_setup(ctx, channels, bs0, bs1, modes=((0, 0), (1, 0)), mappings=None, floors=None, tables=None):

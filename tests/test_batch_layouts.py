@@ -44,10 +44,10 @@ def flags(bf):
 
 
 class Kind:
-    """A setup of the test; oracle_twin=False for tables the oracle does not have."""
+    """A setup of the test; tables: the caller's own [(dict for bs0), (dict for bs1)], which its oracle twin gets too."""
 
-    def __init__(self, ctx, C, bs0, bs1, coupling=None, tables=None, oracle_twin=True):
-        self.C, self.bs0, self.bs1, self.oracle_twin = C, bs0, bs1, oracle_twin
+    def __init__(self, ctx, C, bs0, bs1, coupling=None, tables=None):
+        self.C, self.bs0, self.bs1, self.tables = C, bs0, bs1, tables
         if coupling is None:
             coupling = [(0, 1)] if C == 2 else []
         self.mappings = [{"coupling": list(coupling), "floor_of_channel": [0] * C}]
@@ -64,8 +64,9 @@ class Stream:
     def __init__(self, oracle, kind):
         self.kind = kind
         self.pwr = L.PreviousWindowRight(kind.su)
-        self.ref = RefStream(oracle, kind.C, kind.bs0, kind.bs1, [(0, 0), (1, 0)], kind.mappings, kind.floors) \
-            if kind.oracle_twin else None
+        tabs = None if kind.tables is None else tuple(oracle.Tables.from_arrays(b, **kind.tables[i])
+                                                      for i, b in enumerate((kind.bs0, kind.bs1)))
+        self.ref = RefStream(oracle, kind.C, kind.bs0, kind.bs1, [(0, 0), (1, 0)], kind.mappings, kind.floors, tables=tabs)
         self.bf = np.zeros(0, np.uint8)
         self.at = 0
 
@@ -424,7 +425,7 @@ def setup_pool(ctx):
     bent = [L.generate_tables(8), L.generate_tables(11)]
     bent[1]["window"][300] = np.nextafter(bent[1]["window"][300], np.float32(2))
     bent[1]["a"][7] = np.nextafter(bent[1]["a"][7], np.float32(2))
-    pool.append(Kind(ctx, 2, 8, 11, tables=bent, oracle_twin=False))    # tables of its own: no oracle twin
+    pool.append(Kind(ctx, 2, 8, 11, tables=bent))                       # tables of its own, the oracle twin's too
     return pool
 
 
