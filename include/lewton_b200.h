@@ -23,7 +23,8 @@
  * All arithmetic is IEEE binary32, round-to-nearest, never contracted, in the
  * reference's operation order: f32 PCM is bit-identical to lewton's own output
  * (up to the sign of zero / NaN payload), i16 PCM is bit-identical, f16 PCM is
- * the round-to-nearest-even binary16 of that f32 PCM.
+ * the round-to-nearest-even binary16 of that f32 PCM, i32 and i24 PCM are that
+ * f32 PCM scaled, truncated and saturated as lewton's i16 rule does.
  */
 #ifndef LEWTON_B200_H
 #define LEWTON_B200_H
@@ -313,13 +314,27 @@ enum { LWB_OUT_F32_PLANAR = 0,        /* Vec<Vec<f32>>            samples.rs:20-
        LWB_OUT_F32_INTERLEAVED = 2,   /* InterleavedSamples<f32>  samples.rs:43-79                 */
        LWB_OUT_I16_INTERLEAVED = 3,   /* InterleavedSamples<i16>                                   */
        LWB_OUT_F16_PLANAR = 4,        /* Vec<Vec<half::f16>>      a caller's `impl Sample for f16` */
-       LWB_OUT_F16_INTERLEAVED = 5 }; /* InterleavedSamples<half::f16>                             */
+       LWB_OUT_F16_INTERLEAVED = 5,   /* InterleavedSamples<half::f16>                             */
+       /* 6 and 7 are not assigned: refused as bad formats */
+       LWB_OUT_I32_PLANAR = 8,        /* Vec<Vec<i32>>            a caller's `impl Sample for i32` */
+       LWB_OUT_I32_INTERLEAVED = 9,   /* InterleavedSamples<i32>                                   */
+       LWB_OUT_I24_PLANAR = 10,       /* Vec<Vec<[u8; 3]>>        packed little-endian 24-bit      */
+       LWB_OUT_I24_INTERLEAVED = 11 };/* InterleavedSamples<[u8; 3]>  (S24_3LE)                    */
 /* F16 formats: each element is an IEEE binary16 (2 bytes, the layout of the F32 / I16 format of the same arrangement)
  * equal to the binary32 sample x that the F32 format would write, rounded to nearest even: binary16 subnormals are
  * kept (no flush to zero), |x| >= 65520 becomes +-inf, a NaN gives a NaN.  They take the same batch paths as the I16
  * formats of the same layout.  Added under ABI 3 (no struct changes): a library without them refuses out_format 4 / 5
  * with LWB_ERR_INVALID ("bad out_format") before it touches any chain result, stream state or arena -- as every
  * library refuses any out_format above the last one it knows -- so a caller detects support by one refused call. */
+/* I32 and I24 formats: samples.rs:92-103 (`Sample for i16`) with the scale changed, as a caller's `impl Sample for i32`
+ * writes it with Rust's saturating `as` casts.  I32: y = x * 2147483648.0f (one binary32 multiply, exact), y >= 2^31
+ * (x == 1.0 included) gives INT32_MAX, y < -2^31 gives INT32_MIN, NaN gives 0, anything else truncates toward zero; an
+ * element is an int32_t.  I24: y = x * 8388608.0f, above 8388607 gives 8388607, below -8388608 gives -8388608, NaN gives
+ * 0, anything else truncates toward zero; an element is the low 3 bytes of that integer, little-endian two's
+ * complement, with no padding (element offsets and strides count 3-byte samples).  Both take the batch paths of the
+ * F32 / I16 formats of the same layout, except that a planar I24 batch takes the fused kernels only when its rows start at
+ * element offsets (and strides) that are multiples of 16 -- 48 bytes, a 16-byte boundary.  Added under ABI 3 (no
+ * struct changes), refused as the F16 formats are by a library without them; 6 and 7 stay unassigned and refused. */
 
 typedef struct lwb_packet {
     uint8_t mode_number;             /* audio.rs:925                                               */

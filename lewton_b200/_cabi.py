@@ -16,6 +16,7 @@ FLOOR_TYPE_ZERO, FLOOR_TYPE_ONE = 0, 1
 FLOOR_UNUSED, FLOOR_ONE, FLOOR_DENSE, FLOOR_ZERO = 0, 1, 2, 3
 OUT_F32_PLANAR, OUT_I16_PLANAR, OUT_F32_INTERLEAVED, OUT_I16_INTERLEAVED = 0, 1, 2, 3
 OUT_F16_PLANAR, OUT_F16_INTERLEAVED = 4, 5
+OUT_I32_PLANAR, OUT_I32_INTERLEAVED, OUT_I24_PLANAR, OUT_I24_INTERLEAVED = 8, 9, 10, 11      # 6 and 7 are unassigned
 ENTRY_SPECTRUM, ENTRY_RESIDUE, ENTRY_VQ = 0, 1, 2
 MEM_HOST, MEM_DEVICE = 0, 1
 # LWB_KERNEL_* ids in order: KERNELS[id] is the kernel's name

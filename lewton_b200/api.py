@@ -483,15 +483,41 @@ class DecodedPacket:
 
 
 # (sample, interleaved) -> (LWB_OUT_*, numpy dtype).  "f16": IEEE binary16, the f32 sample rounded to nearest even.
+# "i32" / "i24": the f32 sample times 2^31 / 2^23, truncated toward zero and saturated (NaN -> 0); an i24 element is 3
+# bytes, little-endian two's complement, so its dtype is the 3-byte void type I24 (widen with i24_to_i32).
+I24 = np.dtype("V3")
 _FORMATS = {("f32", False): (cabi.OUT_F32_PLANAR, np.float32), ("i16", False): (cabi.OUT_I16_PLANAR, np.int16),
             ("f32", True): (cabi.OUT_F32_INTERLEAVED, np.float32), ("i16", True): (cabi.OUT_I16_INTERLEAVED, np.int16),
-            ("f16", False): (cabi.OUT_F16_PLANAR, np.float16), ("f16", True): (cabi.OUT_F16_INTERLEAVED, np.float16)}
+            ("f16", False): (cabi.OUT_F16_PLANAR, np.float16), ("f16", True): (cabi.OUT_F16_INTERLEAVED, np.float16),
+            ("i32", False): (cabi.OUT_I32_PLANAR, np.int32), ("i32", True): (cabi.OUT_I32_INTERLEAVED, np.int32),
+            ("i24", False): (cabi.OUT_I24_PLANAR, I24), ("i24", True): (cabi.OUT_I24_INTERLEAVED, I24)}
 
 
 def sample_format(sample, interleaved=False):
-    """(LWB_OUT_* format, numpy dtype) of sample type "f32" | "i16" | "f16" in the planar or interleaved layout (KeyError
-    for any other sample type)."""
+    """(LWB_OUT_* format, numpy dtype) of sample type "f32" | "i16" | "f16" | "i32" | "i24" in the planar or interleaved
+    layout (KeyError for any other sample type)."""
     return _FORMATS[(sample, bool(interleaved))]
+
+
+def i24_to_i32(arr):
+    """I24 PCM widened to int32, sign-extended.  arr: a numpy array of I24 elements (any shape), or a numpy array or torch
+    tensor of uint8 whose last dimension holds 3 bytes per sample (a torch tensor stays on its device)."""
+    if hasattr(arr, "data_ptr"):                                         # torch
+        import torch
+        if arr.dtype != torch.uint8 or arr.shape[-1] % 3:
+            raise ValueError("i24_to_i32: a torch tensor must be uint8 with 3 bytes per sample in its last dimension")
+        b = arr.reshape(*arr.shape[:-1], arr.shape[-1] // 3, 3).to(torch.int32)
+        v = b[..., 0] | (b[..., 1] << 8) | (b[..., 2] << 16)
+        return (v << 8) >> 8
+    a = np.ascontiguousarray(arr)
+    if a.dtype == I24:
+        b = a.view(np.uint8).reshape(a.shape + (3,))
+    elif a.dtype == np.uint8 and a.ndim and a.shape[-1] % 3 == 0:
+        b = a.reshape(a.shape[:-1] + (a.shape[-1] // 3, 3))
+    else:
+        raise ValueError("i24_to_i32: need I24 elements or uint8 bytes, 3 per sample in the last dimension")
+    v = b[..., 0].astype(np.uint32) | (b[..., 1].astype(np.uint32) << 8) | (b[..., 2].astype(np.uint32) << 16)
+    return (v << 8).view(np.int32) >> 8
 
 
 def mix_mono(channels):

@@ -35,15 +35,18 @@ def check_no_fma(so=SO):
     return len(bad)
 
 
-_K_LONG_TYPES = {"f": "float", "s": "int16_t", "6__half": "__half"}     # mangled sample types of k_long's instances
+# mangled sample types of k_long's instances
+_K_LONG_TYPES = {"f": "float", "s": "int16_t", "6__half": "__half", "i": "int32_t", "NS_3i24E": "i24"}
 
 
 def hot_kernel_registers(log):
-    """Registers per thread of k_long<float> / k_long<int16_t> / k_long<__half> from ptxas -v output.  The headline kernel
-    is bound by per-warp latency and sensitive to its allocation (a changed helper template that only its sibling k_long_s
-    uses can move it); K_LONG_REGS is the allocation the H100 numbers in DESIGN.md belong to."""
+    """Registers per thread of every k_long instance (k_long<float>, <int16_t>, <__half>, <int32_t>, <i24>) from ptxas -v
+    output.  The headline kernel is bound by per-warp latency and sensitive to its allocation (a changed helper template
+    that only its sibling k_long_s uses can move it); K_LONG_REGS is the allocation the H100 numbers in DESIGN.md belong
+    to."""
     regs = {}
-    for m in re.finditer(r"Compiling entry function '(_ZN3lwb6k_longI(f|s|6__half)EE[^']*)'.*?Used (\d+) registers", log, re.S):
+    types = "|".join(re.escape(t) for t in _K_LONG_TYPES)
+    for m in re.finditer(r"Compiling entry function '(_ZN3lwb6k_longI(" + types + r")EE[^']*)'.*?Used (\d+) registers", log, re.S):
         regs[f"k_long<{_K_LONG_TYPES[m.group(2)]}>"] = int(m.group(3))
     return regs
 

@@ -94,7 +94,7 @@ struct lwb_setup {
     unsigned out_channels() const { return host.n_out ? host.n_out : channels; }
 };
 
-// One row for k_row_copy: `bytes` (even) from src to dst, both 2-byte aligned (rows of any sample type and alignment)
+// One row for k_row_copy: `bytes` from src to dst at any byte alignment (rows of any sample type, 3-byte ones included)
 struct RowCopy { const void *src; void *dst; uint64_t bytes; };
 constexpr int kRowCopyThreads = 256;
 struct ChainShape { unsigned warps; size_t smem; int n1max, wpc, np; };     // k_chain's block and shared memory
@@ -379,24 +379,28 @@ static size_t host_chunks(size_t in_bytes, size_t n_chains)
 template <int F = LWB_OUT_F32_PLANAR, typename Fn>
 static int with_out_format(int fmt, Fn &&f)
 {
-    if constexpr (out_format_known(F))
-        return fmt == F ? f(std::integral_constant<int, F>()) : with_out_format<F + 1>(fmt, f);
-    else
+    if constexpr (F > kOutFormatLast)
         return LWB_ERR_INVALID;
+    else if constexpr (!out_format_known(F))
+        return with_out_format<F + 1>(fmt, f);
+    else
+        return fmt == F ? f(std::integral_constant<int, F>()) : with_out_format<F + 1>(fmt, f);
 }
 
-// The layout the fused kernels take: planar out (f32, i16 or f16), and 16-byte aligned addresses, which their TMA bulk
-// loads of coefficients and vector stores of PCM need.  Element offsets that are multiples of 4 keep that when the arenas
+// The layout the fused kernels take: planar out, and 16-byte aligned addresses, which their TMA bulk loads of
+// coefficients and vector stores of PCM need.  Coefficient offsets that are multiples of 4 and PCM offsets that are
+// multiples of the format's OutFormat::align (4; 16 for i24, whose 16 samples are 48 bytes) keep that when the arenas
 // are 16-byte aligned: the library's staging of host-memory batches always is, a caller's device arena may not be (the
 // chain kernel takes those).
 static bool fused_layout(const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io)
 {
-    if (!out_format_of(io->out_format).planar) return false;
+    const OutFormat of = out_format_of(io->out_format);
+    if (!of.planar) return false;
     if (io->memory == LWB_MEM_DEVICE && ((reinterpret_cast<uintptr_t>(io->coeffs) | reinterpret_cast<uintptr_t>(io->pcm) |
                                           reinterpret_cast<uintptr_t>(io->dense_floor)) & 15))
         return false;
     for (size_t i = 0; i < n_chains; i++)
-        if ((chains[i].out_offset | chains[i].out_stride | chains[i].coeff_offset) & 3) return false;
+        if (((chains[i].out_offset | chains[i].out_stride) & (of.align - 1)) || (chains[i].coeff_offset & 3)) return false;
     return true;
 }
 

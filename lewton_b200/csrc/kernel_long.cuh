@@ -53,7 +53,7 @@ constexpr int kLongN2 = 1024;
 // one run = consecutive packets of one channel of one stream
 struct alignas(16) LongRun {      // 48 bytes: fetched by the kernel with one 1-D TMA copy
     const float *in;        // first packet's spectrum (1024 floats); next packet at +in_stride
-    void *out;              // first emitted packet's PCM (f32, i16 or f16 elements); next at +1024
+    void *out;              // first emitted packet's PCM (elements of the batch's format); next at +1024
     float *state;           // stream state row of this channel (1024 floats)
     uint32_t in_stride;
     uint32_t n_packets;     // including a primer packet if prime != 0
@@ -597,20 +597,53 @@ __device__ __forceinline__ __half d_sample_f16(float v)
     asm("cvt.rn.f16.f32 %0, %1;" : "=h"(r) : "f"(v));
     return __ushort_as_half(r);
 }
+// The integer rules with a 2^31 and a 2^23 scale (LWB_OUT_I32_*, LWB_OUT_I24_*): `Sample for i16` as a caller's
+// `impl Sample for i32` writes it.  The scales are powers of two, so the product is exact (up to overflow to +-inf,
+// which saturates like any value past the range); cvt.rzi.s32.f32 truncates toward zero, saturates (1.0 * 2^31 gives
+// INT32_MAX, as Rust's `as` does) and turns NaN into 0.  I24 clamps the s32 afterwards, which equals clamping the float
+// first for the same reason as in d_sample_i16.
+__device__ __forceinline__ int32_t d_sample_i32(float v)
+{
+    int32_t r;
+    asm("cvt.rzi.s32.f32 %0, %1;" : "=r"(r) : "f"(__fmul_rn(v, 2147483648.0f)));
+    return r;
+}
+__device__ __forceinline__ int32_t d_sample_i24(float v)
+{
+    int32_t r;
+    asm("cvt.rzi.s32.f32 %0, %1;" : "=r"(r) : "f"(__fmul_rn(v, 8388608.0f)));
+    return min(max(r, -8388608), 8388607);
+}
 // one sample as the element type of its format
 __device__ __forceinline__ float d_sample(float v, float *) { return v; }
 __device__ __forceinline__ int16_t d_sample(float v, int16_t *) { return d_sample_i16(v); }
 __device__ __forceinline__ __half d_sample(float v, __half *) { return d_sample_f16(v); }
+__device__ __forceinline__ int32_t d_sample(float v, int32_t *) { return d_sample_i32(v); }
+__device__ __forceinline__ int32_t d_sample(float v, i24 *) { return d_sample_i24(v); }     // the low 3 bytes are stored
 __device__ __forceinline__ void st_pcm(float *p, float v) { __stcs(p, v); }    // streaming: the PCM is not read again
 __device__ __forceinline__ void st_pcm(int16_t *p, float v) { __stcs(reinterpret_cast<short *>(p), (short)d_sample_i16(v)); }
 __device__ __forceinline__ void st_pcm(__half *p, float v) { __stcs(reinterpret_cast<short *>(p), __half_as_short(d_sample_f16(v))); }
+__device__ __forceinline__ void st_pcm(int32_t *p, float v) { __stcs(reinterpret_cast<int *>(p), (int)d_sample_i32(v)); }
+// A 3-byte sample has no store instruction of its own: three 1-byte streaming stores off one address.  (A 2-byte and a
+// 1-byte store picked by the address's parity needs 254 registers in k_long, past K_LONG_REGS; packing four lanes'
+// samples into three words by shuffles would need a lane order per store site.  DESIGN.md 4.1 has the numbers.)
+__device__ __forceinline__ void st_pcm(i24 *p, float v)
+{
+    const uint32_t s = (uint32_t)d_sample_i24(v);
+    unsigned char *b = reinterpret_cast<unsigned char *>(p);
+    __stcs(b, (unsigned char)s);
+    __stcs(b + 1, (unsigned char)(s >> 8));
+    __stcs(b + 2, (unsigned char)(s >> 16));
+}
 
 // the element type of a sample kind
 template <SampleKind K>
-using sample_t = std::conditional_t<K == kSampleF32, float, std::conditional_t<K == kSampleI16, int16_t, __half>>;
+using sample_t = std::conditional_t<K == kSampleF32, float,
+                 std::conditional_t<K == kSampleI16, int16_t,
+                 std::conditional_t<K == kSampleF16, __half, std::conditional_t<K == kSampleI32, int32_t, i24>>>>;
 
 // f(SampleType<T>()) with T = the element type of a runtime sample kind, for code that handles the fused kernels
-// templated on their element type (k_long, k_long_s, k_mid, k_short, k_short_g).  Instantiates f for all three types.
+// templated on their element type (k_long, k_long_s, k_mid, k_short, k_short_g).  Instantiates f for every type.
 template <typename T>
 struct SampleType { using type = T; };
 template <typename Fn>
@@ -619,19 +652,25 @@ inline auto with_sample_type(SampleKind kind, Fn &&f)
     switch (kind) {
     case kSampleI16: return f(SampleType<int16_t>());
     case kSampleF16: return f(SampleType<__half>());
+    case kSampleI32: return f(SampleType<int32_t>());
+    case kSampleI24: return f(SampleType<i24>());
     default: return f(SampleType<float>());
     }
 }
 
 // Stores sample i of channel ch of a chain or packet whose PCM starts at element `off`, in format FORMAT (k_chain and
-// the four-kernel path's k_overlap)
+// the four-kernel path's k_overlap).  3-byte samples take st_pcm's byte stores.
 template <int FORMAT>
 __device__ __forceinline__ void store_sample(void *pcm, uint64_t off, uint64_t stride, unsigned channels, unsigned ch,
                                              uint64_t i, float v)
 {
     constexpr OutFormat F = out_format_of(FORMAT);
     using T = sample_t<F.kind>;
-    static_cast<T *>(pcm)[off + (F.planar ? (uint64_t)ch * stride + i : i * channels + ch)] = d_sample(v, static_cast<T *>(nullptr));
+    T *p = static_cast<T *>(pcm) + off + (F.planar ? (uint64_t)ch * stride + i : i * channels + ch);
+    if constexpr (F.kind == kSampleI24)
+        st_pcm(p, v);
+    else
+        *p = d_sample(v, static_cast<T *>(nullptr));
 }
 
 // Step 8 + window + overlap-add + stores of one block, all 8 slots (k_long, k_long_s, k_mid).  The lane's samples are
@@ -1255,6 +1294,8 @@ inline int long_launch_static(cudaStream_t stream, const LongRun *d_runs, uint32
     switch (kind) {
     case kSampleI16: k_long_s<int16_t><<<grid, kLongWarps * 32, kLongSmemBytesS, stream>>>(d_runs, n_runs, d_pack, d_w_short); break;
     case kSampleF16: k_long_s<__half><<<grid, kLongWarps * 32, kLongSmemBytesS, stream>>>(d_runs, n_runs, d_pack, d_w_short); break;
+    case kSampleI32: k_long_s<int32_t><<<grid, kLongWarps * 32, kLongSmemBytesS, stream>>>(d_runs, n_runs, d_pack, d_w_short); break;
+    case kSampleI24: k_long_s<i24><<<grid, kLongWarps * 32, kLongSmemBytesS, stream>>>(d_runs, n_runs, d_pack, d_w_short); break;
     default: k_long_s<float><<<grid, kLongWarps * 32, kLongSmemBytesS, stream>>>(d_runs, n_runs, d_pack, d_w_short); break;
     }
     return cudaGetLastError() != cudaSuccess;
@@ -1262,7 +1303,7 @@ inline int long_launch_static(cudaStream_t stream, const LongRun *d_runs, uint32
 
 inline void long_kernel_configure()
 {
-    for (SampleKind k : {kSampleF32, kSampleI16, kSampleF16})
+    for (SampleKind k : kSampleKinds)
         with_sample_type(k, [](auto t) {
             using T = typename decltype(t)::type;
             cudaFuncSetAttribute(k_long<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLongSmemBytes);
@@ -1280,6 +1321,8 @@ inline int long_launch(cudaStream_t stream, const LongRun *d_runs, uint32_t n_gr
     switch (kind) {
     case kSampleI16: k_long<int16_t><<<grid, kLongWarps * 32, kLongSmemBytes, stream>>>(d_runs, n_groups, d_pack, ticket, d_w_short, ls); break;
     case kSampleF16: k_long<__half><<<grid, kLongWarps * 32, kLongSmemBytes, stream>>>(d_runs, n_groups, d_pack, ticket, d_w_short, ls); break;
+    case kSampleI32: k_long<int32_t><<<grid, kLongWarps * 32, kLongSmemBytes, stream>>>(d_runs, n_groups, d_pack, ticket, d_w_short, ls); break;
+    case kSampleI24: k_long<i24><<<grid, kLongWarps * 32, kLongSmemBytes, stream>>>(d_runs, n_groups, d_pack, ticket, d_w_short, ls); break;
     default: k_long<float><<<grid, kLongWarps * 32, kLongSmemBytes, stream>>>(d_runs, n_groups, d_pack, ticket, d_w_short, ls); break;
     }
     return cudaGetLastError() != cudaSuccess;

@@ -304,7 +304,7 @@ k_mid(const LongRun *__restrict__ runs, uint32_t n_groups, const float *__restri
 inline void mid_kernel_configure()
 {
     static_assert(MidDev<1>::Smem <= 232448 && MidDev<2>::Smem <= 232448, "k_mid's shared memory must fit one SM");
-    for (SampleKind k : {kSampleF32, kSampleI16, kSampleF16})
+    for (SampleKind k : kSampleKinds)
         with_sample_type(k, [](auto t) {
             using T = typename decltype(t)::type;
             cudaFuncSetAttribute(k_mid<T, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MidDev<1>::Smem);
@@ -321,12 +321,16 @@ inline int mid_launch(cudaStream_t stream, const LongRun *d_runs, uint32_t n_gro
         switch (kind) {
         case kSampleI16: k_mid<int16_t, 1><<<grid, kLongWarps * 32, MidDev<1>::Smem, stream>>>(d_runs, n_groups, d_pack); break;
         case kSampleF16: k_mid<__half, 1><<<grid, kLongWarps * 32, MidDev<1>::Smem, stream>>>(d_runs, n_groups, d_pack); break;
+        case kSampleI32: k_mid<int32_t, 1><<<grid, kLongWarps * 32, MidDev<1>::Smem, stream>>>(d_runs, n_groups, d_pack); break;
+        case kSampleI24: k_mid<i24, 1><<<grid, kLongWarps * 32, MidDev<1>::Smem, stream>>>(d_runs, n_groups, d_pack); break;
         default: k_mid<float, 1><<<grid, kLongWarps * 32, MidDev<1>::Smem, stream>>>(d_runs, n_groups, d_pack); break;
         }
     } else {
         switch (kind) {
         case kSampleI16: k_mid<int16_t, 2><<<grid, kLongWarps * 32, MidDev<2>::Smem, stream>>>(d_runs, n_groups, d_pack); break;
         case kSampleF16: k_mid<__half, 2><<<grid, kLongWarps * 32, MidDev<2>::Smem, stream>>>(d_runs, n_groups, d_pack); break;
+        case kSampleI32: k_mid<int32_t, 2><<<grid, kLongWarps * 32, MidDev<2>::Smem, stream>>>(d_runs, n_groups, d_pack); break;
+        case kSampleI24: k_mid<i24, 2><<<grid, kLongWarps * 32, MidDev<2>::Smem, stream>>>(d_runs, n_groups, d_pack); break;
         default: k_mid<float, 2><<<grid, kLongWarps * 32, MidDev<2>::Smem, stream>>>(d_runs, n_groups, d_pack); break;
         }
     }

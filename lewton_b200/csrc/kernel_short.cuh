@@ -31,7 +31,7 @@ constexpr int kShortOct = 8;               // blocks a warp transforms together
 
 struct alignas(16) ShortRun {              // 48 bytes
     const float *in;        // first packet's spectrum (128 floats); next packet at +in_stride
-    void *out;              // first emitted packet's PCM (f32, i16 or f16 elements); next at +128
+    void *out;              // first emitted packet's PCM (elements of the batch's format); next at +128
     float *state;           // stream state row of this channel (>= 128 floats)
     uint32_t in_stride;
     uint32_t n_packets;     // including a primer packet (has_prev == 0: packet 0 emits nothing)
@@ -267,21 +267,36 @@ __device__ __forceinline__ void short_cta_setup(const float *pack, V *s_pack, ui
 }
 constexpr int kSTwRegs = kSTwReg1 - kSTwReg0 > 0 ? kSTwReg1 - kSTwReg0 : 1;
 
-// PCM staging: one sample as OutT (samples.rs:86-103)
+// PCM staging: one sample as OutT (samples.rs:86-103).  An i24 sample is staged as its 4-byte integer (stage_esz) and
+// packed on the way out.
+template <typename OutT>
+constexpr uint32_t stage_esz = std::is_same_v<OutT, i24> ? 4u : (uint32_t)sizeof(OutT);
 __device__ __forceinline__ void sts_pcm(uint32_t addr, float v, float *) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory"); }
-// 2-byte samples (i16, f16) differ only in the conversion: one staging store for both
+// integer and 2-byte samples differ only in the conversion: one staging store per staged size
 template <typename OutT>
 __device__ __forceinline__ void sts_pcm(uint32_t addr, float v, OutT *)
 {
-    static_assert(sizeof(OutT) == 2, "2-byte samples");
-    const OutT s = d_sample(v, static_cast<OutT *>(nullptr));
-    asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"(*reinterpret_cast<const unsigned short *>(&s)) : "memory");
+    const auto s = d_sample(v, static_cast<OutT *>(nullptr));
+    if constexpr (sizeof(s) == 4) {
+        asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"((uint32_t)s) : "memory");
+    } else {
+        static_assert(sizeof(s) == 2, "2-byte samples");
+        asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"(*reinterpret_cast<const unsigned short *>(&s)) : "memory");
+    }
 }
-// four staged samples of one lane -> global, streaming: one 16-byte (f32) or 8-byte (2-byte samples) store
+// four staged samples of one lane -> global, streaming: one 16-byte (f32, i32) or 8-byte (2-byte samples) store; i24:
+// the four integers' low 3 bytes packed into three words, three 4-byte stores (12 bytes per lane: 4-byte aligned only)
 template <typename OutT>
 __device__ __forceinline__ void copy_out4(OutT *dst, uint32_t src)
 {
-    if constexpr (sizeof(OutT) == 4) {
+    if constexpr (std::is_same_v<OutT, i24>) {
+        uint32_t a, b, c, d;
+        asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d) : "r"(src) : "memory");
+        unsigned int *w = reinterpret_cast<unsigned int *>(dst);
+        __stcs(w, __byte_perm(a, b, 0x4210));          // a0 a1 a2 b0
+        __stcs(w + 1, __byte_perm(b, c, 0x5421));      // b1 b2 c0 c1
+        __stcs(w + 2, __byte_perm(c, d, 0x6542));      // c2 d0 d1 d2
+    } else if constexpr (sizeof(OutT) == 4) {
         float4 v;
         asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(src) : "memory");
         __stcs(reinterpret_cast<float4 *>(dst), v);
@@ -306,7 +321,7 @@ struct ShortLanes {
     uint32_t wA0, wA1, wC0, wC1, wP0, wP1;
     __device__ __forceinline__ ShortLanes(int l, int blk)
     {
-        constexpr uint32_t ESZ = sizeof(OutT);
+        constexpr uint32_t ESZ = stage_esz<OutT>;
         wA0 = 4u * (uint32_t)swzS(blk, elemA_s(l, 0, 0)); wA1 = 4u * (uint32_t)swzS(blk, elemA_s(l, 0, 1));
         wC0 = 4u * (uint32_t)swzS(blk, elemC_s(l, 0, 0)); wC1 = 4u * (uint32_t)swzS(blk, elemC_s(l, 0, 1));
         wP0 = (128u * ESZ + 4u * ESZ) * (uint32_t)blk + ESZ * (uint32_t)l;
@@ -343,7 +358,7 @@ __device__ __forceinline__ void transpose_s(const ShortLanes<OutT> &ln, uint32_t
 template <typename OutT>
 __device__ __forceinline__ void stage_pcm_slot(const ShortLanes<OutT> &ln, uint32_t stage_s, int j, V lo, V hi)
 {
-    constexpr uint32_t CH = 4u * sizeof(OutT);
+    constexpr uint32_t CH = 4u * stage_esz<OutT>;
     const uint32_t p0 = stage_s + ln.wP0, p1 = stage_s + ln.wP1;
     const int r = rev3(j);
     const uint32_t cA = CH * (2 * r), cB = CH * (2 * r + 1), cC = CH * (31 - 2 * r), cD = CH * (30 - 2 * r);
@@ -405,7 +420,7 @@ __global__ void __launch_bounds__(kShortWarps * 32, 1)
 k_short(const ShortRun *__restrict__ runs, uint32_t n_runs, const float *__restrict__ pack)
 {
     extern __shared__ __align__(128) unsigned char smem_s[];
-    constexpr uint32_t ESZ = sizeof(OutT);
+    constexpr uint32_t ESZ = stage_esz<OutT>;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int l = lane & 3, blk = lane >> 2;
     const ShortSmem<kShortRing, kShortStageBytes, kShortDescSlots * sizeof(ShortRun)> sm(smem_s, warp);
@@ -542,7 +557,7 @@ __global__ void __launch_bounds__(kShortWarps * 32, 1)
 k_short_g(const ShortRun *__restrict__ runs, uint32_t n_groups, const float *__restrict__ pack)
 {
     extern __shared__ __align__(128) unsigned char smem_s[];
-    constexpr uint32_t ESZ = sizeof(OutT);
+    constexpr uint32_t ESZ = stage_esz<OutT>;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int l = lane & 3, blk = lane >> 2;
     const ShortSmem<kShortGRing, kShortGStageBytes, kShortGDescSlots * kShortGDescBytes> sm(smem_s, warp);
@@ -637,6 +652,8 @@ inline int short_launch_groups(cudaStream_t stream, const ShortRun *d_runs, uint
     switch (kind) {
     case kSampleI16: k_short_g<int16_t><<<grid, kShortWarps * 32, kShortGSmemBytes, stream>>>(d_runs, n_groups, d_pack); break;
     case kSampleF16: k_short_g<__half><<<grid, kShortWarps * 32, kShortGSmemBytes, stream>>>(d_runs, n_groups, d_pack); break;
+    case kSampleI32: k_short_g<int32_t><<<grid, kShortWarps * 32, kShortGSmemBytes, stream>>>(d_runs, n_groups, d_pack); break;
+    case kSampleI24: k_short_g<i24><<<grid, kShortWarps * 32, kShortGSmemBytes, stream>>>(d_runs, n_groups, d_pack); break;
     default: k_short_g<float><<<grid, kShortWarps * 32, kShortGSmemBytes, stream>>>(d_runs, n_groups, d_pack); break;
     }
     return cudaGetLastError() != cudaSuccess;
@@ -644,7 +661,7 @@ inline int short_launch_groups(cudaStream_t stream, const ShortRun *d_runs, uint
 
 inline void short_kernel_configure()
 {
-    for (SampleKind k : {kSampleF32, kSampleI16, kSampleF16})
+    for (SampleKind k : kSampleKinds)
         with_sample_type(k, [](auto t) {
             using T = typename decltype(t)::type;
             cudaFuncSetAttribute(k_short<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kShortSmemBytes);
@@ -659,6 +676,8 @@ inline int short_launch(cudaStream_t stream, const ShortRun *d_runs, uint32_t n_
     switch (kind) {
     case kSampleI16: k_short<int16_t><<<grid, kShortWarps * 32, kShortSmemBytes, stream>>>(d_runs, n_runs, d_pack); break;
     case kSampleF16: k_short<__half><<<grid, kShortWarps * 32, kShortSmemBytes, stream>>>(d_runs, n_runs, d_pack); break;
+    case kSampleI32: k_short<int32_t><<<grid, kShortWarps * 32, kShortSmemBytes, stream>>>(d_runs, n_runs, d_pack); break;
+    case kSampleI24: k_short<i24><<<grid, kShortWarps * 32, kShortSmemBytes, stream>>>(d_runs, n_runs, d_pack); break;
     default: k_short<float><<<grid, kShortWarps * 32, kShortSmemBytes, stream>>>(d_runs, n_runs, d_pack); break;
     }
     return cudaGetLastError() != cudaSuccess;

@@ -798,19 +798,22 @@ static int walk_batch(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, co
 // Output windows (lwb_stream_set_window).  A clipped chain (ChainWalk::clipped) keeps the path its batch would take
 // without a window: at end of stream nearly every step of a decode server has some stream ending, and routing those to
 // the chain kernel would take most batches off k_long.  So it decodes its full output, laid out as the fused kernels
-// want it -- planes of a multiple of 8 elements, 16-byte aligned -- into scratch, and BatchArenas::download moves the
-// samples it writes to their place with k_row_copy.  This writes bw->clip, the chain array the paths then decode: the
-// clipped chains point into the scratch, the others are the caller's.  A host-memory batch's scratch follows the PCM
-// extent in its staging (whose start moves down to an 8-element boundary), so only written samples cross PCIe.  A
-// device-memory batch's scratch is ctx->win, addressed from io->pcm by a wrapping element offset -- as the staged arenas
-// are addressed from bases biased by their first element -- and placed at io->pcm's offset mod 16.
+// want it -- planes of a multiple of g elements (8; 16 for i24, OutFormat::align), 16-byte aligned -- into scratch, and
+// BatchArenas::download moves the samples it writes to their place with k_row_copy.  This writes bw->clip, the chain
+// array the paths then decode: the clipped chains point into the scratch, the others are the caller's.  A host-memory
+// batch's scratch follows the PCM extent in its staging (whose start moves down to a g-element boundary), so only
+// written samples cross PCIe.  A device-memory batch's scratch is ctx->win, addressed from io->pcm by a wrapping element
+// offset -- as the staged arenas are addressed from bases biased by their first element -- and placed at io->pcm's
+// offset mod 16.  That offset is the byte distance over the element size modulo 2^64: the distance is a multiple of 16,
+// so an exact quotient for 2- and 4-byte elements, and for 3-byte ones its product with the inverse of 3 mod 2^64.
 static int place_clipped_chains(lwb_ctx *ctx, const lwb_chain *chains, size_t n_chains, const lwb_batch_io *io, BatchWalk *bw)
 {
     const OutFormat of = out_format_of(io->out_format);
+    const uint64_t g = std::max(8u, of.align);
     auto region = [&](size_t i, uint64_t *stride) {
         const uint64_t K = chains[i].stream->setup->out_channels(), n = bw->walks[i].n_samples;
-        *stride = (n + 7) & ~7ull;
-        return of.planar ? K * *stride : (n * K + 7) & ~7ull;
+        *stride = (n + g - 1) & ~(g - 1);
+        return of.planar ? K * *stride : (n * K + g - 1) & ~(g - 1);
     };
     uint64_t total = 0, stride;
     for (size_t i = 0; i < n_chains; i++)
@@ -819,16 +822,17 @@ static int place_clipped_chains(lwb_ctx *ctx, const lwb_chain *chains, size_t n_
     uint64_t at, end;
     if (io->memory == LWB_MEM_HOST) {
         BatchExtent &ext = bw->ext;
-        at = (ext.o_hi + 7) & ~7ull;
+        at = (ext.o_hi + g - 1) & ~(g - 1);
         if (at < ext.o_hi || __builtin_add_overflow(at, total, &end) || __builtin_mul_overflow(end, (uint64_t)of.esz, &end))
             return fail(ctx, LWB_ERR_BUFFER, "chain: the staged PCM of a windowed batch does not fit in 64 bits");
-        ext.o_lo &= ~7ull;
+        ext.o_lo &= ~(g - 1);
         ext.o_hi = at + total;
     } else {
         int rc;
         if ((rc = ensure(ctx, ctx->win, total * of.esz + 16))) return rc;
         const uintptr_t pcm = reinterpret_cast<uintptr_t>(io->pcm), win = reinterpret_cast<uintptr_t>(ctx->win.p) + (pcm & 15);
-        at = (uint64_t)(win - pcm) / of.esz;
+        const uint64_t d = (uint64_t)(win - pcm);
+        at = of.esz == 3 ? d * 0xAAAAAAAAAAAAAAABull : d / of.esz;      // 3 * 0xAAAAAAAAAAAAAAAB == 1 mod 2^64
     }
     bw->clip.assign(chains, chains + n_chains);
     for (size_t i = 0; i < n_chains; i++) {

@@ -22,21 +22,37 @@ namespace lwb {
 
 // The PCM formats (LWB_OUT_*): all that the batch paths, the launchers and the kernels know about one.  A sample kind
 // is one conversion from the f32 sample (samples.rs:86-103); kernel_long.cuh maps it to its element type.
-enum SampleKind { kSampleF32 = 0, kSampleI16 = 1, kSampleF16 = 2 };
+enum SampleKind { kSampleF32 = 0, kSampleI16 = 1, kSampleF16 = 2, kSampleI32 = 3, kSampleI24 = 4 };
+constexpr SampleKind kSampleKinds[] = {kSampleF32, kSampleI16, kSampleF16, kSampleI32, kSampleI24};
+// The element type of the I24 formats: 3 bytes, little-endian two's complement, byte-aligned (kernel_long.cuh stores it)
+struct i24 { unsigned char b[3]; };
+static_assert(sizeof(i24) == 3, "packed 3-byte samples");
 struct OutFormat {
     unsigned esz;             // bytes per element
     bool planar;              // [channel][out_stride] planes, else [t][channel]
     SampleKind kind;
+    unsigned align;           // planar rows at element offsets that are multiples of this start 16-byte aligned (f32, i32)
+                              // or at least 8-byte aligned (2-byte samples) in a 16-byte aligned arena: fused_layout
 };
-LWB_CHD bool out_format_known(int f) { return f >= LWB_OUT_F32_PLANAR && f <= LWB_OUT_F16_INTERLEAVED; }
+constexpr int kOutFormatLast = LWB_OUT_I24_INTERLEAVED;
+LWB_CHD bool out_format_known(int f)
+{
+    return f == LWB_OUT_F32_PLANAR || f == LWB_OUT_I16_PLANAR || f == LWB_OUT_F32_INTERLEAVED || f == LWB_OUT_I16_INTERLEAVED ||
+           f == LWB_OUT_F16_PLANAR || f == LWB_OUT_F16_INTERLEAVED || f == LWB_OUT_I32_PLANAR || f == LWB_OUT_I32_INTERLEAVED ||
+           f == LWB_OUT_I24_PLANAR || f == LWB_OUT_I24_INTERLEAVED;
+}
 LWB_CHD OutFormat out_format_of(int f)
 {
-    return f == LWB_OUT_I16_PLANAR        ? OutFormat{2, true, kSampleI16}
-           : f == LWB_OUT_F32_INTERLEAVED ? OutFormat{4, false, kSampleF32}
-           : f == LWB_OUT_I16_INTERLEAVED ? OutFormat{2, false, kSampleI16}
-           : f == LWB_OUT_F16_PLANAR      ? OutFormat{2, true, kSampleF16}
-           : f == LWB_OUT_F16_INTERLEAVED ? OutFormat{2, false, kSampleF16}
-                                          : OutFormat{4, true, kSampleF32};
+    return f == LWB_OUT_I16_PLANAR        ? OutFormat{2, true, kSampleI16, 4}
+           : f == LWB_OUT_F32_INTERLEAVED ? OutFormat{4, false, kSampleF32, 4}
+           : f == LWB_OUT_I16_INTERLEAVED ? OutFormat{2, false, kSampleI16, 4}
+           : f == LWB_OUT_F16_PLANAR      ? OutFormat{2, true, kSampleF16, 4}
+           : f == LWB_OUT_F16_INTERLEAVED ? OutFormat{2, false, kSampleF16, 4}
+           : f == LWB_OUT_I32_PLANAR      ? OutFormat{4, true, kSampleI32, 4}
+           : f == LWB_OUT_I32_INTERLEAVED ? OutFormat{4, false, kSampleI32, 4}
+           : f == LWB_OUT_I24_PLANAR      ? OutFormat{3, true, kSampleI24, 16}     // 16 samples = 48 bytes
+           : f == LWB_OUT_I24_INTERLEAVED ? OutFormat{3, false, kSampleI24, 16}
+                                          : OutFormat{4, true, kSampleF32, 4};
 }
 
 struct DevTables {            // CachedBlocksizeDerived, header_cached.rs:27-31 (device pointers)

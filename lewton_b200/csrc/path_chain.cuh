@@ -35,11 +35,12 @@ static ChainShape chain_shape(unsigned maxc, int n1max, bool residue, bool vq = 
 // the same chain that ends the batch -- in the one-pass schedule (path_mixed.cuh) that one may store the new state before
 // the first one has read the old; and the state rows lwb_streams_save / lwb_streams_load move, whose offsets in the
 // caller's buffer may leave a row unaligned or of a length that is not a multiple of 4; and the written samples of a
-// clipped chain (BatchWalk::clip), f32, i16 or f16 rows from its full output to their place at any 2-byte alignment.
-// Every row is stored in full 16-byte lines between a 2-byte head (up to dst's next 16-byte boundary) and a 2-byte tail.
-// Where source and destination agree mod 16 the lines are plain vector copies; otherwise each line is funnel-shifted
-// out of the two aligned 16-byte source lines it straddles (Q: its offset in words, r: the 0 or 16 bits left over).
-// Those lines hold at least one byte of the row each, so the loads stay inside the row's 16-byte lines.
+// clipped chain (BatchWalk::clip), rows of any sample type from its full output to their place -- at any byte alignment
+// and of any byte length, as rows of 3-byte samples are.  Every row is stored in full 16-byte lines between a byte-wise
+// head (up to dst's next 16-byte boundary) and a byte-wise tail, each under 16 bytes.  Where source and destination
+// agree mod 16 the lines are plain vector copies; otherwise each line is funnel-shifted out of the two aligned 16-byte
+// source lines it straddles (Q: its offset in words, r: the 0, 8, 16 or 24 bits left over).  Those lines hold at least
+// one byte of the row each, so the loads stay inside the row's 16-byte lines.
 template <int Q>
 __device__ __forceinline__ void row_copy_shifted(const uint4 *__restrict__ a, uint4 *__restrict__ d, uint64_t nv, unsigned r)
 {
@@ -51,6 +52,7 @@ __device__ __forceinline__ void row_copy_shifted(const uint4 *__restrict__ a, ui
     }
 }
 
+static_assert(kRowCopyThreads >= 16, "one thread per byte of a row's head and of its tail");
 __global__ void __launch_bounds__(kRowCopyThreads) k_row_copy(const RowCopy *__restrict__ rc)
 {
     const RowCopy c = rc[blockIdx.x];
@@ -58,10 +60,8 @@ __global__ void __launch_bounds__(kRowCopyThreads) k_row_copy(const RowCopy *__r
     char *dst = static_cast<char *>(c.dst);
     const uint64_t head = min(c.bytes, (uint64_t)((16 - (reinterpret_cast<uintptr_t>(dst) & 15)) & 15));
     const uint64_t nv = (c.bytes - head) >> 4;
-    for (uint64_t i = 2 * threadIdx.x; i < head; i += 2 * blockDim.x)
-        *reinterpret_cast<uint16_t *>(dst + i) = *reinterpret_cast<const uint16_t *>(src + i);
-    for (uint64_t i = head + nv * 16 + 2 * threadIdx.x; i < c.bytes; i += 2 * blockDim.x)
-        *reinterpret_cast<uint16_t *>(dst + i) = *reinterpret_cast<const uint16_t *>(src + i);
+    if (threadIdx.x < head) dst[threadIdx.x] = src[threadIdx.x];
+    if (head + nv * 16 + threadIdx.x < c.bytes) dst[head + nv * 16 + threadIdx.x] = src[head + nv * 16 + threadIdx.x];
     uint4 *d = reinterpret_cast<uint4 *>(dst + head);
     const char *s = src + head;
     const unsigned sh = reinterpret_cast<uintptr_t>(s) & 15, r = (sh & 3) * 8;

@@ -16,6 +16,7 @@
 #include <vector>
 
 #include "batcher.h"
+#include "lwb_common.h"
 
 using lwfb::Granule;
 using lwfb::ogg_clone;
@@ -330,7 +331,7 @@ void commit(lwf_readers *rs, Reader &r, Job &j, const lwf_stream_job &sj, lwf_re
     if (counted != sj.n_samples && !out.status) out.status = LWB_ERR_MISMATCH;
 }
 
-bool planar(int fmt) { return fmt == LWB_OUT_F32_PLANAR || fmt == LWB_OUT_I16_PLANAR || fmt == LWB_OUT_F16_PLANAR; }
+bool planar(int fmt) { return lwb::out_format_of(fmt).planar; }
 
 // The most samples per channel n consecutive packets of reader r's stream can return: n * blocksize_1 / 2, and once
 // (blocksize_1 - blocksize_0) / 4 more, which a long block before a short one returns beyond its half.
@@ -771,8 +772,7 @@ extern "C" uint32_t lwf_readers_setup_count(const lwf_readers *rs) { return rs ?
 extern "C" int lwf_readers_read(lwf_readers *rs, lwf_read_job *jobs, size_t n_jobs, int out_format, void *pcm, int pcm_memory,
                                 uint64_t *ticket)
 {
-    if (!rs || !jobs || !n_jobs || !pcm || !ticket || (pcm_memory != LWB_MEM_HOST && pcm_memory != LWB_MEM_DEVICE) || out_format < 0 ||
-        out_format > LWB_OUT_F16_INTERLEAVED)
+    if (!rs || !jobs || !n_jobs || !pcm || !ticket || (pcm_memory != LWB_MEM_HOST && pcm_memory != LWB_MEM_DEVICE) || !lwb::out_format_known(out_format))
         return LWB_ERR_INVALID;
     return lwfb::guarded([&] { return read(rs, jobs, n_jobs, out_format, pcm, pcm_memory, ticket); });
 }
@@ -786,8 +786,7 @@ extern "C" int lwf_readers_seek_absgp_pg(lwf_readers *rs, const uint32_t *reader
 extern "C" int lwf_readers_skip_samples_linear(lwf_readers *rs, lwf_skip_job *jobs, size_t n_jobs, int out_format, void *pcm,
                                                int pcm_memory, uint64_t *ticket)
 {
-    if (!rs || !jobs || !n_jobs || !pcm || !ticket || (pcm_memory != LWB_MEM_HOST && pcm_memory != LWB_MEM_DEVICE) || out_format < 0 ||
-        out_format > LWB_OUT_F16_INTERLEAVED)
+    if (!rs || !jobs || !n_jobs || !pcm || !ticket || (pcm_memory != LWB_MEM_HOST && pcm_memory != LWB_MEM_DEVICE) || !lwb::out_format_known(out_format))
         return LWB_ERR_INVALID;
     return lwfb::guarded([&] { return skip(rs, jobs, n_jobs, out_format, pcm, pcm_memory, ticket); });
 }

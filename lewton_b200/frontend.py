@@ -426,14 +426,15 @@ class OggStreamReader:
 
     def read_dec_packet_generic(self, sample="f32", interleaved=False):
         """inside_ogg.rs:191-205, read_dec_packet_generic::<S>: sample "f32" | "i16" | "f16" (numpy float16: the f32
-        samples rounded to nearest even); planar [channels] arrays or one interleaved array, or None at the end."""
+        samples rounded to nearest even) | "i32" | "i24" (api.I24 elements); planar [channels] arrays or one interleaved
+        array, or None at the end."""
         fmt, dt = sample_format(sample, interleaved)
         return self._read(fmt, dt, bool(interleaved))
 
     def skip_samples_linear(self, to_skip, sample="f32"):
         """inside_ogg.rs:244-283 -> (Option<S>, usize): (planar packet or None, samples left to skip inside it).  sample:
-        "f32", "f16", else i16."""
-        fmt, dt = sample_format(sample if sample in ("f32", "f16") else "i16")
+        "f32", "f16", "i32", "i24", else i16."""
+        fmt, dt = sample_format(sample if sample in ("f32", "f16", "i32", "i24") else "i16")
         pck = self._read(fmt, dt, False, skip=int(to_skip))
         return pck, self._skip_left
 
